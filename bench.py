@@ -1,4 +1,4 @@
-"""bench.py -- images/sec of the MI-GAN generator forward on B200 (BASELINE.json metric).
+"""bench.py -- images/sec of the MI-GAN generator forward on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # our arm (torchrun for N > 1)
     python bench.py --impl reference [--steps K] [--warmup W]      # reference arm: CPU forward on host cores
@@ -10,9 +10,14 @@ the outputs are all-gathered over NCCL.  Prints ONE JSON line (rank 0).
   value        whole-job images/s, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e          same metric through the host-buffer C-ABI call (pinned H2D + forward + D2H per step)
   roofline     dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json HBM copy rate
+               (H100 SXM data-sheet 3.35 TB/s when that file is absent)
   cpu_baseline the reference algorithm (oracle port, torch CPU ops) on this box's host cores
   parity       max-abs / mean-abs error of image 0 of the timed batch vs the CPU reference algorithm (same run)
   clocks       SM clock / throttle reasons sampled during the timed region
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float32; an output
+larger than the dump budget is a fixed, seeded subset of its images, whose indices go to DIR/<name>_index.npy).  Inputs
+and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -28,7 +33,8 @@ if ROOT not in sys.path:
 
 import torch  # noqa: E402
 
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_FALLBACK_GBS = 3350.0  # H100 SXM data sheet
+DUMP_BUDGET_BYTES = 60_000_000
 print_json = print
 
 
@@ -44,7 +50,7 @@ def parse_args():
     ap.add_argument("--batch", type=int, default=None, help="images per GPU; default 32 (migan) / 16 (comodgan)")
     ap.add_argument("--path", default=os.environ.get("MIGAN_B200_PATH", "tc"))
     ap.add_argument("--comod-gemm", default=None, choices=["simt", "tc"],
-                    help="comodgan workload: GEMM engine (tc = staged tcgen05 route, not yet run on hardware)")
+                    help="comodgan workload: GEMM engine (tc = staged wgmma route)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gather", action="store_true",
                     help="N > 1: skip the output all-gather (shows what the collective costs; not the north_star configuration)")
@@ -53,6 +59,8 @@ def parse_args():
                          "with 8 SMs left free for its 8 channels (nccl), or whichever measured faster at this world size (auto: ce at 2 GPUs, nccl above)")
     ap.add_argument("--masks", default="free_form", choices=["free_form", "blocks"], help="synthetic hole masks")
     ap.add_argument("--profile-out", default=None, help="write the per-launch table (JSON) here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, at most 60 MB in all)")
     args = ap.parse_args()
     if args.res is None:
         args.res = 512 if args.workload == "migan" else 256
@@ -116,7 +124,25 @@ def measured_peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        return HBM_FALLBACK_GBS, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+        return HBM_FALLBACK_GBS, "H100 SXM data sheet 3.35 TB/s (not measured)"
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each output tensor as <out_dir>/<name>.npy in float32.  When the outputs exceed DUMP_BUDGET_BYTES, each keeps
+    a fixed, seeded subset of its images (axis 0), sorted, whose indices are written to <name>_index.npy (float64)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BUDGET_BYTES // len(arrays)
+    for name, t in arrays.items():
+        t = t.detach().float()
+        n = t.shape[0]
+        keep = max(1, min(n, share // (t[0].numel() * 4)))
+        if keep < n:
+            idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.numpy().astype(np.float64))
+            t = t[idx.to(t.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
 
 
 def usable_cpus() -> int:
@@ -178,7 +204,7 @@ def cpu_reference_forward_rate(res: int, seconds: float, max_iters: int, warmup:
 
 # ------------------------------------------------------------------------------------------
 def run_reference(args):
-    """Reference arm: the reference's own CPU forward (oracle port; /root/reference does not exist
+    """Reference arm: the reference's own CPU forward (oracle port; the reference project does not exist
     on the GPU box), all host threads, one bs=1 forward of migan-<res> per step."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -192,8 +218,10 @@ def run_reference(args):
         O.generator_forward(sd, x, args.res)
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        O.generator_forward(sd, x, args.res)
+        y = O.generator_forward(sd, x, args.res)
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"y": y})
     value = args.steps / dt
     line = {
         "impl": "reference", "metric": "images/sec", "value": value, "unit": "images/s",
@@ -269,6 +297,8 @@ def run_b200(args):
     barrier()
     clocks = sampler.stop()
     elapsed_ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:   # the last timed step's output (all ranks' images, gathered, when sharded)
+        dump_outputs(args.dump_outputs, {"y": h if sharded is None else h.wait()})
     if world > 1:
         t = torch.tensor([elapsed_ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -357,13 +387,6 @@ def run_b200(args):
     d = by_kernel[dom]
     achieved = d["alg_bytes"] / (d["ms"] * 1e-3) / 1e9
     traffic, traffic_note = None, None
-    try:  # DRAM bytes of one profiled launch of the dominant kernel (ncu --set full), committed under profiles/
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tj = json.load(f).get(dom)
-        if tj:
-            traffic, traffic_note = tj["dram_bytes"], tj
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic, "traffic_launch": traffic_note, "peak_source": peak_src,
                 "launches_per_step": d["launches"], "share_of_step": d["ms"] / total_ms,
@@ -424,10 +447,10 @@ def run_b200(args):
         "data": "synthetic",
         "config": {"workload": "migan-%d Generator.forward, %d images/GPU%s" % (R, B, (", all-gather of outputs (%s)" % ("copy-engine peer reads over NVLink + 8-byte NCCL ready signal" if sharded.gather == "ce" else "NCCL all_gather_into_tensor, %s channels, %s SMs left free for them" % (os.environ.get("NCCL_MAX_NCHANNELS", "?"), os.environ.get("MIGAN_TC_RESERVE_SMS", "0")))) if sharded is not None else (", no gather" if world > 1 else "")),
                    "masks": "free-form (rectangles + brush strokes, evaluate_fid_lpips.py protocol)" if args.masks == "free_form" else "8x8-cell blocks",
-                   "path": args.path, "arithmetic": "fp32 CUDA-core depthwise/FIR; 1x1 convs on tcgen05 as fp16 hi/lo 3-pass split with fp32 accumulate"
+                   "path": args.path, "arithmetic": "fp32 CUDA-core depthwise/FIR; 1x1 convs on wgmma as fp16 hi/lo 3-pass split with fp32 accumulate"
                    if args.path == "tc" else args.path,
                    "global_batch": world * B, "weights": "seeded export-style random (unit-L2 filters)",
-                   "l2": "per-step working set (input 134 MB + ~10 GB of activations at 512/32) exceeds the 126 MB L2; no flush needed",
+                   "l2": "per-step working set (input 134 MB + ~10 GB of activations at 512/32) exceeds the 50 MB L2; no flush needed",
                    "kernel_timing": "separate pass of K steps with cudaEvents around every launch",
                    "e2e": ("K host batches submitted back to back through migan_forward_host_async (pinned H2D + forward + D2H "
                            "per batch, two staging slots so the copies of batch t+1 / t-1 run under the kernels of batch t), timed until the last "
@@ -502,6 +525,8 @@ def run_comodgan(args):
     torch.cuda.synchronize(dev)
     clocks = sampler.stop()
     elapsed_ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"y": y})
     y_host = torch.empty((B, 3, R, R), dtype=torch.float32).pin_memory()
     t0 = time.perf_counter()
     for _ in range(K):
@@ -518,7 +543,7 @@ def run_comodgan(args):
             peaks = json.load(f)
     except Exception:
         pass
-    tpeak = float(peaks.get("bf16_tflops_sustained", 0) or 0) or 1392.6
+    tpeak = float(peaks.get("bf16_tflops_sustained", 0) or 0) or 989.0   # H100 SXM data sheet, dense FP16
     achieved = flops / (elapsed_ms / K * 1e-3) / 1e12
     cpu = None
     if not args.no_cpu_baseline:
@@ -540,14 +565,14 @@ def run_comodgan(args):
         "warmup": Wm, "ms_per_step": elapsed_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": "comodgan-%d Generator.forward (z given, noise_mode=const), %d images/GPU" % (R, B),
-                   "arithmetic": "exact fp32: im2col + CUDA-core GEMM (round-1 first path; tcgen05 implicit GEMM is the next step)"
-                   if os.environ.get("COMOD_GEMM") != "tc" else "im2col fp16 hi/lo split + tcgen05 3-pass GEMM (staged route)",
+                   "arithmetic": "exact fp32: im2col + CUDA-core GEMM (round-1 first path; wgmma implicit GEMM is the next step)"
+                   if os.environ.get("COMOD_GEMM") != "tc" else "im2col fp16 hi/lo split + wgmma 3-pass GEMM (staged route)",
                    "global_batch": world * B, "weights": "constructor-style N(0,1) + non-zero biases / noise strengths",
-                   "l2": "col matrices are GBs per layer: far beyond the 126 MB L2"},
+                   "l2": "col matrices are GBs per layer: far beyond the 50 MB L2"},
         "roofline": {"bound": "tensor", "kernel": "pw_gemm_simt (all GEMM launches)", "achieved": achieved, "peak": tpeak,
                      "unit": "TFLOP/s", "frac": achieved / tpeak, "traffic": None,
                      "note": "achieved = closed-form GEMM FLOPs of the step / whole step time (upper bound on the GEMM kernel's "
-                             "own time); peak = MEASURED_PEAKS.json bf16_tflops_sustained"},
+                             "own time); peak = MEASURED_PEAKS.json bf16_tflops_sustained, else the H100 SXM data-sheet 989 TFLOP/s"},
         "cpu_baseline": cpu, "clocks": clocks,
         "e2e": {"value": world * B * K / e2e_s, "unit": "images/s", "h2d_bytes_per_step": (x_host.numel() + z_host.numel()) * 4,
                 "d2h_bytes_per_step": y_host.numel() * 4},

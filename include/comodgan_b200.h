@@ -1,4 +1,4 @@
-/* comodgan_b200.h -- C ABI of the B200-native Co-Mod-GAN generator forward and of conv2d_resample.
+/* comodgan_b200.h -- C ABI of the H100-native Co-Mod-GAN generator forward and of conv2d_resample.
  *
  * Same shared library and conventions as migan_b200.h (return 0 / non-zero code, comodgan_last_error(), fp32
  * device pointers, `stream` = cudaStream_t as void*, no CPU fallback).  Reference interfaces replaced

@@ -1,4 +1,4 @@
-/* migan_b200.h -- C ABI of the B200-native MI-GAN generator forward.
+/* migan_b200.h -- C ABI of the H100-native MI-GAN generator forward.
  *
  * The shared library (mi-gan_b200/lib/libmigan_b200.so, built by __graft_entry__.build())
  * exports exactly the entry points declared here: plain pointers and sizes, no torch types.
@@ -38,8 +38,8 @@ extern "C" {
 
 /* Contraction engine for the 1x1 pointwise convs. */
 #define MIGAN_PATH_SIMT 0     /* fp32 CUDA-core FMA (bring-up / cross-check path) */
-#define MIGAN_PATH_TC 1       /* tcgen05 tensor cores, fp16 hi/lo 3-pass split, fp32 accumulate (fp32-faithful) */
-#define MIGAN_PATH_TC_FAST 2  /* tcgen05, single fp16 pass (stated lower accuracy, see DESIGN.md) */
+#define MIGAN_PATH_TC 1       /* wgmma tensor cores, fp16 hi/lo 3-pass split, fp32 accumulate (fp32-faithful) */
+#define MIGAN_PATH_TC_FAST 2  /* wgmma, single fp16 pass (stated lower accuracy, see DESIGN.md) */
 
 typedef struct migan_ctx migan_ctx;
 
@@ -180,7 +180,7 @@ int migan_set_tap(migan_ctx* ctx, const char* name, float* dst);
  * past the end).  shape = {C, H, W} of one image. */
 int migan_tap_info(const migan_ctx* ctx, int path, int index, const char** name, int shape[3]);
 
-/* Debug: every pipeline wait inside the tcgen05 kernel is bounded (seconds of wall-clock time); a wait that gives up records
+/* Debug: every pipeline wait inside the wgmma kernel is bounded (seconds of wall-clock time); a wait that gives up records
  * (wait code | parity << 12 | block << 16) in a host-mapped word and traps.  Returns that record for `device` (0: none). */
 int migan_debug_tc_timeout(int device);
 

@@ -119,7 +119,7 @@ def load(build_if_missing: bool = False):
         else:
             raise ImportError(
                 "migan_b200: %s not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU / pure-PyTorch fallback." % path)
+                "(nvcc, sm_90a). There is no CPU / pure-PyTorch fallback." % path)
     lib = ctypes.CDLL(path)
     bind(lib, SYMBOLS)
     bind(lib, COMOD_SYMBOLS)

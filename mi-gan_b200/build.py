@@ -1,8 +1,8 @@
-"""Build the C-ABI shared library in-tree with nvcc for sm_100a (no torch dependency).
+"""Build the C-ABI shared library in-tree with nvcc for sm_90a (no torch dependency).
 
     python -m migan_b200.build          # or __graft_entry__.build()
 
-Output: mi-gan_b200/lib/libmigan_b200.so (git-ignored, travels with gpurun snapshots).
+Output: mi-gan_b200/lib/libmigan_b200.so (git-ignored build product).
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ STAMP = os.path.join(LIBDIR, "libmigan_b200.stamp")
 
 SOURCES = ["elementwise.cu", "gemm_simt.cu", "ops.cu", "sepconv_tc.cu", "migan_abi.cu", "comodgan_abi.cu", "prepost.cu", "pipeline.cu", "reparam.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]

@@ -1,4 +1,4 @@
-"""Co-Mod-GAN generator on B200: drop-in for `lib.model_zoo.comodgan.{Mapping, Encoder, Synthesis, Generator}`.
+"""Co-Mod-GAN generator on H100: drop-in for `lib.model_zoo.comodgan.{Mapping, Encoder, Synthesis, Generator}`.
 
 Reference construction (scripts/demo.py:95-100):
 
@@ -217,7 +217,7 @@ class Generator(nn.Module):
         if not isinstance(x, torch.Tensor) or x.dim() != 4 or tuple(x.shape[1:]) != (4, r, r):
             raise RuntimeError("expected x of shape [N, 4, %d, %d] (mask-0.5, img*mask)" % (r, r))
         if not x.is_cuda:
-            raise RuntimeError("migan_b200.comodgan.Generator runs on B200 (sm_100a) only; got a %s tensor. "
+            raise RuntimeError("migan_b200.comodgan.Generator runs on H100 (sm_90a) only; got a %s tensor. "
                                "There is no CPU fallback (the CPU oracle lives in oracle/ for tests)." % x.device)
         if x.dtype != torch.float32:
             raise RuntimeError("expected float32 input, got %s" % x.dtype)

@@ -1,4 +1,4 @@
-// Shared device helpers for the MI-GAN B200 generator kernels (sm_100a only).
+// Shared device helpers for the MI-GAN generator kernels (sm_90a only).
 //
 // Activation semantics follow lrelu_agc in the reference,
 // lib/model_zoo/migan_inference.py:20-28 with the constants every block passes
@@ -48,7 +48,7 @@ __device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __ha
 }
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-stream-serialization attribute may start while
-// its predecessor in the stream is still draining; everything before pdl_wait() (barrier / TMEM setup, weight-table loads --
+// its predecessor in the stream is still draining; everything before pdl_wait() (barrier setup, weight-table loads --
 // nothing the predecessor writes) overlaps the predecessor's tail, everything after it sees the predecessor's memory.
 // pdl_trigger() lets the successor's blocks start launching as soon as every block of this grid has passed it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

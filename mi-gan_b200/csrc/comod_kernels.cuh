@@ -132,7 +132,7 @@ struct Im2col4K {      // items = P*KP/4 (one float4 each); needs Cg, c0, Ct mul
 };
 
 // Same gather, written as the fp16 hi / lo pair of v * a_scale (v*a_scale ~= hi + lo, 22 significant bits): the A operand
-// of the tcgen05 GEMM (sepconv_tc.cu, A_TMA mode), K-major rows of KP halves (KP a multiple of 64).
+// of the wgmma GEMM (sepconv_tc.cu, A_TMA mode), K-major rows of KP halves (KP a multiple of 64).
 struct Im2colSplit4K { // items = P*KP/4; needs Cg, c0, Ct multiples of 4
     const float* in; const float* scale; ck_half* hi; ck_half* lo; float a_scale;
     int H, W, Ct, c0, Cg, kh, kw, stride, pad_y, pad_x, OH, OW, KP;

@@ -1,4 +1,4 @@
-// C ABI + host runtime of the B200-native Co-Mod-GAN generator and of conv2d_resample (include/comodgan_b200.h).
+// C ABI + host runtime of the H100-native Co-Mod-GAN generator and of conv2d_resample (include/comodgan_b200.h).
 //
 // Replaces the module tree of lib/model_zoo/comodgan.py (Encoder :113-204, synthesis_block_first :207-258,
 // synthesis_block :261-343, Synthesis :346-421, Generator :424-455) and the layers of lib/model_zoo/stylegan.py it
@@ -80,7 +80,7 @@ int gemm_f32(const float* A, const float* Bt, float* out, int64_t P, int K, int 
     }
     return 0;
 }
-// Emulation of the tcgen05 3-pass GEMM (sepconv_tc.cu, A_TMA mode): out = inv_scale * (Ah*Bh + Ah*Bl + Al*Bh), K-major operands.
+// Emulation of the wgmma 3-pass GEMM (sepconv_tc.cu, A_TMA mode): out = inv_scale * (Ah*Bh + Ah*Bl + Al*Bh), K-major operands.
 const char* gemm_tc(const ck_half* a_hi, const ck_half* a_lo, const ck_half* b_hi, const ck_half* b_lo, float inv_scale,
                     float* out, int n, int res, int K, int N, ck_stream_t) {
     const int64_t P = (int64_t)n * res * res;
@@ -109,8 +109,8 @@ const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
 int gemm_f32(const float* A, const float* Bt, float* out, int64_t P, int K, int N, ck_stream_t s) {
     return (int)migan::launch_pw_gemm_simt(A, Bt, out, P, K, N, nullptr, 1, 0, s);
 }
-// The tcgen05 kernel of the MI-GAN path in its plain-GEMM configuration (pre-split A operand by TMA, no activation):
-// out[n][res][res][N] = inv_scale * A[P][K] * B[N][K]^T with the fp16 hi/lo 3-pass split, fp32 accumulation in TMEM.
+// The wgmma kernel of the MI-GAN path in its plain-GEMM configuration (pre-split A operand by TMA, no activation):
+// out[n][res][res][N] = inv_scale * A[P][K] * B[N][K]^T with the fp16 hi/lo 3-pass split, fp32 accumulation in registers.
 const char* gemm_tc(const ck_half* a_hi, const ck_half* a_lo, const ck_half* b_hi, const ck_half* b_lo, float inv_scale,
                     float* out, int n, int res, int K, int N, ck_stream_t s) {
     migan::SepconvTcArgs args;
@@ -158,7 +158,7 @@ struct Runner {
     void gemm_tc_(const ck_half* a_hi, const ck_half* a_lo, const ck_half* b_hi, const ck_half* b_lo, float inv_scale, float* out,
                   int n, int res, int K, int N) {
         if (dry || rc || n <= 0) return;
-        if (const char* err = gemm_tc(a_hi, a_lo, b_hi, b_lo, inv_scale, out, n, res, K, N, s)) rc = fail(ERR_CUDA, "tcgen05 GEMM: %s", err);
+        if (const char* err = gemm_tc(a_hi, a_lo, b_hi, b_lo, inv_scale, out, n, res, K, N, s)) rc = fail(ERR_CUDA, "wgmma GEMM: %s", err);
         ++launches;
     }
     void im2col_split(const float* in, const float* scale, ck_half* hi, ck_half* lo, float a_scale, int64_t n, int H, int W, int C,
@@ -211,7 +211,7 @@ struct ConvL {
     int ws_index = 0;
     int KP = 0, NP = 0;
     float* Bt = nullptr;     // plain: [KP][NP] ; up: [round16(cin)][round64(k*k*cout)]
-    // tcgen05 route (COMOD_GEMM=tc, up == 1 layers): K-major fp16 hi/lo of w * 2^k, [NPc][KPc], KPc = round64(k*k*cin)
+    // wgmma route (COMOD_GEMM=tc, up == 1 layers): K-major fp16 hi/lo of w * 2^k, [NPc][KPc], KPc = round64(k*k*cin)
     ck_half* Bh = nullptr;
     ck_half* Bl = nullptr;
     int KPc = 0, NPc = 0;
@@ -258,7 +258,7 @@ struct comodgan_ctx {
     float* tap_dst = nullptr;
     int last_launches = 0;
     size_t col_cap_floats = (size_t)512 << 20;
-    bool use_tc = false;     // COMOD_GEMM=tc: k x k / 1x1 convolutions (not the transposed ones, not the dense layers) on tcgen05
+    bool use_tc = false;     // COMOD_GEMM=tc: k x k / 1x1 convolutions (not the transposed ones, not the dense layers) on wgmma
 };
 
 namespace {
@@ -582,7 +582,7 @@ struct Walk {
         const bool g_sep = (L.up == 1) && L.NP != cout;              // GEMM output needs its own buffer
         const int Hf = Hin + 1;                                       // FIR-padded input of the down path
         const int Ht = (Hin - 1) * L.up + L.k;                        // conv_transpose2d output (padding 0)
-        const bool tc = c->use_tc && L.up == 1 && L.Bh != nullptr;   // tcgen05 route (staged, off by default)
+        const bool tc = c->use_tc && L.up == 1 && L.Bh != nullptr;   // wgmma route (staged, off by default)
         const bool g_sep_tc = tc && L.NPc != cout;
         const bool tc_up = c->use_tc && L.up > 1 && L.Bh != nullptr;
         size_t per_img = 0;
@@ -660,7 +660,7 @@ struct Walk {
                 // conv2d_resample.py:94-98,124-142 with k=3, up=2, padding=1, 4x4 filter: px0 = 1+2-2 = 1, px1 = 1+1-1 = 1,
                 // pxt = 0: conv_transpose2d(stride 2, padding 0) then upfirdn2d(pad 1,1,1,1, gain 4).
                 if (tc_up) {
-                    // one tcgen05 GEMM per tap: G[tap][p][NPc] = X[p][:] * B_tap[:][:]^T (N = cout is a power-of-two number of
+                    // one wgmma GEMM per tap: G[tap][p][NPc] = X[p][:] * B_tap[:][:]^T (N = cout is a power-of-two number of
                     // N tiles, 9*cout is not), gathered by the same col2im with tap_stride = rows * NPc
                     R.im2col_split(in_c, scale_c, ch, cl, kTcActScale, cnt, Hin, Hin, cin, 1, 1, 1, 0, 0, Hin, Hin, L.KPc);
                     const int64_t rows = cnt * HWi;
@@ -787,7 +787,7 @@ int comodgan_create(int resolution, int device, comodgan_ctx** out) {
     if (const char* e = getenv("COMOD_COL_CAP_MB")) c->col_cap_floats = (size_t)std::max(1, atoi(e)) * (1 << 20) / 4;
     if (const char* e = getenv("COMOD_GEMM")) c->use_tc = (strcmp(e, "tc") == 0);
     if (c->use_tc && device >= 0) {
-        if (int e2 = tc_configure()) { delete c; return fail(ERR_CUDA, "tcgen05 kernel setup failed: %s", dev_err(e2)); }
+        if (int e2 = tc_configure()) { delete c; return fail(ERR_CUDA, "wgmma kernel setup failed: %s", dev_err(e2)); }
     }
     *out = c;
     return 0;

@@ -1,4 +1,4 @@
-// CUDA-core kernels of the MI-GAN generator forward (sm_100a): everything that is not the
+// CUDA-core kernels of the MI-GAN generator forward (sm_90a): everything that is not the
 // 1x1 pointwise contraction.  All are HBM-bound streaming kernels: NHWC fp32, one 128-bit
 // vector of 4 channels per thread so that a warp touches whole 128-byte lines.
 //
@@ -29,8 +29,7 @@ __device__ __forceinline__ int ilog2(int v) { return 31 - __clz(v); }
 
 // Thread = (4 output channels, 4 adjacent pixels): the 4x4 weights + bias stay in registers, x is read as one
 // 128-bit load per input plane, and the thread writes four 128-bit vectors (each warp instruction covers whole
-// 256-byte pixel rows).  The first version re-loaded weights per output vector and saturated the L1 (ncu: L1/TEX
-// throughput 99 %, DRAM 21 %).
+// 256-byte pixel rows).  Re-loading the weights per output vector would saturate the L1 instead of HBM.
 __global__ void __launch_bounds__(256)
 stem_fromrgb_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
                     float* __restrict__ out, uint32_t items, int lhw, int lcv) {
@@ -93,7 +92,7 @@ cudaError_t launch_stem(const float* x, const float* w, const float* b, float* o
 }
 
 // --------------------------------------------------------------------------------------
-// depthwise 3x3 + bias + act, NHWC -> NHWC (used by the CUDA-core path; the tcgen05 path
+// depthwise 3x3 + bias + act, NHWC -> NHWC (used by the CUDA-core path; the wgmma path
 // fuses this stage into the GEMM prologue)
 // --------------------------------------------------------------------------------------
 typedef unsigned long long u64;
@@ -107,11 +106,17 @@ __device__ __forceinline__ float2 unpk2(u64 v) {
     asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v));
     return make_float2(__uint_as_float(lo), __uint_as_float(hi));
 }
-__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) {
+    const float2 x = unpk2(a), y = unpk2(b), z = unpk2(c);
+    return pk2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+}
 __device__ __forceinline__ u64 ldg2(const float* p) { return __ldg(reinterpret_cast<const unsigned long long*>(p)); }
-__device__ __forceinline__ u64 fmul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+__device__ __forceinline__ u64 fmul2(u64 a, u64 b) {
+    const float2 x = unpk2(a), y = unpk2(b);
+    return pk2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
+}
 // lrelu_agc on a channel pair, bit-identical to the scalar form: max(v, 0.2 v) == leaky_relu(v) exactly,
-// then * sqrt2 and clamp; the two multiplies run packed.
+// then * sqrt2 and clamp.
 __device__ __forceinline__ u64 lrelu_agc2(u64 v) {
     const float2 a = unpk2(v), b = unpk2(fmul2(v, pk2(kLreluAlpha, kLreluAlpha)));
     const float2 m = unpk2(fmul2(pk2(fmaxf(a.x, b.x), fmaxf(a.y, b.y)), pk2(kActGain, kActGain)));
@@ -120,7 +125,7 @@ __device__ __forceinline__ u64 lrelu_agc2(u64 v) {
 
 // Thread = (channel PAIR, PAIR of adjacent columns x0 = 2*xp, x0 + 1, strip of RS rows): the 9 taps + bias stay in
 // registers, a 3-row x 4-column window slides down the strip (4 L1-served 64-bit loads per row feed 2 outputs),
-// all MACs are packed FFMA2, and the next row is fetched one iteration ahead.
+// all MACs are FFMAs on channel pairs, and the next row is fetched one iteration ahead.
 template <int RS>
 __global__ void __launch_bounds__(256)
 dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, const float* __restrict__ bias,
@@ -172,7 +177,7 @@ dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, con
             const float2 v = unpk2(lrelu_agc2(acc));
             const size_t o = ((img * H + y) * (size_t)W + x0 + e) * C + c;
             if (out) *reinterpret_cast<float2*>(out + o) = v;
-            if (out_hi) {   // pre-split A operand for the tcgen05 GEMM (layers whose Cout spans several CTA N tiles)
+            if (out_hi) {   // pre-split A operand for the wgmma GEMM (layers whose Cout spans several CTA N tiles)
                 __half h0, l0, h1, l1;
                 split_f16(v.x, kActSplitScale, h0, l0);
                 split_f16(v.y, kActSplitScale, h1, l1);
@@ -205,7 +210,7 @@ cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, fl
 // input rows once, keeping a rolling 3-row x 6-column window in registers (L1-served 64-bit loads,
 // a warp reads 256 contiguous bytes per pixel), evaluates each activated depthwise value of its 4
 // columns exactly once per row and scatters it into the two FIR accumulators it contributes to
-// (rows 2oy-1..2oy+2 feed output oy).  All MACs are packed FFMA2 (two channels per instruction).
+// (rows 2oy-1..2oy+2 feed output oy).  All MACs are FFMAs on channel pairs.
 // Depthwise outputs outside the image are ZERO (the FIR zero-pads the ACTIVATED tensor,
 // migan_inference.py:62-70), not act(bias).
 // --------------------------------------------------------------------------------------
@@ -355,15 +360,17 @@ cudaError_t launch_dw3x3_down(const float* in, const float* w9, const float* bia
 
 // --------------------------------------------------------------------------------------
 // Tensor-core feed variant of the kernel above: same thread mapping and row walk, specialised for the pre-split fp16
-// hi/lo output.  Round-2 ncu of the generic kernel: 54 % issue utilisation, 23 % of the instructions were address
-// arithmetic (eight 64-bit column pointers, runtime C) and 13 % scalar min/max.  Here
+// hi/lo output.  The generic kernel spends a large share of its instructions on address arithmetic (eight 64-bit column
+// pointers, runtime C) and scalar min/max.  Here
 //   * C is a template parameter: one row pointer, every column / tap offset is an immediate;
-//   * the taps and bias arrive pre-multiplied by kActSplitScale * sqrt(2) (the table the tcgen05 prologue uses), so the
-//     activation is clamp(max(v, 0.2 v), +-256 * 64) -- one packed multiply, one 3-input max and one min per value -- and
+//   * the taps and bias arrive pre-multiplied by kActSplitScale * sqrt(2) (the table the wgmma prologue uses), so the
+//     activation is clamp(max(v, 0.2 v), +-256 * 64) -- one multiply, two max and one min per value -- and
 //     the FIR output is already scaled for the fp16 hi/lo split (the FIR is linear);
-//   * packed fp32x2 arithmetic goes through the sm_100 float2 intrinsics (no inline-asm register moves).
+//   * two channels per thread, kept as float2 pairs.
 // --------------------------------------------------------------------------------------
-__device__ __forceinline__ float fmax3f(float a, float b, float c) { float d; asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c)); return d; }
+__device__ __forceinline__ float fmax3f(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
+__device__ __forceinline__ float2 ffma2f(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2f(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 template <int RS, int C>
 __global__ void __launch_bounds__(256, 2)
@@ -432,9 +439,9 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
         for (int tx = 0; tx < 6; ++tx) {
 #pragma unroll
             for (int kx = 0; kx < 3; ++kx) {
-                dw[(r + 1) % 3][tx] = __ffma2_rn(wv[6 + kx], v[tx + kx], dw[(r + 1) % 3][tx]);
-                dw[(r + 2) % 3][tx] = __ffma2_rn(wv[3 + kx], v[tx + kx], dw[(r + 2) % 3][tx]);
-                dw[r % 3][tx] = __ffma2_rn(wv[kx], v[tx + kx], dw[r % 3][tx]);
+                dw[(r + 1) % 3][tx] = ffma2f(wv[6 + kx], v[tx + kx], dw[(r + 1) % 3][tx]);
+                dw[(r + 2) % 3][tx] = ffma2f(wv[3 + kx], v[tx + kx], dw[(r + 2) % 3][tx]);
+                dw[r % 3][tx] = ffma2f(wv[kx], v[tx + kx], dw[r % 3][tx]);
             }
         }
         if (r >= 2) {                                     // depthwise row gy = iy - 1 is complete
@@ -445,15 +452,15 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
 #pragma unroll
                 for (int tx = 0; tx < 6; ++tx) {
                     if ((tx == 0 && !left_ok) || (tx == 5 && !right_ok)) continue;   // depthwise column outside the image: zero
-                    const float2 a = dw[(r + 1) % 3][tx], b = __fmul2_rn(a, alpha2);
+                    const float2 a = dw[(r + 1) % 3][tx], b = fmul2f(a, alpha2);
                     const float2 d = make_float2(fminf(fmax3f(a.x, b.x, -kLim), kLim), fminf(fmax3f(a.y, b.y, -kLim), kLim));
                     if (tx < 4) {                         // tap column tx of output ox0
-                        accB[0] = __ffma2_rn(firp[(tyB * 4 + tx) * CP], d, accB[0]);
-                        accA[0] = __ffma2_rn(firp[(tyA * 4 + tx) * CP], d, accA[0]);
+                        accB[0] = ffma2f(firp[(tyB * 4 + tx) * CP], d, accB[0]);
+                        accA[0] = ffma2f(firp[(tyA * 4 + tx) * CP], d, accA[0]);
                     }
                     if (tx >= 2) {                        // tap column tx-2 of output ox0+1
-                        accB[1] = __ffma2_rn(firp[(tyB * 4 + tx - 2) * CP], d, accB[1]);
-                        accA[1] = __ffma2_rn(firp[(tyA * 4 + tx - 2) * CP], d, accA[1]);
+                        accB[1] = ffma2f(firp[(tyB * 4 + tx - 2) * CP], d, accB[1]);
+                        accA[1] = ffma2f(firp[(tyA * 4 + tx - 2) * CP], d, accA[1]);
                     }
                 }
             }
@@ -512,8 +519,7 @@ cudaError_t launch_dw3x3_down_split(const float* in, const float* w9s, const flo
 // --------------------------------------------------------------------------------------
 // TMA-staged variant of dw3x3_down_split: same arithmetic per thread, but the input rows come from a shared-memory ring
 // that a producer warp fills with cp.async.bulk.tensor -- six rows (55 KB) in flight per block instead of one register row
-// per thread.  Round-2 ncu of the register-streaming kernel: 40 % of the warp time was long-scoreboard (global load) stall
-// at 24 % occupancy.  Block = (image, strip of RS low-res rows, 16 low-res columns, 64-channel slab): 256 compute threads
+// per thread, which keeps more loads in flight than the register-streaming kernel's low occupancy allows.  Block = (image, strip of RS low-res rows, 16 low-res columns, 64-channel slab): 256 compute threads
 // (channel pair x column pair) + 1 producer warp.  Rows / columns outside the image arrive as zeros (TMA out-of-bounds
 // fill), which is exactly the depthwise conv's zero padding.
 // --------------------------------------------------------------------------------------
@@ -615,9 +621,9 @@ dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* _
         for (int tx = 0; tx < 6; ++tx) {
 #pragma unroll
             for (int kx = 0; kx < 3; ++kx) {
-                dw[(r + 1) % 3][tx] = __ffma2_rn(wv[6 + kx], v[tx + kx], dw[(r + 1) % 3][tx]);
-                dw[(r + 2) % 3][tx] = __ffma2_rn(wv[3 + kx], v[tx + kx], dw[(r + 2) % 3][tx]);
-                dw[r % 3][tx] = __ffma2_rn(wv[kx], v[tx + kx], dw[r % 3][tx]);
+                dw[(r + 1) % 3][tx] = ffma2f(wv[6 + kx], v[tx + kx], dw[(r + 1) % 3][tx]);
+                dw[(r + 2) % 3][tx] = ffma2f(wv[3 + kx], v[tx + kx], dw[(r + 2) % 3][tx]);
+                dw[r % 3][tx] = ffma2f(wv[kx], v[tx + kx], dw[r % 3][tx]);
             }
         }
         if (r >= 2) {                                     // depthwise row gy = iy - 1 is complete
@@ -628,15 +634,15 @@ dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* _
 #pragma unroll
                 for (int tx = 0; tx < 6; ++tx) {
                     if ((tx == 0 && !left_ok) || (tx == 5 && !right_ok)) continue;   // depthwise column outside the image: zero
-                    const float2 a = dw[(r + 1) % 3][tx], bb = __fmul2_rn(a, alpha2);
+                    const float2 a = dw[(r + 1) % 3][tx], bb = fmul2f(a, alpha2);
                     const float2 d = make_float2(fminf(fmax3f(a.x, bb.x, -kLim), kLim), fminf(fmax3f(a.y, bb.y, -kLim), kLim));
                     if (tx < 4) {
-                        accB[0] = __ffma2_rn(firp[(tyB * 4 + tx) * 32], d, accB[0]);
-                        accA[0] = __ffma2_rn(firp[(tyA * 4 + tx) * 32], d, accA[0]);
+                        accB[0] = ffma2f(firp[(tyB * 4 + tx) * 32], d, accB[0]);
+                        accA[0] = ffma2f(firp[(tyA * 4 + tx) * 32], d, accA[0]);
                     }
                     if (tx >= 2) {
-                        accB[1] = __ffma2_rn(firp[(tyB * 4 + tx - 2) * 32], d, accB[1]);
-                        accA[1] = __ffma2_rn(firp[(tyA * 4 + tx - 2) * 32], d, accA[1]);
+                        accB[1] = ffma2f(firp[(tyB * 4 + tx - 2) * 32], d, accB[1]);
+                        accA[1] = ffma2f(firp[(tyA * 4 + tx - 2) * 32], d, accA[1]);
                     }
                 }
             }

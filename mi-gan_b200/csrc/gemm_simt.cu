@@ -1,7 +1,7 @@
 // fp32 CUDA-core GEMM for the 1x1 pointwise conv (SeparableConv2d.conv2,
 // lib/model_zoo/migan_inference.py:161) with the fused "+noise -> lrelu_agc" epilogue
 // (:165-169).  This is the bring-up / cross-check path (MIGAN_B200_PATH=simt): exact fp32
-// FMA arithmetic, no tensor cores.  The production path is sepconv_tc.cu (tcgen05).
+// FMA arithmetic, no tensor cores.  The production path is sepconv_tc.cu (wgmma).
 //
 //   out[p][n] = epi( sum_k A[p][k] * Bt[k][n] )      A [P][K] row-major (NHWC pixels x Cin)
 //                                                    Bt [K][N] (conv2.weight transposed)

@@ -22,7 +22,7 @@ cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, fl
                          int n, int H, int W, int C, cudaStream_t s);
 // depthwise 3x3 + bias + lrelu_agc, then 4x4 FIR stride 2 pad 1 (taps fir16 [16][C]).
 // Writes fp32 [n,H/2,W/2,C] to out_f32 (if non-null) and/or the scaled fp16 hi/lo split
-// (if out_hi non-null) that the tcgen05 GEMM consumes directly through TMA.
+// (if out_hi non-null) that the wgmma GEMM consumes directly through TMA.
 cudaError_t launch_dw3x3_down(const float* in, const float* w9, const float* bias, const float* fir16,
                               float* out_f32, __half* out_hi, __half* out_lo,
                               int n, int H, int W, int C, cudaStream_t s);

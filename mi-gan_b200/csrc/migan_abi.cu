@@ -1,4 +1,4 @@
-// C ABI + host runtime of the B200-native MI-GAN generator (include/migan_b200.h).
+// C ABI + host runtime of the H100-native MI-GAN generator (include/migan_b200.h).
 //
 // Host side of the hot path: weight registry in the reference's state_dict layout, one-time
 // repacking for the kernels, a per-batch-size execution plan (a flat list of kernel launches
@@ -70,10 +70,10 @@ struct SepConv {
     // device pointers into the weight arena
     float* w9 = nullptr;      // [9][cin]   depthwise taps, tap-major
     float* bias = nullptr;    // [cin]
-    float* w9_tc = nullptr;   // same, pre-multiplied by kActSplitScale * sqrt(2) for the tcgen05 prologue
+    float* w9_tc = nullptr;   // same, pre-multiplied by kActSplitScale * sqrt(2) for the wgmma prologue
     float* bias_tc = nullptr;
     float* pw_t = nullptr;    // [cin][cout] fp32 (CUDA-core GEMM)
-    __half* pw_hi = nullptr;  // [cout][cin] fp16 hi part of w * 2^k   (tcgen05, K-major)
+    __half* pw_hi = nullptr;  // [cout][cin] fp16 hi part of w * 2^k   (wgmma, K-major)
     __half* pw_lo = nullptr;  // [cout][cin] fp16 lo part
     float tc_inv_scale = 1.f; // 1 / (kActSplitScale * 2^k)
     float* fir16 = nullptr;   // [16][cin] (down) or [16][cout] (up), tap-major
@@ -112,7 +112,7 @@ struct Step {
     int n = 0, H = 0, W = 0, C = 0;  // meaning depends on kind (input dims)
     int act = 0;
     bool want_f32 = false;
-    migan::SepconvTcArgs tc;  // resolved tcgen05 launch (tensor maps, tiling)
+    migan::SepconvTcArgs tc;  // resolved wgmma launch (tensor maps, tiling)
     migan::DownTensorMap down_map;   // K_DWDOWN on the TMA-staged kernel: tensor map of the input
     bool down_tma = false;
     // roofline bookkeeping: algorithmic bytes = own input(s) read once + output written once
@@ -243,7 +243,7 @@ struct ArenaBuilder {
 extern "C" {
 
 const char* migan_last_error(void) { return g_last_error.c_str(); }
-const char* migan_version(void) { return "migan_b200 0.1 (sm_100a)"; }
+const char* migan_version(void) { return "migan_b200 0.1 (sm_90a)"; }
 
 int migan_create(int resolution, int device, migan_ctx** out) {
     if (!out) return fail(MIGAN_ERR_INVALID, "out is null");
@@ -314,8 +314,8 @@ int migan_create(int resolution, int device, migan_ctx** out) {
         CUDA_TRY(cudaSetDevice(device));
         cudaDeviceProp prop;
         CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10)
-            return fail(MIGAN_ERR_CUDA, "device %d is sm_%d%d; this build targets sm_100a (B200) only", device, prop.major, prop.minor);
+        if (prop.major != 9 || prop.minor != 0)
+            return fail(MIGAN_ERR_CUDA, "device %d is sm_%d%d; this build targets sm_90a (H100) only", device, prop.major, prop.minor);
         CUDA_TRY(migan::configure_elementwise());
         CUDA_TRY(migan::configure_sepconv_tc());
     }  // device < 0: description-only context (weight registry / workspace sizes), cannot compute
@@ -390,7 +390,7 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
         memcpy(ab.bytes.data() + off, b.data(), sizeof(float) * cin);
         fix.push_back({reinterpret_cast<void**>(&L.bias), off});
     }
-    {   // tcgen05 prologue: activation gain and fp16-split scale folded into the depthwise taps
+    {   // wgmma prologue: activation gain and fp16-split scale folded into the depthwise taps
         const float S = 64.0f /* kActSplitScale */ * 1.41421356237309515f;
         const std::vector<float>& w = W(ctx, L.p + "conv1.weight");
         const std::vector<float>& b = W(ctx, L.p + "conv1.bias");
@@ -648,7 +648,7 @@ struct PlanBuilder {
             steps.push_back(s);
             gemm_in = S[t1];
         } else if (L.cout >= 512 && !rgb && (L.res_in >= 64 || fuse_mask_dw() == 0)) {
-            // Cout spans 4 accumulator regions: a fused prologue would re-run the depthwise stage, so run it once as its
+            // Cout spans 8 N tiles: a fused prologue would re-run the depthwise stage per tile, so run it once as its
             // own kernel and hand the GEMM a pre-split operand (these layers are small: res <= 64)
             Step s; s.kind = K_DW; s.L = &L; s.in = in; s.n = n; s.H = L.res_in; s.W = L.res_in; s.C = L.cin;
             s.hi = reinterpret_cast<__half*>(S[t1]);
@@ -694,7 +694,7 @@ struct PlanBuilder {
                     s.io_flags |= rgb_flags;
                     s.tap2 = rgb_tap; s.tap2_src = rgb->img_out; s.tap2C = 3; s.tap2H = L.res_pw; s.tap2W = L.res_pw; s.tap2_flags = rgb_flags;
                 }
-                if (err) return fail(MIGAN_ERR_CUDA, "tcgen05 plan for %s failed: %s", L.p.c_str(), err);
+                if (err) return fail(MIGAN_ERR_CUDA, "wgmma plan for %s failed: %s", L.p.c_str(), err);
             } else {
                 s.kind = K_GEMM_SIMT; s.in = gemm_in;
             }
@@ -760,7 +760,7 @@ struct PlanBuilder {
             const float* img_lo = (img_cur >= 0) ? IMG[img_cur] : nullptr;
             float* img_out = last ? nullptr : IMG[img_next];      // last level: the caller's y (bound at launch)
             const ToRgb& T = c->torgb[i];
-            const bool fuse_rgb = tcp && channels(r) <= 256;   // all output channels of a pixel tile in one CTA (two N halves at 256)
+            const bool fuse_rgb = tcp && channels(r) <= (path == MIGAN_PATH_TC_FAST ? 128 : 64);   // all output channels in one CTA tile
             // conv1's FIR + noise + activation + skip can be rebuilt in conv2's prologue (the up-sampled tensor then never
             // exists in HBM) when conv2 runs its depthwise stage in the tensor-core kernel with 8 x 16 tiles.
             const SepConv& L1 = c->syn1[i];
@@ -884,7 +884,7 @@ int run_step(migan_ctx* ctx, Step& s, const float* x, float* y, cudaStream_t st)
             break;
     }
     if (e != cudaSuccess)   // asynchronous failures of EARLIER launches surface here too: the pipeline-timeout record names the wait
-        return fail(MIGAN_ERR_CUDA, "kernel launch (step %s) failed: %s [tcgen05 pipeline timeout record 0x%x]", s.label.c_str(),
+        return fail(MIGAN_ERR_CUDA, "kernel launch (step %s) failed: %s [wgmma pipeline timeout record 0x%x]", s.label.c_str(),
                     cudaGetErrorString(e), (unsigned)migan::sepconv_tc_timeout_record(ctx->device));
     ctx->last_launches++;
     if (ctx->tap_dst && !s.tap.empty() && s.tap == ctx->tap_name) {
@@ -1037,9 +1037,9 @@ static int forward_host_enqueue(migan_ctx* ctx, const float* x_host, float* y_ho
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaSetDevice(ctx->device));
     // Micro-batch pipeline: H2D of micro-batch k+1 and D2H of k-1 overlap the kernels of k (three streams).
-    // The small-resolution layers cost a fixed ~0.4 ms per forward, so the split is kept coarse.
+    // The small-resolution layers cost a fixed time per forward, so the split is kept coarse.
     // Synchronous call (one batch, then wait): split it so the copies of one half overlap the kernels of the other
-    // (measured at 512x512, n = 32: M = 1 / 2 / 4 / 8 -> 1770 / 1926 / 1896 / 1678 img/s).  Enqueue-only call: consecutive
+    // (two micro-batches: more would pay the fixed per-forward cost of the small layers more often).  Enqueue-only call: consecutive
     // batches already overlap through the two staging slots (H2D of batch t+1 and D2H of batch t-1 run under the kernels of
     // batch t), so the batch stays whole and does not pay the fixed per-forward cost of the small layers twice.
     int M = (slot_out != nullptr && n >= 8 && n % 2 == 0) ? 2 : 1;

@@ -1,4 +1,4 @@
-// Standalone sm_100a versions of the reference's two CUDA plugin ops (forward only):
+// Standalone sm_90a versions of the reference's two CUDA plugin ops (forward only):
 //   upfirdn2d : torch_utils/ops/upfirdn2d.cpp:16-94 + upfirdn2d.cu:29-200
 //   bias_act  : torch_utils/ops/bias_act.cpp:32-90  + bias_act.cu:23-147
 // Both are pure HBM streaming ops on NCHW fp32 tensors (the plugin's public layout).

@@ -14,10 +14,10 @@
 //   NZ   [10 rows][24 cols]        fp32   UP: noise map rows y0-1 .. y0+8, cols x0-4 .. x0+19
 //   XA   [4 planes][10 rows][24 cols] fp32 STEM: the generator input x (NCHW planes), same window as NZ
 //        (W is the innermost tensor-map dimension of these two: the box starts 4 elements = 16 bytes left of the tile.
-//         A box starting at x0-2, i.e. 8 bytes off a 16-byte boundary, faults the TMA unit on B200 -- measured: illegal
-//         instruction -- so the window is 24 wide and the 18 columns used sit at indices 3 .. 20.)
+//         The box start is kept 16-byte aligned -- one starting at x0-2, 8 bytes off a 16-byte boundary, faulted the TMA
+//         unit (illegal instruction) -- so the window is 24 wide and the 18 columns used sit at indices 3 .. 20.)
 //   DIN  [20 rows][36 cols][16 ch] fp32   DOWN: input rows 2*y0-2 .. 2*y0+17, cols 2*x0-2 .. 2*x0+33 (16-ch chunk)
-// A operand (one K block of 64 channels, M = 128 pixel rows): fp16 hi and lo planes, UMMA K-major SWIZZLE_128B:
+// A operand (one K block of 64 channels, M = 128 pixel rows): fp16 hi and lo planes, wgmma K-major SWIZZLE_128B:
 //   byte(m, k) = (m >> 3) * 1024 + (m & 7) * 128 + (((k >> 3) ^ (m & 7)) << 4) + (k & 7) * 2
 #pragma once
 #include <stdint.h>
@@ -42,10 +42,9 @@ constexpr float kSplit = 64.0f;                // power-of-two scale of the fp16
 constexpr int kAuxW = 24;                      // row length of the NZ / XA windows
 constexpr int kAuxLeft = 4;                    // the windows start at column x0 - kAuxLeft; IN column c <-> window column c + 3
 
-// A pair of fp32 values processed by ONE packed instruction (Blackwell FFMA2 / FMUL2 / FADD2: one issue slot per two fp32
-// operations).  On the device P2 is float2 and the arithmetic goes through the sm_100 intrinsics (__ffma2_rn ...): the
-// compiler then allocates the even-aligned register pairs itself.  (Inline-asm "mov.b64 {lo, hi}" wrappers cost one
-// register move per packed operand: 15-19 % of all instructions the kernel executed in the round-2 ncu source view.)
+// A pair of fp32 values (two channels) handled together.  On the device P2 is float2 and every operation is two scalar
+// FFMA / FMUL / FADD with round-to-nearest (Hopper has no packed fp32 instructions), so the emulation build below
+// computes bit-identical results.
 #ifdef MIGAN_EMULATE
 struct P2 { float x, y; };
 typedef P2 f2;
@@ -69,18 +68,18 @@ typedef float2 P2;
 typedef float2 f2;
 typedef float4 f4;
 SC_DEV P2 pk(float lo, float hi) { return make_float2(lo, hi); }
-SC_DEV P2 ffma2(P2 a, P2 b, P2 c) { return __ffma2_rn(a, b, c); }
-SC_DEV P2 fmul2(P2 a, P2 b) { return __fmul2_rn(a, b); }
-SC_DEV P2 fadd2(P2 a, P2 b) { return __fadd2_rn(a, b); }
+SC_DEV P2 ffma2(P2 a, P2 b, P2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+SC_DEV P2 fmul2(P2 a, P2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+SC_DEV P2 fadd2(P2 a, P2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 SC_DEV uint32_t f2_to_h2(float lo, float hi) { __half2 h = __floats2half2_rn(lo, hi); return *reinterpret_cast<uint32_t*>(&h); }
 SC_DEV uint32_t fbits(float v) { return __float_as_uint(v); }
 SC_DEV float bitsf(uint32_t u) { return __uint_as_float(u); }
 SC_DEV float ldg1(const float* p) { return __ldg(p); }
 SC_DEV void st_u2(uint8_t* p, uint32_t a, uint32_t b) { *reinterpret_cast<uint2*>(p) = make_uint2(a, b); }
-SC_DEV float fmax3(float a, float b, float c) { float d; asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c)); return d; }   // FMNMX3
+SC_DEV float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 #endif
 SC_DEV P2 unpk(P2 v) { return v; }
-SC_DEV P2 fsub2(P2 a, P2 b) { return ffma2(b, pk(-1.0f, -1.0f), a); }     // a - b, exact (one FFMA2)
+SC_DEV P2 fsub2(P2 a, P2 b) { return ffma2(b, pk(-1.0f, -1.0f), a); }     // a - b, exact
 SC_DEV P2 p2zero() { return pk(0.0f, 0.0f); }
 typedef P2 u64;   // historical name of the packed pair in this file
 

@@ -1,4 +1,4 @@
-// Fused SeparableConv2d on Blackwell tensor cores (sm_100a): the hot kernel of the generator.
+// Fused SeparableConv2d on Hopper tensor cores (sm_90a): the hot kernel of the generator.
 //
 //   out = epi( PW( act( DW3x3( src ) + b ) ) )          lib/model_zoo/migan_inference.py:154-170
 //
@@ -10,24 +10,21 @@
 //                                STEM   fromrgb 1x1 (4 -> C0) + activation (:193-196) recomputed on the halo from the
 //                                       generator input x -- the stem tensor never exists in HBM
 //                                SPLIT  no depthwise stage: a pre-split fp16 hi/lo A operand is loaded by TMA
-//   DW3x3 + bias + lrelu_agc   CUDA cores (packed FFMA2), fp32 (sepconv_stages.cuh)
-//   PW (1x1 conv, Cin -> Cout) tcgen05.mma kind::f16, M = 128 pixels x N <= 128 channels per accumulator, accumulators
-//                              in TMEM.  fp32-faithful mode: both operands are split into fp16 (hi, lo) pairs;
-//                              [main | corr] = Ah * [Bh ; Bl]^T (one N = 2*n_tile instruction), corr += Al * Bh,
-//                              main + corr summed in the epilogue (separate accumulators: the tensor core truncates
-//                              on accumulate).  Fast mode: Ah * Bh only.
-//   epi                        TMEM -> registers: * 2^-k, + noise, lrelu_agc [-> torgb + image] -> NHWC fp32, either
-//                              through swizzled staging + per-warp TMA store or straight from registers (256-bit stores)
+//   DW3x3 + bias + lrelu_agc   CUDA cores, fp32 (sepconv_stages.cuh)
+//   PW (1x1 conv, Cin -> Cout) wgmma.mma_async m64nNk16 kind f16 with fp32 accumulators in registers: M = 128 pixels (two
+//                              m64 instructions) x n_tile channels per CTA tile.  fp32-faithful mode (n_tile = 64): both
+//                              operands are split into fp16 (hi, lo) pairs; main = Ah * Bh, corr = Ah * Bl + Al * Bh in
+//                              separate accumulators, summed in the epilogue.  Fast mode (n_tile <= 128): Ah * Bh only.
+//   epi                        registers: * 2^-k, + noise, lrelu_agc [-> torgb + image] -> NHWC fp32 (each quad of lanes
+//                              writes 32 contiguous bytes per pixel row and column block)
 //
-// One persistent CTA per SM, 14 warps x 128 registers, warp-specialised:
-//   warps 0-7    prologue      two groups of 4: pre-stage (UP / STEM) + depthwise conv -> fp16 hi/lo A operand
-//   warps 8-11   epilogue      one TMEM lane quarter each
-//   warp 12      TMA producer  input chunks, weight K blocks, L2 prefetch
-//   warp 13      MMA issuer    one elected lane issues tcgen05.mma / tcgen05.commit; owns TMEM
-// The two 256-column accumulator regions are either the double buffer of consecutive M tiles (nt_share = 1) or the two
-// N halves of ONE M tile (nt_share = 2, Cout >= 256: the A operand -- and the whole prologue -- is produced once and
-// multiplied against both weight halves; the epilogue drains half 0 while the MMAs of half 1 finish).
-// All hand-offs are mbarrier pipelines (input ring, A ring, B ring, accumulator regions).
+// One persistent CTA per SM, 16 warps = 4 warpgroups, warp-specialised:
+//   warpgroups 0-1  prologue       two groups of 4 warps: pre-stage (UP / STEM) + depthwise conv -> fp16 hi/lo A operand
+//   warpgroup 2     MMA + epilogue issues the wgmma of an M tile, then drains its accumulators
+//   warpgroup 3     TMA producer   one lane: input chunks, weight K blocks, L2 prefetch
+// The accumulators of an M = 128 tile (main + corr of 64 channels, or 128 channels in fast mode) are 128 registers per thread of one warpgroup, so setmaxnreg moves
+// registers from the producer warpgroup (which needs few) to the MMA warpgroup; the prologue keeps 128.
+// All hand-offs are mbarrier pipelines (input ring, A ring, B ring).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -50,41 +47,42 @@ namespace {
 
 using namespace stages;
 
-constexpr int kThreads = 448;      // 14 warps; registers are allocated per 4 warps: 16 x 32 x 128 = the whole file
-constexpr int kNumProWarps = 8;    // warps 0-7: the SM's issue arbiter favours higher warp ids, so the latency-critical
-constexpr int kEpiWarp0 = 8;       // single-warp roles get the highest ids and the throughput-oriented prologue the lowest
-constexpr int kProducerWarp = 12;
-constexpr int kMmaWarp = 13;
+constexpr int kThreads = 512;      // 4 warpgroups
+constexpr int kNumProWarps = 8;    // warps 0-7
+constexpr int kMmaWarp0 = 8;       // warps 8-11: one warpgroup (wgmma is issued by all four warps together)
+constexpr int kProducerWarp = 12;  // warps 12-15: lane 0 of warp 12 is the producer, the rest only release registers
+constexpr int kProRegs = 144;      // setmaxnreg per thread: 2 x 144 (prologue) + 184 (MMA) + 40 (producer) = 4 x 128,
+constexpr int kMmaRegs = 184;      // the whole register file
+constexpr int kProducerRegs = 40;
 constexpr int kTileM = 128;
+constexpr int kMaxTileN = 128;     // accumulator registers of the MMA warpgroup: kMaxTileN per thread
 constexpr int kKBlock = 64;        // channels per A/B stage (128 bytes of fp16: one SW128 row)
 constexpr int kChunkC = 32;        // channels per input chunk (128 bytes of fp32)
 constexpr uint32_t kABytes = kTileM * kKBlock * 2;   // 16 KB per hi or lo
 constexpr uint32_t kAStage = 2 * kABytes;            // hi + lo
-constexpr uint32_t kEpiWarpBuf = 32 * 32 * 4;        // 4 KB: 32 pixel rows x 32 fp32 of one epilogue warp
 constexpr uint32_t kSmemLimit = 232448;              // 227 KB
-constexpr int kRgbBias = 3 * 256, kRgbFir = 3 * 256 + 4;   // offsets inside the torgb table s_rgb
+constexpr int kRgbBias = 3 * kMaxTileN, kRgbFir = 3 * kMaxTileN + 4;   // offsets inside the torgb table s_rgb
 constexpr uint32_t kStaticSmem = 4096;               // barriers + torgb table (static __shared__), rounded up
 
 struct Params {
-    CUtensorMap map_in, map_t, map_aux, map_a_hi, map_a_lo, map_w_hi, map_w_lo, map_out;   // map_out box = 32 pixels x 32 channels
+    CUtensorMap map_in, map_t, map_aux, map_a_hi, map_a_lo, map_w_hi, map_w_lo;
     const float* w9;                          // [9][cin] depthwise taps * (kActSplitScale * sqrt 2)
     const float* bias;                        // [cin]              * (kActSplitScale * sqrt 2)
     const float* noise;
-    float* out;                               // NHWC output (direct-store epilogue)
+    float* out;                               // NHWC output
     float inv_scale;
     int n, H, W, cin, cout;
     int act, passes;
     int source;                               // SepconvSource
-    int nt_share;                             // accumulator regions per M tile (1 or 2)
-    int tile_n, tile_h, tile_w, n_tile;      // n_tile = N per accumulator region (64 or 128)
-    int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / (n_tile * nt_share)
+    int tile_n, tile_h, tile_w, n_tile;      // n_tile = output channels per CTA tile (64 or 128)
+    int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / n_tile
     int l_tx, l_ty, l_nt;                     // log2 of tiles_x, tiles_y, num_n_tiles (all powers of two: no runtime division)
     int num_kb;                               // cin / 64
-    int in_stages, a_stages, b_stages, b_resident, epi_bufs, epi_direct;
+    int in_stages, a_stages, b_stages, b_resident;
     uint32_t in_tx_bytes;                     // bytes the TMA unit delivers per input stage
     uint32_t in_stage_stride;                 // rounded to 1024
     uint32_t off_t, off_aux;                  // T / NZ|XA areas inside an input stage
-    uint32_t off_in, off_a, off_b, off_epi;   // smem offsets from the 1024-aligned base
+    uint32_t off_in, off_a, off_b;            // smem offsets from the 1024-aligned base
     uint32_t off_dw;                          // [10][cin] depthwise taps + bias staged in smem (0xFFFFFFFF: read from global)
     uint32_t off_stem;                        // STEM: [cin][4] + [cin] fromrgb table
     int prefetch;                             // L2 prefetch distance of the producer, in chunks / K-blocks
@@ -94,7 +92,7 @@ struct Params {
     // STEM pre-stage
     const float* stem_w;
     const float* stem_b;
-    // fused torgb + image path (SynthesisBlock.forward, migan_inference.py:308-313); needs all of cout in one region
+    // fused torgb + image path (SynthesisBlock.forward, migan_inference.py:308-313); needs all of cout in one tile
     int torgb, store_out;
     const float* rgb_w;                       // [3][cout]
     const float* rgb_b;                       // [3]
@@ -118,9 +116,8 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// try_wait with a suspend-time hint: the warp sleeps in hardware (NANOSLEEP.SYNCS) until the phase completes or the hint
-// elapses, instead of burning issue slots.  (The round-2 ncu source view attributed 25-32 % of all executed instructions
-// to the previous wait loop, which read %globaltimer on every iteration.)
+// try_wait with a suspend-time hint: the warp sleeps in hardware until the phase completes or the hint elapses,
+// instead of burning issue slots.
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -136,9 +133,9 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     return t;
 }
 // Bounded wait: a protocol bug must never hang the GPU -- record which wait gave up and trap instead.  The bound is
-// wall-clock time (seconds), so profiler replay, sanitizers or a co-tenant cannot turn a legitimately long wait into a
-// false positive.  The record goes to a host-mapped word (it survives the trap).  The clock is only looked at every
-// 1024 failed probes: the common path is the probe loop alone.
+// wall-clock time (seconds), so a profiler replay or a co-tenant cannot turn a legitimately long wait into a false
+// positive.  The record goes to a host-mapped word (it survives the trap).  The clock is only looked at every 1024
+// failed probes: the common path is the probe loop alone.
 __device__ __noinline__ void mbar_timeout(int code, uint32_t parity, int* error_flag) {
     if (error_flag) {
         *reinterpret_cast<volatile int*>(error_flag) = code | ((int)parity << 12) | ((int)(blockIdx.x & 0xFFF) << 16);
@@ -146,8 +143,8 @@ __device__ __noinline__ void mbar_timeout(int code, uint32_t parity, int* error_
     }
     __trap();
 }
-// kRelaxed: a waiter with slack (the consumers behind a double buffer) backs off between probes, so that it does not
-// compete for issue slots with the warps doing the arithmetic (round-2 ncu: a quarter of all executed instructions were probes).
+// kRelaxed: a waiter with slack (the producer behind a ring) backs off between probes, so that it does not compete for
+// issue slots with the warps doing the arithmetic.
 template <bool kRelaxed = false>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int code, int* error_flag) {
     if (mbar_try_wait(bar, parity)) return;
@@ -185,73 +182,58 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, 
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
                  ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-        ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void tma_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// wgmma: all 128 threads of the warpgroup issue together; the accumulators live in their registers.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Ties the accumulator registers to a point in the program: the compiler may not move their reads or writes across it
+// (the asynchronous wgmma writes them until wg_wait).
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-// The loaded registers are tied to the wait as in/out operands so the compiler cannot hoist
-// their uses above it (tcgen05.ld is asynchronous until wait::ld).
-__device__ __forceinline__ void tc_wait_ld(uint32_t (&v)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-                 :: "memory");
-}
-__device__ __forceinline__ void stg_v8(float* p, const float (&o)[32], int i) {
-    asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(o[i]), "f"(o[i + 1]), "f"(o[i + 2]),
-                 "f"(o[i + 3]), "f"(o[i + 4]), "f"(o[i + 5]), "f"(o[i + 6]), "f"(o[i + 7]) : "memory");
-}
+template <int N> struct Wgmma;
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major fp16 in shared memory, fp32 accumulators.
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(da), "l"(db), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(da), "l"(db), "r"(accumulate));
+    }
+};
 
-// UMMA shared-memory descriptor: K-major operand, 128-byte swizzle, rows of 64 fp16 (128 B),
-// 8-row groups 1024 B apart (SBO).  Bit layout: cute/arch/mma_sm100_desc.hpp SmemDescriptor.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// wgmma shared-memory descriptor: K-major operand, 128-byte swizzle, rows of 64 fp16 (128 B), 8-row groups 1024 B apart
+// (SBO).  Bit layout: cute/arch/mma_sm90_desc.hpp GmmaDescriptor.  Advancing the start address by 32 bytes steps 16
+// elements along K inside the swizzled row; by 64 rows x 128 B it selects the second m64 half of the M tile.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address  [0,14)
     d |= (uint64_t)1 << 16;                              // LBO (unused for swizzled K-major) [16,30)
     d |= (uint64_t)(1024 >> 4) << 32;                    // SBO = 1024 B   [32,46)
-    d |= (uint64_t)1 << 46;                              // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                              // layout type: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                              // layout type: SWIZZLE_128B [62,64)
     return d;
-}
-// Instruction descriptor (InstrDescriptor in the same header): D=f32, A=B=f16, K-major both, M=128.
-__device__ __forceinline__ uint32_t umma_idesc_f16(int n) {
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
 }
 
 struct TileCoord {
-    int n0, y0, x0, nt;   // first image / row / column of the M tile, N-tile (group) index
+    int n0, y0, x0, nt;   // first image / row / column of the M tile, N-tile index
 };
 __device__ __forceinline__ TileCoord decode_tile(const Params& p, int tile) {
     TileCoord c;
@@ -274,15 +256,157 @@ struct Ring {
     }
 };
 
+// mbarriers: [0,8) full_in  [8,16) empty_in  [16,20) full_a  [20,24) empty_a  [24,32) full_b  [32,40) empty_b
+constexpr int kNumBars = 40;
+__device__ __forceinline__ uint32_t bar_full_a(uint32_t bar0, int s) { return bar0 + 8u * (16 + s); }
+__device__ __forceinline__ uint32_t bar_empty_a(uint32_t bar0, int s) { return bar0 + 8u * (20 + s); }
+__device__ __forceinline__ uint32_t bar_full_b(uint32_t bar0, int s) { return bar0 + 8u * (24 + s); }
+__device__ __forceinline__ void mma_release(const Params& p, uint32_t bar0, int sa, int sb) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) {             // one arrival per warp: each warp waited for its own wgmma groups
+        mbar_arrive(bar_empty_a(bar0, sa));
+        if (!p.b_resident) mbar_arrive(bar0 + 8u * (32 + sb));
+    }
+}
+
+// ---------------------------------------------------------------------------------------
+// MMA + epilogue warpgroup.  NT = n_tile.  Accumulator register j * 4 + i * 2 + c of m64 half h holds
+// pixel row 64 h + 16 (warp % 4) + lane / 4 + 8 i, output channel 8 j + 2 (lane % 4) + c of the tile.
+// kSplit (fp32-faithful mode): main = Ah * Bh and corr = Ah * Bl + Al * Bh in two accumulator arrays, summed in the
+// epilogue.  Every wgmma has the same shape (m64 nNT k16), so the hardware orders the accumulator accesses of
+// consecutive instructions without a fence and they pipeline.  The 2^-11-sized corrections have their own accumulator
+// because the tensor core truncates on every accumulate: added into the large main sum they cost ~0.5 ulp of the MAIN
+// sum per MMA (one accumulator measured on the H100: mean-abs error 1.6e-4 on the migan-256 reference fixture, above
+// the 1e-4 bound).
+// ---------------------------------------------------------------------------------------
+template <int NT, bool kSplit>
+__device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base, uint32_t bar0, const float* s_rgb, int my_tiles) {
+    constexpr int NA = NT / 2;                       // accumulator registers per m64 half
+    constexpr int NC = kSplit ? NA : 1;              // correction accumulator (unused in fast mode)
+    const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int num_kb = p.num_kb;
+    const uint32_t b_stage_bytes = (uint32_t)NT * kKBlock * 2 * 2;   // [Bh ; Bl]
+    const int hw = p.tile_h * p.tile_w;
+    float acc[2][NA], cor[2][NC];
+    Ring ra(p.a_stages), rb(p.b_stages);
+    for (int it = 0; it < my_tiles; ++it) {
+        const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+        int prev_sa = 0, prev_sb = 0;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            const int sa = ra.stage;
+            mbar_wait(bar_full_a(bar0, sa), ra.phase, 210 + sa, p.error_flag);
+            ra.advance();
+            const int sb = p.b_resident ? kb : rb.stage;
+            mbar_wait(bar_full_b(bar0, sb), p.b_resident ? 0 : rb.phase, 220 + sb, p.error_flag);
+            if (!p.b_resident) rb.advance();
+            const uint32_t a_hi = smem_base + p.off_a + sa * kAStage;
+            const uint32_t b_hi = smem_base + p.off_b + sb * b_stage_bytes;
+            const uint64_t dah = wgmma_desc_sw128(a_hi), dal = wgmma_desc_sw128(a_hi + kABytes);
+            const uint64_t dbh = wgmma_desc_sw128(b_hi), dbl = wgmma_desc_sw128(b_hi + b_stage_bytes / 2);
+            wg_fence_acc(acc[0]);
+            wg_fence_acc(acc[1]);
+            if constexpr (kSplit) { wg_fence_acc(cor[0]); wg_fence_acc(cor[1]); }
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < kKBlock / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 32 >> 4);   // 16 fp16 = 32 bytes along K inside the SW128 row
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint64_t mh = (uint64_t)(h * 64 * 128 >> 4);
+                    Wgmma<NT>::mma(acc[h], dah + mh + adv, dbh + adv, (kb | k) != 0);
+                    if constexpr (kSplit) {
+                        Wgmma<NT>::mma(cor[h], dah + mh + adv, dbl + adv, (kb | k) != 0);
+                        Wgmma<NT>::mma(cor[h], dal + mh + adv, dbh + adv, 1u);
+                    }
+                }
+            }
+            wg_commit();
+            if (kb > 0) {                        // the previous K block's MMAs have retired: its A / B slots are free
+                wg_wait<1>();
+                mma_release(p, bar0, prev_sa, prev_sb);
+            }
+            prev_sa = sa; prev_sb = sb;
+        }
+        wg_wait<0>();
+        wg_fence_acc(acc[0]);
+        wg_fence_acc(acc[1]);
+        if constexpr (kSplit) { wg_fence_acc(cor[0]); wg_fence_acc(cor[1]); }
+        mma_release(p, bar0, prev_sa, prev_sb);
+
+        // ---- epilogue: the four pixel rows of this thread, straight from the accumulators ----
+        const int chan0 = tc.nt * NT;
+        const float scale_g = p.inv_scale * kActGain;
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int h = r >> 1, i = r & 1;
+            const int m = h * 64 + wq * 16 + (lane >> 2) + 8 * i;
+            const int pimg = tc.n0 + m / hw, poy = tc.y0 + (m / p.tile_w) % p.tile_h, pox = tc.x0 + m % p.tile_w;
+            const bool valid = pimg < p.n;
+            const float nz = p.noise ? __ldg(p.noise + poy * p.W + pox) : 0.f;
+            const float nz_g = nz * kActGain;
+            float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0 + 2 * (lane & 3);
+            float s0 = 0.f, s1 = 0.f, s2 = 0.f;      // torgb partial sums over this thread's channels
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+                float o[2];
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const float v = kSplit ? acc[h][j * 4 + i * 2 + c] + cor[h][(j * 4 + i * 2 + c) % NC] : acc[h][j * 4 + i * 2 + c];
+                    if (p.act) {                     // clamp(lrelu(f) * sqrt2) with the gain folded into the scale
+                        const float a = fmaf(v, scale_g, nz_g);
+                        o[c] = fminf(fmax3(a, a * kLreluAlpha, -kActClamp), kActClamp);
+                    } else {
+                        o[c] = fmaf(v, p.inv_scale, nz);
+                    }
+                }
+                if (p.torgb) {                       // 1x1 conv Cout -> 3 on the activated row (the tile holds all of cout)
+                    const int ch = 8 * j + 2 * (lane & 3);
+                    s0 = fmaf(o[1], s_rgb[ch + 1], fmaf(o[0], s_rgb[ch], s0));
+                    s1 = fmaf(o[1], s_rgb[p.cout + ch + 1], fmaf(o[0], s_rgb[p.cout + ch], s1));
+                    s2 = fmaf(o[1], s_rgb[2 * p.cout + ch + 1], fmaf(o[0], s_rgb[2 * p.cout + ch], s2));
+                }
+                if (p.store_out && valid) *reinterpret_cast<float2*>(out_px + 8 * j) = make_float2(o[0], o[1]);
+            }
+            if (p.torgb) {
+                // img = upsample(img_lo) + (torgb(x) + b)   (migan_inference.py:308-313); planar NCHW.  The quad holds the
+                // pixel's channels: sum its partials, then lane k of the quad writes colour k.
+#pragma unroll
+                for (int x = 1; x < 4; x <<= 1) {
+                    s0 += __shfl_xor_sync(0xffffffffu, s0, x);
+                    s1 += __shfl_xor_sync(0xffffffffu, s1, x);
+                    s2 += __shfl_xor_sync(0xffffffffu, s2, x);
+                }
+                const int k = lane & 3;
+                if (k < 3 && valid) {
+                    float rv = (k == 0 ? s0 : (k == 1 ? s1 : s2)) + s_rgb[kRgbBias + k];
+                    if (p.img_lo) {
+                        const int hl = p.H >> 1, wl = p.W >> 1;
+                        float up = 0.f;
+#pragma unroll
+                        for (int a = 0; a < 2; ++a)
+#pragma unroll
+                            for (int bb = 0; bb < 2; ++bb) {
+                                const int iy = (poy + (poy & 1) + 2 * a - 2) >> 1, ix = (pox + (pox & 1) + 2 * bb - 2) >> 1;
+                                const int ty = (poy & 1) + 2 * a, tx = (pox & 1) + 2 * bb;
+                                const bool ok = iy >= 0 && iy < hl && ix >= 0 && ix < wl;
+                                const float lo = ok ? __ldg(p.img_lo + (((size_t)pimg * 3 + k) * hl + iy) * wl + ix) : 0.f;
+                                up = fmaf(s_rgb[kRgbFir + (ty * 4 + tx) * 3 + k], lo, up);
+                            }
+                        rv = up + rv;
+                    }
+                    p.img_out[(((size_t)pimg * 3 + k) * p.H + poy) * p.W + pox] = rv;
+                }
+            }
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads, 1)
 sepconv_tc_kernel(const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
-    // mbarriers: [0,8) full_in  [8,16) empty_in  [16,20) full_a  [20,24) empty_a
-    //            [24,32) full_b  [32,40) empty_b  [40,42) full_acc  [42,44) empty_acc
-    __shared__ __align__(8) uint64_t bars[44];
-    __shared__ uint32_t tmem_base_slot;
-    __shared__ __align__(16) float s_rgb[3 * 256 + 4 + 48];   // torgb weights [3][cout<=256], bias[3(+1)], fir[16][3]
+    __shared__ __align__(8) uint64_t bars[kNumBars];
+    __shared__ __align__(16) float s_rgb[3 * kMaxTileN + 4 + 48];   // torgb weights [3][cout<=128], bias[3(+1)], fir[16][3]
 
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -291,19 +415,16 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
     const uint32_t bar0 = smem_u32(bars);
     auto full_in = [&](int s) { return bar0 + 8u * (0 + s); };
     auto empty_in = [&](int s) { return bar0 + 8u * (8 + s); };
-    auto full_a = [&](int s) { return bar0 + 8u * (16 + s); };
-    auto empty_a = [&](int s) { return bar0 + 8u * (20 + s); };
-    auto full_b = [&](int s) { return bar0 + 8u * (24 + s); };
-    auto empty_b2 = [&](int s) { return bar0 + 8u * (32 + s); };
-    auto full_acc = [&](int s) { return bar0 + 8u * (40 + s); };
-    auto empty_acc = [&](int s) { return bar0 + 8u * (42 + s); };
+    auto full_a = [&](int s) { return bar_full_a(bar0, s); };
+    auto empty_a = [&](int s) { return bar_empty_a(bar0, s); };
+    auto full_b = [&](int s) { return bar_full_b(bar0, s); };
+    auto empty_b = [&](int s) { return bar0 + 8u * (32 + s); };
 
     const int a_dw = (p.source != SEPCONV_SRC_SPLIT);
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.in_stages; ++s) { mbar_init(full_in(s), 1); mbar_init(empty_in(s), kNumProWarps / 2); }
-        for (int s = 0; s < p.a_stages; ++s) { mbar_init(full_a(s), a_dw ? kNumProWarps : 1); mbar_init(empty_a(s), 1); }
-        for (int s = 0; s < p.b_stages; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b2(s), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(full_acc(s), 1); mbar_init(empty_acc(s), 4); }
+        for (int s = 0; s < p.a_stages; ++s) { mbar_init(full_a(s), a_dw ? kNumProWarps : 1); mbar_init(empty_a(s), 4); }
+        for (int s = 0; s < p.b_stages; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (warp == kProducerWarp && lane == 0) {
@@ -311,7 +432,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
         else if (p.source == SEPCONV_SRC_STEM) prefetch_tensormap(&p.map_aux);
         else prefetch_tensormap(&p.map_in);
         if (p.source == SEPCONV_SRC_UP) { prefetch_tensormap(&p.map_t); if (p.up_has_noise) prefetch_tensormap(&p.map_aux); }
-        prefetch_tensormap(&p.map_w_hi); prefetch_tensormap(&p.map_w_lo); prefetch_tensormap(&p.map_out);
+        prefetch_tensormap(&p.map_w_hi); prefetch_tensormap(&p.map_w_lo);
     }
     if (p.torgb) {
         for (int i = threadIdx.x; i < 3 * p.cout; i += kThreads) s_rgb[i] = __ldg(p.rgb_w + i);
@@ -330,24 +451,17 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
         for (int i = threadIdx.x; i < p.cin; i += kThreads) st[4 * p.cin + i] = __ldg(p.stem_b + i);
     }
     pdl_trigger();           // the successor's blocks may start their own setup as soon as SMs free up
-    if (warp == kMmaWarp) {  // TMEM: all 512 columns (one CTA per SM by construction)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&tmem_base_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    pdl_wait();              // barriers, TMEM and the weight tables above are set up under the predecessor's tail; its output is read below
-    tc_fence_before();
+    pdl_wait();              // barriers and the weight tables above are set up under the predecessor's tail; its output is read below
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_slot;
 
     const int num_kb = p.num_kb;
     const int my_tiles = (p.num_tiles > (int)blockIdx.x) ? (p.num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    const int nts = p.nt_share;
-    const uint32_t b_stage_bytes = (uint32_t)p.n_tile * kKBlock * 2 * 2;   // [Bh ; Bl] of one accumulator region
+    const uint32_t b_stage_bytes = (uint32_t)p.n_tile * kKBlock * 2 * 2;   // [Bh ; Bl] of one N tile
 
-    if (warp == kProducerWarp) {
+    if (warp >= kProducerWarp) {
         // ================================ TMA producer ================================
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        if (warp == kProducerWarp && lane == 0) {
             // L2 prefetch cursor: the smem rings are too shallow to cover HBM latency at full bandwidth, so the
             // producer also asks the L2 for the data `prefetch` loads ahead (possibly in the next tile).
             int pf_it = 0, pf_kb = 0, pf_g = 0;
@@ -393,7 +507,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                     } else {
                         const int s = ra.stage;
                         if (p.prefetch) prefetch_next();
-                        mbar_wait(empty_a(s), ra.phase ^ 1, 110 + s, p.error_flag);
+                        mbar_wait<true>(empty_a(s), ra.phase ^ 1, 110 + s, p.error_flag);
                         ra.advance();
                         mbar_expect_tx(full_a(s), kAStage);
                         const int row0 = ((blockIdx.x + it * gridDim.x) >> p.l_nt) * kTileM;
@@ -401,223 +515,27 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                         tma_load_2d(smem_base + p.off_a + s * kAStage + kABytes, &p.map_a_lo, full_a(s), kb * kKBlock, row0);
                     }
                     if (!p.b_resident || it == 0) {
-                        for (int sub = 0; sub < nts; ++sub) {
-                            const int s = p.b_resident ? kb : rb.stage;
-                            if (!p.b_resident) { mbar_wait(empty_b2(s), rb.phase ^ 1, 120 + s, p.error_flag); rb.advance(); }
-                            mbar_expect_tx(full_b(s), b_stage_bytes);
-                            const uint32_t dst = smem_base + p.off_b + s * b_stage_bytes;
-                            const int row = (tc.nt * nts + sub) * p.n_tile;
-                            tma_load_2d(dst, &p.map_w_hi, full_b(s), kb * kKBlock, row);
-                            tma_load_2d(dst + b_stage_bytes / 2, &p.map_w_lo, full_b(s), kb * kKBlock, row);
-                        }
+                        const int s = p.b_resident ? kb : rb.stage;
+                        if (!p.b_resident) { mbar_wait<true>(empty_b(s), rb.phase ^ 1, 120 + s, p.error_flag); rb.advance(); }
+                        mbar_expect_tx(full_b(s), b_stage_bytes);
+                        const uint32_t dst = smem_base + p.off_b + s * b_stage_bytes;
+                        const int row = tc.nt * p.n_tile;
+                        tma_load_2d(dst, &p.map_w_hi, full_b(s), kb * kKBlock, row);
+                        tma_load_2d(dst + b_stage_bytes / 2, &p.map_w_lo, full_b(s), kb * kKBlock, row);
                     }
                 }
             }
         }
-    } else if (warp == kMmaWarp) {
-        // ================================ MMA issuer ==================================
-        const uint32_t idesc = umma_idesc_f16(p.n_tile), idesc2 = umma_idesc_f16(2 * p.n_tile);
-        Ring ra(p.a_stages), rb(p.b_stages);
-        for (int it = 0; it < my_tiles; ++it) {
-            // Accumulator region = [main | correction] column blocks.  The 2^-11-sized correction products
-            // (Al*Bh + Ah*Bl) go to their own accumulator: the tensor core truncates on every accumulate,
-            // and adding them into the large main sum would cost ~0.5 ulp of the MAIN sum per MMA.
-            if (nts == 1) {
-                mbar_wait(empty_acc(it & 1), ((it >> 1) & 1) ^ 1, 200 + (it & 1), p.error_flag);
-            } else {
-                mbar_wait(empty_acc(0), (it & 1) ^ 1, 200, p.error_flag);
-                mbar_wait(empty_acc(1), (it & 1) ^ 1, 201, p.error_flag);
-            }
-            tc_fence_after();
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int sa = ra.stage;
-                mbar_wait(full_a(sa), ra.phase, 210 + sa, p.error_flag);
-                ra.advance();
-                for (int sub = 0; sub < nts; ++sub) {
-                    const int sb = p.b_resident ? kb : rb.stage;
-                    mbar_wait(full_b(sb), p.b_resident ? 0 : rb.phase, 220 + sb, p.error_flag);
-                    if (!p.b_resident) rb.advance();
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const int region = (nts == 1) ? (it & 1) : sub;
-                        const uint32_t tmem_d = tmem_base + (uint32_t)(region * 2 * p.n_tile);
-                        const uint32_t tmem_c = tmem_d + (uint32_t)p.n_tile;
-                        const uint32_t a_hi = smem_base + p.off_a + sa * kAStage, a_lo = a_hi + kABytes;
-                        const uint32_t b_hi = smem_base + p.off_b + sb * b_stage_bytes;
-                        const uint64_t dah = umma_desc_sw128(a_hi), dal = umma_desc_sw128(a_lo);
-                        const uint64_t dbh = umma_desc_sw128(b_hi);   // Bl sits right behind Bh: [Bh ; Bl] is one K-major operand of 2*n_tile rows
-#pragma unroll
-                        for (int k = 0; k < kKBlock / 16; ++k) {
-                            const uint64_t adv = (uint64_t)(k * 32 >> 4);   // 16 fp16 = 32 bytes along K inside the SW128 row
-                            if (p.passes == 3) {
-                                // [main | corr] = Ah * [Bh ; Bl]^T in ONE instruction (N = 2*n_tile): Ah is read from shared
-                                // memory once for both products; then corr += Al * Bh.
-                                tc_mma_f16(tmem_d, dah + adv, dbh + adv, idesc2, (kb | k) != 0);
-                                tc_mma_f16(tmem_c, dal + adv, dbh + adv, idesc, 1u);
-                            } else {
-                                tc_mma_f16(tmem_d, dah + adv, dbh + adv, idesc, (kb | k) != 0);
-                            }
-                        }
-                        if (!p.b_resident) tc_commit(empty_b2(sb));
-                        if (sub == nts - 1) tc_commit(empty_a(sa));      // A slot reusable once these MMAs retire
-                        if (kb == num_kb - 1) tc_commit(full_acc(region));   // accumulator region complete
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp >= kEpiWarp0) {
-        // ================================ epilogue ====================================
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access
-        const int row = q * 32 + lane;               // pixel row of the M tile
-        const int hw = p.tile_h * p.tile_w;
-        const int img_l = row / hw, yl = (row / p.tile_w) % p.tile_h, xl = row % p.tile_w;   // once per kernel
-        const int chunks = p.n_tile / 32;
-        int buf = 0;
-        // each epilogue warp stages and TMA-stores its own 32 pixel rows: no cross-warp barrier in the loop
-        const int q_img = (q * 32) / hw, q_rem = (q * 32) % hw, q_y = q_rem / p.tile_w, q_x = q_rem % p.tile_w;
-        const uint32_t stage_base = smem_base + p.off_epi + (uint32_t)(q * p.epi_bufs) * kEpiWarpBuf;
-        for (int it = 0; it < my_tiles; ++it) {
-            const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
-          // torgb partial sums live across the N halves of the tile (nts = 2: the same thread drains both regions of its pixel)
-          P2 rgb0 = p2zero(), rgb1 = p2zero(), rgb2 = p2zero();   // (even, odd) partial sums of the three torgb outputs
-          float lo_tap[12];
-          for (int sub = 0; sub < nts; ++sub) {
-            // accumulator region + the parity of its current use: consecutive tiles alternate regions (nts = 1), or
-            // every tile uses both regions for its two N halves (nts = 2)
-            const int e = (nts == 1) ? (it & 1) : sub;
-            const uint32_t use_parity = (nts == 1) ? ((it >> 1) & 1) : (it & 1);
-            const uint32_t acc_col = (uint32_t)(e * 2 * p.n_tile);
-            const int chan0 = (tc.nt * nts + sub) * p.n_tile;
-            // operands of the tile's tail (noise, low-res image taps) are fetched BEFORE waiting for the
-            // accumulator so that their L2 latency hides behind the MMA
-            float nz = 0.f;
-            const int pimg = tc.n0 + img_l, poy = tc.y0 + yl, pox = tc.x0 + xl;
-            if (p.noise) nz = __ldg(p.noise + poy * p.W + pox);
-            if (p.torgb && p.img_lo && sub == 0) {
-                const int h = p.H >> 1, w = p.W >> 1;
-#pragma unroll
-                for (int a = 0; a < 2; ++a)
-#pragma unroll
-                    for (int bb = 0; bb < 2; ++bb) {
-                        const int iy = (poy + (poy & 1) + 2 * a - 2) >> 1, ix = (pox + (pox & 1) + 2 * bb - 2) >> 1;
-                        const bool ok = pimg < p.n && iy >= 0 && iy < h && ix >= 0 && ix < w;
-#pragma unroll
-                        for (int k = 0; k < 3; ++k)
-                            lo_tap[(a * 2 + bb) * 3 + k] = ok ? __ldg(p.img_lo + (((size_t)pimg * 3 + k) * h + iy) * w + ix) : 0.f;
-                    }
-            }
-            mbar_wait<true>(full_acc(e), use_parity, 300 + e, p.error_flag);
-            tc_fence_after();
-            const float scale_g = p.inv_scale * kActGain, nz_g = nz * kActGain;
-            float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0;
-            for (int j = 0; j < chunks; ++j) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc_col + (uint32_t)(j * 32);
-                tc_ld32(taddr, v);
-                if (p.passes == 3) {
-                    uint32_t c[32];
-                    tc_ld32(taddr + (uint32_t)p.n_tile, c);   // both loads in flight before the wait
-                    tc_wait_ld(v);
-                    tc_wait_ld(c);
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        const f2 t = unpk(fadd2(pk(__uint_as_float(v[i]), __uint_as_float(v[i + 1])),
-                                                pk(__uint_as_float(c[i]), __uint_as_float(c[i + 1]))));
-                        v[i] = __float_as_uint(t.x); v[i + 1] = __float_as_uint(t.y);
-                    }
-                } else {
-                    tc_wait_ld(v);
-                }
-                if (j == chunks - 1) {               // accumulator fully read: hand it back to the MMA warp
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(empty_acc(e));
-                }
-                float o[32];
-                if (p.act) {                         // clamp(lrelu(f) * sqrt2) with the gain folded into the scale
-                    const P2 sc2 = pk(scale_g, scale_g), nz2 = pk(nz_g, nz_g), al2 = pk(kLreluAlpha, kLreluAlpha);
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        const P2 a = ffma2(pk(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), sc2, nz2);
-                        const P2 b = fmul2(a, al2);
-                        o[i] = fminf(fmax3(a.x, b.x, -kActClamp), kActClamp);
-                        o[i + 1] = fminf(fmax3(a.y, b.y, -kActClamp), kActClamp);
-                    }
-                } else {
-                    const P2 sc2 = pk(p.inv_scale, p.inv_scale), nz2 = pk(nz, nz);
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        const f2 a = unpk(ffma2(pk(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), sc2, nz2));
-                        o[i] = a.x; o[i + 1] = a.y;
-                    }
-                }
-                if (p.torgb) {   // 1x1 conv Cout -> 3 on the activated row: even/odd partial sums, packed FMAs, weights broadcast from smem
-                    const float4* w0 = reinterpret_cast<const float4*>(s_rgb + chan0 + j * 32);
-                    const float4* w1 = reinterpret_cast<const float4*>(s_rgb + p.cout + chan0 + j * 32);
-                    const float4* w2 = reinterpret_cast<const float4*>(s_rgb + 2 * p.cout + chan0 + j * 32);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const float4 a = w0[i], b = w1[i], c = w2[i];
-                        const P2 o01 = pk(o[4 * i], o[4 * i + 1]), o23 = pk(o[4 * i + 2], o[4 * i + 3]);
-                        rgb0 = ffma2(o01, pk(a.x, a.y), rgb0); rgb0 = ffma2(o23, pk(a.z, a.w), rgb0);
-                        rgb1 = ffma2(o01, pk(b.x, b.y), rgb1); rgb1 = ffma2(o23, pk(b.z, b.w), rgb1);
-                        rgb2 = ffma2(o01, pk(c.x, c.y), rgb2); rgb2 = ffma2(o23, pk(c.z, c.w), rgb2);
-                    }
-                }
-                if (!p.store_out) continue;          // last block: the feature map is consumed by torgb only
-                if (p.epi_direct) {                  // 128 contiguous bytes per thread, four 256-bit stores
-                    if (pimg < p.n) {
-                        float* dstp = out_px + j * 32;
-                        stg_v8(dstp, o, 0); stg_v8(dstp + 8, o, 8); stg_v8(dstp + 16, o, 16); stg_v8(dstp + 24, o, 24);
-                    }
-                    continue;
-                }
-                // this warp's staging buffer `buf` must have been drained by its own TMA store issued epi_bufs chunks ago
-                if (lane == 0) { if (p.epi_bufs == 2) tma_wait_group_read<1>(); else tma_wait_group_read<0>(); }
-                __syncwarp();
-                const uint32_t dst = stage_base + buf * kEpiWarpBuf + lane * 128;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const uint32_t a = dst + (((uint32_t)c ^ (uint32_t)(lane & 7)) << 4);
-                    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(o[4 * c]), "f"(o[4 * c + 1]),
-                                 "f"(o[4 * c + 2]), "f"(o[4 * c + 3]) : "memory");
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) {
-                    tma_store_4d(&p.map_out, stage_base + buf * kEpiWarpBuf, chan0 + j * 32, tc.x0 + q_x, tc.y0 + q_y, tc.n0 + q_img);
-                    tma_commit_group();
-                }
-                buf = (buf + 1 == p.epi_bufs) ? 0 : buf + 1;
-            }
-            if (p.torgb && sub == nts - 1) {
-                // img = upsample(img_lo) + (torgb(x) + b)   (migan_inference.py:308-313); planar NCHW
-                if (pimg < p.n) {
-                    float r[3] = {rgb0.x + rgb0.y + s_rgb[kRgbBias], rgb1.x + rgb1.y + s_rgb[kRgbBias + 1], rgb2.x + rgb2.y + s_rgb[kRgbBias + 2]};
-                    if (p.img_lo) {
-                        float up[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-                        for (int a = 0; a < 2; ++a)
-#pragma unroll
-                            for (int bb = 0; bb < 2; ++bb) {
-                                const int ty = (poy & 1) + 2 * a, tx = (pox & 1) + 2 * bb;
-#pragma unroll
-                                for (int k = 0; k < 3; ++k)
-                                    up[k] = fmaf(s_rgb[kRgbFir + (ty * 4 + tx) * 3 + k], lo_tap[(a * 2 + bb) * 3 + k], up[k]);
-                            }
-#pragma unroll
-                        for (int k = 0; k < 3; ++k) r[k] = up[k] + r[k];
-                    }
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) p.img_out[(((size_t)pimg * 3 + k) * p.H + poy) * p.W + pox] = r[k];
-                }
-            }
-          }
-        }
-        if (lane == 0) tma_wait_group_all();
-    } else if (a_dw) {
+    } else if (warp >= kMmaWarp0) {
+        // ================================ MMA + epilogue ==============================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMmaRegs));
+        if (p.passes == 3) mma_epilogue<64, true>(p, smem_base, bar0, s_rgb, my_tiles);
+        else if (p.n_tile == 128) mma_epilogue<128, false>(p, smem_base, bar0, s_rgb, my_tiles);
+        else mma_epilogue<64, false>(p, smem_base, bar0, s_rgb, my_tiles);
+    } else {
         // ================================ prologue (pre-stage + depthwise) ========================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kProRegs));
+        if (!a_dw) return;
         const int g = warp >> 2;                          // channel half of the K-block this group produces
         const int tg = threadIdx.x - g * 128;
         Ring rin(p.in_stages, g, 2), ra(p.a_stages);     // this group owns input stages g, g+2, ...
@@ -658,13 +576,6 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                 }
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
     }
 }
 
@@ -770,10 +681,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     if ((d.source == SEPCONV_SRC_UP || d.source == SEPCONV_SRC_STEM) && res < 16) return "fused prologues need 8 x 16 tiles (res >= 16)";
     p.w9 = d.w9; p.bias = d.bias; p.noise = d.noise; p.inv_scale = d.inv_scale; p.out = d.out;
     p.n = n; p.H = res; p.W = res; p.cin = cin; p.cout = cout; p.act = d.act; p.passes = d.passes;
-    p.n_tile = (cout == 64) ? 64 : 128;
-    // Two 128-column accumulator regions can hold the two N halves of one M tile: the A operand (and for the fused
-    // sources the whole prologue) is then produced once per pixel tile instead of once per N tile.
-    p.nt_share = (cout >= 256 && (env_int("MIGAN_TC_NT_SHARE", 1) != 0 || (d.rgb && cout == 256))) ? 2 : 1;   // fused torgb at 256 needs both halves in one CTA
+    p.n_tile = (cout == 64 || d.passes == 3) ? 64 : kMaxTileN;   // main + corr of 64 channels fill the accumulators
     p.num_kb = cin / kKBlock;
     if (dw) {   // spatial tiles with halo
         p.tile_w = res >= 16 ? 16 : res;
@@ -784,16 +692,16 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     }
     p.tile_n = kTileM / (p.tile_w * p.tile_h);
     p.tiles_x = res / p.tile_w; p.tiles_y = res / p.tile_h; p.tiles_n = (n + p.tile_n - 1) / p.tile_n;
-    int dev0 = 0, sms0 = 148;
+    int dev0 = 0, sms0 = 132;
     cudaGetDevice(&dev0);
     cudaDeviceGetAttribute(&sms0, cudaDevAttrMultiProcessorCount, dev0);
-    // Few pixel tiles (the 4 x 4 ... 16 x 16 levels at small batches): a CTA that owns 256 output channels streams the whole
-    // weight matrix and issues every MMA of its tile while most SMs idle.  Narrow N tiles spread the layer over 4 x the CTAs.
-    if (!d.rgb && cout >= 256 && p.tiles_x * p.tiles_y * p.tiles_n * (cout / (p.n_tile * p.nt_share)) * 2 < sms0 &&
+    // Few pixel tiles (the 4 x 4 ... 16 x 16 levels at small batches): most SMs would idle while a few CTAs stream the
+    // weight matrix.  Narrow N tiles spread the layer over 2 x the CTAs.
+    if (!d.rgb && p.n_tile > 64 && cout >= 256 && p.tiles_x * p.tiles_y * p.tiles_n * (cout / p.n_tile) * 2 < sms0 &&
         env_int("MIGAN_TC_SMALL_N", 1) != 0) {
-        p.n_tile = 64; p.nt_share = 1;
+        p.n_tile = 64;
     }
-    p.num_n_tiles = cout / (p.n_tile * p.nt_share);
+    p.num_n_tiles = cout / p.n_tile;
     p.num_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.num_n_tiles;
     auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
     p.l_tx = ilog2(p.tiles_x); p.l_ty = ilog2(p.tiles_y); p.l_nt = ilog2(p.num_n_tiles);
@@ -819,7 +727,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
 
     p.store_out = 1;
     if (d.rgb) {
-        if (p.num_n_tiles != 1 || cout > 256) return "fused torgb needs all output channels of a pixel tile in one CTA (cout <= 256)";
+        if (p.num_n_tiles != 1) return "fused torgb needs all output channels of a pixel tile in one CTA tile (cout <= 64, or 128 in fast mode)";
         p.torgb = 1; p.store_out = d.rgb->store_out;
         p.rgb_w = d.rgb->w; p.rgb_b = d.rgb->b; p.rgb_fir = d.rgb->fir; p.img_lo = d.rgb->img_lo; p.img_out = d.rgb->img_out;
     }
@@ -830,19 +738,16 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     // The input ring is shared by the two prologue groups (even chunks -> group 0, odd -> group 1):
     // the stage count must be EVEN so that each stage always belongs to one group and every waiter
     // observes every phase of its barriers (parity waits alias otherwise).
-    p.b_resident = (p.num_n_tiles == 1 && p.nt_share == 1 && (uint32_t)p.num_kb * b_stage <= 65536) ? 1 : 0;
+    p.b_resident = (p.num_n_tiles == 1 && (uint32_t)p.num_kb * b_stage <= 65536) ? 1 : 0;
     const uint32_t tables = dw ? 40u * cin + (d.source == SEPCONV_SRC_STEM ? 20u * cin : 0u) : 0u;
-    const int epi_mode = env_int("MIGAN_TC_EPI", 0);   // 0 auto, 1 staged only, 2 direct
     bool found = false;
-    // candidate configurations in order of preference: deeper input ring first, then more staging, then the
-    // staging-free epilogue (256-bit stores straight from registers)
-    struct Cand { int in_stages, epi_bufs, direct, b_stages, a_stages; };
+    // candidate configurations in order of preference: deeper input ring first, then a deeper A ring (the prologue runs
+    // ahead while the MMA warpgroup drains its accumulators)
+    struct Cand { int in_stages, b_stages, a_stages; };
     std::vector<Cand> cands;
     {
-        const int a_st = dw ? 2 : 3;
         const int b_res = p.b_resident ? p.num_kb : 0;
-        // input ring depths to try, deepest first (even: each prologue group owns every other stage).  Round-2 ncu: with two
-        // stages per group the prologue warps of a 128 -> 128 layer wait for TMA data 29 % of the time.
+        // input ring depths to try, deepest first (even: each prologue group owns every other stage)
         const int max_in = env_int("MIGAN_TC_MAX_IN", 6);
         std::vector<int> ins;
         if (dw) { for (int v = 6; v >= 2; v -= 2) if (v <= max_in) ins.push_back(v); } else ins.push_back(0);
@@ -850,25 +755,19 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
         for (int bi = 0; bi < 2; ++bi) {
             if (bi == 1 && bopts[1] == bopts[0]) break;
             const int bs = bopts[bi];
-            for (int in_st : ins) {
-                if (!p.store_out) { cands.push_back({in_st, 0, 0, bs, a_st}); continue; }
-                if (epi_mode != 2) { cands.push_back({in_st, 2, 0, bs, a_st}); cands.push_back({in_st, 1, 0, bs, a_st}); }
-                if (epi_mode != 1) cands.push_back({in_st, 0, 1, bs, a_st});
-            }
+            for (int in_st : ins)
+                for (int a_st : {4, dw ? 2 : 3}) cands.push_back({in_st, bs, a_st});
         }
     }
     uint32_t smem_bytes = 0;
     for (const Cand& c : cands) {
-        const uint32_t epi = (uint32_t)c.epi_bufs * 4u * kEpiWarpBuf;
-        const uint32_t total = (uint32_t)c.in_stages * p.in_stage_stride + (uint32_t)c.a_stages * kAStage + (uint32_t)c.b_stages * b_stage + epi + tables;
+        const uint32_t total = (uint32_t)c.in_stages * p.in_stage_stride + (uint32_t)c.a_stages * kAStage + (uint32_t)c.b_stages * b_stage + tables;
         if (total > budget) continue;
-        p.in_stages = c.in_stages; p.a_stages = c.a_stages; p.b_stages = c.b_stages; p.epi_bufs = std::max(c.epi_bufs, 1);
-        p.epi_direct = c.direct;
+        p.in_stages = c.in_stages; p.a_stages = c.a_stages; p.b_stages = c.b_stages;
         p.off_in = 0;
         p.off_a = (uint32_t)c.in_stages * p.in_stage_stride;
         p.off_b = p.off_a + (uint32_t)c.a_stages * kAStage;
-        p.off_epi = p.off_b + (uint32_t)c.b_stages * b_stage;
-        p.off_dw = dw ? p.off_epi + epi : 0xFFFFFFFFu;
+        p.off_dw = dw ? p.off_b + (uint32_t)c.b_stages * b_stage : 0xFFFFFFFFu;
         p.off_stem = p.off_dw + 40u * cin;
         smem_bytes = total + 1024;
         found = true;
@@ -876,7 +775,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     }
     if (!found) return "shared memory budget exceeded";
     if (p.in_stages > 8 || p.a_stages > 4 || p.b_stages > 8) return "internal: ring too deep for the barrier table";
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     p.error_flag = (dev >= 0 && dev < kMaxDevices) ? g_error_flag[dev] : nullptr;
@@ -918,16 +817,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
         if ((err = encode_map(&p.map_w_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.w_hi, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
         if ((err = encode_map(&p.map_w_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.w_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
     }
-    if (d.out) {
-        const uint64_t dims[4] = {(uint64_t)cout, (uint64_t)res, (uint64_t)res, (uint64_t)n};
-        const uint64_t str[3] = {(uint64_t)cout * 4, (uint64_t)res * cout * 4, (uint64_t)res * res * cout * 4};
-        // one epilogue warp stores 32 consecutive pixel rows of the tile: quarter box
-        const uint32_t qw = (uint32_t)std::min(p.tile_w, 32), qh = (uint32_t)std::min(p.tile_h, 32 / (int)qw), qn = 32u / (qw * qh);
-        const uint32_t box[4] = {32u, qw, qh, qn};
-        if ((err = encode_map(&p.map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
-    } else if (p.store_out) {
-        return "no output tensor";
-    }
+    if (!d.out && p.store_out) return "no output tensor";
     // Persistent grid = one CTA per SM.  MIGAN_TC_RESERVE_SMS leaves SMs free for a concurrently running collective.
     const int reserve = std::max(0, std::min(env_int("MIGAN_TC_RESERVE_SMS", 0), sms / 2));
     args->grid = (unsigned)std::min(p.num_tiles, sms - reserve);

@@ -1,4 +1,4 @@
-// tcgen05 fused SeparableConv2d kernel: host-side plan + launcher (sepconv_tc.cu).
+// wgmma fused SeparableConv2d kernel: host-side plan + launcher (sepconv_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

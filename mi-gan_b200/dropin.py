@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference script with the B200 generator swapped in.
+"""Run an UNMODIFIED reference script with the H100 generator swapped in.
 
     PYTHONPATH=/path/to/MI-GAN:/path/to/this/repo python -m migan_b200.dropin scripts.demo \
         --model-name migan-512 --model-path models/migan_512_places2.pt \

@@ -1,4 +1,4 @@
-"""`Generator(resolution).forward(x[N,4,R,R]) -> img[N,3,R,R]` on B200.
+"""`Generator(resolution).forward(x[N,4,R,R]) -> img[N,3,R,R]` on H100.
 
 Drop-in for `lib.model_zoo.migan_inference.Generator` (reference
 lib/model_zoo/migan_inference.py:355-369): same constructor, same `state_dict` keys /
@@ -114,7 +114,7 @@ class _Engine:
 
 
 class Generator(nn.Module):
-    """MI-GAN inference generator, B200-native.  See module docstring."""
+    """MI-GAN inference generator, H100-native.  See module docstring."""
 
     def __init__(self, resolution: int = 256, path: Optional[str] = None):
         super().__init__()
@@ -193,7 +193,7 @@ class Generator(nn.Module):
         if x.dim() != 4 or x.shape[1] != 4 or x.shape[2] != r or x.shape[3] != r:
             raise RuntimeError("expected x of shape [N, 4, %d, %d] (mask-0.5, img*mask), got %s" % (r, r, tuple(x.shape)))
         if not x.is_cuda:
-            raise RuntimeError("migan_b200.Generator runs on B200 (sm_100a) only; got a %s tensor. "
+            raise RuntimeError("migan_b200.Generator runs on H100 (sm_90a) only; got a %s tensor. "
                                "There is no CPU fallback (the CPU oracle lives in oracle/ for tests)." % x.device)
         if x.dtype != torch.float32:
             raise RuntimeError("expected float32 input, got %s" % x.dtype)

@@ -1,4 +1,4 @@
-"""sm_100a drop-ins for the reference's `torch_utils/ops` used around the generator path:
+"""sm_90a drop-ins for the reference's `torch_utils/ops` used around the generator path:
 `upfirdn2d` (+ `setup_filter`, `filter2d`, `upsample2d`, `downsample2d`), `bias_act` and the 1x1
 branches of `conv2d_resample`.  Same function names, argument meaning and error behaviour as the
 reference (torch_utils/ops/upfirdn2d.py:72-384, bias_act.py:55-89, conv2d_resample.py:59-154);

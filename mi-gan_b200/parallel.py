@@ -19,20 +19,16 @@ import torch.distributed as dist
 
 
 def resolve_gather(gather: str, world_size: int) -> str:
-    """'auto' -> the implementation that measured best at this world size on B200s (round 2, migan-512, 32 images per GPU):
-    2 GPUs: copy engines 10.23 ms/step vs NCCL all-gather 10.52 (one GPU 9.97);  8 GPUs: NCCL all-gather 11.90 ms/step vs copy
-    engines 13.8-14.9 (one GPU 9.70).  4 GPUs were not measured and take the NCCL path."""
+    """'auto' -> the copy-engine gather at 2 GPUs (no SM is taken from the compute kernels), the NCCL all-gather above
+    (the per-peer copies of the copy-engine form serialise against the compute stream as the peer count grows)."""
     if gather != "auto":
         return gather
     return "ce" if world_size == 2 else "nccl"
 
 
 def nccl_channels_for(world_size: int) -> int:
-    """Channels (= SMs left free) for the NCCL all-gather.  Measured with 8 channels: the collective moves ~59 GB/s into each
-    rank (7.4 GB/s per channel) -- 700 MB per step at 8 GPUs = 11.9 ms, longer than the 9.7 ms step it should hide under, and
-    exactly the step time measured there (profiles/r02_scale_variants.md); 300 MB at 4 GPUs = 5 ms.  12 channels bring the
-    8-GPU gather to ~8 ms for 4 more SMs (+0.3 ms of compute).  The 12-channel point is DERIVED from the 8-channel
-    measurement, not measured itself (the round's GPU budget was spent)."""
+    """Channels (= SMs left free) for the NCCL all-gather: the bytes to gather grow with the world size while the step
+    they should hide under does not, so 8 GPUs get more channels than 4.  Not tuned on H100s."""
     return 12 if world_size > 4 else 8
 
 
@@ -41,13 +37,11 @@ def configure_overlap(reserve_sms: int = None, nccl_channels: int = None, gather
 
     gather = "ce": the output all-gather moves its bytes with the copy engines (peer-to-peer reads over NVLink, see
     `ShardedGenerator`); the only NCCL kernel per step is an 8-byte all-reduce used as the ready signal, so the persistent
-    tensor-core kernel keeps all 148 SMs (no reservation).
+    tensor-core kernel keeps every SM (no reservation).
     gather = "nccl": `all_gather_into_tensor` runs on NCCL's SM-resident copy kernels, one SM per channel, concurrently with
     the next batch's kernels.  The persistent kernel uses one CTA per SM -- if they collide, its last CTAs run as a second
     wave -- so NCCL is limited to `nccl_channels` channels (default `nccl_channels_for(world_size)`) and the persistent grids
-    leave as many SMs free (`reserve_sms`).  Measured
-    on 2 B200s (migan-512, 32 img/GPU, round 1): 14.27 ms/step without the reservation, 13.3-13.4 ms with 4-8 SMs reserved
-    (12.9 ms on one GPU).
+    leave as many SMs free (`reserve_sms`).
     gather = "auto" (default): see `resolve_gather`; `world_size` defaults to the WORLD_SIZE of the launcher.
     Respects values already present in the environment."""
     if world_size is None:
@@ -91,7 +85,7 @@ class GatherHandle:
 
 class ShardedGenerator:
     """Data-parallel wrapper.  `model` is any callable x[n,4,R,R] -> y[n,3,R,R] on this rank's device
-    (the B200 `Generator`; CPU stand-ins are used by the gloo tests).
+    (the H100 `Generator`; CPU stand-ins are used by the gloo tests).
 
     gather = "nccl": one `all_gather_into_tensor` per batch (NCCL's copy kernels, SM-resident).
     gather = "ce" (CUDA tensors, all ranks on one box): the same all-gather with the bytes moved by the copy engines.  Every
@@ -100,13 +94,9 @@ class ShardedGenerator:
       rank's y is in place" signal -- and (3) pulls the 7 peer shards into a fresh gathered tensor with peer-to-peer
       `cudaMemcpyAsync` reads over NVLink on a side stream.  No SM is taken from the compute kernels, so nothing has to be
       reserved for the collective, and the pull of batch t overlaps the compute of batch t+1.
-      Measured (round 2): 2 B200s 10.23 ms/step = 0.975 of 2 x one GPU; 8 B200s 13.8-14.9 ms/step -- there the NCCL path is
-      faster (11.9).  Variants tried on hardware and dropped: the same pull with a staggered source order and 2 SMs left
-      free for the signal's kernel (13.8 ms at 8 GPUs); a push form with bare `cudaMemcpyAsync` on the sender's own
-      streams (10.26 ms at 2 GPUs, 41 ms at 8); signalling with `cuStreamWaitValue32` and 4-byte peer writes instead of
-      the all-reduce (no collective kernel; bit-exact but 11.3 ms at 2 GPUs: a stream parked in a memory wait delays the
-      streams sharing its hardware queue).  `tools/p2p_probe.py` holds the primitive measurements (peer copy 475-550 GB/s,
-      signal latency 8 us, no slow-down of a concurrent forward).
+      Variants that were tried and dropped: a push form with bare `cudaMemcpyAsync` on the sender's own streams, and
+      signalling with `cuStreamWaitValue32` plus 4-byte peer writes instead of the all-reduce (a stream parked in a memory
+      wait delays the streams sharing its hardware queue).  `tools/p2p_probe.py` measures the primitives.
     gather = "auto" (default): `resolve_gather` -- "ce" at 2 GPUs, "nccl" above."""
 
     RING = 3   # published y buffers per rank: slot t % RING is rewritten only after the ready signal of step t - RING + 1

@@ -36,7 +36,7 @@ def main():
     except Exception as e:  # a trapped pipeline wait leaves a host-mapped record naming the barrier
         from migan_b200 import _abi
         print("[diag] FAILED: %s" % str(e).splitlines()[-1])
-        print("[diag] tcgen05 timeout record: 0x%x" % (_abi.load().migan_debug_tc_timeout(0) & 0xFFFFFFFF), flush=True)
+        print("[diag] tensor-core pipeline timeout record: 0x%x" % (_abi.load().migan_debug_tc_timeout(0) & 0xFFFFFFFF), flush=True)
         sys.exit(3)
     d = (y.cpu() - want).abs()
     print("[diag] path=%s R=%d N=%d launches=%d  FINAL max-abs=%.3e mean-abs=%.3e |y|max=%.3f"

@@ -1,9 +1,8 @@
 #!/bin/bash
-# Bring-up matrix of the fused tensor-core kernel's switches (one process per configuration: a trap poisons the context).
+# Bring-up matrix of the fused tensor-core kernel's fusion switches (one process per configuration: a trap poisons the context).
 #   tests/bringup/tc_matrix.sh <res> <n>
 R=${1:-128}; N=${2:-2}
-for cfg in "0 0 1" "0 1 1" "0 0 2" "0 1 0" "1 0 1" "2 0 1" "3 1 0"; do
-  set -- $cfg
-  echo "== MIGAN_FUSE=$1 MIGAN_TC_NT_SHARE=$2 MIGAN_TC_EPI=$3  (R=$R N=$N)"
-  CUDA_LAUNCH_BLOCKING=1 MIGAN_FUSE=$1 MIGAN_TC_NT_SHARE=$2 MIGAN_TC_EPI=$3 timeout 120 python tests/bringup/gpu_diag.py --path tc --res $R --n $N --taps 1 2>&1 | grep -E "FINAL|MISMATCH|FAILED|record" | head -12
+for fuse in 0 1 2 3; do
+  echo "== MIGAN_FUSE=$fuse  (R=$R N=$N)"
+  CUDA_LAUNCH_BLOCKING=1 MIGAN_FUSE=$fuse timeout 120 python tests/bringup/gpu_diag.py --path tc --res $R --n $N --taps 1 2>&1 | grep -E "FINAL|MISMATCH|FAILED|record" | head -12
 done

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on the GPU box)")
     # The CPU oracle runs on oneDNN: on boxes whose CPU quota is far below the visible core count (GPU box:
     # 128 visible, 16 usable) the default thread count makes it ~25x slower.
     import torch

@@ -1,6 +1,6 @@
 """Generate the committed golden fixtures by running the REAL reference.
 
-Run in the build container only (needs /root/reference, which does not exist on the
+Run in the build container only (needs a checkout of the reference, MIGAN_REF, which does not exist on the
 GPU box):   python tests/golden/make_golden.py
 
 For each case it
@@ -23,7 +23,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("MIGAN_REF", "/root/reference")
+REF = os.environ.get("MIGAN_REF", "../MI-GAN")   # a checkout of the reference project
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 

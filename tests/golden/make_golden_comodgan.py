@@ -1,6 +1,6 @@
 """Pin the Co-Mod-GAN oracle against the REAL reference and write the committed fixtures.
 
-Run in the build container only (needs /root/reference):   python tests/golden/make_golden_comodgan.py
+Needs a checkout of the reference (MIGAN_REF):   python tests/golden/make_golden_comodgan.py
 
 For each case it builds ``lib.model_zoo.comodgan.Generator(Mapping, Encoder, Synthesis)`` the way
 ``scripts/demo.py:95-100`` does, loads the oracle's seeded state_dict with ``strict=True`` (key names, order and shapes
@@ -18,7 +18,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("MIGAN_REF", "/root/reference")
+REF = os.environ.get("MIGAN_REF", "../MI-GAN")   # a checkout of the reference project
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 warnings.filterwarnings("ignore")

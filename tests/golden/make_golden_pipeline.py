@@ -1,5 +1,5 @@
 """Pin oracle/pipeline_oracle.py against the reference's own ``MIGAN_Pipeline`` (scripts/create_onnx_pipeline.py:121-264) and
-write tests/golden/pipeline.npz.  Build container only (needs /root/reference and torchvision); the class does not use its
+write tests/golden/pipeline.npz.  Needs a checkout of the reference (MIGAN_REF) and torchvision; the class does not use its
 module's cv2 / onnxruntime imports, which are stubbed.
 
 Every case records the inputs' SEED (the tests regenerate image / mask with ``case_inputs`` below), the crop window, the
@@ -17,7 +17,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("MIGAN_REF", "/root/reference")
+REF = os.environ.get("MIGAN_REF", "../MI-GAN")   # a checkout of the reference project
 sys.path.insert(0, ROOT)
 
 # (tag, res, padding, H, W, mask H, mask W, hole rows, hole cols, extra)
@@ -43,6 +43,22 @@ def case_inputs(case):
         mask[:, :, MH // 2, : MW // 3] = 128
         mask[:, :, 3, 5] = 254
     return torch.from_numpy(image), torch.from_numpy(mask)
+
+
+def load_fixture():
+    """pipeline.npz + pipeline_r256.npz (the r256 request, stored apart by shrink_golden.py) as one dict."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    gold = {}
+    for name in ("pipeline.npz", "pipeline_r256.npz"):
+        z = np.load(os.path.join(here, name))
+        gold.update({k: z[k] for k in z.files})
+    return gold
+
+
+def on_stored_rows(gold, key, tag, a):
+    """`a` (a full x or final image of request `tag`) restricted to the rows the fixture stores for it."""
+    rows = gold.get(("rows_" if key == "x" else "frows_") + tag)
+    return a if rows is None else a[:, :, rows]
 
 
 def main():

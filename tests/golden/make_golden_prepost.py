@@ -8,7 +8,7 @@ from PIL import Image
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("MIGAN_REF", "/root/reference")
+REF = os.environ.get("MIGAN_REF", "../MI-GAN")   # a checkout of the reference project
 sys.path.insert(0, ROOT)
 sys.path.insert(0, REF)
 

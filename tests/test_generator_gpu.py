@@ -1,7 +1,7 @@
-"""Parity of the CUDA generator (through the C ABI) against the CPU oracle -- needs a B200.
+"""Parity of the CUDA generator (through the C ABI) against the CPU oracle -- needs an H100.
 
 Tolerance (north_star): max-abs error < 1e-3 vs the fp32 reference on identical inputs, for the
-fp32-faithful paths ("simt": fp32 FMA, "tc": tcgen05 fp16 hi/lo 3-pass).  Outputs have
+fp32-faithful paths ("simt": fp32 FMA, "tc": wgmma fp16 hi/lo 3-pass).  Outputs have
 magnitude ~5-25, and the fp32-vs-fp64 noise floor of the reference itself is ~1e-5.
 """
 import glob
@@ -83,6 +83,8 @@ def test_golden_fixture(cuda_device, path, fixture):
     g, sd = make_model(R, path, seed=int(z["wseed"]))
     x = O.make_input(R, N, seed=int(z["xseed"]))
     got = g(x.to(cuda_device))
+    if "y_rows" in z.files:                              # large outputs are stored on a row sample (shrink_golden.py)
+        got = got[:, :, torch.from_numpy(z["y_rows"]).to(cuda_device)]
     mx, mean = errs(got, torch.from_numpy(z["y"]))
     print("golden %s path=%s max-abs=%.3e mean-abs=%.3e" % (os.path.basename(fixture), path, mx, mean))
     assert mx < TOL_MAX_ABS and mean < TOL_MEAN_ABS

@@ -30,6 +30,8 @@ def test_forward_matches_reference_golden(path):
     taps = {}
     y = O.generator_forward(sd, x, R, taps=taps)
     want = torch.from_numpy(z["y"])
+    if "y_rows" in z.files:                              # large outputs are stored on a row sample (shrink_golden.py)
+        y = y[:, :, z["y_rows"]]
     # same torch build => bit exact; allow fp32 reassociation noise across CPUs (different oneDNN kernels)
     assert float((y - want).abs().max()) <= 2e-4
     for name, (cs, mx) in zip(z["tap_names"], z["tap_stats"]):
@@ -140,11 +142,20 @@ def _c2r_cases(g):
             up=a[0], down=a[1], groups=a[2], flip_weight=bool(a[3]), padding=a[4:8], flip_filter=bool(a[8]) if len(a) > 8 else False)
 
 
+def _c2r_stored_rows(g, name, y):
+    """y (computed, full) on the rows the fixture stores: large outputs are kept as a row sample (shrink_golden.py)."""
+    if name + ".yrows" not in g.files:
+        assert tuple(y.shape) == g[name + ".y"].shape, name
+        return y
+    assert tuple(y.shape) == tuple(int(v) for v in g[name + ".yshape"]), name
+    return y[:, :, g[name + ".yrows"]]
+
+
 def test_conv2d_resample_oracle_reproduces_reference_vectors():
     from oracle import comodgan_oracle as C
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "conv2d_resample.npz"))
     cases = list(_c2r_cases(g))
     assert len(cases) == 15
     for name, x, w, f, kw in cases:
-        y = C.conv2d_resample_ref(x, w, f=f, **kw)
+        y = _c2r_stored_rows(g, name, C.conv2d_resample_ref(x, w, f=f, **kw))
         assert float((y - torch.from_numpy(g[name + ".y"])).abs().max()) <= 1e-4, name

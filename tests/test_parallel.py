@@ -34,7 +34,7 @@ def _worker(rank, world, port, out_dir):
     torch.set_num_threads(2)
     R = 32
     sd = O.make_state_dict(R, seed=1)
-    model = lambda x: O.generator_forward(sd, x, R)          # noqa: E731  (stand-in for the B200 Generator)
+    model = lambda x: O.generator_forward(sd, x, R)          # noqa: E731  (stand-in for the H100 Generator)
     sg = parallel.ShardedGenerator(model)
     sg.check_replicas(sd)
     x_global = O.make_input(R, 6, seed=3)

@@ -1,7 +1,7 @@
 """CPU checks of the arbitrary-resolution crop pipeline (SURVEY.md 8(f) row f4, scripts/create_onnx_pipeline.py:121-264):
 
 * the oracle (oracle/pipeline_oracle.py) against the vectors the reference's own MIGAN_Pipeline produced
-  (tests/golden/pipeline.npz, written by tests/golden/make_golden_pipeline.py where /root/reference exists);
+  (tests/golden/pipeline.npz, written by tests/golden/make_golden_pipeline.py where a checkout of the reference exists);
 * the kernel functors of mi-gan_b200/csrc/pipeline.cu, compiled for the host by the emulation build (test infrastructure),
   against the same vectors -- bit for bit: crop window, model input x, final image given the reference generator's y;
 * the host crop arithmetic of the PRODUCT library (`migan_crop_box`, no GPU involved) on the 300 pinned random masks.
@@ -24,7 +24,7 @@ from migan_b200 import _abi, ops  # noqa: E402
 import build_emul  # noqa: E402
 import make_golden_pipeline as MG  # noqa: E402  (case table + seeded inputs; its main() needs the reference and is not run here)
 
-GOLD = np.load(os.path.join(ROOT, "tests", "golden", "pipeline.npz"))
+GOLD = MG.load_fixture()
 PIPE_SYMBOLS = [s for s in _abi.SYMBOLS if s[0] in ("b200_pipeline_scratch_bytes", "b200_resize_nearest_u8", "b200_hole_flags",
                                                     "migan_crop_box", "b200_pipeline_preprocess", "b200_pipeline_postprocess")]
 
@@ -67,8 +67,8 @@ def test_oracle_matches_reference_pipeline(case):
     taps = {}
     final = PO.forward(lambda x: y_ref, image.clone(), mask, res, pad, taps)      # the generator's output is the reference's
     assert taps["box"] == tuple(int(v) for v in GOLD["box_" + tag])
-    assert torch.equal(taps["x"], torch.from_numpy(GOLD["x_" + tag]))
-    assert np.array_equal(final.numpy(), GOLD["final_" + tag])
+    assert torch.equal(MG.on_stored_rows(GOLD, "x", tag, taps["x"]), torch.from_numpy(GOLD["x_" + tag]))
+    assert np.array_equal(MG.on_stored_rows(GOLD, "final", tag, final.numpy()), GOLD["final_" + tag])
 
 
 def test_aa_weights_against_torch():
@@ -113,6 +113,7 @@ def test_kernels_match_reference_pipeline(emul, case):
     image, mask = MG.case_inputs(case)
     box, x, final = _run_emul_pipeline(emul, image.numpy().copy(), mask.numpy(), res, pad, GOLD["y_" + tag])
     assert box == tuple(int(v) for v in GOLD["box_" + tag])
+    x, final = MG.on_stored_rows(GOLD, "x", tag, x), MG.on_stored_rows(GOLD, "final", tag, final)
     assert np.array_equal(x, GOLD["x_" + tag]), "model input differs on %d values" % int((x != GOLD["x_" + tag]).sum())
     want = GOLD["final_" + tag]
     assert np.array_equal(final, want), "final image differs on %d bytes (max %d)" % (

@@ -1,6 +1,6 @@
-"""Opt-in code paths (off by default) -- validated on a B200 in round 2 (profiles/r02_comodgan_tc_route.log).
+"""Opt-in code paths (off by default).
 
-  COMOD_GEMM=tc   Co-Mod-GAN plain / strided / 1x1 convolutions on the tcgen05 GEMM of the MI-GAN path (sepconv_tc.cu in its
+  COMOD_GEMM=tc   Co-Mod-GAN plain / strided / 1x1 convolutions on the wgmma GEMM of the MI-GAN path (sepconv_tc.cu in its
                   A_TMA configuration, K up to 4608) fed by an fp16 hi/lo split im2col.  Operand packing is covered on the
                   CPU by tests/test_comodgan_emul.py::test_staged_tcgen05_route_operands.
 """
@@ -30,5 +30,5 @@ def test_comodgan_tcgen05_route(cuda_device, name, monkeypatch):
     x, z = O.make_input(R, N, seed=int(gold["xseed"])), C.make_latent(N, seed=int(gold["xseed"]) + 1)
     y = g(x.to(cuda_device), z=z.to(cuda_device), noise_mode="const").cpu()
     err = (y - torch.from_numpy(gold["y"])).abs()
-    print("%s [tcgen05 route]: max-abs %.3e mean-abs %.3e" % (name, float(err.max()), float(err.mean())))
+    print("%s [wgmma route]: max-abs %.3e mean-abs %.3e" % (name, float(err.max()), float(err.mean())))
     assert float(err.max()) < 1e-3

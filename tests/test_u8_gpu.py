@@ -1,4 +1,4 @@
-"""uint8 request path (SURVEY.md 8(f) rank 1) on the B200: the pre/post-processing kernels are bit-exact against the
+"""uint8 request path (SURVEY.md 8(f) rank 1) on the H100: the pre/post-processing kernels are bit-exact against the
 oracle restatement of scripts/demo.py:56-66 / :135-142; the fused host call equals kernel-by-kernel composition."""
 import os
 

@@ -1,6 +1,6 @@
 """Small-batch latency of Generator.forward on cuda:0: p50 / p90 of (launch + wait) per call, CUDA-graph replay vs the plain
 launch sequence, device-resident input; plus the host-buffer call at batch 1.
-    python tools/latency.py --res 512 --out gpurun_out/latency.json
+    python tools/latency.py --res 512 --out tools/out/latency.json
 Measurement tooling (scripts/demo.py:125-142 is the batch-1 caller this path serves)."""
 import argparse
 import json
@@ -70,6 +70,7 @@ def main():
     rows.append({"n": 1, "mode": "forward_host", "p50_ms": statistics.median(lat), "p90_ms": pct(lat, 0.9)})
     print(rows[-1], flush=True)
     if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         json.dump({"res": a.res, "rows": rows}, open(a.out, "w"), indent=1)
 
 

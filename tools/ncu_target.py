@@ -1,5 +1,5 @@
 """Minimal process for ncu captures: `forwards` generator forwards at (res, n) on cuda:0, nothing else.
-    ncu --set full -k regex:sepconv_tc -s 32 -c 3 -o gpurun_out/x python tools/ncu_target.py --res 512 --n 32
+    ncu --set full -k regex:sepconv_tc -s 32 -c 3 -o tools/out/sepconv_tc python tools/ncu_target.py --res 512 --n 32
 Profiling tooling (no oracle import: weights are seeded random, outputs are not checked here)."""
 import argparse
 import os

@@ -46,8 +46,8 @@ def main():
                      "crop_window_stage_p50_ms": statistics.median(box_ms)})
         print(rows[-1], flush=True)
     out = {"resolution": res, "padding": 128, "requests": rows}
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(out, open("gpurun_out/r02_pipeline_latency_%d.json" % res, "w"), indent=1)
+    os.makedirs("tools/out", exist_ok=True)
+    json.dump(out, open("tools/out/pipeline_latency_%d.json" % res, "w"), indent=1)
 
 
 if __name__ == "__main__":
