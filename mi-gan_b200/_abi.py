@@ -107,6 +107,14 @@ def library_path() -> str:
     return os.environ.get("MIGAN_B200_LIB", _build.LIBPATH)
 
 
+def path_id(name) -> int:
+    """Id of the kernel path `name`; None selects $MIGAN_B200_PATH, or "tc" when that is unset."""
+    name = name or os.environ.get("MIGAN_B200_PATH", "tc")
+    if name not in PATHS:
+        raise ValueError("unknown path %r (expected one of %s)" % (name, sorted(PATHS)))
+    return PATHS[name]
+
+
 def load(build_if_missing: bool = False):
     """dlopen the shared library and bind every declared symbol."""
     global _lib

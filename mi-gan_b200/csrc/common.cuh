@@ -7,7 +7,6 @@
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 namespace migan {
 
@@ -54,11 +53,7 @@ __device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __ha
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// Host: kernel launch with the PDL attribute (MIGAN_PDL=0 turns the attribute off for A/B measurements).
-inline bool pdl_enabled() {
-    static const bool on = [] { const char* e = getenv("MIGAN_PDL"); return !e || atoi(e) != 0; }();
-    return on;
-}
+// Host: kernel launch with the PDL attribute.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
     cudaLaunchConfig_t cfg = {};
@@ -66,7 +61,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 

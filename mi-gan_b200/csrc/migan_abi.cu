@@ -136,6 +136,29 @@ struct Plan {
     std::vector<Step> steps;
 };
 
+// Two staging slots taken in turn by consecutive host-memory calls of one kind (fp32 or uint8): the copies of call c+1
+// (copy-in stream) and c-1 (copy-out stream) run under the kernels of call c on the caller's stream.
+struct SlotRing {
+    struct Slot {
+        const void* base = nullptr;   // staging memory the slot last used
+        bool used = false;
+        // in: copy-in done, for the uint8 call (the fp32 call records one per micro-batch in host_events)
+        cudaEvent_t start = nullptr, in = nullptr, compute_done = nullptr, out_done = nullptr;
+    };
+    Slot slot[2];
+    unsigned calls = 0;
+    int cur = 0;   // slot of the call in progress
+
+    int next() { return cur = (int)(calls++ & 1); }
+    int begin(migan_ctx* ctx, const void* slot_base, cudaStream_t st);
+    int end(migan_ctx* ctx, cudaStream_t st);
+    void destroy() {
+        for (Slot& s : slot)
+            for (cudaEvent_t e : {s.start, s.in, s.compute_done, s.out_done})
+                if (e) cudaEventDestroy(e);
+    }
+};
+
 }  // namespace
 
 struct migan_ctx {
@@ -165,18 +188,11 @@ struct migan_ctx {
     float* tap_dst = nullptr;
     bool profiling = false;
     std::vector<cudaEvent_t> events;  // 2 per step of the current plan
-    // host-buffer pipeline (migan_forward_host): copy streams + events, created on first use
+    // host-memory calls (migan_forward_host / _u8): copy streams created on first use, one slot ring per call kind
+    // (a shared ring would see new staging memory, and re-order after the caller's stream, on every switch of kind)
     cudaStream_t s_in = nullptr, s_out = nullptr;
-    std::vector<cudaEvent_t> host_events;
-    cudaEvent_t slot_compute_done[2] = {nullptr, nullptr}, slot_out_done[2] = {nullptr, nullptr};
-    bool slot_used[2] = {false, false};
-    const void* slot_base[2] = {nullptr, nullptr};   // staging memory each slot last used (re-ordered after the caller's stream when it changes)
-    unsigned host_calls = 0;
-    // uint8 request pipeline (migan_forward_u8 / _async): its own two staging slots and events
-    cudaEvent_t u8_in[2] = {nullptr, nullptr}, u8_compute_done[2] = {nullptr, nullptr}, u8_out_done[2] = {nullptr, nullptr}, u8_start = nullptr;
-    bool u8_used[2] = {false, false};
-    const void* u8_base[2] = {nullptr, nullptr};
-    unsigned u8_calls = 0;
+    SlotRing host_ring, u8_ring;
+    std::vector<cudaEvent_t> host_events;   // fp32 host call: [copy-in done, compute done] per micro-batch, per slot
     // captured forward (migan_forward_graph): valid for one (n, path, workspace)
     cudaGraphExec_t graph_exec = nullptr;
     cudaStream_t s_cap = nullptr;
@@ -187,6 +203,49 @@ struct migan_ctx {
 };
 
 namespace {
+
+int create_copy_streams(migan_ctx* ctx) {
+    if (!ctx->s_in) {
+        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
+        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
+    }
+    return MIGAN_OK;
+}
+
+// Takes the current slot, whose staging memory starts at slot_base, for a call on stream st.
+// In steady state the copy-in stream does NOT wait for the caller's stream: the host input is valid from the call on, and
+// the only device hazard -- the slot still being read by the forward that used it two calls ago -- is covered by
+// compute_done.  Waiting on st here would serialise the copy-in of call c+1 behind the kernels of call c, which is exactly
+// the overlap the two slots exist for.
+// The FIRST use of staging memory is different: it may have just been handed over by a stream-ordered allocator (torch's
+// caching allocator assumes same-stream reuse), so work still pending on the caller's stream may be using it.  Both copy
+// streams are ordered after the caller's stream once, whenever a slot sees new memory.
+int SlotRing::begin(migan_ctx* ctx, const void* slot_base, cudaStream_t st) {
+    if (int rc = create_copy_streams(ctx)) return rc;
+    Slot& s = slot[cur];
+    for (cudaEvent_t* e : {&s.start, &s.in, &s.compute_done, &s.out_done})
+        if (!*e) CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    if (!s.used || s.base != slot_base) {
+        CUDA_TRY(cudaEventRecord(s.start, st));
+        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, s.start, 0));
+        CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, s.start, 0));
+        s.base = slot_base;
+    }
+    if (s.used) {
+        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, s.compute_done, 0));   // the slot's inputs are free again
+        CUDA_TRY(cudaStreamWaitEvent(st, s.out_done, 0));              // its outputs have been copied out
+    }
+    return MIGAN_OK;
+}
+
+// Marks the end of the call's kernels on st and of its copy-out, which must all be enqueued.
+int SlotRing::end(migan_ctx* ctx, cudaStream_t st) {
+    Slot& s = slot[cur];
+    CUDA_TRY(cudaEventRecord(s.compute_done, st));
+    CUDA_TRY(cudaEventRecord(s.out_done, ctx->s_out));
+    s.used = true;
+    return MIGAN_OK;
+}
 
 void add_spec(migan_ctx* c, const std::string& name, std::initializer_list<int64_t> shape) {
     WeightSpec s;
@@ -327,16 +386,8 @@ int migan_destroy(migan_ctx* ctx) {
     if (!ctx) return MIGAN_OK;
     for (cudaEvent_t e : ctx->events) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->host_events) cudaEventDestroy(e);
-    for (int i = 0; i < 2; ++i) {
-        if (ctx->slot_compute_done[i]) cudaEventDestroy(ctx->slot_compute_done[i]);
-        if (ctx->slot_out_done[i]) cudaEventDestroy(ctx->slot_out_done[i]);
-    }
-    for (int i = 0; i < 2; ++i) {
-        if (ctx->u8_in[i]) cudaEventDestroy(ctx->u8_in[i]);
-        if (ctx->u8_compute_done[i]) cudaEventDestroy(ctx->u8_compute_done[i]);
-        if (ctx->u8_out_done[i]) cudaEventDestroy(ctx->u8_out_done[i]);
-    }
-    if (ctx->u8_start) cudaEventDestroy(ctx->u8_start);
+    ctx->host_ring.destroy();
+    ctx->u8_ring.destroy();
     if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
     if (ctx->s_cap) cudaStreamDestroy(ctx->s_cap);
     if (ctx->s_in) cudaStreamDestroy(ctx->s_in);
@@ -567,15 +618,35 @@ size_t migan_workspace_bytes(const migan_ctx* ctx, int n) {
     return total;
 }
 
-size_t migan_host_staging_bytes(const migan_ctx* ctx, int n) {
-    if (!ctx || n <= 0) return 0;
-    const size_t px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
-    return 2 * (align_up(4 * px, 1024) + align_up(3 * px, 1024));   // two slots: consecutive calls overlap
-}
-
 }  // extern "C"
 
 namespace {
+
+// One staging slot: x fp32 [n,4,R,R] and y fp32 [n,3,R,R], then for uint8 requests img [n,R,R,3], out [n,R,R,3] and
+// mask [n,R,R].  Every part starts on a 1024-byte boundary.
+struct StagingSlot {
+    float* x;
+    float* y;
+    uint8_t* img;
+    uint8_t* out;
+    uint8_t* mask;
+    size_t bytes;
+};
+
+// Slot `slot` of the staging area that starts at `area`; without an area only `bytes` is meaningful.
+StagingSlot staging_slot(const migan_ctx* c, int n, bool u8, unsigned char* area = nullptr, int slot = 0) {
+    const size_t px = (size_t)n * c->resolution * c->resolution;
+    const size_t sizes[5] = {4 * px * sizeof(float), 3 * px * sizeof(float), u8 ? 3 * px : 0, u8 ? 3 * px : 0, u8 ? px : 0};
+    size_t off[5], bytes = 0;
+    for (int i = 0; i < 5; ++i) {
+        off[i] = bytes;
+        bytes += align_up(sizes[i], 1024);
+    }
+    unsigned char* part[5] = {};
+    if (area)
+        for (int i = 0; i < 5; ++i) part[i] = area + slot * bytes + off[i];
+    return {reinterpret_cast<float*>(part[0]), reinterpret_cast<float*>(part[1]), part[2], part[3], part[4], bytes};
+}
 
 // What the tensor-core kernel's prologue rebuilds on chip instead of reading it from HBM (sepconv_tc.h SepconvSource).
 struct Fuse {
@@ -603,18 +674,6 @@ struct PlanBuilder {
         s.tap = name; s.tap_src = src; s.tapC = C; s.tapH = H; s.tapW = W; s.tap_planar = planar; s.tap_flags = flags;
     }
 
-    static bool down_tma_enabled() {    // MIGAN_DOWN_TMA=0: register-streaming kernel (A/B measurements)
-        const char* e = getenv("MIGAN_DOWN_TMA");
-        return !e || atoi(e) != 0;
-    }
-    static int fuse_mask_dw() {         // MIGAN_FUSE bit 2: run the depthwise stage of the small Cout = 512 levels (res <= 32) inside the
-        return fuse_mask() & 4;         // tensor-core kernel (its prologue repeats per N tile, which is cheap there) instead of as its own launch
-    }
-    static int fuse_mask() {            // MIGAN_FUSE bit 0: UP, bit 1: STEM, bit 2: small-level depthwise (debug / A-B measurements; default all on)
-        const char* e = getenv("MIGAN_FUSE");
-        return e ? atoi(e) : 7;
-    }
-
     // Emit one SeparableConv2d reading `in` (NHWC [n,res_in,res_in,cin]); `skip` is added after the
     // final activation (decoder conv1, migan_inference.py:304-305).  Returns the output pointer.
     // in_idx: scratch index holding `in` (or -1 if it is a feat buffer); out_fixed: write there if non-null.
@@ -632,7 +691,7 @@ struct PlanBuilder {
                 s.hi = reinterpret_cast<__half*>(S[t1]);
                 s.lo = s.hi + (size_t)n * L.res_pw * L.res_pw * L.cin;
                 ghi = s.hi; glo = s.lo;
-                if (L.res_pw >= 16 && down_tma_enabled()) {   // rows staged through shared memory by TMA (elementwise.cu)
+                if (L.res_pw >= 16) {   // rows staged through shared memory by TMA (elementwise.cu)
                     if (const char* err = migan::make_down_tensor_map(&s.down_map, in, n, L.res_in, L.res_in, L.cin))
                         return fail(MIGAN_ERR_CUDA, "tensor map for %sdownsample failed: %s", L.p.c_str(), err);
                     s.down_tma = true;
@@ -647,9 +706,10 @@ struct PlanBuilder {
             set_tap(s, L.p + "dw_act", S[t1], L.cin, L.res_in, L.res_in);
             steps.push_back(s);
             gemm_in = S[t1];
-        } else if (L.cout >= 512 && !rgb && (L.res_in >= 64 || fuse_mask_dw() == 0)) {
+        } else if (L.cout >= 512 && !rgb && L.res_in >= 64) {
             // Cout spans 8 N tiles: a fused prologue would re-run the depthwise stage per tile, so run it once as its
-            // own kernel and hand the GEMM a pre-split operand (these layers are small: res <= 64)
+            // own kernel and hand the GEMM a pre-split operand.  Below 64 x 64 the repeated prologue is cheap and
+            // saves a launch, so those levels keep the depthwise stage in the tensor-core kernel.
             Step s; s.kind = K_DW; s.L = &L; s.in = in; s.n = n; s.H = L.res_in; s.W = L.res_in; s.C = L.cin;
             s.hi = reinterpret_cast<__half*>(S[t1]);
             s.lo = s.hi + (size_t)n * L.res_in * L.res_in * L.cin;
@@ -727,11 +787,10 @@ struct PlanBuilder {
         for (int i = 0; i < 2; ++i) { IMG[i] = reinterpret_cast<float*>(base + off); off += img_bytes(c, n); }
         const int R = c->resolution;
         const bool tcp = (path != MIGAN_PATH_SIMT);
-        const int fm = fuse_mask();
         // ---- encoder (migan_inference.py:235-246) ----
         // The stem (fromrgb + activation, :193-196) is recomputed inside encoder.b{R}.conv1's prologue when that layer runs
         // on the fused tensor-core kernel with 8 x 16 tiles; otherwise it is its own kernel.
-        const bool fuse_stem = tcp && (fm & 2) && R >= 16 && channels(R) < 512;
+        const bool fuse_stem = tcp && R >= 16 && channels(R) < 512;
         if (!fuse_stem) {
             Step s; s.kind = K_STEM; s.io_flags = PTR_X; s.out = S[0]; s.n = n; s.H = R; s.W = R; s.C = channels(R);
             set_tap(s, "encoder.b" + std::to_string(R) + ".fromrgb", S[0], channels(R), R, R);
@@ -764,7 +823,7 @@ struct PlanBuilder {
             // conv1's FIR + noise + activation + skip can be rebuilt in conv2's prologue (the up-sampled tensor then never
             // exists in HBM) when conv2 runs its depthwise stage in the tensor-core kernel with 8 x 16 tiles.
             const SepConv& L1 = c->syn1[i];
-            const bool fuse_up = tcp && (fm & 1) && L1.up && L1.up_uniform && r >= 16 && (channels(r) < 512 || fuse_rgb);
+            const bool fuse_up = tcp && L1.up && L1.up_uniform && r >= 16 && (channels(r) < 512 || fuse_rgb);
             Fuse f1; f1.defer_up = fuse_up;
             int rc = emit_sepconv(L1, cur, cur_idx, nullptr, feat[r], oi, op, nullptr, std::string(), 0, f1);  // x = conv1(x) + enc_feat
             if (rc) return rc;
@@ -945,8 +1004,7 @@ int migan_forward(migan_ctx* ctx, const float* x, float* y, int n, void* workspa
 
 size_t migan_graph_staging_bytes(const migan_ctx* ctx, int n) {
     if (!ctx || n <= 0) return 0;
-    const size_t px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
-    return align_up(4 * px, 1024) + align_up(3 * px, 1024);
+    return staging_slot(ctx, n, false).bytes;
 }
 
 int migan_forward_graph(migan_ctx* ctx, const float* x, float* y, int n, void* workspace, size_t workspace_bytes,
@@ -958,8 +1016,9 @@ int migan_forward_graph(migan_ctx* ctx, const float* x, float* y, int n, void* w
         return fail(MIGAN_ERR_WORKSPACE, "workspace too small for the graph staging buffers: %zu < %zu bytes", workspace_bytes,
                     ws + migan_graph_staging_bytes(ctx, n));
     const size_t px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
-    float* xg = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + ws);
-    float* yg = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + ws + align_up(4 * px, 1024));
+    const StagingSlot stage = staging_slot(ctx, n, false, static_cast<unsigned char*>(workspace) + ws);
+    float* xg = stage.x;
+    float* yg = stage.y;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaSetDevice(ctx->device));
     if (!ctx->graph_exec || ctx->graph_n != n || ctx->graph_path != path || ctx->graph_ws != workspace || ctx->profiling || ctx->tap_dst) {
@@ -1017,6 +1076,11 @@ int migan_profile_step(migan_ctx* ctx, int index, const char** label, float* ms,
     return MIGAN_OK;
 }
 
+size_t migan_host_staging_bytes(const migan_ctx* ctx, int n) {
+    if (!ctx || n <= 0) return 0;
+    return 2 * staging_slot(ctx, n, false).bytes;   // two slots: consecutive calls overlap
+}
+
 // Enqueue H2D -> forward -> D2H for one host batch without waiting for it.  Two staging slots alternate, so the
 // copies of call c+1 overlap the kernels / copy-out of call c (a serving loop submits batches back to back and
 // collects them with migan_host_wait).  Within a call the batch is split into micro-batches for the same reason.
@@ -1028,12 +1092,9 @@ static int forward_host_enqueue(migan_ctx* ctx, const float* x_host, float* y_ho
     if (workspace_bytes < ws + migan_host_staging_bytes(ctx, n))
         return fail(MIGAN_ERR_WORKSPACE, "workspace too small for host staging: %zu < %zu bytes", workspace_bytes,
                     ws + migan_host_staging_bytes(ctx, n));
-    const size_t px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
-    const size_t slot_bytes = align_up(4 * px, 1024) + align_up(3 * px, 1024);
-    const int slot = (int)(ctx->host_calls++ & 1);
-    unsigned char* sbase = static_cast<unsigned char*>(workspace) + ws + slot * slot_bytes;
-    float* xd = reinterpret_cast<float*>(sbase);
-    float* yd = reinterpret_cast<float*>(sbase + align_up(4 * px, 1024));
+    SlotRing& ring = ctx->host_ring;
+    const int slot = ring.next();
+    const StagingSlot stage = staging_slot(ctx, n, false, static_cast<unsigned char*>(workspace) + ws, slot);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaSetDevice(ctx->device));
     // Micro-batch pipeline: H2D of micro-batch k+1 and D2H of k-1 overlap the kernels of k (three streams).
@@ -1042,63 +1103,32 @@ static int forward_host_enqueue(migan_ctx* ctx, const float* x_host, float* y_ho
     // (two micro-batches: more would pay the fixed per-forward cost of the small layers more often).  Enqueue-only call: consecutive
     // batches already overlap through the two staging slots (H2D of batch t+1 and D2H of batch t-1 run under the kernels of
     // batch t), so the batch stays whole and does not pay the fixed per-forward cost of the small layers twice.
-    int M = (slot_out != nullptr && n >= 8 && n % 2 == 0) ? 2 : 1;
-    if (const char* e = getenv("MIGAN_HOST_PIPELINE")) {
-        const int v = atoi(e);
-        if (v >= 1 && n % v == 0) M = v;
-    }
-    if (!ctx->s_in) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
-        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i) {
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->slot_compute_done[i], cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->slot_out_done[i], cudaEventDisableTiming));
-        }
-    }
-    while ((int)ctx->host_events.size() < 2 * (2 * M + 1)) {
+    const int M = (slot_out != nullptr && n >= 8 && n % 2 == 0) ? 2 : 1;
+    while ((int)ctx->host_events.size() < 2 * 2 * M) {
         cudaEvent_t e;
         CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         ctx->host_events.push_back(e);
     }
-    cudaEvent_t* ev = ctx->host_events.data() + slot * (2 * M + 1);   // per-slot events: [in_k, c_k] x M, start
-    cudaEvent_t ev_start = ev[2 * M];
+    cudaEvent_t* ev = ctx->host_events.data() + slot * 2 * M;   // per-slot events: [in_k, c_k] x M
+    if (int rc = ring.begin(ctx, stage.x, st)) return rc;
     const int m = n / M;
     const size_t xs = (size_t)m * 4 * ctx->resolution * ctx->resolution, ys = (size_t)m * 3 * ctx->resolution * ctx->resolution;
-    // In steady state the copy-in stream does NOT wait for the caller's stream: x_host is host memory (valid from the call
-    // on) and the only device hazard -- the staging slot still being read by the forward that used it two calls ago -- is
-    // covered by slot_compute_done below.  Waiting on `stream` here would serialise the H2D of batch t+1 behind the kernels
-    // of batch t, which is exactly the overlap the two slots exist for.
-    // The FIRST use of a staging area is different: the memory may have just been handed over by a stream-ordered
-    // allocator (torch's caching allocator assumes same-stream reuse), so work still pending on the caller's stream may be
-    // using it.  Order both copy streams after the caller's stream once, whenever a slot sees new memory.
-    if (!ctx->slot_used[slot] || ctx->slot_base[slot] != sbase) {
-        CUDA_TRY(cudaEventRecord(ev_start, st));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, ev_start, 0));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ev_start, 0));
-        ctx->slot_base[slot] = sbase;
-    }
-    if (ctx->slot_used[slot]) {
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, ctx->slot_compute_done[slot], 0));   // xd[slot] free again
-        CUDA_TRY(cudaStreamWaitEvent(st, ctx->slot_out_done[slot], 0));              // yd[slot] copied out
-    }
     for (int k = 0; k < M; ++k) {
-        CUDA_TRY(cudaMemcpyAsync(xd + k * xs, x_host + k * xs, xs * sizeof(float), cudaMemcpyHostToDevice, ctx->s_in));
+        CUDA_TRY(cudaMemcpyAsync(stage.x + k * xs, x_host + k * xs, xs * sizeof(float), cudaMemcpyHostToDevice, ctx->s_in));
         CUDA_TRY(cudaEventRecord(ev[2 * k], ctx->s_in));
     }
     int launches = 0;
     for (int k = 0; k < M; ++k) {
         CUDA_TRY(cudaStreamWaitEvent(st, ev[2 * k], 0));
-        int rc = migan_forward(ctx, xd + k * xs, yd + k * ys, m, workspace, ws, path, stream);
+        int rc = migan_forward(ctx, stage.x + k * xs, stage.y + k * ys, m, workspace, ws, path, stream);
         if (rc) return rc;
         launches += ctx->last_launches;
         CUDA_TRY(cudaEventRecord(ev[2 * k + 1], st));
         CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ev[2 * k + 1], 0));
-        CUDA_TRY(cudaMemcpyAsync(y_host + k * ys, yd + k * ys, ys * sizeof(float), cudaMemcpyDeviceToHost, ctx->s_out));
+        CUDA_TRY(cudaMemcpyAsync(y_host + k * ys, stage.y + k * ys, ys * sizeof(float), cudaMemcpyDeviceToHost, ctx->s_out));
     }
     ctx->last_launches = launches;
-    CUDA_TRY(cudaEventRecord(ctx->slot_compute_done[slot], st));
-    CUDA_TRY(cudaEventRecord(ctx->slot_out_done[slot], ctx->s_out));
-    ctx->slot_used[slot] = true;
+    if (int rc = ring.end(ctx, st)) return rc;
     if (slot_out) *slot_out = slot;
     return MIGAN_OK;
 }
@@ -1108,7 +1138,7 @@ int migan_forward_host(migan_ctx* ctx, const float* x_host, float* y_host, int n
     int slot = 0;
     int rc = forward_host_enqueue(ctx, x_host, y_host, n, workspace, workspace_bytes, path, stream, &slot);
     if (rc) return rc;
-    CUDA_TRY(cudaEventSynchronize(ctx->slot_out_done[slot]));   // y_host is complete on return
+    CUDA_TRY(cudaEventSynchronize(ctx->host_ring.slot[slot].out_done));   // y_host is complete on return
     return MIGAN_OK;
 }
 
@@ -1117,14 +1147,9 @@ int migan_forward_host_async(migan_ctx* ctx, const float* x_host, float* y_host,
     return forward_host_enqueue(ctx, x_host, y_host, n, workspace, workspace_bytes, path, stream, nullptr);
 }
 
-static size_t u8_slot_bytes(const migan_ctx* ctx, int n) {
-    const size_t px = (size_t)n * ctx->resolution * ctx->resolution;
-    return align_up(4 * px * sizeof(float), 1024) + align_up(3 * px * sizeof(float), 1024) + 2 * align_up(3 * px, 1024) + align_up(px, 1024);
-}
-
 size_t migan_u8_staging_bytes(const migan_ctx* ctx, int n) {
     if (!ctx || n <= 0) return 0;
-    return 2 * u8_slot_bytes(ctx, n);     // two slots: consecutive calls overlap
+    return 2 * staging_slot(ctx, n, true).bytes;     // two slots: consecutive calls overlap
 }
 
 // Enqueue H2D(img, mask) -> preprocess -> forward -> postprocess -> D2H(out) for one uint8 request batch.  Same three-stream,
@@ -1139,55 +1164,25 @@ static int forward_u8_enqueue(migan_ctx* ctx, const uint8_t* img_host, const uin
                     ws + migan_u8_staging_bytes(ctx, n));
     const int R = ctx->resolution;
     const size_t px = (size_t)n * R * R;
-    const int slot = (int)(ctx->u8_calls++ & 1);
-    unsigned char* sbase = static_cast<unsigned char*>(workspace) + ws + slot * u8_slot_bytes(ctx, n);
-    unsigned char* b = sbase;
-    float* xd = reinterpret_cast<float*>(b);               b += align_up(4 * px * sizeof(float), 1024);
-    float* yd = reinterpret_cast<float*>(b);               b += align_up(3 * px * sizeof(float), 1024);
-    uint8_t* img_d = b;                                     b += align_up(3 * px, 1024);
-    uint8_t* out_d = b;                                     b += align_up(3 * px, 1024);
-    uint8_t* mask_d = b;
+    SlotRing& ring = ctx->u8_ring;
+    const int slot = ring.next();
+    const StagingSlot stage = staging_slot(ctx, n, true, static_cast<unsigned char*>(workspace) + ws, slot);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaSetDevice(ctx->device));
-    if (!ctx->s_in) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
-        CUDA_TRY(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i) {
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->slot_compute_done[i], cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->slot_out_done[i], cudaEventDisableTiming));
-        }
-    }
-    if (!ctx->u8_start) {
-        CUDA_TRY(cudaEventCreateWithFlags(&ctx->u8_start, cudaEventDisableTiming));
-        for (int i = 0; i < 2; ++i) {
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->u8_in[i], cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->u8_compute_done[i], cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreateWithFlags(&ctx->u8_out_done[i], cudaEventDisableTiming));
-        }
-    }
-    if (!ctx->u8_used[slot] || ctx->u8_base[slot] != sbase) {   // new staging memory: order the copy streams after the caller's stream once
-        CUDA_TRY(cudaEventRecord(ctx->u8_start, st));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, ctx->u8_start, 0));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ctx->u8_start, 0));
-        ctx->u8_base[slot] = sbase;
-    }
-    if (ctx->u8_used[slot]) {
-        CUDA_TRY(cudaStreamWaitEvent(ctx->s_in, ctx->u8_compute_done[slot], 0));   // img_d / mask_d of this slot are free again
-        CUDA_TRY(cudaStreamWaitEvent(st, ctx->u8_out_done[slot], 0));              // out_d of this slot has been copied out
-    }
-    CUDA_TRY(cudaMemcpyAsync(img_d, img_host, 3 * px, cudaMemcpyHostToDevice, ctx->s_in));
-    CUDA_TRY(cudaMemcpyAsync(mask_d, mask_host, px, cudaMemcpyHostToDevice, ctx->s_in));
-    CUDA_TRY(cudaEventRecord(ctx->u8_in[slot], ctx->s_in));
-    CUDA_TRY(cudaStreamWaitEvent(st, ctx->u8_in[slot], 0));
-    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img_d, mask_d, xd, n, R, st));
-    if (int rc = migan_forward(ctx, xd, yd, n, workspace, ws, path, stream)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(yd, img_d, mask_d, out_d, n, R, st));
+    if (int rc = ring.begin(ctx, stage.x, st)) return rc;
+    const SlotRing::Slot& ev = ring.slot[slot];
+    CUDA_TRY(cudaMemcpyAsync(stage.img, img_host, 3 * px, cudaMemcpyHostToDevice, ctx->s_in));
+    CUDA_TRY(cudaMemcpyAsync(stage.mask, mask_host, px, cudaMemcpyHostToDevice, ctx->s_in));
+    CUDA_TRY(cudaEventRecord(ev.in, ctx->s_in));
+    CUDA_TRY(cudaStreamWaitEvent(st, ev.in, 0));
+    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(stage.img, stage.mask, stage.x, n, R, st));
+    if (int rc = migan_forward(ctx, stage.x, stage.y, n, workspace, ws, path, stream)) return rc;
+    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(stage.y, stage.img, stage.mask, stage.out, n, R, st));
     ctx->last_launches += 2;
-    CUDA_TRY(cudaEventRecord(ctx->u8_compute_done[slot], st));
-    CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ctx->u8_compute_done[slot], 0));
-    CUDA_TRY(cudaMemcpyAsync(out_host, out_d, 3 * px, cudaMemcpyDeviceToHost, ctx->s_out));
-    CUDA_TRY(cudaEventRecord(ctx->u8_out_done[slot], ctx->s_out));
-    ctx->u8_used[slot] = true;
+    CUDA_TRY(cudaEventRecord(ev.compute_done, st));   // recorded again by ring.end() at the same point of st
+    CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ev.compute_done, 0));
+    CUDA_TRY(cudaMemcpyAsync(out_host, stage.out, 3 * px, cudaMemcpyDeviceToHost, ctx->s_out));
+    if (int rc = ring.end(ctx, st)) return rc;
     if (slot_out) *slot_out = slot;
     return MIGAN_OK;
 }
@@ -1196,7 +1191,7 @@ int migan_forward_u8(migan_ctx* ctx, const uint8_t* img_host, const uint8_t* mas
                      void* workspace, size_t workspace_bytes, int path, void* stream) {
     int slot = 0;
     if (int rc = forward_u8_enqueue(ctx, img_host, mask_host, out_host, n, workspace, workspace_bytes, path, stream, &slot)) return rc;
-    CUDA_TRY(cudaEventSynchronize(ctx->u8_out_done[slot]));   // out_host is complete on return
+    CUDA_TRY(cudaEventSynchronize(ctx->u8_ring.slot[slot].out_done));   // out_host is complete on return
     return MIGAN_OK;
 }
 

@@ -697,10 +697,8 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     cudaDeviceGetAttribute(&sms0, cudaDevAttrMultiProcessorCount, dev0);
     // Few pixel tiles (the 4 x 4 ... 16 x 16 levels at small batches): most SMs would idle while a few CTAs stream the
     // weight matrix.  Narrow N tiles spread the layer over 2 x the CTAs.
-    if (!d.rgb && p.n_tile > 64 && cout >= 256 && p.tiles_x * p.tiles_y * p.tiles_n * (cout / p.n_tile) * 2 < sms0 &&
-        env_int("MIGAN_TC_SMALL_N", 1) != 0) {
+    if (!d.rgb && p.n_tile > 64 && cout >= 256 && p.tiles_x * p.tiles_y * p.tiles_n * (cout / p.n_tile) * 2 < sms0)
         p.n_tile = 64;
-    }
     p.num_n_tiles = cout / p.n_tile;
     p.num_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.num_n_tiles;
     auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
@@ -748,9 +746,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     {
         const int b_res = p.b_resident ? p.num_kb : 0;
         // input ring depths to try, deepest first (even: each prologue group owns every other stage)
-        const int max_in = env_int("MIGAN_TC_MAX_IN", 6);
-        std::vector<int> ins;
-        if (dw) { for (int v = 6; v >= 2; v -= 2) if (v <= max_in) ins.push_back(v); } else ins.push_back(0);
+        const std::vector<int> ins = dw ? std::vector<int>{6, 4, 2} : std::vector<int>{0};
         const int bopts[2] = {b_res ? b_res : 3, b_res ? b_res : 2};
         for (int bi = 0; bi < 2; ++bi) {
             if (bi == 1 && bopts[1] == bopts[0]) break;
@@ -779,7 +775,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     p.error_flag = (dev >= 0 && dev < kMaxDevices) ? g_error_flag[dev] : nullptr;
-    p.prefetch = env_int("MIGAN_TC_PREFETCH", dw ? 4 : 2);
+    p.prefetch = dw ? 4 : 2;
 
     // ---- tensor maps ----
     const char* err = nullptr;

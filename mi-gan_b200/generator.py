@@ -15,7 +15,6 @@ from __future__ import annotations
 
 import ctypes
 import math
-import os
 from typing import Dict, Optional
 
 import torch
@@ -91,22 +90,22 @@ class _Engine:
         _abi.check(self.lib.migan_finalize_weights(self.handle))
         self.weights_version = version
 
-    def workspace(self, n: int, host_staging=False):
-        """host_staging: False (device forward), True (host-buffer call: two staging slots) or "graph" (captured forward:
-        one staging slot)."""
-        key = (n, host_staging)
+    _STAGING_BYTES = {"graph": "migan_graph_staging_bytes", "host": "migan_host_staging_bytes", "u8": "migan_u8_staging_bytes"}
+
+    def workspace(self, n: int, kind: Optional[str] = None):
+        """kind: None (device forward), "graph" (captured forward: one staging slot), "host" (fp32 host-buffer call) or
+        "u8" (uint8 request call); the host-memory calls get two staging slots."""
+        key = (n, kind)
         ws = self.workspaces.get(key)
         if ws is None:
             nbytes = self.lib.migan_workspace_bytes(self.handle, n)
-            if host_staging == "graph":
-                nbytes += self.lib.migan_graph_staging_bytes(self.handle, n)
-            elif host_staging:
-                nbytes += self.lib.migan_host_staging_bytes(self.handle, n)
+            if kind is not None:
+                nbytes += getattr(self.lib, self._STAGING_BYTES[kind])(self.handle, n)
             raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
             off = (-raw.data_ptr()) % 1024
             ws = raw[off:off + nbytes]
             if any(k[0] != n for k in self.workspaces):
-                # copies enqueued by forward_host(wait=False) may still be using a staging area that is about to be released
+                # copies enqueued with wait=False may still be using a staging area that is about to be released
                 _abi.check(self.lib.migan_host_wait(self.handle))
             self.workspaces = {k: v for k, v in self.workspaces.items() if k[0] == n}  # keep one batch size
             self.workspaces[key] = ws
@@ -122,7 +121,7 @@ class Generator(nn.Module):
         self.resolution = resolution
         self.path = path  # None -> $MIGAN_B200_PATH -> "tc"
         # batches up to this size go through the CUDA-graph replay of the forward (0 disables it)
-        self.graph_max_batch = int(os.environ.get("MIGAN_GRAPH_MAX_N", "4"))
+        self.graph_max_batch = 4
         for key, shape, kind in arch.state_entries(resolution):
             *mods, leaf = key.split(".")
             node = self
@@ -152,12 +151,6 @@ class Generator(nn.Module):
         return state
 
     # -- plumbing ---------------------------------------------------------------------
-    def _path_id(self) -> int:
-        name = self.path or os.environ.get("MIGAN_B200_PATH", "tc")
-        if name not in _abi.PATHS:
-            raise ValueError("unknown path %r (expected one of %s)" % (name, sorted(_abi.PATHS)))
-        return _abi.PATHS[name]
-
     def _state_version(self):
         # Cheap per-call check that the uploaded weights are still current: the tensor list is collected once (and again
         # after load_state_dict / .to() / .cuda(), which may replace tensors) and each call only sums version counters.
@@ -218,11 +211,11 @@ class Generator(nn.Module):
                 # small batches (the demo runs batch 1) are launch-bound: replay the captured launch sequence
                 ws = eng.workspace(n, "graph")
                 _abi.check(eng.lib.migan_forward_graph(eng.handle, x.data_ptr(), y.data_ptr(), n, ws.data_ptr(), ws.numel(),
-                                                       self._path_id(), stream))
+                                                       _abi.path_id(self.path), stream))
             else:
                 ws = eng.workspace(n)
                 _abi.check(eng.lib.migan_forward(eng.handle, x.data_ptr(), y.data_ptr(), n, ws.data_ptr(), ws.numel(),
-                                                 self._path_id(), stream))
+                                                 _abi.path_id(self.path), stream))
         return y
 
     @torch.no_grad()
@@ -246,10 +239,10 @@ class Generator(nn.Module):
             raise RuntimeError("out must be a contiguous CPU float32 tensor of shape [N, 3, %d, %d]" % (r, r))
         with torch.cuda.device(device):
             eng = self._engine(device)
-            ws = eng.workspace(n, host_staging=True)
+            ws = eng.workspace(n, "host")
             stream = torch.cuda.current_stream(device).cuda_stream
             fn = eng.lib.migan_forward_host if wait else eng.lib.migan_forward_host_async
-            _abi.check(fn(eng.handle, x_host.data_ptr(), out.data_ptr(), n, ws.data_ptr(), ws.numel(), self._path_id(), stream))
+            _abi.check(fn(eng.handle, x_host.data_ptr(), out.data_ptr(), n, ws.data_ptr(), ws.numel(), _abi.path_id(self.path), stream))
         return out
 
     @torch.no_grad()
@@ -278,20 +271,11 @@ class Generator(nn.Module):
             raise RuntimeError("out must be a contiguous CPU uint8 tensor of shape [N, %d, %d, 3]" % (r, r))
         with torch.cuda.device(device):
             eng = self._engine(device)
-            nbytes = eng.lib.migan_workspace_bytes(eng.handle, n) + eng.lib.migan_u8_staging_bytes(eng.handle, n)
-            ws = eng.workspaces.get((n, "u8"))
-            if ws is None:
-                raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=device)
-                off = (-raw.data_ptr()) % 1024
-                ws = raw[off:off + nbytes]
-                if any(k[0] != n for k in eng.workspaces):
-                    _abi.check(eng.lib.migan_host_wait(eng.handle))
-                eng.workspaces = {k: v for k, v in eng.workspaces.items() if k[0] == n}
-                eng.workspaces[(n, "u8")] = ws
+            ws = eng.workspace(n, "u8")
             stream = torch.cuda.current_stream(device).cuda_stream
             fn = eng.lib.migan_forward_u8 if wait else eng.lib.migan_forward_u8_async
             _abi.check(fn(eng.handle, img_u8.data_ptr(), mask_u8.data_ptr(), out.data_ptr(), n,
-                          ws.data_ptr(), ws.numel(), self._path_id(), stream))
+                          ws.data_ptr(), ws.numel(), _abi.path_id(self.path), stream))
         return out
 
     def host_wait(self) -> None:
@@ -331,7 +315,7 @@ class Generator(nn.Module):
         out, i = [], 0
         name = ctypes.c_char_p()
         shape = (ctypes.c_int * 3)()
-        while eng.lib.migan_tap_info(eng.handle, self._path_id(), i, ctypes.byref(name), shape) == 0:
+        while eng.lib.migan_tap_info(eng.handle, _abi.path_id(self.path), i, ctypes.byref(name), shape) == 0:
             out.append((name.value.decode(), (shape[0], shape[1], shape[2])))
             i += 1
         return out

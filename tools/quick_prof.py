@@ -1,5 +1,6 @@
 """Quick A/B of kernel variants: per-kernel and per-layer CUDA-event times of the generator forward (no oracle, no e2e).
-    MIGAN_TC_MAX_IN=4 python tools/quick_prof.py --res 512 --n 32 --tag in4
+    python tools/quick_prof.py --res 512 --n 32 --tag base
+To compare two variants, run it on each revision with its own --tag.
 Prints one summary line + the launches above --min-ms.  Profiling tooling."""
 import argparse
 import json
