@@ -141,6 +141,30 @@ int b200_pipeline_preprocess(const uint8_t* image_chw, const uint8_t* mask_hw, i
 int b200_pipeline_postprocess(const float* y_nchw, uint8_t* image_chw, const uint8_t* mask_hw, int H, int W, const int* box4_host,
                               int resolution, const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The same stages for a batch of 1..MIGAN_PIPE_MAX_BATCH requests of any sizes, one launch per stage for the whole batch
+ * (the request table is passed to the kernels by value).  reqs_host is a HOST array of n requests; every request must be
+ * at least 3 x 3, and images must not overlap each other or any mask.  Request i's results equal the single-request
+ * stages' bit for bit:
+ *   b200_hole_flags_batch            request i's flags start at sum_{j<i} (W_j + H_j), laid out as b200_hole_flags;
+ *                                    the boxes are not read
+ *   b200_pipeline_batch_scratch_bytes  exact scratch size for these boxes (0 on a bad argument)
+ *   b200_pipeline_preprocess_batch   request i -> x[i] of a contiguous x [n,4,res,res]
+ *   b200_pipeline_postprocess_batch  y[i] of a contiguous y [n,3,res,res] -> request i's image[crop], in place
+ * Fills the boxes with migan_crop_box (one call per request, on the host flags) between the flags and the pre-processing. */
+#define MIGAN_PIPE_MAX_BATCH 32
+typedef struct {
+    uint8_t* image;        /* DEVICE u8 [3][H][W]; the post-processing writes image[crop] in place */
+    const uint8_t* mask;   /* DEVICE u8 [H][W], 255 = known (already at the image size) */
+    int H, W;
+    int box[4];            /* x_min, x_max, y_min, y_max from migan_crop_box; not read by b200_hole_flags_batch */
+} migan_pipe_request;
+int b200_hole_flags_batch(const migan_pipe_request* reqs_host, int n, uint8_t* flags, void* stream);
+size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* reqs_host, int n, int resolution);
+int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs_host, int n, int resolution, float* x_n4rr,
+                                   void* scratch, size_t scratch_bytes, void* stream);
+int b200_pipeline_postprocess_batch(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
+                                    const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
+
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0
  * (k = 1).  w_dev: HOST array of k DEVICE pointers to [cout][fan] fp32 tensors (fan = cin/groups * kh * kw); out: device.

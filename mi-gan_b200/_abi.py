@@ -11,6 +11,13 @@ from . import build as _build
 OK, ERR_INVALID, ERR_CUDA, ERR_STATE, ERR_WORKSPACE = 0, 1, 2, 3, 4
 PATH_SIMT, PATH_TC, PATH_TC_FAST = 0, 1, 2
 PATHS = {"simt": PATH_SIMT, "tc": PATH_TC, "tc_fast": PATH_TC_FAST}
+PIPE_MAX_BATCH = 32
+
+
+class PipeRequest(ctypes.Structure):
+    """migan_pipe_request: one request of the batched crop-pipeline entry points."""
+    _fields_ = [("image", c_void_p), ("mask", c_void_p), ("H", c_int), ("W", c_int), ("box", c_int * 4)]
+
 
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
@@ -42,6 +49,10 @@ SYMBOLS = [
     ("migan_crop_box", c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     ("b200_pipeline_preprocess", c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_postprocess", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_hole_flags_batch", c_int, [POINTER(PipeRequest), c_int, c_void_p, c_void_p]),
+    ("b200_pipeline_batch_scratch_bytes", c_size_t, [POINTER(PipeRequest), c_int, c_int]),
+    ("b200_pipeline_preprocess_batch", c_int, [POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_postprocess_batch", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

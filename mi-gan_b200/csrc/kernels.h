@@ -6,6 +6,8 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include "../../include/migan_b200.h"
+
 namespace migan {
 
 // Per-device one-time setup (dynamic shared memory opt-in); called by migan_create.
@@ -81,6 +83,13 @@ int launch_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H,
                                void* scratch, cudaStream_t s);
 int launch_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
                                 const float* k25_host, void* scratch, cudaStream_t s);
+// batches of 1..MIGAN_PIPE_MAX_BATCH requests of any sizes, one launch per stage
+size_t pipeline_batch_scratch_bytes(const migan_pipe_request* reqs, int n, int res);
+int check_pipe_batch(const migan_pipe_request* reqs, int n, int res, bool boxes, char* msg, size_t len);
+int launch_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flags, cudaStream_t s);
+int launch_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
+int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
+                                      void* scratch, cudaStream_t s);
 
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------

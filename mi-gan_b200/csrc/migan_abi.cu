@@ -1335,6 +1335,44 @@ int b200_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mas
     return MIGAN_OK;
 }
 
+static int check_pipe_batch(const char* who, const migan_pipe_request* reqs, int n, int res, bool boxes) {
+    char msg[256];
+    if (int rc = migan::check_pipe_batch(reqs, n, res, boxes, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+int b200_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flags, void* stream) {
+    if (int rc = check_pipe_batch("hole_flags_batch", reqs, n, 1, false)) return rc;
+    if (!flags) return fail(MIGAN_ERR_INVALID, "hole_flags_batch: null flags");
+    CUDA_TRY((cudaError_t)migan::launch_hole_flags_batch(reqs, n, flags, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* reqs, int n, int res) {
+    if (check_pipe_batch("pipeline_batch_scratch_bytes", reqs, n, res, true)) return 0;
+    return migan::pipeline_batch_scratch_bytes(reqs, n, res);
+}
+
+int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
+                                   void* stream) {
+    if (int rc = check_pipe_batch("pipeline_preprocess_batch", reqs, n, res, true)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_pipeline_preprocess_batch(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
+                                    size_t scratch_bytes, void* stream) {
+    if (int rc = check_pipe_batch("pipeline_postprocess_batch", reqs, n, res, true)) return rc;
+    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess_batch(y, reqs, n, res, k25, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
 int migan_host_wait(migan_ctx* ctx) {
     if (!ctx) return fail(MIGAN_ERR_INVALID, "null ctx");
     if (!ctx->s_out) return MIGAN_OK;

@@ -13,11 +13,18 @@
 // right with fused multiply-adds in fp32; the weight table is evaluated exactly like the C++ (float scale / support /
 // centre, the filter argument through double, w / total).  A pass whose size does not change is the identity there;
 // here it runs with the table {xmin = i, 1 tap, w = 1}, which is the same value bit for bit.
-// Item kernels (comod_kernels.cuh style): the emulation build runs the very same functors on the CPU against the oracle.
+//
+// Every stage serves a batch of up to MIGAN_PIPE_MAX_BATCH requests of different sizes in one launch.  The requests'
+// descriptors travel by value in the kernel parameter (PipeBatch, < 4 KB) together with the launch's item prefix
+// start[]: item i belongs to the request k with start[k] <= i < start[k + 1].  The single-request entry points are the
+// batch of one.  Item kernels (comod_kernels.cuh style): the emulation build runs the very same functors on the CPU
+// against the oracle; the hole flags use a shared-memory kernel on the GPU and the per-request HoleFlagsK there.
 #include "comod_kernels.cuh"
+#include "../../include/migan_b200.h"
 
 #ifdef MIGAN_EMULATE
 #include <cmath>
+#include <cstdio>
 #define PL_MUL(a, b) ((a) * (b))
 #define PL_ADD(a, b) ((a) + (b))
 #define PL_DIV(a, b) ((a) / (b))
@@ -25,6 +32,7 @@
 #define PL_RINT(a) rintf(a)
 #define PL_D inline
 #else
+#include <cstdio>
 #include "kernels.h"
 #define PL_MUL(a, b) __fmul_rn((a), (b))
 #define PL_ADD(a, b) __fadd_rn((a), (b))
@@ -52,6 +60,7 @@ struct NearestU8K {    // items = oh*ow: one uint8 plane [H][W] -> [oh][ow]
     }
 };
 
+#ifdef MIGAN_EMULATE   // the GPU build runs hole_flags_batch_kernel (shared memory, warp votes) instead
 struct HoleFlagsK {    // items = W + H: flags[x] = column x contains a value < 255, flags[W + y] likewise for row y  (:144-149)
     const uint8_t* mask; uint8_t* flags; int H, W;
     PL_D void operator()(int64_t i) const {
@@ -61,106 +70,160 @@ struct HoleFlagsK {    // items = W + H: flags[x] = column x contains a value < 
         flags[i] = f;
     }
 };
+#endif
 
 // One axis of the anti-aliased bilinear filter: for output index i the first source index, the tap count and the taps.
 struct AaTable { int* xmin; int* xsize; float* w; int maxk; };
 
-struct AaWeightsK {    // items = out_size
-    AaTable t; int in_size, out_size;
+CK_HD size_t pl_align256(size_t b) { return (b + 255) & ~(size_t)255; }
+// The table of `out_size` outputs carved at `base`: xmin[out] | xsize[out], the taps [out][maxk] at the next 256 bytes.
+CK_HD AaTable aa_table(int* base, int out_size, int maxk) {
+    AaTable t;
+    t.maxk = maxk;
+    t.xmin = base;
+    t.xsize = base + out_size;
+    t.w = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(base) + pl_align256((size_t)out_size * 2 * sizeof(int)));
+    return t;
+}
+
+PL_D void aa_weights(const AaTable& t, int in_size, int out_size, int64_t i) {    // entry i of the table in_size -> out_size
+    float* w = t.w + i * t.maxk;
+    if (in_size == out_size) {                          // the reference skips this pass: identity table
+        t.xmin[i] = (int)i; t.xsize[i] = 1; w[0] = 1.f;
+        for (int j = 1; j < t.maxk; ++j) w[j] = 0.f;
+        return;
+    }
+    const float scale = PL_DIV((float)in_size, (float)out_size);           // area_pixel_compute_scale<float>
+    const bool down = scale >= 1.0f;
+    const float support = down ? scale : 1.f;                              // (interp_size * 0.5) * scale, interp_size = 2
+    const float invscale = down ? (float)(1.0 / (double)scale) : 1.f;
+    const float center = (float)((double)scale * ((double)i + 0.5));
+    int lo = (int)((double)PL_ADD(center, -support) + 0.5);
+    if (lo < 0) lo = 0;
+    int hi = (int)((double)PL_ADD(center, support) + 0.5);
+    if (hi > in_size) hi = in_size;
+    int n = hi - lo;
+    n = n < 0 ? 0 : (n > t.maxk ? t.maxk : n);
+    float total = 0.f;
+    for (int j = 0; j < n; ++j) {
+        float a = (float)(((double)PL_ADD((float)(j + lo), -center) + 0.5) * (double)invscale);
+        a = fabsf(a);
+        const float v = a < 1.0f ? PL_ADD(1.f, -a) : 0.f;                  // aa_filter (triangle)
+        w[j] = v;
+        total = PL_ADD(total, v);
+    }
+    if (total != 0.f)
+        for (int j = 0; j < n; ++j) w[j] = PL_DIV(w[j], total);
+    for (int j = n; j < t.maxk; ++j) w[j] = 0.f;
+    t.xmin[i] = lo; t.xsize[i] = n;
+}
+
+// One request of a batched launch.  image / mask point at the crop origin (row stride W, plane stride H*W); tw / th are
+// the width / height tables (aa_table layout) and tmp the width pass's output, all in the caller's scratch.
+struct PipeReq {
+    uint8_t* image; const uint8_t* mask; float* tmp; int* tw; int* th;
+    int H, W, hc, wc, kw, kh;
+};
+struct PipeBatch {
+    int64_t start[MIGAN_PIPE_MAX_BATCH + 1];   // item prefix of the launch
+    PipeReq r[MIGAN_PIPE_MAX_BATCH];
+    const float* y; float* x;                  // generator output [n][3][res][res] / model input [n][4][res][res]
+    float k[25];                               // feather smoothing taps
+    int n, res;
+    PL_D int find(int64_t i) const {           // the request item i belongs to
+        int lo = 0, hi = n - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (start[mid] <= i) lo = mid; else hi = mid - 1;
+        }
+        return lo;
+    }
+};
+static_assert(sizeof(PipeBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
+
+// Both axis tables of every request.  POST = 0: crop -> res (pre-processing); 1: res -> crop (post-processing).
+// items per request = out_w + out_h
+template <int POST>
+struct AaWeightsBatchK {
+    PipeBatch b;
     PL_D void operator()(int64_t i) const {
-        float* w = t.w + i * t.maxk;
-        if (in_size == out_size) {                          // the reference skips this pass: identity table
-            t.xmin[i] = (int)i; t.xsize[i] = 1; w[0] = 1.f;
-            for (int j = 1; j < t.maxk; ++j) w[j] = 0.f;
-            return;
-        }
-        const float scale = PL_DIV((float)in_size, (float)out_size);           // area_pixel_compute_scale<float>
-        const bool down = scale >= 1.0f;
-        const float support = down ? scale : 1.f;                              // (interp_size * 0.5) * scale, interp_size = 2
-        const float invscale = down ? (float)(1.0 / (double)scale) : 1.f;
-        const float center = (float)((double)scale * ((double)i + 0.5));
-        int lo = (int)((double)PL_ADD(center, -support) + 0.5);
-        if (lo < 0) lo = 0;
-        int hi = (int)((double)PL_ADD(center, support) + 0.5);
-        if (hi > in_size) hi = in_size;
-        int n = hi - lo;
-        n = n < 0 ? 0 : (n > t.maxk ? t.maxk : n);
-        float total = 0.f;
-        for (int j = 0; j < n; ++j) {
-            float a = (float)(((double)PL_ADD((float)(j + lo), -center) + 0.5) * (double)invscale);
-            a = fabsf(a);
-            const float v = a < 1.0f ? PL_ADD(1.f, -a) : 0.f;                  // aa_filter (triangle)
-            w[j] = v;
-            total = PL_ADD(total, v);
-        }
-        if (total != 0.f)
-            for (int j = 0; j < n; ++j) w[j] = PL_DIV(w[j], total);
-        for (int j = n; j < t.maxk; ++j) w[j] = 0.f;
-        t.xmin[i] = lo; t.xsize[i] = n;
+        const int k = b.find(i);
+        const PipeReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int ow = POST ? r.wc : b.res, oh = POST ? r.hc : b.res;
+        if (j < ow) aa_weights(aa_table(r.tw, ow, r.kw), POST ? b.res : r.wc, ow, j);
+        else aa_weights(aa_table(r.th, oh, r.kh), POST ? b.res : r.hc, oh, j - ow);
     }
 };
 
-// Width pass.  SRC = 0: uint8 planes of the image crop; SRC = 1: generator output y mapped to [0, 255] on load (:239).
+// Width pass.  SRC = 0: uint8 planes of the image crop -> tmp [3][hc][res]; SRC = 1: generator output y mapped to [0, 255]
+// on load (:239) -> tmp [3][res][wc].  items per request = 3 * rows * ow
 template <int SRC>
-struct ResizeWidthK {  // items = C * rows * ow -> tmp [C][rows][ow]
-    const void* src; int64_t plane_stride; int row_stride; AaTable t; float* out; int rows, ow;
-    PL_D float load(int64_t o) const {
+struct ResizeWidthBatchK {
+    PipeBatch b;
+    PL_D float load(const void* src, int64_t o) const {
         if (SRC == 0) return (float)static_cast<const uint8_t*>(src)[o];
         float g = PL_MUL(PL_ADD(PL_MUL(static_cast<const float*>(src)[o], 0.5f), 0.5f), 255.f);   // ((y * 0.5 + 0.5) * 255)
         return fminf(fmaxf(g, 0.f), 255.f);                                                       // .clamp(0, 255)
     }
     PL_D void operator()(int64_t i) const {
-        const int x = (int)(i % ow); int64_t r = i / ow;
-        const int y = (int)(r % rows); const int c = (int)(r / rows);
+        const int k = b.find(i);
+        const PipeReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int ow = SRC ? r.wc : b.res, rows = SRC ? b.res : r.hc;
+        const int64_t plane_stride = SRC ? (int64_t)b.res * b.res : (int64_t)r.H * r.W;
+        const int row_stride = SRC ? b.res : r.W;
+        const void* src = SRC ? static_cast<const void*>(b.y + (int64_t)k * 3 * b.res * b.res) : static_cast<const void*>(r.image);
+        const AaTable t = aa_table(r.tw, ow, r.kw);
+        const int x = (int)(j % ow); const int64_t q = j / ow;
+        const int y = (int)(q % rows); const int c = (int)(q / rows);
         const int64_t base = c * plane_stride + (int64_t)y * row_stride + t.xmin[x];
         const float* w = t.w + (int64_t)x * t.maxk;
-        float acc = PL_MUL(load(base), w[0]);
-        for (int j = 1; j < t.xsize[x]; ++j) acc = PL_FMA(load(base + j), w[j], acc);
-        out[i] = acc;
-    }
-};
-
-struct ResizeHeightK { // items = C * oh * ow: tmp [C][ih][ow] -> out [C][oh][ow]
-    const float* in; AaTable t; float* out; int ih, oh, ow;
-    PL_D void operator()(int64_t i) const {
-        const int x = (int)(i % ow); int64_t r = i / ow;
-        const int y = (int)(r % oh); const int c = (int)(r / oh);
-        const float* p = in + ((int64_t)c * ih + t.xmin[y]) * ow + x;
-        const float* w = t.w + (int64_t)y * t.maxk;
-        float acc = PL_MUL(p[0], w[0]);
-        for (int j = 1; j < t.xsize[y]; ++j) acc = PL_FMA(p[(int64_t)j * ow], w[j], acc);
-        out[i] = acc;
+        float acc = PL_MUL(load(src, base), w[0]);
+        for (int jj = 1; jj < t.xsize[x]; ++jj) acc = PL_FMA(load(src, base + jj), w[jj], acc);
+        r.tmp[j] = acc;
     }
 };
 
 // Height pass of the image crop fused with the rest of MIGAN_Pipeline.preprocess (:229-236): round to uint8, nearest
-// mask, normalise, x = cat([mask - 0.5, image * mask]).
-struct PreprocessK {   // items = res * res
-    const float* in; AaTable t; const uint8_t* mask; int mask_row_stride; int hc, wc, res; float* x;
+// mask, normalise, x[k] = cat([mask - 0.5, image * mask]).  items per request = res * res
+struct PreprocessBatchK {
+    PipeBatch b;
     PL_D void operator()(int64_t i) const {
-        const int ox = (int)(i % res), oy = (int)(i / res);
+        const int k = b.find(i);
+        const PipeReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int res = b.res, hc = r.hc;
+        const int ox = (int)(j % res), oy = (int)(j / res);
         const int64_t plane = (int64_t)res * res;
-        const float m = PL_DIV((float)mask[(int64_t)nearest_src(oy, hc, res) * mask_row_stride + nearest_src(ox, wc, res)], 255.f);
-        x[i] = PL_ADD(m, -0.5f);
+        float* x = b.x + (int64_t)k * 4 * plane;
+        const AaTable t = aa_table(r.th, res, r.kh);
+        const float m = PL_DIV((float)r.mask[(int64_t)nearest_src(oy, hc, res) * r.W + nearest_src(ox, r.wc, res)], 255.f);
+        x[j] = PL_ADD(m, -0.5f);
         const float* w = t.w + (int64_t)oy * t.maxk;
         for (int c = 0; c < 3; ++c) {
-            const float* p = in + ((int64_t)c * hc + t.xmin[oy]) * res + ox;
+            const float* p = r.tmp + ((int64_t)c * hc + t.xmin[oy]) * res + ox;
             float acc = PL_MUL(p[0], w[0]);
-            for (int j = 1; j < t.xsize[oy]; ++j) acc = PL_FMA(p[(int64_t)j * res], w[j], acc);
+            for (int jj = 1; jj < t.xsize[oy]; ++jj) acc = PL_FMA(p[(int64_t)jj * res], w[jj], acc);
             const float v = (float)(uint8_t)PL_RINT(acc);                                        // round(), .to(uint8)
             const float n = PL_ADD(PL_DIV(PL_MUL(v, 2.f), 255.f), -1.f);                         // image * 2 / 255 - 1
-            x[(c + 1) * plane + i] = PL_MUL(n, m);
+            x[(c + 1) * plane + j] = PL_MUL(n, m);
         }
     }
 };
 
-// Feathered blend of the resized generator output into the crop, in place (:241-248, :262).  Same arithmetic as FeatherK
-// (prepost.cu) on a window of the full image: max-pool and reflect padding act at the CROP border, like the reference,
-// which slices the crop before post-processing.
-struct FeatherCropK {  // items = hc * wc
-    const float* g; uint8_t* img; const uint8_t* mask; int64_t img_plane; int W; int hc, wc; float k[25];
+// Height pass of the generator output fused with the feathered blend into the crop, in place (:241-248, :262).  The
+// resized value of each channel is the same FMA chain a separate height pass would store.  The blend is FeatherK's
+// arithmetic (prepost.cu) on a window of the full image: max-pool and reflect padding act at the CROP border, like the
+// reference, which slices the crop before post-processing.  items per request = hc * wc
+struct FeatherResizeBatchK {
+    PipeBatch b;
     PL_D void operator()(int64_t i) const {
-        const int h = (int)(i / wc), w = (int)(i - (int64_t)h * wc);
+        const int k = b.find(i);
+        const PipeReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int hc = r.hc, wc = r.wc, W = r.W;
+        const int h = (int)(j / wc), w = (int)(j - (int64_t)h * wc);
         double acc = 0.0;
         for (int dy = -2; dy <= 2; ++dy) {
             int yy = h + dy;
@@ -172,25 +235,125 @@ struct FeatherCropK {  // items = hc * wc
                 for (int a = -1; a <= 1; ++a) {
                     const int y2 = yy + a;
                     if (y2 < 0 || y2 >= hc) continue;
-                    for (int b = -1; b <= 1; ++b) {
-                        const int x2 = xx + b;
+                    for (int c = -1; c <= 1; ++c) {
+                        const int x2 = xx + c;
                         if (x2 < 0 || x2 >= wc) continue;
-                        const int v = mask[(int64_t)y2 * W + x2];
+                        const int v = r.mask[(int64_t)y2 * W + x2];
                         mx = v > mx ? v : mx;
                     }
                 }
-                acc += (double)k[(dy + 2) * 5 + (dx + 2)] * (double)mx;
+                acc += (double)b.k[(dy + 2) * 5 + (dx + 2)] * (double)mx;
             }
         }
         const float wgt = PL_DIV((float)acc, 255.f);
         const float inv = PL_ADD(1.f, -wgt);
+        const AaTable t = aa_table(r.th, hc, r.kh);
+        const float* wt = t.w + (int64_t)h * t.maxk;
+        const int y0 = t.xmin[h], taps = t.xsize[h];
+        const int64_t img_plane = (int64_t)r.H * W;
         for (int c = 0; c < 3; ++c) {
-            uint8_t* px = img + c * img_plane + (int64_t)h * W + w;
-            const float v = PL_ADD(PL_MUL((float)*px, wgt), PL_MUL(g[(int64_t)c * hc * wc + i], inv));
+            const float* p = r.tmp + ((int64_t)c * b.res + y0) * wc + w;                      // tmp [3][res][wc]
+            float g = PL_MUL(p[0], wt[0]);
+            for (int jj = 1; jj < taps; ++jj) g = PL_FMA(p[(int64_t)jj * wc], wt[jj], g);
+            uint8_t* px = r.image + c * img_plane + (int64_t)h * W + w;
+            const float v = PL_ADD(PL_MUL((float)*px, wgt), PL_MUL(g, inv));
             *px = (uint8_t)fminf(fmaxf(v, 0.f), 255.f);
         }
     }
 };
+
+#ifdef MIGAN_EMULATE
+template <class F>
+inline int pipe_launch(const F& f, ck_stream_t s) { return ck_launch(f, f.b.start[f.b.n], s); }
+#else
+// Same one-thread-per-item launch as ck_launch; __grid_constant__ lets the functors index the descriptor table in the
+// parameter space (no per-thread copy of the 2.5 KB struct).
+template <class F>
+__global__ void __launch_bounds__(256) pipe_items_kernel(const __grid_constant__ F f, const int64_t items) {
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i < items) f(i);
+}
+template <class F>
+inline cudaError_t pipe_launch(const F& f, ck_stream_t s) {
+    const int64_t items = f.b.start[f.b.n];
+    if (items <= 0) return cudaSuccess;
+    pipe_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(f, items);
+    return cudaGetLastError();
+}
+
+// ---- batched hole flags -------------------------------------------------------------------------------------------
+// One CTA covers a band of HF_BAND rows x up to HF_TILE columns of one mask.  Each warp takes whole rows: 16-byte loads
+// over the aligned middle of the row, byte loads for the (< 16-byte) head and tail.  The row flag is a warp vote; the
+// column flags are OR-ed over the band into a shared bit mask and only the set bits are stored.  Flags are zeroed before
+// the launch, and racing stores of 1 from other bands / tiles are benign.
+constexpr int HF_THREADS = 256, HF_BAND = 16, HF_TILE = 8192;
+struct FlagsBatch {
+    const uint8_t* mask[MIGAN_PIPE_MAX_BATCH];
+    int64_t foff[MIGAN_PIPE_MAX_BATCH];        // request k's flags start at flags + foff[k]
+    int H[MIGAN_PIPE_MAX_BATCH], W[MIGAN_PIPE_MAX_BATCH], tiles[MIGAN_PIPE_MAX_BATCH];
+    int block_start[MIGAN_PIPE_MAX_BATCH + 1];
+    int n;
+};
+
+__device__ __forceinline__ uint32_t hole_bits4(uint32_t v) {   // bit b set <=> byte b of v is < 255
+    const uint32_t m = __vcmpne4(v, 0xffffffffu) & 0x01010101u;
+    return (m | (m >> 7) | (m >> 14) | (m >> 21)) & 0xfu;
+}
+
+__global__ void __launch_bounds__(HF_THREADS) hole_flags_batch_kernel(const __grid_constant__ FlagsBatch b, uint8_t* flags) {
+    __shared__ uint32_t cols[HF_TILE / 32];
+    int k = 0;
+    {
+        int hi = b.n - 1;
+        while (k < hi) {
+            const int mid = (k + hi + 1) >> 1;
+            if (b.block_start[mid] <= (int)blockIdx.x) k = mid; else hi = mid - 1;
+        }
+    }
+    const int blk = (int)blockIdx.x - b.block_start[k];
+    const int H = b.H[k], W = b.W[k];
+    const int tile = blk % b.tiles[k], band = blk / b.tiles[k];
+    const int c0 = tile * HF_TILE, c1 = min(c0 + HF_TILE, W);
+    const int y0 = band * HF_BAND, y1 = min(y0 + HF_BAND, H);
+    uint8_t* f = flags + b.foff[k];
+    for (int w = threadIdx.x; w < HF_TILE / 32; w += HF_THREADS) cols[w] = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    for (int y = y0 + (threadIdx.x >> 5); y < y1; y += HF_THREADS / 32) {
+        const uint8_t* p0 = b.mask[k] + (int64_t)y * W + c0;
+        const uint8_t* p1 = p0 + (c1 - c0);
+        const uint8_t* a0 = reinterpret_cast<const uint8_t*>((reinterpret_cast<uintptr_t>(p0) + 15) & ~(uintptr_t)15);
+        if (a0 > p1) a0 = p1;
+        const uint8_t* a1 = a0 + ((p1 - a0) & ~(ptrdiff_t)15);
+        bool hole = false;
+        const int nh = (int)(a0 - p0), nt = (int)(p1 - a1);            // both < 16
+        if (lane < nh && p0[lane] != 255) { hole = true; atomicOr(&cols[lane >> 5], 1u << (lane & 31)); }
+        if (lane < nt && a1[lane] != 255) {
+            const int pos = (int)(a1 - p0) + lane;
+            hole = true; atomicOr(&cols[pos >> 5], 1u << (pos & 31));
+        }
+        for (const uint8_t* v = a0 + 16 * lane; v < a1; v += 16 * 32) {
+            const uint4 q = *reinterpret_cast<const uint4*>(v);
+            const uint32_t bits = hole_bits4(q.x) | (hole_bits4(q.y) << 4) | (hole_bits4(q.z) << 8) | (hole_bits4(q.w) << 12);
+            if (bits) {
+                const int pos = (int)(v - p0), sh = pos & 31;
+                hole = true;
+                atomicOr(&cols[pos >> 5], bits << sh);
+                if (sh > 16) atomicOr(&cols[(pos >> 5) + 1], bits >> (32 - sh));
+            }
+        }
+        if (__any_sync(0xffffffffu, hole) && lane == 0) f[W + y] = 1;
+    }
+    __syncthreads();
+    for (int w = threadIdx.x; w < (c1 - c0 + 31) / 32; w += HF_THREADS) {
+        uint32_t m = cols[w];
+        while (m) {
+            f[c0 + w * 32 + __ffs(m) - 1] = 1;
+            m &= m - 1;
+        }
+    }
+}
+#endif
 
 }  // namespace comod
 
@@ -204,31 +367,98 @@ inline int aa_maxk(int in_size, int out_size) {    // max_interp_size of _comput
     const float support = scale >= 1.0f ? scale : 1.f;
     return (int)ceilf(support) * 2 + 1;
 }
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+inline size_t align256(size_t b) { return comod::pl_align256(b); }
 inline size_t table_bytes(int in_size, int out_size) {
     return align256((size_t)out_size * 2 * sizeof(int)) + align256((size_t)out_size * aa_maxk(in_size, out_size) * sizeof(float));
 }
-// carve one axis table out of the scratch area
-inline comod::AaTable take_table(unsigned char*& p, int in_size, int out_size) {
-    comod::AaTable t;
-    t.maxk = aa_maxk(in_size, out_size);
-    t.xmin = reinterpret_cast<int*>(p);
-    t.xsize = t.xmin + out_size;
-    p += align256((size_t)out_size * 2 * sizeof(int));
-    t.w = reinterpret_cast<float*>(p);
-    p += align256((size_t)out_size * t.maxk * sizeof(float));
-    return t;
+// Scratch of one request in either phase: the two axis tables and the width pass's output.
+inline size_t pre_bytes(int hc, int wc, int res) {    // crop -> res: tmp [3][hc][res]
+    return table_bytes(wc, res) + table_bytes(hc, res) + align256((size_t)3 * hc * res * sizeof(float));
+}
+inline size_t post_bytes(int hc, int wc, int res) {   // res -> crop: tmp [3][res][wc]
+    return table_bytes(res, wc) + table_bytes(res, hc) + align256((size_t)3 * res * wc * sizeof(float));
+}
+
+// Descriptors of the whole batch for one phase, carved out of `scratch` request after request.
+comod::PipeBatch plan_batch(const migan_pipe_request* q, int n, int res, bool post, void* scratch) {
+    comod::PipeBatch b = {};
+    b.n = n; b.res = res;
+    unsigned char* p = static_cast<unsigned char*>(scratch);
+    for (int k = 0; k < n; ++k) {
+        const int x0 = q[k].box[0], y0 = q[k].box[2];
+        comod::PipeReq& r = b.r[k];
+        r.H = q[k].H; r.W = q[k].W;
+        r.wc = q[k].box[1] - x0; r.hc = q[k].box[3] - y0;
+        r.image = q[k].image + (int64_t)y0 * r.W + x0;
+        r.mask = q[k].mask + (int64_t)y0 * r.W + x0;
+        const int ow = post ? r.wc : res, oh = post ? r.hc : res;
+        r.kw = post ? aa_maxk(res, r.wc) : aa_maxk(r.wc, res);
+        r.kh = post ? aa_maxk(res, r.hc) : aa_maxk(r.hc, res);
+        r.tw = reinterpret_cast<int*>(p);
+        p += align256((size_t)ow * 2 * sizeof(int)) + align256((size_t)ow * r.kw * sizeof(float));
+        r.th = reinterpret_cast<int*>(p);
+        p += align256((size_t)oh * 2 * sizeof(int)) + align256((size_t)oh * r.kh * sizeof(float));
+        r.tmp = reinterpret_cast<float*>(p);
+        p += align256((size_t)3 * (post ? (size_t)res * r.wc : (size_t)r.hc * res) * sizeof(float));
+    }
+    return b;
+}
+
+// start[] of the next launch: items(request) summed in request order.
+template <class Items>
+void set_items(comod::PipeBatch& b, Items items) {
+    b.start[0] = 0;
+    for (int k = 0; k < b.n; ++k) b.start[k + 1] = b.start[k] + items(b.r[k]);
+}
+
+migan_pipe_request one_request(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box) {
+    migan_pipe_request q;
+    q.image = const_cast<uint8_t*>(image); q.mask = mask; q.H = H; q.W = W;
+    for (int i = 0; i < 4; ++i) q.box[i] = box ? box[i] : 0;
+    return q;
 }
 
 }  // namespace
 
 size_t pipeline_scratch_bytes(int H, int W, int res) {
     // the crop is at most the whole image: pre = tables (H -> res, W -> res) + [3][H][res]; post = tables (res -> H, res -> W)
-    // + [3][res][W] + [3][H][W]; the two phases reuse the same area
+    // + [3][res][W] + [3][H][W]; the two phases reuse the same area.  The batched kernels need at most pre / post of the
+    // actual crop (pipeline_batch_scratch_bytes), so this over-provisions; kept so existing callers size as before.
     const size_t pre = table_bytes(H, res) + table_bytes(W, res) + align256((size_t)3 * H * res * sizeof(float));
     const size_t post = table_bytes(res, H) + table_bytes(res, W) + align256((size_t)3 * res * W * sizeof(float)) +
                         align256((size_t)3 * H * W * sizeof(float));
     return (pre > post ? pre : post) + 1024;
+}
+
+size_t pipeline_batch_scratch_bytes(const migan_pipe_request* q, int n, int res) {
+    size_t pre = 0, post = 0;     // the phases reuse the same area
+    for (int k = 0; k < n; ++k) {
+        const int wc = q[k].box[1] - q[k].box[0], hc = q[k].box[3] - q[k].box[2];
+        pre += pre_bytes(hc, wc, res);
+        post += post_bytes(hc, wc, res);
+    }
+    return pre > post ? pre : post;
+}
+
+int check_pipe_batch(const migan_pipe_request* q, int n, int res, bool boxes, char* msg, size_t len) {
+    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
+    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
+        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
+        return MIGAN_ERR_INVALID;
+    }
+    if (res < 1) { snprintf(msg, len, "bad resolution %d", res); return MIGAN_ERR_INVALID; }
+    for (int k = 0; k < n; ++k) {
+        const migan_pipe_request& r = q[k];
+        if (!r.image || !r.mask) { snprintf(msg, len, "request %d: null image or mask", k); return MIGAN_ERR_INVALID; }
+        if (r.H < 3 || r.W < 3) { snprintf(msg, len, "request %d: image of %d x %d, need at least 3 x 3", k, r.H, r.W); return MIGAN_ERR_INVALID; }
+        const int* b = r.box;
+        if (boxes && (b[0] < 0 || b[1] > r.W || b[2] < 0 || b[3] > r.H || b[1] - b[0] < 3 || b[3] - b[2] < 3)) {
+            snprintf(msg, len, "request %d: crop window x[%d,%d) y[%d,%d) must lie inside the %d x %d image and be at least 3 x 3",
+                     k, b[0], b[1], b[2], b[3], r.H, r.W);
+            return MIGAN_ERR_INVALID;
+        }
+    }
+    return MIGAN_OK;
 }
 
 int launch_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, ck_stream_t s) {
@@ -236,9 +466,34 @@ int launch_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int 
     return (int)comod::ck_launch(k, (int64_t)oh * ow, s);
 }
 
+int launch_hole_flags_batch(const migan_pipe_request* q, int n, uint8_t* flags, ck_stream_t s) {
+#ifdef MIGAN_EMULATE
+    int64_t off = 0;
+    for (int k = 0; k < n; ++k) {
+        comod::ck_launch(comod::HoleFlagsK{q[k].mask, flags + off, q[k].H, q[k].W}, (int64_t)q[k].W + q[k].H, s);
+        off += (int64_t)q[k].W + q[k].H;
+    }
+    return 0;
+#else
+    comod::FlagsBatch b = {};
+    b.n = n;
+    int64_t off = 0;
+    for (int k = 0; k < n; ++k) {
+        b.mask[k] = q[k].mask; b.H[k] = q[k].H; b.W[k] = q[k].W; b.foff[k] = off;
+        b.tiles[k] = (q[k].W + comod::HF_TILE - 1) / comod::HF_TILE;
+        b.block_start[k + 1] = b.block_start[k] + b.tiles[k] * ((q[k].H + comod::HF_BAND - 1) / comod::HF_BAND);
+        off += (int64_t)q[k].W + q[k].H;
+    }
+    cudaError_t e = cudaMemsetAsync(flags, 0, (size_t)off, s);
+    if (e != cudaSuccess) return (int)e;
+    comod::hole_flags_batch_kernel<<<b.block_start[n], comod::HF_THREADS, 0, s>>>(b, flags);
+    return (int)cudaGetLastError();
+#endif
+}
+
 int launch_hole_flags(const uint8_t* mask, int H, int W, uint8_t* flags, ck_stream_t s) {
-    comod::HoleFlagsK k{mask, flags, H, W};
-    return (int)comod::ck_launch(k, (int64_t)W + H, s);
+    const migan_pipe_request q = one_request(nullptr, mask, H, W, nullptr);
+    return launch_hole_flags_batch(&q, 1, flags, s);
 }
 
 // Host arithmetic of get_masked_bbox (:151-227) on the hole flags (flags[x] for columns, flags[W + y] for rows).
@@ -262,49 +517,49 @@ void crop_box_from_flags(const uint8_t* flags, int H, int W, int res, int paddin
     box[0] = x_min; box[1] = x_max; box[2] = y_min; box[3] = y_max;
 }
 
+// Three launches for the whole batch: both tables of every request, the width pass, the height pass fused into x.
+int launch_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res, float* x, void* scratch, ck_stream_t s) {
+    comod::PipeBatch b = plan_batch(q, n, res, false, scratch);
+    b.x = x;
+    int e;
+    set_items(b, [&](const comod::PipeReq&) { return (int64_t)2 * res; });
+    if ((e = (int)comod::pipe_launch(comod::AaWeightsBatchK<0>{b}, s))) return e;
+    set_items(b, [&](const comod::PipeReq& r) { return (int64_t)3 * r.hc * res; });
+    if ((e = (int)comod::pipe_launch(comod::ResizeWidthBatchK<0>{b}, s))) return e;
+    set_items(b, [&](const comod::PipeReq&) { return (int64_t)res * res; });
+    return (int)comod::pipe_launch(comod::PreprocessBatchK{b}, s);
+}
+
+// Three launches for the whole batch: both tables of every request, the width pass, the height pass fused into the blend.
+int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* q, int n, int res, const float* k25_host,
+                                      void* scratch, ck_stream_t s) {
+    comod::PipeBatch b = plan_batch(q, n, res, true, scratch);
+    b.y = y;
+    for (int i = 0; i < 25; ++i) b.k[i] = k25_host[i];
+    int e;
+    set_items(b, [&](const comod::PipeReq& r) { return (int64_t)r.wc + r.hc; });
+    if ((e = (int)comod::pipe_launch(comod::AaWeightsBatchK<1>{b}, s))) return e;
+    set_items(b, [&](const comod::PipeReq& r) { return (int64_t)3 * res * r.wc; });
+    if ((e = (int)comod::pipe_launch(comod::ResizeWidthBatchK<1>{b}, s))) return e;
+    set_items(b, [&](const comod::PipeReq& r) { return (int64_t)r.hc * r.wc; });
+    return (int)comod::pipe_launch(comod::FeatherResizeBatchK{b}, s);
+}
+
 int launch_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
                                void* scratch, ck_stream_t s) {
-    const int x0 = box[0], x1 = box[1], y0 = box[2], y1 = box[3];
-    const int wc = x1 - x0, hc = y1 - y0;
-    unsigned char* p = static_cast<unsigned char*>(scratch);
-    comod::AaTable tw = take_table(p, wc, res), th = take_table(p, hc, res);
-    float* tmp = reinterpret_cast<float*>(p);                                   // [3][hc][res]
-    int e;
-    if ((e = (int)comod::ck_launch(comod::AaWeightsK{tw, wc, res}, res, s))) return e;
-    if ((e = (int)comod::ck_launch(comod::AaWeightsK{th, hc, res}, res, s))) return e;
-    comod::ResizeWidthK<0> kw{image + (int64_t)y0 * W + x0, (int64_t)H * W, W, tw, tmp, hc, res};
-    if ((e = (int)comod::ck_launch(kw, (int64_t)3 * hc * res, s))) return e;
-    comod::PreprocessK kp{tmp, th, mask + (int64_t)y0 * W + x0, W, hc, wc, res, x};
-    return (int)comod::ck_launch(kp, (int64_t)res * res, s);
+    const migan_pipe_request q = one_request(image, mask, H, W, box);
+    return launch_pipeline_preprocess_batch(&q, 1, res, x, scratch, s);
 }
 
 int launch_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
                                 const float* k25_host, void* scratch, ck_stream_t s) {
-    const int x0 = box[0], x1 = box[1], y0 = box[2], y1 = box[3];
-    const int wc = x1 - x0, hc = y1 - y0;
-    unsigned char* p = static_cast<unsigned char*>(scratch);
-    comod::AaTable tw = take_table(p, res, wc), th = take_table(p, res, hc);
-    float* tmp = reinterpret_cast<float*>(p);                                   // [3][res][wc]
-    p += align256((size_t)3 * res * wc * sizeof(float));
-    float* g = reinterpret_cast<float*>(p);                                     // [3][hc][wc]
-    int e;
-    if ((e = (int)comod::ck_launch(comod::AaWeightsK{tw, res, wc}, wc, s))) return e;
-    if ((e = (int)comod::ck_launch(comod::AaWeightsK{th, res, hc}, hc, s))) return e;
-    comod::ResizeWidthK<1> kw{y, (int64_t)res * res, res, tw, tmp, res, wc};
-    if ((e = (int)comod::ck_launch(kw, (int64_t)3 * res * wc, s))) return e;
-    comod::ResizeHeightK kh{tmp, th, g, res, hc, wc};
-    if ((e = (int)comod::ck_launch(kh, (int64_t)3 * hc * wc, s))) return e;
-    comod::FeatherCropK kf{g, image + (int64_t)y0 * W + x0, mask + (int64_t)y0 * W + x0, (int64_t)H * W, W, hc, wc, {0}};
-    for (int i = 0; i < 25; ++i) kf.k[i] = k25_host[i];
-    return (int)comod::ck_launch(kf, (int64_t)hc * wc, s);
+    const migan_pipe_request q = one_request(image, mask, H, W, box);
+    return launch_pipeline_postprocess_batch(y, &q, 1, res, k25_host, scratch, s);
 }
 
 }  // namespace migan
 
 #ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (argument checks, error strings) live in migan_abi.cu
-namespace migan {
-size_t pipeline_scratch_bytes(int H, int W, int res);
-}
 extern "C" size_t b200_pipeline_scratch_bytes(int H, int W, int res) { return migan::pipeline_scratch_bytes(H, W, res); }
 extern "C" int b200_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, void* s) {
     return migan::launch_resize_nearest_u8(in, H, W, out, oh, ow, s);
@@ -321,5 +576,33 @@ extern "C" int b200_pipeline_preprocess(const uint8_t* image, const uint8_t* mas
 extern "C" int b200_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
                                          const float* k25, void* scratch, size_t, void* s) {
     return migan::launch_pipeline_postprocess(y, image, mask, H, W, box, res, k25, scratch, s);
+}
+// The batched entry points with the product's argument checks (return codes only: no error string here).
+extern "C" int b200_hole_flags_batch(const migan_pipe_request* q, int n, uint8_t* flags, void* s) {
+    char msg[256];
+    if (int rc = migan::check_pipe_batch(q, n, 1, false, msg, sizeof msg)) return rc;
+    if (!flags) return MIGAN_ERR_INVALID;
+    return migan::launch_hole_flags_batch(q, n, flags, s);
+}
+extern "C" size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* q, int n, int res) {
+    char msg[256];
+    if (migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return 0;
+    return migan::pipeline_batch_scratch_bytes(q, n, res);
+}
+extern "C" int b200_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res, float* x, void* scratch, size_t scratch_bytes,
+                                              void* s) {
+    char msg[256];
+    if (int rc = migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return rc;
+    if (!x || !scratch) return MIGAN_ERR_INVALID;
+    if (scratch_bytes < migan::pipeline_batch_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
+    return migan::launch_pipeline_preprocess_batch(q, n, res, x, scratch, s);
+}
+extern "C" int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* q, int n, int res, const float* k25,
+                                               void* scratch, size_t scratch_bytes, void* s) {
+    char msg[256];
+    if (int rc = migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return rc;
+    if (!y || !k25 || !scratch) return MIGAN_ERR_INVALID;
+    if (scratch_bytes < migan::pipeline_batch_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
+    return migan::launch_pipeline_postprocess_batch(y, q, n, res, k25, scratch, s);
 }
 #endif

@@ -4,18 +4,25 @@ Same constructor and call as the reference class:
 
     pipe = MIGAN_Pipeline(model_path, resolution, padding=128, device="cuda")
     result = pipe(image, mask)       # image (1,3,H,W) uint8, mask (1,1,h,w) uint8 (255 = known); image is updated in place
+    results = pipe.forward_batch([image_0, image_1, ...], [mask_0, mask_1, ...])   # requests of different sizes at once
 
 What happens per request (all on the GPU, kernels in csrc/pipeline.cu behind include/migan_b200.h):
-mask -> image size (nearest) -> hole flags per column / row -> [4 ints to the host] crop window (`get_masked_bbox`
+mask -> image size (nearest) -> hole flags per column / row -> [flags to the host] crop window (`get_masked_bbox`
 arithmetic) -> crop resized to the model resolution (anti-aliased bilinear, bit-identical to torchvision's tensor resize on the
-CPU) and turned into the generator input -> `Generator.forward` (the captured CUDA graph at batch 1) -> output mapped to
-[0, 255], resized to the crop, blended into the image under the feathered mask.  The one host round trip is the crop
-window: the sizes of everything after it depend on it.  There is no CPU path.
+CPU) and turned into the generator input -> `Generator.forward` -> output mapped to [0, 255], resized to the crop, blended
+into the image under the feathered mask.  The one host round trip is the crop window: the sizes of everything after it
+depend on it.  There is no CPU path.
+
+Every call, single request or many, runs in passes of up to 32 requests: one launch per stage covers every request of the
+pass (hole flags, weight tables, width pass, height pass; the post-processing's height pass is fused into the blend), the
+flags of the whole pass come to the host in one copy, and the generator runs once at the pass's batch size (the captured
+CUDA graph when that is at most `model.graph_max_batch`).  The generator's output does not depend on the batch size, so
+request i of a pass gets the same bytes as a call with request i alone.
 """
 from __future__ import annotations
 
 import ctypes
-from typing import Tuple, Union
+from typing import List, Tuple, Union
 
 import torch
 
@@ -47,7 +54,8 @@ class MIGAN_Pipeline(torch.nn.Module):
         self.padding = int(padding)
         self.device_ = device
         self._scratch = None
-        self.last_box: Tuple[int, int, int, int] = (0, 0, 0, 0)
+        self.last_box: Tuple[int, int, int, int] = (0, 0, 0, 0)     # the last request's crop window
+        self.last_boxes: List[Tuple[int, int, int, int]] = []        # every request's crop window of the last call
 
     # -- stages (each a call into the C ABI) ------------------------------------------------------------------------
     def get_masked_bbox(self, mask: torch.Tensor) -> Tuple[int, int, int, int]:
@@ -63,48 +71,113 @@ class MIGAN_Pipeline(torch.nn.Module):
         _abi.check(lib.migan_crop_box(flags_h.data_ptr(), H, W, self.res, int(self.padding), ctypes.cast(box, ctypes.c_void_p)))
         return int(box[0]), int(box[1]), int(box[2]), int(box[3])
 
-    def _scratch_for(self, H: int, W: int, device) -> torch.Tensor:
-        need = int(_abi.load().b200_pipeline_scratch_bytes(H, W, self.res))
+    def _scratch_for(self, need: int, device) -> torch.Tensor:
         if self._scratch is None or self._scratch.numel() < need or self._scratch.device != device:
             self._scratch = torch.empty(need, dtype=torch.uint8, device=device)
         return self._scratch
 
-    def _one(self, image: torch.Tensor, mask: torch.Tensor) -> None:
-        """image [3,H,W] uint8 CUDA contiguous (updated in place), mask [h,w] uint8 CUDA."""
+    def _chunk(self, images, masks) -> list:
+        """One pass over <= 32 requests: images [3,H,W] uint8 CUDA contiguous (updated in place), masks [h,w] uint8 CUDA
+        contiguous, all on one device.  Returns the crop windows."""
         lib = _abi.load()
-        H, W = int(image.shape[1]), int(image.shape[2])
-        if H < 3 or W < 3:
-            raise RuntimeError("image of %d x %d: the feathering needs at least 3 x 3 pixels" % (H, W))
-        stream = ops._stream(image)
-        with torch.cuda.device(image.device):
-            if tuple(mask.shape) != (H, W):                       # :255
-                m2 = torch.empty((H, W), dtype=torch.uint8, device=image.device)
-                _abi.check(lib.b200_resize_nearest_u8(mask.data_ptr(), int(mask.shape[0]), int(mask.shape[1]), m2.data_ptr(), H, W, stream))
-                mask = m2
-            x0, x1, y0, y1 = self.get_masked_bbox(mask)
-            self.last_box = (x0, x1, y0, y1)
-            box = (ctypes.c_int * 4)(x0, x1, y0, y1)
-            pbox = ctypes.cast(box, ctypes.c_void_p)
-            scratch = self._scratch_for(H, W, image.device)
-            x = torch.empty((1, 4, self.res, self.res), dtype=torch.float32, device=image.device)
-            _abi.check(lib.b200_pipeline_preprocess(image.data_ptr(), mask.data_ptr(), H, W, pbox, self.res, x.data_ptr(),
-                                                    scratch.data_ptr(), scratch.numel(), stream))
+        n = len(images)
+        dev = images[0].device
+        stream = ops._stream(images[0])
+        reqs = (_abi.PipeRequest * n)()
+        keep = []                                                  # resized masks stay alive until the launches are enqueued
+        with torch.cuda.device(dev):
+            for i, (image, mask) in enumerate(zip(images, masks)):
+                H, W = int(image.shape[1]), int(image.shape[2])
+                if tuple(mask.shape) != (H, W):                   # :255
+                    m2 = torch.empty((H, W), dtype=torch.uint8, device=dev)
+                    _abi.check(lib.b200_resize_nearest_u8(mask.data_ptr(), int(mask.shape[0]), int(mask.shape[1]), m2.data_ptr(), H, W, stream))
+                    keep.append(m2)
+                    mask = m2
+                reqs[i].image, reqs[i].mask, reqs[i].H, reqs[i].W = image.data_ptr(), mask.data_ptr(), H, W
+            flags = torch.empty(sum(r.W + r.H for r in reqs), dtype=torch.uint8, device=dev)
+            _abi.check(lib.b200_hole_flags_batch(reqs, n, flags.data_ptr(), stream))
+            flags_h = flags.cpu()                                  # the one synchronisation of the pass
+            off = 0
+            for r in reqs:
+                _abi.check(lib.migan_crop_box(flags_h.data_ptr() + off, r.H, r.W, self.res, int(self.padding), ctypes.addressof(r.box)))
+                off += r.W + r.H
+            scratch = self._scratch_for(int(lib.b200_pipeline_batch_scratch_bytes(reqs, n, self.res)), dev)
+            x = torch.empty((n, 4, self.res, self.res), dtype=torch.float32, device=dev)
+            _abi.check(lib.b200_pipeline_preprocess_batch(reqs, n, self.res, x.data_ptr(), scratch.data_ptr(), scratch.numel(), stream))
             y = self.model(x)
-            _abi.check(lib.b200_pipeline_postprocess(y.data_ptr(), image.data_ptr(), mask.data_ptr(), H, W, pbox, self.res,
-                                                     self._k25.data_ptr(), scratch.data_ptr(), scratch.numel(), stream))
+            if y.dtype != torch.float32 or tuple(y.shape) != (n, 3, self.res, self.res) or not y.is_contiguous():
+                raise RuntimeError("generator output must be contiguous float32 (%d,3,%d,%d)" % (n, self.res, self.res))
+            _abi.check(lib.b200_pipeline_postprocess_batch(y.data_ptr(), reqs, n, self.res, self._k25.data_ptr(),
+                                                           scratch.data_ptr(), scratch.numel(), stream))
+        return [tuple(int(v) for v in r.box) for r in reqs]
+
+    def _run(self, images, masks) -> None:
+        """images [3,H,W] / masks [h,w]: CUDA, contiguous, one device; chunks of _abi.PIPE_MAX_BATCH requests."""
+        for image in images:
+            H, W = int(image.shape[1]), int(image.shape[2])
+            if H < 3 or W < 3:
+                raise RuntimeError("image of %d x %d: the feathering needs at least 3 x 3 pixels" % (H, W))
+            if image.device != images[0].device:
+                raise RuntimeError("MIGAN_Pipeline: the requests of one call must be on one device (%s and %s)" % (images[0].device, image.device))
+        boxes = []
+        for c in range(0, len(images), _abi.PIPE_MAX_BATCH):
+            boxes += self._chunk(images[c:c + _abi.PIPE_MAX_BATCH], masks[c:c + _abi.PIPE_MAX_BATCH])
+        if boxes:
+            self.last_boxes = boxes
+            self.last_box = boxes[-1]
 
     @torch.no_grad()
     def forward(self, image: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
         """image: (N,3,H,W) uint8, mask: (N,1,h,w) uint8 (255 = known).  The image is updated in place and returned (like the
-        reference, whose deployed form takes N = 1; N > 1 runs the requests one after the other, each with its own crop)."""
+        reference, whose deployed form takes N = 1; N > 1 gives each request its own crop, as if run one after the other)."""
         if image.dtype != torch.uint8 or mask.dtype != torch.uint8:
             raise RuntimeError("MIGAN_Pipeline expects uint8 image and mask")
         if image.dim() != 4 or image.shape[1] != 3 or mask.dim() != 4 or mask.shape[1] != 1 or mask.shape[0] != image.shape[0]:
             raise RuntimeError("MIGAN_Pipeline expects image (N,3,H,W) and mask (N,1,h,w)")
         img_d = image if (image.is_cuda and image.is_contiguous()) else image.to(self.device_).contiguous()
         mask_d = mask.to(img_d.device).contiguous()
-        for i in range(img_d.shape[0]):
-            self._one(img_d[i], mask_d[i, 0])
+        self._run([img_d[i] for i in range(img_d.shape[0])], [mask_d[i, 0] for i in range(img_d.shape[0])])
         if img_d is not image:
             image.copy_(img_d)
         return image
+
+    @torch.no_grad()
+    def forward_batch(self, images, masks) -> list:
+        """Many requests of any sizes in one pass per 32: images[i] (1,3,H_i,W_i) uint8 and masks[i] (1,1,h_i,w_i) uint8
+        (255 = known), CUDA or CPU tensors.  Each image is updated in place, and the list of images is returned;
+        `forward_batch(images, masks)[i]` is bit-identical to `pipe(images[i], masks[i])`.  `last_boxes` holds every crop
+        window.  An image may not overlap another image or any mask: a batch cannot reproduce requests that read what an
+        earlier one wrote."""
+        images, masks = list(images), list(masks)
+        if len(images) != len(masks):
+            raise RuntimeError("MIGAN_Pipeline.forward_batch: %d images and %d masks" % (len(images), len(masks)))
+        for image, mask in zip(images, masks):
+            if image.dtype != torch.uint8 or mask.dtype != torch.uint8:
+                raise RuntimeError("MIGAN_Pipeline expects uint8 images and masks")
+            if image.dim() != 4 or tuple(image.shape[:2]) != (1, 3) or mask.dim() != 4 or tuple(mask.shape[:2]) != (1, 1):
+                raise RuntimeError("MIGAN_Pipeline.forward_batch expects images (1,3,H,W) and masks (1,1,h,w)")
+        spans = [_span(t) for t in images + masks]
+        for i in range(len(images)):
+            for j in range(len(spans)):
+                if j != i and _overlap(spans[i], spans[j]):
+                    raise RuntimeError("MIGAN_Pipeline.forward_batch: image %d overlaps %s %d in memory" % (
+                        i, "image" if j < len(images) else "mask", j if j < len(images) else j - len(images)))
+        imgs_d = [im if (im.is_cuda and im.is_contiguous()) else im.to(self.device_).contiguous() for im in images]
+        masks_d = [m.to(im.device).contiguous() for m, im in zip(masks, imgs_d)]
+        self._run([im[0] for im in imgs_d], [m[0, 0] for m in masks_d])
+        for image, img_d in zip(images, imgs_d):
+            if img_d is not image:
+                image.copy_(img_d)
+        return images
+
+
+def _span(t: torch.Tensor):
+    """(device, first byte, one past the last byte) of the memory a tensor's elements occupy."""
+    if t.numel() == 0:
+        return (t.device, 0, 0)
+    extent = 1 + sum((s - 1) * st for s, st in zip(t.shape, t.stride()))
+    return (t.device, t.data_ptr(), t.data_ptr() + extent * t.element_size())
+
+
+def _overlap(a, b) -> bool:
+    return a[0] == b[0] and a[1] < b[2] and b[1] < a[2]
