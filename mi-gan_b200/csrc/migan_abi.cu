@@ -819,11 +819,20 @@ struct PlanBuilder {
             const float* img_lo = (img_cur >= 0) ? IMG[img_cur] : nullptr;
             float* img_out = last ? nullptr : IMG[img_next];      // last level: the caller's y (bound at launch)
             const ToRgb& T = c->torgb[i];
-            const bool fuse_rgb = tcp && channels(r) <= (path == MIGAN_PATH_TC_FAST ? 128 : 64);   // all output channels in one CTA tile
             // conv1's FIR + noise + activation + skip can be rebuilt in conv2's prologue (the up-sampled tensor then never
             // exists in HBM) when conv2 runs its depthwise stage in the tensor-core kernel with 8 x 16 tiles.
             const SepConv& L1 = c->syn1[i];
-            const bool fuse_up = tcp && L1.up && L1.up_uniform && r >= 16 && (channels(r) < 512 || fuse_rgb);
+            const SepConv& L2 = c->syn2[i];
+            const bool fuse_up = tcp && L1.up && L1.up_uniform && r >= 16 && channels(r) < 512;
+            // torgb runs in conv2's epilogue when the plan puts all of conv2's output channels in one CTA tile
+            bool fuse_rgb = false;
+            if (tcp) {
+                migan::SepconvTcDesc q;
+                q.passes = (path == MIGAN_PATH_TC_FAST) ? 1 : 3;
+                q.source = fuse_up ? migan::SEPCONV_SRC_UP : migan::SEPCONV_SRC_NHWC;
+                q.n = n; q.res = L2.res_pw; q.cin = L2.cin; q.cout = L2.cout;
+                fuse_rgb = migan::sepconv_tc_fuses_rgb(q);
+            }
             Fuse f1; f1.defer_up = fuse_up;
             int rc = emit_sepconv(L1, cur, cur_idx, nullptr, feat[r], oi, op, nullptr, std::string(), 0, f1);  // x = conv1(x) + enc_feat
             if (rc) return rc;

@@ -25,6 +25,11 @@
 // The accumulators of an M = 128 tile (main + corr of 64 channels, or 128 channels in fast mode) are 128 registers per thread of one warpgroup, so setmaxnreg moves
 // registers from the producer warpgroup (which needs few) to the MMA warpgroup; the prologue keeps 128.
 // All hand-offs are mbarrier pipelines (input ring, A ring, B ring).
+//
+// Stationary A (n_group > 1): a CTA tile is one pixel tile x n_group consecutive N tiles.  The A ring then has one slot
+// per K block (a_stages = num_kb): the prologue runs once per pixel tile and the whole K extent of A stays resident
+// while the MMA warpgroup walks the group's N tiles; a slot is released only after the group's last N tile has retired
+// it.  n_group = 1 is the plain schedule (one N tile per CTA tile, A streamed through a shallow ring).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -61,7 +66,8 @@ constexpr int kChunkC = 32;        // channels per input chunk (128 bytes of fp3
 constexpr uint32_t kABytes = kTileM * kKBlock * 2;   // 16 KB per hi or lo
 constexpr uint32_t kAStage = 2 * kABytes;            // hi + lo
 constexpr uint32_t kSmemLimit = 232448;              // 227 KB
-constexpr int kRgbBias = 3 * kMaxTileN, kRgbFir = 3 * kMaxTileN + 4;   // offsets inside the torgb table s_rgb
+constexpr int kMaxRgbC = 256;      // fused torgb: the widest cout whose weights the static table s_rgb holds
+constexpr int kRgbBias = 3 * kMaxRgbC, kRgbFir = 3 * kMaxRgbC + 4;   // offsets inside the torgb table s_rgb
 constexpr uint32_t kStaticSmem = 4096;               // barriers + torgb table (static __shared__), rounded up
 
 struct Params {
@@ -74,9 +80,10 @@ struct Params {
     int n, H, W, cin, cout;
     int act, passes;
     int source;                               // SepconvSource
-    int tile_n, tile_h, tile_w, n_tile;      // n_tile = output channels per CTA tile (64 or 128)
+    int tile_n, tile_h, tile_w, n_tile;      // n_tile = output channels per N tile (64 or 128)
     int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / n_tile
-    int l_tx, l_ty, l_nt;                     // log2 of tiles_x, tiles_y, num_n_tiles (all powers of two: no runtime division)
+    int n_group;                              // N tiles per CTA tile (power of two; > 1: stationary A)
+    int l_tx, l_ty, l_nt;                     // log2 of tiles_x, tiles_y, num_n_tiles / n_group (all powers of two: no runtime division)
     int num_kb;                               // cin / 64
     int in_stages, a_stages, b_stages, b_resident;
     uint32_t in_tx_bytes;                     // bytes the TMA unit delivers per input stage
@@ -92,7 +99,8 @@ struct Params {
     // STEM pre-stage
     const float* stem_w;
     const float* stem_b;
-    // fused torgb + image path (SynthesisBlock.forward, migan_inference.py:308-313); needs all of cout in one tile
+    // fused torgb + image path (SynthesisBlock.forward, migan_inference.py:308-313); needs all of cout in one CTA tile
+    // (n_group == num_n_tiles)
     int torgb, store_out;
     const float* rgb_w;                       // [3][cout]
     const float* rgb_b;                       // [3]
@@ -233,11 +241,11 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
 }
 
 struct TileCoord {
-    int n0, y0, x0, nt;   // first image / row / column of the M tile, N-tile index
+    int n0, y0, x0, nt;   // first image / row / column of the M tile, first N tile of the CTA tile's group
 };
 __device__ __forceinline__ TileCoord decode_tile(const Params& p, int tile) {
     TileCoord c;
-    c.nt = tile & (p.num_n_tiles - 1);
+    c.nt = (tile & ((1 << p.l_nt) - 1)) * p.n_group;
     int m = tile >> p.l_nt;
     c.x0 = (m & (p.tiles_x - 1)) * p.tile_w;
     m >>= p.l_tx;
@@ -256,16 +264,19 @@ struct Ring {
     }
 };
 
-// mbarriers: [0,8) full_in  [8,16) empty_in  [16,20) full_a  [20,24) empty_a  [24,32) full_b  [32,40) empty_b
-constexpr int kNumBars = 40;
+// mbarriers: [0,8) full_in  [8,16) empty_in  [16,24) full_a  [24,32) empty_a  [32,40) full_b  [40,48) empty_b
+constexpr int kNumBars = 48;
+constexpr int kMaxAStages = 8;
+static_assert(kNumBars * 8 + (3 * kMaxRgbC + 4 + 48) * 4 <= (int)kStaticSmem, "static shared memory outgrew kStaticSmem");
 __device__ __forceinline__ uint32_t bar_full_a(uint32_t bar0, int s) { return bar0 + 8u * (16 + s); }
-__device__ __forceinline__ uint32_t bar_empty_a(uint32_t bar0, int s) { return bar0 + 8u * (20 + s); }
-__device__ __forceinline__ uint32_t bar_full_b(uint32_t bar0, int s) { return bar0 + 8u * (24 + s); }
-__device__ __forceinline__ void mma_release(const Params& p, uint32_t bar0, int sa, int sb) {
+__device__ __forceinline__ uint32_t bar_empty_a(uint32_t bar0, int s) { return bar0 + 8u * (24 + s); }
+__device__ __forceinline__ uint32_t bar_full_b(uint32_t bar0, int s) { return bar0 + 8u * (32 + s); }
+__device__ __forceinline__ uint32_t bar_empty_b(uint32_t bar0, int s) { return bar0 + 8u * (40 + s); }
+__device__ __forceinline__ void mma_release(const Params& p, uint32_t bar0, int sa, int sb, bool release_a) {
     __syncwarp();
     if ((threadIdx.x & 31) == 0) {             // one arrival per warp: each warp waited for its own wgmma groups
-        mbar_arrive(bar_empty_a(bar0, sa));
-        if (!p.b_resident) mbar_arrive(bar0 + 8u * (32 + sb));
+        if (release_a) mbar_arrive(bar_empty_a(bar0, sa));
+        if (!p.b_resident) mbar_arrive(bar_empty_b(bar0, sb));
     }
 }
 
@@ -288,14 +299,21 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
     const uint32_t b_stage_bytes = (uint32_t)NT * kKBlock * 2 * 2;   // [Bh ; Bl]
     const int hw = p.tile_h * p.tile_w;
     float acc[2][NA], cor[2][NC];
+    float rgb_acc[4];                                // torgb sum of colour lane % 4 over the group's N tiles, per pixel row
     Ring ra(p.a_stages), rb(p.b_stages);
     for (int it = 0; it < my_tiles; ++it) {
-        const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+      const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+      for (int j = 0; j < p.n_group; ++j) {
+        // Stationary A (n_group > 1): slot kb holds K block kb for the whole group.  The first N tile waits for it, the
+        // last one releases it.
+        const bool first_n = (j == 0), last_n = (j == p.n_group - 1);
         int prev_sa = 0, prev_sb = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
-            const int sa = ra.stage;
-            mbar_wait(bar_full_a(bar0, sa), ra.phase, 210 + sa, p.error_flag);
-            ra.advance();
+            const int sa = (p.n_group > 1) ? kb : ra.stage;
+            if (first_n) {
+                mbar_wait(bar_full_a(bar0, sa), ra.phase, 210 + sa, p.error_flag);
+                ra.advance();
+            }
             const int sb = p.b_resident ? kb : rb.stage;
             mbar_wait(bar_full_b(bar0, sb), p.b_resident ? 0 : rb.phase, 220 + sb, p.error_flag);
             if (!p.b_resident) rb.advance();
@@ -323,7 +341,7 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
             wg_commit();
             if (kb > 0) {                        // the previous K block's MMAs have retired: its A / B slots are free
                 wg_wait<1>();
-                mma_release(p, bar0, prev_sa, prev_sb);
+                mma_release(p, bar0, prev_sa, prev_sb, last_n);
             }
             prev_sa = sa; prev_sb = sb;
         }
@@ -331,10 +349,10 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
         wg_fence_acc(acc[0]);
         wg_fence_acc(acc[1]);
         if constexpr (kSplit) { wg_fence_acc(cor[0]); wg_fence_acc(cor[1]); }
-        mma_release(p, bar0, prev_sa, prev_sb);
+        mma_release(p, bar0, prev_sa, prev_sb, last_n);
 
         // ---- epilogue: the four pixel rows of this thread, straight from the accumulators ----
-        const int chan0 = tc.nt * NT;
+        const int chan0 = (tc.nt + j) * NT;
         const float scale_g = p.inv_scale * kActGain;
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
@@ -347,11 +365,11 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
             float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0 + 2 * (lane & 3);
             float s0 = 0.f, s1 = 0.f, s2 = 0.f;      // torgb partial sums over this thread's channels
 #pragma unroll
-            for (int j = 0; j < NT / 8; ++j) {
+            for (int jj = 0; jj < NT / 8; ++jj) {
                 float o[2];
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
-                    const float v = kSplit ? acc[h][j * 4 + i * 2 + c] + cor[h][(j * 4 + i * 2 + c) % NC] : acc[h][j * 4 + i * 2 + c];
+                    const float v = kSplit ? acc[h][jj * 4 + i * 2 + c] + cor[h][(jj * 4 + i * 2 + c) % NC] : acc[h][jj * 4 + i * 2 + c];
                     if (p.act) {                     // clamp(lrelu(f) * sqrt2) with the gain folded into the scale
                         const float a = fmaf(v, scale_g, nz_g);
                         o[c] = fminf(fmax3(a, a * kLreluAlpha, -kActClamp), kActClamp);
@@ -359,17 +377,18 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                         o[c] = fmaf(v, p.inv_scale, nz);
                     }
                 }
-                if (p.torgb) {                       // 1x1 conv Cout -> 3 on the activated row (the tile holds all of cout)
-                    const int ch = 8 * j + 2 * (lane & 3);
+                if (p.torgb) {                       // 1x1 conv Cout -> 3 on the activated row (the CTA tile holds all of cout)
+                    const int ch = chan0 + 8 * jj + 2 * (lane & 3);
                     s0 = fmaf(o[1], s_rgb[ch + 1], fmaf(o[0], s_rgb[ch], s0));
                     s1 = fmaf(o[1], s_rgb[p.cout + ch + 1], fmaf(o[0], s_rgb[p.cout + ch], s1));
                     s2 = fmaf(o[1], s_rgb[2 * p.cout + ch + 1], fmaf(o[0], s_rgb[2 * p.cout + ch], s2));
                 }
-                if (p.store_out && valid) *reinterpret_cast<float2*>(out_px + 8 * j) = make_float2(o[0], o[1]);
+                if (p.store_out && valid) *reinterpret_cast<float2*>(out_px + 8 * jj) = make_float2(o[0], o[1]);
             }
             if (p.torgb) {
                 // img = upsample(img_lo) + (torgb(x) + b)   (migan_inference.py:308-313); planar NCHW.  The quad holds the
-                // pixel's channels: sum its partials, then lane k of the quad writes colour k.
+                // pixel's channels of this N tile: sum its partials; lane k of the quad owns colour k of the row and adds
+                // the N tiles up in registers.  After the group's last N tile it writes the pixel.
 #pragma unroll
                 for (int x = 1; x < 4; x <<= 1) {
                     s0 += __shfl_xor_sync(0xffffffffu, s0, x);
@@ -377,8 +396,10 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                     s2 += __shfl_xor_sync(0xffffffffu, s2, x);
                 }
                 const int k = lane & 3;
-                if (k < 3 && valid) {
-                    float rv = (k == 0 ? s0 : (k == 1 ? s1 : s2)) + s_rgb[kRgbBias + k];
+                const float sk = k == 0 ? s0 : (k == 1 ? s1 : s2);
+                rgb_acc[r] = first_n ? sk : rgb_acc[r] + sk;
+                if (last_n && k < 3 && valid) {
+                    float rv = rgb_acc[r] + s_rgb[kRgbBias + k];
                     if (p.img_lo) {
                         const int hl = p.H >> 1, wl = p.W >> 1;
                         float up = 0.f;
@@ -398,6 +419,7 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                 }
             }
         }
+      }
     }
 }
 
@@ -406,7 +428,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 sepconv_tc_kernel(const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t bars[kNumBars];
-    __shared__ __align__(16) float s_rgb[3 * kMaxTileN + 4 + 48];   // torgb weights [3][cout<=128], bias[3(+1)], fir[16][3]
+    __shared__ __align__(16) float s_rgb[3 * kMaxRgbC + 4 + 48];    // torgb weights [3][cout<=256], bias[3(+1)], fir[16][3]
 
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -418,7 +440,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
     auto full_a = [&](int s) { return bar_full_a(bar0, s); };
     auto empty_a = [&](int s) { return bar_empty_a(bar0, s); };
     auto full_b = [&](int s) { return bar_full_b(bar0, s); };
-    auto empty_b = [&](int s) { return bar0 + 8u * (32 + s); };
+    auto empty_b = [&](int s) { return bar_empty_b(bar0, s); };
 
     const int a_dw = (p.source != SEPCONV_SRC_SPLIT);
     if (threadIdx.x == 0) {
@@ -483,9 +505,11 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
             for (int c = 0; c < p.prefetch; ++c) prefetch_next();
             Ring rin(p.in_stages), ra(p.a_stages), rb(p.b_stages);
             for (int it = 0; it < my_tiles; ++it) {
-                const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+              const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+              for (int j = 0; j < p.n_group; ++j) {
                 for (int kb = 0; kb < num_kb; ++kb) {
-                    if (a_dw) {
+                    // A (or the prologue's input) once per pixel tile; the group's later N tiles only need their weights
+                    if (j == 0 && a_dw) {
                         for (int g = 0; g < 2; ++g) {
                             const int s = rin.stage;
                             if (p.prefetch) prefetch_next();
@@ -504,7 +528,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                                 }
                             }
                         }
-                    } else {
+                    } else if (j == 0) {
                         const int s = ra.stage;
                         if (p.prefetch) prefetch_next();
                         mbar_wait<true>(empty_a(s), ra.phase ^ 1, 110 + s, p.error_flag);
@@ -519,11 +543,12 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                         if (!p.b_resident) { mbar_wait<true>(empty_b(s), rb.phase ^ 1, 120 + s, p.error_flag); rb.advance(); }
                         mbar_expect_tx(full_b(s), b_stage_bytes);
                         const uint32_t dst = smem_base + p.off_b + s * b_stage_bytes;
-                        const int row = tc.nt * p.n_tile;
+                        const int row = (tc.nt + j) * p.n_tile;
                         tma_load_2d(dst, &p.map_w_hi, full_b(s), kb * kKBlock, row);
                         tma_load_2d(dst + b_stage_bytes / 2, &p.map_w_lo, full_b(s), kb * kKBlock, row);
                     }
                 }
+              }
             }
         }
     } else if (warp >= kMmaWarp0) {
@@ -666,20 +691,25 @@ int sepconv_tc_timeout_record(int device) {
     return (device >= 0 && device < kMaxDevices && g_error_flag_host[device]) ? *g_error_flag_host[device] : 0;
 }
 
-const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
-    Params p;
-    memset(&p, 0, sizeof(p));
+namespace {
+
+// SMs the persistent grid may use.  MIGAN_TC_RESERVE_SMS leaves SMs free for a concurrently running collective.
+int grid_sms() {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms - std::max(0, std::min(env_int("MIGAN_TC_RESERVE_SMS", 0), sms / 2));
+}
+
+// Tiling, N grouping, ring depths and shared-memory layout of a launch.  They depend on the shapes, the source and
+// whether torgb is fused, never on a pointer, so the generator's planner can ask before it commits to fusing torgb.
+const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& smem_bytes) {
     const int n = d.n, res = d.res, cin = d.cin, cout = d.cout;
     if (cin % kKBlock != 0 || cout % 64 != 0) return "cin must be a multiple of 64 and cout of 64";
     if (res < 4 || (res & (res - 1))) return "resolution must be a power of two >= 4";
     p.source = d.source;
     const bool dw = (d.source != SEPCONV_SRC_SPLIT);
-    if (d.source == SEPCONV_SRC_SPLIT && !(d.a_hi && d.a_lo)) return "no A operand";
-    if ((d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) && !d.in_f32) return "no input tensor";
-    if (d.source == SEPCONV_SRC_UP && !d.up_t) return "no low-resolution tensor for the up-sampling prologue";
-    if (d.source == SEPCONV_SRC_STEM && !(d.stem_w && d.stem_b)) return "no fromrgb weights for the stem prologue";
     if ((d.source == SEPCONV_SRC_UP || d.source == SEPCONV_SRC_STEM) && res < 16) return "fused prologues need 8 x 16 tiles (res >= 16)";
-    p.w9 = d.w9; p.bias = d.bias; p.noise = d.noise; p.inv_scale = d.inv_scale; p.out = d.out;
     p.n = n; p.H = res; p.W = res; p.cin = cin; p.cout = cout; p.act = d.act; p.passes = d.passes;
     p.n_tile = (cout == 64 || d.passes == 3) ? 64 : kMaxTileN;   // main + corr of 64 channels fill the accumulators
     p.num_kb = cin / kKBlock;
@@ -692,17 +722,14 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     }
     p.tile_n = kTileM / (p.tile_w * p.tile_h);
     p.tiles_x = res / p.tile_w; p.tiles_y = res / p.tile_h; p.tiles_n = (n + p.tile_n - 1) / p.tile_n;
-    int dev0 = 0, sms0 = 132;
-    cudaGetDevice(&dev0);
-    cudaDeviceGetAttribute(&sms0, cudaDevAttrMultiProcessorCount, dev0);
+    const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
     // Few pixel tiles (the 4 x 4 ... 16 x 16 levels at small batches): most SMs would idle while a few CTAs stream the
     // weight matrix.  Narrow N tiles spread the layer over 2 x the CTAs.
-    if (!d.rgb && p.n_tile > 64 && cout >= 256 && p.tiles_x * p.tiles_y * p.tiles_n * (cout / p.n_tile) * 2 < sms0)
+    if (!d.rgb && p.n_tile > 64 && cout >= 256 && m_tiles * (cout / p.n_tile) * 2 < sms)
         p.n_tile = 64;
     p.num_n_tiles = cout / p.n_tile;
-    p.num_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.num_n_tiles;
     auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
-    p.l_tx = ilog2(p.tiles_x); p.l_ty = ilog2(p.tiles_y); p.l_nt = ilog2(p.num_n_tiles);
+    p.l_tx = ilog2(p.tiles_x); p.l_ty = ilog2(p.tiles_y);
 
     // ---- input stage: IN area (+ T, NZ | XA) ----
     const uint32_t in_chunk_bytes = (uint32_t)(p.tile_n * (p.tile_h + 2) * (p.tile_w + 2) * kChunkC * 4);
@@ -714,23 +741,14 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
         p.off_aux = p.off_t + 6 * 10 * kChunkC * 4;
         stage_bytes = p.off_aux + 10 * kAuxW * 4;
         p.in_tx_bytes = in_chunk_bytes + 6 * 10 * kChunkC * 4 + (p.up_has_noise ? 10 * kAuxW * 4 : 0);
-        memcpy(p.up_taps.f, d.up_taps, sizeof(p.up_taps.f));
     } else if (d.source == SEPCONV_SRC_STEM) {
         p.off_aux = in_chunk_bytes;
         stage_bytes = p.off_aux + 4 * 10 * kAuxW * 4;
         p.in_tx_bytes = 4 * 10 * kAuxW * 4;
-        p.stem_w = d.stem_w; p.stem_b = d.stem_b;
     }
     p.in_stage_stride = (stage_bytes + 1023u) & ~1023u;
 
-    p.store_out = 1;
-    if (d.rgb) {
-        if (p.num_n_tiles != 1) return "fused torgb needs all output channels of a pixel tile in one CTA tile (cout <= 64, or 128 in fast mode)";
-        p.torgb = 1; p.store_out = d.rgb->store_out;
-        p.rgb_w = d.rgb->w; p.rgb_b = d.rgb->b; p.rgb_fir = d.rgb->fir; p.img_lo = d.rgb->img_lo; p.img_out = d.rgb->img_out;
-    }
-
-    // ---- shared-memory budget -> stage counts ----
+    // ---- shared-memory budget -> N group and stage counts ----
     const uint32_t b_stage = (uint32_t)p.n_tile * kKBlock * 2 * 2;
     const uint32_t budget = kSmemLimit - kStaticSmem - 1024;   // static smem + alignment slack
     // The input ring is shared by the two prologue groups (even chunks -> group 0, odd -> group 1):
@@ -738,12 +756,26 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     // observes every phase of its barriers (parity waits alias otherwise).
     p.b_resident = (p.num_n_tiles == 1 && (uint32_t)p.num_kb * b_stage <= 65536) ? 1 : 0;
     const uint32_t tables = dw ? 40u * cin + (d.source == SEPCONV_SRC_STEM ? 20u * cin : 0u) : 0u;
-    bool found = false;
-    // candidate configurations in order of preference: deeper input ring first, then a deeper A ring (the prologue runs
-    // ahead while the MMA warpgroup drains its accumulators)
-    struct Cand { int in_stages, b_stages, a_stages; };
+    // candidate configurations in order of preference
+    struct Cand { int n_group, in_stages, b_stages, a_stages; bool dw_global; };
     std::vector<Cand> cands;
+    // Stationary A, for the sources with a prologue: it then runs once per pixel tile instead of once per N tile.  The
+    // group is the widest that still gives every SM a CTA tile (all N tiles when torgb is fused).  The depthwise taps
+    // move from shared memory to global (L1-cached) loads only where that is what makes the resident A fit.
+    if (dw && p.num_n_tiles > 1 && p.num_kb <= kMaxAStages) {
+        int g = p.num_n_tiles;
+        if (!d.rgb)
+            while (g > 1 && m_tiles * (p.num_n_tiles / g) < sms) g >>= 1;
+        if (g > 1)
+            for (bool dw_global : {false, true}) {
+                if (dw_global && d.source == SEPCONV_SRC_STEM) continue;   // the fromrgb table lives next to the taps
+                for (int bs : {3, 2})
+                    for (int in_st : {6, 4, 2}) cands.push_back({g, in_st, bs, p.num_kb, dw_global});
+            }
+    }
     {
+        // plain schedule: deeper input ring first, then a deeper A ring (the prologue runs ahead while the MMA warpgroup
+        // drains its accumulators)
         const int b_res = p.b_resident ? p.num_kb : 0;
         // input ring depths to try, deepest first (even: each prologue group owns every other stage)
         const std::vector<int> ins = dw ? std::vector<int>{6, 4, 2} : std::vector<int>{0};
@@ -752,28 +784,68 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
             if (bi == 1 && bopts[1] == bopts[0]) break;
             const int bs = bopts[bi];
             for (int in_st : ins)
-                for (int a_st : {4, dw ? 2 : 3}) cands.push_back({in_st, bs, a_st});
+                for (int a_st : {4, dw ? 2 : 3}) cands.push_back({1, in_st, bs, a_st, false});
         }
     }
-    uint32_t smem_bytes = 0;
+    bool found = false;
     for (const Cand& c : cands) {
-        const uint32_t total = (uint32_t)c.in_stages * p.in_stage_stride + (uint32_t)c.a_stages * kAStage + (uint32_t)c.b_stages * b_stage + tables;
+        const uint32_t tab = c.dw_global ? 0u : tables;
+        const uint32_t total = (uint32_t)c.in_stages * p.in_stage_stride + (uint32_t)c.a_stages * kAStage + (uint32_t)c.b_stages * b_stage + tab;
         if (total > budget) continue;
+        p.n_group = c.n_group;
         p.in_stages = c.in_stages; p.a_stages = c.a_stages; p.b_stages = c.b_stages;
         p.off_in = 0;
         p.off_a = (uint32_t)c.in_stages * p.in_stage_stride;
         p.off_b = p.off_a + (uint32_t)c.a_stages * kAStage;
-        p.off_dw = dw ? p.off_b + (uint32_t)c.b_stages * b_stage : 0xFFFFFFFFu;
-        p.off_stem = p.off_dw + 40u * cin;
+        p.off_dw = (dw && !c.dw_global) ? p.off_b + (uint32_t)c.b_stages * b_stage : 0xFFFFFFFFu;
+        p.off_stem = p.off_b + (uint32_t)c.b_stages * b_stage + 40u * cin;
         smem_bytes = total + 1024;
         found = true;
         break;
     }
     if (!found) return "shared memory budget exceeded";
-    if (p.in_stages > 8 || p.a_stages > 4 || p.b_stages > 8) return "internal: ring too deep for the barrier table";
-    int dev = 0, sms = 132;
+    if (d.rgb && (p.n_group != p.num_n_tiles || cout > kMaxRgbC))
+        return "fused torgb needs all output channels of a pixel tile in one CTA tile (cout <= 256 with a resident A operand)";
+    if (p.in_stages > 8 || p.a_stages > kMaxAStages || p.b_stages > 8) return "internal: ring too deep for the barrier table";
+    p.l_nt = ilog2(p.num_n_tiles / p.n_group);
+    p.num_tiles = m_tiles * (p.num_n_tiles / p.n_group);
+    return nullptr;
+}
+
+}  // namespace
+
+bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d) {
+    SepconvTcRgb rgb{};
+    SepconvTcDesc q = d;
+    q.rgb = &rgb;
+    Params p;
+    memset(&p, 0, sizeof(p));
+    uint32_t smem_bytes = 0;
+    return plan_layout(p, q, grid_sms(), smem_bytes) == nullptr;
+}
+
+const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
+    Params p;
+    memset(&p, 0, sizeof(p));
+    const int n = d.n, res = d.res, cin = d.cin, cout = d.cout;
+    const bool dw = (d.source != SEPCONV_SRC_SPLIT);
+    if (d.source == SEPCONV_SRC_SPLIT && !(d.a_hi && d.a_lo)) return "no A operand";
+    if ((d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) && !d.in_f32) return "no input tensor";
+    if (d.source == SEPCONV_SRC_UP && !d.up_t) return "no low-resolution tensor for the up-sampling prologue";
+    if (d.source == SEPCONV_SRC_STEM && !(d.stem_w && d.stem_b)) return "no fromrgb weights for the stem prologue";
+    const int sms = grid_sms();
+    uint32_t smem_bytes = 0;
+    if (const char* err = plan_layout(p, d, sms, smem_bytes)) return err;
+    p.w9 = d.w9; p.bias = d.bias; p.noise = d.noise; p.inv_scale = d.inv_scale; p.out = d.out;
+    if (d.source == SEPCONV_SRC_UP) memcpy(p.up_taps.f, d.up_taps, sizeof(p.up_taps.f));
+    if (d.source == SEPCONV_SRC_STEM) { p.stem_w = d.stem_w; p.stem_b = d.stem_b; }
+    p.store_out = 1;
+    if (d.rgb) {
+        p.torgb = 1; p.store_out = d.rgb->store_out;
+        p.rgb_w = d.rgb->w; p.rgb_b = d.rgb->b; p.rgb_fir = d.rgb->fir; p.img_lo = d.rgb->img_lo; p.img_out = d.rgb->img_out;
+    }
+    int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     p.error_flag = (dev >= 0 && dev < kMaxDevices) ? g_error_flag[dev] : nullptr;
     p.prefetch = dw ? 4 : 2;
 
@@ -814,9 +886,8 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
         if ((err = encode_map(&p.map_w_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.w_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
     }
     if (!d.out && p.store_out) return "no output tensor";
-    // Persistent grid = one CTA per SM.  MIGAN_TC_RESERVE_SMS leaves SMs free for a concurrently running collective.
-    const int reserve = std::max(0, std::min(env_int("MIGAN_TC_RESERVE_SMS", 0), sms / 2));
-    args->grid = (unsigned)std::min(p.num_tiles, sms - reserve);
+    // Persistent grid = one CTA per usable SM.
+    args->grid = (unsigned)std::min(p.num_tiles, sms);
     args->smem_bytes = smem_bytes;
     args->num_tiles = p.num_tiles;
     args->bound_x = nullptr;

@@ -62,6 +62,9 @@ struct SepconvTcDesc {
 
 // Returns nullptr on success, else an error string.
 const char* sepconv_tc_plan_ex(SepconvTcArgs* a, const SepconvTcDesc& d);
+// Whether a launch with d's shapes and source can fuse torgb, i.e. hold all of cout in one CTA tile (d.rgb and the
+// pointers are not read).
+bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d);
 // Legacy form (plain / pre-split sources).
 const char* sepconv_tc_plan(SepconvTcArgs* a, int passes, const float* in_f32, const __half* a_hi, const __half* a_lo,
                             const float* w9, const float* bias, const __half* w_hi, const __half* w_lo,
