@@ -165,6 +165,24 @@ int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs_host, int n, i
 int b200_pipeline_postprocess_batch(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
                                     const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The same batch with the crop windows planned on the DEVICE, so a whole pass is enqueued without a host round trip:
+ *   b200_hole_flags_batch -> b200_pipeline_plan_batch -> b200_pipeline_preprocess_planned -> [generator]
+ *   -> b200_pipeline_postprocess_planned
+ * The boxes in reqs_host are not read.  Every call of a pass gets the same reqs_host (the same n, images, masks and sizes),
+ * resolution and scratch; resolution must be at least 3.  Request i's boxes, x[i] and image[crop] equal the host-box
+ * batched calls' on the windows migan_crop_box gives, bit for bit.
+ *   b200_pipeline_batch_scratch_bound  scratch for every crop window the images allow, from the image sizes alone (0 on a
+ *                                      bad argument); the phases' descriptors live there from the plan to the post-processing
+ *   b200_pipeline_plan_batch           one launch: boxes_dev int32 [n][4] (DEVICE; x_min, x_max, y_min, y_max per request)
+ *                                      and the descriptors of both phases, from the flags of b200_hole_flags_batch */
+size_t b200_pipeline_batch_scratch_bound(const migan_pipe_request* reqs_host, int n, int resolution);
+int b200_pipeline_plan_batch(const migan_pipe_request* reqs_host, int n, int resolution, int padding, const uint8_t* flags,
+                             int* boxes_dev, void* scratch, size_t scratch_bytes, void* stream);
+int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs_host, int n, int resolution, float* x_n4rr,
+                                     void* scratch, size_t scratch_bytes, void* stream);
+int b200_pipeline_postprocess_planned(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
+                                      const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
+
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0
  * (k = 1).  w_dev: HOST array of k DEVICE pointers to [cout][fan] fp32 tensors (fan = cin/groups * kh * kw); out: device.

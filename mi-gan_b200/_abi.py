@@ -53,6 +53,10 @@ SYMBOLS = [
     ("b200_pipeline_batch_scratch_bytes", c_size_t, [POINTER(PipeRequest), c_int, c_int]),
     ("b200_pipeline_preprocess_batch", c_int, [POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_postprocess_batch", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_batch_scratch_bound", c_size_t, [POINTER(PipeRequest), c_int, c_int]),
+    ("b200_pipeline_plan_batch", c_int, [POINTER(PipeRequest), c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_preprocess_planned", c_int, [POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_postprocess_planned", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

@@ -90,6 +90,14 @@ int launch_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flag
 int launch_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
 int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
                                       void* scratch, cudaStream_t s);
+// the same batches with the crop windows planned on the device from the flags (no host round trip)
+int check_pipe_planned(const migan_pipe_request* reqs, int n, int res, char* msg, size_t len);
+size_t pipeline_batch_scratch_bound(const migan_pipe_request* reqs, int n, int res);
+int launch_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int padding, const uint8_t* flags, int* boxes,
+                               void* scratch, cudaStream_t s);
+int launch_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
+int launch_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
+                                        void* scratch, cudaStream_t s);
 
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------

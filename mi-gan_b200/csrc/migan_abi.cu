@@ -1382,6 +1382,48 @@ int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* re
     return MIGAN_OK;
 }
 
+static int check_pipe_planned(const char* who, const migan_pipe_request* reqs, int n, int res) {
+    char msg[256];
+    if (int rc = migan::check_pipe_planned(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+size_t b200_pipeline_batch_scratch_bound(const migan_pipe_request* reqs, int n, int res) {
+    if (check_pipe_planned("pipeline_batch_scratch_bound", reqs, n, res)) return 0;
+    return migan::pipeline_batch_scratch_bound(reqs, n, res);
+}
+
+int b200_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int padding, const uint8_t* flags, int* boxes,
+                             void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = check_pipe_planned("pipeline_plan_batch", reqs, n, res)) return rc;
+    if (padding < 0) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: padding %d", padding);
+    if (!flags || !boxes || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_plan_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_pipeline_plan_batch(reqs, n, res, padding, flags, boxes, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
+                                     void* stream) {
+    if (int rc = check_pipe_planned("pipeline_preprocess_planned", reqs, n, res)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_planned: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_pipeline_preprocess_planned(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
+                                      size_t scratch_bytes, void* stream) {
+    if (int rc = check_pipe_planned("pipeline_postprocess_planned", reqs, n, res)) return rc;
+    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_planned: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess_planned(y, reqs, n, res, k25, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
 int migan_host_wait(migan_ctx* ctx) {
     if (!ctx) return fail(MIGAN_ERR_INVALID, "null ctx");
     if (!ctx->s_out) return MIGAN_OK;

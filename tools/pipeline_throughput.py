@@ -1,10 +1,17 @@
-"""Requests/s of `MIGAN_Pipeline` on cuda:0 for a seeded traffic mix of 32 requests (photos of 512x512, 720x1280, 1080x1920
-and 2160x3840 with rectangular holes; resolution 512, padding 128): one `pipe(image_i, mask_i)` per request (sequential)
-against one `forward_batch` of all of them (batched).  Both are warmed up, then timed alternately over the repeats, each
-repeat ending in a device synchronise; p50 and range are reported.  The two forms must give identical images.
-Records the card name and power limit of the same run.  Measurement tooling (seeded random weights, no oracle).
+"""Requests/s of `MIGAN_Pipeline` on cuda:0 for a seeded traffic mix (photos of 512x512, 720x1280, 1080x1920 and 2160x3840
+with rectangular holes; resolution 512, padding 128), in two forms:
 
-    python tools/pipeline_throughput.py [--repeats 10] [--res 512]
+* device-resident, 32 requests: one `pipe(image_i, mask_i)` per request (sequential) against one `forward_batch` of all of
+  them (batched);
+* host-resident, `--host-passes` passes of 32 requests whose images and masks are pinned CPU tensors (how decoded photos
+  arrive): `forward_batch` pass by pass, each call waiting for its results (host sync), against `forward_batch(...,
+  wait=False)` for every pass followed by one `wait()` (host async).
+
+Each pair is warmed up, then timed alternately over the repeats, each repeat ending when every result is in place; p50 and
+range are reported.  The two forms of a pair must give identical images.  Records the card name and power limit of the same
+run.  Measurement tooling (seeded random weights, no oracle).
+
+    python tools/pipeline_throughput.py [--repeats 10] [--res 512] [--host-passes 4]
 """
 import argparse
 import json
@@ -39,6 +46,52 @@ def traffic(n, dev, seed=0):
     return reqs
 
 
+def rates(ts, requests):
+    rate = [requests / t for t in ts]
+    return {"requests_per_s_p50": statistics.median(rate), "requests_per_s_min": min(rate), "requests_per_s_max": max(rate),
+            "ms_p50": statistics.median(ts) * 1e3}
+
+
+def host_resident(pipe, passes, repeats, dev):
+    """Pinned CPU requests in passes of 32: synchronous calls pass by pass against wait=False calls and one wait()."""
+    src = [(im.cpu(), m.cpu()) for im, m in traffic(32 * passes, dev, seed=1)]
+    images = [im.pin_memory() for im, _ in src]
+    masks = [m.pin_memory() for _, m in src]
+
+    def restore():                                                  # host copies, outside the timed window
+        for im, (s, _) in zip(images, src):
+            im.copy_(s)
+
+    def sync():
+        for c in range(0, len(images), 32):
+            pipe.forward_batch(images[c:c + 32], masks[c:c + 32])
+
+    def asynchronous():
+        for c in range(0, len(images), 32):
+            pipe.forward_batch(images[c:c + 32], masks[c:c + 32], wait=False)
+        pipe.wait()
+
+    restore(); sync()
+    a = [im.clone() for im in images]
+    restore(); asynchronous()
+    identical = all(torch.equal(x, y) for x, y in zip(a, images))
+    del a
+    times = {"host_sync": [], "host_async": []}
+    for _ in range(repeats):
+        for name, f in (("host_sync", sync), ("host_async", asynchronous)):
+            restore()
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            f()
+            torch.cuda.synchronize()
+            times[name].append(time.perf_counter() - t0)
+    out = {"requests": len(images), "passes": passes, "outputs_identical": identical}
+    for name, ts in times.items():
+        out[name] = rates(ts, len(images))
+    out["speedup_p50"] = out["host_async"]["requests_per_s_p50"] / out["host_sync"]["requests_per_s_p50"]
+    return out
+
+
 def card():
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -53,6 +106,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=10)
     ap.add_argument("--res", type=int, default=512)
     ap.add_argument("--requests", type=int, default=32)
+    ap.add_argument("--host-passes", type=int, default=4, help="passes of 32 pinned CPU requests (0: skip the host-resident form)")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     pipe = MIGAN_Pipeline(synthetic.export_style_state_dict(args.res, seed=1), args.res, padding=128, device=dev)
@@ -89,16 +143,17 @@ def main():
     out = {"card": card(), "resolution": args.res, "padding": 128, "requests": args.requests, "repeats": args.repeats,
            "sizes": [list(im.shape[2:]) for im, _ in reqs], "outputs_identical": identical}
     for name, ts in times.items():
-        rate = [args.requests / t for t in ts]
-        out[name] = {"requests_per_s_p50": statistics.median(rate), "requests_per_s_min": min(rate),
-                     "requests_per_s_max": max(rate), "ms_p50": statistics.median(ts) * 1e3}
+        out[name] = rates(ts, args.requests)
     out["speedup_p50"] = out["batched"]["requests_per_s_p50"] / out["sequential"]["requests_per_s_p50"]
+    if args.host_passes > 0:
+        out["host_resident"] = host_resident(pipe, args.host_passes, args.repeats, dev)
+        identical = identical and out["host_resident"]["outputs_identical"]
     print(json.dumps(out, indent=1), flush=True)
     os.makedirs("tools/out", exist_ok=True)
     with open("tools/out/pipeline_throughput_%d.json" % args.res, "w") as f:
         json.dump(out, f, indent=1)
     if not identical:
-        sys.exit("sequential and batched outputs differ")
+        sys.exit("the two forms of a pair gave different outputs")
 
 
 if __name__ == "__main__":
