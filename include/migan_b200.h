@@ -183,6 +183,35 @@ int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs_host, int n,
 int b200_pipeline_postprocess_planned(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
                                       const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The reference demo's request path at any photo size (scripts/demo.py:26-66, :120-143), for a batch of
+ * 1..MIGAN_PIPE_MAX_BATCH requests, one launch per stage:
+ *   photo  -> PIL BICUBIC down-scale to at most R (only when W > R or H > R): img_resized, out_w x out_h
+ *   mask   -> PIL NEAREST to at most 512 -> channel (alpha of LA / RGBA, R of RGB, L) -> 255 - v if invert -> v < 255 -> 0
+ *             -> PIL NEAREST to at most R: mask_resized, which must come out at out_w x out_h
+ *   b200_demo_preprocess   img_resized -> PIL BICUBIC R x R, mask_resized -> NEAREST R x R -> x[i] of x [n,4,R,R]
+ *   [generator]
+ *   b200_demo_postprocess  y[i] -> (y*0.5+0.5).clamp(0,1)*255 -> uint8 -> cv2.resize INTER_CUBIC to out_w x out_h ->
+ *                          img_resized where mask_resized is 255, else the resized result -> out
+ * Every resize reproduces its library's uint8 arithmetic bit for bit (OpenCV: the scalar path, cv2.setUseOptimized(False)).
+ * The sizes follow demo.py's `resize`: (int(w * r), int(h * r)) with r = max_size / w if w > h else max_size / h;
+ * migan_demo_resized_size computes them.  reqs_host is a HOST array; both calls of a pass get the same reqs_host,
+ * resolution and scratch (b200_demo_scratch_bytes bytes of device memory; 0 on a bad argument). */
+typedef struct {
+    const uint8_t* img;    /* DEVICE u8 [H][W][3] */
+    int H, W;
+    const uint8_t* mask;   /* DEVICE u8 [Hm][Wm][mask_channels]: 1 (L), 2 (LA), 3 (RGB) or 4 (RGBA) */
+    int Hm, Wm, mask_channels;
+    int invert;            /* non-zero: 255 - v before the threshold */
+    uint8_t* out;          /* DEVICE u8 [out_h][out_w][3], written by b200_demo_postprocess */
+    int out_w, out_h;      /* the size of img_resized: migan_demo_resized_size(W, H, resolution) */
+} migan_demo_request;
+int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h);
+size_t b200_demo_scratch_bytes(const migan_demo_request* reqs_host, int n, int resolution);
+int b200_demo_preprocess(const migan_demo_request* reqs_host, int n, int resolution, float* x_n4rr, void* scratch,
+                         size_t scratch_bytes, void* stream);
+int b200_demo_postprocess(const float* y_n3rr, const migan_demo_request* reqs_host, int n, int resolution, void* scratch,
+                          size_t scratch_bytes, void* stream);
+
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0
  * (k = 1).  w_dev: HOST array of k DEVICE pointers to [cout][fan] fp32 tensors (fan = cin/groups * kh * kw); out: device.

@@ -19,6 +19,12 @@ class PipeRequest(ctypes.Structure):
     _fields_ = [("image", c_void_p), ("mask", c_void_p), ("H", c_int), ("W", c_int), ("box", c_int * 4)]
 
 
+class DemoRequest(ctypes.Structure):
+    """migan_demo_request: one request of the demo request path (b200_demo_*)."""
+    _fields_ = [("img", c_void_p), ("H", c_int), ("W", c_int), ("mask", c_void_p), ("Hm", c_int), ("Wm", c_int),
+                ("mask_channels", c_int), ("invert", c_int), ("out", c_void_p), ("out_w", c_int), ("out_h", c_int)]
+
+
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("migan_last_error", c_char_p, []),
@@ -57,6 +63,10 @@ SYMBOLS = [
     ("b200_pipeline_plan_batch", c_int, [POINTER(PipeRequest), c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_preprocess_planned", c_int, [POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_postprocess_planned", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("migan_demo_resized_size", c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]),
+    ("b200_demo_scratch_bytes", c_size_t, [POINTER(DemoRequest), c_int, c_int]),
+    ("b200_demo_preprocess", c_int, [POINTER(DemoRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_demo_postprocess", c_int, [c_void_p, POINTER(DemoRequest), c_int, c_int, c_void_p, c_size_t, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

@@ -99,6 +99,13 @@ int launch_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, in
 int launch_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
                                         void* scratch, cudaStream_t s);
 
+// ---- the reference demo's request path at any photo size (demo_resize.cu): scripts/demo.py:26-66, :120-143 ------
+int demo_resized_size(int w, int h, int max_size, int* ow, int* oh);
+int check_demo_batch(const migan_demo_request* reqs, int n, int res, char* msg, size_t len);
+size_t demo_scratch_bytes(const migan_demo_request* reqs, int n, int res);
+int launch_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
+int launch_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, cudaStream_t s);
+
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------
 int launch_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fan, float* out, cudaStream_t s);

@@ -1424,6 +1424,42 @@ int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* 
     return MIGAN_OK;
 }
 
+int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h) {
+    if (!out_w || !out_h) return fail(MIGAN_ERR_INVALID, "demo_resized_size: null argument");
+    if (w < 1 || h < 1 || max_size < 1) return fail(MIGAN_ERR_INVALID, "demo_resized_size: bad arguments (%d x %d, max size %d)", w, h, max_size);
+    return migan::demo_resized_size(w, h, max_size, out_w, out_h);
+}
+
+static int check_demo_batch(const char* who, const migan_demo_request* reqs, int n, int res) {
+    char msg[256];
+    if (int rc = migan::check_demo_batch(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+size_t b200_demo_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
+    if (check_demo_batch("demo_scratch_bytes", reqs, n, res)) return 0;
+    return migan::demo_scratch_bytes(reqs, n, res);
+}
+
+int b200_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = check_demo_batch("demo_preprocess", reqs, n, res)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "demo_preprocess: null argument");
+    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_demo_preprocess(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, size_t scratch_bytes,
+                          void* stream) {
+    if (int rc = check_demo_batch("demo_postprocess", reqs, n, res)) return rc;
+    if (!y || !scratch) return fail(MIGAN_ERR_INVALID, "demo_postprocess: null argument");
+    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_demo_postprocess(y, reqs, n, res, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
 int migan_host_wait(migan_ctx* ctx) {
     if (!ctx) return fail(MIGAN_ERR_INVALID, "null ctx");
     if (!ctx->s_out) return MIGAN_OK;
