@@ -72,6 +72,18 @@ size_t migan_workspace_bytes(const migan_ctx* ctx, int n);
 int migan_forward(migan_ctx* ctx, const float* x, float* y, int n,
                   void* workspace, size_t workspace_bytes, int path, void* stream);
 
+/* Fully convolutional forward: y[n,3,H,W] from x[n,4,H,W] for H, W >= R that are multiples of R/4 (need not be equal or
+ * powers of two), with n*H*W*ch(R) < 2^31 (ch(R) = min(32768/R, 512): the largest activation).  Nominal level r keeps its
+ * weights and channels and runs at the extent (H r/R, W r/R); each noise plane is its noise_const tiled,
+ * noise[i][j] = noise_const[i mod r][j mod r] * noise_strength, and every up-sampling is zero insertion at its output extent.
+ * At H = W = R this is migan_forward, byte for byte.
+ * migan_workspace_bytes_hw returns 0 for a refused shape (the reason, with the nearest valid sizes, in migan_last_error());
+ * migan_workspace_bytes(ctx, n) == migan_workspace_bytes_hw(ctx, n, R, R) for every n the latter accepts.
+ * migan_forward_hw has migan_forward's contract and returns MIGAN_ERR_INVALID for a refused shape. */
+size_t migan_workspace_bytes_hw(const migan_ctx* ctx, int n, int H, int W);
+int migan_forward_hw(migan_ctx* ctx, const float* x, float* y, int n, int H, int W,
+                     void* workspace, size_t workspace_bytes, int path, void* stream);
+
 /* Latency form for small batches (the reference's primary caller runs batch 1: scripts/demo.py:125-142): the launch
  * sequence of one forward is captured ONCE into a CUDA graph that works on fixed staging buffers at the end of the
  * workspace, and replayed per call between two device-to-device copies (x in, y out) -- 3 submissions instead of ~50.
@@ -111,6 +123,10 @@ int migan_forward_u8_async(migan_ctx* ctx, const uint8_t* img_host, const uint8_
 int b200_preprocess_u8(const uint8_t* img_hwc, const uint8_t* mask_hw, float* x_nchw, int n, int r, void* stream);
 int b200_postprocess_u8(const float* y_nchw, const uint8_t* img_hwc, const uint8_t* mask_hw, uint8_t* out_hwc, int n, int r,
                         void* stream);
+/* The same at any H x W: img [n,H,W,3], mask [n,H,W] -> x [n,4,H,W]; y [n,3,H,W] -> out [n,H,W,3]. */
+int b200_preprocess_u8_hw(const uint8_t* img_hwc, const uint8_t* mask_hw, float* x_nchw, int n, int H, int W, void* stream);
+int b200_postprocess_u8_hw(const float* y_nchw, const uint8_t* img_hwc, const uint8_t* mask_hw, uint8_t* out_hwc, int n, int H,
+                           int W, void* stream);
 
 /* Feathered composite of the deployed (ONNX) pipeline, scripts/create_onnx_pipeline.py:233-245, for a crop at the model
  * resolution (DEVICE pointers, NCHW like the pipeline): blend weight = 5x5 smoothing (reflect border) of the 3x3 max-pooled

@@ -37,6 +37,8 @@ SYMBOLS = [
     ("migan_finalize_weights", c_int, [c_void_p]),
     ("migan_workspace_bytes", c_size_t, [c_void_p, c_int]),
     ("migan_forward", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_int, c_void_p]),
+    ("migan_workspace_bytes_hw", c_size_t, [c_void_p, c_int, c_int, c_int]),
+    ("migan_forward_hw", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_int, c_void_p]),
     ("migan_graph_staging_bytes", c_size_t, [c_void_p, c_int]),
     ("migan_forward_graph", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_int, c_void_p]),
     ("migan_host_staging_bytes", c_size_t, [c_void_p, c_int]),
@@ -48,6 +50,8 @@ SYMBOLS = [
     ("migan_forward_u8_async", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_int, c_void_p]),
     ("b200_preprocess_u8", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     ("b200_postprocess_u8", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    ("b200_preprocess_u8_hw", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    ("b200_postprocess_u8_hw", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     ("b200_feather_composite", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("b200_pipeline_scratch_bytes", c_size_t, [c_int, c_int, c_int]),
     ("b200_resize_nearest_u8", c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
@@ -105,7 +109,8 @@ COMOD_SYMBOLS = [
      [c_void_p, c_size_t, POINTER(c_size_t), POINTER(c_int), POINTER(c_int), c_void_p]),
 ]
 
-PREPOST_SYMBOLS = [s for s in SYMBOLS if s[0] in ("b200_preprocess_u8", "b200_postprocess_u8", "b200_feather_composite")]
+PREPOST_SYMBOLS = [s for s in SYMBOLS if s[0] in ("b200_preprocess_u8", "b200_postprocess_u8", "b200_feather_composite",
+                                                   "b200_preprocess_u8_hw", "b200_postprocess_u8_hw")]
 
 _lib = None
 

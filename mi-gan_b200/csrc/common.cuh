@@ -31,6 +31,20 @@ __device__ __forceinline__ float4 lrelu_agc4(float4 v) {
     return v;
 }
 
+// n / d for 0 <= n < 2^31 by a divisor fixed per launch: one multiply-high, an add and a shift (the round-up method:
+// m = floor(2^32 (2^s - d) / d) + 1 with 2^s >= d; a power of two gives m = 1, i.e. a plain shift).  Lets the streaming
+// kernels index extents that are not powers of two without a 32-bit division per element.
+struct FastDiv {
+    uint32_t d = 1, m = 1, s = 0;
+    FastDiv() = default;
+    explicit FastDiv(uint32_t d_) : d(d_), m(1), s(0) {
+        while ((1ull << s) < d) ++s;
+        m = (uint32_t)((((1ull << 32) * ((1ull << s) - d)) / d) + 1);
+    }
+    __device__ __forceinline__ uint32_t div(uint32_t n) const { return (__umulhi(n, m) + n) >> s; }
+    __device__ __forceinline__ uint32_t mod(uint32_t n) const { return n - div(n) * d; }
+};
+
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void stg4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 

@@ -107,7 +107,7 @@ int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t st) { return (int
 int dev_sync() { return (int)cudaDeviceSynchronize(); }
 const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
 int gemm_f32(const float* A, const float* Bt, float* out, int64_t P, int K, int N, ck_stream_t s) {
-    return (int)migan::launch_pw_gemm_simt(A, Bt, out, P, K, N, nullptr, 1, 0, s);
+    return (int)migan::launch_pw_gemm_simt(A, Bt, out, P, K, N, nullptr, 1, 1, 1, 0, s);
 }
 // The wgmma kernel of the MI-GAN path in its plain-GEMM configuration (pre-split A operand by TMA, no activation):
 // out[n][res][res][N] = inv_scale * A[P][K] * B[N][K]^T with the fp16 hi/lo 3-pass split, fp32 accumulation in registers.

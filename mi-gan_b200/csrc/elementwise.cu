@@ -23,26 +23,26 @@ static inline unsigned blocks_for(int64_t items, int threads) {
 // --------------------------------------------------------------------------------------
 // stem: x NCHW [n,4,H,W] -> NHWC [n,H,W,C0]
 // --------------------------------------------------------------------------------------
-// All spatial sizes and channel counts are powers of two: index math is 32-bit shifts/masks
-// (64-bit div/mod costs ~100 instructions per thread and dominated these kernels otherwise).
-__device__ __forceinline__ int ilog2(int v) { return 31 - __clz(v); }
+// Channel counts are powers of two (shifts / masks); spatial extents need not be (a fully convolutional forward), so
+// pixel indices are split with FastDiv (common.cuh): 64-bit div/mod costs ~100 instructions per thread and dominated these
+// kernels otherwise.
 
 // Thread = (4 output channels, 4 adjacent pixels): the 4x4 weights + bias stay in registers, x is read as one
 // 128-bit load per input plane, and the thread writes four 128-bit vectors (each warp instruction covers whole
 // 256-byte pixel rows).  Re-loading the weights per output vector would saturate the L1 instead of HBM.
 __global__ void __launch_bounds__(256)
 stem_fromrgb_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
-                    float* __restrict__ out, uint32_t items, int lhw, int lcv) {
+                    float* __restrict__ out, uint32_t items, FastDiv hw, int lcv) {
     pdl_trigger();
     pdl_wait();
     const uint32_t idx = blockIdx.x * 256u + threadIdx.x;     // over (pixel quads) x (channel quads)
     if (idx >= items) return;
     const uint32_t c4 = idx & ((1u << lcv) - 1);
-    const uint32_t pq = idx >> lcv;                           // pixel-quad index over the image group
+    const uint32_t pq = idx >> lcv;                           // pixel-quad index over the image group (H * W % 4 == 0)
     const uint32_t p = pq << 2;
-    const uint32_t q = p & ((1u << lhw) - 1);
-    const uint32_t img = p >> lhw;
-    const size_t HW = (size_t)1 << lhw;
+    const uint32_t img = hw.div(p);
+    const uint32_t q = p - img * hw.d;
+    const size_t HW = hw.d;
     const float* xp = x + (size_t)img * 4 * HW + q;
     const float4 x0 = ldg4(xp), x1 = ldg4(xp + HW), x2 = ldg4(xp + 2 * HW), x3 = ldg4(xp + 3 * HW);
     float4 wc[4];
@@ -83,11 +83,12 @@ static inline int host_log2(int v) { int l = 0; while ((1 << l) < v) ++l; return
 
 cudaError_t launch_stem(const float* x, const float* w, const float* b, float* out,
                         int n, int H, int W, int C0, cudaStream_t s) {
+    if ((H * W) % 4 != 0) return cudaErrorInvalidValue;
     const size_t per_img = (size_t)H * W / 4 * (C0 / 4);
     return for_image_groups(n, per_img, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         launch_pdl(stem_fromrgb_kernel, dim3((items + 255) / 256), dim3(256), 0, s, x + (size_t)i0 * 4 * H * W, w, b, out + (size_t)i0 * H * W * C0,
-                   items, host_log2(H * W), host_log2(C0 / 4));
+                   items, FastDiv((uint32_t)(H * W)), host_log2(C0 / 4));
     });
 }
 
@@ -125,36 +126,36 @@ __device__ __forceinline__ u64 lrelu_agc2(u64 v) {
 
 // Thread = (channel PAIR, PAIR of adjacent columns x0 = 2*xp, x0 + 1, strip of RS rows): the 9 taps + bias stay in
 // registers, a 3-row x 4-column window slides down the strip (4 L1-served 64-bit loads per row feed 2 outputs),
-// all MACs are FFMAs on channel pairs, and the next row is fetched one iteration ahead.
+// all MACs are FFMAs on channel pairs, and the next row is fetched one iteration ahead.  An odd W leaves the last pair
+// with one column, a height that is not a multiple of RS the last strip with fewer rows: those outputs are not stored.
 template <int RS>
 __global__ void __launch_bounds__(256)
 dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, const float* __restrict__ bias,
                  float* __restrict__ out, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                 uint32_t items, int lw, int lh, int lcp, int lstrips) {
+                 uint32_t items, int H, int W, int lcp, FastDiv pairs, FastDiv strips) {
     pdl_trigger();
     pdl_wait();
     const uint32_t idx = blockIdx.x * 256u + threadIdx.x;
     if (idx >= items) return;
-    const int W = 1 << lw, H = 1 << lh, C = 2 << lcp;
+    const int C = 2 << lcp;
     const int c = (int)(idx & ((1u << lcp) - 1)) * 2;
-    uint32_t t = idx >> lcp;
-    const int x0 = (int)(t & ((W >> 1) - 1)) * 2;
-    t >>= (lw - 1);
-    const int strip = (int)(t & ((1u << lstrips) - 1));
-    const size_t img = t >> lstrips;
+    const uint32_t t = idx >> lcp, t2 = pairs.div(t), t3 = strips.div(t2);
+    const int x0 = (int)(t - t2 * pairs.d) * 2;
+    const int strip = (int)(t2 - t3 * strips.d);
+    const size_t img = t3;
     const int y0 = strip * RS;
     u64 w[9];
 #pragma unroll
     for (int k = 0; k < 9; ++k) w[k] = ldg2(w9 + k * C + c);
     const u64 bv = ldg2(bias + c);
     const float* base = in + img * (size_t)H * W * C + c;
-    const bool okl = x0 > 0, okr = x0 + 2 < W;
+    const bool okl = x0 > 0, okm = x0 + 1 < W, okr = x0 + 2 < W;
     auto load_row = [&](int y, u64 (&r)[4]) {
         if (y < 0 || y >= H) { r[0] = r[1] = r[2] = r[3] = 0ull; return; }
         const float* p = base + ((size_t)y * W + x0) * C;
         r[0] = okl ? ldg2(p - C) : 0ull;
         r[1] = ldg2(p);
-        r[2] = ldg2(p + C);
+        r[2] = okm ? ldg2(p + C) : 0ull;
         r[3] = okr ? ldg2(p + 2 * C) : 0ull;
     };
     u64 r0[4], r1[4], r2[4], rn[4];
@@ -175,6 +176,7 @@ dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, con
                 acc = ffma2(w[6 + d], r2[e + d], acc);
             }
             const float2 v = unpk2(lrelu_agc2(acc));
+            if (y >= H || x0 + e >= W) continue;
             const size_t o = ((img * H + y) * (size_t)W + x0 + e) * C + c;
             if (out) *reinterpret_cast<float2*>(out + o) = v;
             if (out_hi) {   // pre-split A operand for the wgmma GEMM (layers whose Cout spans several CTA N tiles)
@@ -192,14 +194,14 @@ dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, con
 
 cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, float* out, __half* out_hi, __half* out_lo,
                          int n, int H, int W, int C, cudaStream_t s) {
-    const int rs = (H >= 8) ? 8 : 4, strips = H / rs;
-    const size_t per_img = (size_t)strips * (W / 2) * (C / 2);
+    const int rs = (H >= 8) ? 8 : 4, strips = (H + rs - 1) / rs, pairs = (W + 1) / 2;
+    const size_t per_img = (size_t)strips * pairs * (C / 2);
     return for_image_groups(n, per_img, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t off = (size_t)i0 * H * W * C;
         auto kern = (rs == 8) ? dw3x3_act_kernel<8> : dw3x3_act_kernel<4>;
         launch_pdl(kern, dim3((items + 255) / 256), dim3(256), 0, s, in + off, w9, bias, out ? out + off : nullptr, out_hi ? out_hi + off : nullptr,
-                   out_lo ? out_lo + off : nullptr, items, host_log2(W), host_log2(H), host_log2(C / 2), host_log2(strips));
+                   out_lo ? out_lo + off : nullptr, items, H, W, host_log2(C / 2), FastDiv((uint32_t)pairs), FastDiv((uint32_t)strips));
     });
 }
 
@@ -221,19 +223,20 @@ cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, fl
 //              depthwise columns feed both outputs, so every activated depthwise value is computed exactly once
 //              horizontally (the one-column version evaluated each column in two threads)
 //   w[9], bias per-channel-pair constants; FIR taps from a shared-memory table; 8 column pointers advanced per row
+// The 8-row walk needs ~170 registers: it gets the whole budget (one block per SM) instead of spilling at two.
 template <int RS>
-__global__ void __launch_bounds__(256, 2)
+__global__ void __launch_bounds__(256, RS == 8 ? 1 : 2)
 dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, const float* __restrict__ bias,
                   const float* __restrict__ fir16, float* __restrict__ out_f32,
-                  __half* __restrict__ out_hi, __half* __restrict__ out_lo, uint32_t items, int lw2, int lh2, int lcp, int lstrips) {
+                  __half* __restrict__ out_hi, __half* __restrict__ out_lo, uint32_t items, int H2, int W2, int lcp,
+                  FastDiv pairs, FastDiv strips) {
     const uint32_t idx = blockIdx.x * 256u + threadIdx.x;
-    const int W2 = 1 << lw2, H2 = 1 << lh2, W = 2 * W2, H = 2 * H2, C = 2 << lcp;
+    const int W = 2 * W2, H = 2 * H2, C = 2 << lcp;
     const int c = (int)(idx & ((1u << lcp) - 1)) * 2;
-    uint32_t t = idx >> lcp;
-    const int ox0 = (int)(t & ((W2 >> 1) - 1)) * 2;
-    t >>= (lw2 - 1);
-    const int strip = (int)(t & ((1u << lstrips) - 1));
-    const size_t img = t >> lstrips;
+    const uint32_t t = idx >> lcp, t2 = pairs.div(t), t3 = strips.div(t2);
+    const int ox0 = (int)(t - t2 * pairs.d) * 2;
+    const int strip = (int)(t2 - t3 * strips.d);
+    const size_t img = t3;
     const int oy0 = strip * RS;
 
     // FIR taps live in shared memory ([16][C], conflict-free 64-bit reads along the channel pairs)
@@ -249,6 +252,8 @@ dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, co
     const u64 bv = ldg2(bias + c);
 
     const int iy_first = 2 * oy0 - 2;
+    const int rows_out = H2 - oy0;                        // output rows of the strip inside the image (< RS: last strip)
+    const bool col1_ok = ox0 + 1 < W2;                    // false: odd W2, the pair's second column is outside
     const float* colp[8];
     bool colok[8];
 #pragma unroll
@@ -321,6 +326,7 @@ dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, co
                 const int orow = oy0 + ((q - 3) >> 1);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
+                    if (((q - 3) >> 1) >= rows_out || (e == 1 && !col1_ok)) continue;   // outside the output
                     const size_t o = ((img * H2 + orow) * W2 + ox0 + e) * (size_t)C + c;
                     const float2 ov = unpk2(accA[e]);
                     if (out_f32) *reinterpret_cast<float2*>(out_f32 + o) = ov;
@@ -346,15 +352,15 @@ cudaError_t launch_dw3x3_down(const float* in, const float* w9, const float* bia
                               float* out_f32, __half* out_hi, __half* out_lo,
                               int n, int H, int W, int C, cudaStream_t s) {
     const int H2 = H / 2, W2 = W / 2;
-    const int rs = (H2 >= 8) ? 8 : 4, strips = H2 / rs;
-    const size_t per_img = (size_t)strips * (W2 / 2) * (C / 2);
+    const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs, pairs = (W2 + 1) / 2;
+    const size_t per_img = (size_t)strips * pairs * (C / 2);
     return for_image_groups(n, per_img, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t oi = (size_t)i0 * H * W * C, oo = (size_t)i0 * H2 * W2 * C;
         auto kern = (rs == 8) ? dw3x3_down_kernel<8> : dw3x3_down_kernel<4>;
         kern<<<(items + 255) / 256, 256, 16 * C * sizeof(float), s>>>(in + oi, w9, bias, fir16, out_f32 ? out_f32 + oo : nullptr,
                                                 out_hi ? out_hi + oo : nullptr, out_lo ? out_lo + oo : nullptr,
-                                                items, host_log2(W2), host_log2(H2), host_log2(C / 2), host_log2(strips));
+                                                items, H2, W2, host_log2(C / 2), FastDiv((uint32_t)pairs), FastDiv((uint32_t)strips));
     });
 }
 
@@ -376,17 +382,16 @@ template <int RS, int C>
 __global__ void __launch_bounds__(256, 2)
 dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ w9s, const float* __restrict__ biass,
                         const float* __restrict__ fir16, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                        uint32_t items, int lw2, int lh2, int lstrips) {
+                        uint32_t items, int H2, int W2, FastDiv pairs, FastDiv strips) {
     constexpr int CP = C / 2;                              // channel pairs
     constexpr float kLim = kActClamp * kActSplitScale;
     const uint32_t idx = blockIdx.x * 256u + threadIdx.x;
-    const int W2 = 1 << lw2, H2 = 1 << lh2, W = 2 * W2, H = 2 * H2;
+    const int W = 2 * W2, H = 2 * H2;
     const int c = (int)(idx % CP) * 2;
-    uint32_t t = idx / CP;
-    const int ox0 = (int)(t & ((W2 >> 1) - 1)) * 2;
-    t >>= (lw2 - 1);
-    const int strip = (int)(t & ((1u << lstrips) - 1));
-    const size_t img = t >> lstrips;
+    const uint32_t t = idx / CP, t2 = pairs.div(t), t3 = strips.div(t2);
+    const int ox0 = (int)(t - t2 * pairs.d) * 2;
+    const int strip = (int)(t2 - t3 * strips.d);
+    const size_t img = t3;
     const int oy0 = strip * RS;
 
     extern __shared__ float s_fir[];                       // [16][C]
@@ -403,6 +408,7 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
 
     const int iy_first = 2 * oy0 - 2;
     const bool left_ok = (ox0 > 0), right_ok = (ox0 + 2 < W2);            // columns 2ox0-2, 2ox0-1 / 2ox0+4, 2ox0+5 exist
+    const bool mid_ok = (ox0 + 1 < W2);                                     // 2ox0+2, 2ox0+3 (false: odd W2, last pair)
     // one row pointer: column j of the 8-column window is at j * C floats (immediate offsets)
     const float* rowp = in + ((img * H + iy_first) * (size_t)W + (2 * ox0 - 2)) * C + c;
     const size_t row_stride = (size_t)W * C;
@@ -421,7 +427,7 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
         const bool rowok = (iy >= 0 && iy < H);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            const bool ok = rowok && (j >= 2 || left_ok) && (j < 6 || right_ok);
+            const bool ok = rowok && (j >= 2 || left_ok) && (j < 4 || mid_ok) && (j < 6 || right_ok);
             vn[j] = ok ? __ldg(reinterpret_cast<const float2*>(rowp + j * C)) : zero2;
         }
         rowp += row_stride;
@@ -451,7 +457,7 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
             if (gy >= 0 && gy < H) {
 #pragma unroll
                 for (int tx = 0; tx < 6; ++tx) {
-                    if ((tx == 0 && !left_ok) || (tx == 5 && !right_ok)) continue;   // depthwise column outside the image: zero
+                    if ((tx == 0 && !left_ok) || ((tx == 3 || tx == 4) && !mid_ok) || (tx == 5 && !right_ok)) continue;   // outside the image: zero
                     const float2 a = dw[(r + 1) % 3][tx], b = fmul2f(a, alpha2);
                     const float2 d = make_float2(fminf(fmax3f(a.x, b.x, -kLim), kLim), fminf(fmax3f(a.y, b.y, -kLim), kLim));
                     if (tx < 4) {                         // tap column tx of output ox0
@@ -468,6 +474,7 @@ dw3x3_down_split_kernel(const float* __restrict__ in, const float* __restrict__ 
                 const int orow = oy0 + ((q - 3) >> 1);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
+                    if (orow >= H2 || ox0 + e >= W2) continue;
                     const size_t o = ((img * H2 + orow) * W2 + ox0 + e) * (size_t)C + c;
                     const float2 ov = accA[e];            // already * kActSplitScale
                     const __half2 h = __floats2half2_rn(ov.x, ov.y);
@@ -487,17 +494,16 @@ template <int RS, int C>
 static void launch_down_split_inst(const float* in, const float* w9s, const float* biass, const float* fir16, __half* hi, __half* lo,
                                    uint32_t items, int W2, int H2, int strips, cudaStream_t s) {
     launch_pdl(dw3x3_down_split_kernel<RS, C>, dim3((items + 255) / 256), dim3(256), 16 * C * sizeof(float), s, in, w9s, biass, fir16, hi, lo, items,
-               host_log2(W2), host_log2(H2), host_log2(strips));
+               H2, W2, FastDiv((uint32_t)((W2 + 1) / 2)), FastDiv((uint32_t)strips));
 }
 
 // w9s / biass: depthwise taps and bias * kActSplitScale * sqrt(2).  C in {64, 128, 256, 512}.
 cudaError_t launch_dw3x3_down_split(const float* in, const float* w9s, const float* biass, const float* fir16,
                                     __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s) {
     const int H2 = H / 2, W2 = W / 2;
-    if (W2 < 2 || (C != 64 && C != 128 && C != 256 && C != 512)) return cudaErrorInvalidValue;
-    const int rs = (H2 >= 8) ? 8 : 4, strips = H2 / rs;
-    if (strips < 1) return cudaErrorInvalidValue;
-    const size_t per_img = (size_t)strips * (W2 / 2) * (C / 2);
+    if (W2 < 2 || H2 < 1 || (C != 64 && C != 128 && C != 256 && C != 512)) return cudaErrorInvalidValue;
+    const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs;
+    const size_t per_img = (size_t)strips * ((W2 + 1) / 2) * (C / 2);
     return for_image_groups(n, per_img, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const float* ip = in + (size_t)i0 * H * W * C;
@@ -541,18 +547,18 @@ template <int RS>
 __global__ void __launch_bounds__(288, 2)
 dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* __restrict__ w9s, const float* __restrict__ biass,
                       const float* __restrict__ fir16, __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                      int C, int lw2, int lh2, int lstrips, int lslabs) {
+                      int C, int H2, int W2, int xtiles, int strips, int lslabs) {
     constexpr float kLim = kActClamp * kActSplitScale;
     constexpr int kRows = 2 * RS + 4;
     extern __shared__ __align__(128) unsigned char s_dyn[];
     __shared__ __align__(8) uint64_t s_bar[2 * kDownRing];
     float* s_fir = reinterpret_cast<float*>(s_dyn + kDownRing * kDownRowBytes);     // [16][64] taps of this slab
-    const int W2 = 1 << lw2, H2 = 1 << lh2, H = 2 * H2;
+    const int H = 2 * H2;
     uint32_t b = blockIdx.x;
     const int slab = (int)(b & ((1u << lslabs) - 1)); b >>= lslabs;
-    const int xtile = (int)(b & ((uint32_t)(W2 >> 4) - 1)); b >>= (lw2 - 4);
-    const int strip = (int)(b & ((1u << lstrips) - 1));
-    const int img = (int)(b >> lstrips);
+    const int xtile = (int)(b % (uint32_t)xtiles); b /= (uint32_t)xtiles;          // once per block
+    const int strip = (int)(b % (uint32_t)strips);
+    const int img = (int)(b / (uint32_t)strips);
     const int oy0 = strip * RS, iy_first = 2 * oy0 - 2;
     const int cs = slab * 64;
     const uint32_t bar0 = smem_addr(s_bar);
@@ -650,6 +656,7 @@ dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* _
                 const int orow = oy0 + ((q - 3) >> 1);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
+                    if (orow >= H2 || ox0 >= W2) continue;   // last strip / column tile past the edge (W2 is even)
                     const size_t o = (((size_t)img * H2 + orow) * W2 + ox0 + e) * (size_t)C + cs + c;
                     const float2 ov = accA[e];
                     const __half2 h = __floats2half2_rn(ov.x, ov.y);
@@ -668,10 +675,10 @@ dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* _
 cudaError_t launch_dw3x3_down_tma(const DownTensorMap& desc, const float* w9s, const float* biass, const float* fir16,
                                   __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s) {
     const int H2 = H / 2, W2 = W / 2;
-    if (W2 < 16 || (W2 & (W2 - 1)) || C % 64 != 0) return cudaErrorInvalidValue;
-    const int rs = (H2 >= 8) ? 8 : 4, strips = H2 / rs, slabs = C / 64;
-    if (strips < 1 || (slabs & (slabs - 1))) return cudaErrorInvalidValue;
-    const size_t blocks = (size_t)n * strips * (W2 / 16) * slabs;
+    if (W2 < 16 || W2 % 2 != 0 || H2 < 1 || C % 64 != 0) return cudaErrorInvalidValue;
+    const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs, slabs = C / 64, xtiles = (W2 + 15) / 16;
+    if (slabs & (slabs - 1)) return cudaErrorInvalidValue;
+    const size_t blocks = (size_t)n * strips * xtiles * slabs;
     if (blocks == 0 || blocks > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     const size_t smem = (size_t)kDownRing * kDownRowBytes + 16 * 64 * sizeof(float);
     static bool attr_set[2] = {false, false};
@@ -681,8 +688,8 @@ cudaError_t launch_dw3x3_down_tma(const DownTensorMap& desc, const float* w9s, c
         if (e != cudaSuccess) return e;
         attr_set[rs == 8] = true;
     }
-    return launch_pdl(kern, dim3((unsigned)blocks), dim3(288), smem, s, desc, w9s, biass, fir16, out_hi, out_lo, C, host_log2(W2), host_log2(H2),
-                      host_log2(strips), host_log2(slabs));
+    return launch_pdl(kern, dim3((unsigned)blocks), dim3(288), smem, s, desc, w9s, biass, fir16, out_hi, out_lo, C, H2, W2, xtiles,
+                      strips, host_log2(slabs));
 }
 
 // --------------------------------------------------------------------------------------
@@ -694,9 +701,9 @@ cudaError_t launch_dw3x3_down_tma(const DownTensorMap& desc, const float* w9s, c
 __global__ void __launch_bounds__(256)
 up2_noise_act_skip_kernel(const float* __restrict__ t, const float* __restrict__ fir16,
                           const float* __restrict__ noise, const float* __restrict__ skip,
-                          float* __restrict__ out, uint32_t items, int lw, int lh, int lcv) {
+                          float* __restrict__ out, uint32_t items, FastDiv fw, FastDiv fh, int lcv, int noise_pitch) {
     extern __shared__ float4 s_taps[];                    // [16][C/4]
-    const int w = 1 << lw, h = 1 << lh, W2 = 2 * w, C = 4 << lcv, CV = 1 << lcv;
+    const int w = (int)fw.d, h = (int)fh.d, W2 = 2 * w, C = 4 << lcv, CV = 1 << lcv;
     pdl_trigger();
     for (int i = threadIdx.x; i < 16 * CV; i += 256) s_taps[i] = ldg4(fir16 + i * 4);
     pdl_wait();
@@ -705,9 +712,10 @@ up2_noise_act_skip_kernel(const float* __restrict__ t, const float* __restrict__
     if (idx >= items) return;
     const int cv = (int)(idx & (CV - 1));
     const uint32_t p = idx >> lcv;                        // low-res pixel index over the image group
-    const int ix = (int)(p & (w - 1));
-    const int iy = (int)((p >> lw) & (h - 1));
-    const size_t img = p >> (lw + lh);
+    const uint32_t q = fw.div(p), qi = fh.div(q);
+    const int ix = (int)(p - q * fw.d);
+    const int iy = (int)(q - qi * fh.d);
+    const size_t img = qi;
     const float* src = t + img * (size_t)h * w * C + cv * 4;
     float4 nb[3][3];
 #pragma unroll
@@ -731,7 +739,7 @@ up2_noise_act_skip_kernel(const float* __restrict__ t, const float* __restrict__
                     fma4(acc, s_taps[((a + 2 * u) * 4 + (b + 2 * v)) * CV + cv], nb[a + u][b + v]);
             const int oy = 2 * iy + a, ox = 2 * ix + b;
             if (noise) {
-                const float nz = __ldg(noise + oy * W2 + ox);
+                const float nz = __ldg(noise + oy * noise_pitch + ox);
                 acc.x += nz; acc.y += nz; acc.z += nz; acc.w += nz;
             }
             acc = lrelu_agc4(acc);
@@ -744,14 +752,15 @@ up2_noise_act_skip_kernel(const float* __restrict__ t, const float* __restrict__
         }
 }
 
-cudaError_t launch_up2(const float* t, const float* fir16, const float* noise, const float* skip,
+cudaError_t launch_up2(const float* t, const float* fir16, const float* noise, int noise_pitch, const float* skip,
                        float* out, int n, int h, int w, int C, cudaStream_t s) {
     const size_t per_img = (size_t)h * w * (C / 4);
     return for_image_groups(n, per_img, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t oi = (size_t)i0 * h * w * C, oo = (size_t)i0 * 4 * h * w * C;
         launch_pdl(up2_noise_act_skip_kernel, dim3((items + 255) / 256), dim3(256), 16 * C * sizeof(float), s,
-                   t + oi, fir16, noise, skip ? skip + oo : nullptr, out + oo, items, host_log2(w), host_log2(h), host_log2(C / 4));
+                   t + oi, fir16, noise, skip ? skip + oo : nullptr, out + oo, items, FastDiv((uint32_t)w), FastDiv((uint32_t)h),
+                   host_log2(C / 4), noise_pitch);
     });
 }
 
@@ -763,7 +772,7 @@ template <int G>
 __global__ void __launch_bounds__(256)
 torgb_img_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
                  const float* __restrict__ img_lo, const float* __restrict__ fir, float* __restrict__ img_out,
-                 int64_t npix, int r, int C) {
+                 int64_t npix, int h, int wd, int C) {
     pdl_trigger();
     pdl_wait();
     const int lane = threadIdx.x & 31;
@@ -788,47 +797,72 @@ torgb_img_kernel(const float* __restrict__ x, const float* __restrict__ w, const
         a2 += __shfl_xor_sync(0xffffffffu, a2, off);
     }
     if (!valid || sub != 0) return;
-    const int ox = (int)(p % r);
-    const int oy = (int)((p / r) % r);
-    const int64_t img = p / ((int64_t)r * r);
+    const int ox = (int)(p % wd);
+    const int oy = (int)((p / wd) % h);
+    const int64_t img = p / ((int64_t)h * wd);
     float acc[3] = {a0 + __ldg(b), a1 + __ldg(b + 1), a2 + __ldg(b + 2)};
     if (img_lo) {
-        const int h = r >> 1;
+        const int hl = h >> 1, wl = wd >> 1;
         float up[3] = {0.f, 0.f, 0.f};
 #pragma unroll
         for (int a = 0; a < 2; ++a) {
             const int ty = (oy & 1) + 2 * a;
             const int iy = (oy + ty - 2) >> 1;
-            if (iy < 0 || iy >= h) continue;
+            if (iy < 0 || iy >= hl) continue;
 #pragma unroll
             for (int bb = 0; bb < 2; ++bb) {
                 const int tx = (ox & 1) + 2 * bb;
                 const int ix = (ox + tx - 2) >> 1;
-                if (ix < 0 || ix >= h) continue;
+                if (ix < 0 || ix >= wl) continue;
 #pragma unroll
                 for (int k = 0; k < 3; ++k)
                     up[k] = fmaf(__ldg(fir + (ty * 4 + tx) * 3 + k),
-                                 __ldg(img_lo + ((img * 3 + k) * h + iy) * h + ix), up[k]);
+                                 __ldg(img_lo + ((img * 3 + k) * hl + iy) * wl + ix), up[k]);
             }
         }
 #pragma unroll
         for (int k = 0; k < 3; ++k) acc[k] = up[k] + acc[k];
     }
 #pragma unroll
-    for (int k = 0; k < 3; ++k) img_out[((img * 3 + k) * r + oy) * r + ox] = acc[k];
+    for (int k = 0; k < 3; ++k) img_out[((img * 3 + k) * h + oy) * wd + ox] = acc[k];
 }
 
 cudaError_t launch_torgb(const float* x, const float* w, const float* b, const float* img_lo,
-                         const float* fir16x3, float* img_out, int n, int r, int C, cudaStream_t s) {
-    const int64_t npix = (int64_t)n * r * r;
+                         const float* fir16x3, float* img_out, int n, int h, int wd, int C, cudaStream_t s) {
+    const int64_t npix = (int64_t)n * h * wd;
     if (C / 4 >= 32) {
         const int64_t threads = npix * 32;
-        launch_pdl(torgb_img_kernel<32>, dim3(blocks_for(threads, 256)), dim3(256), 0, s, x, w, b, img_lo, fir16x3, img_out, npix, r, C);
+        launch_pdl(torgb_img_kernel<32>, dim3(blocks_for(threads, 256)), dim3(256), 0, s, x, w, b, img_lo, fir16x3, img_out, npix, h, wd, C);
     } else {
         const int64_t threads = npix * 16;
-        launch_pdl(torgb_img_kernel<16>, dim3(blocks_for(threads, 256)), dim3(256), 0, s, x, w, b, img_lo, fir16x3, img_out, npix, r, C);
+        launch_pdl(torgb_img_kernel<16>, dim3(blocks_for(threads, 256)), dim3(256), 0, s, x, w, b, img_lo, fir16x3, img_out, npix, h, wd, C);
     }
     return cudaGetLastError();
+}
+
+// --------------------------------------------------------------------------------------
+// Noise planes of a fully convolutional forward: every plane of the batch is its level's r x r plane (noise_const *
+// noise_strength [* sqrt 2], as uploaded) tiled over H x W, rows `pitch` floats apart, padding columns zero.  One launch
+// fills every plane (blockIdx.y = plane): a copy, so the values are bit-identical to the r x r plane's.
+// --------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+noise_tile_kernel(const __grid_constant__ NoiseTileBatch b) {
+    pdl_trigger();
+    pdl_wait();
+    const NoiseTile& t = b.t[blockIdx.y];
+    const int items = t.H * t.pitch;
+    for (int i = blockIdx.x * 256 + threadIdx.x; i < items; i += gridDim.x * 256) {
+        const int y = i / t.pitch, x = i - y * t.pitch;
+        t.dst[i] = x < t.W ? __ldg(t.src + (y % t.r) * t.r + x % t.r) : 0.f;
+    }
+}
+
+cudaError_t launch_noise_tile(const NoiseTileBatch& b, cudaStream_t s) {
+    if (b.count < 1 || b.count > kMaxNoiseTiles) return cudaErrorInvalidValue;
+    int64_t most = 0;
+    for (int i = 0; i < b.count; ++i) most = std::max<int64_t>(most, (int64_t)b.t[i].H * b.t[i].pitch);
+    const unsigned bx = (unsigned)std::min<int64_t>(blocks_for(most, 256), 512);
+    return launch_pdl(noise_tile_kernel, dim3(bx, (unsigned)b.count), dim3(256), 0, s, b);
 }
 
 // --------------------------------------------------------------------------------------

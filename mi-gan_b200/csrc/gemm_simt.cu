@@ -15,7 +15,7 @@ constexpr int BM = 128, BN = 64, BK = 16, TM = 8, TN = 4;
 
 __global__ void __launch_bounds__(256)
 pw_gemm_simt_kernel(const float* __restrict__ A, const float* __restrict__ Bt, float* __restrict__ out,
-                    int64_t P, int K, int N, const float* __restrict__ noise, int HW, int act) {
+                    int64_t P, int K, int N, const float* __restrict__ noise, int HW, int W, int noise_pitch, int act) {
     __shared__ float As[BK][BM + 4];
     __shared__ float Bs[BK][BN];
     const int tid = threadIdx.x;
@@ -69,7 +69,8 @@ pw_gemm_simt_kernel(const float* __restrict__ A, const float* __restrict__ Bt, f
         if (p >= P) continue;
         float4 v = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
         if (noise) {
-            const float nz = __ldg(noise + (p % HW));
+            const int q = (int)(p % HW);               // pixel of the image; the plane's rows are noise_pitch apart
+            const float nz = __ldg(noise + q + (q / W) * (noise_pitch - W));
             v.x += nz; v.y += nz; v.z += nz; v.w += nz;
         }
         if (act) v = lrelu_agc4(v);
@@ -78,10 +79,10 @@ pw_gemm_simt_kernel(const float* __restrict__ A, const float* __restrict__ Bt, f
 }
 
 cudaError_t launch_pw_gemm_simt(const float* A, const float* Bt, float* out, int64_t P, int K, int N,
-                                const float* noise, int HW, int act, cudaStream_t s) {
+                                const float* noise, int H, int W, int noise_pitch, int act, cudaStream_t s) {
     if (K % BK != 0 || N % BN != 0) return cudaErrorInvalidValue;
     dim3 grid((unsigned)((P + BM - 1) / BM), N / BN);
-    pw_gemm_simt_kernel<<<grid, 256, 0, s>>>(A, Bt, out, P, K, N, noise, HW, act);
+    pw_gemm_simt_kernel<<<grid, 256, 0, s>>>(A, Bt, out, P, K, N, noise, H * W, W, noise_pitch, act);
     return cudaGetLastError();
 }
 

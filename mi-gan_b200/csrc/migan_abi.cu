@@ -1,7 +1,7 @@
 // C ABI + host runtime of the H100-native MI-GAN generator (include/migan_b200.h).
 //
 // Host side of the hot path: weight registry in the reference's state_dict layout, one-time
-// repacking for the kernels, a per-batch-size execution plan (a flat list of kernel launches
+// repacking for the kernels, an execution plan per (batch size, input extent) (a flat list of kernel launches
 // with every pointer / tensor map resolved) and the launcher.  Replaces the module tree of
 // lib/model_zoo/migan_inference.py:173-369 (EncoderBlock / Encoder / SynthesisBlock* /
 // Synthesis / Generator): the control flow of those forward() methods is the plan below.
@@ -77,7 +77,7 @@ struct SepConv {
     __half* pw_lo = nullptr;  // [cout][cin] fp16 lo part
     float tc_inv_scale = 1.f; // 1 / (kActSplitScale * 2^k)
     float* fir16 = nullptr;   // [16][cin] (down) or [16][cout] (up), tap-major
-    float* noise_dev = nullptr;  // [res_out^2] = noise_const * noise_strength
+    float* noise_dev = nullptr;  // [res_out^2] = noise_const * noise_strength (the plane of an R x R forward)
     // fused up-sampling prologue of the NEXT layer (sepconv_tc SEPCONV_SRC_UP): needs channel-uniform FIR taps
     bool up_uniform = false;
     float up_taps_s2[16] = {0};      // taps * sqrt(2)
@@ -93,7 +93,7 @@ struct ToRgb {
     float* fir = nullptr;  // [16][3]
 };
 
-enum StepKind { K_STEM, K_DW, K_DWDOWN, K_GEMM_SIMT, K_SEPCONV_TC, K_UP2, K_TORGB, K_ADD };
+enum StepKind { K_STEM, K_DW, K_DWDOWN, K_GEMM_SIMT, K_SEPCONV_TC, K_UP2, K_TORGB, K_ADD, K_NOISE };
 
 constexpr int PTR_X = 1, PTR_Y = 2;  // flags: operand is the caller's x / y
 
@@ -104,6 +104,8 @@ struct Step {
     const float* in = nullptr;
     const float* aux = nullptr;  // skip tensor / low-res image / noise
     const float* aux2 = nullptr; // fused up-sampling prologue: the low-resolution raw tensor
+    const float* noise = nullptr; // K_GEMM_SIMT / K_UP2: the layer's noise plane, rows noise_pitch floats apart
+    int noise_pitch = 0;
     bool fused_stem = false, fused_up = false;
     float* out = nullptr;
     __half* hi = nullptr;
@@ -115,6 +117,7 @@ struct Step {
     migan::SepconvTcArgs tc;  // resolved wgmma launch (tensor maps, tiling)
     migan::DownTensorMap down_map;   // K_DWDOWN on the TMA-staged kernel: tensor map of the input
     bool down_tma = false;
+    migan::NoiseTileBatch noise_tiles;   // K_NOISE: the tiled noise planes of a fully convolutional forward
     // roofline bookkeeping: algorithmic bytes = own input(s) read once + output written once
     std::string label;
     double alg_bytes = 0, flops = 0;
@@ -131,7 +134,7 @@ struct Step {
 };
 
 struct Plan {
-    int n = 0, path = -1;
+    int n = 0, path = -1, H = 0, W = 0;
     void* ws = nullptr;
     std::vector<Step> steps;
 };
@@ -599,23 +602,69 @@ int migan_finalize_weights(migan_ctx* ctx) {
 }
 
 // ---- workspace layout -------------------------------------------------------------------
-//   feats[r]  n * r^2 * ch(r) fp32, one per encoder resolution (the decoder skip inputs)
-//   S0..S2    three rotating scratch tensors of n * R^2 * ch(R) fp32 (largest activation)
-//   IMG0/1    ping-pong planar RGB images n * 3 * R^2 fp32
-static size_t feat_bytes(int n, int r) { return align_up((size_t)n * r * r * channels(r) * sizeof(float), 1024); }
-static size_t scratch_bytes(const migan_ctx* c, int n) {
-    return align_up((size_t)n * c->resolution * c->resolution * channels(c->resolution) * sizeof(float), 1024);
+// For an n x H x W forward (H = W = R: the fixed-resolution forward), nominal level r has the extent
+// (H r / R, W r / R); channels are a function of r alone.
+//   feats[r]  n * h_r * w_r * ch(r) fp32, one per encoder level (the decoder skip inputs)
+//   S0..S2    three rotating scratch tensors of n * H * W * ch(R) fp32 (largest activation)
+//   IMG0/1    ping-pong planar RGB images n * 3 * H * W fp32
+//   NOISE     unless H = W = R: every noise plane tiled to its level's extent (rows padded to 16 bytes for TMA), plus the
+//             * sqrt 2 copy of the up-sampling layers'; at R x R the uploaded r x r planes are used as they are
+struct Ext { int h, w; };
+static Ext level_ext(const migan_ctx* c, int r, int H, int W) {
+    return {(int)((int64_t)H * r / c->resolution), (int)((int64_t)W * r / c->resolution)};
 }
-static size_t img_bytes(const migan_ctx* c, int n) {
-    return align_up((size_t)n * 3 * c->resolution * c->resolution * sizeof(float), 1024);
+static int noise_pitch(int w) { return (int)align_up((size_t)w, 4); }
+static bool full_res(const migan_ctx* c, int H, int W) { return H == c->resolution && W == c->resolution; }
+static size_t feat_bytes(int n, Ext e, int r) { return align_up((size_t)n * e.h * e.w * channels(r) * sizeof(float), 1024); }
+static size_t scratch_bytes(const migan_ctx* c, int n, int H, int W) {
+    return align_up((size_t)n * H * W * channels(c->resolution) * sizeof(float), 1024);
+}
+static size_t img_bytes(int n, int H, int W) { return align_up((size_t)n * 3 * H * W * sizeof(float), 1024); }
+static size_t noise_plane_bytes(Ext e) { return align_up((size_t)e.h * noise_pitch(e.w) * sizeof(float), 1024); }
+static size_t noise_bytes(const migan_ctx* c, int H, int W) {
+    if (full_res(c, H, W)) return 0;
+    size_t total = 0;
+    for (const auto* vec : {&c->syn1, &c->syn2})
+        for (const SepConv& L : *vec)
+            if (L.noise) total += noise_plane_bytes(level_ext(c, L.res_out, H, W)) * (L.up ? 2 : 1);
+    return total;
+}
+static size_t workspace_layout_bytes(const migan_ctx* ctx, int n, int H, int W) {
+    size_t total = 0;
+    for (int r : ctx->enc_res) total += feat_bytes(n, level_ext(ctx, r, H, W), r);
+    total += 3 * scratch_bytes(ctx, n, H, W) + 2 * img_bytes(n, H, W) + noise_bytes(ctx, H, W);
+    return total;
+}
+
+// The sizes a fully convolutional forward accepts: H, W >= R and multiples of R / 4 (every level's extent is then an
+// integer and at least the level's side, and every up-sampling lands on its skip feature), and a largest activation
+// n * H * W * ch(R) below 2^31 elements (the kernels use 32-bit offsets and TMA coordinates).
+static int check_shape(const migan_ctx* c, int n, int H, int W) {
+    const int R = c->resolution, q = R / 4;
+    if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
+    if (H < R || W < R || H % q != 0 || W % q != 0) {
+        auto down = [&](int v) { return std::max(R, v / q * q); };
+        auto up = [&](int v) { return std::max(R, (std::max(v, 0) + q - 1) / q * q); };
+        return fail(MIGAN_ERR_INVALID, "H x W = %d x %d is not a valid size for resolution %d: H and W must be multiples of %d "
+                    "(R/4) and at least %d; nearest valid sizes: %d x %d and %d x %d", H, W, R, q, R, down(H), down(W), up(H), up(W));
+    }
+    const int64_t per_img = (int64_t)H * W * channels(R);
+    if ((int64_t)n * per_img > INT32_MAX)
+        return fail(MIGAN_ERR_INVALID, "n x H x W x ch(R) = %d x %d x %d x %d = %lld elements in the largest activation is more than "
+                    "2^31 - 1 (32-bit kernel offsets); at %d x %d the largest batch is %lld", n, H, W, channels(R),
+                    (long long)(n * per_img), H, W, (long long)(INT32_MAX / per_img));
+    return MIGAN_OK;
 }
 
 size_t migan_workspace_bytes(const migan_ctx* ctx, int n) {
     if (!ctx || n <= 0) return 0;
-    size_t total = 0;
-    for (int r : ctx->enc_res) total += feat_bytes(n, r);
-    total += 3 * scratch_bytes(ctx, n) + 2 * img_bytes(ctx, n);
-    return total;
+    return workspace_layout_bytes(ctx, n, ctx->resolution, ctx->resolution);
+}
+
+size_t migan_workspace_bytes_hw(const migan_ctx* ctx, int n, int H, int W) {
+    if (!ctx) { fail(MIGAN_ERR_INVALID, "null ctx"); return 0; }
+    if (check_shape(ctx, n, H, W)) return 0;
+    return workspace_layout_bytes(ctx, n, H, W);
 }
 
 }  // extern "C"
@@ -659,11 +708,16 @@ struct Fuse {
 struct PlanBuilder {
     migan_ctx* c;
     int n, path;
+    int H = 0, W = 0;                 // input extent (R x R: the fixed-resolution forward)
     unsigned char* base;
     std::map<int, float*> feat;
     float* S[3];
     float* IMG[2];
+    struct NoiseRef { const float* plain = nullptr; const float* s2 = nullptr; int pitch = 0; };
+    std::map<const SepConv*, NoiseRef> noise;   // per noise layer: its plane at the layer's extent
     std::vector<Step> steps;
+
+    Ext ext(int r) const { return level_ext(c, r, H, W); }
 
     int other(int a, int b = -1) const {
         for (int i = 0; i < 3; ++i)
@@ -674,7 +728,7 @@ struct PlanBuilder {
         s.tap = name; s.tap_src = src; s.tapC = C; s.tapH = H; s.tapW = W; s.tap_planar = planar; s.tap_flags = flags;
     }
 
-    // Emit one SeparableConv2d reading `in` (NHWC [n,res_in,res_in,cin]); `skip` is added after the
+    // Emit one SeparableConv2d reading `in` (NHWC [n,h,w,cin] at res_in's extent); `skip` is added after the
     // final activation (decoder conv1, migan_inference.py:304-305).  Returns the output pointer.
     // in_idx: scratch index holding `in` (or -1 if it is a feat buffer); out_fixed: write there if non-null.
     int emit_sepconv(const SepConv& L, const float* in, int in_idx, float* out_fixed, const float* skip, int& out_idx, float*& out_ptr,
@@ -682,37 +736,39 @@ struct PlanBuilder {
                      const Fuse& fuse = Fuse()) {
         const int t1 = other(in_idx), t2 = other(in_idx, t1);
         const bool tc = (path != MIGAN_PATH_SIMT);
+        const Ext ein = ext(L.res_in), epw = ext(L.res_pw), eout = ext(L.res_out);
+        const NoiseRef nz = L.noise ? noise.at(&L) : NoiseRef();
         const float* gemm_in = nullptr;
         __half *ghi = nullptr, *glo = nullptr;
         bool presplit = L.down;
         if (L.down) {
-            Step s; s.kind = K_DWDOWN; s.L = &L; s.in = in; s.n = n; s.H = L.res_in; s.W = L.res_in; s.C = L.cin;
+            Step s; s.kind = K_DWDOWN; s.L = &L; s.in = in; s.n = n; s.H = ein.h; s.W = ein.w; s.C = L.cin;
             if (tc) {
                 s.hi = reinterpret_cast<__half*>(S[t1]);
-                s.lo = s.hi + (size_t)n * L.res_pw * L.res_pw * L.cin;
+                s.lo = s.hi + (size_t)n * epw.h * epw.w * L.cin;
                 ghi = s.hi; glo = s.lo;
                 if (L.res_pw >= 16) {   // rows staged through shared memory by TMA (elementwise.cu)
-                    if (const char* err = migan::make_down_tensor_map(&s.down_map, in, n, L.res_in, L.res_in, L.cin))
+                    if (const char* err = migan::make_down_tensor_map(&s.down_map, in, n, ein.h, ein.w, L.cin))
                         return fail(MIGAN_ERR_CUDA, "tensor map for %sdownsample failed: %s", L.p.c_str(), err);
                     s.down_tma = true;
                 }
             } else {
                 s.out = S[t1]; gemm_in = S[t1];
-                set_tap(s, L.p + "down", S[t1], L.cin, L.res_pw, L.res_pw);
+                set_tap(s, L.p + "down", S[t1], L.cin, epw.h, epw.w);
             }
             steps.push_back(s);
         } else if (!tc) {
-            Step s; s.kind = K_DW; s.L = &L; s.in = in; s.out = S[t1]; s.n = n; s.H = L.res_in; s.W = L.res_in; s.C = L.cin;
-            set_tap(s, L.p + "dw_act", S[t1], L.cin, L.res_in, L.res_in);
+            Step s; s.kind = K_DW; s.L = &L; s.in = in; s.out = S[t1]; s.n = n; s.H = ein.h; s.W = ein.w; s.C = L.cin;
+            set_tap(s, L.p + "dw_act", S[t1], L.cin, ein.h, ein.w);
             steps.push_back(s);
             gemm_in = S[t1];
         } else if (L.cout >= 512 && !rgb && L.res_in >= 64) {
             // Cout spans 8 N tiles: a fused prologue would re-run the depthwise stage per tile, so run it once as its
             // own kernel and hand the GEMM a pre-split operand.  Below 64 x 64 the repeated prologue is cheap and
             // saves a launch, so those levels keep the depthwise stage in the tensor-core kernel.
-            Step s; s.kind = K_DW; s.L = &L; s.in = in; s.n = n; s.H = L.res_in; s.W = L.res_in; s.C = L.cin;
+            Step s; s.kind = K_DW; s.L = &L; s.in = in; s.n = n; s.H = ein.h; s.W = ein.w; s.C = L.cin;
             s.hi = reinterpret_cast<__half*>(S[t1]);
-            s.lo = s.hi + (size_t)n * L.res_in * L.res_in * L.cin;
+            s.lo = s.hi + (size_t)n * ein.h * ein.w * L.cin;
             ghi = s.hi; glo = s.lo;
             steps.push_back(s);
             presplit = true;
@@ -725,9 +781,9 @@ struct PlanBuilder {
         else if (out_fixed) { pw_out = out_fixed; pw_idx = -1; }
         else { pw_out = S[t2]; pw_idx = t2; }
         {
-            Step s; s.L = &L; s.n = n; s.H = L.res_pw; s.W = L.res_pw; s.C = L.cin; s.out = pw_out;
+            Step s; s.L = &L; s.n = n; s.H = epw.h; s.W = epw.w; s.C = L.cin; s.out = pw_out;
             s.act = raw ? 0 : 1;
-            s.aux = (!raw && L.noise) ? L.noise_dev : nullptr;
+            if (!raw && L.noise) { s.noise = nz.plain; s.noise_pitch = nz.pitch; }
             if (tc) {
                 s.kind = K_SEPCONV_TC;
                 s.in = presplit ? nullptr : in;  // pre-split A operand from K_DWDOWN / K_DW
@@ -737,7 +793,8 @@ struct PlanBuilder {
                 d.source = presplit ? migan::SEPCONV_SRC_SPLIT : migan::SEPCONV_SRC_NHWC;
                 d.in_f32 = s.in; d.a_hi = ghi; d.a_lo = glo;
                 d.w9 = L.w9_tc; d.bias = L.bias_tc; d.w_hi = L.pw_hi; d.w_lo = L.pw_lo; d.inv_scale = L.tc_inv_scale;
-                d.noise = s.aux; d.out = pw_out; d.n = n; d.res = L.res_pw; d.cin = L.cin; d.cout = L.cout; d.act = s.act; d.rgb = rgb;
+                d.noise = s.noise; d.out = pw_out; d.n = n; d.h = epw.h; d.w = epw.w; d.cin = L.cin; d.cout = L.cout; d.act = s.act; d.rgb = rgb;
+                d.noise_pitch = noise_pitch(epw.w);
                 if (fuse.stem) {
                     d.source = migan::SEPCONV_SRC_STEM; d.in_f32 = nullptr;
                     d.stem_w = c->fromrgb_w_s2; d.stem_b = c->fromrgb_b_s2;
@@ -745,20 +802,20 @@ struct PlanBuilder {
                 } else if (fuse.up) {
                     d.source = migan::SEPCONV_SRC_UP;      // d.in_f32 = `in` = the encoder feature (skip tensor)
                     d.up_t = fuse.up_t;
-                    d.up_noise = fuse.up->noise ? fuse.up->noise_s2_dev : nullptr;
+                    d.up_noise = fuse.up->noise ? noise.at(fuse.up).s2 : nullptr;
                     memcpy(d.up_taps, fuse.up->up_taps_s2, sizeof(d.up_taps));
                     s.aux2 = fuse.up_t; s.fused_up = true;
                 }
                 const char* err = migan::sepconv_tc_plan_ex(&s.tc, d);
                 if (rgb) {
                     s.io_flags |= rgb_flags;
-                    s.tap2 = rgb_tap; s.tap2_src = rgb->img_out; s.tap2C = 3; s.tap2H = L.res_pw; s.tap2W = L.res_pw; s.tap2_flags = rgb_flags;
+                    s.tap2 = rgb_tap; s.tap2_src = rgb->img_out; s.tap2C = 3; s.tap2H = epw.h; s.tap2W = epw.w; s.tap2_flags = rgb_flags;
                 }
                 if (err) return fail(MIGAN_ERR_CUDA, "wgmma plan for %s failed: %s", L.p.c_str(), err);
             } else {
                 s.kind = K_GEMM_SIMT; s.in = gemm_in;
             }
-            if (!(rgb && !rgb->store_out)) set_tap(s, L.p + (raw ? "pw" : "out"), pw_out, L.cout, L.res_pw, L.res_pw);
+            if (!(rgb && !rgb->store_out)) set_tap(s, L.p + (raw ? "pw" : "out"), pw_out, L.cout, epw.h, epw.w);
             steps.push_back(s);
         }
         out_ptr = pw_out; out_idx = pw_idx;
@@ -768,13 +825,14 @@ struct PlanBuilder {
             if (out_fixed) { up_out = out_fixed; up_idx = -1; }
             else { up_idx = other(pw_idx); up_out = S[up_idx]; }
             Step s; s.kind = K_UP2; s.L = &L; s.in = pw_out; s.out = up_out; s.aux = skip;
-            s.n = n; s.H = L.res_pw; s.W = L.res_pw; s.C = L.cout;
-            set_tap(s, L.p + (skip ? "out_skip" : "out"), up_out, L.cout, L.res_out, L.res_out);
+            s.noise = nz.plain; s.noise_pitch = nz.pitch;
+            s.n = n; s.H = epw.h; s.W = epw.w; s.C = L.cout;
+            set_tap(s, L.p + (skip ? "out_skip" : "out"), up_out, L.cout, eout.h, eout.w);
             steps.push_back(s);
             out_ptr = up_out; out_idx = up_idx;
         } else if (skip) {
-            Step s; s.kind = K_ADD; s.out = pw_out; s.aux = skip; s.n = n; s.H = L.res_out; s.W = L.res_out; s.C = L.cout;
-            set_tap(s, L.p + "out_skip", pw_out, L.cout, L.res_out, L.res_out);
+            Step s; s.kind = K_ADD; s.out = pw_out; s.aux = skip; s.n = n; s.H = eout.h; s.W = eout.w; s.C = L.cout;
+            set_tap(s, L.p + "out_skip", pw_out, L.cout, eout.h, eout.w);
             steps.push_back(s);
         }
         return MIGAN_OK;
@@ -782,18 +840,45 @@ struct PlanBuilder {
 
     int build() {
         size_t off = 0;
-        for (int r : c->enc_res) { feat[r] = reinterpret_cast<float*>(base + off); off += feat_bytes(n, r); }
-        for (int i = 0; i < 3; ++i) { S[i] = reinterpret_cast<float*>(base + off); off += scratch_bytes(c, n); }
-        for (int i = 0; i < 2; ++i) { IMG[i] = reinterpret_cast<float*>(base + off); off += img_bytes(c, n); }
+        for (int r : c->enc_res) { feat[r] = reinterpret_cast<float*>(base + off); off += feat_bytes(n, ext(r), r); }
+        for (int i = 0; i < 3; ++i) { S[i] = reinterpret_cast<float*>(base + off); off += scratch_bytes(c, n, H, W); }
+        for (int i = 0; i < 2; ++i) { IMG[i] = reinterpret_cast<float*>(base + off); off += img_bytes(n, H, W); }
         const int R = c->resolution;
         const bool tcp = (path != MIGAN_PATH_SIMT);
+        // ---- noise planes: noise[i, j] = noise_const[i mod r, j mod r] * noise_strength at a level of extent h x w ----
+        if (full_res(c, H, W)) {
+            for (const auto* vec : {&c->syn1, &c->syn2})
+                for (const SepConv& L : *vec)
+                    if (L.noise) noise[&L] = {L.noise_dev, L.noise_s2_dev, L.res_out};
+        } else {   // one launch tiles every plane into the workspace (the uploaded r x r planes are its sources)
+            Step s; s.kind = K_NOISE; s.n = n;
+            migan::NoiseTileBatch& b = s.noise_tiles;
+            b.count = 0;
+            auto add = [&](const float* src, int r, Ext e) {
+                float* dst = reinterpret_cast<float*>(base + off);
+                off += noise_plane_bytes(e);
+                b.t[b.count++] = {src, dst, r, e.h, e.w, noise_pitch(e.w)};
+                return dst;
+            };
+            for (const auto* vec : {&c->syn1, &c->syn2})
+                for (const SepConv& L : *vec) {
+                    if (!L.noise) continue;
+                    if (b.count + 2 > migan::kMaxNoiseTiles) return fail(MIGAN_ERR_INVALID, "too many noise planes");
+                    const Ext e = ext(L.res_out);
+                    NoiseRef& ref = noise[&L];
+                    ref.pitch = noise_pitch(e.w);
+                    ref.plain = add(L.noise_dev, L.res_out, e);
+                    if (L.up) ref.s2 = add(L.noise_s2_dev, L.res_out, e);
+                }
+            if (b.count) steps.push_back(s);
+        }
         // ---- encoder (migan_inference.py:235-246) ----
         // The stem (fromrgb + activation, :193-196) is recomputed inside encoder.b{R}.conv1's prologue when that layer runs
         // on the fused tensor-core kernel with 8 x 16 tiles; otherwise it is its own kernel.
         const bool fuse_stem = tcp && R >= 16 && channels(R) < 512;
         if (!fuse_stem) {
-            Step s; s.kind = K_STEM; s.io_flags = PTR_X; s.out = S[0]; s.n = n; s.H = R; s.W = R; s.C = channels(R);
-            set_tap(s, "encoder.b" + std::to_string(R) + ".fromrgb", S[0], channels(R), R, R);
+            Step s; s.kind = K_STEM; s.io_flags = PTR_X; s.out = S[0]; s.n = n; s.H = H; s.W = W; s.C = channels(R);
+            set_tap(s, "encoder.b" + std::to_string(R) + ".fromrgb", S[0], channels(R), H, W);
             steps.push_back(s);
         }
         const float* cur = S[0];
@@ -830,7 +915,7 @@ struct PlanBuilder {
                 migan::SepconvTcDesc q;
                 q.passes = (path == MIGAN_PATH_TC_FAST) ? 1 : 3;
                 q.source = fuse_up ? migan::SEPCONV_SRC_UP : migan::SEPCONV_SRC_NHWC;
-                q.n = n; q.res = L2.res_pw; q.cin = L2.cin; q.cout = L2.cout;
+                q.n = n; q.h = ext(L2.res_pw).h; q.w = ext(L2.res_pw).w; q.cin = L2.cin; q.cout = L2.cout;
                 fuse_rgb = migan::sepconv_tc_fuses_rgb(q);
             }
             Fuse f1; f1.defer_up = fuse_up;
@@ -850,11 +935,11 @@ struct PlanBuilder {
                 rc = emit_sepconv(c->syn2[i], in2, cur_idx, nullptr, nullptr, oi, op, nullptr, std::string(), 0, f2);
                 if (rc) return rc;
                 cur = op; cur_idx = oi;
-                Step s; s.kind = K_TORGB; s.T = &T; s.in = cur; s.n = n; s.H = r; s.W = r; s.C = channels(r);
+                Step s; s.kind = K_TORGB; s.T = &T; s.in = cur; s.n = n; s.H = ext(r).h; s.W = ext(r).w; s.C = channels(r);
                 s.aux = img_lo;
                 if (last) { s.io_flags = PTR_Y; s.out = nullptr; }
                 else s.out = img_out;
-                set_tap(s, T.p + "img", s.out, 3, r, r, true, last ? PTR_Y : 0);
+                set_tap(s, T.p + "img", s.out, 3, s.H, s.W, true, last ? PTR_Y : 0);
                 steps.push_back(s);
             }
             img_cur = img_next;
@@ -873,6 +958,7 @@ struct PlanBuilder {
             case K_UP2: return "up2_noise_act_skip";
             case K_TORGB: return "torgb_img";
             case K_ADD: return "add_inplace";
+            case K_NOISE: return "noise_tile";
         }
         return "?";
     }
@@ -899,18 +985,24 @@ struct PlanBuilder {
                 case K_UP2: s.alg_bytes = px * s.C * f * (1 + 4 + (s.aux ? 4 : 0)); s.flops = px * 4 * s.C * 8; break;
                 case K_TORGB: s.alg_bytes = px * (s.C + 3 + (s.aux ? 0.75 : 0)) * f; s.flops = px * s.C * 6; break;
                 case K_ADD: s.alg_bytes = px * s.C * 3 * f; s.flops = px * s.C; break;
+                case K_NOISE:
+                    s.alg_bytes = 0; s.flops = 0;
+                    for (int i = 0; i < s.noise_tiles.count; ++i)
+                        s.alg_bytes += (double)s.noise_tiles.t[i].H * s.noise_tiles.t[i].pitch * f;
+                    break;
             }
-            s.label = (s.L ? s.L->p : s.T ? s.T->p + "torgb." : std::string("encoder.fromrgb.")) + kernel_name(s.kind);
+            s.label = (s.L ? s.L->p : s.T ? s.T->p + "torgb." : s.kind == K_NOISE ? std::string("synthesis.") : std::string("encoder.fromrgb.")) +
+                      kernel_name(s.kind);
         }
     }
 };
 
-int build_plan(migan_ctx* ctx, int n, int path, void* ws) {
+int build_plan(migan_ctx* ctx, int n, int H, int W, int path, void* ws) {
     PlanBuilder pb;
-    pb.c = ctx; pb.n = n; pb.path = path; pb.base = static_cast<unsigned char*>(ws);
+    pb.c = ctx; pb.n = n; pb.H = H; pb.W = W; pb.path = path; pb.base = static_cast<unsigned char*>(ws);
     int rc = pb.build();
     if (rc) return rc;
-    ctx->plan.n = n; ctx->plan.path = path; ctx->plan.ws = ws;
+    ctx->plan.n = n; ctx->plan.path = path; ctx->plan.ws = ws; ctx->plan.H = H; ctx->plan.W = W;
     ctx->plan.steps.swap(pb.steps);
     return MIGAN_OK;
 }
@@ -936,16 +1028,19 @@ int run_step(migan_ctx* ctx, Step& s, const float* x, float* y, cudaStream_t st)
             break;
         case K_GEMM_SIMT:
             e = migan::launch_pw_gemm_simt(in, s.L->pw_t, out, (int64_t)s.n * s.H * s.W, s.L->cin, s.L->cout,
-                                           s.aux, s.H * s.W, s.act, st);
+                                           s.noise, s.H, s.W, s.noise_pitch, s.act, st);
             break;
         case K_SEPCONV_TC:
             e = migan::launch_sepconv_tc(s.tc, st, (s.io_flags & PTR_Y) ? y : nullptr, s.fused_stem ? x : nullptr);
             break;
         case K_UP2:
-            e = migan::launch_up2(in, s.L->fir16, s.L->noise ? s.L->noise_dev : nullptr, s.aux, out, s.n, s.H, s.W, s.C, st);
+            e = migan::launch_up2(in, s.L->fir16, s.noise, s.noise_pitch, s.aux, out, s.n, s.H, s.W, s.C, st);
             break;
         case K_TORGB:
-            e = migan::launch_torgb(in, s.T->w, s.T->b, s.aux, s.T->fir, out, s.n, s.H, s.C, st);
+            e = migan::launch_torgb(in, s.T->w, s.T->b, s.aux, s.T->fir, out, s.n, s.H, s.W, s.C, st);
+            break;
+        case K_NOISE:
+            e = migan::launch_noise_tile(s.noise_tiles, st);
             break;
         case K_ADD:
             e = migan::launch_add(out, s.aux, (int64_t)s.n * s.H * s.W * s.C, st);
@@ -973,22 +1068,23 @@ int run_step(migan_ctx* ctx, Step& s, const float* x, float* y, cudaStream_t st)
 
 }  // namespace
 
-extern "C" {
-
-int migan_forward(migan_ctx* ctx, const float* x, float* y, int n, void* workspace, size_t workspace_bytes,
-                  int path, void* stream) {
+// The forward at any accepted extent: x [n,4,H,W] -> y [n,3,H,W].  H = W = R is migan_forward.
+static int forward_impl(migan_ctx* ctx, const float* x, float* y, int n, int H, int W, void* workspace, size_t workspace_bytes,
+                        int path, void* stream) {
     if (!ctx || !x || !y || !workspace) return fail(MIGAN_ERR_INVALID, "null argument");
     if (!ctx->finalized) return fail(MIGAN_ERR_STATE, "weights not finalized (call migan_finalize_weights)");
     if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
     if (path != MIGAN_PATH_SIMT && path != MIGAN_PATH_TC && path != MIGAN_PATH_TC_FAST)
         return fail(MIGAN_ERR_INVALID, "unknown path %d", path);
-    if (workspace_bytes < migan_workspace_bytes(ctx, n))
-        return fail(MIGAN_ERR_WORKSPACE, "workspace too small: %zu < %zu bytes", workspace_bytes, migan_workspace_bytes(ctx, n));
+    const size_t need = workspace_layout_bytes(ctx, n, H, W);
+    if (workspace_bytes < need)
+        return fail(MIGAN_ERR_WORKSPACE, "workspace too small: %zu < %zu bytes", workspace_bytes, need);
     if ((reinterpret_cast<uintptr_t>(workspace) & 1023) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15))
         return fail(MIGAN_ERR_WORKSPACE, "workspace must be 1024-byte aligned, x / y 16-byte aligned");
     CUDA_TRY(cudaSetDevice(ctx->device));
-    if (ctx->plan.n != n || ctx->plan.path != path || ctx->plan.ws != workspace) {
-        int rc = build_plan(ctx, n, path, workspace);
+    // alternating shapes rebuild the plan (tensor maps, tile grids and noise planes depend on the extent)
+    if (ctx->plan.n != n || ctx->plan.path != path || ctx->plan.ws != workspace || ctx->plan.H != H || ctx->plan.W != W) {
+        int rc = build_plan(ctx, n, H, W, path, workspace);
         if (rc) return rc;
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1009,6 +1105,21 @@ int migan_forward(migan_ctx* ctx, const float* x, float* y, int n, void* workspa
         ++i;
     }
     return MIGAN_OK;
+}
+
+extern "C" {
+
+int migan_forward(migan_ctx* ctx, const float* x, float* y, int n, void* workspace, size_t workspace_bytes,
+                  int path, void* stream) {
+    if (!ctx) return fail(MIGAN_ERR_INVALID, "null argument");
+    return forward_impl(ctx, x, y, n, ctx->resolution, ctx->resolution, workspace, workspace_bytes, path, stream);
+}
+
+int migan_forward_hw(migan_ctx* ctx, const float* x, float* y, int n, int H, int W, void* workspace, size_t workspace_bytes,
+                     int path, void* stream) {
+    if (!ctx) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (int rc = check_shape(ctx, n, H, W)) return rc;
+    return forward_impl(ctx, x, y, n, H, W, workspace, workspace_bytes, path, stream);
 }
 
 size_t migan_graph_staging_bytes(const migan_ctx* ctx, int n) {
@@ -1184,9 +1295,9 @@ static int forward_u8_enqueue(migan_ctx* ctx, const uint8_t* img_host, const uin
     CUDA_TRY(cudaMemcpyAsync(stage.mask, mask_host, px, cudaMemcpyHostToDevice, ctx->s_in));
     CUDA_TRY(cudaEventRecord(ev.in, ctx->s_in));
     CUDA_TRY(cudaStreamWaitEvent(st, ev.in, 0));
-    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(stage.img, stage.mask, stage.x, n, R, st));
+    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(stage.img, stage.mask, stage.x, n, R, R, st));
     if (int rc = migan_forward(ctx, stage.x, stage.y, n, workspace, ws, path, stream)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(stage.y, stage.img, stage.mask, stage.out, n, R, st));
+    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(stage.y, stage.img, stage.mask, stage.out, n, R, R, st));
     ctx->last_launches += 2;
     CUDA_TRY(cudaEventRecord(ev.compute_done, st));   // recorded again by ring.end() at the same point of st
     CUDA_TRY(cudaStreamWaitEvent(ctx->s_out, ev.compute_done, 0));
@@ -1211,13 +1322,25 @@ int migan_forward_u8_async(migan_ctx* ctx, const uint8_t* img_host, const uint8_
 
 int b200_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, void* stream) {
     if (!img || !mask || !x || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img, mask, x, n, r, static_cast<cudaStream_t>(stream)));
+    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img, mask, x, n, r, r, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 
 int b200_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, void* stream) {
     if (!y || !img || !mask || !out || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(y, img, mask, out, n, r, static_cast<cudaStream_t>(stream)));
+    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(y, img, mask, out, n, r, r, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_preprocess_u8_hw(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, void* stream) {
+    if (!img || !mask || !x || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8_hw: bad arguments");
+    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img, mask, x, n, H, W, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_postprocess_u8_hw(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, void* stream) {
+    if (!y || !img || !mask || !out || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8_hw: bad arguments");
+    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(y, img, mask, out, n, H, W, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 
@@ -1488,7 +1611,7 @@ int migan_tap_info(const migan_ctx* ctx, int path, int index, const char** name,
         // Build a throw-away plan for n = 1 on a fake base address (nothing is launched; tensor maps are
         // only encoded, never dereferenced).
         PlanBuilder pb;
-        pb.c = const_cast<migan_ctx*>(ctx); pb.n = 1; pb.path = path;
+        pb.c = const_cast<migan_ctx*>(ctx); pb.n = 1; pb.path = path; pb.H = pb.W = ctx->resolution;
         pb.base = reinterpret_cast<unsigned char*>(uintptr_t(1) << 30);
         int rc = pb.build();
         if (rc) return rc;
@@ -1537,7 +1660,7 @@ int b200_conv1x1_nhwc(const float* x, const float* w_t, float* y, int64_t pixels
     if (cin % 16 != 0 || cout % 64 != 0 || cin < 16 || cout < 64)
         return fail(MIGAN_ERR_INVALID, "conv1x1: cin must be a multiple of 16 and cout of 64, got %d -> %d", cin, cout);
     if (pixels == 0) return MIGAN_OK;
-    cudaError_t e = migan::launch_pw_gemm_simt(x, w_t, y, pixels, cin, cout, nullptr, 1, 0, static_cast<cudaStream_t>(stream));
+    cudaError_t e = migan::launch_pw_gemm_simt(x, w_t, y, pixels, cin, cout, nullptr, 1, 1, 1, 0, static_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "conv1x1 launch failed: %s", cudaGetErrorString(e));
     return MIGAN_OK;
 }

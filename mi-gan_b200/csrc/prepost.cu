@@ -1,7 +1,7 @@
 // uint8 pre/post-processing around the generator (SURVEY.md 8(f) rank 1; scripts/demo.py:56-66 and :135-142):
-//   pre : img u8 [n][R][R][3] + mask u8 [n][R][R] (255 = known)  ->  x fp32 NCHW [n][4][R][R] = cat([mask-0.5, img*mask])
-//   post: y fp32 NCHW [n][3][R][R] -> (y*0.5+0.5).clamp(0,1)*255 -> u8 (truncation) -> composite with the known pixels,
-//         u8 HWC [n][R][R][3].
+//   pre : img u8 [n][H][W][3] + mask u8 [n][H][W] (255 = known)  ->  x fp32 NCHW [n][4][H][W] = cat([mask-0.5, img*mask])
+//   post: y fp32 NCHW [n][3][H][W] -> (y*0.5+0.5).clamp(0,1)*255 -> u8 (truncation) -> composite with the known pixels,
+//         u8 HWC [n][H][W][3].   (H = W = R for the fixed-resolution forward.)
 // With these the host<->device traffic of a request is 4 + 3 bytes per pixel instead of 16 + 12.
 // Item kernels (one pixel per thread) in the comod_kernels.cuh style, so the emulation build checks them on the CPU.
 // Every product of the reference is rounded separately (no FMA contraction) to stay bit-exact with torch.
@@ -20,7 +20,7 @@
 
 namespace comod {
 
-struct PreU8K {        // items = n*R*R
+struct PreU8K {        // items = n*H*W
     const uint8_t* img; const uint8_t* mask; float* x; int64_t HW;
 #ifdef MIGAN_EMULATE
     inline
@@ -39,7 +39,7 @@ struct PreU8K {        // items = n*R*R
     }
 };
 
-struct PostU8K {       // items = n*R*R
+struct PostU8K {       // items = n*H*W
     const float* y; const uint8_t* img; const uint8_t* mask; uint8_t* out; int64_t HW;
 #ifdef MIGAN_EMULATE
     inline
@@ -118,13 +118,13 @@ int launch_feather_composite(const float* y, const uint8_t* img, const uint8_t* 
     for (int i = 0; i < 25; ++i) k.k[i] = k25_host[i];
     return (int)comod::ck_launch(k, (int64_t)n * H * W, s);
 }
-int launch_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, ck_stream_t s) {
-    comod::PreU8K k{img, mask, x, (int64_t)r * r};
-    return (int)comod::ck_launch(k, (int64_t)n * r * r, s);
+int launch_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, ck_stream_t s) {
+    comod::PreU8K k{img, mask, x, (int64_t)H * W};
+    return (int)comod::ck_launch(k, (int64_t)n * H * W, s);
 }
-int launch_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, ck_stream_t s) {
-    comod::PostU8K k{y, img, mask, out, (int64_t)r * r};
-    return (int)comod::ck_launch(k, (int64_t)n * r * r, s);
+int launch_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, ck_stream_t s) {
+    comod::PostU8K k{y, img, mask, out, (int64_t)H * W};
+    return (int)comod::ck_launch(k, (int64_t)n * H * W, s);
 }
 }  // namespace migan
 
@@ -135,9 +135,15 @@ extern "C" int b200_feather_composite(const float* y, const uint8_t* img, const 
     return migan::launch_feather_composite(y, img, mask, out, n, H, W, k25, s);
 }
 extern "C" int b200_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, void* s) {
-    return migan::launch_preprocess_u8(img, mask, x, n, r, s);
+    return migan::launch_preprocess_u8(img, mask, x, n, r, r, s);
 }
 extern "C" int b200_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, void* s) {
-    return migan::launch_postprocess_u8(y, img, mask, out, n, r, s);
+    return migan::launch_postprocess_u8(y, img, mask, out, n, r, r, s);
+}
+extern "C" int b200_preprocess_u8_hw(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, void* s) {
+    return migan::launch_preprocess_u8(img, mask, x, n, H, W, s);
+}
+extern "C" int b200_postprocess_u8_hw(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, void* s) {
+    return migan::launch_postprocess_u8(y, img, mask, out, n, H, W, s);
 }
 #endif

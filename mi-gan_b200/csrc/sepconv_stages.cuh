@@ -174,8 +174,9 @@ SC_DEV void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_h
 //   x = lrelu_agc( Upsample2d(t) + noise ) + skip          migan_inference.py:98-103, :165-169, :304-305
 // Upsample2d = zero insertion + pad(2,1,2,1) + 4x4 FIR, i.e. the polyphase form
 //   out[2i + a][2j + b] = sum_{u,v in {0,1}} f[a + 2u][b + 2v] * t[i - 1 + a + u][j - 1 + b + v]      (t = 0 outside)
-// IN arrives holding the skip tensor (encoder feature, zero outside the image); pixels outside the image must stay
-// ZERO (they are the depthwise conv's zero padding), not act(noise).
+// IN arrives holding the skip tensor (encoder feature, zero outside the image); pixels outside the H x W image must
+// stay ZERO (they are the depthwise conv's zero padding), not act(noise).  That covers the halo of every tile and, for a
+// tile that reaches past the right or bottom edge, every IN row / column beyond it.
 // `f` = the 16 taps * sqrt(2) (channel-uniform: checked on the host), NZ = noise * sqrt(2).
 //
 // Decomposition: the tile origin is even, so IN row 2i is the ODD image row 2m-1 and IN row 2i+1 the even row 2m
@@ -187,7 +188,7 @@ SC_DEV void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_h
 struct UpTaps { float f[16]; };
 
 SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
-                        int y0, int x0, int R, int has_noise, int tg) {
+                        int y0, int x0, int H, int W, int has_noise, int tg) {
     const int cvec = tg & 7;
 #pragma unroll 1
     for (int item = tg; item < 360; item += 128) {
@@ -195,9 +196,10 @@ SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const fl
         const int i = cell / 9, j = cell - i * 9;
         const f4* tp = ta + (i * 10 + j) * 8 + cvec;
         const F4 t00 = as_f4(tp[0]), t01 = as_f4(tp[8]), t10 = as_f4(tp[80]), t11 = as_f4(tp[88]);
-        // rows / columns of the block that lie outside the image (only on border tiles)
-        const bool row_out[2] = {(y0 == 0) && (i == 0), (y0 + 8 == R) && (i == 4)};
-        const bool col_out[2] = {(x0 == 0) && (j == 0), (x0 + 16 == R) && (j == 8)};
+        // rows / columns of the block that lie outside the image: IN rows 2i, 2i+1 are image rows y0-1+2i, y0+2i
+        const int ya = y0 - 1 + 2 * i, xa = x0 - 1 + 2 * j;
+        const bool row_out[2] = {ya < 0 || ya >= H, ya + 1 >= H};
+        const bool col_out[2] = {xa < 0 || xa >= W, xa + 1 >= W};
         f4* px0 = in + ((2 * i) * 18 + 2 * j) * 8 + cvec;
         const float* nzp = nz + (2 * i) * kAuxW + 2 * j + kAuxLeft - 1;
 #pragma unroll
@@ -226,6 +228,12 @@ SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const fl
     }
 }
 
+// The same on a square R x R image.
+SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
+                        int y0, int x0, int R, int has_noise, int tg) {
+    prestage_up(in, ta, nz, taps, y0, x0, R, R, has_noise, tg);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // STEM pre-stage: IN[r][c][ch] = lrelu_agc( fromrgb(x)[ch] + b[ch] ) for the chunk's 32 channels (zero outside the
 // image): EncoderBlock.fromrgb + activation, migan_inference.py:193-196, recomputed on the halo so the 64-channel
@@ -235,7 +243,7 @@ SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const fl
 // ---------------------------------------------------------------------------------------------------------------
 template <bool kBorder>
 SC_DEV void prestage_stem_t(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
-                            const float* __restrict__ bs, int cg0, int y0, int x0, int R, int tg) {
+                            const float* __restrict__ bs, int cg0, int y0, int x0, int H, int W, int tg) {
     const int cvec = tg & 7;
     const int ch = cg0 + cvec * 4;
     // ws is pair-interleaved: [channel pair][plane][2] = (w[ch][i], w[ch+1][i]) adjacent, so a 128-bit load is two ready pairs
@@ -263,15 +271,21 @@ SC_DEV void prestage_stem_t(f4* __restrict__ in, const float* __restrict__ xa, c
         F4 o;
         o.lo = act_pair(lo, kClamp);
         o.hi = act_pair(hi, kClamp);
-        if (kBorder && !((Y >= 0) && (Y < R) && (X >= 0) && (X < R))) { o.lo = p2zero(); o.hi = p2zero(); }
+        if (kBorder && !((Y >= 0) && (Y < H) && (X >= 0) && (X < W))) { o.lo = p2zero(); o.hi = p2zero(); }
         in[px * 8 + cvec] = to_f4(o);
     }
 }
-// Tiles that touch the image border zero the halo pixels outside the image; interior tiles (most of them) skip the test.
+// Tiles that touch (or reach past) the image border zero the pixels outside the image; interior tiles (most of them)
+// skip the test.
+SC_DEV void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
+                          const float* __restrict__ bs, int cg0, int y0, int x0, int H, int W, int tg) {
+    if (y0 == 0 || x0 == 0 || y0 + 8 >= H || x0 + 16 >= W) prestage_stem_t<true>(in, xa, ws, bs, cg0, y0, x0, H, W, tg);
+    else prestage_stem_t<false>(in, xa, ws, bs, cg0, y0, x0, H, W, tg);
+}
+// The same on a square R x R image.
 SC_DEV void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
                           const float* __restrict__ bs, int cg0, int y0, int x0, int R, int tg) {
-    if (y0 == 0 || x0 == 0 || y0 + 8 == R || x0 + 16 == R) prestage_stem_t<true>(in, xa, ws, bs, cg0, y0, x0, R, tg);
-    else prestage_stem_t<false>(in, xa, ws, bs, cg0, y0, x0, R, tg);
+    prestage_stem(in, xa, ws, bs, cg0, y0, x0, R, R, tg);
 }
 
 }  // namespace stages

@@ -74,16 +74,17 @@ struct Params {
     CUtensorMap map_in, map_t, map_aux, map_a_hi, map_a_lo, map_w_hi, map_w_lo;
     const float* w9;                          // [9][cin] depthwise taps * (kActSplitScale * sqrt 2)
     const float* bias;                        // [cin]              * (kActSplitScale * sqrt 2)
-    const float* noise;
+    const float* noise;                       // [H][noise_pitch]
     float* out;                               // NHWC output
     float inv_scale;
-    int n, H, W, cin, cout;
+    int n, H, W, cin, cout, noise_pitch;
     int act, passes;
     int source;                               // SepconvSource
     int tile_n, tile_h, tile_w, n_tile;      // n_tile = output channels per N tile (64 or 128)
-    int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / n_tile
+    int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / n_tile; tiles_x = ceil(W / tile_w) ...
     int n_group;                              // N tiles per CTA tile (power of two; > 1: stationary A)
-    int l_tx, l_ty, l_nt;                     // log2 of tiles_x, tiles_y, num_n_tiles / n_group (all powers of two: no runtime division)
+    int l_nt;                                 // log2 of num_n_tiles / n_group (a power of two)
+    FastDiv div_tx, div_ty;                   // by tiles_x / tiles_y (not powers of two at a rectangular extent)
     int num_kb;                               // cin / 64
     int in_stages, a_stages, b_stages, b_resident;
     uint32_t in_tx_bytes;                     // bytes the TMA unit delivers per input stage
@@ -186,10 +187,6 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, 
     asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
                  ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -243,14 +240,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
 struct TileCoord {
     int n0, y0, x0, nt;   // first image / row / column of the M tile, first N tile of the CTA tile's group
 };
+// Every source uses spatial tiles (tile_n images x tile_h rows x tile_w columns = 128 pixels).  The tile counts are not
+// powers of two once the extents are not: two multiply-high divisions per tile (FastDiv), few registers -- the producer
+// warpgroup decodes tiles under a 40-register budget.
 __device__ __forceinline__ TileCoord decode_tile(const Params& p, int tile) {
     TileCoord c;
     c.nt = (tile & ((1 << p.l_nt) - 1)) * p.n_group;
-    int m = tile >> p.l_nt;
-    c.x0 = (m & (p.tiles_x - 1)) * p.tile_w;
-    m >>= p.l_tx;
-    c.y0 = (m & (p.tiles_y - 1)) * p.tile_h;
-    c.n0 = (m >> p.l_ty) * p.tile_n;
+    const uint32_t m = (uint32_t)tile >> p.l_nt;
+    const uint32_t q = p.div_tx.div(m), q2 = p.div_ty.div(q);
+    c.x0 = (int)(m - q * p.div_tx.d) * p.tile_w;
+    c.y0 = (int)(q - q2 * p.div_ty.d) * p.tile_h;
+    c.n0 = (int)q2 * p.tile_n;
     return c;
 }
 
@@ -359,8 +359,8 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
             const int h = r >> 1, i = r & 1;
             const int m = h * 64 + wq * 16 + (lane >> 2) + 8 * i;
             const int pimg = tc.n0 + m / hw, poy = tc.y0 + (m / p.tile_w) % p.tile_h, pox = tc.x0 + m % p.tile_w;
-            const bool valid = pimg < p.n;
-            const float nz = p.noise ? __ldg(p.noise + poy * p.W + pox) : 0.f;
+            const bool valid = pimg < p.n && poy < p.H && pox < p.W;   // partial tiles at the right / bottom edge
+            const float nz = (p.noise && valid) ? __ldg(p.noise + poy * p.noise_pitch + pox) : 0.f;
             const float nz_g = nz * kActGain;
             float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0 + 2 * (lane & 3);
             float s0 = 0.f, s1 = 0.f, s2 = 0.f;      // torgb partial sums over this thread's channels
@@ -496,9 +496,9 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                     if (++pf_g < 2) return;
                     pf_g = 0;
                 } else {
-                    const int row0 = ((blockIdx.x + pf_it * gridDim.x) >> p.l_nt) * kTileM;
-                    tma_prefetch_2d(&p.map_a_hi, pf_kb * kKBlock, row0);
-                    tma_prefetch_2d(&p.map_a_lo, pf_kb * kKBlock, row0);
+                    const TileCoord t2 = decode_tile(p, blockIdx.x + pf_it * gridDim.x);
+                    tma_prefetch_4d(&p.map_a_hi, pf_kb * kKBlock, t2.x0, t2.y0, t2.n0);
+                    tma_prefetch_4d(&p.map_a_lo, pf_kb * kKBlock, t2.x0, t2.y0, t2.n0);
                 }
                 if (++pf_kb == num_kb) { pf_kb = 0; ++pf_it; }
             };
@@ -534,9 +534,8 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                         mbar_wait<true>(empty_a(s), ra.phase ^ 1, 110 + s, p.error_flag);
                         ra.advance();
                         mbar_expect_tx(full_a(s), kAStage);
-                        const int row0 = ((blockIdx.x + it * gridDim.x) >> p.l_nt) * kTileM;
-                        tma_load_2d(smem_base + p.off_a + s * kAStage, &p.map_a_hi, full_a(s), kb * kKBlock, row0);
-                        tma_load_2d(smem_base + p.off_a + s * kAStage + kABytes, &p.map_a_lo, full_a(s), kb * kKBlock, row0);
+                        tma_load_4d(smem_base + p.off_a + s * kAStage, &p.map_a_hi, full_a(s), kb * kKBlock, tc.x0, tc.y0, tc.n0);
+                        tma_load_4d(smem_base + p.off_a + s * kAStage + kABytes, &p.map_a_lo, full_a(s), kb * kKBlock, tc.x0, tc.y0, tc.n0);
                     }
                     if (!p.b_resident || it == 0) {
                         const int s = p.b_resident ? kb : rb.stage;
@@ -567,8 +566,8 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
         const float* w9p = (p.off_dw != 0xFFFFFFFFu) ? reinterpret_cast<const float*>(smem_gen + p.off_dw) : p.w9;
         const float* bp = (p.off_dw != 0xFFFFFFFFu) ? w9p + 9 * p.cin : p.bias;
         const float* stem_tab = reinterpret_cast<const float*>(smem_gen + p.off_stem);
-        for (int it = 0; it < my_tiles; ++it) {
-            const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
+        int tile = blockIdx.x;
+        for (int it = 0; it < my_tiles; ++it, tile += gridDim.x) {
             for (int kb = 0; kb < num_kb; ++kb) {
                 const int s = rin.stage;
                 const int sa = ra.stage;
@@ -577,13 +576,17 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                 uint8_t* stage = smem_gen + p.off_in + s * p.in_stage_stride;
                 f4* sin = reinterpret_cast<f4*>(stage);
                 const int cg0 = kb * kKBlock + g * kChunkC;
+                // the tile origin is only needed by the pre-stages: decoded per chunk there, so that it is not held in
+                // registers across the depthwise stage (which runs at the prologue's register limit)
                 if (p.source == SEPCONV_SRC_UP) {
+                    const TileCoord tc = decode_tile(p, tile);
                     prestage_up(sin, reinterpret_cast<const f4*>(stage + p.off_t), reinterpret_cast<const float*>(stage + p.off_aux),
-                                p.up_taps, tc.y0, tc.x0, p.H, p.up_has_noise, tg);
+                                p.up_taps, tc.y0, tc.x0, p.H, p.W, p.up_has_noise, tg);
                     bar_sync_named(1 + g, 128);
                 } else if (p.source == SEPCONV_SRC_STEM) {
+                    const TileCoord tc = decode_tile(p, tile);
                     prestage_stem(sin, reinterpret_cast<const float*>(stage + p.off_aux), stem_tab, stem_tab + 4 * p.cin,
-                                  cg0, tc.y0, tc.x0, p.H, tg);
+                                  cg0, tc.y0, tc.x0, p.H, p.W, tg);
                     bar_sync_named(1 + g, 128);
                 }
                 mbar_wait(empty_a(sa), ra.phase ^ 1, 410 + sa, p.error_flag);
@@ -641,9 +644,9 @@ const char* encode_map(CUtensorMap* m, CUtensorMapDataType dt, int rank, const v
     return nullptr;
 }
 
-const char* encode_x_map(CUtensorMap* m, const void* x, int n, int res) {
-    const uint64_t dims[4] = {(uint64_t)res, (uint64_t)res, 4, (uint64_t)n};
-    const uint64_t str[3] = {(uint64_t)res * 4, (uint64_t)res * res * 4, (uint64_t)res * res * 16};
+const char* encode_x_map(CUtensorMap* m, const void* x, int n, int H, int W) {
+    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, 4, (uint64_t)n};
+    const uint64_t str[3] = {(uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)H * W * 16};
     const uint32_t box[4] = {(uint32_t)kAuxW, 10, 4, 1};
     return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
@@ -704,24 +707,33 @@ int grid_sms() {
 // Tiling, N grouping, ring depths and shared-memory layout of a launch.  They depend on the shapes, the source and
 // whether torgb is fused, never on a pointer, so the generator's planner can ask before it commits to fusing torgb.
 const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& smem_bytes) {
-    const int n = d.n, res = d.res, cin = d.cin, cout = d.cout;
+    const int n = d.n, h = d.h, w = d.w, cin = d.cin, cout = d.cout;
     if (cin % kKBlock != 0 || cout % 64 != 0) return "cin must be a multiple of 64 and cout of 64";
-    if (res < 4 || (res & (res - 1))) return "resolution must be a power of two >= 4";
+    if (h < 4 || w < 4) return "extents must be >= 4";
+    if ((d.noise || d.up_noise) && (d.noise_pitch < w || d.noise_pitch % 4 != 0)) return "noise pitch must be >= w and a multiple of 4";
     p.source = d.source;
     const bool dw = (d.source != SEPCONV_SRC_SPLIT);
-    if ((d.source == SEPCONV_SRC_UP || d.source == SEPCONV_SRC_STEM) && res < 16) return "fused prologues need 8 x 16 tiles (res >= 16)";
-    p.n = n; p.H = res; p.W = res; p.cin = cin; p.cout = cout; p.act = d.act; p.passes = d.passes;
+    if ((d.source == SEPCONV_SRC_UP || d.source == SEPCONV_SRC_STEM) && std::min(h, w) < 16) return "fused prologues need 8 x 16 tiles (extents >= 16)";
+    if (d.source == SEPCONV_SRC_STEM && w % 4 != 0) return "the stem prologue needs a width that is a multiple of 4 (16-byte x rows)";
+    p.n = n; p.H = h; p.W = w; p.cin = cin; p.cout = cout; p.act = d.act; p.passes = d.passes;
+    p.noise_pitch = d.noise_pitch;
     p.n_tile = (cout == 64 || d.passes == 3) ? 64 : kMaxTileN;   // main + corr of 64 channels fill the accumulators
     p.num_kb = cin / kKBlock;
+    // Tile shapes are picked from the largest powers of two that fit the extents (at a square power-of-two level: the
+    // level's side), so a level keeps its R x R tiling whatever its rectangular extent; the last tile of a row / column may
+    // be partial.
+    auto p2floor = [](int v) { int q = 1; while (2 * q <= v) q *= 2; return q; };
     if (dw) {   // spatial tiles with halo
-        p.tile_w = res >= 16 ? 16 : res;
-        p.tile_h = res >= 8 ? 8 : res;
-    } else {    // linear tiles (rows of the [P][cin] operand) expressed as a 4-D box for the store
-        p.tile_w = res >= 128 ? 128 : res;
-        p.tile_h = std::min(res, kTileM / p.tile_w);
+        const int m = p2floor(std::min(h, w));
+        p.tile_w = std::min(m, 16);
+        p.tile_h = std::min(m, 8);
+    } else {    // the pre-split operand: whole 128-pixel rows where the width allows (contiguous TMA boxes)
+        p.tile_w = std::min(p2floor(w), 128);
+        p.tile_h = std::min(p2floor(h), kTileM / p.tile_w);
     }
     p.tile_n = kTileM / (p.tile_w * p.tile_h);
-    p.tiles_x = res / p.tile_w; p.tiles_y = res / p.tile_h; p.tiles_n = (n + p.tile_n - 1) / p.tile_n;
+    p.tiles_x = (w + p.tile_w - 1) / p.tile_w; p.tiles_y = (h + p.tile_h - 1) / p.tile_h; p.tiles_n = (n + p.tile_n - 1) / p.tile_n;
+    p.div_tx = FastDiv((uint32_t)p.tiles_x); p.div_ty = FastDiv((uint32_t)p.tiles_y);
     const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
     // Few pixel tiles (the 4 x 4 ... 16 x 16 levels at small batches): most SMs would idle while a few CTAs stream the
     // weight matrix.  Narrow N tiles spread the layer over 2 x the CTAs.
@@ -729,7 +741,6 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
         p.n_tile = 64;
     p.num_n_tiles = cout / p.n_tile;
     auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
-    p.l_tx = ilog2(p.tiles_x); p.l_ty = ilog2(p.tiles_y);
 
     // ---- input stage: IN area (+ T, NZ | XA) ----
     const uint32_t in_chunk_bytes = (uint32_t)(p.tile_n * (p.tile_h + 2) * (p.tile_w + 2) * kChunkC * 4);
@@ -827,7 +838,7 @@ bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d) {
 const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     Params p;
     memset(&p, 0, sizeof(p));
-    const int n = d.n, res = d.res, cin = d.cin, cout = d.cout;
+    const int n = d.n, h = d.h, w = d.w, cin = d.cin, cout = d.cout;
     const bool dw = (d.source != SEPCONV_SRC_SPLIT);
     if (d.source == SEPCONV_SRC_SPLIT && !(d.a_hi && d.a_lo)) return "no A operand";
     if ((d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) && !d.in_f32) return "no input tensor";
@@ -851,32 +862,31 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
 
     // ---- tensor maps ----
     const char* err = nullptr;
-    const uint64_t P = (uint64_t)n * res * res;
     if (d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) {
-        const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)res, (uint64_t)res, (uint64_t)n};
-        const uint64_t str[3] = {(uint64_t)cin * 4, (uint64_t)res * cin * 4, (uint64_t)res * res * cin * 4};
+        const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)w, (uint64_t)h, (uint64_t)n};
+        const uint64_t str[3] = {(uint64_t)cin * 4, (uint64_t)w * cin * 4, (uint64_t)h * w * cin * 4};
         const uint32_t box[4] = {(uint32_t)kChunkC, (uint32_t)p.tile_w + 2, (uint32_t)p.tile_h + 2, (uint32_t)p.tile_n};
         if ((err = encode_map(&p.map_in, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.in_f32, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE))) return err;
     }
     if (d.source == SEPCONV_SRC_UP) {
-        const int h = res / 2;
-        const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)h, (uint64_t)h, (uint64_t)n};
-        const uint64_t str[3] = {(uint64_t)cin * 4, (uint64_t)h * cin * 4, (uint64_t)h * h * cin * 4};
+        const int hl = h / 2, wl = w / 2;
+        const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)wl, (uint64_t)hl, (uint64_t)n};
+        const uint64_t str[3] = {(uint64_t)cin * 4, (uint64_t)wl * cin * 4, (uint64_t)hl * wl * cin * 4};
         const uint32_t box[4] = {(uint32_t)kChunkC, 10, 6, 1};
         if ((err = encode_map(&p.map_t, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.up_t, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE))) return err;
         if (p.up_has_noise) {
-            const uint64_t nd[2] = {(uint64_t)res, (uint64_t)res};
-            const uint64_t ns[1] = {(uint64_t)res * 4};
+            const uint64_t nd[2] = {(uint64_t)w, (uint64_t)h};
+            const uint64_t ns[1] = {(uint64_t)d.noise_pitch * 4};
             const uint32_t nb[2] = {(uint32_t)kAuxW, 10};
             if ((err = encode_map(&p.map_aux, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, d.up_noise, nd, ns, nb, CU_TENSOR_MAP_SWIZZLE_NONE))) return err;
         }
     }
-    if (d.source == SEPCONV_SRC_SPLIT) {
-        const uint64_t dims[2] = {(uint64_t)cin, P};
-        const uint64_t str[1] = {(uint64_t)cin * 2};
-        const uint32_t box[2] = {(uint32_t)kKBlock, (uint32_t)kTileM};
-        if ((err = encode_map(&p.map_a_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.a_hi, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
-        if ((err = encode_map(&p.map_a_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.a_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
+    if (d.source == SEPCONV_SRC_SPLIT) {   // one 64-channel K block of a spatial tile: 128 rows of 128 bytes, in tile order
+        const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)w, (uint64_t)h, (uint64_t)n};
+        const uint64_t str[3] = {(uint64_t)cin * 2, (uint64_t)w * cin * 2, (uint64_t)h * w * cin * 2};
+        const uint32_t box[4] = {(uint32_t)kKBlock, (uint32_t)p.tile_w, (uint32_t)p.tile_h, (uint32_t)p.tile_n};
+        if ((err = encode_map(&p.map_a_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d.a_hi, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
+        if ((err = encode_map(&p.map_a_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, d.a_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
     }
     {
         const uint64_t dims[2] = {(uint64_t)cin, (uint64_t)cout};
@@ -903,7 +913,8 @@ const char* sepconv_tc_plan(SepconvTcArgs* args, int passes, const float* in_f32
     d.passes = passes;
     d.source = in_f32 ? SEPCONV_SRC_NHWC : SEPCONV_SRC_SPLIT;
     d.in_f32 = in_f32; d.a_hi = a_hi; d.a_lo = a_lo; d.w9 = w9; d.bias = bias; d.w_hi = w_hi; d.w_lo = w_lo;
-    d.inv_scale = inv_scale; d.noise = noise; d.out = out; d.n = n; d.res = res; d.cin = cin; d.cout = cout; d.act = act; d.rgb = rgb;
+    d.inv_scale = inv_scale; d.noise = noise; d.out = out; d.n = n; d.h = res; d.w = res; d.cin = cin; d.cout = cout; d.act = act; d.rgb = rgb;
+    d.noise_pitch = res;
     return sepconv_tc_plan_ex(args, d);
 }
 
@@ -912,7 +923,7 @@ cudaError_t launch_sepconv_tc(SepconvTcArgs& a, cudaStream_t s, float* img_out_o
     if (pp->source == SEPCONV_SRC_STEM) {
         if (!x_nchw) return cudaErrorInvalidValue;
         if (a.bound_x != x_nchw) {    // the caller's x changes between calls: re-point the input tensor map
-            if (encode_x_map(&pp->map_aux, x_nchw, pp->n, pp->H)) return cudaErrorInvalidValue;
+            if (encode_x_map(&pp->map_aux, x_nchw, pp->n, pp->H, pp->W)) return cudaErrorInvalidValue;
             a.bound_x = x_nchw;
         }
     }

@@ -22,18 +22,20 @@ struct SepconvTcRgb {
     const float* w;       // [3][cout]
     const float* b;       // [3]
     const float* fir;     // [16][3] taps of the image up-sampling (unused if img_lo == null)
-    const float* img_lo;  // [n][3][res/2][res/2] planar or null
-    float* img_out;       // [n][3][res][res] planar (may be overridden at launch: the caller's y)
+    const float* img_lo;  // [n][3][h/2][w/2] planar or null
+    float* img_out;       // [n][3][h][w] planar (may be overridden at launch: the caller's y)
     int store_out;        // 0: do not write the feature map (last block)
 };
 
-// Where the depthwise conv's input (or the A operand itself) comes from.
+// Where the depthwise conv's input (or the A operand itself) comes from.  Every tensor is [n, h, w, ...]: h and w need not
+// be equal or powers of two (a fully convolutional forward); tiles that reach past the right / bottom edge are zero-filled
+// on load and masked on store.
 enum SepconvSource {
-    SEPCONV_SRC_NHWC = 0,   // in_f32: NHWC fp32 tensor [n, res, res, cin] (TMA tile + halo)
-    SEPCONV_SRC_SPLIT = 1,  // a_hi / a_lo: pre-split fp16 operand [n*res*res][cin] loaded by TMA (no prologue)
-    SEPCONV_SRC_UP = 2,     // in_f32 = skip tensor [n,res,res,cin]; x = lrelu_agc(up2(up_t) + noise) + skip is rebuilt
-                            // in shared memory from up_t [n,res/2,res/2,cin] (the previous layer's raw 1x1 output)
-    SEPCONV_SRC_STEM = 3,   // x NCHW [n,4,res,res] (bound at launch); fromrgb + activation recomputed on the halo
+    SEPCONV_SRC_NHWC = 0,   // in_f32: NHWC fp32 tensor [n, h, w, cin] (TMA tile + halo)
+    SEPCONV_SRC_SPLIT = 1,  // a_hi / a_lo: pre-split fp16 operand [n, h, w, cin] loaded by TMA (no prologue)
+    SEPCONV_SRC_UP = 2,     // in_f32 = skip tensor [n,h,w,cin]; x = lrelu_agc(up2(up_t) + noise) + skip is rebuilt
+                            // in shared memory from up_t [n,h/2,w/2,cin] (the previous layer's raw 1x1 output)
+    SEPCONV_SRC_STEM = 3,   // x NCHW [n,4,h,w] (bound at launch); fromrgb + activation recomputed on the halo
 };
 
 struct SepconvTcDesc {
@@ -47,13 +49,14 @@ struct SepconvTcDesc {
     const __half* w_hi = nullptr;   // [cout][cin] fp16 hi / lo of w * 2^k
     const __half* w_lo = nullptr;
     float inv_scale = 1.f;
-    const float* noise = nullptr;   // [res][res] added before the epilogue activation
-    float* out = nullptr;           // [n, res, res, cout] NHWC fp32
-    int n = 0, res = 0, cin = 0, cout = 0, act = 0;
+    const float* noise = nullptr;   // [h][noise_pitch] added before the epilogue activation
+    float* out = nullptr;           // [n, h, w, cout] NHWC fp32
+    int n = 0, h = 0, w = 0, cin = 0, cout = 0, act = 0;
+    int noise_pitch = 0;            // row pitch (floats, a multiple of 4) of noise and up_noise
     const SepconvTcRgb* rgb = nullptr;
     // SEPCONV_SRC_UP
     const float* up_t = nullptr;
-    const float* up_noise = nullptr;   // [res][res] * sqrt2 or null
+    const float* up_noise = nullptr;   // [h][noise_pitch] * sqrt2 or null
     float up_taps[16] = {0};           // 4x4 FIR taps * sqrt2 (channel-uniform)
     // SEPCONV_SRC_STEM
     const float* stem_w = nullptr;     // [cin][4] * sqrt2
@@ -65,7 +68,7 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* a, const SepconvTcDesc& d);
 // Whether a launch with d's shapes and source can fuse torgb, i.e. hold all of cout in one CTA tile (d.rgb and the
 // pointers are not read).
 bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d);
-// Legacy form (plain / pre-split sources).
+// Legacy form (plain / pre-split sources, res x res).
 const char* sepconv_tc_plan(SepconvTcArgs* a, int passes, const float* in_f32, const __half* a_hi, const __half* a_lo,
                             const float* w9, const float* bias, const __half* w_hi, const __half* w_lo,
                             float inv_scale, const float* noise, float* out, int n, int res, int cin, int cout, int act,

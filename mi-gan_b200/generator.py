@@ -92,24 +92,39 @@ class _Engine:
 
     _STAGING_BYTES = {"graph": "migan_graph_staging_bytes", "host": "migan_host_staging_bytes", "u8": "migan_u8_staging_bytes"}
 
-    def workspace(self, n: int, kind: Optional[str] = None):
+    def workspace(self, n: int, kind: Optional[str] = None, hw=None):
         """kind: None (device forward), "graph" (captured forward: one staging slot), "host" (fp32 host-buffer call) or
-        "u8" (uint8 request call); the host-memory calls get two staging slots."""
-        key = (n, kind)
+        "u8" (uint8 request call); the host-memory calls get two staging slots.  hw = (H, W): the fully convolutional
+        forward at that extent (shape already accepted by `fullconv_workspace_bytes`)."""
+        key = (n, kind) if hw is None else (n, "fc", hw)
         ws = self.workspaces.get(key)
         if ws is None:
-            nbytes = self.lib.migan_workspace_bytes(self.handle, n)
+            if hw is not None:
+                nbytes = self.fullconv_workspace_bytes(n, *hw)
+            else:
+                nbytes = self.lib.migan_workspace_bytes(self.handle, n)
             if kind is not None:
                 nbytes += getattr(self.lib, self._STAGING_BYTES[kind])(self.handle, n)
-            raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
-            off = (-raw.data_ptr()) % 1024
-            ws = raw[off:off + nbytes]
+            # keep one batch size, and one fully convolutional extent: alternating shapes re-allocate (the plan is rebuilt
+            # for them anyway) instead of holding a workspace per shape; the released ones go before the new allocation
+            keep = {k: v for k, v in self.workspaces.items() if k[0] == n and not (hw is not None and k[1] == "fc")}
             if any(k[0] != n for k in self.workspaces):
                 # copies enqueued with wait=False may still be using a staging area that is about to be released
                 _abi.check(self.lib.migan_host_wait(self.handle))
-            self.workspaces = {k: v for k, v in self.workspaces.items() if k[0] == n}  # keep one batch size
+            self.workspaces = keep
+            raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
+            off = (-raw.data_ptr()) % 1024
+            ws = raw[off:off + nbytes]
             self.workspaces[key] = ws
         return ws
+
+    def fullconv_workspace_bytes(self, n: int, H: int, W: int) -> int:
+        """Workspace of an n x H x W fully convolutional forward; ValueError (naming the nearest valid sizes) for a shape
+        the model does not accept."""
+        nbytes = self.lib.migan_workspace_bytes_hw(self.handle, n, H, W)
+        if nbytes == 0:
+            raise ValueError(self.lib.migan_last_error().decode())
+        return nbytes
 
 
 class Generator(nn.Module):
@@ -276,6 +291,92 @@ class Generator(nn.Module):
             fn = eng.lib.migan_forward_u8 if wait else eng.lib.migan_forward_u8_async
             _abi.check(fn(eng.handle, img_u8.data_ptr(), mask_u8.data_ptr(), out.data_ptr(), n,
                           ws.data_ptr(), ws.numel(), _abi.path_id(self.path), stream))
+        return out
+
+    # -- fully convolutional forward --------------------------------------------------
+    def _validate_fc(self, x: torch.Tensor) -> torch.Tensor:
+        if not isinstance(x, torch.Tensor):
+            raise TypeError("x must be a torch.Tensor")
+        if x.dim() != 4 or x.shape[1] != 4:
+            raise RuntimeError("expected x of shape [N, 4, H, W] (mask-0.5, img*mask), got %s" % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise RuntimeError("migan_b200.Generator runs on H100 (sm_90a) only; got a %s tensor. "
+                               "There is no CPU fallback (the CPU oracle lives in oracle/ for tests)." % x.device)
+        if x.dtype != torch.float32:
+            raise RuntimeError("expected float32 input, got %s" % x.dtype)
+        p = next(self.parameters())
+        if p.device != x.device:
+            raise RuntimeError("input is on %s but the module parameters are on %s" % (x.device, p.device))
+        if x.shape[0] == 0:
+            raise RuntimeError("empty batch")
+        return x.contiguous()
+
+    @torch.no_grad()
+    def forward_fc(self, x: torch.Tensor, tap: Optional[str] = None):
+        """Fully convolutional forward: x [N, 4, H, W] -> img [N, 3, H, W] for H, W >= R that are multiples of R/4.
+
+        Level r of the network runs at (H r/R, W r/R) with its own weights; each noise plane is the layer's noise_const
+        tiled over that extent (noise[i, j] = noise_const[i mod r, j mod r] * noise_strength) and every Upsample2d inserts
+        zeros at its output extent -- the reference's forward with `filter_const` / `noise_const` made size-dependent.  At
+        H = W = R it returns the same bytes as `forward`.  A shape outside the rule (or whose largest activation,
+        N*H*W*ch(R) elements, reaches 2^31) raises ValueError before anything is allocated or enqueued.
+
+        tap: name of an intermediate (see `tap_names`); then returns (img, intermediate as NCHW at its level's extent).
+        Runs the launch sequence directly (no CUDA graph)."""
+        x = self._validate_fc(x)
+        n, _, H, W = x.shape
+        with torch.cuda.device(x.device):
+            eng = self._engine(x.device)
+            ws_bytes = eng.fullconv_workspace_bytes(n, H, W)      # ValueError for a refused shape
+            buf = None
+            if tap is not None:
+                shapes = dict(self.tap_names(x.device))
+                if tap not in shapes:
+                    raise ValueError("unknown tap %r" % tap)
+                c, h, w = shapes[tap]
+                R = self.resolution
+                buf = torch.zeros((n, c, h * H // R, w * W // R), dtype=torch.float32, device=x.device)
+            ws = eng.workspace(n, hw=(H, W))
+            y = torch.empty((n, 3, H, W), dtype=torch.float32, device=x.device)
+            stream = torch.cuda.current_stream(x.device).cuda_stream
+            if buf is not None:
+                _abi.check(eng.lib.migan_set_tap(eng.handle, tap.encode(), buf.data_ptr()))
+            try:
+                _abi.check(eng.lib.migan_forward_hw(eng.handle, x.data_ptr(), y.data_ptr(), n, H, W, ws.data_ptr(), ws_bytes,
+                                                    _abi.path_id(self.path), stream))
+            finally:
+                if buf is not None:
+                    eng.lib.migan_set_tap(eng.handle, None, None)
+        return y if tap is None else (y, buf)
+
+    @torch.no_grad()
+    def forward_fc_u8(self, img_u8: torch.Tensor, mask_u8: torch.Tensor) -> torch.Tensor:
+        """scripts/demo.py's request at the photo's own size, on the device: img_u8 [N, H, W, 3] RGB and mask_u8 [N, H, W]
+        (255 = known) are CUDA uint8 tensors; returns the composed uint8 [N, H, W, 3] on the same device (known pixels of
+        img, generated pixels elsewhere).  preprocess -> forward_fc -> (y * 0.5 + 0.5).clamp(0, 1) * 255 -> uint8 ->
+        composite; H and W follow forward_fc's rule."""
+        if not (img_u8.is_cuda and mask_u8.is_cuda) or img_u8.dtype != torch.uint8 or mask_u8.dtype != torch.uint8:
+            raise RuntimeError("forward_fc_u8 expects CUDA uint8 tensors")
+        if img_u8.dim() != 4 or img_u8.shape[3] != 3 or tuple(mask_u8.shape) != tuple(img_u8.shape[:3]):
+            raise RuntimeError("forward_fc_u8 expects img [N, H, W, 3] and mask [N, H, W], got %s and %s"
+                               % (tuple(img_u8.shape), tuple(mask_u8.shape)))
+        if img_u8.device != mask_u8.device:
+            raise RuntimeError("img and mask are on different devices")
+        n, H, W, _ = img_u8.shape
+        if n == 0:
+            raise RuntimeError("empty batch")
+        img_u8, mask_u8 = img_u8.contiguous(), mask_u8.contiguous()
+        dev = img_u8.device
+        with torch.cuda.device(dev):
+            eng = self._engine(dev)
+            eng.fullconv_workspace_bytes(n, H, W)                   # ValueError before anything is enqueued
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            x = torch.empty((n, 4, H, W), dtype=torch.float32, device=dev)
+            _abi.check(eng.lib.b200_preprocess_u8_hw(img_u8.data_ptr(), mask_u8.data_ptr(), x.data_ptr(), n, H, W, stream))
+            y = self.forward_fc(x)
+            out = torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev)
+            _abi.check(eng.lib.b200_postprocess_u8_hw(y.data_ptr(), img_u8.data_ptr(), mask_u8.data_ptr(), out.data_ptr(),
+                                                      n, H, W, stream))
         return out
 
     def host_wait(self) -> None:
