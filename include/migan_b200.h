@@ -228,6 +228,34 @@ int b200_demo_preprocess(const migan_demo_request* reqs_host, int n, int resolut
 int b200_demo_postprocess(const float* y_n3rr, const migan_demo_request* reqs_host, int n, int resolution, void* scratch,
                           size_t scratch_bytes, void* stream);
 
+/* Full-resolution request path: a photo of ANY size (H, W >= 1) inpainted at its own resolution by migan_forward_hw.
+ *   migan_fullres_extent   the padded extent Hp = max(R, q ceil(H / q)), Wp likewise (q = R / 4): the smallest size
+ *                          migan_forward_hw accepts that holds the photo (a valid size is not padded), and the largest batch
+ *                          migan_forward_hw accepts there.  MIGAN_ERR_INVALID when one photo alone is too large for a forward.
+ *   b200_fullres_preprocess   photo + mask -> x of each request: the photo at the origin, padded on the bottom and right by
+ *                          numpy's np.pad(mode="reflect") rule (no edge repeat, iterated when the pad is longer than the side;
+ *                          a 1-pixel side replicates).  The mask's per-pixel steps are read_mask's without its resize (channel:
+ *                          alpha of LA / RGBA, R of RGB, L; 255 - v if invert; v < 255 -> 0) and the known-mask is reflected
+ *                          with the photo: x = cat([mask - 0.5, img * mask]) at Hp x Wp.
+ *   [migan_forward_hw at Hp x Wp, one call per chunk of requests that share an extent]
+ *   b200_fullres_postprocess  y -> (y*0.5+0.5).clamp(0,1)*255 -> uint8 on the top-left H x W; known pixels from the photo.
+ * The result is byte for byte b200_preprocess_u8_hw -> migan_forward_hw -> b200_postprocess_u8_hw on the host-padded photo
+ * and known-mask, cropped to H x W (at a valid size: on the photo itself).  reqs_host is a HOST array of 1..MIGAN_PIPE_MAX_BATCH
+ * requests of any sizes and extents; each call is one launch. */
+typedef struct {
+    const uint8_t* img;    /* DEVICE u8 [H][W][3] */
+    const uint8_t* mask;   /* DEVICE u8 [H][W][mask_channels]: 1 (L), 2 (LA), 3 (RGB) or 4 (RGBA) */
+    int H, W, mask_channels;
+    int invert;            /* non-zero: 255 - v before the threshold */
+    float* x;              /* DEVICE, 16-byte aligned: the request's slot [4][Hp][Wp] of its chunk's x [n,4,Hp,Wp] */
+    const float* y;        /* DEVICE: the request's slot [3][Hp][Wp] of its chunk's y [n,3,Hp,Wp] */
+    int Hp, Wp;            /* migan_fullres_extent(H, W); at least H x W */
+    uint8_t* out;          /* DEVICE u8 [H][W][3], written by b200_fullres_postprocess */
+} migan_fullres_request;
+int migan_fullres_extent(const migan_ctx* ctx, int H, int W, int* Hp, int* Wp, int* max_n);
+int b200_fullres_preprocess(const migan_fullres_request* reqs_host, int n, void* stream);
+int b200_fullres_postprocess(const migan_fullres_request* reqs_host, int n, void* stream);
+
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0
  * (k = 1).  w_dev: HOST array of k DEVICE pointers to [cout][fan] fp32 tensors (fan = cin/groups * kh * kw); out: device.
@@ -247,7 +275,9 @@ int b200_memcpy_async(void* dst, const void* src, size_t bytes, void* stream);
  * devices' memory then go directly over NVLink instead of being staged. */
 int b200_enable_peer_access(int peer_device);
 
-/* Kernels launched by the most recent migan_forward on this context. */
+/* Kernels launched by the most recent migan_forward on this context.
+ * Execution plans (tensor maps, tile grids, noise-plane tables) are cached per (n, path, workspace, H, W), up to 8 of them,
+ * least recently used first out; new weights clear the cache.  The profiling calls below report the plan of the last forward. */
 int migan_last_launch_count(const migan_ctx* ctx);
 
 /* Per-launch timing for roofline reports: when enabled, every kernel launch of subsequent

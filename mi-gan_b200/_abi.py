@@ -25,6 +25,12 @@ class DemoRequest(ctypes.Structure):
                 ("mask_channels", c_int), ("invert", c_int), ("out", c_void_p), ("out_w", c_int), ("out_h", c_int)]
 
 
+class FullResRequest(ctypes.Structure):
+    """migan_fullres_request: one request of the full-resolution request path (b200_fullres_*)."""
+    _fields_ = [("img", c_void_p), ("mask", c_void_p), ("H", c_int), ("W", c_int), ("mask_channels", c_int),
+                ("invert", c_int), ("x", c_void_p), ("y", c_void_p), ("Hp", c_int), ("Wp", c_int), ("out", c_void_p)]
+
+
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("migan_last_error", c_char_p, []),
@@ -71,6 +77,9 @@ SYMBOLS = [
     ("b200_demo_scratch_bytes", c_size_t, [POINTER(DemoRequest), c_int, c_int]),
     ("b200_demo_preprocess", c_int, [POINTER(DemoRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_demo_postprocess", c_int, [c_void_p, POINTER(DemoRequest), c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    ("migan_fullres_extent", c_int, [c_void_p, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
+    ("b200_fullres_preprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
+    ("b200_fullres_postprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

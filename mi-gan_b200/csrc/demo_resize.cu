@@ -28,7 +28,7 @@
 //   -> OpenCV height pass + composite.
 // Item kernels (comod_kernels.cuh style): the emulation build (tests/emul/build_demo.py) runs the very same functors on
 // the CPU.  Every product and sum is rounded on its own (no FMA contraction), in double where the libraries use double.
-#include "comod_kernels.cuh"
+#include "prepost.cuh"
 #include "../../include/migan_b200.h"
 
 #include <cstdio>
@@ -175,13 +175,8 @@ CK_HD int64_t demo_tab_ints(const DemoReq& r, int R, DemoTabs* t) {
 }
 CK_HD DemoTabs demo_tabs(const DemoReq& r, int R) { DemoTabs t; demo_tab_ints(r, R, &t); return t; }
 
-// read_mask's per-pixel steps at one source pixel of the original mask: the channel (alpha of LA / RGBA, R of RGB, L),
-// 255 - v if invert, then v < 255 -> 0.  True where the result is 255 (known).
-CK_HD bool demo_known(const DemoReq& r, int y, int x) {
-    const int ch = r.C == 4 ? 3 : (r.C == 2 ? 1 : 0);
-    const int v = r.mask[((int64_t)y * r.Wm + x) * r.C + ch];
-    return r.invert ? v == 0 : v == 255;
-}
+// read_mask's per-pixel steps (prepost.cuh mask_known) at one source pixel of the original mask.
+CK_HD bool demo_known(const DemoReq& r, int y, int x) { return mask_known(r.mask, r.Wm, r.C, r.invert, y, x); }
 
 enum { DS_TABLES, DS_DOWN_W, DS_DOWN_H, DS_SQUARE, DS_POST_W, DS_OUT, DS_COUNT };
 CK_HD int64_t demo_items(int stage, const DemoReq& r, int R) {
@@ -298,11 +293,8 @@ struct DemoSquareK {
         const int64_t plane = (int64_t)R * R;
         float* x = b.x + (int64_t)k * 4 * plane + j;
         const float m = demo_known(r, t.mry[oy], t.mrx[ox]) ? 1.f : 0.f;                     // mask // 255   (:60)
-        x[0] = DM_FADD(m, -0.5f);                                                             // mask - 0.5    (:65)
-        for (int c = 0; c < 3; ++c) {
-            const float v = DM_FADD(DM_FDIV(DM_FMUL((float)pil_clip8(acc[c]), 2.f), 255.f), -1.f);    // img * 2 / 255 - 1  (:61)
-            x[(c + 1) * plane] = DM_FMUL(v, m);                                               // img * mask    (:65)
-        }
+        x[0] = pre_mask_value(m);
+        for (int c = 0; c < 3; ++c) x[(c + 1) * plane] = pre_img_value(pil_clip8(acc[c]), m);
     }
 };
 
@@ -323,11 +315,8 @@ struct DemoPostWK {
         int* o = r.ptmp + j * 3;
         for (int c = 0; c < 3; ++c) {
             int acc = 0;
-            for (int tp = 0; tp < 4; ++tp) {
-                float v = DM_FADD(DM_FMUL(y[(int64_t)c * R * R + dm_clamp(s - 1 + tp, 0, R - 1)], 0.5f), 0.5f);   // (:135)
-                v = DM_FMUL(fminf(fmaxf(v, 0.f), 1.f), 255.f);
-                acc += (int)(uint8_t)v * cx[tp];                                                                // .to(uint8)
-            }
+            for (int tp = 0; tp < 4; ++tp)
+                acc += (int)post_u8(y[(int64_t)c * R * R + dm_clamp(s - 1 + tp, 0, R - 1)]) * cx[tp];
             o[c] = acc;
         }
     }

@@ -1,0 +1,208 @@
+// Full-resolution request path: a photo of any size inpainted at its own resolution by the fully convolutional forward.
+//
+//   photo u8 [H][W][3] + mask u8 [H][W][C]  --reflect-pad (bottom / right) to Hp x Wp, mask per-pixel steps-->
+//   x [4][Hp][Wp] = cat([mask - 0.5, img * mask])  ->  forward_fc at Hp x Wp  ->  y [3][Hp][Wp]
+//   -> (y*0.5+0.5).clamp(0,1)*255 -> uint8 on the top-left H x W, known pixels from the photo -> out [H][W][3]
+//
+// The padded extent (migan_fullres_extent, migan_abi.cu) is the smallest valid forward_fc size that holds the photo.
+// Padded row i reads source row src(i) by numpy's np.pad(mode="reflect") rule (no edge repeat, iterated when the pad is
+// longer than the side; a 1-pixel side replicates), columns likewise.  The mask is reflected with the photo, so a hole
+// that touches the border continues into the pad as a hole instead of zeroed pixels marked known.
+//
+// A pass of up to MIGAN_PIPE_MAX_BATCH requests of mixed sizes is one launch per phase; the request table travels by
+// value in the kernel parameter (FullResBatch, < 4 KB) with the phase's item prefix, as in demo_resize.cu.  Each
+// request's x / y point at its slot of its chunk's tensors, so requests of different extents share the launch.
+// Item functors (comod_kernels.cuh style): the emulation build (tests/emul/build_fullres.py) runs them on the CPU.
+// The per-pixel arithmetic is prepost.cuh's, so the bytes equal forward_fc_u8's on the padded photo by construction.
+#include "prepost.cuh"
+#include "../../include/migan_b200.h"
+#ifndef MIGAN_EMULATE
+#include "kernels.h"
+#endif
+
+#include <cstdio>
+
+namespace comod {
+
+// np.pad(mode="reflect") source index of padded index i >= n of a side of n: with p = 2 (n - 1) and t = i mod p,
+// t if t < n else p - t.
+CK_HD int reflect_index(int i, int n) {
+    if (n == 1) return 0;
+    const int p = 2 * (n - 1), t = i % p;
+    return t < n ? t : p - t;
+}
+CK_HD int src_index(int i, int n) { return i < n ? i : reflect_index(i, n); }
+
+struct FullResReq {
+    const uint8_t* img; const uint8_t* mask; uint8_t* out;
+    float* x; const float* y;    // the request's slot of its chunk's x [n][4][Hp][Wp] / y [n][3][Hp][Wp]
+    int H, W, C, invert, Hp, Wp;
+};
+struct FullResBatch {
+    int64_t start[MIGAN_PIPE_MAX_BATCH + 1];   // item prefix of the launch
+    FullResReq r[MIGAN_PIPE_MAX_BATCH];
+    int n;
+    CK_HD int find(int64_t i) const {           // the request item i belongs to
+        int lo = 0, hi = n - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (start[mid] <= i) lo = mid; else hi = mid - 1;
+        }
+        return lo;
+    }
+};
+static_assert(sizeof(FullResBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
+
+CK_HD int64_t fullres_pre_items(const FullResReq& r) { return (int64_t)r.Hp * ((r.Wp + 3) / 4); }
+CK_HD int64_t fullres_post_items(const FullResReq& r) { return (int64_t)r.H * r.W; }
+
+// Four consecutive padded pixels of one row -> x.  items per request = Hp * ceil(Wp / 4).  16-byte stores to each plane
+// when Wp % 4 == 0 (always at R >= 16: Wp is a multiple of R / 4), scalar stores otherwise.
+struct FullResPreK {
+    const FullResBatch& b;
+    PP_D void operator()(int64_t i) const {
+        const int k = b.find(i);
+        const FullResReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int groups = (r.Wp + 3) >> 2;
+        const int row = (int)(j / groups);
+        const int x0 = (int)(j - (int64_t)row * groups) * 4;
+        const int sy = src_index(row, r.H);
+        const uint8_t* img_row = r.img + (int64_t)sy * r.W * 3;
+        const bool direct = x0 + 4 <= r.W;   // the four columns lie inside the photo
+        float m[4];                          // mask // 255 of the four pixels
+        const uint8_t* px[4];
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+            const int sx = direct ? x0 + p : src_index(x0 + p < r.Wp ? x0 + p : r.Wp - 1, r.W);
+            m[p] = mask_known(r.mask, r.W, r.C, r.invert, sy, sx) ? 1.f : 0.f;
+            px[p] = img_row + (int64_t)sx * 3;
+        }
+        // plane by plane, so that only one plane's four values are live across the divisions' slow-path calls
+        const int64_t plane = (int64_t)r.Hp * r.Wp;
+        float* xo = r.x + (int64_t)row * r.Wp + x0;
+        const bool vec = (r.Wp & 3) == 0;
+        const int cnt = r.Wp - x0;           // pixels of this group inside the row
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            float v[4];
+#pragma unroll
+            for (int p = 0; p < 4; ++p) v[p] = c == 0 ? pre_mask_value(m[p]) : pre_img_value(px[p][c - 1], m[p]);
+            if (vec) {
+                st4(xo + c * plane, f4{v[0], v[1], v[2], v[3]});
+            } else {
+#pragma unroll
+                for (int p = 0; p < 4; ++p)
+                    if (p < cnt) xo[c * plane + p] = v[p];
+            }
+        }
+    }
+};
+
+// One photo pixel: y (pitch Wp) -> uint8, composed with the photo's known pixels.  items per request = H * W
+struct FullResPostK {
+    const FullResBatch& b;
+    PP_D void operator()(int64_t i) const {
+        const int k = b.find(i);
+        const FullResReq& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int row = (int)(j / r.W), col = (int)(j - (int64_t)row * r.W);
+        const bool known = mask_known(r.mask, r.W, r.C, r.invert, row, col);
+        const int64_t plane = (int64_t)r.Hp * r.Wp;
+        const float* y = r.y + (int64_t)row * r.Wp + col;
+        uint8_t* o = r.out + j * 3;
+        const uint8_t* p = r.img + j * 3;
+        for (int c = 0; c < 3; ++c) o[c] = known ? p[c] : post_u8(y[c * plane]);
+    }
+};
+
+#ifdef MIGAN_EMULATE
+template <class F>
+inline int fullres_launch(const FullResBatch& b, ck_stream_t s) { return ck_launch(F{b}, b.start[b.n], s); }
+#else
+// One thread per item; __grid_constant__ lets the functors index the request table in the parameter space.
+template <class F>
+__global__ void __launch_bounds__(256) fullres_items_kernel(const __grid_constant__ FullResBatch b, const int64_t items) {
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i < items) F{b}(i);
+}
+template <class F>
+inline cudaError_t fullres_launch(const FullResBatch& b, ck_stream_t s) {
+    const int64_t items = b.start[b.n];
+    if (items <= 0) return cudaSuccess;
+    fullres_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(b, items);
+    return cudaGetLastError();
+}
+#endif
+
+}  // namespace comod
+
+namespace migan {
+
+namespace {
+
+comod::FullResBatch fullres_batch(const migan_fullres_request* q, int n, bool pre) {
+    comod::FullResBatch b;
+    b.n = n;
+    b.start[0] = 0;
+    for (int k = 0; k < n; ++k) {
+        comod::FullResReq& r = b.r[k];
+        r.img = q[k].img; r.mask = q[k].mask; r.out = q[k].out; r.x = q[k].x; r.y = q[k].y;
+        r.H = q[k].H; r.W = q[k].W; r.C = q[k].mask_channels; r.invert = q[k].invert != 0; r.Hp = q[k].Hp; r.Wp = q[k].Wp;
+        b.start[k + 1] = b.start[k] + (pre ? comod::fullres_pre_items(r) : comod::fullres_post_items(r));
+    }
+    return b;
+}
+
+}  // namespace
+
+int check_fullres_batch(const migan_fullres_request* q, int n, bool pre, char* msg, size_t len) {
+    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
+    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
+        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
+        return MIGAN_ERR_INVALID;
+    }
+    for (int k = 0; k < n; ++k) {
+        const migan_fullres_request& r = q[k];
+        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out)) {
+            snprintf(msg, len, "request %d: null photo, mask, %s", k, pre ? "or x" : "y or output");
+            return MIGAN_ERR_INVALID;
+        }
+        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) {
+            snprintf(msg, len, "request %d: x must be 16-byte aligned", k);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.H < 1 || r.W < 1 || r.Hp < r.H || r.Wp < r.W) {
+            snprintf(msg, len, "request %d: photo of %d x %d, padded extent %d x %d (H x W)", k, r.H, r.W, r.Hp, r.Wp);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.mask_channels < 1 || r.mask_channels > 4) {
+            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
+            return MIGAN_ERR_INVALID;
+        }
+    }
+    return MIGAN_OK;
+}
+
+int launch_fullres_preprocess(const migan_fullres_request* q, int n, ck_stream_t s) {
+    return (int)comod::fullres_launch<comod::FullResPreK>(fullres_batch(q, n, true), s);
+}
+
+int launch_fullres_postprocess(const migan_fullres_request* q, int n, ck_stream_t s) {
+    return (int)comod::fullres_launch<comod::FullResPostK>(fullres_batch(q, n, false), s);
+}
+
+}  // namespace migan
+
+#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
+static char g_fullres_msg[256];
+extern "C" const char* migan_emul_fullres_error(void) { return g_fullres_msg; }
+extern "C" int b200_fullres_preprocess(const migan_fullres_request* q, int n, void* s) {
+    if (int rc = migan::check_fullres_batch(q, n, true, g_fullres_msg, sizeof g_fullres_msg)) return rc;
+    return migan::launch_fullres_preprocess(q, n, s);
+}
+extern "C" int b200_fullres_postprocess(const migan_fullres_request* q, int n, void* s) {
+    if (int rc = migan::check_fullres_batch(q, n, false, g_fullres_msg, sizeof g_fullres_msg)) return rc;
+    return migan::launch_fullres_postprocess(q, n, s);
+}
+#endif

@@ -115,6 +115,11 @@ size_t demo_scratch_bytes(const migan_demo_request* reqs, int n, int res);
 int launch_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
 int launch_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, cudaStream_t s);
 
+// ---- full-resolution request path (fullres.cu): reflect padding and the composite around migan_forward_hw ------
+int check_fullres_batch(const migan_fullres_request* reqs, int n, bool pre, char* msg, size_t len);
+int launch_fullres_preprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
+int launch_fullres_postprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
+
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------
 int launch_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fan, float* out, cudaStream_t s);

@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <list>
 #include <map>
 #include <memory>
 #include <string>
@@ -185,7 +186,13 @@ struct migan_ctx {
     std::vector<ToRgb> torgb;
     void* arena = nullptr;
 
-    Plan plan;
+    // Execution plans per (n, path, workspace, H, W), most recently used first, at most kMaxPlans; `plan` is the last
+    // forward's (migan_profile_*).  A plan depends only on the weights and its key, so plans that share a workspace
+    // (different extents or batch sizes carved from the same memory) stay correct: every forward writes each workspace
+    // buffer before it reads it, and a fully convolutional forward re-tiles its noise planes (K_NOISE) each time.
+    static constexpr size_t kMaxPlans = 8;
+    std::list<Plan> plans;
+    const Plan* plan = nullptr;
     int last_launches = 0;
     std::string tap_name;
     float* tap_dst = nullptr;
@@ -595,7 +602,8 @@ int migan_finalize_weights(migan_ctx* ctx) {
     CUDA_TRY(cudaMalloc(&ctx->arena, ab.bytes.size()));
     CUDA_TRY(cudaMemcpy(ctx->arena, ab.bytes.data(), ab.bytes.size(), cudaMemcpyHostToDevice));
     for (auto& f : fix) *f.first = static_cast<unsigned char*>(ctx->arena) + f.second;
-    ctx->plan = Plan();  // pointers changed
+    ctx->plans.clear();  // pointers changed
+    ctx->plan = nullptr;
     if (ctx->graph_exec) { cudaGraphExecDestroy(ctx->graph_exec); ctx->graph_exec = nullptr; }
     ctx->finalized = true;
     return MIGAN_OK;
@@ -639,6 +647,7 @@ static size_t workspace_layout_bytes(const migan_ctx* ctx, int n, int H, int W) 
 // The sizes a fully convolutional forward accepts: H, W >= R and multiples of R / 4 (every level's extent is then an
 // integer and at least the level's side, and every up-sampling lands on its skip feature), and a largest activation
 // n * H * W * ch(R) below 2^31 elements (the kernels use 32-bit offsets and TMA coordinates).
+static int64_t max_batch(const migan_ctx* c, int H, int W) { return INT32_MAX / ((int64_t)H * W * channels(c->resolution)); }
 static int check_shape(const migan_ctx* c, int n, int H, int W) {
     const int R = c->resolution, q = R / 4;
     if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
@@ -649,10 +658,10 @@ static int check_shape(const migan_ctx* c, int n, int H, int W) {
                     "(R/4) and at least %d; nearest valid sizes: %d x %d and %d x %d", H, W, R, q, R, down(H), down(W), up(H), up(W));
     }
     const int64_t per_img = (int64_t)H * W * channels(R);
-    if ((int64_t)n * per_img > INT32_MAX)
+    if ((int64_t)n > max_batch(c, H, W))
         return fail(MIGAN_ERR_INVALID, "n x H x W x ch(R) = %d x %d x %d x %d = %lld elements in the largest activation is more than "
                     "2^31 - 1 (32-bit kernel offsets); at %d x %d the largest batch is %lld", n, H, W, channels(R),
-                    (long long)(n * per_img), H, W, (long long)(INT32_MAX / per_img));
+                    (long long)(n * per_img), H, W, (long long)max_batch(c, H, W));
     return MIGAN_OK;
 }
 
@@ -997,13 +1006,26 @@ struct PlanBuilder {
     }
 };
 
-int build_plan(migan_ctx* ctx, int n, int H, int W, int path, void* ws) {
-    PlanBuilder pb;
-    pb.c = ctx; pb.n = n; pb.H = H; pb.W = W; pb.path = path; pb.base = static_cast<unsigned char*>(ws);
-    int rc = pb.build();
-    if (rc) return rc;
-    ctx->plan.n = n; ctx->plan.path = path; ctx->plan.ws = ws; ctx->plan.H = H; ctx->plan.W = W;
-    ctx->plan.steps.swap(pb.steps);
+// The cached plan of (n, path, ws, H, W), built on a miss; it becomes the most recently used (and ctx->plan).
+int find_plan(migan_ctx* ctx, int n, int H, int W, int path, void* ws, Plan** out) {
+    auto& plans = ctx->plans;
+    auto it = std::find_if(plans.begin(), plans.end(), [&](const Plan& p) {
+        return p.n == n && p.path == path && p.ws == ws && p.H == H && p.W == W;
+    });
+    if (it != plans.end()) {
+        plans.splice(plans.begin(), plans, it);
+    } else {
+        PlanBuilder pb;
+        pb.c = ctx; pb.n = n; pb.H = H; pb.W = W; pb.path = path; pb.base = static_cast<unsigned char*>(ws);
+        int rc = pb.build();
+        if (rc) return rc;
+        Plan p;
+        p.n = n; p.path = path; p.ws = ws; p.H = H; p.W = W;
+        p.steps.swap(pb.steps);
+        plans.push_front(std::move(p));
+        if (plans.size() > migan_ctx::kMaxPlans) plans.pop_back();
+    }
+    ctx->plan = *out = &plans.front();
     return MIGAN_OK;
 }
 
@@ -1082,22 +1104,20 @@ static int forward_impl(migan_ctx* ctx, const float* x, float* y, int n, int H, 
     if ((reinterpret_cast<uintptr_t>(workspace) & 1023) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15))
         return fail(MIGAN_ERR_WORKSPACE, "workspace must be 1024-byte aligned, x / y 16-byte aligned");
     CUDA_TRY(cudaSetDevice(ctx->device));
-    // alternating shapes rebuild the plan (tensor maps, tile grids and noise planes depend on the extent)
-    if (ctx->plan.n != n || ctx->plan.path != path || ctx->plan.ws != workspace || ctx->plan.H != H || ctx->plan.W != W) {
-        int rc = build_plan(ctx, n, H, W, path, workspace);
-        if (rc) return rc;
-    }
+    // tensor maps, tile grids and noise planes depend on the extent: alternating shapes hit the plan cache
+    Plan* plan = nullptr;
+    if (int rc = find_plan(ctx, n, H, W, path, workspace, &plan)) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     ctx->last_launches = 0;
     if (ctx->profiling) {
-        while (ctx->events.size() < 2 * ctx->plan.steps.size()) {
+        while (ctx->events.size() < 2 * plan->steps.size()) {
             cudaEvent_t e;
             CUDA_TRY(cudaEventCreate(&e));
             ctx->events.push_back(e);
         }
     }
     size_t i = 0;
-    for (Step& s : ctx->plan.steps) {
+    for (Step& s : plan->steps) {
         if (ctx->profiling) CUDA_TRY(cudaEventRecord(ctx->events[2 * i], st));
         int rc = run_step(ctx, s, x, y, st);
         if (rc) return rc;
@@ -1178,11 +1198,11 @@ int migan_set_profiling(migan_ctx* ctx, int enable) {
     return MIGAN_OK;
 }
 
-int migan_profile_num_steps(const migan_ctx* ctx) { return ctx ? (int)ctx->plan.steps.size() : 0; }
+int migan_profile_num_steps(const migan_ctx* ctx) { return ctx && ctx->plan ? (int)ctx->plan->steps.size() : 0; }
 
 int migan_profile_step(migan_ctx* ctx, int index, const char** label, float* ms, double* alg_bytes, double* flops) {
-    if (!ctx || index < 0 || index >= (int)ctx->plan.steps.size()) return fail(MIGAN_ERR_INVALID, "bad step index %d", index);
-    const Step& s = ctx->plan.steps[index];
+    if (!ctx || index < 0 || index >= migan_profile_num_steps(ctx)) return fail(MIGAN_ERR_INVALID, "bad step index %d", index);
+    const Step& s = ctx->plan->steps[index];
     if (label) *label = s.label.c_str();
     if (alg_bytes) *alg_bytes = s.alg_bytes;
     if (flops) *flops = s.flops;
@@ -1544,6 +1564,39 @@ int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* 
     const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
     CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess_planned(y, reqs, n, res, k25, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+// The smallest extent forward_fc accepts that holds an H x W photo: each side rounded up to a multiple of R / 4, at least R.
+int migan_fullres_extent(const migan_ctx* ctx, int H, int W, int* Hp, int* Wp, int* max_n) {
+    if (!ctx || !Hp || !Wp || !max_n) return fail(MIGAN_ERR_INVALID, "fullres_extent: null argument");
+    if (H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "fullres_extent: photo of %d x %d (H x W)", H, W);
+    const int R = ctx->resolution, q = R / 4;
+    const int64_t hp = std::max<int64_t>(R, ((int64_t)H + q - 1) / q * q), wp = std::max<int64_t>(R, ((int64_t)W + q - 1) / q * q);
+    if (hp > INT32_MAX || wp > INT32_MAX || check_shape(ctx, 1, (int)hp, (int)wp))
+        return fail(MIGAN_ERR_INVALID, "photo of %d x %d (H x W) pads to %lld x %lld at resolution %d, too large for one forward: "
+                    "its largest activation, %lld x %lld x %d elements, reaches 2^31", H, W, (long long)hp, (long long)wp, R,
+                    (long long)hp, (long long)wp, channels(R));
+    *Hp = (int)hp; *Wp = (int)wp;
+    *max_n = (int)max_batch(ctx, *Hp, *Wp);
+    return MIGAN_OK;
+}
+
+static int check_fullres(const char* who, const migan_fullres_request* reqs, int n, bool pre) {
+    char msg[256];
+    if (int rc = migan::check_fullres_batch(reqs, n, pre, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+int b200_fullres_preprocess(const migan_fullres_request* reqs, int n, void* stream) {
+    if (int rc = check_fullres("fullres_preprocess", reqs, n, true)) return rc;
+    CUDA_TRY((cudaError_t)migan::launch_fullres_preprocess(reqs, n, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_fullres_postprocess(const migan_fullres_request* reqs, int n, void* stream) {
+    if (int rc = check_fullres("fullres_postprocess", reqs, n, false)) return rc;
+    CUDA_TRY((cudaError_t)migan::launch_fullres_postprocess(reqs, n, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 

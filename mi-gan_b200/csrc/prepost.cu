@@ -5,17 +5,10 @@
 // With these the host<->device traffic of a request is 4 + 3 bytes per pixel instead of 16 + 12.
 // Item kernels (one pixel per thread) in the comod_kernels.cuh style, so the emulation build checks them on the CPU.
 // Every product of the reference is rounded separately (no FMA contraction) to stay bit-exact with torch.
-#include "comod_kernels.cuh"
+#include "prepost.cuh"
 
-#ifdef MIGAN_EMULATE
-#define PP_MUL(a, b) ((a) * (b))
-#define PP_ADD(a, b) ((a) + (b))
-#define PP_DIV(a, b) ((a) / (b))
-#else
+#ifndef MIGAN_EMULATE
 #include "kernels.h"
-#define PP_MUL(a, b) __fmul_rn((a), (b))
-#define PP_ADD(a, b) __fadd_rn((a), (b))
-#define PP_DIV(a, b) __fdiv_rn((a), (b))
 #endif
 
 namespace comod {
@@ -31,11 +24,8 @@ struct PreU8K {        // items = n*H*W
         const int64_t n = i / HW, p = i - n * HW;
         const float m = mask[i] == 255 ? 1.f : 0.f;                        // mask // 255            (demo.py:60)
         float* xo = x + n * 4 * HW + p;
-        xo[0] = PP_ADD(m, -0.5f);                                          // mask - 0.5             (:65)
-        for (int c = 0; c < 3; ++c) {
-            const float v = PP_ADD(PP_DIV(PP_MUL((float)img[i * 3 + c], 2.f), 255.f), -1.f);   // img * 2 / 255 - 1  (:61)
-            xo[(c + 1) * HW] = PP_MUL(v, m);                               // img * mask             (:65)
-        }
+        xo[0] = pre_mask_value(m);
+        for (int c = 0; c < 3; ++c) xo[(c + 1) * HW] = pre_img_value(img[i * 3 + c], m);
     }
 };
 
@@ -49,12 +39,8 @@ struct PostU8K {       // items = n*H*W
     void operator()(int64_t i) const {
         const int64_t n = i / HW, p = i - n * HW;
         const bool known = mask[i] == 255;
-        for (int c = 0; c < 3; ++c) {
-            float t = PP_ADD(PP_MUL(y[(n * 3 + c) * HW + p], 0.5f), 0.5f);  // y * 0.5 + 0.5         (demo.py:135)
-            t = fminf(fmaxf(t, 0.f), 1.f);                                  // .clamp(0, 1)
-            t = PP_MUL(t, 255.f);
-            out[i * 3 + c] = known ? img[i * 3 + c] : (uint8_t)t;           // .to(uint8); img*mask + result*(1-mask)  (:136,140)
-        }
+        for (int c = 0; c < 3; ++c)                                         // img*mask + result*(1-mask)  (demo.py:140)
+            out[i * 3 + c] = known ? img[i * 3 + c] : post_u8(y[(n * 3 + c) * HW + p]);
     }
 };
 

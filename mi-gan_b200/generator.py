@@ -115,6 +115,12 @@ class _Engine:
             raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
             off = (-raw.data_ptr()) % 1024
             ws = raw[off:off + nbytes]
+            if kind in ("host", "u8"):
+                # The library fills these staging slots on its own copy streams, which it orders after the caller's
+                # stream only when a slot's address changes.  The caching allocator may return an address a slot used
+                # before while kernels queued on the caller's stream still use that memory (as another shape's
+                # workspace), so those kernels must finish before the first copy into the new workspace.
+                torch.cuda.current_stream(self.device).synchronize()
             self.workspaces[key] = ws
         return ws
 
