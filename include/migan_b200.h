@@ -256,6 +256,51 @@ int migan_fullres_extent(const migan_ctx* ctx, int H, int W, int* Hp, int* Wp, i
 int b200_fullres_preprocess(const migan_fullres_request* reqs_host, int n, void* stream);
 int b200_fullres_postprocess(const migan_fullres_request* reqs_host, int n, void* stream);
 
+/* Hole-window request path: only margin-padded windows around the holes of a photo of ANY size are inpainted, each at its
+ * own resolution by the full-resolution path; every other pixel keeps the photo's value.  With q = R / 4:
+ *   b200_hole_cells        the photo is split into q x q cells anchored at the origin (gh = ceil(H / q) rows by
+ *                          gw = ceil(W / q) columns; the last ones may be partial).  cells[cy * gw + cx] = 1 when the cell
+ *                          holds a hole pixel (not known by the full-resolution path's mask steps), else 0.  One launch for
+ *                          1..MIGAN_PIPE_MAX_BATCH requests (reqs_host: HOST array); request i's cells follow request i - 1's;
+ *                          b200_hole_cells_bytes gives the total (0 on a bad argument).  Each mask byte is read once.
+ *   migan_hole_windows     HOST: the windows of one request from a HOST copy of its cells, sorted by (y0, x0), as
+ *                          {y0, x0, h, w} quadruples in windows4 (room for max_windows).  On each axis (side n) a span of
+ *                          cells [c0, c1] with a margin of m cells gives a = max(0, (c0 - m) q), b = min(n, (c1 + 1 + m) q),
+ *                          L = min(n, max(R, q ceil((b - a) / q))), s = min(max(a - (L - (b - a)) / 2, 0), n - L) and the
+ *                          window [s, s + L).  The hole cells are visited in row-major order; each starts as its own span,
+ *                          and while its window overlaps (positive area) a window already listed, the first such window
+ *                          is removed and the spans are united; the result is appended.  The windows are disjoint, cover
+ *                          every hole pixel, and each side is a valid forward_fc size or the photo's side.
+ *   migan_hole_windows_max the most windows an H x W photo can have: floor(H / min(R, H)) * floor(W / min(R, W)).
+ *   b200_window_preprocess / b200_window_postprocess   the full-resolution pre- and post-processing of each window's crop
+ *                          (reflect padding of the crop to Hp x Wp = migan_fullres_extent(h, w), composite); the
+ *                          post-processing writes only the window's pixels of `out`, which holds a copy of the photo (it
+ *                          may be the photo itself).  One launch for 1..MIGAN_PIPE_MAX_BATCH windows of any requests.
+ * resolution: a power of two >= 8 (the generator's). */
+typedef struct {
+    const uint8_t* mask;   /* DEVICE u8 [H][W][mask_channels]: 1 (L), 2 (LA), 3 (RGB) or 4 (RGBA) */
+    int H, W, mask_channels;
+    int invert;            /* non-zero: 255 - v before the threshold */
+} migan_cells_request;
+size_t b200_hole_cells_bytes(const migan_cells_request* reqs_host, int n, int resolution);
+int b200_hole_cells(const migan_cells_request* reqs_host, int n, int resolution, uint8_t* cells, void* stream);
+int migan_hole_windows(const uint8_t* cells_host, int H, int W, int resolution, int margin, int* windows4, int max_windows,
+                       int* count);
+int migan_hole_windows_max(int H, int W, int resolution, int* max_windows);
+typedef struct {
+    const uint8_t* img;    /* DEVICE u8 [H][W][3]: the photo */
+    const uint8_t* mask;   /* DEVICE u8 [H][W][mask_channels] */
+    int H, W, mask_channels;
+    int invert;            /* non-zero: 255 - v before the threshold */
+    int y0, x0, h, w;      /* the window, inside the photo */
+    float* x;              /* DEVICE, 16-byte aligned: the window's slot [4][Hp][Wp] of its chunk's x [n,4,Hp,Wp] */
+    const float* y;        /* DEVICE: the window's slot [3][Hp][Wp] of its chunk's y [n,3,Hp,Wp] */
+    int Hp, Wp;            /* migan_fullres_extent(h, w) */
+    uint8_t* out;          /* DEVICE u8 [H][W][3]: a copy of the photo (or the photo); the window is written */
+} migan_window_request;
+int b200_window_preprocess(const migan_window_request* reqs_host, int n, void* stream);
+int b200_window_postprocess(const migan_window_request* reqs_host, int n, void* stream);
+
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0
  * (k = 1).  w_dev: HOST array of k DEVICE pointers to [cout][fan] fp32 tensors (fan = cin/groups * kh * kw); out: device.

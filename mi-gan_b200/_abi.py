@@ -31,6 +31,18 @@ class FullResRequest(ctypes.Structure):
                 ("invert", c_int), ("x", c_void_p), ("y", c_void_p), ("Hp", c_int), ("Wp", c_int), ("out", c_void_p)]
 
 
+class CellsRequest(ctypes.Structure):
+    """migan_cells_request: one mask of b200_hole_cells."""
+    _fields_ = [("mask", c_void_p), ("H", c_int), ("W", c_int), ("mask_channels", c_int), ("invert", c_int)]
+
+
+class WindowRequest(ctypes.Structure):
+    """migan_window_request: one window of the hole-window request path (b200_window_*)."""
+    _fields_ = [("img", c_void_p), ("mask", c_void_p), ("H", c_int), ("W", c_int), ("mask_channels", c_int),
+                ("invert", c_int), ("y0", c_int), ("x0", c_int), ("h", c_int), ("w", c_int), ("x", c_void_p),
+                ("y", c_void_p), ("Hp", c_int), ("Wp", c_int), ("out", c_void_p)]
+
+
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("migan_last_error", c_char_p, []),
@@ -80,6 +92,12 @@ SYMBOLS = [
     ("migan_fullres_extent", c_int, [c_void_p, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     ("b200_fullres_preprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
     ("b200_fullres_postprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
+    ("b200_hole_cells_bytes", c_size_t, [POINTER(CellsRequest), c_int, c_int]),
+    ("b200_hole_cells", c_int, [POINTER(CellsRequest), c_int, c_int, c_void_p, c_void_p]),
+    ("migan_hole_windows", c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_int, POINTER(c_int)]),
+    ("migan_hole_windows_max", c_int, [c_int, c_int, c_int, POINTER(c_int)]),
+    ("b200_window_preprocess", c_int, [POINTER(WindowRequest), c_int, c_void_p]),
+    ("b200_window_postprocess", c_int, [POINTER(WindowRequest), c_int, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

@@ -14,6 +14,8 @@
 // request's x / y point at its slot of its chunk's tensors, so requests of different extents share the launch.
 // Item functors (comod_kernels.cuh style): the emulation build (tests/emul/build_fullres.py) runs them on the CPU.
 // The per-pixel arithmetic is prepost.cuh's, so the bytes equal forward_fc_u8's on the padded photo by construction.
+// The hole-window path (holewin.cu) runs the same functors on windows of a photo (b200_window_*): a request is an H x W
+// crop at the photo's row pitch, reflect-padded within the crop, and the post-processing writes only the crop.
 #include "prepost.cuh"
 #include "../../include/migan_b200.h"
 #ifndef MIGAN_EMULATE
@@ -33,9 +35,12 @@ CK_HD int reflect_index(int i, int n) {
 }
 CK_HD int src_index(int i, int n) { return i < n ? i : reflect_index(i, n); }
 
+// One request: an H x W window of a photo whose rows are `pitch` pixels apart.  img / mask / out point at the window's
+// top-left pixel (the window origin is applied on the host), so a whole photo is the window (0, 0, H, W), pitch = W.
 struct FullResReq {
     const uint8_t* img; const uint8_t* mask; uint8_t* out;
     float* x; const float* y;    // the request's slot of its chunk's x [n][4][Hp][Wp] / y [n][3][Hp][Wp]
+    int64_t pitch;
     int H, W, C, invert, Hp, Wp;
 };
 struct FullResBatch {
@@ -68,14 +73,14 @@ struct FullResPreK {
         const int row = (int)(j / groups);
         const int x0 = (int)(j - (int64_t)row * groups) * 4;
         const int sy = src_index(row, r.H);
-        const uint8_t* img_row = r.img + (int64_t)sy * r.W * 3;
+        const uint8_t* img_row = r.img + (int64_t)sy * r.pitch * 3;
         const bool direct = x0 + 4 <= r.W;   // the four columns lie inside the photo
         float m[4];                          // mask // 255 of the four pixels
         const uint8_t* px[4];
 #pragma unroll
         for (int p = 0; p < 4; ++p) {
             const int sx = direct ? x0 + p : src_index(x0 + p < r.Wp ? x0 + p : r.Wp - 1, r.W);
-            m[p] = mask_known(r.mask, r.W, r.C, r.invert, sy, sx) ? 1.f : 0.f;
+            m[p] = mask_known(r.mask, r.pitch, r.C, r.invert, sy, sx) ? 1.f : 0.f;
             px[p] = img_row + (int64_t)sx * 3;
         }
         // plane by plane, so that only one plane's four values are live across the divisions' slow-path calls
@@ -99,7 +104,8 @@ struct FullResPreK {
     }
 };
 
-// One photo pixel: y (pitch Wp) -> uint8, composed with the photo's known pixels.  items per request = H * W
+// One window pixel: y (pitch Wp) -> uint8, composed with the photo's known pixels.  items per request = H * W; nothing
+// outside the window is written.
 struct FullResPostK {
     const FullResBatch& b;
     PP_D void operator()(int64_t i) const {
@@ -107,11 +113,12 @@ struct FullResPostK {
         const FullResReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int row = (int)(j / r.W), col = (int)(j - (int64_t)row * r.W);
-        const bool known = mask_known(r.mask, r.W, r.C, r.invert, row, col);
+        const bool known = mask_known(r.mask, r.pitch, r.C, r.invert, row, col);
         const int64_t plane = (int64_t)r.Hp * r.Wp;
         const float* y = r.y + (int64_t)row * r.Wp + col;
-        uint8_t* o = r.out + j * 3;
-        const uint8_t* p = r.img + j * 3;
+        const int64_t px = (int64_t)row * r.pitch + col;
+        uint8_t* o = r.out + px * 3;
+        const uint8_t* p = r.img + px * 3;
         for (int c = 0; c < 3; ++c) o[c] = known ? p[c] : post_u8(y[c * plane]);
     }
 };
@@ -147,8 +154,25 @@ comod::FullResBatch fullres_batch(const migan_fullres_request* q, int n, bool pr
     b.start[0] = 0;
     for (int k = 0; k < n; ++k) {
         comod::FullResReq& r = b.r[k];
-        r.img = q[k].img; r.mask = q[k].mask; r.out = q[k].out; r.x = q[k].x; r.y = q[k].y;
+        r.img = q[k].img; r.mask = q[k].mask; r.out = q[k].out; r.x = q[k].x; r.y = q[k].y; r.pitch = q[k].W;
         r.H = q[k].H; r.W = q[k].W; r.C = q[k].mask_channels; r.invert = q[k].invert != 0; r.Hp = q[k].Hp; r.Wp = q[k].Wp;
+        b.start[k + 1] = b.start[k] + (pre ? comod::fullres_pre_items(r) : comod::fullres_post_items(r));
+    }
+    return b;
+}
+
+// A window request is the full-resolution request of its crop: the pointers move to the window origin and the rows keep
+// the photo's pitch.
+comod::FullResBatch window_batch(const migan_window_request* q, int n, bool pre) {
+    comod::FullResBatch b;
+    b.n = n;
+    b.start[0] = 0;
+    for (int k = 0; k < n; ++k) {
+        comod::FullResReq& r = b.r[k];
+        const int64_t origin = (int64_t)q[k].y0 * q[k].W + q[k].x0;
+        r.img = q[k].img + origin * 3; r.mask = q[k].mask + origin * q[k].mask_channels; r.out = q[k].out + origin * 3;
+        r.x = q[k].x; r.y = q[k].y; r.pitch = q[k].W;
+        r.H = q[k].h; r.W = q[k].w; r.C = q[k].mask_channels; r.invert = q[k].invert != 0; r.Hp = q[k].Hp; r.Wp = q[k].Wp;
         b.start[k + 1] = b.start[k] + (pre ? comod::fullres_pre_items(r) : comod::fullres_post_items(r));
     }
     return b;
@@ -192,6 +216,47 @@ int launch_fullres_postprocess(const migan_fullres_request* q, int n, ck_stream_
     return (int)comod::fullres_launch<comod::FullResPostK>(fullres_batch(q, n, false), s);
 }
 
+int check_window_batch(const migan_window_request* q, int n, bool pre, char* msg, size_t len) {
+    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
+    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
+        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
+        return MIGAN_ERR_INVALID;
+    }
+    for (int k = 0; k < n; ++k) {
+        const migan_window_request& r = q[k];
+        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out)) {
+            snprintf(msg, len, "request %d: null photo, mask, %s", k, pre ? "or x" : "y or output");
+            return MIGAN_ERR_INVALID;
+        }
+        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) {
+            snprintf(msg, len, "request %d: x must be 16-byte aligned", k);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.H < 1 || r.W < 1 || r.h < 1 || r.w < 1 || r.y0 < 0 || r.x0 < 0 || r.y0 > r.H - r.h || r.x0 > r.W - r.w) {
+            snprintf(msg, len, "request %d: window (y0 %d, x0 %d, h %d, w %d) of a photo of %d x %d (H x W)", k, r.y0, r.x0,
+                     r.h, r.w, r.H, r.W);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.Hp < r.h || r.Wp < r.w) {
+            snprintf(msg, len, "request %d: window of %d x %d, padded extent %d x %d (h x w)", k, r.h, r.w, r.Hp, r.Wp);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.mask_channels < 1 || r.mask_channels > 4) {
+            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
+            return MIGAN_ERR_INVALID;
+        }
+    }
+    return MIGAN_OK;
+}
+
+int launch_window_preprocess(const migan_window_request* q, int n, ck_stream_t s) {
+    return (int)comod::fullres_launch<comod::FullResPreK>(window_batch(q, n, true), s);
+}
+
+int launch_window_postprocess(const migan_window_request* q, int n, ck_stream_t s) {
+    return (int)comod::fullres_launch<comod::FullResPostK>(window_batch(q, n, false), s);
+}
+
 }  // namespace migan
 
 #ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
@@ -204,5 +269,13 @@ extern "C" int b200_fullres_preprocess(const migan_fullres_request* q, int n, vo
 extern "C" int b200_fullres_postprocess(const migan_fullres_request* q, int n, void* s) {
     if (int rc = migan::check_fullres_batch(q, n, false, g_fullres_msg, sizeof g_fullres_msg)) return rc;
     return migan::launch_fullres_postprocess(q, n, s);
+}
+extern "C" int b200_window_preprocess(const migan_window_request* q, int n, void* s) {
+    if (int rc = migan::check_window_batch(q, n, true, g_fullres_msg, sizeof g_fullres_msg)) return rc;
+    return migan::launch_window_preprocess(q, n, s);
+}
+extern "C" int b200_window_postprocess(const migan_window_request* q, int n, void* s) {
+    if (int rc = migan::check_window_batch(q, n, false, g_fullres_msg, sizeof g_fullres_msg)) return rc;
+    return migan::launch_window_postprocess(q, n, s);
 }
 #endif

@@ -119,6 +119,18 @@ int launch_demo_postprocess(const float* y, const migan_demo_request* reqs, int 
 int check_fullres_batch(const migan_fullres_request* reqs, int n, bool pre, char* msg, size_t len);
 int launch_fullres_preprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
 int launch_fullres_postprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
+// the same kernels on windows of a photo (the whole photo is the window (0, 0, H, W))
+int check_window_batch(const migan_window_request* reqs, int n, bool pre, char* msg, size_t len);
+int launch_window_preprocess(const migan_window_request* reqs, int n, cudaStream_t s);
+int launch_window_postprocess(const migan_window_request* reqs, int n, cudaStream_t s);
+
+// ---- hole-window request path (holewin.cu): hole cells on the device, the window planner on the host ------
+int check_hole_cells(const migan_cells_request* reqs, int n, int res, char* msg, size_t len);
+size_t hole_cells_bytes(const migan_cells_request* reqs, int n, int res);
+int launch_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* cells, cudaStream_t s);
+int hole_windows_max(int H, int W, int res, int* max_windows, char* msg, size_t len);
+int hole_windows(const uint8_t* cells_host, int H, int W, int res, int margin, int* win4, int max_windows, int* count, char* msg,
+                 size_t len);
 
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------

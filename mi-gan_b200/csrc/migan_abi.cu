@@ -1600,6 +1600,57 @@ int b200_fullres_postprocess(const migan_fullres_request* reqs, int n, void* str
     return MIGAN_OK;
 }
 
+static int check_window(const char* who, const migan_window_request* reqs, int n, bool pre) {
+    char msg[256];
+    if (int rc = migan::check_window_batch(reqs, n, pre, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+int b200_window_preprocess(const migan_window_request* reqs, int n, void* stream) {
+    if (int rc = check_window("window_preprocess", reqs, n, true)) return rc;
+    CUDA_TRY((cudaError_t)migan::launch_window_preprocess(reqs, n, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_window_postprocess(const migan_window_request* reqs, int n, void* stream) {
+    if (int rc = check_window("window_postprocess", reqs, n, false)) return rc;
+    CUDA_TRY((cudaError_t)migan::launch_window_postprocess(reqs, n, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+static int check_hole_cells(const char* who, const migan_cells_request* reqs, int n, int res) {
+    char msg[256];
+    if (int rc = migan::check_hole_cells(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
+    return MIGAN_OK;
+}
+
+size_t b200_hole_cells_bytes(const migan_cells_request* reqs, int n, int res) {
+    if (check_hole_cells("hole_cells_bytes", reqs, n, res)) return 0;
+    return migan::hole_cells_bytes(reqs, n, res);
+}
+
+int b200_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* cells, void* stream) {
+    if (int rc = check_hole_cells("hole_cells", reqs, n, res)) return rc;
+    if (!cells) return fail(MIGAN_ERR_INVALID, "hole_cells: null cells");
+    CUDA_TRY((cudaError_t)migan::launch_hole_cells(reqs, n, res, cells, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int migan_hole_windows_max(int H, int W, int res, int* max_windows) {
+    char msg[256];
+    if (!max_windows) return fail(MIGAN_ERR_INVALID, "hole_windows_max: null argument");
+    if (int rc = migan::hole_windows_max(H, W, res, max_windows, msg, sizeof msg)) return fail(rc, "hole_windows_max: %s", msg);
+    return MIGAN_OK;
+}
+
+int migan_hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* win4, int max_windows, int* count) {
+    char msg[256];
+    if (!cells || !win4 || !count) return fail(MIGAN_ERR_INVALID, "hole_windows: null argument");
+    if (int rc = migan::hole_windows(cells, H, W, res, margin, win4, max_windows, count, msg, sizeof msg))
+        return fail(rc, "hole_windows: %s", msg);
+    return MIGAN_OK;
+}
+
 int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h) {
     if (!out_w || !out_h) return fail(MIGAN_ERR_INVALID, "demo_resized_size: null argument");
     if (w < 1 || h < 1 || max_size < 1) return fail(MIGAN_ERR_INVALID, "demo_resized_size: bad arguments (%d x %d, max size %d)", w, h, max_size);

@@ -22,10 +22,11 @@ namespace comod {
 
 // read_mask's per-pixel steps at pixel (y, x) of a mask [.][W][C]: the channel (alpha of LA / RGBA, R of RGB, L), 255 - v
 // if invert, then v < 255 -> 0.  True where the result is 255 (known).
+// mask_channel and known_value are its two halves, for kernels that load the mask bytes themselves (holewin.cu).
+CK_HD int mask_channel(int C) { return C == 4 ? 3 : (C == 2 ? 1 : 0); }
+CK_HD bool known_value(int v, int invert) { return invert ? v == 0 : v == 255; }
 CK_HD bool mask_known(const uint8_t* mask, int64_t W, int C, int invert, int y, int x) {
-    const int ch = C == 4 ? 3 : (C == 2 ? 1 : 0);
-    const int v = mask[((int64_t)y * W + x) * C + ch];
-    return invert ? v == 0 : v == 255;
+    return known_value(mask[((int64_t)y * W + x) * C + mask_channel(C)], invert);
 }
 
 // x channel 0 from the mask value m = mask // 255 (0 or 1): mask - 0.5                          (demo.py:60, :65)

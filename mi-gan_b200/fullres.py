@@ -65,14 +65,15 @@ def plan_passes(extents: Sequence[Tuple[int, int]], max_n: Dict[Tuple[int, int],
     return passes
 
 
-class FullResPipeline(torch.nn.Module):
-    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from."""
+class _PhotoPipeline(torch.nn.Module):
+    """What the photo pipelines share: the generator, the per-request input checks, one workspace and `wait()`.
+    `model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from."""
 
     def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda"):
         super().__init__()
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("migan_b200.FullResPipeline runs on a CUDA device (there is no CPU path); got %s" % device)
+            raise RuntimeError("migan_b200.%s runs on a CUDA device (there is no CPU path); got %s" % (self._name(), device))
         if isinstance(model_or_state_dict, Generator):
             if model_or_state_dict.resolution != resolution:
                 raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_or_state_dict.resolution, resolution))
@@ -85,8 +86,10 @@ class FullResPipeline(torch.nn.Module):
         self.res = int(resolution)
         self._ws = None                                      # the generator workspace, grown to the largest chunk seen
         self._pending: List[_Call] = []
-        self.last_extents: List[Tuple[int, int]] = []      # (Hp, Wp) of every result of the last completed call(s)
-        self.last_launches = 0                              # kernel launches of the last pass, generator included
+
+    @classmethod
+    def _name(cls) -> str:
+        return cls.__name__
 
     def __call__(self, img, mask, invert: bool = False):
         return self.forward_batch([img], [mask], invert=invert)[0]
@@ -94,33 +97,45 @@ class FullResPipeline(torch.nn.Module):
     def _device(self) -> torch.device:
         return next(self.model.parameters()).device
 
-    def _extent(self, eng, i: int, H: int, W: int) -> Tuple[Tuple[int, int], int]:
-        """((Hp, Wp), largest batch there) of request i; ValueError when the photo is too large for one forward."""
+    def _extent(self, eng, i: int, H: int, W: int, what: str = "") -> Tuple[Tuple[int, int], int]:
+        """((Hp, Wp), largest batch there) of an H x W photo (or window) of request i; ValueError when it is too large
+        for one forward."""
         Hp, Wp, mx = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         if eng.lib.migan_fullres_extent(eng.handle, H, W, ctypes.byref(Hp), ctypes.byref(Wp), ctypes.byref(mx)) != 0:
-            raise ValueError("FullResPipeline: request %d: %s" % (i, eng.lib.migan_last_error().decode()))
+            raise ValueError("%s: request %d: %s%s" % (self._name(), i, what, eng.lib.migan_last_error().decode()))
         return (Hp.value, Wp.value), mx.value
 
     def _check(self, i, img, mask):
         """(photo tensor [H,W,3], mask tensor [H,W,C]) of request i."""
+        name = self._name()
         img = torch.from_numpy(np.ascontiguousarray(img)) if isinstance(img, np.ndarray) else img
         mask = torch.from_numpy(np.ascontiguousarray(mask)) if isinstance(mask, np.ndarray) else mask
         if not isinstance(img, torch.Tensor) or not isinstance(mask, torch.Tensor):
-            raise TypeError("FullResPipeline: request %d: photo and mask must be numpy arrays or torch tensors" % i)
+            raise TypeError("%s: request %d: photo and mask must be numpy arrays or torch tensors" % (name, i))
         if img.dtype != torch.uint8 or mask.dtype != torch.uint8:
-            raise ValueError("FullResPipeline: request %d: photo and mask must be uint8" % i)
+            raise ValueError("%s: request %d: photo and mask must be uint8" % (name, i))
         if img.dim() != 3 or img.shape[2] != 3 or img.shape[0] < 1 or img.shape[1] < 1:
-            raise ValueError("FullResPipeline: request %d: photo of shape %s, expected [H, W, 3]" % (i, tuple(img.shape)))
+            raise ValueError("%s: request %d: photo of shape %s, expected [H, W, 3]" % (name, i, tuple(img.shape)))
         if mask.dim() == 2:
             mask = mask.unsqueeze(2)
         if mask.dim() != 3 or not 1 <= mask.shape[2] <= 4:
-            raise ValueError("FullResPipeline: request %d: mask of shape %s, expected [H, W] or [H, W, 1..4]" % (i, tuple(mask.shape)))
+            raise ValueError("%s: request %d: mask of shape %s, expected [H, W] or [H, W, 1..4]" % (name, i, tuple(mask.shape)))
         if tuple(mask.shape[:2]) != tuple(img.shape[:2]):
-            raise ValueError("FullResPipeline: request %d: mask of %d x %d, photo of %d x %d (H x W); they must match"
-                             % (i, mask.shape[0], mask.shape[1], img.shape[0], img.shape[1]))
+            raise ValueError("%s: request %d: mask of %d x %d, photo of %d x %d (H x W); they must match"
+                             % (name, i, mask.shape[0], mask.shape[1], img.shape[0], img.shape[1]))
         if img.is_cuda and img.device != self._device():
-            raise ValueError("FullResPipeline: request %d: photo on %s, the pipeline runs on %s" % (i, img.device, self._device()))
+            raise ValueError("%s: request %d: photo on %s, the pipeline runs on %s" % (name, i, img.device, self._device()))
         return img, mask
+
+    def _kind(self, i: int, img, wait: bool) -> str:
+        """"numpy", "cpu" or "cuda" for photo i; refuses a photo that cannot be copied asynchronously when wait=False."""
+        if not isinstance(img, (np.ndarray, torch.Tensor)):
+            raise TypeError("%s: request %d: photo and mask must be numpy arrays or torch tensors" % (self._name(), i))
+        kind = "numpy" if isinstance(img, np.ndarray) else ("cuda" if img.is_cuda else "cpu")
+        if not wait and kind != "cuda" and not (kind == "cpu" and img.is_pinned() and img.is_contiguous()):
+            raise RuntimeError("%s.forward_batch(wait=False): CPU photo %d must be a pinned contiguous tensor (it is "
+                               "copied asynchronously); use torch.from_numpy(img).pin_memory() or wait=True" % (self._name(), i))
+        return kind
 
     def _workspace(self, eng, nbytes: int) -> torch.Tensor:
         """The one workspace, 1024-byte aligned, grown (never shrunk) to nbytes.  A grown workspace is a new address, so
@@ -131,6 +146,24 @@ class FullResPipeline(torch.nn.Module):
             off = (-raw.data_ptr()) % 1024
             self._ws = raw[off:off + nbytes]
         return self._ws
+
+    def _finish(self, calls) -> None:
+        raise NotImplementedError
+
+    def wait(self) -> None:
+        """Block until every call enqueued with `forward_batch(..., wait=False)` has finished: its outputs are written and
+        the per-request record of those calls (`last_extents` / `last_windows`) is set, in submission order."""
+        calls, self._pending = self._pending, []
+        self._finish(calls)
+
+
+class FullResPipeline(_PhotoPipeline):
+    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from."""
+
+    def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda"):
+        super().__init__(model_or_state_dict, resolution, device)
+        self.last_extents: List[Tuple[int, int]] = []      # (Hp, Wp) of every result of the last completed call(s)
+        self.last_launches = 0                              # kernel launches of the last pass, generator included
 
     def _pass(self, eng, chunks: List[Chunk], imgs, masks, inverts, outs, ws, stream) -> list:
         """Enqueue one pass; returns the tensors its work reads or writes."""
@@ -184,13 +217,7 @@ class FullResPipeline(torch.nn.Module):
             eng = self.model._engine(dev)
             kinds, checked, extents, max_n = [], [], [], {}
             for i, (img, mask) in enumerate(zip(imgs, masks)):
-                if not isinstance(img, (np.ndarray, torch.Tensor)):
-                    raise TypeError("FullResPipeline: request %d: photo and mask must be numpy arrays or torch tensors" % i)
-                kinds.append("numpy" if isinstance(img, np.ndarray) else ("cuda" if img.is_cuda else "cpu"))
-                if not wait and kinds[-1] != "cuda" and not (kinds[-1] == "cpu" and img.is_pinned() and img.is_contiguous()):
-                    raise RuntimeError("FullResPipeline.forward_batch(wait=False): CPU photo %d must be a pinned contiguous "
-                                       "tensor (it is copied asynchronously); use torch.from_numpy(img).pin_memory() or "
-                                       "wait=True" % i)
+                kinds.append(self._kind(i, img, wait))
                 img, mask = self._check(i, img, mask)
                 ext, mx = self._extent(eng, i, int(img.shape[0]), int(img.shape[1]))
                 checked.append((img, mask))
@@ -233,9 +260,3 @@ class FullResPipeline(torch.nn.Module):
             extents += call.sizes
         if extents:
             self.last_extents = extents
-
-    def wait(self) -> None:
-        """Block until every call enqueued with `forward_batch(..., wait=False)` has finished: its outputs are written and
-        `last_extents` holds the extents of all those calls' results, in submission order."""
-        calls, self._pending = self._pending, []
-        self._finish(calls)
