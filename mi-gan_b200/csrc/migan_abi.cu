@@ -604,6 +604,7 @@ int migan_finalize_weights(migan_ctx* ctx) {
     for (auto& f : fix) *f.first = static_cast<unsigned char*>(ctx->arena) + f.second;
     ctx->plans.clear();  // pointers changed
     ctx->plan = nullptr;
+    ctx->tap_cache_path = -1;   // the FIR taps decide which stages are fused, so the tap list may change with the weights
     if (ctx->graph_exec) { cudaGraphExecDestroy(ctx->graph_exec); ctx->graph_exec = nullptr; }
     ctx->finalized = true;
     return MIGAN_OK;

@@ -89,8 +89,9 @@ def generator_forward_fc(sd: Dict[str, torch.Tensor], x: torch.Tensor, resolutio
     return O.synthesis_forward(sd, x4, feats, resolution, taps)
 
 
-def fixture_rows(n: int):
-    """Rows of an output kept in tests/golden/fullconv.npz: r % 8 in {0, 1} (both phases of every 2x resampling) and
-    the last two rows (the bottom edge, where tiles are partial)."""
+def fixture_rows(n: int, period: int = 8):
+    """Rows of an output kept in a fixture: r % period in {0, 1} (both phases of every 2x resampling) and the last two
+    rows (the bottom edge, where tiles are partial).  tests/golden/fullconv.npz uses period 8; tests/golden/fir.npz uses
+    16, which keeps its four cases near 500 KB."""
     r = torch.arange(n)
-    return r[(r % 8 < 2) | (r >= n - 2)]
+    return r[(r % period < 2) | (r >= n - 2)]

@@ -131,25 +131,52 @@ def state_dict_spec(resolution: int) -> "OrderedDict[str, Tuple[int, ...]]":
     return OrderedDict(spec)
 
 
-def make_state_dict(resolution: int, seed: int = 1, *, style: str = "export") -> "OrderedDict[str, torch.Tensor]":
+FIR_MODES = ("constructor", "uniform", "per_channel")
+
+
+def random_fir(n: int, gain: float, g: torch.Generator) -> torch.Tensor:
+    """n asymmetric 4x4 FIR filters [n,1,4,4]: rand + 0.1, each normalised to sum `gain` (1 for down-sampling, 4 for
+    up-sampling), so activations keep the scale the constructor's [1,3,3,1] filter gives them."""
+    f = torch.rand(n, 1, 4, 4, generator=g) + 0.1
+    return f * (gain / f.sum(dim=(2, 3), keepdim=True))
+
+
+def make_state_dict(resolution: int, seed: int = 1, *, style: str = "export",
+                    fir: str = "constructor") -> "OrderedDict[str, torch.Tensor]":
     """Seeded weights with the statistics of a released checkpoint (SURVEY.md 8c).
 
     style="export": every conv weight (depthwise 3x3, 1x1, fromrgb, torgb) is randn
     normalised to unit L2 norm per output channel -- what
     scripts/export_inference_model.py:26 produces; biases ~ 0.1 randn;
     noise_strength ~ 0.1 randn (ctor default 0 would leave the noise path untested,
-    migan_inference.py:150); noise_const ~ randn (ctor :149); FIR taps and
-    filter_const at their constructor values (:71-72, :83-85, :95-96).
+    migan_inference.py:150); noise_const ~ randn (ctor :149); filter_const at its
+    constructor value (:83-85).
     style="default": like torch's default Conv2d init scale (small outputs).
+
+    fir: the `*.filter.weight` taps, which are parameters in the reference (:72, :96), so a
+    trained checkpoint may carry any values there.
+      "constructor"  setup_filter([1,3,3,1]) for every channel (:71-72, :95-96): symmetric,
+                     separable and channel-uniform;
+      "uniform"      one random asymmetric filter per layer, shared by its channels;
+      "per_channel"  an independent random asymmetric filter for every channel.
+    Random taps come from their own generator (`random_fir`), so the other weights of a seed
+    are the same in every mode.
     """
+    if fir not in FIR_MODES:
+        raise ValueError("fir must be one of %s, got %r" % (FIR_MODES, fir))
     g = torch.Generator().manual_seed(seed)
+    g_fir = torch.Generator().manual_seed(seed + 7919)
     sd = OrderedDict()
     f_down = setup_filter([1, 3, 3, 1], gain=1)
     f_up = setup_filter([1, 3, 3, 1], gain=4)
     for key, shape in state_dict_spec(resolution).items():
         if key.endswith("filter.weight"):
-            f = f_down if "downsample" in key else f_up
-            t = f.repeat(shape[0], 1, 1, 1).clone()
+            down = "downsample" in key
+            if fir == "constructor":
+                t = (f_down if down else f_up).repeat(shape[0], 1, 1, 1).clone()
+            else:
+                t = random_fir(shape[0] if fir == "per_channel" else 1, 1.0 if down else 4.0, g_fir)
+                t = t.expand(shape[0], 1, 4, 4).clone()
         elif key.endswith("filter_const"):
             w = torch.tensor([[1.0, 0.0], [0.0, 0.0]])
             t = w.repeat(1, 1, shape[2] // 2, shape[3] // 2).clone()

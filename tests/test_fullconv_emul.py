@@ -205,13 +205,17 @@ EDGE_TILES = [(40, 48, 32, 32), (40, 48, 0, 32), (36, 52, 32, 48), (36, 52, 32, 
 
 
 @pytest.mark.parametrize("H,W,y0,x0", EDGE_TILES)
-def test_prestage_up_hw_edge_tiles(stages, H, W, y0, x0):
+@pytest.mark.parametrize("fir", ["constructor", "asymmetric"])
+def test_prestage_up_hw_edge_tiles(stages, H, W, y0, x0, fir):
     C = 32
     g = torch.Generator().manual_seed(H + W + y0 + x0)
     t = torch.randn(1, C, H // 2, W // 2, generator=g) * 3
     skip = torch.randn(1, C, H, W, generator=g)
     noise = torch.randn(H, W, generator=g) * 0.3
-    taps = O.setup_filter([1, 3, 3, 1], gain=4.0)
+    if fir == "constructor":   # symmetric: blind to flipped or transposed taps
+        taps = O.setup_filter([1, 3, 3, 1], gain=4.0)
+    else:                      # one asymmetric filter, as a trained checkpoint may carry
+        taps = O.random_fir(1, 4.0, torch.Generator().manual_seed(11))[0, 0]
     want = O.lrelu_agc(O.upsample2d(t, taps[None, None].repeat(C, 1, 1, 1), FC.zero_insertion(H, W)) + noise) + skip
     want = F.pad(want, (1, 17, 1, 9))[0].permute(1, 2, 0).numpy()          # zero outside the image, index +1
     t_hwc = np.ascontiguousarray(t[0].permute(1, 2, 0).numpy())

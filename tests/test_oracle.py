@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import fullconv_oracle as FC
 from oracle import migan_oracle as O
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
@@ -63,8 +64,24 @@ def test_resolution_validation():
         O.encode_res(96)
 
 
+def _polyphase_up(x, f):
+    """The polyphase form of Upsample2d the kernels implement, for any 4x4 filter f [C,1,4,4]:
+    out[2i + a][2j + b] = sum_{u,v in {0,1}} f[a + 2u][b + 2v] * x[i - 1 + a + u][j - 1 + b + v]   (x = 0 outside)."""
+    n, c, h, w = x.shape
+    xp = torch.nn.functional.pad(x, (1, 1, 1, 1))
+    out = torch.zeros(n, c, 2 * h, 2 * w, dtype=x.dtype)
+    for a in (0, 1):
+        for b in (0, 1):
+            for u in (0, 1):
+                for v in (0, 1):
+                    tap = f[:, 0, a + 2 * u, b + 2 * v].view(1, c, 1, 1)
+                    out[:, :, a::2, b::2] += tap * xp[:, :, a + u:a + u + h, b + v:b + v + w]
+    return out
+
+
 def test_polyphase_identity():
-    """Upsample2d == the 2-tap polyphase form the kernels use (SURVEY.md 7.4(4))."""
+    """Upsample2d == the 2-tap polyphase form the kernels use (SURVEY.md 7.4(4)), for the constructor's filter and for
+    asymmetric per-channel filters (a checkpoint may carry trained taps)."""
     g = torch.Generator().manual_seed(3)
     x = torch.randn(1, 2, 5, 5, generator=g)
     f = O.setup_filter([1, 3, 3, 1], gain=4).repeat(2, 1, 1, 1)
@@ -78,6 +95,56 @@ def test_polyphase_identity():
     cols_o = 0.75 * rows[..., 1:6] + 0.25 * rows[..., 2:7]
     out = torch.stack([cols_e, cols_o], 4).reshape(1, 2, 10, 10)
     assert float((out - ref).abs().max()) < 1e-6
+    assert float((_polyphase_up(x, f) - ref).abs().max()) < 1e-6
+    # asymmetric taps, different per channel, on a non-square input
+    x = torch.randn(2, 3, 5, 7, generator=g, dtype=torch.float64)
+    f = O.random_fir(3, 4.0, g).double()
+    assert not torch.equal(f, f.flip([2, 3])) and not torch.equal(f, f.transpose(2, 3)) and not torch.equal(f[0], f[1])
+    ref = O.upsample2d(x, f, FC.zero_insertion(10, 14).double())
+    assert float((_polyphase_up(x, f) - ref).abs().max()) < 1e-12
+    for wrong in (f.flip([2, 3]), f.transpose(2, 3), f[:1].expand_as(f)):   # the oracle tells each mistake apart
+        assert float((_polyphase_up(x, wrong) - ref).abs().max()) > 1e-2
+
+
+def test_make_state_dict_fir_modes():
+    """fir= changes the FIR taps only; the constructor mode is the default, and random taps keep their gain."""
+    base = O.make_state_dict(64, seed=1)
+    assert all(torch.equal(a, b) for a, b in zip(base.values(), O.make_state_dict(64, seed=1, fir="constructor").values()))
+    for mode in ("uniform", "per_channel"):
+        sd = O.make_state_dict(64, seed=1, fir=mode)
+        assert list(sd.keys()) == list(base.keys())
+        for k, v in sd.items():
+            if not k.endswith("filter.weight"):
+                assert torch.equal(v, base[k]), k
+                continue
+            assert v.shape == base[k].shape and v.is_contiguous()
+            gain = 1.0 if "downsample" in k else 4.0
+            assert torch.allclose(v.sum(dim=(2, 3)), torch.full(v.shape[:2], gain), atol=1e-5), k
+            assert (v > 0).all() and not torch.equal(v, v.flip([2, 3])) and not torch.equal(v, v.transpose(2, 3)), k
+            assert torch.equal(v, v[:1].expand_as(v)) == (mode == "uniform"), k
+    with pytest.raises(ValueError):
+        O.make_state_dict(64, fir="symmetric")
+
+
+def _fir_cases():
+    return list(range(int(np.load(os.path.join(GOLDEN, "fir.npz"))["num_cases"])))
+
+
+@pytest.mark.parametrize("case", _fir_cases())
+def test_oracle_reproduces_fir_fixture(case):
+    """The oracle with asymmetric FIR taps against outputs of the reference itself (make_golden_fir.py)."""
+    z = np.load(os.path.join(GOLDEN, "fir.npz"))
+    R, N, H, W, wseed, xseed = [int(v) for v in z["case%d_meta" % case]]
+    sd = O.make_state_dict(R, seed=wseed, fir=str(z["case%d_fir" % case]))
+    x = FC.make_input_hw(R, N, H, W, seed=xseed)
+    assert sum(_checksum(v) for v in sd.values()) == pytest.approx(float(z["case%d_w_checksum" % case]), rel=1e-12)
+    assert _checksum(x) == pytest.approx(float(z["case%d_x_checksum" % case]), rel=1e-12)
+    y = FC.generator_forward_fc(sd, x, R)
+    if (H, W) == (R, R):
+        assert torch.equal(y, O.generator_forward(sd, x, R))
+    rows = z["case%d_rows" % case]
+    assert np.array_equal(rows, np.arange(H) if R == 64 else FC.fixture_rows(H, period=16).numpy())
+    assert float((y[:, :, rows] - torch.from_numpy(z["case%d_y" % case])).abs().max()) <= 1e-5
 
 
 def test_op_oracles_match_golden():

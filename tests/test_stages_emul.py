@@ -5,7 +5,8 @@ TMA unit fills a pipeline stage (box layout, out-of-bounds zero fill).  Checked 
   * UP pre-stage   == lrelu_agc(Upsample2d(t) + noise) + skip on the halo'd tile, ZERO outside the image
   * STEM pre-stage == lrelu_agc(fromrgb(x) + b) on the halo'd tile, ZERO outside the image
   * depthwise prologue -> A operand (fp16 hi/lo, SWIZZLE_128B K-major) == 64 * lrelu_agc(dw3x3(in) + b)
-for tiles at every image corner / edge / interior position.  No GPU involved.
+for tiles at every image corner / edge / interior position.  The UP pre-stage runs with the constructor's symmetric filter
+and with an asymmetric one, which shows flipped or transposed taps.  No GPU involved.
 """
 import ctypes
 import os
@@ -72,15 +73,24 @@ def decode_a(a_hi, a_lo):
 TILE_POS = [(0, 0), (0, 16), (8, 0), (24, 48), (56, 48), (56, 0), (0, 48), (16, 32)]   # R = 64: corners, edges, interior
 
 
+def up_taps(fir):
+    """The 4x4 up-sampling filter (gain 4) the pre-stage gets: the constructor's [1,3,3,1] (symmetric, so blind to a
+    flip or a transpose) or one asymmetric filter, as a trained checkpoint may carry."""
+    if fir == "constructor":
+        return O.setup_filter([1, 3, 3, 1], gain=4.0)
+    return O.random_fir(1, 4.0, torch.Generator().manual_seed(11))[0, 0]
+
+
 @pytest.mark.parametrize("y0,x0", TILE_POS)
 @pytest.mark.parametrize("has_noise", [1, 0])
-def test_prestage_up_matches_oracle(lib, y0, x0, has_noise):
+@pytest.mark.parametrize("fir", ["constructor", "asymmetric"])
+def test_prestage_up_matches_oracle(lib, y0, x0, has_noise, fir):
     R, C = 64, 64
     g = torch.Generator().manual_seed(7)
     t = torch.randn(1, C, R // 2, R // 2, generator=g) * 3
     skip = torch.randn(1, C, R, R, generator=g)
     noise = torch.randn(R, R, generator=g) * 0.3 if has_noise else torch.zeros(R, R)
-    taps = O.setup_filter([1, 3, 3, 1], gain=4.0)
+    taps = up_taps(fir)
     fw = taps[None, None].repeat(C, 1, 1, 1)
     fconst = torch.zeros(1, 1, R, R); fconst[:, :, ::2, ::2] = 1
     want = O.lrelu_agc(O.upsample2d(t, fw, fconst) + noise) + skip            # [1, C, R, R]
