@@ -84,6 +84,7 @@ struct Params {
     int tiles_x, tiles_y, tiles_n, num_n_tiles, num_tiles;   // num_n_tiles = cout / n_tile; tiles_x = ceil(W / tile_w) ...
     int n_group;                              // N tiles per CTA tile (power of two; > 1: stationary A)
     int l_nt;                                 // log2 of num_n_tiles / n_group (a power of two)
+    int l_tw, l_th;                           // log2 of tile_w / tile_h (powers of two): the epilogue's pixel decode
     FastDiv div_tx, div_ty;                   // by tiles_x / tiles_y (not powers of two at a rectangular extent)
     int num_kb;                               // cin / 64
     int in_stages, a_stages, b_stages, b_resident;
@@ -297,7 +298,6 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
     const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int num_kb = p.num_kb;
     const uint32_t b_stage_bytes = (uint32_t)NT * kKBlock * 2 * 2;   // [Bh ; Bl]
-    const int hw = p.tile_h * p.tile_w;
     float acc[2][NA], cor[2][NC];
     float rgb_acc[4];                                // torgb sum of colour lane % 4 over the group's N tiles, per pixel row
     Ring ra(p.a_stages), rb(p.b_stages);
@@ -358,7 +358,7 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
         for (int r = 0; r < 4; ++r) {
             const int h = r >> 1, i = r & 1;
             const int m = h * 64 + wq * 16 + (lane >> 2) + 8 * i;
-            const int pimg = tc.n0 + m / hw, poy = tc.y0 + (m / p.tile_w) % p.tile_h, pox = tc.x0 + m % p.tile_w;
+            const int pimg = tc.n0 + (m >> (p.l_tw + p.l_th)), poy = tc.y0 + ((m >> p.l_tw) & (p.tile_h - 1)), pox = tc.x0 + (m & (p.tile_w - 1));
             const bool valid = pimg < p.n && poy < p.H && pox < p.W;   // partial tiles at the right / bottom edge
             const float nz = (p.noise && valid) ? __ldg(p.noise + poy * p.noise_pitch + pox) : 0.f;
             const float nz_g = nz * kActGain;
@@ -819,6 +819,7 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
         return "fused torgb needs all output channels of a pixel tile in one CTA tile (cout <= 256 with a resident A operand)";
     if (p.in_stages > 8 || p.a_stages > kMaxAStages || p.b_stages > 8) return "internal: ring too deep for the barrier table";
     p.l_nt = ilog2(p.num_n_tiles / p.n_group);
+    p.l_tw = ilog2(p.tile_w); p.l_th = ilog2(p.tile_h);
     p.num_tiles = m_tiles * (p.num_n_tiles / p.n_group);
     return nullptr;
 }
