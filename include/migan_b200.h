@@ -346,6 +346,47 @@ int migan_tap_info(const migan_ctx* ctx, int path, int index, const char** name,
  * (wait code | parity << 12 | block << 16) in a host-mapped word and traps.  Returns that record for `device` (0: none). */
 int migan_debug_tc_timeout(int device);
 
+/* Test hook: one launch of the tensor-core SeparableConv2d kernel on caller-provided operands, packed by the same
+ * functions the weight loader uses.  Device pointers, reference layouts.  The package never calls it. */
+typedef struct migan_sepconv_tc_io {
+    int source;                 /* 0 NHWC, 1 SPLIT (pre-split fp16 A operand), 2 UP, 3 STEM */
+    int n, h, w, cin, cout;
+    int act, passes;            /* act: lrelu_agc in the epilogue; passes: 3 (fp16 hi/lo split) or 1 */
+    const float* in;            /* NHWC [n,h,w,cin]; UP: the skip tensor */
+    const float* up_t;          /* UP: [n,h/2,w/2,cin], the up-sampling layer's raw 1x1 output */
+    const float* up_noise;      /* UP: [h][noise_pitch] added before the prologue's activation, or NULL */
+    const float* up_fir;        /* UP: [4][4] channel-uniform FIR taps */
+    const float* x;             /* STEM: NCHW [n,4,h,w] */
+    const float* fromrgb_w;     /* STEM: [cin,4] */
+    const float* fromrgb_b;     /* STEM: [cin] */
+    const void* a_hi;           /* SPLIT: fp16 [n,h,w,cin], 64 * activation split into hi + lo */
+    const void* a_lo;
+    const float* dw_w;          /* depthwise [cin,1,3,3] */
+    const float* dw_b;          /* [cin] */
+    const float* pw_w;          /* pointwise [cout,cin]; NULL plans only (no device is touched; needs sms > 0) */
+    const float* noise;         /* [h][noise_pitch] added before the epilogue's activation, or NULL */
+    int noise_pitch;            /* floats, a multiple of 4, >= w */
+    int torgb;                  /* fuse torgb + image into the epilogue */
+    const float* rgb_w;         /* [3,cout] */
+    const float* rgb_b;         /* [3] */
+    const float* rgb_fir;       /* [3,4,4] image up-sampling taps (read if img_lo != NULL) */
+    const float* img_lo;        /* [n,3,h/2,w/2] or NULL */
+    float* img_out;             /* [n,3,h,w] */
+    int store_out;              /* with torgb: 0 writes no feature map */
+    float* out;                 /* NHWC [n,h,w,cout] */
+} migan_sepconv_tc_io;
+
+typedef struct migan_sepconv_tc_plan {
+    int n_group, in_stages, a_stages, b_stages, b_resident, dw_global;
+    int tile_w, tile_h, tile_n, n_tile, grid, num_tiles;
+    int num_candidates;         /* length of the planner's candidate list for these shapes */
+} migan_sepconv_tc_plan;
+
+/* Plans (and, unless io->pw_w is NULL, runs to completion on `stream`) one launch.  sms: SMs of the persistent grid
+ * (0: what a forward uses, the device's minus MIGAN_TC_RESERVE_SMS).  candidate: -1 the planner's choice, i >= 0 the
+ * i-th entry of its candidate list (MIGAN_ERR_INVALID if that layout does not fit).  `plan` receives the record. */
+int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate, migan_sepconv_tc_plan* plan, void* stream);
+
 /* upfirdn2d(x[n,c,h,w], f[fh,fw]) -> y[n,c,oh,ow], oh = (h*upy + pady0 + pady1 - fh + downy) / downy
  * (upfirdn2d.cpp:32-33).  f == NULL means the 1x1 identity filter.  Device pointers. */
 int b200_upfirdn2d(const float* x, const float* f, float* y, int n, int c, int h, int w, int fh, int fw,

@@ -43,6 +43,27 @@ class WindowRequest(ctypes.Structure):
                 ("y", c_void_p), ("Hp", c_int), ("Wp", c_int), ("out", c_void_p)]
 
 
+class SepconvTcIO(ctypes.Structure):
+    """migan_sepconv_tc_io: the operands of one tensor-core SeparableConv2d launch (test hook)."""
+    _fields_ = [("source", c_int), ("n", c_int), ("h", c_int), ("w", c_int), ("cin", c_int), ("cout", c_int),
+                ("act", c_int), ("passes", c_int), ("in_", c_void_p), ("up_t", c_void_p), ("up_noise", c_void_p),
+                ("up_fir", c_void_p), ("x", c_void_p), ("fromrgb_w", c_void_p), ("fromrgb_b", c_void_p),
+                ("a_hi", c_void_p), ("a_lo", c_void_p), ("dw_w", c_void_p), ("dw_b", c_void_p), ("pw_w", c_void_p),
+                ("noise", c_void_p), ("noise_pitch", c_int), ("torgb", c_int), ("rgb_w", c_void_p), ("rgb_b", c_void_p),
+                ("rgb_fir", c_void_p), ("img_lo", c_void_p), ("img_out", c_void_p), ("store_out", c_int),
+                ("out", c_void_p)]
+
+
+class SepconvTcPlan(ctypes.Structure):
+    """migan_sepconv_tc_plan: what the planner chose for one launch."""
+    _fields_ = [(name, c_int) for name in ("n_group", "in_stages", "a_stages", "b_stages", "b_resident", "dw_global",
+                                           "tile_w", "tile_h", "tile_n", "n_tile", "grid", "num_tiles",
+                                           "num_candidates")]
+
+    def as_dict(self):
+        return {name: getattr(self, name) for name, _ in self._fields_}
+
+
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("migan_last_error", c_char_p, []),
@@ -111,6 +132,7 @@ SYMBOLS = [
     ("migan_set_tap", c_int, [c_void_p, c_char_p, c_void_p]),
     ("migan_tap_info", c_int, [c_void_p, c_int, c_int, POINTER(c_char_p), POINTER(c_int)]),
     ("migan_debug_tc_timeout", c_int, [c_int]),
+    ("migan_debug_sepconv_tc", c_int, [POINTER(SepconvTcIO), c_int, c_int, POINTER(SepconvTcPlan), c_void_p]),
     ("b200_upfirdn2d", c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 14 + [c_int, c_float, c_void_p]),
     ("b200_conv1x1_nhwc", c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     ("b200_bias_act", c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_float, c_float, c_float, c_void_p]),

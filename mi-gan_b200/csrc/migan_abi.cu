@@ -49,6 +49,54 @@ int fail(int code, const char* fmt, ...) {
 inline int channels(int res) { return std::min(32768 / res, 512); }  // migan_inference.py:222-223
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// ---- operand packing of the tensor-core SeparableConv2d kernel (sepconv_tc.h), shared by the weight loader and the
+// single-launch test hook (migan_debug_sepconv_tc) so that a test runs on exactly the tables a forward uses ----
+constexpr float kSqrt2 = 1.41421356237309515f;
+
+// depthwise taps [cin,1,3,3] -> [9][cin] and bias [cin], both * kActSplitScale * sqrt 2 (gain and fp16-split scale
+// folded into the prologue)
+void pack_dw_tc(const float* w, const float* b, int cin, float* w9, float* bias) {
+    const float S = 64.0f /* kActSplitScale */ * kSqrt2;
+    for (int c = 0; c < cin; ++c)
+        for (int t = 0; t < 9; ++t) w9[t * cin + c] = w[c * 9 + t] * S;
+    for (int c = 0; c < cin; ++c) bias[c] = b[c] * S;
+}
+
+// pointwise [cout,cin] -> fp16 hi / lo [cout][cin] of w * 2^k2 (round to nearest); returns the epilogue's
+// 1 / (kActSplitScale * 2^k2).  The power-of-two scale puts the largest weight in [8192, 16384): hi and lo both stay
+// well inside fp16's normal range, and the scale is undone exactly in the epilogue.
+float pack_pw_split(const float* w, int cout, int cin, __half* hi, __half* lo) {
+    float maxabs = 0.f;
+    for (size_t i = 0; i < (size_t)cin * cout; ++i)
+        if (std::isfinite(w[i])) maxabs = std::max(maxabs, std::fabs(w[i]));
+    int k2 = 0;
+    if (maxabs > 0.f) k2 = (int)std::floor(std::log2(16384.0 / (double)maxabs));
+    k2 = std::max(-14, std::min(24, k2));
+    const float wscale = std::ldexp(1.0f, k2);
+    for (size_t i = 0; i < (size_t)cin * cout; ++i) {
+        const float s = w[i] * wscale;
+        const __half h = __float2half_rn(s);
+        hi[i] = h;
+        lo[i] = __float2half_rn(s - __half2float(h));
+    }
+    return 1.0f / (wscale * 64.0f /* kActSplitScale */);
+}
+
+// * sqrt 2: the up-sampling taps, noise planes and fromrgb weights that the fused prologues use with the gain folded in
+void scale_sqrt2(const float* src, size_t count, float* dst) {
+    for (size_t i = 0; i < count; ++i) dst[i] = src[i] * kSqrt2;
+}
+
+// torgb tables of the fused epilogue: weights [3][cout] as they are, bias padded to 4, image FIR [3][16] -> [16][3]
+void pack_torgb(const float* w, const float* b, const float* fir, int cout, float* w_out, float* b_out, float* fir_out) {
+    memcpy(w_out, w, sizeof(float) * 3 * cout);
+    memcpy(b_out, b, sizeof(float) * 3);
+    b_out[3] = 0.f;
+    if (fir)
+        for (int c = 0; c < 3; ++c)
+            for (int k = 0; k < 16; ++k) fir_out[k * 3 + c] = fir[c * 16 + k];
+}
+
 struct WeightSpec {
     std::string name;
     int ndim;
@@ -452,47 +500,26 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
         fix.push_back({reinterpret_cast<void**>(&L.bias), off});
     }
     {   // wgmma prologue: activation gain and fp16-split scale folded into the depthwise taps
-        const float S = 64.0f /* kActSplitScale */ * 1.41421356237309515f;
         const std::vector<float>& w = W(ctx, L.p + "conv1.weight");
         const std::vector<float>& b = W(ctx, L.p + "conv1.bias");
         size_t off = ab.alloc(sizeof(float) * 9 * cin);
-        float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        for (int c = 0; c < cin; ++c)
-            for (int t = 0; t < 9; ++t) d[t * cin + c] = w[c * 9 + t] * S;
-        fix.push_back({reinterpret_cast<void**>(&L.w9_tc), off});
         size_t offb = ab.alloc(sizeof(float) * cin);
-        float* db = reinterpret_cast<float*>(ab.bytes.data() + offb);
-        for (int c = 0; c < cin; ++c) db[c] = b[c] * S;
+        pack_dw_tc(w.data(), b.data(), cin, reinterpret_cast<float*>(ab.bytes.data() + off),
+                   reinterpret_cast<float*>(ab.bytes.data() + offb));
+        fix.push_back({reinterpret_cast<void**>(&L.w9_tc), off});
         fix.push_back({reinterpret_cast<void**>(&L.bias_tc), offb});
     }
     {   // pointwise [cout,cin,1,1] -> fp32 [cin][cout] and fp16 hi/lo [cout][cin]
         const std::vector<float>& w = W(ctx, L.p + "conv2.weight");
         size_t off = ab.alloc(sizeof(float) * cin * cout);
         float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        float maxabs = 0.f;
         for (int o = 0; o < cout; ++o)
-            for (int k = 0; k < cin; ++k) {
-                d[(size_t)k * cout + o] = w[(size_t)o * cin + k];
-                if (std::isfinite(w[(size_t)o * cin + k])) maxabs = std::max(maxabs, std::fabs(w[(size_t)o * cin + k]));
-            }
+            for (int k = 0; k < cin; ++k) d[(size_t)k * cout + o] = w[(size_t)o * cin + k];
         fix.push_back({reinterpret_cast<void**>(&L.pw_t), off});
-        // power-of-two scale so the largest weight lands in [8192, 16384): hi and lo both stay
-        // well inside fp16's normal range, and the scale is undone exactly in the epilogue.
-        int k2 = 0;
-        if (maxabs > 0.f) k2 = (int)std::floor(std::log2(16384.0 / (double)maxabs));
-        k2 = std::max(-14, std::min(24, k2));
-        const float wscale = std::ldexp(1.0f, k2);
-        L.tc_inv_scale = 1.0f / (wscale * 64.0f /* kActSplitScale */);
         size_t off_hi = ab.alloc(sizeof(__half) * cin * cout);
         size_t off_lo = ab.alloc(sizeof(__half) * cin * cout);
-        __half* hi = reinterpret_cast<__half*>(ab.bytes.data() + off_hi);
-        __half* lo = reinterpret_cast<__half*>(ab.bytes.data() + off_lo);
-        for (size_t i = 0; i < (size_t)cin * cout; ++i) {
-            const float s = w[i] * wscale;
-            const __half h = __float2half_rn(s);
-            hi[i] = h;
-            lo[i] = __float2half_rn(s - __half2float(h));
-        }
+        L.tc_inv_scale = pack_pw_split(w.data(), cout, cin, reinterpret_cast<__half*>(ab.bytes.data() + off_hi),
+                                       reinterpret_cast<__half*>(ab.bytes.data() + off_lo));
         fix.push_back({reinterpret_cast<void**>(&L.pw_hi), off_hi});
         fix.push_back({reinterpret_cast<void**>(&L.pw_lo), off_lo});
     }
@@ -509,7 +536,7 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
             for (int c = 1; c < cf && L.up_uniform; ++c)
                 for (int t = 0; t < 16; ++t)
                     if (f[c * 16 + t] != f[t]) { L.up_uniform = false; break; }
-            for (int t = 0; t < 16; ++t) L.up_taps_s2[t] = f[t] * 1.41421356237309515f;
+            scale_sqrt2(f.data(), 16, L.up_taps_s2);
         }
     }
     if (L.up) {
@@ -532,8 +559,7 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
         fix.push_back({reinterpret_cast<void**>(&L.noise_dev), off});
         if (L.up) {
             size_t off2 = ab.alloc(sizeof(float) * nc.size());
-            float* d2 = reinterpret_cast<float*>(ab.bytes.data() + off2);
-            for (size_t i = 0; i < nc.size(); ++i) d2[i] = nc[i] * ns * 1.41421356237309515f;
+            scale_sqrt2(reinterpret_cast<const float*>(ab.bytes.data() + off), nc.size(), reinterpret_cast<float*>(ab.bytes.data() + off2));
             fix.push_back({reinterpret_cast<void**>(&L.noise_s2_dev), off2});
         }
     }
@@ -558,10 +584,8 @@ int migan_finalize_weights(migan_ctx* ctx) {
         fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_w), ow});
         fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_b), ob});
         size_t ow2 = ab.alloc(sizeof(float) * w.size()), ob2 = ab.alloc(sizeof(float) * b.size());
-        float* dw2 = reinterpret_cast<float*>(ab.bytes.data() + ow2);
-        float* db2 = reinterpret_cast<float*>(ab.bytes.data() + ob2);
-        for (size_t i = 0; i < w.size(); ++i) dw2[i] = w[i] * 1.41421356237309515f;
-        for (size_t i = 0; i < b.size(); ++i) db2[i] = b[i] * 1.41421356237309515f;
+        scale_sqrt2(w.data(), w.size(), reinterpret_cast<float*>(ab.bytes.data() + ow2));
+        scale_sqrt2(b.data(), b.size(), reinterpret_cast<float*>(ab.bytes.data() + ob2));
         fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_w_s2), ow2});
         fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_b_s2), ob2});
     }
@@ -574,24 +598,23 @@ int migan_finalize_weights(migan_ctx* ctx) {
         const std::vector<float>& w = W(ctx, t.p + "torgb.weight");
         const std::vector<float>& b = W(ctx, t.p + "torgb.bias");
         size_t ow = ab.alloc(sizeof(float) * w.size());
-        memcpy(ab.bytes.data() + ow, w.data(), sizeof(float) * w.size());
         size_t ob = ab.alloc(sizeof(float) * 4);
-        memcpy(ab.bytes.data() + ob, b.data(), sizeof(float) * 3);
         fix.push_back({reinterpret_cast<void**>(&t.w), ow});
         fix.push_back({reinterpret_cast<void**>(&t.b), ob});
+        const float* f = nullptr;
+        size_t of = 0;
         if (t.has_up) {
             const std::vector<float>& fc = W(ctx, t.p + "upsample.filter_const");
             for (int y = 0; y < t.res; ++y)
                 for (int x = 0; x < t.res; ++x)
                     if (fc[(size_t)y * t.res + x] != (((y | x) & 1) ? 0.f : 1.f))
                         return fail(MIGAN_ERR_INVALID, "%supsample.filter_const is not the zero-insertion pattern", t.p.c_str());
-            const std::vector<float>& f = W(ctx, t.p + "upsample.filter.weight");
-            size_t of = ab.alloc(sizeof(float) * 48);
-            float* d = reinterpret_cast<float*>(ab.bytes.data() + of);
-            for (int c = 0; c < 3; ++c)
-                for (int k = 0; k < 16; ++k) d[k * 3 + c] = f[c * 16 + k];
+            f = W(ctx, t.p + "upsample.filter.weight").data();
+            of = ab.alloc(sizeof(float) * 48);
             fix.push_back({reinterpret_cast<void**>(&t.fir), of});
         }
+        pack_torgb(w.data(), b.data(), f, (int)(w.size() / 3), reinterpret_cast<float*>(ab.bytes.data() + ow),
+                   reinterpret_cast<float*>(ab.bytes.data() + ob), f ? reinterpret_cast<float*>(ab.bytes.data() + of) : nullptr);
     }
     CUDA_TRY(cudaSetDevice(ctx->device));
     if (ctx->arena) {
@@ -1734,6 +1757,103 @@ int migan_tap_info(const migan_ctx* ctx, int path, int index, const char** name,
 }
 
 int migan_debug_tc_timeout(int device) { return migan::sepconv_tc_timeout_record(device); }
+
+int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate, migan_sepconv_tc_plan* plan, void* stream) {
+    if (!io) return fail(MIGAN_ERR_INVALID, "sepconv_tc: null io");
+    if (io->source < migan::SEPCONV_SRC_NHWC || io->source > migan::SEPCONV_SRC_STEM) return fail(MIGAN_ERR_INVALID, "sepconv_tc: bad source %d", io->source);
+    if (io->passes != 1 && io->passes != 3) return fail(MIGAN_ERR_INVALID, "sepconv_tc: passes must be 1 or 3");
+    if (io->n < 1 || io->h < 1 || io->w < 1 || io->cin < 1 || io->cout < 1) return fail(MIGAN_ERR_INVALID, "sepconv_tc: bad shape");
+    const bool run = io->pw_w != nullptr;
+    if (!run && sms < 1) return fail(MIGAN_ERR_INVALID, "sepconv_tc: planning without a device needs an explicit sms");
+    const int n = io->n, h = io->h, w = io->w, cin = io->cin, cout = io->cout;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    migan::SepconvTcDesc d;
+    d.passes = io->passes; d.source = io->source; d.n = n; d.h = h; d.w = w; d.cin = cin; d.cout = cout; d.act = io->act;
+    d.noise_pitch = io->noise_pitch;
+    migan::SepconvTcRgb rgb{};
+    if (io->torgb) d.rgb = &rgb;
+    migan::SepconvTcPlanInfo info{};
+    auto record = [&]() {
+        if (plan) *plan = {info.n_group, info.in_stages, info.a_stages, info.b_stages, info.b_resident, info.dw_global,
+                           info.tile_w, info.tile_h, info.tile_n, info.n_tile, info.grid, info.num_tiles, info.num_candidates};
+    };
+    if (!run) {
+        if (const char* err = migan::sepconv_tc_plan_debug(nullptr, d, sms, candidate, &info)) return fail(MIGAN_ERR_INVALID, "sepconv_tc: %s", err);
+        record();
+        return MIGAN_OK;
+    }
+    int dev = 0, dev_sms = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, dev));
+    if (sms < 0 || sms > dev_sms) return fail(MIGAN_ERR_INVALID, "sepconv_tc: sms must be in 0..%d, got %d", dev_sms, sms);
+    CUDA_TRY(migan::configure_sepconv_tc());
+    const bool dwsrc = io->source != migan::SEPCONV_SRC_SPLIT;
+    const bool up = io->source == migan::SEPCONV_SRC_UP, stem = io->source == migan::SEPCONV_SRC_STEM;
+    // the caller's operands, fetched after the work already queued on `stream`
+    auto fetch = [&](const float* src, size_t count) {
+        std::vector<float> v(count);
+        if (count && cudaMemcpyAsync(v.data(), src, count * sizeof(float), cudaMemcpyDeviceToHost, st) != cudaSuccess) v.clear();
+        return v;
+    };
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const size_t cc = (size_t)cin * cout;
+    const std::vector<float> dw_w = dwsrc ? fetch(io->dw_w, 9 * (size_t)cin) : std::vector<float>();
+    const std::vector<float> dw_b = dwsrc ? fetch(io->dw_b, cin) : std::vector<float>();
+    const std::vector<float> pw_w = fetch(io->pw_w, cc);
+    const std::vector<float> up_fir = up ? fetch(io->up_fir, 16) : std::vector<float>();
+    const std::vector<float> up_noise = up && io->up_noise ? fetch(io->up_noise, (size_t)h * io->noise_pitch) : std::vector<float>();
+    const std::vector<float> rgb_w = io->torgb ? fetch(io->rgb_w, 3 * (size_t)cout) : std::vector<float>();
+    const std::vector<float> rgb_b = io->torgb ? fetch(io->rgb_b, 3) : std::vector<float>();
+    const std::vector<float> rgb_fir = io->torgb && io->img_lo ? fetch(io->rgb_fir, 48) : std::vector<float>();
+    const std::vector<float> st_w = stem ? fetch(io->fromrgb_w, 4 * (size_t)cin) : std::vector<float>();
+    const std::vector<float> st_b = stem ? fetch(io->fromrgb_b, cin) : std::vector<float>();
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (pw_w.size() != cc || (dwsrc && (dw_w.empty() || dw_b.empty())) || (up && up_fir.empty()) ||
+        (stem && (st_w.empty() || st_b.empty())) || (io->torgb && (rgb_w.empty() || rgb_b.empty())) ||
+        (up && io->up_noise && up_noise.empty()) || (io->torgb && io->img_lo && rgb_fir.empty()))
+        return fail(MIGAN_ERR_INVALID, "sepconv_tc: an operand the source needs is missing or unreadable");
+    // packed tables, one host buffer -> one device allocation
+    std::vector<unsigned char> host;
+    auto alloc = [&](size_t bytes) { const size_t off = host.size(); host.resize(off + align_up(bytes, 256)); return off; };
+    const size_t o_w9 = alloc(sizeof(float) * 9 * cin), o_b = alloc(sizeof(float) * cin);
+    const size_t o_hi = alloc(sizeof(__half) * cc), o_lo = alloc(sizeof(__half) * cc);
+    const size_t o_sw = alloc(sizeof(float) * st_w.size()), o_sb = alloc(sizeof(float) * st_b.size());
+    const size_t o_nz = alloc(sizeof(float) * up_noise.size());
+    const size_t o_rw = alloc(sizeof(float) * 3 * cout), o_rb = alloc(sizeof(float) * 4), o_rf = alloc(sizeof(float) * 48);
+    auto hf = [&](size_t off) { return reinterpret_cast<float*>(host.data() + off); };
+    if (dwsrc) pack_dw_tc(dw_w.data(), dw_b.data(), cin, hf(o_w9), hf(o_b));
+    d.inv_scale = pack_pw_split(pw_w.data(), cout, cin, reinterpret_cast<__half*>(host.data() + o_hi), reinterpret_cast<__half*>(host.data() + o_lo));
+    if (stem) { scale_sqrt2(st_w.data(), st_w.size(), hf(o_sw)); scale_sqrt2(st_b.data(), st_b.size(), hf(o_sb)); }
+    if (up) scale_sqrt2(up_fir.data(), 16, d.up_taps);
+    if (!up_noise.empty()) scale_sqrt2(up_noise.data(), up_noise.size(), hf(o_nz));
+    if (io->torgb) pack_torgb(rgb_w.data(), rgb_b.data(), rgb_fir.empty() ? nullptr : rgb_fir.data(), cout, hf(o_rw), hf(o_rb), hf(o_rf));
+    unsigned char* dbuf = nullptr;
+    CUDA_TRY(cudaMalloc(&dbuf, host.size()));
+    std::unique_ptr<unsigned char, decltype(&cudaFree)> hold(dbuf, &cudaFree);
+    CUDA_TRY(cudaMemcpy(dbuf, host.data(), host.size(), cudaMemcpyHostToDevice));
+    auto df = [&](size_t off) { return reinterpret_cast<float*>(dbuf + off); };
+    d.in_f32 = io->in;
+    d.a_hi = static_cast<const __half*>(io->a_hi); d.a_lo = static_cast<const __half*>(io->a_lo);
+    if (dwsrc) { d.w9 = df(o_w9); d.bias = df(o_b); }
+    d.w_hi = reinterpret_cast<const __half*>(dbuf + o_hi); d.w_lo = reinterpret_cast<const __half*>(dbuf + o_lo);
+    d.noise = io->noise; d.out = io->out;
+    if (up) { d.up_t = io->up_t; d.up_noise = up_noise.empty() ? nullptr : df(o_nz); }
+    if (stem) { d.stem_w = df(o_sw); d.stem_b = df(o_sb); }
+    if (io->torgb) {
+        rgb.w = df(o_rw); rgb.b = df(o_rb); rgb.fir = df(o_rf);
+        rgb.img_lo = io->img_lo; rgb.img_out = io->img_out; rgb.store_out = io->store_out;
+        if (!io->img_out) return fail(MIGAN_ERR_INVALID, "sepconv_tc: torgb needs img_out");
+    }
+    if (stem && !io->x) return fail(MIGAN_ERR_INVALID, "sepconv_tc: the stem source needs x");
+    migan::SepconvTcArgs args;
+    if (const char* err = migan::sepconv_tc_plan_debug(&args, d, sms, candidate, &info)) return fail(MIGAN_ERR_INVALID, "sepconv_tc: %s", err);
+    record();
+    CUDA_TRY(migan::launch_sepconv_tc(args, st, nullptr, io->x));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess)
+        return fail(MIGAN_ERR_CUDA, "sepconv_tc launch failed: %s (timeout record %d)", cudaGetErrorString(e), migan::sepconv_tc_timeout_record(dev));
+    return MIGAN_OK;
+}
 
 int b200_upfirdn2d(const float* x, const float* f, float* y, int n, int c, int h, int w, int fh, int fw,
                    int upx, int upy, int downx, int downy, int padx0, int padx1, int pady0, int pady1,

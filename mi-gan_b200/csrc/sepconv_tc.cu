@@ -706,7 +706,9 @@ int grid_sms() {
 
 // Tiling, N grouping, ring depths and shared-memory layout of a launch.  They depend on the shapes, the source and
 // whether torgb is fused, never on a pointer, so the generator's planner can ask before it commits to fusing torgb.
-const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& smem_bytes) {
+// candidate < 0 takes the first candidate layout that fits (production); candidate = i takes the i-th or fails (tests).
+const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& smem_bytes, int candidate = -1,
+                        int* num_candidates = nullptr, bool* dw_global = nullptr) {
     const int n = d.n, h = d.h, w = d.w, cin = d.cin, cout = d.cout;
     if (cin % kKBlock != 0 || cout % 64 != 0) return "cin must be a multiple of 64 and cout of 64";
     if (h < 4 || w < 4) return "extents must be >= 4";
@@ -798,11 +800,18 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
                 for (int a_st : {4, dw ? 2 : 3}) cands.push_back({1, in_st, bs, a_st, false});
         }
     }
+    if (num_candidates) *num_candidates = (int)cands.size();
+    if (candidate >= (int)cands.size()) return "no such candidate layout";
     bool found = false;
-    for (const Cand& c : cands) {
+    for (size_t i = candidate < 0 ? 0 : (size_t)candidate; i < cands.size(); ++i) {
+        const Cand& c = cands[i];
         const uint32_t tab = c.dw_global ? 0u : tables;
         const uint32_t total = (uint32_t)c.in_stages * p.in_stage_stride + (uint32_t)c.a_stages * kAStage + (uint32_t)c.b_stages * b_stage + tab;
-        if (total > budget) continue;
+        if (total > budget) {
+            if (candidate >= 0) return "candidate layout exceeds the shared-memory budget";
+            continue;
+        }
+        if (dw_global) *dw_global = c.dw_global;
         p.n_group = c.n_group;
         p.in_stages = c.in_stages; p.a_stages = c.a_stages; p.b_stages = c.b_stages;
         p.off_in = 0;
@@ -836,18 +845,28 @@ bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d) {
     return plan_layout(p, q, grid_sms(), smem_bytes) == nullptr;
 }
 
-const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
+namespace {
+
+const char* plan_launch(SepconvTcArgs* args, const SepconvTcDesc& d, int sms, int candidate, SepconvTcPlanInfo* info) {
     Params p;
     memset(&p, 0, sizeof(p));
     const int n = d.n, h = d.h, w = d.w, cin = d.cin, cout = d.cout;
     const bool dw = (d.source != SEPCONV_SRC_SPLIT);
-    if (d.source == SEPCONV_SRC_SPLIT && !(d.a_hi && d.a_lo)) return "no A operand";
-    if ((d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) && !d.in_f32) return "no input tensor";
-    if (d.source == SEPCONV_SRC_UP && !d.up_t) return "no low-resolution tensor for the up-sampling prologue";
-    if (d.source == SEPCONV_SRC_STEM && !(d.stem_w && d.stem_b)) return "no fromrgb weights for the stem prologue";
-    const int sms = grid_sms();
+    if (args) {
+        if (d.source == SEPCONV_SRC_SPLIT && !(d.a_hi && d.a_lo)) return "no A operand";
+        if ((d.source == SEPCONV_SRC_NHWC || d.source == SEPCONV_SRC_UP) && !d.in_f32) return "no input tensor";
+        if (d.source == SEPCONV_SRC_UP && !d.up_t) return "no low-resolution tensor for the up-sampling prologue";
+        if (d.source == SEPCONV_SRC_STEM && !(d.stem_w && d.stem_b)) return "no fromrgb weights for the stem prologue";
+    }
     uint32_t smem_bytes = 0;
-    if (const char* err = plan_layout(p, d, sms, smem_bytes)) return err;
+    int num_candidates = 0;
+    bool dw_global = false;
+    if (const char* err = plan_layout(p, d, sms, smem_bytes, candidate, &num_candidates, &dw_global)) return err;
+    if (info) {
+        *info = {p.n_group, p.in_stages, p.a_stages, p.b_stages, p.b_resident, dw_global ? 1 : 0,
+                 p.tile_w, p.tile_h, p.tile_n, p.n_tile, std::min(p.num_tiles, sms), p.num_tiles, num_candidates};
+    }
+    if (!args) return nullptr;
     p.w9 = d.w9; p.bias = d.bias; p.noise = d.noise; p.inv_scale = d.inv_scale; p.out = d.out;
     if (d.source == SEPCONV_SRC_UP) memcpy(p.up_taps.f, d.up_taps, sizeof(p.up_taps.f));
     if (d.source == SEPCONV_SRC_STEM) { p.stem_w = d.stem_w; p.stem_b = d.stem_b; }
@@ -904,6 +923,18 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
     args->bound_x = nullptr;
     memcpy(args->params_blob, &p, sizeof(p));
     return nullptr;
+}
+
+}  // namespace
+
+const char* sepconv_tc_plan_ex(SepconvTcArgs* args, const SepconvTcDesc& d) {
+    return plan_launch(args, d, grid_sms(), -1, nullptr);
+}
+
+const char* sepconv_tc_plan_debug(SepconvTcArgs* args, const SepconvTcDesc& d, int sms, int candidate, SepconvTcPlanInfo* info) {
+    if (sms == 0) sms = grid_sms();
+    if (sms < 1) return "sms must be >= 1";
+    return plan_launch(args, d, sms, candidate, info);
 }
 
 const char* sepconv_tc_plan(SepconvTcArgs* args, int passes, const float* in_f32, const __half* a_hi, const __half* a_lo,

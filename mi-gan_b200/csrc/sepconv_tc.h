@@ -65,6 +65,17 @@ struct SepconvTcDesc {
 
 // Returns nullptr on success, else an error string.
 const char* sepconv_tc_plan_ex(SepconvTcArgs* a, const SepconvTcDesc& d);
+
+// What the planner chose for one launch (tests enumerate schedules with it).
+struct SepconvTcPlanInfo {
+    int n_group, in_stages, a_stages, b_stages, b_resident, dw_global;
+    int tile_w, tile_h, tile_n, n_tile, grid, num_tiles, num_candidates;
+};
+// sepconv_tc_plan_ex with the planner's two inputs made explicit, for tests: `sms` SMs for the persistent grid (0: the
+// device's minus MIGAN_TC_RESERVE_SMS, as in production) and, if candidate >= 0, the candidate-th layout of the planner's own
+// preference list (an error if it does not fit) instead of the first that fits.  a == nullptr plans only: no tensor
+// map, no pointer and no CUDA call.
+const char* sepconv_tc_plan_debug(SepconvTcArgs* a, const SepconvTcDesc& d, int sms, int candidate, SepconvTcPlanInfo* info);
 // Whether a launch with d's shapes and source can fuse torgb, i.e. hold all of cout in one CTA tile (d.rgb and the
 // pointers are not read).
 bool sepconv_tc_fuses_rgb(const SepconvTcDesc& d);

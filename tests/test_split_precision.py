@@ -11,23 +11,7 @@ The 1x1 convs run on fp16 tensor cores as  Ah*Bh + Al*Bh + Ah*Bl  with fp32 accu
 """
 import numpy as np
 
-
-def split_trunc(s):
-    """Prologue split (sepconv_tc.cu split_pack2): hi = s with the low 13 mantissa bits cleared, lo = fp16(s - hi)."""
-    s = s.astype(np.float32)
-    hi32 = (s.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
-    hi = hi32.astype(np.float16)
-    assert np.array_equal(hi.astype(np.float32), hi32)          # exactly representable
-    lo = (s - hi32).astype(np.float16)
-    return hi, lo
-
-
-def split_round(s):
-    """Host-side weight split (migan_abi.cu pack_sepconv): hi = fp16(s), lo = fp16(s - hi)."""
-    s = s.astype(np.float32)
-    hi = s.astype(np.float16)
-    lo = (s - hi.astype(np.float32)).astype(np.float16)
-    return hi, lo
+from oracle.sepconv_oracle import split_round, split_trunc
 
 
 def dot32(a16, b16):
@@ -69,6 +53,9 @@ def test_truncation_split_keeps_22_bits():
     s = (rng.standard_normal(100000) * 300).astype(np.float32)
     s = np.clip(s, -16384, 16384)
     hi, lo = split_trunc(s)
+    hi32 = (s.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+    normal = np.abs(s) >= 2.0 ** -14
+    assert np.array_equal(hi.astype(np.float32)[normal], hi32[normal])     # hi is exact in fp16
     rec = hi.astype(np.float64) + lo.astype(np.float64)
     err = np.abs(rec - s.astype(np.float64))
     assert np.all(err <= np.maximum(2.0 ** -22 * np.abs(s), 2.0 ** -25))
