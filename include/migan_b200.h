@@ -228,6 +228,21 @@ int b200_demo_preprocess(const migan_demo_request* reqs_host, int n, int resolut
 int b200_demo_postprocess(const float* y_n3rr, const migan_demo_request* reqs_host, int n, int resolution, void* scratch,
                           size_t scratch_bytes, void* stream);
 
+/* The evaluation batch of scripts/evaluate_fid_lpips.py (InferenceDataset and :246-249) on the demo path's stages, for
+ * 1..MIGAN_PIPE_MAX_BATCH requests of migan_demo_request (out, out_w and out_h are not read):
+ *   b200_eval_preprocess   photo -> PIL BICUBIC to R x R when it is not that size (one resize of both axes), mask ->
+ *                          PIL NEAREST to R x R and the demo's per-pixel steps (L: 255 known) -> x[i] of x [n,4,R,R], and
+ *                          the unmasked photo v * 2 / 255 - 1 -> img[i] of img [n,3,R,R].  Scratch:
+ *                          b200_eval_scratch_bytes (0 on a bad argument).
+ *   [generator]
+ *   b200_eval_composite    composed = m * img + (1 - m) * y (m = x channel 0 + 0.5), then (v * 0.5 + 0.5).clamp(0, 1) of
+ *                          img, in place (the script's `imgs`), and of composed, each product and sum rounded on its own. */
+size_t b200_eval_scratch_bytes(const migan_demo_request* reqs_host, int n, int resolution);
+int b200_eval_preprocess(const migan_demo_request* reqs_host, int n, int resolution, float* x_n4rr, float* img_n3rr,
+                         void* scratch, size_t scratch_bytes, void* stream);
+int b200_eval_composite(const float* x_n4rr, const float* y_n3rr, int n, int resolution, float* img_n3rr,
+                        float* composed_n3rr, void* stream);
+
 /* Full-resolution request path: a photo of ANY size (H, W >= 1) inpainted at its own resolution by migan_forward_hw.
  *   migan_fullres_extent   the padded extent Hp = max(R, q ceil(H / q)), Wp likewise (q = R / 4): the smallest size
  *                          migan_forward_hw accepts that holds the photo (a valid size is not padded), and the largest batch
@@ -300,6 +315,45 @@ typedef struct {
 } migan_window_request;
 int b200_window_preprocess(const migan_window_request* reqs_host, int n, void* stream);
 int b200_window_postprocess(const migan_window_request* reqs_host, int n, void* stream);
+
+/* Free-form masks of the evaluation protocol: RandomMask(s) of scripts/generate_masks.py (hole_range [0, 1]), byte for
+ * byte and at the same position of numpy's legacy global stream.  One RandomMask result is the first *attempt* whose hole
+ * count lies in (0, s^2); an attempt's draws never depend on earlier results, so the stream is a fixed sequence of
+ * attempts:
+ *   migan_np_seed            HOST: np.random.seed(seed) for an integer seed (MT19937 init_genrand, no cached gaussian).
+ *   migan_mask_plan          HOST: the draws of the next n_attempts attempts of RandomMask(s), from *state (advanced):
+ *                            one migan_mask_record each (records_host), and, when states_host is not NULL, the state
+ *                            after each attempt (states_host[k]: after attempt k) so the caller can rewind to the last
+ *                            attempt it uses.
+ *   b200_mask_raster         DEVICE: paints every attempt into attempts [n_attempts][s][s] (16-byte aligned; 255 known, 0 hole; Pillow's
+ *                            wide-line polygons and ellipse stamps, exact) and writes its hole count to holes[k].
+ *   b200_mask_compact        DEVICE: copies the first min(n, accepted) accepted attempts (0 < holes < s^2), in attempt
+ *                            order, to out [n][s][s].
+ * s: MIGAN_MASK_MIN_SIZE..MIGAN_MASK_MAX_SIZE; n_attempts: 1..MIGAN_MASK_MAX_ATTEMPTS per call. */
+#define MIGAN_MASK_MIN_SIZE 2
+#define MIGAN_MASK_MAX_SIZE 4096
+#define MIGAN_MASK_MAX_ATTEMPTS 65535
+#define MIGAN_MASK_MAX_RECTS 13       /* randint(10) + randint(5) rectangles */
+#define MIGAN_MASK_MAX_SEGMENTS 323   /* randint(20) brush tries x (randint(4, 18) segments) */
+#define MIGAN_MASK_MAX_DISCS 342      /* the same tries x (segments + 1) vertex discs */
+typedef struct {
+    uint32_t key[624];     /* np.random.get_state()[1] */
+    int pos;               /* [2] */
+    int has_gauss;         /* [3] */
+    double gauss;          /* [4] */
+} migan_np_random;
+typedef struct {
+    int32_t n_rects, n_segments, n_discs;
+    int32_t flips;                                  /* bit 0: brush rows flipped, bit 1: brush columns (not the rects) */
+    int16_t rects[MIGAN_MASK_MAX_RECTS][4];         /* y0, y1, x0, x1: rows [y0, y1) x columns [x0, x1) become holes */
+    int16_t quads[MIGAN_MASK_MAX_SEGMENTS][8];      /* Pillow's wide-line quad, (x, y) x 4; 4 equal vertices: one pixel */
+    int16_t discs[MIGAN_MASK_MAX_DISCS][4];         /* x, y, r (6..23), 0 */
+} migan_mask_record;
+int migan_np_seed(migan_np_random* state, uint32_t seed);
+int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_record* records_host,
+                    migan_np_random* states_host);
+int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream);
+int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream);
 
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0

@@ -7,16 +7,21 @@ Public surface (mirrors the reference's for this path):
     demo.DemoPipeline                scripts/demo.py's request path at any photo size (PIL / OpenCV resizes on the GPU)
     fullres.FullResPipeline          photos of any size inpainted at their own resolution (reflect padding on the GPU)
     holewin.HoleWindowPipeline       the same, but only on windows around the holes; the rest of the photo is untouched
+    masks.RandomMaskStream           scripts/generate_masks.py's RandomMask(s) on the GPU: same bytes, same numpy stream
+    evaluate.EvalPipeline            evaluate_fid_lpips.py's batch around the generator: resizes, composite, normalisations
+    generate_masks                   python -m migan_b200.generate_masks: the reference script's CLI and files
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
     build.build()                    compile the C-ABI library (nvcc, sm_90a)
 
 The directory is named `mi-gan_b200`; import it as `migan_b200` (repo-root shim `migan_b200.py`).
 """
-from . import arch, build, demo, export, fullres, holewin, ops, parallel, pipeline, synthetic  # noqa: F401
+from . import arch, build, demo, evaluate, export, fullres, holewin, masks, ops, parallel, pipeline, synthetic  # noqa: F401
 from .fullres import FullResPipeline  # noqa: F401
 from .holewin import HoleWindowPipeline  # noqa: F401
+from .evaluate import EvalPipeline  # noqa: F401
+from .masks import RandomMaskStream  # noqa: F401
 from .generator import Generator  # noqa: F401
 
-__all__ = ["FullResPipeline", "Generator", "HoleWindowPipeline", "arch", "build", "demo", "export", "fullres", "holewin", "ops", "parallel", "pipeline", "synthetic"]
+__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "arch", "build", "demo", "evaluate", "export", "fullres", "holewin", "masks", "ops", "parallel", "pipeline", "synthetic"]
 __version__ = "0.1.0"

@@ -43,6 +43,21 @@ class WindowRequest(ctypes.Structure):
                 ("y", c_void_p), ("Hp", c_int), ("Wp", c_int), ("out", c_void_p)]
 
 
+MASK_MIN_SIZE, MASK_MAX_SIZE, MASK_MAX_ATTEMPTS = 2, 4096, 65535
+
+
+class NpRandom(ctypes.Structure):
+    """migan_np_random: numpy's legacy RandomState state, as np.random.get_state() lists it."""
+    _fields_ = [("key", ctypes.c_uint32 * 624), ("pos", c_int), ("has_gauss", c_int), ("gauss", ctypes.c_double)]
+
+
+class MaskRecord(ctypes.Structure):
+    """migan_mask_record: the primitives of one RandomMask attempt."""
+    _fields_ = [("n_rects", c_int), ("n_segments", c_int), ("n_discs", c_int), ("flips", c_int),
+                ("rects", (ctypes.c_int16 * 4) * 13), ("quads", (ctypes.c_int16 * 8) * 323),
+                ("discs", (ctypes.c_int16 * 4) * 342)]
+
+
 class SepconvTcIO(ctypes.Structure):
     """migan_sepconv_tc_io: the operands of one tensor-core SeparableConv2d launch (test hook)."""
     _fields_ = [("source", c_int), ("n", c_int), ("h", c_int), ("w", c_int), ("cin", c_int), ("cout", c_int),
@@ -110,6 +125,9 @@ SYMBOLS = [
     ("b200_demo_scratch_bytes", c_size_t, [POINTER(DemoRequest), c_int, c_int]),
     ("b200_demo_preprocess", c_int, [POINTER(DemoRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_demo_postprocess", c_int, [c_void_p, POINTER(DemoRequest), c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    ("b200_eval_scratch_bytes", c_size_t, [POINTER(DemoRequest), c_int, c_int]),
+    ("b200_eval_preprocess", c_int, [POINTER(DemoRequest), c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_eval_composite", c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("migan_fullres_extent", c_int, [c_void_p, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     ("b200_fullres_preprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
     ("b200_fullres_postprocess", c_int, [POINTER(FullResRequest), c_int, c_void_p]),
@@ -119,6 +137,10 @@ SYMBOLS = [
     ("migan_hole_windows_max", c_int, [c_int, c_int, c_int, POINTER(c_int)]),
     ("b200_window_preprocess", c_int, [POINTER(WindowRequest), c_int, c_void_p]),
     ("b200_window_postprocess", c_int, [POINTER(WindowRequest), c_int, c_void_p]),
+    ("migan_np_seed", c_int, [POINTER(NpRandom), ctypes.c_uint32]),
+    ("migan_mask_plan", c_int, [POINTER(NpRandom), c_int, c_int, c_void_p, c_void_p]),
+    ("b200_mask_raster", c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    ("b200_mask_compact", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

@@ -144,6 +144,7 @@ struct DemoBatch {
     int64_t start[MIGAN_PIPE_MAX_BATCH + 1];   // item prefix of the launch
     DemoReq r[MIGAN_PIPE_MAX_BATCH];
     const float* y; float* x;                  // generator output [n][3][R][R] / model input [n][4][R][R]
+    float* img;                                // evaluation batch only: the unmasked photo v * 2 / 255 - 1 [n][3][R][R]
     int n, res;
     CK_HD int find(int64_t i) const {           // the request item i belongs to (requests with no items are never found)
         int lo = 0, hi = n - 1;
@@ -295,6 +296,26 @@ struct DemoSquareK {
         const float m = demo_known(r, t.mry[oy], t.mrx[ox]) ? 1.f : 0.f;                     // mask // 255   (:60)
         x[0] = pre_mask_value(m);
         for (int c = 0; c < 3; ++c) x[(c + 1) * plane] = pre_img_value(pil_clip8(acc[c]), m);
+        if (b.img)
+            for (int c = 0; c < 3; ++c) b.img[((int64_t)k * 3 + c) * plane + j] = pre_img_value(pil_clip8(acc[c]), 1.f);
+    }
+};
+
+// The evaluation script's composite and normalisations (scripts/evaluate_fid_lpips.py:246-249), every product and sum
+// rounded on its own: composed = m * img + (1 - m) * y, then (v * 0.5 + 0.5).clamp(0, 1) of img (in place: `real`) and of
+// composed.  m = x channel 0 + 0.5.  items = n * R * R
+struct EvalCompositeK {
+    const float* x; const float* y; float* real; float* composed; int64_t plane;
+    PP_D static float unit(float v) { return fminf(fmaxf(PP_ADD(PP_MUL(v, 0.5f), 0.5f), 0.f), 1.f); }
+    PP_D void operator()(int64_t i) const {
+        const int64_t k = i / plane, p = i - k * plane;
+        const float m = PP_ADD(x[k * 4 * plane + p], 0.5f);
+        for (int c = 0; c < 3; ++c) {
+            const int64_t o = (k * 3 + c) * plane + p;
+            const float v = real[o];
+            composed[o] = unit(PP_ADD(PP_MUL(m, v), PP_MUL(PP_ADD(1.f, -m), y[o])));
+            real[o] = unit(v);
+        }
     }
 };
 
@@ -392,8 +413,10 @@ namespace {
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // The descriptors of a pass, with every request's regions carved out of `scratch` (nullptr: sizes only); returns the bytes.
-size_t demo_layout(const migan_demo_request* q, int n, int res, void* scratch, comod::DemoBatch* b) {
-    b->n = n; b->res = res; b->y = nullptr; b->x = nullptr;
+// eval: the evaluation batch's layout -- the photo goes straight to R x R (one PIL resize, w1 = h1 = R, when it is not
+// that size already) and the mask by one NEAREST step (wa, ha = the mask's size); no post-processing regions.
+size_t demo_layout(const migan_demo_request* q, int n, int res, void* scratch, comod::DemoBatch* b, bool eval = false) {
+    b->n = n; b->res = res; b->y = nullptr; b->x = nullptr; b->img = nullptr;
     unsigned char* base = static_cast<unsigned char*>(scratch);
     size_t off = 0;
     auto carve = [&](size_t bytes) { unsigned char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
@@ -402,14 +425,15 @@ size_t demo_layout(const migan_demo_request* q, int n, int res, void* scratch, c
         r = {};
         r.img = q[k].img; r.mask = q[k].mask; r.out = q[k].out;
         r.H = q[k].H; r.W = q[k].W; r.Hm = q[k].Hm; r.Wm = q[k].Wm; r.C = q[k].mask_channels; r.invert = q[k].invert != 0;
-        r.w1 = q[k].out_w; r.h1 = q[k].out_h;
-        demo_resized_size(r.Wm, r.Hm, comod::DEMO_MASK_MAX, &r.wa, &r.ha);
+        r.w1 = eval ? res : q[k].out_w; r.h1 = eval ? res : q[k].out_h;
+        if (eval) { r.wa = r.Wm; r.ha = r.Hm; }
+        else demo_resized_size(r.Wm, r.Hm, comod::DEMO_MASK_MAX, &r.wa, &r.ha);
         const bool down = r.w1 != r.W || r.h1 != r.H;
         r.kdw = down ? comod::pil_ksize(r.W, r.w1) : 0;
         r.kdh = down ? comod::pil_ksize(r.H, r.h1) : 0;
         r.tab = nullptr;
         r.tab = reinterpret_cast<int*>(carve((size_t)comod::demo_tab_ints(r, res, nullptr) * sizeof(int)));
-        r.ptmp = reinterpret_cast<int*>(carve((size_t)res * r.w1 * 3 * sizeof(int)));
+        r.ptmp = eval ? nullptr : reinterpret_cast<int*>(carve((size_t)res * r.w1 * 3 * sizeof(int)));
         if (down) {
             r.dtmp = carve((size_t)r.H * r.w1 * 3);
             r.rs = carve((size_t)r.h1 * r.w1 * 3);
@@ -499,6 +523,55 @@ int launch_demo_preprocess(const migan_demo_request* q, int n, int res, float* x
     return (int)comod::demo_launch<comod::DemoSquareK>(b, s);
 }
 
+int check_eval_batch(const migan_demo_request* q, int n, int res, char* msg, size_t len) {
+    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
+    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
+        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
+        return MIGAN_ERR_INVALID;
+    }
+    if (res < 1 || res > 8192) { snprintf(msg, len, "bad resolution %d", res); return MIGAN_ERR_INVALID; }
+    for (int k = 0; k < n; ++k) {
+        const migan_demo_request& r = q[k];
+        if (!r.img || !r.mask) { snprintf(msg, len, "request %d: null image or mask", k); return MIGAN_ERR_INVALID; }
+        if (r.H < 1 || r.W < 1 || r.Hm < 1 || r.Wm < 1) {
+            snprintf(msg, len, "request %d: photo of %d x %d, mask of %d x %d", k, r.H, r.W, r.Hm, r.Wm);
+            return MIGAN_ERR_INVALID;
+        }
+        if (r.mask_channels < 1 || r.mask_channels > 4) {
+            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
+            return MIGAN_ERR_INVALID;
+        }
+    }
+    return MIGAN_OK;
+}
+
+size_t eval_scratch_bytes(const migan_demo_request* q, int n, int res) {
+    comod::DemoBatch b;
+    return demo_layout(q, n, res, nullptr, &b, true);
+}
+
+// The demo's preprocess stages on the evaluation layout, with the unmasked photo values written to img as well.
+int launch_eval_preprocess(const migan_demo_request* q, int n, int res, float* x, float* img, void* scratch, ck_stream_t s) {
+    comod::DemoBatch b;
+    demo_layout(q, n, res, scratch, &b, true);
+    b.x = x;
+    b.img = img;
+    int e;
+    set_items(b, comod::DS_TABLES);
+    if ((e = (int)comod::demo_launch<comod::DemoTablesK>(b, s))) return e;
+    set_items(b, comod::DS_DOWN_W);
+    if ((e = (int)comod::demo_launch<comod::DemoDownWK>(b, s))) return e;
+    set_items(b, comod::DS_DOWN_H);
+    if ((e = (int)comod::demo_launch<comod::DemoDownHK>(b, s))) return e;
+    set_items(b, comod::DS_SQUARE);
+    return (int)comod::demo_launch<comod::DemoSquareK>(b, s);
+}
+
+int launch_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, ck_stream_t s) {
+    const int64_t plane = (int64_t)res * res;
+    return (int)comod::ck_launch(comod::EvalCompositeK{x, y, real, composed, plane}, n * plane, s);
+}
+
 // y -> uint8 + OpenCV width pass, then the height pass fused with the composite into each request's output.
 int launch_demo_postprocess(const float* y, const migan_demo_request* q, int n, int res, void* scratch, ck_stream_t s) {
     comod::DemoBatch b;
@@ -529,6 +602,21 @@ extern "C" int b200_demo_preprocess(const migan_demo_request* q, int n, int res,
     if (!x || !scratch) return MIGAN_ERR_INVALID;
     if (bytes < migan::demo_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
     return migan::launch_demo_preprocess(q, n, res, x, scratch, s);
+}
+extern "C" size_t b200_eval_scratch_bytes(const migan_demo_request* q, int n, int res) {
+    if (migan::check_eval_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return 0;
+    return migan::eval_scratch_bytes(q, n, res);
+}
+extern "C" int b200_eval_preprocess(const migan_demo_request* q, int n, int res, float* x, float* img, void* scratch, size_t bytes,
+                                    void* s) {
+    if (int rc = migan::check_eval_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return rc;
+    if (!x || !img || !scratch) return MIGAN_ERR_INVALID;
+    if (bytes < migan::eval_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
+    return migan::launch_eval_preprocess(q, n, res, x, img, scratch, s);
+}
+extern "C" int b200_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, void* s) {
+    if (!x || !y || !real || !composed || n < 1 || res < 1) return MIGAN_ERR_INVALID;
+    return migan::launch_eval_composite(x, y, n, res, real, composed, s);
 }
 extern "C" int b200_demo_postprocess(const float* y, const migan_demo_request* q, int n, int res, void* scratch, size_t bytes, void* s) {
     if (int rc = migan::check_demo_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return rc;

@@ -113,6 +113,11 @@ int demo_resized_size(int w, int h, int max_size, int* ow, int* oh);
 int check_demo_batch(const migan_demo_request* reqs, int n, int res, char* msg, size_t len);
 size_t demo_scratch_bytes(const migan_demo_request* reqs, int n, int res);
 int launch_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
+// the evaluation batch (evaluate_fid_lpips.py InferenceDataset + :246-249) on the same stages
+int check_eval_batch(const migan_demo_request* reqs, int n, int res, char* msg, size_t len);
+size_t eval_scratch_bytes(const migan_demo_request* reqs, int n, int res);
+int launch_eval_preprocess(const migan_demo_request* reqs, int n, int res, float* x, float* img, void* scratch, cudaStream_t s);
+int launch_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, cudaStream_t s);
 int launch_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, cudaStream_t s);
 
 // ---- full-resolution request path (fullres.cu): reflect padding and the composite around migan_forward_hw ------
@@ -131,6 +136,13 @@ int launch_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* 
 int hole_windows_max(int H, int W, int res, int* max_windows, char* msg, size_t len);
 int hole_windows(const uint8_t* cells_host, int H, int W, int res, int margin, int* win4, int max_windows, int* count, char* msg,
                  size_t len);
+
+// ---- free-form masks of the evaluation protocol (masks.cu): numpy's stream on the host, the rasterizer on the device ----
+void np_seed(migan_np_random* st, uint32_t seed);
+int check_mask_size(int s, int n_att, char* msg, size_t len);
+int mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states, char* msg, size_t len);
+int launch_mask_raster(const migan_mask_record* recs, int n_att, int s, uint8_t* attempts, int* holes, cudaStream_t s_);
+int launch_mask_compact(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out, cudaStream_t s_);
 
 
 // ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------

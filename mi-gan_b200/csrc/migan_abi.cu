@@ -1675,6 +1675,37 @@ int migan_hole_windows(const uint8_t* cells, int H, int W, int res, int margin, 
     return MIGAN_OK;
 }
 
+int migan_np_seed(migan_np_random* state, uint32_t seed) {
+    if (!state) return fail(MIGAN_ERR_INVALID, "np_seed: null state");
+    migan::np_seed(state, seed);
+    return MIGAN_OK;
+}
+
+int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_record* records, migan_np_random* states) {
+    char msg[256];
+    if (!state || !records) return fail(MIGAN_ERR_INVALID, "mask_plan: null argument");
+    if (int rc = migan::mask_plan(state, s, n_attempts, records, states, msg, sizeof msg)) return fail(rc, "mask_plan: %s", msg);
+    return MIGAN_OK;
+}
+
+int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream) {
+    char msg[256];
+    if (int rc = migan::check_mask_size(s, n_attempts, msg, sizeof msg)) return fail(rc, "mask_raster: %s", msg);
+    if (!records || !attempts || !holes) return fail(MIGAN_ERR_INVALID, "mask_raster: null argument");
+    if (reinterpret_cast<uintptr_t>(attempts) & 15) return fail(MIGAN_ERR_INVALID, "mask_raster: attempts not 16-byte aligned");
+    CUDA_TRY((cudaError_t)migan::launch_mask_raster(records, n_attempts, s, attempts, holes, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream) {
+    char msg[256];
+    if (int rc = migan::check_mask_size(s, n_attempts, msg, sizeof msg)) return fail(rc, "mask_compact: %s", msg);
+    if (n < 0 || n > 65535) return fail(MIGAN_ERR_INVALID, "mask_compact: %d masks (0 to 65535 per call)", n);
+    if (!attempts || !holes || (n && !out)) return fail(MIGAN_ERR_INVALID, "mask_compact: null argument");
+    CUDA_TRY((cudaError_t)migan::launch_mask_compact(attempts, holes, n_attempts, s, n, out, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
 int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h) {
     if (!out_w || !out_h) return fail(MIGAN_ERR_INVALID, "demo_resized_size: null argument");
     if (w < 1 || h < 1 || max_size < 1) return fail(MIGAN_ERR_INVALID, "demo_resized_size: bad arguments (%d x %d, max size %d)", w, h, max_size);
@@ -1708,6 +1739,30 @@ int b200_demo_postprocess(const float* y, const migan_demo_request* reqs, int n,
     const size_t need = migan::demo_scratch_bytes(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
     CUDA_TRY((cudaError_t)migan::launch_demo_postprocess(y, reqs, n, res, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+size_t b200_eval_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
+    char msg[256];
+    if (int rc = migan::check_eval_batch(reqs, n, res, msg, sizeof msg)) { fail(rc, "eval_scratch_bytes: %s", msg); return 0; }
+    return migan::eval_scratch_bytes(reqs, n, res);
+}
+
+int b200_eval_preprocess(const migan_demo_request* reqs, int n, int res, float* x, float* img, void* scratch,
+                         size_t scratch_bytes, void* stream) {
+    char msg[256];
+    if (int rc = migan::check_eval_batch(reqs, n, res, msg, sizeof msg)) return fail(rc, "eval_preprocess: %s", msg);
+    if (!x || !img || !scratch) return fail(MIGAN_ERR_INVALID, "eval_preprocess: null argument");
+    const size_t need = migan::eval_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "eval_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY((cudaError_t)migan::launch_eval_preprocess(reqs, n, res, x, img, scratch, static_cast<cudaStream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_eval_composite(const float* x, const float* y, int n, int res, float* img, float* composed, void* stream) {
+    if (!x || !y || !img || !composed) return fail(MIGAN_ERR_INVALID, "eval_composite: null argument");
+    if (n < 1 || res < 1 || res > 8192) return fail(MIGAN_ERR_INVALID, "eval_composite: %d images at resolution %d", n, res);
+    CUDA_TRY((cudaError_t)migan::launch_eval_composite(x, y, n, res, img, composed, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 
