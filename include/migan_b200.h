@@ -434,6 +434,10 @@ typedef struct migan_sepconv_tc_plan {
     int n_group, in_stages, a_stages, b_stages, b_resident, dw_global;
     int tile_w, tile_h, tile_n, n_tile, grid, num_tiles;
     int num_candidates;         /* length of the planner's candidate list for these shapes */
+    int ep_stages;              /* stages of the epilogue's noise / image window ring (0: the epilogue reads global memory) */
+    int ep_offset;              /* its byte offset and stage size in the 1024-aligned dynamic shared memory */
+    int ep_stage_bytes;
+    int smem_bytes;             /* dynamic shared memory of the launch (layout + 1024 bytes of alignment slack) */
 } migan_sepconv_tc_plan;
 
 /* Plans (and, unless io->pw_w is NULL, runs to completion on `stream`) one launch.  sms: SMs of the persistent grid

@@ -73,10 +73,18 @@ class SepconvTcPlan(ctypes.Structure):
     """migan_sepconv_tc_plan: what the planner chose for one launch."""
     _fields_ = [(name, c_int) for name in ("n_group", "in_stages", "a_stages", "b_stages", "b_resident", "dw_global",
                                            "tile_w", "tile_h", "tile_n", "n_tile", "grid", "num_tiles",
-                                           "num_candidates")]
+                                           "num_candidates", "ep_stages", "ep_offset", "ep_stage_bytes",
+                                           "smem_bytes")]
+
+    # Where the epilogue window ring went: it depends on the launch's noise and image pointers, not only on its shapes.
+    RING_FIELDS = ("ep_stages", "ep_offset", "ep_stage_bytes", "smem_bytes")
 
     def as_dict(self):
-        return {name: getattr(self, name) for name, _ in self._fields_}
+        """The schedule: a function of the shapes, the source and torgb alone."""
+        return {name: getattr(self, name) for name, _ in self._fields_ if name not in self.RING_FIELDS}
+
+    def ring(self):
+        return {name: getattr(self, name) for name in self.RING_FIELDS}
 
 
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)

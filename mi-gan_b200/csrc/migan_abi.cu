@@ -1830,8 +1830,12 @@ int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate
     migan::SepconvTcPlanInfo info{};
     auto record = [&]() {
         if (plan) *plan = {info.n_group, info.in_stages, info.a_stages, info.b_stages, info.b_resident, info.dw_global,
-                           info.tile_w, info.tile_h, info.tile_n, info.n_tile, info.grid, info.num_tiles, info.num_candidates};
+                           info.tile_w, info.tile_h, info.tile_n, info.n_tile, info.grid, info.num_tiles, info.num_candidates,
+                           info.ep_stages, info.ep_offset, info.ep_stage_bytes, info.smem_bytes};
     };
+    // the epilogue ring is planned for launches with noise or an image to up-sample: plan-only reads the pointers as flags
+    d.noise = io->noise;
+    if (io->torgb) rgb.img_lo = io->img_lo;
     if (!run) {
         if (const char* err = migan::sepconv_tc_plan_debug(nullptr, d, sms, candidate, &info)) return fail(MIGAN_ERR_INVALID, "sepconv_tc: %s", err);
         record();

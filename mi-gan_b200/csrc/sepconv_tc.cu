@@ -72,6 +72,7 @@ constexpr uint32_t kStaticSmem = 4096;               // barriers + torgb table (
 
 struct Params {
     CUtensorMap map_in, map_t, map_aux, map_a_hi, map_a_lo, map_w_hi, map_w_lo;
+    CUtensorMap map_nz, map_img;              // epilogue windows: noise [H][W] (pitch noise_pitch), img_lo [n][3][H/2][W/2]
     const float* w9;                          // [9][cin] depthwise taps * (kActSplitScale * sqrt 2)
     const float* bias;                        // [cin]              * (kActSplitScale * sqrt 2)
     const float* noise;                       // [H][noise_pitch]
@@ -109,6 +110,12 @@ struct Params {
     const float* rgb_fir;                     // [16][3] up-sampling taps of the image path
     const float* img_lo;                      // [n][3][H/2][W/2] planar, or null (first block)
     float* img_out;                           // [n][3][H][W] planar
+    // Epilogue window ring: per CTA tile, the producer brings the tile's noise (NZ, tile_h x tile_w, at the stage's start)
+    // and the low-resolution image window (IMG, [tile_n][3][img_bh][img_bw] at ep_off_img) into shared memory.  0 stages:
+    // no ring (nothing to bring, or no room left by the layout); the epilogue then reads global memory.
+    int ep_stages;
+    uint32_t off_ep, ep_stage_stride, ep_off_img, ep_tx_bytes;
+    int img_bw, img_bh;
     int* error_flag;
 };
 
@@ -266,13 +273,21 @@ struct Ring {
 };
 
 // mbarriers: [0,8) full_in  [8,16) empty_in  [16,24) full_a  [24,32) empty_a  [32,40) full_b  [40,48) empty_b
-constexpr int kNumBars = 48;
+//            [48,52) full_ep  [52,56) empty_ep
+constexpr int kNumBars = 56;
 constexpr int kMaxAStages = 8;
+constexpr int kMaxEpStages = 4;
 static_assert(kNumBars * 8 + (3 * kMaxRgbC + 4 + 48) * 4 <= (int)kStaticSmem, "static shared memory outgrew kStaticSmem");
 __device__ __forceinline__ uint32_t bar_full_a(uint32_t bar0, int s) { return bar0 + 8u * (16 + s); }
 __device__ __forceinline__ uint32_t bar_empty_a(uint32_t bar0, int s) { return bar0 + 8u * (24 + s); }
 __device__ __forceinline__ uint32_t bar_full_b(uint32_t bar0, int s) { return bar0 + 8u * (32 + s); }
 __device__ __forceinline__ uint32_t bar_empty_b(uint32_t bar0, int s) { return bar0 + 8u * (40 + s); }
+__device__ __forceinline__ uint32_t bar_full_ep(uint32_t bar0, int s) { return bar0 + 8u * (48 + s); }
+__device__ __forceinline__ uint32_t bar_empty_ep(uint32_t bar0, int s) { return bar0 + 8u * (52 + s); }
+// Origin of a tile's low-resolution image window: one row above the tile's first tap row, and the first tap column
+// rounded down to 4 floats, so that the TMA box starts on a 16-byte boundary.
+__device__ __forceinline__ int img_win_y(int y0) { return (y0 >> 1) - 1; }
+__device__ __forceinline__ int img_win_x(int x0) { return ((x0 >> 1) - 1) & ~3; }
 __device__ __forceinline__ void mma_release(const Params& p, uint32_t bar0, int sa, int sb, bool release_a) {
     __syncwarp();
     if ((threadIdx.x & 31) == 0) {             // one arrival per warp: each warp waited for its own wgmma groups
@@ -290,9 +305,14 @@ __device__ __forceinline__ void mma_release(const Params& p, uint32_t bar0, int 
 // because the tensor core truncates on every accumulate: added into the large main sum they cost ~0.5 ulp of the MAIN
 // sum per MMA (one accumulator measured on the H100: mean-abs error 1.6e-4 on the migan-256 reference fixture, above
 // the 1e-4 bound).
+// kRing: the tile's noise and image taps come from the epilogue window ring in shared memory (Params::ep_stages); the
+// compiler may then move those loads freely around the global stores.  Without it they are read from global memory.
+// The ring is planned for activated 3-pass launches only, so kRing also fixes act = 1: the unactivated path's constants
+// are not kept around the row loop.
 // ---------------------------------------------------------------------------------------
-template <int NT, bool kSplit>
-__device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base, uint32_t bar0, const float* s_rgb, int my_tiles) {
+template <int NT, bool kSplit, bool kRing>
+__device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base, const uint8_t* smem_gen, uint32_t bar0,
+                                             const float* s_rgb, int my_tiles) {
     constexpr int NA = NT / 2;                       // accumulator registers per m64 half
     constexpr int NC = kSplit ? NA : 1;              // correction accumulator (unused in fast mode)
     const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
@@ -300,7 +320,7 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
     const uint32_t b_stage_bytes = (uint32_t)NT * kKBlock * 2 * 2;   // [Bh ; Bl]
     float acc[2][NA], cor[2][NC];
     float rgb_acc[4];                                // torgb sum of colour lane % 4 over the group's N tiles, per pixel row
-    Ring ra(p.a_stages), rb(p.b_stages);
+    Ring ra(p.a_stages), rb(p.b_stages), re(kRing ? p.ep_stages : 1);
     for (int it = 0; it < my_tiles; ++it) {
       const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
       for (int j = 0; j < p.n_group; ++j) {
@@ -354,13 +374,25 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
         // ---- epilogue: the four pixel rows of this thread, straight from the accumulators ----
         const int chan0 = (tc.nt + j) * NT;
         const float scale_g = p.inv_scale * kActGain;
+        // The stage holding this tile's windows: waited for before the group's first epilogue, released after its last.
+        const float* ep_nz = nullptr;
+        const float* ep_img = nullptr;
+        if constexpr (kRing) {
+            if (first_n) mbar_wait(bar_full_ep(bar0, re.stage), re.phase, 230 + re.stage, p.error_flag);
+            ep_nz = reinterpret_cast<const float*>(smem_gen + p.off_ep + re.stage * p.ep_stage_stride);
+            ep_img = ep_nz + p.ep_off_img / 4;
+        }
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
             const int h = r >> 1, i = r & 1;
             const int m = h * 64 + wq * 16 + (lane >> 2) + 8 * i;
-            const int pimg = tc.n0 + (m >> (p.l_tw + p.l_th)), poy = tc.y0 + ((m >> p.l_tw) & (p.tile_h - 1)), pox = tc.x0 + (m & (p.tile_w - 1));
+            const int limg = m >> (p.l_tw + p.l_th), ly = (m >> p.l_tw) & (p.tile_h - 1), lx = m & (p.tile_w - 1);
+            const int pimg = tc.n0 + limg, poy = tc.y0 + ly, pox = tc.x0 + lx;
             const bool valid = pimg < p.n && poy < p.H && pox < p.W;   // partial tiles at the right / bottom edge
-            const float nz = (p.noise && valid) ? __ldg(p.noise + poy * p.noise_pitch + pox) : 0.f;
+            // The NZ window is zero past the extents; rows of images past n read some noise but are never stored.
+            float nz;
+            if constexpr (kRing) nz = p.noise ? ep_nz[(ly << p.l_tw) + lx] : 0.f;
+            else nz = (p.noise && valid) ? __ldg(p.noise + poy * p.noise_pitch + pox) : 0.f;
             const float nz_g = nz * kActGain;
             float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0 + 2 * (lane & 3);
             float s0 = 0.f, s1 = 0.f, s2 = 0.f;      // torgb partial sums over this thread's channels
@@ -370,7 +402,7 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
                     const float v = kSplit ? acc[h][jj * 4 + i * 2 + c] + cor[h][(jj * 4 + i * 2 + c) % NC] : acc[h][jj * 4 + i * 2 + c];
-                    if (p.act) {                     // clamp(lrelu(f) * sqrt2) with the gain folded into the scale
+                    if (kRing || p.act) {            // clamp(lrelu(f) * sqrt2) with the gain folded into the scale
                         const float a = fmaf(v, scale_g, nz_g);
                         o[c] = fminf(fmax3(a, a * kLreluAlpha, -kActClamp), kActClamp);
                     } else {
@@ -402,6 +434,14 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                     float rv = rgb_acc[r] + s_rgb[kRgbBias + k];
                     if (p.img_lo) {
                         const int hl = p.H >> 1, wl = p.W >> 1;
+                        // IMG window: plane (limg, k), rows from img_win_y(y0), columns from img_win_x(x0), zero outside
+                        // the low-resolution image (TMA out-of-bounds fill, the taps' zero padding)
+                        const float* win = nullptr;
+                        int wy0 = 0, wx0 = 0;
+                        if constexpr (kRing) {
+                            win = ep_img + (limg * 3 + k) * p.img_bh * p.img_bw;
+                            wy0 = img_win_y(tc.y0); wx0 = img_win_x(tc.x0);
+                        }
                         float up = 0.f;
 #pragma unroll
                         for (int a = 0; a < 2; ++a)
@@ -409,14 +449,26 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                             for (int bb = 0; bb < 2; ++bb) {
                                 const int iy = (poy + (poy & 1) + 2 * a - 2) >> 1, ix = (pox + (pox & 1) + 2 * bb - 2) >> 1;
                                 const int ty = (poy & 1) + 2 * a, tx = (pox & 1) + 2 * bb;
-                                const bool ok = iy >= 0 && iy < hl && ix >= 0 && ix < wl;
-                                const float lo = ok ? __ldg(p.img_lo + (((size_t)pimg * 3 + k) * hl + iy) * wl + ix) : 0.f;
+                                float lo;
+                                if constexpr (kRing) {
+                                    lo = win[(iy - wy0) * p.img_bw + (ix - wx0)];
+                                } else {
+                                    const bool ok = iy >= 0 && iy < hl && ix >= 0 && ix < wl;
+                                    lo = ok ? __ldg(p.img_lo + (((size_t)pimg * 3 + k) * hl + iy) * wl + ix) : 0.f;
+                                }
                                 up = fmaf(s_rgb[kRgbFir + (ty * 4 + tx) * 3 + k], lo, up);
                             }
                         rv = up + rv;
                     }
                     p.img_out[(((size_t)pimg * 3 + k) * p.H + poy) * p.W + pox] = rv;
                 }
+            }
+        }
+        if constexpr (kRing) {
+            if (last_n) {                              // the group's last epilogue has read the stage
+                __syncwarp();
+                if (lane == 0) mbar_arrive(bar_empty_ep(bar0, re.stage));
+                re.advance();
             }
         }
       }
@@ -447,6 +499,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
         for (int s = 0; s < p.in_stages; ++s) { mbar_init(full_in(s), 1); mbar_init(empty_in(s), kNumProWarps / 2); }
         for (int s = 0; s < p.a_stages; ++s) { mbar_init(full_a(s), a_dw ? kNumProWarps : 1); mbar_init(empty_a(s), 4); }
         for (int s = 0; s < p.b_stages; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 4); }
+        for (int s = 0; s < p.ep_stages; ++s) { mbar_init(bar_full_ep(bar0, s), 1); mbar_init(bar_empty_ep(bar0, s), 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (warp == kProducerWarp && lane == 0) {
@@ -455,6 +508,10 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
         else prefetch_tensormap(&p.map_in);
         if (p.source == SEPCONV_SRC_UP) { prefetch_tensormap(&p.map_t); if (p.up_has_noise) prefetch_tensormap(&p.map_aux); }
         prefetch_tensormap(&p.map_w_hi); prefetch_tensormap(&p.map_w_lo);
+        if (p.ep_stages) {
+            if (p.noise) prefetch_tensormap(&p.map_nz);
+            if (p.torgb && p.img_lo) prefetch_tensormap(&p.map_img);
+        }
     }
     if (p.torgb) {
         for (int i = threadIdx.x; i < 3 * p.cout; i += kThreads) s_rgb[i] = __ldg(p.rgb_w + i);
@@ -503,7 +560,7 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                 if (++pf_kb == num_kb) { pf_kb = 0; ++pf_it; }
             };
             for (int c = 0; c < p.prefetch; ++c) prefetch_next();
-            Ring rin(p.in_stages), ra(p.a_stages), rb(p.b_stages);
+            Ring rin(p.in_stages), ra(p.a_stages), rb(p.b_stages), rep(p.ep_stages ? p.ep_stages : 1);
             for (int it = 0; it < my_tiles; ++it) {
               const TileCoord tc = decode_tile(p, blockIdx.x + it * gridDim.x);
               for (int j = 0; j < p.n_group; ++j) {
@@ -546,6 +603,17 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
                         tma_load_2d(dst, &p.map_w_hi, full_b(s), kb * kKBlock, row);
                         tma_load_2d(dst + b_stage_bytes / 2, &p.map_w_lo, full_b(s), kb * kKBlock, row);
                     }
+                    // The epilogue's windows, once per CTA tile, after the tile's operand loads (the epilogue runs last)
+                    if (p.ep_stages && j == 0 && kb == num_kb - 1) {
+                        const int s = rep.stage;
+                        mbar_wait<true>(bar_empty_ep(bar0, s), rep.phase ^ 1, 130 + s, p.error_flag);
+                        rep.advance();
+                        mbar_expect_tx(bar_full_ep(bar0, s), p.ep_tx_bytes);
+                        const uint32_t dst = smem_base + p.off_ep + s * p.ep_stage_stride;
+                        if (p.noise) tma_load_2d(dst, &p.map_nz, bar_full_ep(bar0, s), tc.x0, tc.y0);
+                        if (p.torgb && p.img_lo)
+                            tma_load_4d(dst + p.ep_off_img, &p.map_img, bar_full_ep(bar0, s), img_win_x(tc.x0), img_win_y(tc.y0), 0, tc.n0);
+                    }
                 }
               }
             }
@@ -553,9 +621,11 @@ sepconv_tc_kernel(const __grid_constant__ Params p) {
     } else if (warp >= kMmaWarp0) {
         // ================================ MMA + epilogue ==============================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMmaRegs));
-        if (p.passes == 3) mma_epilogue<64, true>(p, smem_base, bar0, s_rgb, my_tiles);
-        else if (p.n_tile == 128) mma_epilogue<128, false>(p, smem_base, bar0, s_rgb, my_tiles);
-        else mma_epilogue<64, false>(p, smem_base, bar0, s_rgb, my_tiles);
+        // the epilogue ring is planned for activated 3-pass launches only (plan_layout)
+        if (p.ep_stages) mma_epilogue<64, true, true>(p, smem_base, smem_gen, bar0, s_rgb, my_tiles);
+        else if (p.passes == 3) mma_epilogue<64, true, false>(p, smem_base, smem_gen, bar0, s_rgb, my_tiles);
+        else if (p.n_tile == 128) mma_epilogue<128, false, false>(p, smem_base, smem_gen, bar0, s_rgb, my_tiles);
+        else mma_epilogue<64, false, false>(p, smem_base, smem_gen, bar0, s_rgb, my_tiles);
     } else {
         // ================================ prologue (pre-stage + depthwise) ========================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kProRegs));
@@ -803,6 +873,7 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
     if (num_candidates) *num_candidates = (int)cands.size();
     if (candidate >= (int)cands.size()) return "no such candidate layout";
     bool found = false;
+    uint32_t used = 0;
     for (size_t i = candidate < 0 ? 0 : (size_t)candidate; i < cands.size(); ++i) {
         const Cand& c = cands[i];
         const uint32_t tab = c.dw_global ? 0u : tables;
@@ -820,6 +891,7 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
         p.off_dw = (dw && !c.dw_global) ? p.off_b + (uint32_t)c.b_stages * b_stage : 0xFFFFFFFFu;
         p.off_stem = p.off_b + (uint32_t)c.b_stages * b_stage + 40u * cin;
         smem_bytes = total + 1024;
+        used = total;
         found = true;
         break;
     }
@@ -827,6 +899,26 @@ const char* plan_layout(Params& p, const SepconvTcDesc& d, int sms, uint32_t& sm
     if (d.rgb && (p.n_group != p.num_n_tiles || cout > kMaxRgbC))
         return "fused torgb needs all output channels of a pixel tile in one CTA tile (cout <= 256 with a resident A operand)";
     if (p.in_stages > 8 || p.a_stages > kMaxAStages || p.b_stages > 8) return "internal: ring too deep for the barrier table";
+
+    // ---- epilogue window ring: placed after the chosen layout, in what it leaves of the budget, so that it never changes
+    // the layout.  4 stages where they fit (the producer may run several CTA tiles ahead of the epilogue), else 2, else
+    // none.  The IMG box needs 16-byte rows of the low-resolution image (W / 2 a multiple of 4).  Only the activated 3-pass
+    // epilogue has a ring variant: more epilogue instances push the prologue's register allocation into spills. ----
+    p.ep_stages = 0;
+    const bool ep_img = d.rgb && d.rgb->img_lo;
+    if (d.passes == 3 && d.act && (d.noise || ep_img) && (!ep_img || (w / 2) % 4 == 0)) {
+        p.img_bh = (p.tile_h + 1) / 2 + 2;                 // tap rows of the tile, from one above (y0 may be odd at tile_h = 1)
+        p.img_bw = (p.tile_w / 2 + 5 + 3) & ~3;            // tap columns + up to 3 of 16-byte alignment, in whole 16 bytes
+        const uint32_t nz_bytes = d.noise ? (uint32_t)(p.tile_h * p.tile_w * 4) : 0u;
+        const uint32_t img_bytes = ep_img ? (uint32_t)(p.tile_n * 3 * p.img_bh * p.img_bw * 4) : 0u;
+        p.ep_off_img = (nz_bytes + 127u) & ~127u;          // TMA destinations: 128-byte aligned
+        p.ep_tx_bytes = nz_bytes + img_bytes;
+        p.ep_stage_stride = (p.ep_off_img + img_bytes + 127u) & ~127u;
+        p.off_ep = (used + 127u) & ~127u;
+        for (int st : {kMaxEpStages, 2})
+            if (p.off_ep + (uint32_t)st * p.ep_stage_stride <= budget) { p.ep_stages = st; break; }
+        if (p.ep_stages) smem_bytes = p.off_ep + (uint32_t)p.ep_stages * p.ep_stage_stride + 1024;
+    }
     p.l_nt = ilog2(p.num_n_tiles / p.n_group);
     p.l_tw = ilog2(p.tile_w); p.l_th = ilog2(p.tile_h);
     p.num_tiles = m_tiles * (p.num_n_tiles / p.n_group);
@@ -862,9 +954,14 @@ const char* plan_launch(SepconvTcArgs* args, const SepconvTcDesc& d, int sms, in
     int num_candidates = 0;
     bool dw_global = false;
     if (const char* err = plan_layout(p, d, sms, smem_bytes, candidate, &num_candidates, &dw_global)) return err;
+    if (args) {   // TMA reads global memory from 16-byte aligned bases only; else the epilogue reads the windows directly
+        const uintptr_t nz_a = reinterpret_cast<uintptr_t>(d.noise), img_a = d.rgb ? reinterpret_cast<uintptr_t>(d.rgb->img_lo) : 0;
+        if ((nz_a | img_a) & 15u) p.ep_stages = 0;
+    }
     if (info) {
         *info = {p.n_group, p.in_stages, p.a_stages, p.b_stages, p.b_resident, dw_global ? 1 : 0,
-                 p.tile_w, p.tile_h, p.tile_n, p.n_tile, std::min(p.num_tiles, sms), p.num_tiles, num_candidates};
+                 p.tile_w, p.tile_h, p.tile_n, p.n_tile, std::min(p.num_tiles, sms), p.num_tiles, num_candidates,
+                 p.ep_stages, p.ep_stages ? (int)p.off_ep : 0, p.ep_stages ? (int)p.ep_stage_stride : 0, (int)smem_bytes};
     }
     if (!args) return nullptr;
     p.w9 = d.w9; p.bias = d.bias; p.noise = d.noise; p.inv_scale = d.inv_scale; p.out = d.out;
@@ -914,6 +1011,19 @@ const char* plan_launch(SepconvTcArgs* args, const SepconvTcDesc& d, int sms, in
         const uint32_t box[2] = {(uint32_t)kKBlock, (uint32_t)p.n_tile};
         if ((err = encode_map(&p.map_w_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.w_hi, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
         if ((err = encode_map(&p.map_w_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, d.w_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return err;
+    }
+    if (p.ep_stages && d.noise) {        // the noise plane's own extent: its padding columns and rows are never read
+        const uint64_t nd[2] = {(uint64_t)w, (uint64_t)h};
+        const uint64_t ns[1] = {(uint64_t)d.noise_pitch * 4};
+        const uint32_t nb[2] = {(uint32_t)p.tile_w, (uint32_t)p.tile_h};
+        if ((err = encode_map(&p.map_nz, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, d.noise, nd, ns, nb, CU_TENSOR_MAP_SWIZZLE_NONE))) return err;
+    }
+    if (p.ep_stages && p.torgb && p.img_lo) {
+        const int hl = h / 2, wl = w / 2;
+        const uint64_t dims[4] = {(uint64_t)wl, (uint64_t)hl, 3, (uint64_t)n};
+        const uint64_t str[3] = {(uint64_t)wl * 4, (uint64_t)hl * wl * 4, (uint64_t)3 * hl * wl * 4};
+        const uint32_t box[4] = {(uint32_t)p.img_bw, (uint32_t)p.img_bh, 3, (uint32_t)p.tile_n};
+        if ((err = encode_map(&p.map_img, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p.img_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE))) return err;
     }
     if (!d.out && p.store_out) return "no output tensor";
     // Persistent grid = one CTA per usable SM.

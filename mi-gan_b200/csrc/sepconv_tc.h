@@ -70,6 +70,8 @@ const char* sepconv_tc_plan_ex(SepconvTcArgs* a, const SepconvTcDesc& d);
 struct SepconvTcPlanInfo {
     int n_group, in_stages, a_stages, b_stages, b_resident, dw_global;
     int tile_w, tile_h, tile_n, n_tile, grid, num_tiles, num_candidates;
+    int ep_stages, ep_offset, ep_stage_bytes;   // epilogue window ring (0 stages: none) and its place in dynamic smem
+    int smem_bytes;                              // dynamic shared memory of the launch
 };
 // sepconv_tc_plan_ex with the planner's two inputs made explicit, for tests: `sms` SMs for the persistent grid (0: the
 // device's minus MIGAN_TC_RESERVE_SMS, as in production) and, if candidate >= 0, the candidate-th layout of the planner's own
