@@ -63,6 +63,46 @@ inline cudaError_t ck_launch(const F& f, int64_t items, ck_stream_t s) {
 }
 #endif
 
+// ---- batches of requests in one launch ---------------------------------------------------------------------------
+// A batch descriptor holds n requests r[] and the launch's item prefix start[]: item i belongs to the request k with
+// start[k] <= i < start[k + 1].  The request of item i (requests with no items are never found):
+template <class T>
+CK_HD int find_request(const T* start, int n, T i) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// start[] of one stage's launch: items(stage, r[k], res) summed in request order.
+template <class Batch, class Items>
+inline void set_items(Batch& b, int stage, Items items) {
+    b.start[0] = 0;
+    for (int k = 0; k < b.n; ++k) b.start[k + 1] = b.start[k] + items(stage, b.r[k], b.res);
+}
+
+// One thread per item of a batch, the functor F built on the descriptor.  The descriptor travels by value in the kernel
+// parameter; __grid_constant__ lets the functors index its request table there (no per-thread copy of the struct).
+#ifdef MIGAN_EMULATE
+template <class F, class Batch>
+inline int batch_launch(const Batch& b, ck_stream_t s) { return ck_launch(F{b}, b.start[b.n], s); }
+#else
+template <class F, class Batch>
+__global__ void __launch_bounds__(256) batch_items_kernel(const __grid_constant__ Batch b, const int64_t items) {
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i < items) F{b}(i);
+}
+template <class F, class Batch>
+inline cudaError_t batch_launch(const Batch& b, ck_stream_t s) {
+    const int64_t items = b.start[b.n];
+    if (items <= 0) return cudaSuccess;
+    batch_items_kernel<F, Batch><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(b, items);
+    return cudaGetLastError();
+}
+#endif
+
 // ---- layout changes at the NCHW boundary ------------------------------------------------------------------------
 struct NchwToNhwcK {   // items = n*H*W*C (output order)
     const float* in; float* out; int H, W, C;

@@ -22,16 +22,15 @@
 // the composed source index of the two or three NEAREST steps.
 //
 // A pass of up to MIGAN_PIPE_MAX_BATCH requests runs one launch per stage covering every request; the request table
-// travels by value in the kernel parameter (DemoBatch, < 4 KB) with the stage's item prefix, as in pipeline.cu:
+// travels by value in the kernel parameter (DemoBatch, < 4 KB) with the stage's item prefix (batch_launch, comod_kernels.cuh):
 //   tables (every resampler's coefficients / indices, computed on the device) -> down-scale width pass -> down-scale
 //   height pass (both only when a photo is larger than R) -> R x R resize + mask + x  |  y -> uint8 + OpenCV width pass
 //   -> OpenCV height pass + composite.
-// Item kernels (comod_kernels.cuh style): the emulation build (tests/emul/build_demo.py) runs the very same functors on
+// Item kernels (comod_kernels.cuh style): the emulation build (tests/emul/build_emul.py) runs the very same functors on
 // the CPU.  Every product and sum is rounded on its own (no FMA contraction), in double where the libraries use double.
 #include "prepost.cuh"
-#include "../../include/migan_b200.h"
+#include "abi_error.h"
 
-#include <cstdio>
 #ifdef MIGAN_EMULATE
 #define DM_DMUL(a, b) ((a) * (b))
 #define DM_DADD(a, b) ((a) + (b))
@@ -41,7 +40,6 @@
 #define DM_FDIV(a, b) ((a) / (b))
 #define DM_D inline
 #else
-#include "kernels.h"
 #define DM_DMUL(a, b) __dmul_rn((a), (b))
 #define DM_DADD(a, b) __dadd_rn((a), (b))
 #define DM_DDIV(a, b) __ddiv_rn((a), (b))
@@ -146,14 +144,6 @@ struct DemoBatch {
     const float* y; float* x;                  // generator output [n][3][R][R] / model input [n][4][R][R]
     float* img;                                // evaluation batch only: the unmasked photo v * 2 / 255 - 1 [n][3][R][R]
     int n, res;
-    CK_HD int find(int64_t i) const {           // the request item i belongs to (requests with no items are never found)
-        int lo = 0, hi = n - 1;
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (start[mid] <= i) lo = mid; else hi = mid - 1;
-        }
-        return lo;
-    }
 };
 static_assert(sizeof(DemoBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
 
@@ -195,7 +185,7 @@ CK_HD int64_t demo_items(int stage, const DemoReq& r, int R) {
 struct DemoTablesK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int R = b.res;
         const DemoTabs t = demo_tabs(r, R);
@@ -227,7 +217,7 @@ struct DemoTablesK {
 struct DemoDownWK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const DemoTabs t = demo_tabs(r, b.res);
@@ -249,7 +239,7 @@ struct DemoDownWK {
 struct DemoDownHK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const DemoTabs t = demo_tabs(r, b.res);
@@ -271,7 +261,7 @@ struct DemoDownHK {
 struct DemoSquareK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int R = b.res;
@@ -324,7 +314,7 @@ struct EvalCompositeK {
 struct DemoPostWK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int R = b.res;
@@ -348,7 +338,7 @@ struct DemoPostWK {
 struct DemoOutK {
     const DemoBatch& b;
     DM_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int R = b.res;
@@ -382,25 +372,6 @@ struct DemoOutK {
         }
     }
 };
-
-#ifdef MIGAN_EMULATE
-template <class F>
-inline int demo_launch(const DemoBatch& b, ck_stream_t s) { return ck_launch(F{b}, b.start[b.n], s); }
-#else
-// One thread per item; __grid_constant__ lets the functors index the request table in the parameter space.
-template <class F>
-__global__ void __launch_bounds__(256) demo_items_kernel(const __grid_constant__ DemoBatch b, const int64_t items) {
-    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i < items) F{b}(i);
-}
-template <class F>
-inline cudaError_t demo_launch(const DemoBatch& b, ck_stream_t s) {
-    const int64_t items = b.start[b.n];
-    if (items <= 0) return cudaSuccess;
-    demo_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(b, items);
-    return cudaGetLastError();
-}
-#endif
 
 }  // namespace comod
 
@@ -444,11 +415,6 @@ size_t demo_layout(const migan_demo_request* q, int n, int res, void* scratch, c
     return off;
 }
 
-void set_items(comod::DemoBatch& b, int stage) {
-    b.start[0] = 0;
-    for (int k = 0; k < b.n; ++k) b.start[k + 1] = b.start[k] + comod::demo_items(stage, b.r[k], b.res);
-}
-
 }  // namespace
 
 // demo.py `resize` (:48-53): (int(w * r), int(h * r)), r = max_size / w if w > h else max_size / h, when either side is
@@ -464,40 +430,30 @@ int demo_resized_size(int w, int h, int max_size, int* ow, int* oh) {
     return 0;
 }
 
-int check_demo_batch(const migan_demo_request* q, int n, int res, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
-    if (res < 1 || res > 8192) { snprintf(msg, len, "bad resolution %d", res); return MIGAN_ERR_INVALID; }
+// The demo batch, or the evaluation batch (eval: no output, and the photo goes straight to R x R).
+int check_demo_batch(const char* who, const migan_demo_request* q, int n, int res, bool eval) {
+    if (int rc = check_batch_size(who, q, n)) return rc;
+    if (res < 1 || res > 8192) return fail(MIGAN_ERR_INVALID, "%s: bad resolution %d", who, res);
     for (int k = 0; k < n; ++k) {
         const migan_demo_request& r = q[k];
-        if (!r.img || !r.mask || !r.out) { snprintf(msg, len, "request %d: null image, mask or output", k); return MIGAN_ERR_INVALID; }
-        if (r.H < 1 || r.W < 1 || r.Hm < 1 || r.Wm < 1) {
-            snprintf(msg, len, "request %d: photo of %d x %d, mask of %d x %d", k, r.H, r.W, r.Hm, r.Wm);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.mask_channels < 1 || r.mask_channels > 4) {
-            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
-            return MIGAN_ERR_INVALID;
-        }
+        if (eval && (!r.img || !r.mask)) return fail(MIGAN_ERR_INVALID, "%s: request %d: null image or mask", who, k);
+        if (!eval && (!r.img || !r.mask || !r.out)) return fail(MIGAN_ERR_INVALID, "%s: request %d: null image, mask or output", who, k);
+        if (r.H < 1 || r.W < 1 || r.Hm < 1 || r.Wm < 1)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: photo of %d x %d, mask of %d x %d", who, k, r.H, r.W, r.Hm, r.Wm);
+        if (int rc = check_mask_channels(who, k, r.mask_channels)) return rc;
+        if (eval) continue;
         int w1, h1, wa, ha, wb, hb;
         demo_resized_size(r.W, r.H, res, &w1, &h1);
         demo_resized_size(r.Wm, r.Hm, comod::DEMO_MASK_MAX, &wa, &ha);
         demo_resized_size(wa, ha, res, &wb, &hb);
-        if (w1 < 1 || h1 < 1 || wa < 1 || ha < 1 || wb < 1 || hb < 1) {
-            snprintf(msg, len, "request %d: a side resizes to 0 (photo %d x %d, mask %d x %d, resolution %d)", k, r.W, r.H, r.Wm, r.Hm, res);
-            return MIGAN_ERR_INVALID;
-        }
-        if (wb != w1 || hb != h1) {
-            snprintf(msg, len, "request %d: the mask resizes to %d x %d and the photo to %d x %d (w x h)", k, wb, hb, w1, h1);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.out_w != w1 || r.out_h != h1) {
-            snprintf(msg, len, "request %d: output of %d x %d, the resized photo is %d x %d (w x h)", k, r.out_w, r.out_h, w1, h1);
-            return MIGAN_ERR_INVALID;
-        }
+        if (w1 < 1 || h1 < 1 || wa < 1 || ha < 1 || wb < 1 || hb < 1)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: a side resizes to 0 (photo %d x %d, mask %d x %d, resolution %d)", who, k,
+                        r.W, r.H, r.Wm, r.Hm, res);
+        if (wb != w1 || hb != h1)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: the mask resizes to %d x %d and the photo to %d x %d (w x h)", who, k, wb, hb, w1, h1);
+        if (r.out_w != w1 || r.out_h != h1)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: output of %d x %d, the resized photo is %d x %d (w x h)", who, k, r.out_w,
+                        r.out_h, w1, h1);
     }
     return MIGAN_OK;
 }
@@ -513,36 +469,14 @@ int launch_demo_preprocess(const migan_demo_request* q, int n, int res, float* x
     demo_layout(q, n, res, scratch, &b);
     b.x = x;
     int e;
-    set_items(b, comod::DS_TABLES);
-    if ((e = (int)comod::demo_launch<comod::DemoTablesK>(b, s))) return e;
-    set_items(b, comod::DS_DOWN_W);
-    if ((e = (int)comod::demo_launch<comod::DemoDownWK>(b, s))) return e;
-    set_items(b, comod::DS_DOWN_H);
-    if ((e = (int)comod::demo_launch<comod::DemoDownHK>(b, s))) return e;
-    set_items(b, comod::DS_SQUARE);
-    return (int)comod::demo_launch<comod::DemoSquareK>(b, s);
-}
-
-int check_eval_batch(const migan_demo_request* q, int n, int res, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
-    if (res < 1 || res > 8192) { snprintf(msg, len, "bad resolution %d", res); return MIGAN_ERR_INVALID; }
-    for (int k = 0; k < n; ++k) {
-        const migan_demo_request& r = q[k];
-        if (!r.img || !r.mask) { snprintf(msg, len, "request %d: null image or mask", k); return MIGAN_ERR_INVALID; }
-        if (r.H < 1 || r.W < 1 || r.Hm < 1 || r.Wm < 1) {
-            snprintf(msg, len, "request %d: photo of %d x %d, mask of %d x %d", k, r.H, r.W, r.Hm, r.Wm);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.mask_channels < 1 || r.mask_channels > 4) {
-            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
-            return MIGAN_ERR_INVALID;
-        }
-    }
-    return MIGAN_OK;
+    comod::set_items(b, comod::DS_TABLES, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoTablesK>(b, s))) return e;
+    comod::set_items(b, comod::DS_DOWN_W, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoDownWK>(b, s))) return e;
+    comod::set_items(b, comod::DS_DOWN_H, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoDownHK>(b, s))) return e;
+    comod::set_items(b, comod::DS_SQUARE, comod::demo_items);
+    return (int)comod::batch_launch<comod::DemoSquareK>(b, s);
 }
 
 size_t eval_scratch_bytes(const migan_demo_request* q, int n, int res) {
@@ -557,14 +491,14 @@ int launch_eval_preprocess(const migan_demo_request* q, int n, int res, float* x
     b.x = x;
     b.img = img;
     int e;
-    set_items(b, comod::DS_TABLES);
-    if ((e = (int)comod::demo_launch<comod::DemoTablesK>(b, s))) return e;
-    set_items(b, comod::DS_DOWN_W);
-    if ((e = (int)comod::demo_launch<comod::DemoDownWK>(b, s))) return e;
-    set_items(b, comod::DS_DOWN_H);
-    if ((e = (int)comod::demo_launch<comod::DemoDownHK>(b, s))) return e;
-    set_items(b, comod::DS_SQUARE);
-    return (int)comod::demo_launch<comod::DemoSquareK>(b, s);
+    comod::set_items(b, comod::DS_TABLES, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoTablesK>(b, s))) return e;
+    comod::set_items(b, comod::DS_DOWN_W, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoDownWK>(b, s))) return e;
+    comod::set_items(b, comod::DS_DOWN_H, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoDownHK>(b, s))) return e;
+    comod::set_items(b, comod::DS_SQUARE, comod::demo_items);
+    return (int)comod::batch_launch<comod::DemoSquareK>(b, s);
 }
 
 int launch_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, ck_stream_t s) {
@@ -578,50 +512,69 @@ int launch_demo_postprocess(const float* y, const migan_demo_request* q, int n, 
     demo_layout(q, n, res, scratch, &b);
     b.y = y;
     int e;
-    set_items(b, comod::DS_POST_W);
-    if ((e = (int)comod::demo_launch<comod::DemoPostWK>(b, s))) return e;
-    set_items(b, comod::DS_OUT);
-    return (int)comod::demo_launch<comod::DemoOutK>(b, s);
+    comod::set_items(b, comod::DS_POST_W, comod::demo_items);
+    if ((e = (int)comod::batch_launch<comod::DemoPostWK>(b, s))) return e;
+    comod::set_items(b, comod::DS_OUT, comod::demo_items);
+    return (int)comod::batch_launch<comod::DemoOutK>(b, s);
 }
 
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
-static char g_demo_msg[256];
-extern "C" const char* migan_emul_demo_error(void) { return g_demo_msg; }
-extern "C" int migan_demo_resized_size(int w, int h, int max_size, int* ow, int* oh) {
-    if (!ow || !oh || max_size < 1) return MIGAN_ERR_INVALID;
-    return migan::demo_resized_size(w, h, max_size, ow, oh);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h) {
+    if (!out_w || !out_h) return fail(MIGAN_ERR_INVALID, "demo_resized_size: null argument");
+    if (w < 1 || h < 1 || max_size < 1) return fail(MIGAN_ERR_INVALID, "demo_resized_size: bad arguments (%d x %d, max size %d)", w, h, max_size);
+    return migan::demo_resized_size(w, h, max_size, out_w, out_h);
 }
-extern "C" size_t b200_demo_scratch_bytes(const migan_demo_request* q, int n, int res) {
-    if (migan::check_demo_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return 0;
-    return migan::demo_scratch_bytes(q, n, res);
+
+size_t b200_demo_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
+    if (migan::check_demo_batch("demo_scratch_bytes", reqs, n, res, false)) return 0;
+    return migan::demo_scratch_bytes(reqs, n, res);
 }
-extern "C" int b200_demo_preprocess(const migan_demo_request* q, int n, int res, float* x, void* scratch, size_t bytes, void* s) {
-    if (int rc = migan::check_demo_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return rc;
-    if (!x || !scratch) return MIGAN_ERR_INVALID;
-    if (bytes < migan::demo_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_demo_preprocess(q, n, res, x, scratch, s);
+
+int b200_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_demo_batch("demo_preprocess", reqs, n, res, false)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "demo_preprocess: null argument");
+    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_demo_preprocess(reqs, n, res, x, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" size_t b200_eval_scratch_bytes(const migan_demo_request* q, int n, int res) {
-    if (migan::check_eval_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return 0;
-    return migan::eval_scratch_bytes(q, n, res);
+
+int b200_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, size_t scratch_bytes,
+                          void* stream) {
+    if (int rc = migan::check_demo_batch("demo_postprocess", reqs, n, res, false)) return rc;
+    if (!y || !scratch) return fail(MIGAN_ERR_INVALID, "demo_postprocess: null argument");
+    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_demo_postprocess(y, reqs, n, res, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_eval_preprocess(const migan_demo_request* q, int n, int res, float* x, float* img, void* scratch, size_t bytes,
-                                    void* s) {
-    if (int rc = migan::check_eval_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return rc;
-    if (!x || !img || !scratch) return MIGAN_ERR_INVALID;
-    if (bytes < migan::eval_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_eval_preprocess(q, n, res, x, img, scratch, s);
+
+size_t b200_eval_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
+    if (migan::check_demo_batch("eval_scratch_bytes", reqs, n, res, true)) return 0;
+    return migan::eval_scratch_bytes(reqs, n, res);
 }
-extern "C" int b200_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, void* s) {
-    if (!x || !y || !real || !composed || n < 1 || res < 1) return MIGAN_ERR_INVALID;
-    return migan::launch_eval_composite(x, y, n, res, real, composed, s);
+
+int b200_eval_preprocess(const migan_demo_request* reqs, int n, int res, float* x, float* img, void* scratch,
+                         size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_demo_batch("eval_preprocess", reqs, n, res, true)) return rc;
+    if (!x || !img || !scratch) return fail(MIGAN_ERR_INVALID, "eval_preprocess: null argument");
+    const size_t need = migan::eval_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "eval_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_eval_preprocess(reqs, n, res, x, img, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_demo_postprocess(const float* y, const migan_demo_request* q, int n, int res, void* scratch, size_t bytes, void* s) {
-    if (int rc = migan::check_demo_batch(q, n, res, g_demo_msg, sizeof g_demo_msg)) return rc;
-    if (!y || !scratch) return MIGAN_ERR_INVALID;
-    if (bytes < migan::demo_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_demo_postprocess(y, q, n, res, scratch, s);
+
+int b200_eval_composite(const float* x, const float* y, int n, int res, float* img, float* composed, void* stream) {
+    if (!x || !y || !img || !composed) return fail(MIGAN_ERR_INVALID, "eval_composite: null argument");
+    if (n < 1 || res < 1 || res > 8192) return fail(MIGAN_ERR_INVALID, "eval_composite: %d images at resolution %d", n, res);
+    CUDA_TRY(migan::launch_eval_composite(x, y, n, res, img, composed, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+}  // extern "C"

@@ -10,19 +10,14 @@
 // that touches the border continues into the pad as a hole instead of zeroed pixels marked known.
 //
 // A pass of up to MIGAN_PIPE_MAX_BATCH requests of mixed sizes is one launch per phase; the request table travels by
-// value in the kernel parameter (FullResBatch, < 4 KB) with the phase's item prefix, as in demo_resize.cu.  Each
+// value in the kernel parameter (FullResBatch, < 4 KB) with the phase's item prefix (batch_launch, comod_kernels.cuh).  Each
 // request's x / y point at its slot of its chunk's tensors, so requests of different extents share the launch.
-// Item functors (comod_kernels.cuh style): the emulation build (tests/emul/build_fullres.py) runs them on the CPU.
+// Item functors (comod_kernels.cuh style): the emulation build (tests/emul/build_emul.py) runs them on the CPU.
 // The per-pixel arithmetic is prepost.cuh's, so the bytes equal forward_fc_u8's on the padded photo by construction.
 // The hole-window path (holewin.cu) runs the same functors on windows of a photo (b200_window_*): a request is an H x W
 // crop at the photo's row pitch, reflect-padded within the crop, and the post-processing writes only the crop.
 #include "prepost.cuh"
-#include "../../include/migan_b200.h"
-#ifndef MIGAN_EMULATE
-#include "kernels.h"
-#endif
-
-#include <cstdio>
+#include "abi_error.h"
 
 namespace comod {
 
@@ -47,14 +42,6 @@ struct FullResBatch {
     int64_t start[MIGAN_PIPE_MAX_BATCH + 1];   // item prefix of the launch
     FullResReq r[MIGAN_PIPE_MAX_BATCH];
     int n;
-    CK_HD int find(int64_t i) const {           // the request item i belongs to
-        int lo = 0, hi = n - 1;
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (start[mid] <= i) lo = mid; else hi = mid - 1;
-        }
-        return lo;
-    }
 };
 static_assert(sizeof(FullResBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
 
@@ -66,7 +53,7 @@ CK_HD int64_t fullres_post_items(const FullResReq& r) { return (int64_t)r.H * r.
 struct FullResPreK {
     const FullResBatch& b;
     PP_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const FullResReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int groups = (r.Wp + 3) >> 2;
@@ -109,7 +96,7 @@ struct FullResPreK {
 struct FullResPostK {
     const FullResBatch& b;
     PP_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const FullResReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int row = (int)(j / r.W), col = (int)(j - (int64_t)row * r.W);
@@ -122,25 +109,6 @@ struct FullResPostK {
         for (int c = 0; c < 3; ++c) o[c] = known ? p[c] : post_u8(y[c * plane]);
     }
 };
-
-#ifdef MIGAN_EMULATE
-template <class F>
-inline int fullres_launch(const FullResBatch& b, ck_stream_t s) { return ck_launch(F{b}, b.start[b.n], s); }
-#else
-// One thread per item; __grid_constant__ lets the functors index the request table in the parameter space.
-template <class F>
-__global__ void __launch_bounds__(256) fullres_items_kernel(const __grid_constant__ FullResBatch b, const int64_t items) {
-    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i < items) F{b}(i);
-}
-template <class F>
-inline cudaError_t fullres_launch(const FullResBatch& b, ck_stream_t s) {
-    const int64_t items = b.start[b.n];
-    if (items <= 0) return cudaSuccess;
-    fullres_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(b, items);
-    return cudaGetLastError();
-}
-#endif
 
 }  // namespace comod
 
@@ -180,102 +148,82 @@ comod::FullResBatch window_batch(const migan_window_request* q, int n, bool pre)
 
 }  // namespace
 
-int check_fullres_batch(const migan_fullres_request* q, int n, bool pre, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
+int check_fullres_batch(const char* who, const migan_fullres_request* q, int n, bool pre) {
+    if (int rc = check_batch_size(who, q, n)) return rc;
     for (int k = 0; k < n; ++k) {
         const migan_fullres_request& r = q[k];
-        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out)) {
-            snprintf(msg, len, "request %d: null photo, mask, %s", k, pre ? "or x" : "y or output");
-            return MIGAN_ERR_INVALID;
-        }
-        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) {
-            snprintf(msg, len, "request %d: x must be 16-byte aligned", k);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.H < 1 || r.W < 1 || r.Hp < r.H || r.Wp < r.W) {
-            snprintf(msg, len, "request %d: photo of %d x %d, padded extent %d x %d (H x W)", k, r.H, r.W, r.Hp, r.Wp);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.mask_channels < 1 || r.mask_channels > 4) {
-            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
-            return MIGAN_ERR_INVALID;
-        }
+        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out))
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: null photo, mask, %s", who, k, pre ? "or x" : "y or output");
+        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) return fail(MIGAN_ERR_INVALID, "%s: request %d: x must be 16-byte aligned", who, k);
+        if (r.H < 1 || r.W < 1 || r.Hp < r.H || r.Wp < r.W)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: photo of %d x %d, padded extent %d x %d (H x W)", who, k, r.H, r.W, r.Hp, r.Wp);
+        if (int rc = check_mask_channels(who, k, r.mask_channels)) return rc;
     }
     return MIGAN_OK;
 }
 
 int launch_fullres_preprocess(const migan_fullres_request* q, int n, ck_stream_t s) {
-    return (int)comod::fullres_launch<comod::FullResPreK>(fullres_batch(q, n, true), s);
+    return (int)comod::batch_launch<comod::FullResPreK>(fullres_batch(q, n, true), s);
 }
 
 int launch_fullres_postprocess(const migan_fullres_request* q, int n, ck_stream_t s) {
-    return (int)comod::fullres_launch<comod::FullResPostK>(fullres_batch(q, n, false), s);
+    return (int)comod::batch_launch<comod::FullResPostK>(fullres_batch(q, n, false), s);
 }
 
-int check_window_batch(const migan_window_request* q, int n, bool pre, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
+int check_window_batch(const char* who, const migan_window_request* q, int n, bool pre) {
+    if (int rc = check_batch_size(who, q, n)) return rc;
     for (int k = 0; k < n; ++k) {
         const migan_window_request& r = q[k];
-        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out)) {
-            snprintf(msg, len, "request %d: null photo, mask, %s", k, pre ? "or x" : "y or output");
-            return MIGAN_ERR_INVALID;
-        }
-        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) {
-            snprintf(msg, len, "request %d: x must be 16-byte aligned", k);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.H < 1 || r.W < 1 || r.h < 1 || r.w < 1 || r.y0 < 0 || r.x0 < 0 || r.y0 > r.H - r.h || r.x0 > r.W - r.w) {
-            snprintf(msg, len, "request %d: window (y0 %d, x0 %d, h %d, w %d) of a photo of %d x %d (H x W)", k, r.y0, r.x0,
-                     r.h, r.w, r.H, r.W);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.Hp < r.h || r.Wp < r.w) {
-            snprintf(msg, len, "request %d: window of %d x %d, padded extent %d x %d (h x w)", k, r.h, r.w, r.Hp, r.Wp);
-            return MIGAN_ERR_INVALID;
-        }
-        if (r.mask_channels < 1 || r.mask_channels > 4) {
-            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, r.mask_channels);
-            return MIGAN_ERR_INVALID;
-        }
+        if (!r.img || !r.mask || !(pre ? (const void*)r.x : (const void*)r.y) || (!pre && !r.out))
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: null photo, mask, %s", who, k, pre ? "or x" : "y or output");
+        if (pre && (reinterpret_cast<uintptr_t>(r.x) & 15)) return fail(MIGAN_ERR_INVALID, "%s: request %d: x must be 16-byte aligned", who, k);
+        if (r.H < 1 || r.W < 1 || r.h < 1 || r.w < 1 || r.y0 < 0 || r.x0 < 0 || r.y0 > r.H - r.h || r.x0 > r.W - r.w)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: window (y0 %d, x0 %d, h %d, w %d) of a photo of %d x %d (H x W)", who, k,
+                        r.y0, r.x0, r.h, r.w, r.H, r.W);
+        if (r.Hp < r.h || r.Wp < r.w)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: window of %d x %d, padded extent %d x %d (h x w)", who, k, r.h, r.w, r.Hp, r.Wp);
+        if (int rc = check_mask_channels(who, k, r.mask_channels)) return rc;
     }
     return MIGAN_OK;
 }
 
 int launch_window_preprocess(const migan_window_request* q, int n, ck_stream_t s) {
-    return (int)comod::fullres_launch<comod::FullResPreK>(window_batch(q, n, true), s);
+    return (int)comod::batch_launch<comod::FullResPreK>(window_batch(q, n, true), s);
 }
 
 int launch_window_postprocess(const migan_window_request* q, int n, ck_stream_t s) {
-    return (int)comod::fullres_launch<comod::FullResPostK>(window_batch(q, n, false), s);
+    return (int)comod::batch_launch<comod::FullResPostK>(window_batch(q, n, false), s);
 }
 
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
-static char g_fullres_msg[256];
-extern "C" const char* migan_emul_fullres_error(void) { return g_fullres_msg; }
-extern "C" int b200_fullres_preprocess(const migan_fullres_request* q, int n, void* s) {
-    if (int rc = migan::check_fullres_batch(q, n, true, g_fullres_msg, sizeof g_fullres_msg)) return rc;
-    return migan::launch_fullres_preprocess(q, n, s);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+int b200_fullres_preprocess(const migan_fullres_request* reqs, int n, void* stream) {
+    if (int rc = migan::check_fullres_batch("fullres_preprocess", reqs, n, true)) return rc;
+    CUDA_TRY(migan::launch_fullres_preprocess(reqs, n, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_fullres_postprocess(const migan_fullres_request* q, int n, void* s) {
-    if (int rc = migan::check_fullres_batch(q, n, false, g_fullres_msg, sizeof g_fullres_msg)) return rc;
-    return migan::launch_fullres_postprocess(q, n, s);
+
+int b200_fullres_postprocess(const migan_fullres_request* reqs, int n, void* stream) {
+    if (int rc = migan::check_fullres_batch("fullres_postprocess", reqs, n, false)) return rc;
+    CUDA_TRY(migan::launch_fullres_postprocess(reqs, n, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_window_preprocess(const migan_window_request* q, int n, void* s) {
-    if (int rc = migan::check_window_batch(q, n, true, g_fullres_msg, sizeof g_fullres_msg)) return rc;
-    return migan::launch_window_preprocess(q, n, s);
+
+int b200_window_preprocess(const migan_window_request* reqs, int n, void* stream) {
+    if (int rc = migan::check_window_batch("window_preprocess", reqs, n, true)) return rc;
+    CUDA_TRY(migan::launch_window_preprocess(reqs, n, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_window_postprocess(const migan_window_request* q, int n, void* s) {
-    if (int rc = migan::check_window_batch(q, n, false, g_fullres_msg, sizeof g_fullres_msg)) return rc;
-    return migan::launch_window_postprocess(q, n, s);
+
+int b200_window_postprocess(const migan_window_request* reqs, int n, void* stream) {
+    if (int rc = migan::check_window_batch("window_postprocess", reqs, n, false)) return rc;
+    CUDA_TRY(migan::launch_window_postprocess(reqs, n, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+}  // extern "C"

@@ -10,15 +10,11 @@
 // load when the chunk lies inside the row's bytes, byte loads at the ends), and a hole marks the cell's byte in shared
 // memory; the block then writes one byte per cell, so every cell byte is written exactly once and needs no clearing.
 // The hole test is prepost.cuh's (mask_channel + known_value), the same as the pre- and post-processing's.
-// The emulation build (tests/emul/build_holewin.py) runs the same block functions with the threads of a block in turn.
+// The emulation build (tests/emul/build_emul.py) runs the same block functions with the threads of a block in turn.
 #include "prepost.cuh"
-#include "../../include/migan_b200.h"
-#ifndef MIGAN_EMULATE
-#include "kernels.h"
-#endif
+#include "abi_error.h"
 
 #include <algorithm>
-#include <cstdio>
 #include <cstring>
 #include <vector>
 
@@ -34,14 +30,6 @@ struct CellsBatch {
     int64_t cell_start[MIGAN_PIPE_MAX_BATCH + 1];    // cell-byte prefix: request k's cells start at cell_start[k]
     CellsReq r[MIGAN_PIPE_MAX_BATCH];
     int n, qshift, S;                                // q = 1 << qshift; S cells per block
-    CK_HD int find(int64_t i) const {
-        int lo = 0, hi = n - 1;
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (block_start[mid] <= i) lo = mid; else hi = mid - 1;
-        }
-        return lo;
-    }
 };
 static_assert(sizeof(CellsBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
 
@@ -50,7 +38,7 @@ struct CellsBlock { int k, cy, cx0, ncx, y0, y1, px0, px1; };
 
 CK_HD CellsBlock cells_block(const CellsBatch& b, int64_t blk) {
     CellsBlock g;
-    g.k = b.find(blk);
+    g.k = find_request(b.block_start, b.n, blk);
     const CellsReq& r = b.r[g.k];
     const int64_t j = blk - b.block_start[g.k];
     g.cy = (int)(j / r.nseg);
@@ -193,25 +181,15 @@ struct Win {
 
 }  // namespace
 
-int check_hole_cells(const migan_cells_request* q, int n, int res, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
-    if (log2_resolution(res) < 0) { snprintf(msg, len, "resolution %d (a power of two >= 8)", res); return MIGAN_ERR_INVALID; }
+int check_hole_cells(const char* who, const migan_cells_request* q, int n, int res) {
+    if (int rc = check_batch_size(who, q, n)) return rc;
+    if (log2_resolution(res) < 0) return fail(MIGAN_ERR_INVALID, "%s: resolution %d (a power of two >= 8)", who, res);
     for (int k = 0; k < n; ++k) {
-        if (!q[k].mask) { snprintf(msg, len, "request %d: null mask", k); return MIGAN_ERR_INVALID; }
-        if (q[k].H < 1 || q[k].W < 1) {
-            snprintf(msg, len, "request %d: mask of %d x %d (H x W)", k, q[k].H, q[k].W);
-            return MIGAN_ERR_INVALID;
-        }
-        if (q[k].mask_channels < 1 || q[k].mask_channels > 4) {
-            snprintf(msg, len, "request %d: mask of %d channels (1 to 4)", k, q[k].mask_channels);
-            return MIGAN_ERR_INVALID;
-        }
+        if (!q[k].mask) return fail(MIGAN_ERR_INVALID, "%s: request %d: null mask", who, k);
+        if (q[k].H < 1 || q[k].W < 1) return fail(MIGAN_ERR_INVALID, "%s: request %d: mask of %d x %d (H x W)", who, k, q[k].H, q[k].W);
+        if (int rc = check_mask_channels(who, k, q[k].mask_channels)) return rc;
     }
-    if (cells_batch(q, n, res).block_start[n] > INT32_MAX) { snprintf(msg, len, "masks too large"); return MIGAN_ERR_INVALID; }
+    if (cells_batch(q, n, res).block_start[n] > INT32_MAX) return fail(MIGAN_ERR_INVALID, "%s: masks too large", who);
     return MIGAN_OK;
 }
 
@@ -221,22 +199,19 @@ int launch_hole_cells(const migan_cells_request* q, int n, int res, uint8_t* cel
     return (int)comod::cells_launch(cells_batch(q, n, res), cells, s);
 }
 
-int hole_windows_max(int H, int W, int res, int* max_windows, char* msg, size_t len) {
-    if (H < 1 || W < 1 || log2_resolution(res) < 0) {
-        snprintf(msg, len, "photo of %d x %d (H x W) at resolution %d (a power of two >= 8)", H, W, res);
-        return MIGAN_ERR_INVALID;
-    }
+int hole_windows_max(const char* who, int H, int W, int res, int* max_windows) {
+    if (H < 1 || W < 1 || log2_resolution(res) < 0)
+        return fail(MIGAN_ERR_INVALID, "%s: photo of %d x %d (H x W) at resolution %d (a power of two >= 8)", who, H, W, res);
     const int64_t m = (int64_t)(H / std::min(res, H)) * (W / std::min(res, W));
-    if (m > INT32_MAX) { snprintf(msg, len, "photo of %d x %d (H x W): too many windows", H, W); return MIGAN_ERR_INVALID; }
+    if (m > INT32_MAX) return fail(MIGAN_ERR_INVALID, "%s: photo of %d x %d (H x W): too many windows", who, H, W);
     *max_windows = (int)m;
     return MIGAN_OK;
 }
 
-int hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* win4, int max_windows, int* count, char* msg,
-                 size_t len) {
+int hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* win4, int max_windows, int* count) {
     int bound = 0;
-    if (int rc = hole_windows_max(H, W, res, &bound, msg, len)) return rc;
-    if (margin < 0) { snprintf(msg, len, "margin of %d cells", margin); return MIGAN_ERR_INVALID; }
+    if (int rc = hole_windows_max("hole_windows", H, W, res, &bound)) return rc;
+    if (margin < 0) return fail(MIGAN_ERR_INVALID, "hole_windows: margin of %d cells", margin);
     const int64_t R = res, q = res / 4;
     const int64_t gh = (H + q - 1) / q, gw = (W + q - 1) / q;
     auto make = [&](int64_t r0, int64_t r1, int64_t c0, int64_t c1) {
@@ -258,10 +233,7 @@ int hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* w
             list.push_back(cur);
         }
     std::sort(list.begin(), list.end(), [](const Win& a, const Win& b) { return a.y.s != b.y.s ? a.y.s < b.y.s : a.x.s < b.x.s; });
-    if ((int64_t)list.size() > max_windows) {
-        snprintf(msg, len, "%zu windows, room for %d", list.size(), max_windows);
-        return MIGAN_ERR_INVALID;
-    }
+    if ((int64_t)list.size() > max_windows) return fail(MIGAN_ERR_INVALID, "hole_windows: %zu windows, room for %d", list.size(), max_windows);
     for (size_t k = 0; k < list.size(); ++k) {
         win4[4 * k] = (int)list[k].y.s; win4[4 * k + 1] = (int)list[k].x.s;
         win4[4 * k + 2] = (int)list[k].y.L; win4[4 * k + 3] = (int)list[k].x.L;
@@ -272,16 +244,31 @@ int hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* w
 
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
-static char g_holewin_msg[256];
-extern "C" const char* migan_emul_holewin_error(void) { return g_holewin_msg; }
-extern "C" size_t b200_hole_cells_bytes(const migan_cells_request* q, int n, int res) {
-    if (migan::check_hole_cells(q, n, res, g_holewin_msg, sizeof g_holewin_msg)) return 0;
-    return migan::hole_cells_bytes(q, n, res);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+size_t b200_hole_cells_bytes(const migan_cells_request* reqs, int n, int res) {
+    if (migan::check_hole_cells("hole_cells_bytes", reqs, n, res)) return 0;
+    return migan::hole_cells_bytes(reqs, n, res);
 }
-extern "C" int b200_hole_cells(const migan_cells_request* q, int n, int res, uint8_t* cells, void* s) {
-    if (int rc = migan::check_hole_cells(q, n, res, g_holewin_msg, sizeof g_holewin_msg)) return rc;
-    if (!cells) return MIGAN_ERR_INVALID;
-    return migan::launch_hole_cells(q, n, res, cells, s);
+
+int b200_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* cells, void* stream) {
+    if (int rc = migan::check_hole_cells("hole_cells", reqs, n, res)) return rc;
+    if (!cells) return fail(MIGAN_ERR_INVALID, "hole_cells: null cells");
+    CUDA_TRY(migan::launch_hole_cells(reqs, n, res, cells, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+int migan_hole_windows_max(int H, int W, int res, int* max_windows) {
+    if (!max_windows) return fail(MIGAN_ERR_INVALID, "hole_windows_max: null argument");
+    return migan::hole_windows_max("hole_windows_max", H, W, res, max_windows);
+}
+
+int migan_hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* win4, int max_windows, int* count) {
+    if (!cells || !win4 || !count) return fail(MIGAN_ERR_INVALID, "hole_windows: null argument");
+    return migan::hole_windows(cells, H, W, res, margin, win4, max_windows, count);
+}
+
+}  // extern "C"

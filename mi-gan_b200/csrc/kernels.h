@@ -74,78 +74,8 @@ cudaError_t launch_bias_act(const float* x, const float* b, float* y, int64_t nu
                             int act, float alpha, float gain, float clamp, cudaStream_t s);
 
 // ---- uint8 pre/post-processing (prepost.cu): demo.py:56-66 and :135-142 around the forward ------
-// feathered composite of the ONNX pipeline (create_onnx_pipeline.py:233-245): NCHW uint8 image / mask, 25 smoothing taps (host array)
-int launch_feather_composite(const float* y_nchw, const uint8_t* img_nchw, const uint8_t* mask_n1hw, uint8_t* out_nchw, int n, int H, int W,
-                             const float* k25_host, cudaStream_t s);
 int launch_preprocess_u8(const uint8_t* img_hwc, const uint8_t* mask_hw, float* x_nchw, int n, int H, int W, cudaStream_t s);
 int launch_postprocess_u8(const float* y_nchw, const uint8_t* img_hwc, const uint8_t* mask_hw, uint8_t* out_hwc, int n, int H, int W,
                           cudaStream_t s);
-
-
-
-// ---- arbitrary-resolution crop pipeline (pipeline.cu): scripts/create_onnx_pipeline.py:121-264 ------
-size_t pipeline_scratch_bytes(int H, int W, int res);
-int launch_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, cudaStream_t s);
-int launch_hole_flags(const uint8_t* mask, int H, int W, uint8_t* flags, cudaStream_t s);
-void crop_box_from_flags(const uint8_t* flags_host, int H, int W, int res, int padding, int* box4);
-int launch_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
-                               void* scratch, cudaStream_t s);
-int launch_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
-                                const float* k25_host, void* scratch, cudaStream_t s);
-// batches of 1..MIGAN_PIPE_MAX_BATCH requests of any sizes, one launch per stage
-size_t pipeline_batch_scratch_bytes(const migan_pipe_request* reqs, int n, int res);
-int check_pipe_batch(const migan_pipe_request* reqs, int n, int res, bool boxes, char* msg, size_t len);
-int launch_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flags, cudaStream_t s);
-int launch_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
-int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
-                                      void* scratch, cudaStream_t s);
-// the same batches with the crop windows planned on the device from the flags (no host round trip)
-int check_pipe_planned(const migan_pipe_request* reqs, int n, int res, char* msg, size_t len);
-size_t pipeline_batch_scratch_bound(const migan_pipe_request* reqs, int n, int res);
-int launch_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int padding, const uint8_t* flags, int* boxes,
-                               void* scratch, cudaStream_t s);
-int launch_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
-int launch_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25_host,
-                                        void* scratch, cudaStream_t s);
-
-// ---- the reference demo's request path at any photo size (demo_resize.cu): scripts/demo.py:26-66, :120-143 ------
-int demo_resized_size(int w, int h, int max_size, int* ow, int* oh);
-int check_demo_batch(const migan_demo_request* reqs, int n, int res, char* msg, size_t len);
-size_t demo_scratch_bytes(const migan_demo_request* reqs, int n, int res);
-int launch_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, cudaStream_t s);
-// the evaluation batch (evaluate_fid_lpips.py InferenceDataset + :246-249) on the same stages
-int check_eval_batch(const migan_demo_request* reqs, int n, int res, char* msg, size_t len);
-size_t eval_scratch_bytes(const migan_demo_request* reqs, int n, int res);
-int launch_eval_preprocess(const migan_demo_request* reqs, int n, int res, float* x, float* img, void* scratch, cudaStream_t s);
-int launch_eval_composite(const float* x, const float* y, int n, int res, float* real, float* composed, cudaStream_t s);
-int launch_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, cudaStream_t s);
-
-// ---- full-resolution request path (fullres.cu): reflect padding and the composite around migan_forward_hw ------
-int check_fullres_batch(const migan_fullres_request* reqs, int n, bool pre, char* msg, size_t len);
-int launch_fullres_preprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
-int launch_fullres_postprocess(const migan_fullres_request* reqs, int n, cudaStream_t s);
-// the same kernels on windows of a photo (the whole photo is the window (0, 0, H, W))
-int check_window_batch(const migan_window_request* reqs, int n, bool pre, char* msg, size_t len);
-int launch_window_preprocess(const migan_window_request* reqs, int n, cudaStream_t s);
-int launch_window_postprocess(const migan_window_request* reqs, int n, cudaStream_t s);
-
-// ---- hole-window request path (holewin.cu): hole cells on the device, the window planner on the host ------
-int check_hole_cells(const migan_cells_request* reqs, int n, int res, char* msg, size_t len);
-size_t hole_cells_bytes(const migan_cells_request* reqs, int n, int res);
-int launch_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* cells, cudaStream_t s);
-int hole_windows_max(int H, int W, int res, int* max_windows, char* msg, size_t len);
-int hole_windows(const uint8_t* cells_host, int H, int W, int res, int margin, int* win4, int max_windows, int* count, char* msg,
-                 size_t len);
-
-// ---- free-form masks of the evaluation protocol (masks.cu): numpy's stream on the host, the rasterizer on the device ----
-void np_seed(migan_np_random* st, uint32_t seed);
-int check_mask_size(int s, int n_att, char* msg, size_t len);
-int mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states, char* msg, size_t len);
-int launch_mask_raster(const migan_mask_record* recs, int n_att, int s, uint8_t* attempts, int* holes, cudaStream_t s_);
-int launch_mask_compact(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out, cudaStream_t s_);
-
-
-// ---- training snapshot -> inference filters (reparam.cu): scripts/export_inference_model.py:18-27 ------
-int launch_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fan, float* out, cudaStream_t s);
 
 }  // namespace migan

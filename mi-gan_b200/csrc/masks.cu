@@ -11,15 +11,11 @@
 // coordinates with Pillow's float32 operations each rounded on its own (PP_MUL / PP_ADD / PP_DIV of prepost.cuh), and the
 // vertex discs are one fixed stamp per radius (kDiscHalf).  The brush is painted at the un-flipped coordinates and each
 // span mirrored into the output, so the flips cost nothing.  oracle/masks_oracle.py states the same rules in numpy.
-// The emulation build (tests/emul/build_masks.py) runs the same block functions with the threads of a block in turn.
+// The emulation build (tests/emul/build_emul.py) runs the same block functions with the threads of a block in turn.
 #include "prepost.cuh"
-#include "../../include/migan_b200.h"
-#ifndef MIGAN_EMULATE
-#include "kernels.h"
-#endif
+#include "abi_error.h"
 
 #include <cmath>
-#include <cstdio>
 #include <cstring>
 
 namespace comod {
@@ -473,22 +469,17 @@ void np_seed(migan_np_random* st, uint32_t seed) {
     st->gauss = 0.0;
 }
 
-int check_mask_size(int s, int n_att, char* msg, size_t len) {
-    if (s < MIGAN_MASK_MIN_SIZE || s > MIGAN_MASK_MAX_SIZE) {
-        snprintf(msg, len, "mask size %d (%d to %d)", s, MIGAN_MASK_MIN_SIZE, MIGAN_MASK_MAX_SIZE);
-        return MIGAN_ERR_INVALID;
-    }
-    if (n_att < 1 || n_att > MIGAN_MASK_MAX_ATTEMPTS) {
-        snprintf(msg, len, "%d attempts (1 to %d per call)", n_att, MIGAN_MASK_MAX_ATTEMPTS);
-        return MIGAN_ERR_INVALID;
-    }
+int check_mask_size(const char* who, int s, int n_att) {
+    if (s < MIGAN_MASK_MIN_SIZE || s > MIGAN_MASK_MAX_SIZE)
+        return fail(MIGAN_ERR_INVALID, "%s: mask size %d (%d to %d)", who, s, MIGAN_MASK_MIN_SIZE, MIGAN_MASK_MAX_SIZE);
+    if (n_att < 1 || n_att > MIGAN_MASK_MAX_ATTEMPTS)
+        return fail(MIGAN_ERR_INVALID, "%s: %d attempts (1 to %d per call)", who, n_att, MIGAN_MASK_MAX_ATTEMPTS);
     return MIGAN_OK;
 }
 
-int mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states, char* msg,
-              size_t len) {
-    if (int rc = check_mask_size(s, n_att, msg, len)) return rc;
-    if (st->pos < 0 || st->pos > MT_N) { snprintf(msg, len, "state position %d (0 to %d)", st->pos, MT_N); return MIGAN_ERR_INVALID; }
+int mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states) {
+    if (int rc = check_mask_size("mask_plan", s, n_att)) return rc;
+    if (st->pos < 0 || st->pos > MT_N) return fail(MIGAN_ERR_INVALID, "mask_plan: state position %d (0 to %d)", st->pos, MT_N);
     for (int k = 0; k < n_att; ++k) {
         plan_attempt(*st, s, recs[k]);
         if (states) states[k] = *st;
@@ -507,24 +498,36 @@ int launch_mask_compact(const uint8_t* attempts, const int* holes, int n_att, in
 
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
-static char g_masks_msg[256];
-extern "C" const char* migan_emul_masks_error(void) { return g_masks_msg; }
-extern "C" int migan_np_seed(migan_np_random* st, uint32_t seed) {
-    if (!st) return MIGAN_ERR_INVALID;
-    migan::np_seed(st, seed);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+int migan_np_seed(migan_np_random* state, uint32_t seed) {
+    if (!state) return fail(MIGAN_ERR_INVALID, "np_seed: null state");
+    migan::np_seed(state, seed);
     return MIGAN_OK;
 }
-extern "C" int migan_mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states) {
-    if (!st || !recs) return MIGAN_ERR_INVALID;
-    return migan::mask_plan(st, s, n_att, recs, states, g_masks_msg, sizeof g_masks_msg);
+
+int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_record* records, migan_np_random* states) {
+    if (!state || !records) return fail(MIGAN_ERR_INVALID, "mask_plan: null argument");
+    return migan::mask_plan(state, s, n_attempts, records, states);
 }
-extern "C" int b200_mask_raster(const migan_mask_record* recs, int n_att, int s, uint8_t* attempts, int* holes, void* st) {
-    if (int rc = migan::check_mask_size(s, n_att, g_masks_msg, sizeof g_masks_msg)) return rc;
-    return migan::launch_mask_raster(recs, n_att, s, attempts, holes, st);
+
+int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream) {
+    if (int rc = migan::check_mask_size("mask_raster", s, n_attempts)) return rc;
+    if (!records || !attempts || !holes) return fail(MIGAN_ERR_INVALID, "mask_raster: null argument");
+    if (reinterpret_cast<uintptr_t>(attempts) & 15) return fail(MIGAN_ERR_INVALID, "mask_raster: attempts not 16-byte aligned");
+    CUDA_TRY(migan::launch_mask_raster(records, n_attempts, s, attempts, holes, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out, void* st) {
-    if (int rc = migan::check_mask_size(s, n_att, g_masks_msg, sizeof g_masks_msg)) return rc;
-    return migan::launch_mask_compact(attempts, holes, n_att, s, n, out, st);
+
+int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream) {
+    if (int rc = migan::check_mask_size("mask_compact", s, n_attempts)) return rc;
+    if (n < 0 || n > 65535) return fail(MIGAN_ERR_INVALID, "mask_compact: %d masks (0 to 65535 per call)", n);
+    if (!attempts || !holes || (n && !out)) return fail(MIGAN_ERR_INVALID, "mask_compact: null argument");
+    CUDA_TRY(migan::launch_mask_compact(attempts, holes, n_attempts, s, n, out, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+}  // extern "C"

@@ -11,7 +11,6 @@
 #include <algorithm>
 #include <array>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -22,29 +21,13 @@
 #include <vector>
 
 #include "../../include/migan_b200.h"
+#include "abi_error.h"
 #include "kernels.h"
 #include "sepconv_tc.h"
 
+using migan::fail;
+
 namespace {
-
-thread_local std::string g_last_error;
-
-int fail(int code, const char* fmt, ...) {
-    char buf[1024];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    g_last_error = buf;
-    return code;
-}
-
-#define CUDA_TRY(expr)                                                                        \
-    do {                                                                                      \
-        cudaError_t _e = (expr);                                                              \
-        if (_e != cudaSuccess)                                                                \
-            return fail(MIGAN_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    } while (0)
 
 inline int channels(int res) { return std::min(32768 / res, 512); }  // migan_inference.py:222-223
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -359,7 +342,6 @@ struct ArenaBuilder {
 
 extern "C" {
 
-const char* migan_last_error(void) { return g_last_error.c_str(); }
 const char* migan_version(void) { return "migan_b200 0.1 (sm_90a)"; }
 
 int migan_create(int resolution, int device, migan_ctx** out) {
@@ -1364,38 +1346,6 @@ int migan_forward_u8_async(migan_ctx* ctx, const uint8_t* img_host, const uint8_
     return forward_u8_enqueue(ctx, img_host, mask_host, out_host, n, workspace, workspace_bytes, path, stream, nullptr);
 }
 
-int b200_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, void* stream) {
-    if (!img || !mask || !x || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img, mask, x, n, r, r, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, void* stream) {
-    if (!y || !img || !mask || !out || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(y, img, mask, out, n, r, r, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_preprocess_u8_hw(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, void* stream) {
-    if (!img || !mask || !x || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8_hw: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(img, mask, x, n, H, W, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_postprocess_u8_hw(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, void* stream) {
-    if (!y || !img || !mask || !out || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8_hw: bad arguments");
-    CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(y, img, mask, out, n, H, W, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_feather_composite(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W,
-                           const float* k25, void* stream) {
-    if (!y || !img || !mask || !out || !k25) return fail(MIGAN_ERR_INVALID, "feather_composite: null argument");
-    if (n <= 0 || H < 3 || W < 3) return fail(MIGAN_ERR_INVALID, "feather_composite: need n >= 1 and H, W >= 3 (reflect padding of 2), got %d x %d x %d", n, H, W);
-    CUDA_TRY((cudaError_t)migan::launch_feather_composite(y, img, mask, out, n, H, W, k25, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
 // ---- stream memory operations (multi-GPU signalling without a kernel) ----------------------------------------------------
 // cuStreamWaitValue32 / cuStreamWriteValue32 through the runtime's driver entry points (the library has no libcuda link
 // dependency).  A wait is executed by the stream's front end: no SM is occupied while a rank waits for its peers.
@@ -1430,17 +1380,6 @@ int b200_stream_write_value32(void* stream, void* addr, uint32_t value) {
     return MIGAN_OK;
 }
 
-// ---- training snapshot -> inference filters (scripts/export_inference_model.py:18-27), kernel in reparam.cu ----
-int b200_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fan, float* out, void* stream) {
-    if (!w_dev || !out) return fail(MIGAN_ERR_INVALID, "reparam_filter: null argument");
-    if (k < 1 || k > 16) return fail(MIGAN_ERR_INVALID, "reparam_filter: %d tensors (1 .. 16 supported)", k);
-    if (cout < 1 || fan < 1) return fail(MIGAN_ERR_INVALID, "reparam_filter: bad shape %d x %lld", cout, (long long)fan);
-    for (int j = 0; j < k; ++j)
-        if (!w_dev[j]) return fail(MIGAN_ERR_INVALID, "reparam_filter: tensor %d is null", j);
-    CUDA_TRY((cudaError_t)migan::launch_reparam_filter(w_dev, k, cout, fan, out, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
 int b200_enable_peer_access(int peer_device) {
     const cudaError_t e = cudaDeviceEnablePeerAccess(peer_device, 0);
     if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); return MIGAN_OK; }
@@ -1451,143 +1390,6 @@ int b200_enable_peer_access(int peer_device) {
 int b200_memcpy_async(void* dst, const void* src, size_t bytes, void* stream) {
     if (!dst || !src) return fail(MIGAN_ERR_INVALID, "memcpy_async: null argument");
     CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-// ---- arbitrary-resolution crop pipeline (scripts/create_onnx_pipeline.py:121-264), kernels in pipeline.cu ----
-size_t b200_pipeline_scratch_bytes(int H, int W, int res) {
-    if (H < 1 || W < 1 || res < 1) return 0;
-    return migan::pipeline_scratch_bytes(H, W, res);
-}
-
-int b200_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, void* stream) {
-    if (!in || !out) return fail(MIGAN_ERR_INVALID, "resize_nearest_u8: null argument");
-    if (H < 1 || W < 1 || oh < 1 || ow < 1) return fail(MIGAN_ERR_INVALID, "resize_nearest_u8: bad size %d x %d -> %d x %d", H, W, oh, ow);
-    CUDA_TRY((cudaError_t)migan::launch_resize_nearest_u8(in, H, W, out, oh, ow, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_hole_flags(const uint8_t* mask, int H, int W, uint8_t* flags, void* stream) {
-    if (!mask || !flags) return fail(MIGAN_ERR_INVALID, "hole_flags: null argument");
-    if (H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "hole_flags: bad size %d x %d", H, W);
-    CUDA_TRY((cudaError_t)migan::launch_hole_flags(mask, H, W, flags, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int migan_crop_box(const uint8_t* flags_host, int H, int W, int res, int padding, int* box4) {
-    if (!flags_host || !box4) return fail(MIGAN_ERR_INVALID, "crop_box: null argument");
-    if (H < 1 || W < 1 || res < 1 || padding < 0) return fail(MIGAN_ERR_INVALID, "crop_box: bad arguments (%d x %d, resolution %d, padding %d)", H, W, res, padding);
-    migan::crop_box_from_flags(flags_host, H, W, res, padding, box4);
-    return MIGAN_OK;
-}
-
-static int check_box(const char* who, int H, int W, const int* box) {
-    if (!box) return fail(MIGAN_ERR_INVALID, "%s: null crop window", who);
-    if (box[0] < 0 || box[1] > W || box[2] < 0 || box[3] > H || box[1] - box[0] < 3 || box[3] - box[2] < 3)
-        return fail(MIGAN_ERR_INVALID, "%s: crop window x[%d,%d) y[%d,%d) must lie inside the %d x %d image and be at least 3 x 3",
-                    who, box[0], box[1], box[2], box[3], H, W);
-    return MIGAN_OK;
-}
-
-int b200_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
-                             void* scratch, size_t scratch_bytes, void* stream) {
-    if (!image || !mask || !x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess: null argument");
-    if (int rc = check_box("pipeline_preprocess", H, W, box)) return rc;
-    if (res < 1) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess: bad resolution %d", res);
-    if (scratch_bytes < migan::pipeline_scratch_bytes(H, W, res))
-        return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, migan::pipeline_scratch_bytes(H, W, res));
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_preprocess(image, mask, H, W, box, res, x, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
-                              const float* k25, void* scratch, size_t scratch_bytes, void* stream) {
-    if (!y || !image || !mask || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess: null argument");
-    if (int rc = check_box("pipeline_postprocess", H, W, box)) return rc;
-    if (res < 1) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess: bad resolution %d", res);
-    if (scratch_bytes < migan::pipeline_scratch_bytes(H, W, res))
-        return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, migan::pipeline_scratch_bytes(H, W, res));
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess(y, image, mask, H, W, box, res, k25, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-static int check_pipe_batch(const char* who, const migan_pipe_request* reqs, int n, int res, bool boxes) {
-    char msg[256];
-    if (int rc = migan::check_pipe_batch(reqs, n, res, boxes, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-int b200_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flags, void* stream) {
-    if (int rc = check_pipe_batch("hole_flags_batch", reqs, n, 1, false)) return rc;
-    if (!flags) return fail(MIGAN_ERR_INVALID, "hole_flags_batch: null flags");
-    CUDA_TRY((cudaError_t)migan::launch_hole_flags_batch(reqs, n, flags, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* reqs, int n, int res) {
-    if (check_pipe_batch("pipeline_batch_scratch_bytes", reqs, n, res, true)) return 0;
-    return migan::pipeline_batch_scratch_bytes(reqs, n, res);
-}
-
-int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
-                                   void* stream) {
-    if (int rc = check_pipe_batch("pipeline_preprocess_batch", reqs, n, res, true)) return rc;
-    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_batch: null argument");
-    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_preprocess_batch(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
-                                    size_t scratch_bytes, void* stream) {
-    if (int rc = check_pipe_batch("pipeline_postprocess_batch", reqs, n, res, true)) return rc;
-    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_batch: null argument");
-    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess_batch(y, reqs, n, res, k25, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-static int check_pipe_planned(const char* who, const migan_pipe_request* reqs, int n, int res) {
-    char msg[256];
-    if (int rc = migan::check_pipe_planned(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-size_t b200_pipeline_batch_scratch_bound(const migan_pipe_request* reqs, int n, int res) {
-    if (check_pipe_planned("pipeline_batch_scratch_bound", reqs, n, res)) return 0;
-    return migan::pipeline_batch_scratch_bound(reqs, n, res);
-}
-
-int b200_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int padding, const uint8_t* flags, int* boxes,
-                             void* scratch, size_t scratch_bytes, void* stream) {
-    if (int rc = check_pipe_planned("pipeline_plan_batch", reqs, n, res)) return rc;
-    if (padding < 0) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: padding %d", padding);
-    if (!flags || !boxes || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: null argument");
-    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_plan_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_plan_batch(reqs, n, res, padding, flags, boxes, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
-                                     void* stream) {
-    if (int rc = check_pipe_planned("pipeline_preprocess_planned", reqs, n, res)) return rc;
-    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_planned: null argument");
-    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_preprocess_planned(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
-                                      size_t scratch_bytes, void* stream) {
-    if (int rc = check_pipe_planned("pipeline_postprocess_planned", reqs, n, res)) return rc;
-    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_planned: null argument");
-    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_pipeline_postprocess_planned(y, reqs, n, res, k25, scratch, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 
@@ -1603,166 +1405,6 @@ int migan_fullres_extent(const migan_ctx* ctx, int H, int W, int* Hp, int* Wp, i
                     (long long)hp, (long long)wp, channels(R));
     *Hp = (int)hp; *Wp = (int)wp;
     *max_n = (int)max_batch(ctx, *Hp, *Wp);
-    return MIGAN_OK;
-}
-
-static int check_fullres(const char* who, const migan_fullres_request* reqs, int n, bool pre) {
-    char msg[256];
-    if (int rc = migan::check_fullres_batch(reqs, n, pre, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-int b200_fullres_preprocess(const migan_fullres_request* reqs, int n, void* stream) {
-    if (int rc = check_fullres("fullres_preprocess", reqs, n, true)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_fullres_preprocess(reqs, n, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_fullres_postprocess(const migan_fullres_request* reqs, int n, void* stream) {
-    if (int rc = check_fullres("fullres_postprocess", reqs, n, false)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_fullres_postprocess(reqs, n, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-static int check_window(const char* who, const migan_window_request* reqs, int n, bool pre) {
-    char msg[256];
-    if (int rc = migan::check_window_batch(reqs, n, pre, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-int b200_window_preprocess(const migan_window_request* reqs, int n, void* stream) {
-    if (int rc = check_window("window_preprocess", reqs, n, true)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_window_preprocess(reqs, n, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_window_postprocess(const migan_window_request* reqs, int n, void* stream) {
-    if (int rc = check_window("window_postprocess", reqs, n, false)) return rc;
-    CUDA_TRY((cudaError_t)migan::launch_window_postprocess(reqs, n, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-static int check_hole_cells(const char* who, const migan_cells_request* reqs, int n, int res) {
-    char msg[256];
-    if (int rc = migan::check_hole_cells(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-size_t b200_hole_cells_bytes(const migan_cells_request* reqs, int n, int res) {
-    if (check_hole_cells("hole_cells_bytes", reqs, n, res)) return 0;
-    return migan::hole_cells_bytes(reqs, n, res);
-}
-
-int b200_hole_cells(const migan_cells_request* reqs, int n, int res, uint8_t* cells, void* stream) {
-    if (int rc = check_hole_cells("hole_cells", reqs, n, res)) return rc;
-    if (!cells) return fail(MIGAN_ERR_INVALID, "hole_cells: null cells");
-    CUDA_TRY((cudaError_t)migan::launch_hole_cells(reqs, n, res, cells, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int migan_hole_windows_max(int H, int W, int res, int* max_windows) {
-    char msg[256];
-    if (!max_windows) return fail(MIGAN_ERR_INVALID, "hole_windows_max: null argument");
-    if (int rc = migan::hole_windows_max(H, W, res, max_windows, msg, sizeof msg)) return fail(rc, "hole_windows_max: %s", msg);
-    return MIGAN_OK;
-}
-
-int migan_hole_windows(const uint8_t* cells, int H, int W, int res, int margin, int* win4, int max_windows, int* count) {
-    char msg[256];
-    if (!cells || !win4 || !count) return fail(MIGAN_ERR_INVALID, "hole_windows: null argument");
-    if (int rc = migan::hole_windows(cells, H, W, res, margin, win4, max_windows, count, msg, sizeof msg))
-        return fail(rc, "hole_windows: %s", msg);
-    return MIGAN_OK;
-}
-
-int migan_np_seed(migan_np_random* state, uint32_t seed) {
-    if (!state) return fail(MIGAN_ERR_INVALID, "np_seed: null state");
-    migan::np_seed(state, seed);
-    return MIGAN_OK;
-}
-
-int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_record* records, migan_np_random* states) {
-    char msg[256];
-    if (!state || !records) return fail(MIGAN_ERR_INVALID, "mask_plan: null argument");
-    if (int rc = migan::mask_plan(state, s, n_attempts, records, states, msg, sizeof msg)) return fail(rc, "mask_plan: %s", msg);
-    return MIGAN_OK;
-}
-
-int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream) {
-    char msg[256];
-    if (int rc = migan::check_mask_size(s, n_attempts, msg, sizeof msg)) return fail(rc, "mask_raster: %s", msg);
-    if (!records || !attempts || !holes) return fail(MIGAN_ERR_INVALID, "mask_raster: null argument");
-    if (reinterpret_cast<uintptr_t>(attempts) & 15) return fail(MIGAN_ERR_INVALID, "mask_raster: attempts not 16-byte aligned");
-    CUDA_TRY((cudaError_t)migan::launch_mask_raster(records, n_attempts, s, attempts, holes, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream) {
-    char msg[256];
-    if (int rc = migan::check_mask_size(s, n_attempts, msg, sizeof msg)) return fail(rc, "mask_compact: %s", msg);
-    if (n < 0 || n > 65535) return fail(MIGAN_ERR_INVALID, "mask_compact: %d masks (0 to 65535 per call)", n);
-    if (!attempts || !holes || (n && !out)) return fail(MIGAN_ERR_INVALID, "mask_compact: null argument");
-    CUDA_TRY((cudaError_t)migan::launch_mask_compact(attempts, holes, n_attempts, s, n, out, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int migan_demo_resized_size(int w, int h, int max_size, int* out_w, int* out_h) {
-    if (!out_w || !out_h) return fail(MIGAN_ERR_INVALID, "demo_resized_size: null argument");
-    if (w < 1 || h < 1 || max_size < 1) return fail(MIGAN_ERR_INVALID, "demo_resized_size: bad arguments (%d x %d, max size %d)", w, h, max_size);
-    return migan::demo_resized_size(w, h, max_size, out_w, out_h);
-}
-
-static int check_demo_batch(const char* who, const migan_demo_request* reqs, int n, int res) {
-    char msg[256];
-    if (int rc = migan::check_demo_batch(reqs, n, res, msg, sizeof msg)) return fail(rc, "%s: %s", who, msg);
-    return MIGAN_OK;
-}
-
-size_t b200_demo_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
-    if (check_demo_batch("demo_scratch_bytes", reqs, n, res)) return 0;
-    return migan::demo_scratch_bytes(reqs, n, res);
-}
-
-int b200_demo_preprocess(const migan_demo_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes, void* stream) {
-    if (int rc = check_demo_batch("demo_preprocess", reqs, n, res)) return rc;
-    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "demo_preprocess: null argument");
-    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_demo_preprocess(reqs, n, res, x, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_demo_postprocess(const float* y, const migan_demo_request* reqs, int n, int res, void* scratch, size_t scratch_bytes,
-                          void* stream) {
-    if (int rc = check_demo_batch("demo_postprocess", reqs, n, res)) return rc;
-    if (!y || !scratch) return fail(MIGAN_ERR_INVALID, "demo_postprocess: null argument");
-    const size_t need = migan::demo_scratch_bytes(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "demo_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_demo_postprocess(y, reqs, n, res, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-size_t b200_eval_scratch_bytes(const migan_demo_request* reqs, int n, int res) {
-    char msg[256];
-    if (int rc = migan::check_eval_batch(reqs, n, res, msg, sizeof msg)) { fail(rc, "eval_scratch_bytes: %s", msg); return 0; }
-    return migan::eval_scratch_bytes(reqs, n, res);
-}
-
-int b200_eval_preprocess(const migan_demo_request* reqs, int n, int res, float* x, float* img, void* scratch,
-                         size_t scratch_bytes, void* stream) {
-    char msg[256];
-    if (int rc = migan::check_eval_batch(reqs, n, res, msg, sizeof msg)) return fail(rc, "eval_preprocess: %s", msg);
-    if (!x || !img || !scratch) return fail(MIGAN_ERR_INVALID, "eval_preprocess: null argument");
-    const size_t need = migan::eval_scratch_bytes(reqs, n, res);
-    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "eval_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY((cudaError_t)migan::launch_eval_preprocess(reqs, n, res, x, img, scratch, static_cast<cudaStream_t>(stream)));
-    return MIGAN_OK;
-}
-
-int b200_eval_composite(const float* x, const float* y, int n, int res, float* img, float* composed, void* stream) {
-    if (!x || !y || !img || !composed) return fail(MIGAN_ERR_INVALID, "eval_composite: null argument");
-    if (n < 1 || res < 1 || res > 8192) return fail(MIGAN_ERR_INVALID, "eval_composite: %d images at resolution %d", n, res);
-    CUDA_TRY((cudaError_t)migan::launch_eval_composite(x, y, n, res, img, composed, static_cast<cudaStream_t>(stream)));
     return MIGAN_OK;
 }
 

@@ -22,11 +22,10 @@
 // functors read them from shared memory, so a pass needs no host round trip.  Item kernels (comod_kernels.cuh style): the emulation build runs the very same functors on the CPU
 // against the oracle; the hole flags use a shared-memory kernel on the GPU and the per-request HoleFlagsK there.
 #include "comod_kernels.cuh"
-#include "../../include/migan_b200.h"
+#include "abi_error.h"
 
 #ifdef MIGAN_EMULATE
 #include <cmath>
-#include <cstdio>
 #define PL_MUL(a, b) ((a) * (b))
 #define PL_ADD(a, b) ((a) + (b))
 #define PL_DIV(a, b) ((a) / (b))
@@ -35,8 +34,6 @@
 #define PL_D inline
 #define PL_GLOBAL(p) (p)
 #else
-#include <cstdio>
-#include "kernels.h"
 #define PL_MUL(a, b) __fmul_rn((a), (b))
 #define PL_ADD(a, b) __fadd_rn((a), (b))
 #define PL_DIV(a, b) __fdiv_rn((a), (b))
@@ -166,14 +163,6 @@ struct PipeBatch {
     const float* y; float* x;                  // generator output [n][3][res][res] / model input [n][4][res][res]
     float k[25];                               // feather smoothing taps
     int n, res;
-    PL_D int find(int64_t i) const {           // the request item i belongs to
-        int lo = 0, hi = n - 1;
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (start[mid] <= i) lo = mid; else hi = mid - 1;
-        }
-        return lo;
-    }
 };
 static_assert(sizeof(PipeBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
 
@@ -214,7 +203,7 @@ template <int POST>
 struct AaWeightsBatchK {
     const PipeBatch& b;
     PL_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int ow = POST ? r.wc : b.res, oh = POST ? r.hc : b.res;
@@ -234,7 +223,7 @@ struct ResizeWidthBatchK {
         return fminf(fmaxf(g, 0.f), 255.f);                                                       // .clamp(0, 255)
     }
     PL_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int ow = SRC ? r.wc : b.res, rows = SRC ? b.res : r.hc;
@@ -257,7 +246,7 @@ struct ResizeWidthBatchK {
 struct PreprocessBatchK {
     const PipeBatch& b;
     PL_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int res = b.res, hc = r.hc;
@@ -286,7 +275,7 @@ struct PreprocessBatchK {
 struct FeatherResizeBatchK {
     const PipeBatch& b;
     PL_D void operator()(int64_t i) const {
-        const int k = b.find(i);
+        const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int hc = r.hc, wc = r.wc, W = r.W;
@@ -373,9 +362,6 @@ inline void flags_extent(const uint8_t* f, int len, int& lo, int& hi) {
 }
 
 #ifdef MIGAN_EMULATE
-template <class F>
-inline int pipe_launch(const PipeBatch& b, ck_stream_t s) { return ck_launch(F{b}, b.start[b.n], s); }
-
 inline int pipe_plan(const PlanArgs& a, ck_stream_t) {
     for (int k = 0; k < a.n; ++k) {
         const uint8_t* f = a.flags + a.q[k].foff;
@@ -397,21 +383,6 @@ inline int pipe_launch_planned(const PlannedLaunch& a, int64_t, ck_stream_t s) {
     return ck_launch(F{b}, b.start[b.n], s);
 }
 #else
-// Same one-thread-per-item launch as ck_launch; __grid_constant__ lets the functors index the descriptor table in the
-// parameter space (no per-thread copy of the 2.5 KB struct).
-template <class F>
-__global__ void __launch_bounds__(256) pipe_items_kernel(const __grid_constant__ PipeBatch b, const int64_t items) {
-    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i < items) F{b}(i);
-}
-template <class F>
-inline cudaError_t pipe_launch(const PipeBatch& b, ck_stream_t s) {
-    const int64_t items = b.start[b.n];
-    if (items <= 0) return cudaSuccess;
-    pipe_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(b, items);
-    return cudaGetLastError();
-}
-
 // A planned launch: each CTA copies its phase's descriptor into shared memory, puts the stage's item prefix and the
 // launch's own arguments in, and runs a grid-stride loop over the items.  The grid comes from the whole-image bound of the
 // items, capped at PIPE_WAVES waves of resident CTAs: a small crop of a large photo costs few idle CTAs (they return
@@ -525,14 +496,7 @@ __device__ __forceinline__ uint32_t hole_bits4(uint32_t v) {   // bit b set <=> 
 
 __global__ void __launch_bounds__(HF_THREADS) hole_flags_batch_kernel(const __grid_constant__ FlagsBatch b, uint8_t* flags) {
     __shared__ uint32_t cols[HF_TILE / 32];
-    int k = 0;
-    {
-        int hi = b.n - 1;
-        while (k < hi) {
-            const int mid = (k + hi + 1) >> 1;
-            if (b.block_start[mid] <= (int)blockIdx.x) k = mid; else hi = mid - 1;
-        }
-    }
+    const int k = find_request(b.block_start, b.n, (int)blockIdx.x);
     const int blk = (int)blockIdx.x - b.block_start[k];
     const int H = b.H[k], W = b.W[k];
     const int tile = blk % b.tiles[k], band = blk / b.tiles[k];
@@ -614,12 +578,6 @@ comod::PipeBatch plan_batch(const migan_pipe_request* q, int n, int res, bool po
         p += align256((size_t)3 * (post ? (size_t)res * r.wc : (size_t)r.hc * res) * sizeof(float));
     }
     return b;
-}
-
-// start[] of the stage's launch: the requests' items summed in request order.
-void set_items(comod::PipeBatch& b, int stage) {
-    b.start[0] = 0;
-    for (int k = 0; k < b.n; ++k) b.start[k + 1] = b.start[k] + comod::stage_items(stage, b.r[k], b.res);
 }
 
 migan_pipe_request one_request(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box) {
@@ -716,23 +674,17 @@ size_t pipeline_batch_scratch_bytes(const migan_pipe_request* q, int n, int res)
     return pre > post ? pre : post;
 }
 
-int check_pipe_batch(const migan_pipe_request* q, int n, int res, bool boxes, char* msg, size_t len) {
-    if (!q) { snprintf(msg, len, "null request table"); return MIGAN_ERR_INVALID; }
-    if (n < 1 || n > MIGAN_PIPE_MAX_BATCH) {
-        snprintf(msg, len, "batch of %d requests (1 to %d per call)", n, MIGAN_PIPE_MAX_BATCH);
-        return MIGAN_ERR_INVALID;
-    }
-    if (res < 1) { snprintf(msg, len, "bad resolution %d", res); return MIGAN_ERR_INVALID; }
+int check_pipe_batch(const char* who, const migan_pipe_request* q, int n, int res, bool boxes) {
+    if (int rc = check_batch_size(who, q, n)) return rc;
+    if (res < 1) return fail(MIGAN_ERR_INVALID, "%s: bad resolution %d", who, res);
     for (int k = 0; k < n; ++k) {
         const migan_pipe_request& r = q[k];
-        if (!r.image || !r.mask) { snprintf(msg, len, "request %d: null image or mask", k); return MIGAN_ERR_INVALID; }
-        if (r.H < 3 || r.W < 3) { snprintf(msg, len, "request %d: image of %d x %d, need at least 3 x 3", k, r.H, r.W); return MIGAN_ERR_INVALID; }
+        if (!r.image || !r.mask) return fail(MIGAN_ERR_INVALID, "%s: request %d: null image or mask", who, k);
+        if (r.H < 3 || r.W < 3) return fail(MIGAN_ERR_INVALID, "%s: request %d: image of %d x %d, need at least 3 x 3", who, k, r.H, r.W);
         const int* b = r.box;
-        if (boxes && (b[0] < 0 || b[1] > r.W || b[2] < 0 || b[3] > r.H || b[1] - b[0] < 3 || b[3] - b[2] < 3)) {
-            snprintf(msg, len, "request %d: crop window x[%d,%d) y[%d,%d) must lie inside the %d x %d image and be at least 3 x 3",
-                     k, b[0], b[1], b[2], b[3], r.H, r.W);
-            return MIGAN_ERR_INVALID;
-        }
+        if (boxes && (b[0] < 0 || b[1] > r.W || b[2] < 0 || b[3] > r.H || b[1] - b[0] < 3 || b[3] - b[2] < 3))
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: crop window x[%d,%d) y[%d,%d) must lie inside the %d x %d image and be at least 3 x 3",
+                        who, k, b[0], b[1], b[2], b[3], r.H, r.W);
     }
     return MIGAN_OK;
 }
@@ -785,12 +737,12 @@ int launch_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res
     comod::PipeBatch b = plan_batch(q, n, res, false, scratch);
     b.x = x;
     int e;
-    set_items(b, comod::ST_AA_PRE);
-    if ((e = (int)comod::pipe_launch<comod::AaWeightsBatchK<0>>(b, s))) return e;
-    set_items(b, comod::ST_WIDTH_PRE);
-    if ((e = (int)comod::pipe_launch<comod::ResizeWidthBatchK<0>>(b, s))) return e;
-    set_items(b, comod::ST_PRE);
-    return (int)comod::pipe_launch<comod::PreprocessBatchK>(b, s);
+    comod::set_items(b, comod::ST_AA_PRE, comod::stage_items);
+    if ((e = (int)comod::batch_launch<comod::AaWeightsBatchK<0>>(b, s))) return e;
+    comod::set_items(b, comod::ST_WIDTH_PRE, comod::stage_items);
+    if ((e = (int)comod::batch_launch<comod::ResizeWidthBatchK<0>>(b, s))) return e;
+    comod::set_items(b, comod::ST_PRE, comod::stage_items);
+    return (int)comod::batch_launch<comod::PreprocessBatchK>(b, s);
 }
 
 // Three launches for the whole batch: both tables of every request, the width pass, the height pass fused into the blend.
@@ -800,18 +752,18 @@ int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* 
     b.y = y;
     for (int i = 0; i < 25; ++i) b.k[i] = k25_host[i];
     int e;
-    set_items(b, comod::ST_AA_POST);
-    if ((e = (int)comod::pipe_launch<comod::AaWeightsBatchK<1>>(b, s))) return e;
-    set_items(b, comod::ST_WIDTH_POST);
-    if ((e = (int)comod::pipe_launch<comod::ResizeWidthBatchK<1>>(b, s))) return e;
-    set_items(b, comod::ST_FEATHER);
-    return (int)comod::pipe_launch<comod::FeatherResizeBatchK>(b, s);
+    comod::set_items(b, comod::ST_AA_POST, comod::stage_items);
+    if ((e = (int)comod::batch_launch<comod::AaWeightsBatchK<1>>(b, s))) return e;
+    comod::set_items(b, comod::ST_WIDTH_POST, comod::stage_items);
+    if ((e = (int)comod::batch_launch<comod::ResizeWidthBatchK<1>>(b, s))) return e;
+    comod::set_items(b, comod::ST_FEATHER, comod::stage_items);
+    return (int)comod::batch_launch<comod::FeatherResizeBatchK>(b, s);
 }
 
 // ---- device-planned batches ----
-int check_pipe_planned(const migan_pipe_request* q, int n, int res, char* msg, size_t len) {
-    if (int rc = check_pipe_batch(q, n, res, false, msg, len)) return rc;
-    if (res < 3) { snprintf(msg, len, "resolution %d: a planned crop window is at least the resolution and must be 3 x 3", res); return MIGAN_ERR_INVALID; }
+int check_pipe_planned(const char* who, const migan_pipe_request* q, int n, int res) {
+    if (int rc = check_pipe_batch(who, q, n, res, false)) return rc;
+    if (res < 3) return fail(MIGAN_ERR_INVALID, "%s: resolution %d: a planned crop window is at least the resolution and must be 3 x 3", who, res);
     return MIGAN_OK;
 }
 
@@ -876,81 +828,138 @@ int launch_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* m
 
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (argument checks, error strings) live in migan_abi.cu
-extern "C" size_t b200_pipeline_scratch_bytes(int H, int W, int res) { return migan::pipeline_scratch_bytes(H, W, res); }
-extern "C" int b200_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, void* s) {
-    return migan::launch_resize_nearest_u8(in, H, W, out, oh, ow, s);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+static int check_box(const char* who, int H, int W, const int* box) {
+    if (!box) return fail(MIGAN_ERR_INVALID, "%s: null crop window", who);
+    if (box[0] < 0 || box[1] > W || box[2] < 0 || box[3] > H || box[1] - box[0] < 3 || box[3] - box[2] < 3)
+        return fail(MIGAN_ERR_INVALID, "%s: crop window x[%d,%d) y[%d,%d) must lie inside the %d x %d image and be at least 3 x 3",
+                    who, box[0], box[1], box[2], box[3], H, W);
+    return MIGAN_OK;
 }
-extern "C" int b200_hole_flags(const uint8_t* mask, int H, int W, uint8_t* flags, void* s) { return migan::launch_hole_flags(mask, H, W, flags, s); }
-extern "C" int migan_crop_box(const uint8_t* flags, int H, int W, int res, int padding, int* box) {
-    migan::crop_box_from_flags(flags, H, W, res, padding, box);
-    return 0;
+
+extern "C" {
+
+size_t b200_pipeline_scratch_bytes(int H, int W, int res) {
+    if (H < 1 || W < 1 || res < 1) return 0;
+    return migan::pipeline_scratch_bytes(H, W, res);
 }
-extern "C" int b200_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
-                                        void* scratch, size_t, void* s) {
-    return migan::launch_pipeline_preprocess(image, mask, H, W, box, res, x, scratch, s);
+
+int b200_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, void* stream) {
+    if (!in || !out) return fail(MIGAN_ERR_INVALID, "resize_nearest_u8: null argument");
+    if (H < 1 || W < 1 || oh < 1 || ow < 1) return fail(MIGAN_ERR_INVALID, "resize_nearest_u8: bad size %d x %d -> %d x %d", H, W, oh, ow);
+    CUDA_TRY(migan::launch_resize_nearest_u8(in, H, W, out, oh, ow, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
-                                         const float* k25, void* scratch, size_t, void* s) {
-    return migan::launch_pipeline_postprocess(y, image, mask, H, W, box, res, k25, scratch, s);
+
+int b200_hole_flags(const uint8_t* mask, int H, int W, uint8_t* flags, void* stream) {
+    if (!mask || !flags) return fail(MIGAN_ERR_INVALID, "hole_flags: null argument");
+    if (H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "hole_flags: bad size %d x %d", H, W);
+    CUDA_TRY(migan::launch_hole_flags(mask, H, W, flags, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-// The batched entry points with the product's argument checks (return codes only: no error string here).
-extern "C" int b200_hole_flags_batch(const migan_pipe_request* q, int n, uint8_t* flags, void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_batch(q, n, 1, false, msg, sizeof msg)) return rc;
-    if (!flags) return MIGAN_ERR_INVALID;
-    return migan::launch_hole_flags_batch(q, n, flags, s);
+
+int migan_crop_box(const uint8_t* flags_host, int H, int W, int res, int padding, int* box4) {
+    if (!flags_host || !box4) return fail(MIGAN_ERR_INVALID, "crop_box: null argument");
+    if (H < 1 || W < 1 || res < 1 || padding < 0) return fail(MIGAN_ERR_INVALID, "crop_box: bad arguments (%d x %d, resolution %d, padding %d)", H, W, res, padding);
+    migan::crop_box_from_flags(flags_host, H, W, res, padding, box4);
+    return MIGAN_OK;
 }
-extern "C" size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* q, int n, int res) {
-    char msg[256];
-    if (migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return 0;
-    return migan::pipeline_batch_scratch_bytes(q, n, res);
+
+int b200_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
+                             void* scratch, size_t scratch_bytes, void* stream) {
+    if (!image || !mask || !x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess: null argument");
+    if (int rc = check_box("pipeline_preprocess", H, W, box)) return rc;
+    if (res < 1) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess: bad resolution %d", res);
+    if (scratch_bytes < migan::pipeline_scratch_bytes(H, W, res))
+        return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess: scratch of %zu bytes, need %zu", scratch_bytes, migan::pipeline_scratch_bytes(H, W, res));
+    CUDA_TRY(migan::launch_pipeline_preprocess(image, mask, H, W, box, res, x, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res, float* x, void* scratch, size_t scratch_bytes,
-                                              void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return rc;
-    if (!x || !scratch) return MIGAN_ERR_INVALID;
-    if (scratch_bytes < migan::pipeline_batch_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_pipeline_preprocess_batch(q, n, res, x, scratch, s);
+
+int b200_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
+                              const float* k25, void* scratch, size_t scratch_bytes, void* stream) {
+    if (!y || !image || !mask || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess: null argument");
+    if (int rc = check_box("pipeline_postprocess", H, W, box)) return rc;
+    if (res < 1) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess: bad resolution %d", res);
+    if (scratch_bytes < migan::pipeline_scratch_bytes(H, W, res))
+        return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess: scratch of %zu bytes, need %zu", scratch_bytes, migan::pipeline_scratch_bytes(H, W, res));
+    CUDA_TRY(migan::launch_pipeline_postprocess(y, image, mask, H, W, box, res, k25, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* q, int n, int res, const float* k25,
-                                               void* scratch, size_t scratch_bytes, void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_batch(q, n, res, true, msg, sizeof msg)) return rc;
-    if (!y || !k25 || !scratch) return MIGAN_ERR_INVALID;
-    if (scratch_bytes < migan::pipeline_batch_scratch_bytes(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_pipeline_postprocess_batch(y, q, n, res, k25, scratch, s);
+
+int b200_hole_flags_batch(const migan_pipe_request* reqs, int n, uint8_t* flags, void* stream) {
+    if (int rc = migan::check_pipe_batch("hole_flags_batch", reqs, n, 1, false)) return rc;
+    if (!flags) return fail(MIGAN_ERR_INVALID, "hole_flags_batch: null flags");
+    CUDA_TRY(migan::launch_hole_flags_batch(reqs, n, flags, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" size_t b200_pipeline_batch_scratch_bound(const migan_pipe_request* q, int n, int res) {
-    char msg[256];
-    if (migan::check_pipe_planned(q, n, res, msg, sizeof msg)) return 0;
-    return migan::pipeline_batch_scratch_bound(q, n, res);
+
+size_t b200_pipeline_batch_scratch_bytes(const migan_pipe_request* reqs, int n, int res) {
+    if (migan::check_pipe_batch("pipeline_batch_scratch_bytes", reqs, n, res, true)) return 0;
+    return migan::pipeline_batch_scratch_bytes(reqs, n, res);
 }
-extern "C" int b200_pipeline_plan_batch(const migan_pipe_request* q, int n, int res, int padding, const uint8_t* flags, int* boxes,
-                                        void* scratch, size_t scratch_bytes, void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_planned(q, n, res, msg, sizeof msg)) return rc;
-    if (padding < 0 || !flags || !boxes || !scratch) return MIGAN_ERR_INVALID;
-    if (scratch_bytes < migan::pipeline_batch_scratch_bound(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_pipeline_plan_batch(q, n, res, padding, flags, boxes, scratch, s);
+
+int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
+                                   void* stream) {
+    if (int rc = migan::check_pipe_batch("pipeline_preprocess_batch", reqs, n, res, true)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_preprocess_batch(reqs, n, res, x, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_pipeline_preprocess_planned(const migan_pipe_request* q, int n, int res, float* x, void* scratch,
-                                                size_t scratch_bytes, void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_planned(q, n, res, msg, sizeof msg)) return rc;
-    if (!x || !scratch) return MIGAN_ERR_INVALID;
-    if (scratch_bytes < migan::pipeline_batch_scratch_bound(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_pipeline_preprocess_planned(q, n, res, x, scratch, s);
+
+int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
+                                    size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_pipe_batch("pipeline_postprocess_batch", reqs, n, res, true)) return rc;
+    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_postprocess_batch(y, reqs, n, res, k25, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* q, int n, int res, const float* k25,
-                                                 void* scratch, size_t scratch_bytes, void* s) {
-    char msg[256];
-    if (int rc = migan::check_pipe_planned(q, n, res, msg, sizeof msg)) return rc;
-    if (!y || !k25 || !scratch) return MIGAN_ERR_INVALID;
-    if (scratch_bytes < migan::pipeline_batch_scratch_bound(q, n, res)) return MIGAN_ERR_WORKSPACE;
-    return migan::launch_pipeline_postprocess_planned(y, q, n, res, k25, scratch, s);
+
+size_t b200_pipeline_batch_scratch_bound(const migan_pipe_request* reqs, int n, int res) {
+    if (migan::check_pipe_planned("pipeline_batch_scratch_bound", reqs, n, res)) return 0;
+    return migan::pipeline_batch_scratch_bound(reqs, n, res);
 }
+
+int b200_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int padding, const uint8_t* flags, int* boxes,
+                             void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_pipe_planned("pipeline_plan_batch", reqs, n, res)) return rc;
+    if (padding < 0) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: padding %d", padding);
+    if (!flags || !boxes || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_plan_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_plan_batch(reqs, n, res, padding, flags, boxes, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs, int n, int res, float* x, void* scratch, size_t scratch_bytes,
+                                     void* stream) {
+    if (int rc = migan::check_pipe_planned("pipeline_preprocess_planned", reqs, n, res)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_planned: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_preprocess_planned(reqs, n, res, x, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* reqs, int n, int res, const float* k25, void* scratch,
+                                      size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_pipe_planned("pipeline_postprocess_planned", reqs, n, res)) return rc;
+    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_planned: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_postprocess_planned(y, reqs, n, res, k25, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+}  // extern "C"
+
+#ifdef MIGAN_EMULATE
 // Test hook of the emulation build: request_bounds and request_exact of one crop window, for checking that the regions the
 // planned calls carve from the image size hold every window the image allows.
 extern "C" void migan_emul_planned_regions(int H, int W, int res, const int* box, size_t* bound6, size_t* exact6) {

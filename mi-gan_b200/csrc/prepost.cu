@@ -6,6 +6,7 @@
 // Item kernels (one pixel per thread) in the comod_kernels.cuh style, so the emulation build checks them on the CPU.
 // Every product of the reference is rounded separately (no FMA contraction) to stay bit-exact with torch.
 #include "prepost.cuh"
+#include "abi_error.h"
 
 #ifndef MIGAN_EMULATE
 #include "kernels.h"
@@ -114,22 +115,41 @@ int launch_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mas
 }
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrappers (with error strings) live in migan_abi.cu
-extern "C" int b200_feather_composite(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W,
-                                      const float* k25, void* s) {
-    if (!k25) return 1;
-    return migan::launch_feather_composite(y, img, mask, out, n, H, W, k25, s);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+int b200_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, void* stream) {
+    if (!img || !mask || !x || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8: bad arguments");
+    CUDA_TRY(migan::launch_preprocess_u8(img, mask, x, n, r, r, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_preprocess_u8(const uint8_t* img, const uint8_t* mask, float* x, int n, int r, void* s) {
-    return migan::launch_preprocess_u8(img, mask, x, n, r, r, s);
+
+int b200_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, void* stream) {
+    if (!y || !img || !mask || !out || n <= 0 || r <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8: bad arguments");
+    CUDA_TRY(migan::launch_postprocess_u8(y, img, mask, out, n, r, r, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_postprocess_u8(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int r, void* s) {
-    return migan::launch_postprocess_u8(y, img, mask, out, n, r, r, s);
+
+int b200_preprocess_u8_hw(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, void* stream) {
+    if (!img || !mask || !x || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "preprocess_u8_hw: bad arguments");
+    CUDA_TRY(migan::launch_preprocess_u8(img, mask, x, n, H, W, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_preprocess_u8_hw(const uint8_t* img, const uint8_t* mask, float* x, int n, int H, int W, void* s) {
-    return migan::launch_preprocess_u8(img, mask, x, n, H, W, s);
+
+int b200_postprocess_u8_hw(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, void* stream) {
+    if (!y || !img || !mask || !out || n <= 0 || H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "postprocess_u8_hw: bad arguments");
+    CUDA_TRY(migan::launch_postprocess_u8(y, img, mask, out, n, H, W, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-extern "C" int b200_postprocess_u8_hw(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W, void* s) {
-    return migan::launch_postprocess_u8(y, img, mask, out, n, H, W, s);
+
+int b200_feather_composite(const float* y, const uint8_t* img, const uint8_t* mask, uint8_t* out, int n, int H, int W,
+                           const float* k25, void* stream) {
+    if (!y || !img || !mask || !out || !k25) return fail(MIGAN_ERR_INVALID, "feather_composite: null argument");
+    if (n <= 0 || H < 3 || W < 3) return fail(MIGAN_ERR_INVALID, "feather_composite: need n >= 1 and H, W >= 3 (reflect padding of 2), got %d x %d x %d", n, H, W);
+    CUDA_TRY(migan::launch_feather_composite(y, img, mask, out, n, H, W, k25, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+}  // extern "C"

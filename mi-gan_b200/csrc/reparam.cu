@@ -8,6 +8,7 @@
 // so the result agrees with the reference to a few ulp, not bit for bit (tests: relative error < 1e-6).
 // Item kernel (comod_kernels.cuh style): the emulation build runs the same functor on the CPU.
 #include "comod_kernels.cuh"
+#include "abi_error.h"
 
 #ifdef MIGAN_EMULATE
 #include <cmath>
@@ -17,7 +18,6 @@
 #define RP_SQRT(a) sqrtf(a)
 #define RP_D inline
 #else
-#include "kernels.h"
 #define RP_ADD(a, b) __fadd_rn((a), (b))
 #define RP_MUL(a, b) __fmul_rn((a), (b))
 #define RP_DIV(a, b) __fdiv_rn((a), (b))
@@ -56,9 +56,19 @@ int launch_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fa
 }
 }  // namespace migan
 
-#ifdef MIGAN_EMULATE   // the product's extern "C" wrapper (argument checks, error strings) lives in migan_abi.cu
-extern "C" int b200_reparam_filter(const float* const* w, int k, int cout, int64_t fan, float* out, void* s) {
-    if (k < 1 || k > comod::kMaxReparam) return 1;
-    return migan::launch_reparam_filter(w, k, cout, fan, out, s);
+// ---- C ABI (include/migan_b200.h) ----
+using migan::fail;
+
+extern "C" {
+
+int b200_reparam_filter(const float* const* w_dev, int k, int cout, int64_t fan, float* out, void* stream) {
+    if (!w_dev || !out) return fail(MIGAN_ERR_INVALID, "reparam_filter: null argument");
+    if (k < 1 || k > 16) return fail(MIGAN_ERR_INVALID, "reparam_filter: %d tensors (1 .. 16 supported)", k);
+    if (cout < 1 || fan < 1) return fail(MIGAN_ERR_INVALID, "reparam_filter: bad shape %d x %lld", cout, (long long)fan);
+    for (int j = 0; j < k; ++j)
+        if (!w_dev[j]) return fail(MIGAN_ERR_INVALID, "reparam_filter: tensor %d is null", j);
+    CUDA_TRY(migan::launch_reparam_filter(w_dev, k, cout, fan, out, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
 }
-#endif
+
+}  // extern "C"

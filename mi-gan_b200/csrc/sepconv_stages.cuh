@@ -3,7 +3,7 @@
 // Every function here is written against plain pointers into one pipeline stage of shared memory and takes the
 // worker index `tg` (0..127: the thread's index inside its 128-thread prologue group) as an argument, with no
 // barrier, shuffle or special register inside.  That is deliberate: the same source compiles as plain C++
-// (-DMIGAN_EMULATE, tests/emul/build_stages.py) where a test loops tg = 0..127 over a host buffer filled the way
+// (-DMIGAN_EMULATE, tests/emul/build_emul.py) where a test loops tg = 0..127 over a host buffer filled the way
 // the TMA unit fills the stage (box layout, out-of-bounds zero fill), so the halo / polyphase / swizzle index math is
 // checked against the oracle on a machine without a GPU (tests/test_stages_emul.py).  The emulation build is TEST
 // INFRASTRUCTURE; the product library is compiled without the macro.

@@ -19,7 +19,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 from migan_b200 import _abi  # noqa: E402
 from oracle import demo_oracle as O  # noqa: E402
-import build_demo  # noqa: E402
+import build_emul  # noqa: E402
 import make_golden_demo as MG  # noqa: E402
 
 NAMES = ("migan_demo_resized_size", "b200_demo_scratch_bytes", "b200_demo_preprocess", "b200_demo_postprocess")
@@ -28,7 +28,7 @@ SYMBOLS = [s for s in _abi.SYMBOLS if s[0] in NAMES]
 
 @pytest.fixture(scope="module")
 def emul():
-    return _abi.bind(ctypes.CDLL(build_demo.build()), SYMBOLS)
+    return _abi.bind(ctypes.CDLL(build_emul.build()), SYMBOLS)
 
 
 def _ptr(a):

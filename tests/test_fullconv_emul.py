@@ -25,7 +25,6 @@ from oracle import prepost_oracle as P
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "emul"))
 import build_emul  # noqa: E402
-import build_stages_hw  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden", "fullconv.npz")
 SQRT2 = np.float32(np.sqrt(2))
@@ -176,7 +175,7 @@ def test_prepost_u8_hw_at_square_equals_r_entry_points(prepost):
 # ---- UP / STEM pre-stages on an H x W image, tiles at the right / bottom edge ---------------------------------------------
 @pytest.fixture(scope="module")
 def stages():
-    L = ctypes.CDLL(build_stages_hw.build())
+    L = ctypes.CDLL(build_emul.build_harness("stages_hw_emul.cpp"))
     vp, ci = ctypes.c_void_p, ctypes.c_int
     L.emul_prestage_up_hw.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci]
     L.emul_prestage_stem_hw.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci]

@@ -20,7 +20,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "emul"))
 from migan_b200 import _abi  # noqa: E402
 from migan_b200.fullres import Chunk, plan_passes  # noqa: E402
 from oracle import fullres_oracle as F  # noqa: E402
-import build_fullres  # noqa: E402
+import build_emul  # noqa: E402
 
 NAMES = ("b200_fullres_preprocess", "b200_fullres_postprocess")
 SYMBOLS = [s for s in _abi.SYMBOLS if s[0] in NAMES]
@@ -34,7 +34,7 @@ CASES = [(256, 256, 256, 1, False), (256, 320, 448, 3, True), (256, 100, 700, 4,
 
 @pytest.fixture(scope="module")
 def emul():
-    return _abi.bind(ctypes.CDLL(build_fullres.build()), SYMBOLS)
+    return _abi.bind(ctypes.CDLL(build_emul.build()), SYMBOLS)
 
 
 def _request(rng, H, W, C):

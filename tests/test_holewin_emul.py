@@ -1,6 +1,6 @@
 """CPU checks of the hole-window request path (mi-gan_b200/csrc/holewin.cu, the window kernels of fullres.cu).
 
-- the window planner of the product library (migan_hole_windows, host code) equals oracle/holewin_oracle.py on a few
+- the window planner (migan_hole_windows, host code) equals oracle/holewin_oracle.py on a few
   hundred seeded random cell grids and on named cases, and every result keeps the invariants: windows disjoint and inside
   the photo, every hole cell's pixels covered, every side a valid forward_fc size or the photo's side, the count within
   migan_hole_windows_max;
@@ -23,18 +23,19 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "emul"))
 from migan_b200 import _abi  # noqa: E402
 from oracle import fullres_oracle as F  # noqa: E402
 from oracle import holewin_oracle as HW  # noqa: E402
-import build_holewin  # noqa: E402
+import build_emul  # noqa: E402
 
-NAMES = ("b200_hole_cells_bytes", "b200_hole_cells", "b200_window_preprocess", "b200_window_postprocess")
+NAMES = ("b200_hole_cells_bytes", "b200_hole_cells", "b200_window_preprocess", "b200_window_postprocess",
+         "migan_hole_windows", "migan_hole_windows_max", "migan_last_error")
 SYMBOLS = [s for s in _abi.SYMBOLS if s[0] in NAMES]
 
 
 @pytest.fixture(scope="module")
 def emul():
-    return _abi.bind(ctypes.CDLL(build_holewin.build()), SYMBOLS)
+    return _abi.bind(ctypes.CDLL(build_emul.build()), SYMBOLS)
 
 
-# ---- the window planner (product library, host code) ---------------------------------------------------------------
+# ---- the window planner (host code) ---------------------------------------------------------------
 def plan(lib, cells, H, W, R, margin=1):
     mx = ctypes.c_int()
     _abi.check(lib.migan_hole_windows_max(H, W, R, ctypes.byref(mx)))
@@ -67,80 +68,80 @@ def _grid(H, W, R):
 
 
 @pytest.mark.parametrize("seed", range(300))
-def test_planner_random_grids(lib, seed):
+def test_planner_random_grids(emul, seed):
     rng = np.random.default_rng(seed)
     R = int(rng.choice([16, 64, 256]))
     H, W = int(rng.integers(1, 12 * R)), int(rng.integers(1, 12 * R))
     margin = int(rng.integers(0, 3))
     g = _grid(H, W, R)
     g[...] = rng.random(g.shape) < float(rng.choice([0.002, 0.02, 0.1, 0.5]))
-    wins = plan(lib, g, H, W, R, margin)
+    wins = plan(emul, g, H, W, R, margin)
     assert wins == HW.windows(g, H, W, R, margin), (R, H, W, margin)
     check_invariants(wins, g, H, W, R)
 
 
-def test_planner_empty_mask_gives_no_windows(lib):
-    assert plan(lib, _grid(3024, 4032, 512), 3024, 4032, 512) == []
+def test_planner_empty_mask_gives_no_windows(emul):
+    assert plan(emul, _grid(3024, 4032, 512), 3024, 4032, 512) == []
 
 
-def test_planner_all_hole_gives_the_whole_photo(lib):
+def test_planner_all_hole_gives_the_whole_photo(emul):
     for R, H, W in [(512, 3024, 4032), (256, 1000, 1001), (64, 30, 70)]:
         g = _grid(H, W, R) + 1
-        assert plan(lib, g, H, W, R) == [(0, 0, H, W)]
+        assert plan(emul, g, H, W, R) == [(0, 0, H, W)]
 
 
-def test_planner_distant_and_close_holes(lib):
+def test_planner_distant_and_close_holes(emul):
     R, H, W = 512, 2160, 3840
     g = _grid(H, W, R)
     g[2, 2] = g[14, 26] = 1                              # opposite ends: two windows of R x R around the cells
-    wins = plan(lib, g, H, W, R)
+    wins = plan(emul, g, H, W, R)
     assert wins == [(64, 64, 512, 512), (1600, 3136, 512, 512)]
     check_invariants(wins, g, H, W, R)
     g[...] = 0
     g[5, 5] = g[5, 9] = 1                                # windows [448, 960) and [960, 1472) only touch: two windows
-    assert plan(lib, g, H, W, R) == [(448, 448, 512, 512), (448, 960, 512, 512)]
+    assert plan(emul, g, H, W, R) == [(448, 448, 512, 512), (448, 960, 512, 512)]
     g[5, 9], g[5, 8] = 0, 1                              # [448, 960) and [832, 1344) overlap: one window over cells 5..8
-    wins = plan(lib, g, H, W, R)
+    wins = plan(emul, g, H, W, R)
     assert wins == HW.windows(g, H, W, R) == [(448, 512, 512, 768)]
     check_invariants(wins, g, H, W, R)
 
 
 @pytest.mark.parametrize("where", ["tl", "tr", "bl", "br", "top", "bottom", "left", "right"])
-def test_planner_corners_and_edges(lib, where):
+def test_planner_corners_and_edges(emul, where):
     R, H, W = 256, 1000, 1500                            # sides not multiples of q = 64: partial last cells
     g = _grid(H, W, R)
     gh, gw = g.shape
     pos = {"tl": (0, 0), "tr": (0, gw - 1), "bl": (gh - 1, 0), "br": (gh - 1, gw - 1), "top": (0, gw // 2),
            "bottom": (gh - 1, gw // 2), "left": (gh // 2, 0), "right": (gh // 2, gw - 1)}[where]
     g[pos] = 1
-    wins = plan(lib, g, H, W, R)
+    wins = plan(emul, g, H, W, R)
     assert wins == HW.windows(g, H, W, R) and len(wins) == 1
     check_invariants(wins, g, H, W, R)
 
 
-def test_planner_photo_smaller_than_R_and_margin_0(lib):
+def test_planner_photo_smaller_than_R_and_margin_0(emul):
     R = 512
     g = _grid(300, 400, R)
     g[1, 1] = 1
-    assert plan(lib, g, 300, 400, R) == [(0, 0, 300, 400)]
+    assert plan(emul, g, 300, 400, R) == [(0, 0, 300, 400)]
     R, H, W = 256, 777, 1333                             # q = 64
     g = _grid(H, W, R)
     g[5, 10:13] = 1                                      # three cells: 5 with the margin (320 wide), 3 without (256)
-    assert plan(lib, g, H, W, R, 1) == HW.windows(g, H, W, R, 1) == [(224, 576, 256, 320)]
-    wins = plan(lib, g, H, W, R, 0)
+    assert plan(emul, g, H, W, R, 1) == HW.windows(g, H, W, R, 1) == [(224, 576, 256, 320)]
+    wins = plan(emul, g, H, W, R, 0)
     assert wins == HW.windows(g, H, W, R, 0) == [(224, 608, 256, 256)]
     check_invariants(wins, g, H, W, R)
 
 
-def test_planner_refusals(lib):
+def test_planner_refusals(emul):
     mx = ctypes.c_int()
-    assert lib.migan_hole_windows_max(0, 5, 256, ctypes.byref(mx)) == _abi.ERR_INVALID
-    assert lib.migan_hole_windows_max(5, 5, 100, ctypes.byref(mx)) == _abi.ERR_INVALID
+    assert emul.migan_hole_windows_max(0, 5, 256, ctypes.byref(mx)) == _abi.ERR_INVALID
+    assert emul.migan_hole_windows_max(5, 5, 100, ctypes.byref(mx)) == _abi.ERR_INVALID
     g = np.ones((1, 1), np.uint8)
     buf, cnt = (ctypes.c_int * 4)(), ctypes.c_int()
-    assert lib.migan_hole_windows(g.ctypes.data, 5, 5, 256, -1, buf, 1, ctypes.byref(cnt)) == _abi.ERR_INVALID
-    assert lib.migan_hole_windows(g.ctypes.data, 5, 5, 256, 1, buf, 0, ctypes.byref(cnt)) == _abi.ERR_INVALID
-    assert "room" in lib.migan_last_error().decode()
+    assert emul.migan_hole_windows(g.ctypes.data, 5, 5, 256, -1, buf, 1, ctypes.byref(cnt)) == _abi.ERR_INVALID
+    assert emul.migan_hole_windows(g.ctypes.data, 5, 5, 256, 1, buf, 0, ctypes.byref(cnt)) == _abi.ERR_INVALID
+    assert "room" in emul.migan_last_error().decode()
 
 
 # ---- the cells kernel (emulation build) ----------------------------------------------------------------------------

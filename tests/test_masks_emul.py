@@ -22,7 +22,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "emul"))
 
 from migan_b200 import _abi  # noqa: E402
 from oracle import masks_oracle as M  # noqa: E402
-import build_masks  # noqa: E402
+import build_emul  # noqa: E402
 
 NAMES = ("migan_np_seed", "migan_mask_plan", "b200_mask_raster", "b200_mask_compact")
 SYMBOLS = [s for s in _abi.SYMBOLS if s[0] in NAMES]
@@ -32,7 +32,7 @@ LISTS = [(0, 32), (0, 64), (0, 256), (0, 512), (7, 128)]
 
 @pytest.fixture(scope="module")
 def emul():
-    return _abi.bind(ctypes.CDLL(build_masks.build()), SYMBOLS)
+    return _abi.bind(ctypes.CDLL(build_emul.build()), SYMBOLS)
 
 
 def seeded(lib, seed):

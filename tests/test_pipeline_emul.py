@@ -141,9 +141,9 @@ def test_kernels_match_oracle_on_random_requests(emul):
         assert np.array_equal(final, want.numpy()), (t, int((final != want.numpy()).sum()))
 
 
-def test_product_crop_box_is_host_arithmetic():
-    """`migan_crop_box` of the PRODUCT library needs no GPU: same 300 pinned masks as the oracle."""
-    lib = _abi.load()
+def test_product_crop_box_is_host_arithmetic(emul):
+    """The product's `migan_crop_box` is host code: same 300 pinned masks as the oracle."""
+    lib = emul
     table = GOLD["bbox_cases"]
     for t, mask, pad in random_bbox_masks():
         H, W = mask.shape

@@ -1,6 +1,6 @@
 """CPU check of the shared-memory stages of the fused SeparableConv2d kernel (mi-gan_b200/csrc/sepconv_stages.cuh).
 
-The stage functions are compiled as plain C++ (tests/emul/build_stages.py) and run over host buffers filled the way the
+The stage functions are compiled as plain C++ (tests/emul/build_emul.py) and run over host buffers filled the way the
 TMA unit fills a pipeline stage (box layout, out-of-bounds zero fill).  Checked against the oracle's torch ops:
   * UP pre-stage   == lrelu_agc(Upsample2d(t) + noise) + skip on the halo'd tile, ZERO outside the image
   * STEM pre-stage == lrelu_agc(fromrgb(x) + b) on the halo'd tile, ZERO outside the image
@@ -20,14 +20,14 @@ import torch.nn.functional as F
 from oracle import migan_oracle as O
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "emul"))
-import build_stages  # noqa: E402
+import build_emul  # noqa: E402
 
 SQRT2 = np.float32(np.sqrt(2))
 
 
 @pytest.fixture(scope="module")
 def lib():
-    L = ctypes.CDLL(build_stages.build())
+    L = ctypes.CDLL(build_emul.build_harness("stages_emul.cpp"))
     vp, ci = ctypes.c_void_p, ctypes.c_int
     L.emul_prologue_chunk.argtypes = [ci, vp, vp, vp, vp, vp, ci, ci, ci]
     L.emul_prestage_up.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci]
