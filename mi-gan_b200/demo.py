@@ -23,11 +23,10 @@ from __future__ import annotations
 
 from typing import List, Sequence, Tuple, Union
 
-import numpy as np
 import torch
 
 from . import _abi
-from .generator import Generator
+from ._request_path import _PhotoPipeline, _to
 
 MASK_MAX = 512          # read_mask's first resize (demo.py:28)
 
@@ -40,31 +39,17 @@ def resized_size(w: int, h: int, max_size: int) -> Tuple[int, int]:
     return w, h
 
 
-class DemoPipeline(torch.nn.Module):
+class DemoPipeline(_PhotoPipeline):
     """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from."""
 
     def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda"):
-        super().__init__()
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("migan_b200.DemoPipeline runs on a CUDA device (there is no CPU path); got %s" % device)
-        if isinstance(model_or_state_dict, Generator):
-            if model_or_state_dict.resolution != resolution:
-                raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_or_state_dict.resolution, resolution))
-            self.model = model_or_state_dict
-        else:
-            self.model = Generator(resolution=resolution)
-            sd = model_or_state_dict if isinstance(model_or_state_dict, dict) else torch.load(model_or_state_dict, map_location="cpu")
-            self.model.load_state_dict(sd)
-        self.model = self.model.to(device).eval()
-        self.res = int(resolution)
-        self.device_ = device
-        self._pending: List["_Call"] = []
+        super().__init__(model_or_state_dict, resolution, device)
+        self.device_ = torch.device(device)
         self.last_sizes: List[Tuple[int, int]] = []       # (w', h') of every result of the last completed call(s)
         self.last_launches = 0                             # kernel launches (generator excluded) of the last pass
 
-    def __call__(self, img, mask, invert: bool = False):
-        return self.forward_batch([img], [mask], invert=invert)[0]
+    def _set_record(self, record: list) -> None:
+        self.last_sizes = record
 
     # -- one pass ---------------------------------------------------------------------------------------------------
     def _pass(self, imgs, masks, inverts, outs) -> None:
@@ -96,21 +81,12 @@ class DemoPipeline(torch.nn.Module):
         self.last_launches = 2 + (2 if down else 0) + 2
 
     # -- public calls -----------------------------------------------------------------------------------------------
-    def _check(self, i, img, mask):
-        """(photo tensor [H,W,3], mask tensor [Hm,Wm,C], (w', h')) of request i; ValueError where demo.py fails."""
-        img = torch.from_numpy(np.ascontiguousarray(img)) if isinstance(img, np.ndarray) else img
-        mask = torch.from_numpy(np.ascontiguousarray(mask)) if isinstance(mask, np.ndarray) else mask
-        if not isinstance(img, torch.Tensor) or not isinstance(mask, torch.Tensor):
-            raise TypeError("DemoPipeline: request %d: photo and mask must be numpy arrays or torch tensors" % i)
-        if img.dtype != torch.uint8 or mask.dtype != torch.uint8:
-            raise ValueError("DemoPipeline: request %d: photo and mask must be uint8" % i)
-        if img.dim() != 3 or img.shape[2] != 3 or img.shape[0] < 1 or img.shape[1] < 1:
-            raise ValueError("DemoPipeline: request %d: photo of shape %s, expected [H, W, 3]" % (i, tuple(img.shape)))
-        if mask.dim() == 2:
-            mask = mask.unsqueeze(2)
-        if mask.dim() != 3 or not 1 <= mask.shape[2] <= 4 or mask.shape[0] < 1 or mask.shape[1] < 1:
-            raise ValueError("DemoPipeline: request %d: mask of shape %s, expected [H, W] or [H, W, 1..4]" % (i, tuple(mask.shape)))
+    def _check_mask_size(self, i, img, mask) -> None:
+        """demo.py resizes the mask on its own, so it may have any size whose two resizes end at the photo's (w', h');
+        ValueError where demo.py fails."""
         H, W, Hm, Wm = int(img.shape[0]), int(img.shape[1]), int(mask.shape[0]), int(mask.shape[1])
+        if Hm < 1 or Wm < 1:
+            raise ValueError("DemoPipeline: request %d: mask of shape %s, expected [H, W] or [H, W, 1..4]" % (i, tuple(mask.shape)))
         w1, h1 = resized_size(W, H, self.res)
         wb, hb = resized_size(*resized_size(Wm, Hm, MASK_MAX), self.res)
         if min(w1, h1, wb, hb) < 1 or min(resized_size(Wm, Hm, MASK_MAX)) < 1:
@@ -119,7 +95,6 @@ class DemoPipeline(torch.nn.Module):
         if (wb, hb) != (w1, h1):
             raise ValueError("DemoPipeline: request %d: the mask resizes to %dx%d and the photo to %dx%d (w x h); demo.py "
                              "cannot compose them" % (i, wb, hb, w1, h1))
-        return img, mask, (w1, h1)
 
     @torch.no_grad()
     def forward_batch(self, imgs: Sequence, masks: Sequence, invert: Union[bool, Sequence[bool]] = False,
@@ -131,72 +106,16 @@ class DemoPipeline(torch.nn.Module):
         wait=False only enqueues the work on the current stream and returns the output tensors, which hold the results
         (and `last_sizes` is set) after `wait()`.  CPU photos must then be pinned tensors (`pin_memory()`), since they are
         copied asynchronously; pageable CPU masks are staged through pinned memory."""
-        imgs, masks = list(imgs), list(masks)
-        if len(imgs) != len(masks):
-            raise ValueError("DemoPipeline.forward_batch: %d photos and %d masks" % (len(imgs), len(masks)))
-        inverts = [bool(invert)] * len(imgs) if isinstance(invert, (bool, int)) else [bool(v) for v in invert]
-        if len(inverts) != len(imgs):
-            raise ValueError("DemoPipeline.forward_batch: %d invert flags for %d requests" % (len(inverts), len(imgs)))
-        kinds, checked = [], []
-        for i, (img, mask) in enumerate(zip(imgs, masks)):
-            kinds.append("numpy" if isinstance(img, np.ndarray) else ("cuda" if img.is_cuda else "cpu"))
-            if not wait and kinds[-1] != "cuda" and not (kinds[-1] == "cpu" and img.is_pinned() and img.is_contiguous()):
-                raise RuntimeError("DemoPipeline.forward_batch(wait=False): CPU photo %d must be a pinned contiguous tensor "
-                                   "(it is copied asynchronously); use torch.from_numpy(img).pin_memory() or wait=True" % i)
-            checked.append(self._check(i, img, mask))
-        if not imgs:
+        kinds, checked, inverts = self._requests(imgs, masks, invert, wait)
+        if not checked:
             return []
-        dev = next((t.device for t, _, _ in checked if t.is_cuda), self.device_)
+        dev = self._device()
+        sizes = [resized_size(int(t.shape[1]), int(t.shape[0]), self.res) for t, _ in checked]
         nb = not wait
-        imgs_d = [_to(t, dev, nb) for t, _, _ in checked]
-        masks_d = [_to(m, dev, nb) for _, m, _ in checked]
-        outs_d = [torch.empty((h, w, 3), dtype=torch.uint8, device=dev) for _, _, (w, h) in checked]
-        for c in range(0, len(imgs), _abi.PIPE_MAX_BATCH):
+        imgs_d = [_to(t, dev, nb) for t, _ in checked]
+        masks_d = [_to(m, dev, nb) for _, m in checked]
+        outs_d = [torch.empty((h, w, 3), dtype=torch.uint8, device=dev) for w, h in sizes]
+        for c in range(0, len(checked), _abi.PIPE_MAX_BATCH):
             s = slice(c, c + _abi.PIPE_MAX_BATCH)
             self._pass(imgs_d[s], masks_d[s], inverts[s], outs_d[s])
-        results = []
-        for kind, out in zip(kinds, outs_d):
-            if kind == "cuda":
-                results.append(out)
-            else:
-                host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
-                host.copy_(out, non_blocking=True)
-                results.append(host)
-        event = torch.cuda.Event()
-        event.record(torch.cuda.current_stream(dev))
-        call = _Call(event, [size for _, _, size in checked], (imgs_d, masks_d, outs_d))
-        if wait:
-            self._finish([call])
-            return [r.numpy() if kind == "numpy" else r for kind, r in zip(kinds, results)]
-        self._pending.append(call)
-        return results
-
-    def _finish(self, calls) -> None:
-        sizes = []
-        for call in calls:
-            call.event.synchronize()
-            sizes += call.sizes
-        if sizes:
-            self.last_sizes = sizes
-
-    def wait(self) -> None:
-        """Block until every call enqueued with `forward_batch(..., wait=False)` has finished: its outputs are written and
-        `last_sizes` holds the sizes of all those calls' results, in submission order."""
-        calls, self._pending = self._pending, []
-        self._finish(calls)
-
-
-class _Call:
-    """One enqueued call: the event after its last copy, the result sizes, and the tensors its enqueued work reads or
-    writes (kept alive until the call is waited for)."""
-
-    def __init__(self, event, sizes, keep):
-        self.event, self.sizes, self.keep = event, sizes, keep
-
-
-def _to(t: torch.Tensor, device, non_blocking: bool) -> torch.Tensor:
-    """`t` contiguous on `device`.  A non-blocking copy from pageable memory would wait for the stream, so a pageable CPU
-    tensor is first staged by a host copy into pinned memory."""
-    if non_blocking and not t.is_cuda and not t.is_pinned():
-        t = t.pin_memory()
-    return t.to(device, non_blocking=non_blocking).contiguous()
+        return self._complete(kinds, outs_d, sizes, (imgs_d, masks_d, outs_d), torch.cuda.current_stream(dev), wait)

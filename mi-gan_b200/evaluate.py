@@ -25,8 +25,7 @@ import numpy as np
 import torch
 
 from . import _abi
-from .demo import _to
-from .generator import Generator
+from ._request_path import _to, load_generator
 from .masks import RandomMaskStream
 
 
@@ -36,21 +35,10 @@ class EvalPipeline(torch.nn.Module):
 
     def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0):
         super().__init__()
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("migan_b200.EvalPipeline runs on a CUDA device (there is no CPU path); got %s" % device)
-        if isinstance(model_or_state_dict, Generator):
-            if model_or_state_dict.resolution != resolution:
-                raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_or_state_dict.resolution, resolution))
-            self.model = model_or_state_dict
-        else:
-            self.model = Generator(resolution=resolution)
-            sd = model_or_state_dict if isinstance(model_or_state_dict, dict) else torch.load(model_or_state_dict, map_location="cpu")
-            self.model.load_state_dict(sd)
-        self.model = self.model.to(device).eval()
+        self.model = load_generator(self, model_or_state_dict, resolution, device)
         self.res = int(resolution)
-        self.device_ = device
-        self.masks = RandomMaskStream(self.res, seed=seed, device=device)
+        self.device_ = torch.device(device)
+        self.masks = RandomMaskStream(self.res, seed=seed, device=self.device_)
         self.last_launches = []                 # kernel launches of each pass of the last call, generator included
 
     @staticmethod

@@ -37,8 +37,8 @@ import numpy as np
 import torch
 
 from . import _abi
-from .demo import _Call, _to
-from .fullres import Chunk, _PhotoPipeline, plan_passes
+from ._request_path import _PhotoPipeline, _to
+from .fullres import plan_passes, window_passes
 
 Window = Tuple[int, int, int, int]          # (y0, x0, h, w)
 
@@ -55,6 +55,9 @@ class HoleWindowPipeline(_PhotoPipeline):
         self._side = None                                   # the stream of the mask uploads and the cells
         self.last_windows: List[List[Window]] = []          # the windows of every result of the last completed call(s)
         self.last_launches = 0                              # kernel launches of the last call, generator included
+
+    def _set_record(self, record: list) -> None:
+        self.last_windows = record
 
     def _side_stream(self, dev) -> torch.cuda.Stream:
         if self._side is None:
@@ -94,37 +97,6 @@ class HoleWindowPipeline(_PhotoPipeline):
             out.append([tuple(buf[4 * k:4 * k + 4]) for k in range(cnt.value)])
         return out
 
-    def _pass(self, eng, chunks: List[Chunk], wins, outs, masks, inverts, ws, stream) -> Tuple[list, int]:
-        """Enqueue one pass over windows; wins[j] = (request, window).  Returns (the tensors its work uses, launches)."""
-        lib = eng.lib
-        dev = eng.device
-        n = sum(len(c.requests) for c in chunks)
-        reqs = (_abi.WindowRequest * n)()
-        xs, ys, k = [], [], 0
-        for c in chunks:
-            x = torch.empty((len(c.requests), 4, c.Hp, c.Wp), dtype=torch.float32, device=dev)
-            y = torch.empty((len(c.requests), 3, c.Hp, c.Wp), dtype=torch.float32, device=dev)
-            xs.append(x)
-            ys.append(y)
-            for slot, j in enumerate(c.requests):
-                i, (y0, x0, h, w) = wins[j]
-                r = reqs[k]
-                k += 1
-                out, m = outs[i], masks[i]
-                r.img, r.out, r.H, r.W = out.data_ptr(), out.data_ptr(), int(out.shape[0]), int(out.shape[1])
-                r.mask, r.mask_channels, r.invert = m.data_ptr(), int(m.shape[2]), int(bool(inverts[i]))
-                r.y0, r.x0, r.h, r.w = y0, x0, h, w
-                r.x, r.y, r.Hp, r.Wp = x[slot].data_ptr(), y[slot].data_ptr(), c.Hp, c.Wp
-        path = _abi.path_id(self.model.path)
-        _abi.check(lib.b200_window_preprocess(reqs, n, stream))
-        launches = 2
-        for c, x, y in zip(chunks, xs, ys):
-            _abi.check(lib.migan_forward_hw(eng.handle, x.data_ptr(), y.data_ptr(), len(c.requests), c.Hp, c.Wp,
-                                            ws.data_ptr(), ws.numel(), path, stream))
-            launches += int(lib.migan_last_launch_count(eng.handle))
-        _abi.check(lib.b200_window_postprocess(reqs, n, stream))
-        return xs + ys, launches
-
     @torch.no_grad()
     def forward_batch(self, imgs: Sequence, masks: Sequence, invert: Union[bool, Sequence[bool]] = False,
                       wait: bool = True) -> list:
@@ -143,21 +115,12 @@ class HoleWindowPipeline(_PhotoPipeline):
         wait=False enqueues the rest on the current stream and returns the output tensors, which hold the results (and
         `last_windows` is set) after `wait()`.  CPU photos must then be pinned tensors (`pin_memory()`), since they are
         copied asynchronously; pageable CPU masks are staged through pinned memory."""
-        imgs, masks = list(imgs), list(masks)
-        if len(imgs) != len(masks):
-            raise ValueError("HoleWindowPipeline.forward_batch: %d photos and %d masks" % (len(imgs), len(masks)))
-        inverts = [bool(invert)] * len(imgs) if isinstance(invert, (bool, int)) else [bool(v) for v in invert]
-        if len(inverts) != len(imgs):
-            raise ValueError("HoleWindowPipeline.forward_batch: %d invert flags for %d requests" % (len(inverts), len(imgs)))
+        kinds, checked, inverts = self._requests(imgs, masks, invert, wait)
+        if not checked:
+            return []
         dev = self._device()
         with torch.cuda.device(dev):
             eng = self.model._engine(dev)
-            kinds, checked = [], []
-            for i, (img, mask) in enumerate(zip(imgs, masks)):
-                kinds.append(self._kind(i, img, wait))
-                checked.append(self._check(i, img, mask))
-            if not imgs:
-                return []
             nb = not wait
             cur = torch.cuda.current_stream(dev)
             side = self._side_stream(dev)
@@ -180,44 +143,12 @@ class HoleWindowPipeline(_PhotoPipeline):
                     extents.append(ext)
                     max_n[ext] = mx
             passes = plan_passes(extents, max_n)
-            ws = None
-            if passes:
-                need = max(eng.lib.migan_workspace_bytes_hw(eng.handle, len(c.requests), c.Hp, c.Wp) for p in passes for c in p)
-                ws = self._workspace(eng, need)
             cur.wait_event(ready)
-            stream = cur.cuda_stream
             outs_d = []
             for img, _ in checked:                          # the output photo: one copy of the input, windows written
                 out = torch.empty((int(img.shape[0]), int(img.shape[1]), 3), dtype=torch.uint8, device=dev)
                 out.copy_(img, non_blocking=nb)
                 outs_d.append(out)
-            keep = [masks_d, outs_d, cells_d, cells_h, ws]
-            for chunks in passes:
-                tensors, n_launch = self._pass(eng, chunks, wins, outs_d, masks_d, inverts, ws, stream)
-                keep.append(tensors)
-                launches += n_launch
-            self.last_launches = launches
-            results = []
-            for kind, out in zip(kinds, outs_d):
-                if kind == "cuda":
-                    results.append(out)
-                else:
-                    host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
-                    host.copy_(out, non_blocking=True)
-                    results.append(host)
-            event = torch.cuda.Event()
-            event.record(cur)
-        call = _Call(event, wins_per, keep)
-        if wait:
-            self._finish([call])
-            return [r.numpy() if kind == "numpy" else r for kind, r in zip(kinds, results)]
-        self._pending.append(call)
-        return results
-
-    def _finish(self, calls) -> None:
-        windows = []
-        for call in calls:
-            call.event.synchronize()
-            windows += call.sizes
-        if windows:
-            self.last_windows = windows
+            keep, pass_launches = window_passes(self, eng, passes, wins, outs_d, masks_d, inverts, outs_d)
+            self.last_launches = launches + sum(pass_launches)
+            return self._complete(kinds, outs_d, wins_per, [masks_d, outs_d, cells_d, cells_h] + keep, cur, wait)

@@ -30,33 +30,19 @@ from typing import List, Tuple, Union
 import torch
 
 from . import _abi, ops
-from .generator import Generator
+from ._request_path import _Call, _Queued, _to
 
 
-class MIGAN_Pipeline(torch.nn.Module):
+class MIGAN_Pipeline(_Queued):
     """Drop-in for scripts/create_onnx_pipeline.py:MIGAN_Pipeline.  `model_path`: a state_dict file written by the reference's
     export script (`torch.load`-able), a state_dict, or a ready `migan_b200.Generator`."""
 
     def __init__(self, model_path, resolution: int, padding: int = 128, device: Union[str, torch.device] = "cuda"):
-        super().__init__()
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("migan_b200.MIGAN_Pipeline runs on a CUDA device (there is no CPU path); got %s" % device)
-        if isinstance(model_path, Generator):
-            if model_path.resolution != resolution:
-                raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_path.resolution, resolution))
-            self.model = model_path
-        else:
-            self.model = Generator(resolution=resolution)
-            sd = model_path if isinstance(model_path, dict) else torch.load(model_path, map_location="cpu")
-            self.model.load_state_dict(sd)
-        self.model = self.model.to(device).eval()
+        super().__init__(model_path, resolution, device)
         self.register_buffer("gaussian_kernel", ops.feather_kernel(5, 1.0))     # GaussianSmoothing(1, 5, 1.0), :127-128
         self._k25 = ops.feather_kernel(5, 1.0).contiguous()                     # host copy handed to the C ABI
-        self.res = int(resolution)
         self.padding = int(padding)
-        self.device_ = device
-        self._pending: List["_Call"] = []                           # calls of forward_batch(..., wait=False) not yet waited for
+        self.device_ = torch.device(device)
         self.last_box: Tuple[int, int, int, int] = (0, 0, 0, 0)     # the last request's crop window
         self.last_boxes: List[Tuple[int, int, int, int]] = []        # every request's crop window of the last call
 
@@ -134,23 +120,10 @@ class MIGAN_Pipeline(torch.nn.Module):
             event.record(torch.cuda.current_stream(images[0].device))
         return _Call(event, boxes, (images, masks, copy_back))
 
-    def _finish(self, calls) -> None:
-        """Wait for `calls` in order; `last_boxes` becomes all their crop windows."""
-        boxes = []
-        for call in calls:
-            if call.event is not None:
-                call.event.synchronize()
-            for b in call.boxes:
-                boxes += [tuple(int(v) for v in row) for row in b.tolist()]
-        if boxes:
-            self.last_boxes = boxes
-            self.last_box = boxes[-1]
-
-    def wait(self) -> None:
-        """Block until every call enqueued with `forward_batch(..., wait=False)` has finished: its images are updated and
-        `last_boxes` / `last_box` hold the crop windows of all those calls, in submission order."""
-        calls, self._pending = self._pending, []
-        self._finish(calls)
+    def _set_record(self, record: list) -> None:
+        """`record`: the pinned crop-window buffers of the passes waited for, read only now that their copies are done."""
+        self.last_boxes = [tuple(int(v) for v in row) for b in record for row in b.tolist()]
+        self.last_box = self.last_boxes[-1]
 
     @torch.no_grad()
     def forward(self, image: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
@@ -207,22 +180,6 @@ class MIGAN_Pipeline(torch.nn.Module):
         else:
             self._pending.append(call)
         return images
-
-
-class _Call:
-    """One enqueued call: the event after its last copy, the pinned crop-window buffers of its passes, and the tensors its
-    enqueued work reads or writes (kept alive until the call is waited for)."""
-
-    def __init__(self, event, boxes, keep):
-        self.event, self.boxes, self.keep = event, boxes, keep
-
-
-def _to(t: torch.Tensor, device, non_blocking: bool) -> torch.Tensor:
-    """`t` contiguous on `device`.  A non-blocking copy from pageable memory would wait for the stream, so a pageable CPU
-    tensor is first staged by a host copy into pinned memory."""
-    if non_blocking and not t.is_cuda and not t.is_pinned():
-        t = t.pin_memory()
-    return t.to(device, non_blocking=non_blocking).contiguous()
 
 
 def _span(t: torch.Tensor):

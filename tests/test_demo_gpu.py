@@ -6,7 +6,8 @@
 * square R x R requests give exactly `Generator.forward_u8`'s bytes;
 * `forward_batch` of 24 mixed requests equals the 24 single calls;
 * two back-to-back `forward_batch(..., wait=False)` calls equal sequential ones, and the call returns before the stream
-  drains; pageable CPU photos are refused with wait=False."""
+  drains; pageable CPU photos are refused with wait=False;
+* a non-array photo is a TypeError, and a CUDA photo on another GPU than the pipeline's a ValueError, before any work."""
 import ctypes
 import os
 import sys
@@ -169,3 +170,24 @@ def test_mask_size_mismatch_is_value_error(cuda_device):
     pipe = _pipe(256, cuda_device)
     with pytest.raises(ValueError, match="mask resizes"):
         pipe(np.zeros((300, 700, 3), np.uint8), np.zeros((300, 600), np.uint8))
+
+
+def test_non_array_photo_is_type_error(cuda_device):
+    pipe = _pipe(256, cuda_device)
+    img, mask = np.zeros((40, 50, 3), np.uint8), np.full((40, 50), 255, np.uint8)
+    with pytest.raises(TypeError, match="DemoPipeline: request 1: photo and mask must be"):
+        pipe.forward_batch([img, [[1, 2, 3]]], [mask, mask])
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_photo_on_another_gpu_refused_before_any_work(cuda_device):
+    pipe = _pipe(256, cuda_device)
+    other = torch.device("cuda", 1)
+    img = torch.zeros((40, 50, 3), dtype=torch.uint8, device=other)
+    mask = torch.full((40, 50), 255, dtype=torch.uint8)
+    torch.cuda.synchronize(other)
+    mem0 = torch.cuda.memory_allocated(other)
+    with pytest.raises(ValueError, match="DemoPipeline: request 0: photo on cuda:1, the pipeline runs on cuda:0"):
+        pipe.forward_batch([img], [mask])
+    torch.cuda.synchronize(other)
+    assert torch.cuda.memory_allocated(other) == mem0
