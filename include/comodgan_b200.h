@@ -1,7 +1,8 @@
 /* comodgan_b200.h -- C ABI of the H100-native Co-Mod-GAN generator forward and of conv2d_resample.
  *
- * Same shared library and conventions as migan_b200.h (return 0 / non-zero code, comodgan_last_error(), fp32
- * device pointers, `stream` = cudaStream_t as void*, no CPU fallback).  Reference interfaces replaced
+ * Same shared library and conventions as migan_b200.h (return 0 / non-zero MIGAN_ERR_* code, fp32 device pointers,
+ * `stream` = cudaStream_t as void*, no CPU fallback).  comodgan_last_error() returns the same thread-local message as
+ * migan_last_error().  Reference interfaces replaced
  * (file:line in /root/reference):
  *
  *   comodgan_create / _destroy        Generator(Mapping(num_ws), Encoder(resolution), Synthesis(resolution))

@@ -244,13 +244,15 @@ def load(build_if_missing: bool = False):
     return lib
 
 
-def check(rc: int) -> None:
+_LAST_ERROR = ctypes.CFUNCTYPE(c_char_p)
+
+
+def check(rc: int, lib=None) -> None:
+    """Raise MiganError for a non-zero return code of `lib` (the loaded library when None), with the calling thread's last
+    error.  The message is read from the library's own migan_last_error export, whichever symbols the caller bound."""
     if rc != 0:
-        msg = load().migan_last_error()
+        msg = _LAST_ERROR(("migan_last_error", lib or load()))()
         raise MiganError(rc, msg.decode() if msg else "unknown error")
 
 
-def check_comod(rc: int, lib=None) -> None:
-    if rc != 0:
-        msg = (lib or load()).comodgan_last_error()
-        raise MiganError(rc, msg.decode() if msg else "unknown error")
+check_comod = check   # the Co-Mod-GAN callers' name: comodgan_last_error() is the same thread-local message

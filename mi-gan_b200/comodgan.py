@@ -39,7 +39,7 @@ def _spec(resolution: int) -> List[Tuple[str, Tuple[int, ...]]]:
     out = []
     name, nd, shape = ctypes.c_char_p(), ctypes.c_int(), (ctypes.c_int64 * 4)()
     for i in range(lib.comodgan_num_weights(h)):
-        _abi.check_comod(lib.comodgan_weight_info(h, i, ctypes.byref(name), ctypes.byref(nd), shape))
+        _abi.check(lib.comodgan_weight_info(h, i, ctypes.byref(name), ctypes.byref(nd), shape))
         out.append((name.value.decode(), tuple(int(v) for v in shape[:nd.value])))
     lib.comodgan_destroy(h)
     return out
@@ -137,7 +137,7 @@ class _Engine:
         self.lib = _abi.load()
         self.device = device
         self.handle = ctypes.c_void_p()
-        _abi.check_comod(self.lib.comodgan_create(resolution, _device_index(device), ctypes.byref(self.handle)))
+        _abi.check(self.lib.comodgan_create(resolution, _device_index(device), ctypes.byref(self.handle)))
         self.weights_version = None
         self.workspaces: Dict[int, torch.Tensor] = {}
         self.noise_res = [self.lib.comodgan_noise_plane_res(self.handle, i)
@@ -161,8 +161,8 @@ class _Engine:
             self.__init__(resolution, dev)
         for key, t in state.items():
             h = t.detach().to(device="cpu", dtype=torch.float32).contiguous()
-            _abi.check_comod(self.lib.comodgan_set_weight(self.handle, key.encode(), h.data_ptr(), h.numel()))
-        _abi.check_comod(self.lib.comodgan_finalize_weights(self.handle))
+            _abi.check(self.lib.comodgan_set_weight(self.handle, key.encode(), h.data_ptr(), h.numel()))
+        _abi.check(self.lib.comodgan_finalize_weights(self.handle))
         self.weights_version = version
 
     def workspace(self, n: int) -> torch.Tensor:
@@ -258,9 +258,9 @@ class Generator(nn.Module):
             tap_buf = None
             if _tap is not None:
                 tap_buf = torch.zeros((n,) + tuple(_tap[1]), dtype=torch.float32, device=x.device)
-                _abi.check_comod(eng.lib.comodgan_set_tap(eng.handle, _tap[0].encode(), tap_buf.data_ptr()))
+                _abi.check(eng.lib.comodgan_set_tap(eng.handle, _tap[0].encode(), tap_buf.data_ptr()))
             try:
-                _abi.check_comod(eng.lib.comodgan_forward(
+                _abi.check(eng.lib.comodgan_forward(
                     eng.handle, x.data_ptr(), z.data_ptr(), y.data_ptr(), n, float(truncation_psi),
                     -1 if truncation_cutoff is None else int(truncation_cutoff), NOISE_MODES[noise_mode],
                     planes.data_ptr() if planes is not None else None, ws.data_ptr(), ws.numel(), stream))

@@ -20,7 +20,6 @@
 // that sizes the workspace, then the launching pass.
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -30,6 +29,7 @@
 
 #include "../../include/comodgan_b200.h"
 #include "comod_kernels.cuh"
+#include "weight_registry.h"
 
 #ifndef MIGAN_EMULATE
 #include "kernels.h"
@@ -38,22 +38,11 @@
 
 namespace {
 using namespace comod;
+using migan::fail;
 
-constexpr int ERR_INVALID = 1, ERR_CUDA = 2, ERR_STATE = 3, ERR_WORKSPACE = 4;
 constexpr int Z_DIM = 512, W_DIM = 512, W0_DIM = 1024, MAP_LAYERS = 8;   // stylegan.py:357-361, comodgan.py:117
 constexpr float MAP_LR = 0.01f;                                          // stylegan.py:365
 constexpr float SQRT2 = 1.41421356237309515f;
-
-thread_local std::string g_err;
-int fail(int code, const char* fmt, ...) {
-    char buf[1024];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    g_err = buf;
-    return code;
-}
 
 inline int channels(int res) { return std::min(32768 / res, 512); }   // comodgan.py:140-141 (ch_base 32768, ch_max 512)
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -136,7 +125,7 @@ struct Runner {
         float* p = reinterpret_cast<float*>(base + off);
         off += align_up(floats * sizeof(float), 256);
         peak = std::max(peak, off);
-        if (!dry && off > cap && !rc) rc = fail(ERR_WORKSPACE, "workspace too small: need > %zu bytes, have %zu", off, cap);
+        if (!dry && off > cap && !rc) rc = fail(MIGAN_ERR_WORKSPACE, "workspace too small: need > %zu bytes, have %zu", off, cap);
         return p;
     }
     size_t mark() const { return off; }
@@ -145,20 +134,20 @@ struct Runner {
     void launch(const F& f, int64_t items) {
         if (dry || rc || items <= 0) return;
         const int e = (int)ck_launch(f, items, s);
-        if (e) rc = fail(ERR_CUDA, "kernel launch failed: %s", dev_err(e));
+        if (e) rc = fail(MIGAN_ERR_CUDA, "kernel launch failed: %s", dev_err(e));
         ++launches;
     }
     void gemm(const float* A, const float* Bt, float* out, int64_t P, int K, int N) {
         if (dry || rc || P <= 0) return;
-        if (K % 16 || N % 64) { rc = fail(ERR_INVALID, "internal: GEMM dims K=%d N=%d not padded", K, N); return; }
+        if (K % 16 || N % 64) { rc = fail(MIGAN_ERR_INVALID, "internal: GEMM dims K=%d N=%d not padded", K, N); return; }
         const int e = gemm_f32(A, Bt, out, P, K, N, s);
-        if (e) rc = fail(ERR_CUDA, "GEMM launch failed: %s", dev_err(e));
+        if (e) rc = fail(MIGAN_ERR_CUDA, "GEMM launch failed: %s", dev_err(e));
         ++launches;
     }
     void gemm_tc_(const ck_half* a_hi, const ck_half* a_lo, const ck_half* b_hi, const ck_half* b_lo, float inv_scale, float* out,
                   int n, int res, int K, int N) {
         if (dry || rc || n <= 0) return;
-        if (const char* err = gemm_tc(a_hi, a_lo, b_hi, b_lo, inv_scale, out, n, res, K, N, s)) rc = fail(ERR_CUDA, "wgmma GEMM: %s", err);
+        if (const char* err = gemm_tc(a_hi, a_lo, b_hi, b_lo, inv_scale, out, n, res, K, N, s)) rc = fail(MIGAN_ERR_CUDA, "wgmma GEMM: %s", err);
         ++launches;
     }
     void im2col_split(const float* in, const float* scale, ck_half* hi, ck_half* lo, float a_scale, int64_t n, int H, int W, int C,
@@ -188,13 +177,6 @@ struct Runner {
 };
 
 // ---- layers ---------------------------------------------------------------------------------------------------------
-struct Spec {
-    std::string name;
-    int ndim;
-    int64_t shape[4];
-    int64_t numel() const { int64_t n = 1; for (int i = 0; i < ndim; ++i) n *= shape[i]; return n; }
-};
-
 struct DenseL {
     std::string p;
     int in = 0, out = 0;
@@ -239,10 +221,7 @@ struct EncBlock {
 struct comodgan_ctx {
     int resolution = 0, log2res = 0, device = -1;
     bool finalized = false;
-    std::vector<Spec> specs;
-    std::map<std::string, int> index;
-    std::vector<std::vector<float>> host;   // per spec; emptied by finalize
-    std::vector<bool> have;
+    migan::WeightRegistry weights;   // host copies emptied by finalize
     std::vector<void*> allocs;
     // packed network
     DenseL mapping[MAP_LAYERS];
@@ -265,42 +244,32 @@ namespace {
 
 constexpr float kTcActScale = 8.f;   // A-operand scale of the fp16 split: |x * style| <= 8188 stays finite in fp16
 
-void add_spec(comodgan_ctx* c, const std::string& name, std::initializer_list<int64_t> shape) {
-    Spec s;
-    s.name = name;
-    s.ndim = (int)shape.size();
-    int i = 0;
-    for (int64_t v : shape) s.shape[i++] = v;
-    for (; i < 4; ++i) s.shape[i] = 1;
-    c->index[name] = (int)c->specs.size();
-    c->specs.push_back(s);
-}
-
 // Reference state_dict order: mapping, synthesis, encoder (stylegan.py:572-579, comodgan.py:431-435).
 void build_specs(comodgan_ctx* c) {
     const int R = c->resolution;
-    add_spec(c, "mapping.w_avg", {W_DIM});
+    migan::WeightRegistry& reg = c->weights;
+    reg.add("mapping.w_avg", {W_DIM});
     for (int i = 0; i < MAP_LAYERS; ++i) {
-        add_spec(c, "mapping.fc" + std::to_string(i) + ".weight", {W_DIM, i == 0 ? Z_DIM : W_DIM});
-        add_spec(c, "mapping.fc" + std::to_string(i) + ".bias", {W_DIM});
+        reg.add("mapping.fc" + std::to_string(i) + ".weight", {W_DIM, i == 0 ? Z_DIM : W_DIM});
+        reg.add("mapping.fc" + std::to_string(i) + ".bias", {W_DIM});
     }
     auto synth_layer = [&](const std::string& p, int cin, int cout, int res, int k, bool filt, bool noise) {
-        add_spec(c, p + ".weight", {cout, cin, k, k});
-        add_spec(c, p + ".bias", {cout});
-        if (noise) add_spec(c, p + ".noise_strength", {});
-        if (filt) add_spec(c, p + ".resample_filter", {4, 4});
-        if (noise) add_spec(c, p + ".noise_const", {res, res});
-        add_spec(c, p + ".affine.weight", {cin, W_DIM + W0_DIM});
-        add_spec(c, p + ".affine.bias", {cin});
+        reg.add(p + ".weight", {cout, cin, k, k});
+        reg.add(p + ".bias", {cout});
+        if (noise) reg.add(p + ".noise_strength", {});
+        if (filt) reg.add(p + ".resample_filter", {4, 4});
+        if (noise) reg.add(p + ".noise_const", {res, res});
+        reg.add(p + ".affine.weight", {cin, W_DIM + W0_DIM});
+        reg.add(p + ".affine.bias", {cin});
     };
     const int c4 = channels(4);
-    add_spec(c, "synthesis.b4.fc.weight", {c4 * 16, W0_DIM});
-    add_spec(c, "synthesis.b4.fc.bias", {c4 * 16});
+    reg.add("synthesis.b4.fc.weight", {c4 * 16, W0_DIM});
+    reg.add("synthesis.b4.fc.bias", {c4 * 16});
     synth_layer("synthesis.b4.conv", c4, c4, 4, 3, true, true);
     synth_layer("synthesis.b4.torgb", c4, 3, 4, 1, false, false);
     for (int r = 8; r <= R; r *= 2) {
         const std::string p = "synthesis.b" + std::to_string(r);
-        add_spec(c, p + ".resample_filter", {4, 4});
+        reg.add(p + ".resample_filter", {4, 4});
         synth_layer(p + ".conv0", channels(r / 2), channels(r), r, 3, true, true);
         synth_layer(p + ".conv1", channels(r), channels(r), r, 3, false, true);
         synth_layer(p + ".torgb", channels(r), 3, r, 1, false, false);
@@ -308,32 +277,30 @@ void build_specs(comodgan_ctx* c) {
     for (int r = R; r >= 8; r /= 2) {
         const std::string p = "encoder.b" + std::to_string(r);
         const int ci = channels(r), co = channels(r / 2);
-        add_spec(c, p + ".resample_filter", {4, 4});
+        reg.add(p + ".resample_filter", {4, 4});
         if (r == R) {
-            add_spec(c, p + ".fromrgb.weight", {ci, 4, 1, 1});
-            add_spec(c, p + ".fromrgb.bias", {ci});
+            reg.add(p + ".fromrgb.weight", {ci, 4, 1, 1});
+            reg.add(p + ".fromrgb.bias", {ci});
         }
-        add_spec(c, p + ".conv0.weight", {ci, ci, 3, 3});
-        add_spec(c, p + ".conv0.bias", {ci});
-        add_spec(c, p + ".conv1.weight", {co, ci, 3, 3});
-        add_spec(c, p + ".conv1.bias", {co});
-        add_spec(c, p + ".conv1.resample_filter", {4, 4});
+        reg.add(p + ".conv0.weight", {ci, ci, 3, 3});
+        reg.add(p + ".conv0.bias", {ci});
+        reg.add(p + ".conv1.weight", {co, ci, 3, 3});
+        reg.add(p + ".conv1.bias", {co});
+        reg.add(p + ".conv1.resample_filter", {4, 4});
     }
-    add_spec(c, "encoder.b4.conv.weight", {c4, c4, 3, 3});
-    add_spec(c, "encoder.b4.conv.bias", {c4});
-    add_spec(c, "encoder.b4.fc.weight", {W0_DIM, c4 * 16});
-    add_spec(c, "encoder.b4.fc.bias", {W0_DIM});
+    reg.add("encoder.b4.conv.weight", {c4, c4, 3, 3});
+    reg.add("encoder.b4.conv.bias", {c4});
+    reg.add("encoder.b4.fc.weight", {W0_DIM, c4 * 16});
+    reg.add("encoder.b4.fc.bias", {W0_DIM});
 }
-
-const std::vector<float>& H(const comodgan_ctx* c, const std::string& name) { return c->host[c->index.at(name)]; }
 
 int upload(comodgan_ctx* c, const std::vector<float>& v, float** out) {
     void* d = nullptr;
     int e = dev_alloc(&d, v.size() * sizeof(float));
-    if (e) return fail(ERR_CUDA, "device allocation of %zu bytes failed: %s", v.size() * sizeof(float), dev_err(e));
+    if (e) return fail(MIGAN_ERR_CUDA, "device allocation of %zu bytes failed: %s", v.size() * sizeof(float), dev_err(e));
     c->allocs.push_back(d);
     e = dev_copy(d, v.data(), v.size() * sizeof(float), nullptr);
-    if (e) return fail(ERR_CUDA, "upload failed: %s", dev_err(e));
+    if (e) return fail(MIGAN_ERR_CUDA, "upload failed: %s", dev_err(e));
     *out = static_cast<float*>(d);
     return 0;
 }
@@ -348,8 +315,8 @@ int pack_dense(comodgan_ctx* c, DenseL& L, const std::string& p, int in, int out
     // stylegan.py:84-96: w * (lr / sqrt(in)), b * lr.  in_perm[k'] = reference column feeding packed row k';
     // out_perm[o'] = reference row producing packed column o'.
     L.p = p; L.in = in; L.out = out; L.act = act;
-    const std::vector<float>& w = H(c, p + ".weight");
-    const std::vector<float>& b = H(c, p + ".bias");
+    const std::vector<float>& w = c->weights.get(p + ".weight");
+    const std::vector<float>& b = c->weights.get(p + ".bias");
     const float wg = lr / std::sqrt((float)in);
     std::vector<float> bt((size_t)in * out), bb(out);
     for (int k = 0; k < in; ++k) {
@@ -372,7 +339,7 @@ int pack_conv(comodgan_ctx* c, ConvL& L, const std::string& p, int cin, int cout
     L.modulated = kind != CONV_PLAIN;
     L.demod = kind == CONV_SYNTH;
     L.act = kind != CONV_TORGB;
-    const std::vector<float>& w = H(c, p + ".weight");
+    const std::vector<float>& w = c->weights.get(p + ".weight");
     const int taps = k * k;
     // per-output-channel scale folded into the packed operand
     std::vector<float> oscale(cout, 1.f);
@@ -423,90 +390,45 @@ int pack_conv(comodgan_ctx* c, ConvL& L, const std::string& p, int cin, int cout
     if (tmp[1]) dev_free(tmp[1]);
     if (e) {
         if (bt) dev_free(bt);
-        return fail(ERR_CUDA, "weight packing failed: %s", dev_err(e));
+        return fail(MIGAN_ERR_CUDA, "weight packing failed: %s", dev_err(e));
     }
     c->allocs.push_back(bt);
     L.Bt = (float*)bt;
-    if (c->use_tc && up > 1 && cin % 64 == 0) {
-        // transposed convolution: one K-major operand per tap, B_t[co][ci] = w[co][ci][tap'] (conv2d_resample.py:140 flip rule)
-        L.KPc = cin;
+    if (c->use_tc && (up > 1 ? cin % 64 == 0 : cin % 4 == 0)) {
+        // The wgmma operand: the fp32 operand's values K-major, split into fp16 hi + lo of w * 2^k.  Transposed convolution:
+        // one operand per tap, B_t[co][ci] = w[co][ci][tap'].  Plain: B[o][k], k = (ky*kw + kx)*cin + ci.
+        L.KPc = up > 1 ? cin : round_up(taps * cin, 64);
         L.NPc = round_up(cout, 64);
         const size_t per_tap = (size_t)L.NPc * L.KPc;
-        std::vector<float> b(per_tap * taps, 0.f);
-        float maxabs = 0.f;
-        for (int t = 0; t < taps; ++t) {
-            const int ts = flip_weight ? taps - 1 - t : t;               // PackWeightTK: flip when the original flip_weight is set
-            for (int o = 0; o < cout; ++o)
-                for (int ci = 0; ci < cin; ++ci) {
-                    const float v = w[((size_t)o * cin + ci) * taps + ts] * gain * oscale[o];
-                    b[t * per_tap + (size_t)o * L.KPc + ci] = v;
-                    if (std::isfinite(v)) maxabs = std::max(maxabs, std::fabs(v));
-                }
-        }
-        int k2 = maxabs > 0.f ? (int)std::floor(std::log2(16384.0 / (double)maxabs)) : 0;
-        k2 = std::max(-14, std::min(24, k2));
-        const float wscale = std::ldexp(1.0f, k2);
-        L.tc_inv_scale = 1.0f / (wscale * kTcActScale);
-        std::vector<ck_half> hi(b.size()), lo(b.size());
-        for (size_t i = 0; i < b.size(); ++i) {
-            const float sv = b[i] * wscale;
-            hi[i] = ck_f2h(sv);
-            lo[i] = ck_f2h(sv - ck_h2f(hi[i]));
-        }
-        void* d[2] = {nullptr, nullptr};
-        for (int j = 0; j < 2; ++j) {
-            if (int e2 = dev_alloc(&d[j], b.size() * sizeof(ck_half))) return fail(ERR_CUDA, "device allocation failed: %s", dev_err(e2));
-            c->allocs.push_back(d[j]);
-            dev_copy(d[j], j == 0 ? (const void*)hi.data() : (const void*)lo.data(), b.size() * sizeof(ck_half), nullptr);
-        }
-        if (int e2 = dev_sync()) return fail(ERR_CUDA, "weight upload failed: %s", dev_err(e2));
-        L.Bh = (ck_half*)d[0];
-        L.Bl = (ck_half*)d[1];
-    }
-    if (c->use_tc && up == 1 && cin % 4 == 0) {
-        // B[o][k], k = (ky*kw + kx)*cin + ci: same values as the fp32 operand, K-major, scaled by a power of two so that the
-        // largest weight lands in [8192, 16384) (both halves well inside fp16's normal range), split into hi + lo.
-        L.KPc = round_up(taps * cin, 64);
-        L.NPc = round_up(cout, 64);
-        std::vector<float> b((size_t)L.NPc * L.KPc, 0.f);
-        float maxabs = 0.f;
+        std::vector<float> b(up > 1 ? per_tap * taps : per_tap, 0.f);
         for (int o = 0; o < cout; ++o)
             for (int t = 0; t < taps; ++t) {
-                const int ts = flip_weight ? t : taps - 1 - t;          // mirrored taps = true convolution
-                for (int ci = 0; ci < cin; ++ci) {
-                    const float v = w[((size_t)o * cin + ci) * taps + ts] * gain * oscale[o];
-                    b[(size_t)o * L.KPc + t * cin + ci] = v;
-                    if (std::isfinite(v)) maxabs = std::max(maxabs, std::fabs(v));
-                }
+                // PackWeightTK flips the taps when flip_weight is set (conv2d_resample.py:140); the plain operand mirrors
+                // them unless it is set (true convolution)
+                const int ts = (up > 1) == flip_weight ? taps - 1 - t : t;
+                float* row = up > 1 ? &b[t * per_tap + (size_t)o * L.KPc] : &b[(size_t)o * L.KPc + (size_t)t * cin];
+                for (int ci = 0; ci < cin; ++ci) row[ci] = w[((size_t)o * cin + ci) * taps + ts] * gain * oscale[o];
             }
-        int k2 = maxabs > 0.f ? (int)std::floor(std::log2(16384.0 / (double)maxabs)) : 0;
-        k2 = std::max(-14, std::min(24, k2));
-        const float wscale = std::ldexp(1.0f, k2);
-        L.tc_inv_scale = 1.0f / (wscale * kTcActScale);
         std::vector<ck_half> hi(b.size()), lo(b.size());
-        for (size_t i = 0; i < b.size(); ++i) {
-            const float sv = b[i] * wscale;
-            hi[i] = ck_f2h(sv);
-            lo[i] = ck_f2h(sv - ck_h2f(hi[i]));
-        }
+        L.tc_inv_scale = 1.0f / (migan::split_pow2(b.data(), b.size(), hi.data(), lo.data()) * kTcActScale);
         void* d[2] = {nullptr, nullptr};
         for (int j = 0; j < 2; ++j) {
-            if (int e2 = dev_alloc(&d[j], b.size() * sizeof(ck_half))) return fail(ERR_CUDA, "device allocation failed: %s", dev_err(e2));
+            if (int e2 = dev_alloc(&d[j], b.size() * sizeof(ck_half))) return fail(MIGAN_ERR_CUDA, "device allocation failed: %s", dev_err(e2));
             c->allocs.push_back(d[j]);
             dev_copy(d[j], j == 0 ? (const void*)hi.data() : (const void*)lo.data(), b.size() * sizeof(ck_half), nullptr);
         }
-        if (int e2 = dev_sync()) return fail(ERR_CUDA, "weight upload failed: %s", dev_err(e2));
+        if (int e2 = dev_sync()) return fail(MIGAN_ERR_CUDA, "weight upload failed: %s", dev_err(e2));
         L.Bh = (ck_half*)d[0];
         L.Bl = (ck_half*)d[1];
     }
-    if (c->index.count(p + ".bias")) {
-        if (int rc = upload(c, H(c, p + ".bias"), &L.bias)) return rc;
+    if (c->weights.has(p + ".bias")) {
+        if (int rc = upload(c, c->weights.get(p + ".bias"), &L.bias)) return rc;
     }
-    if (c->index.count(p + ".resample_filter")) fir_taps(H(c, p + ".resample_filter"), up > 1 ? (float)(up * up) : 1.f, L.fir);
-    if (c->index.count(p + ".noise_const")) {
+    if (c->weights.has(p + ".resample_filter")) fir_taps(c->weights.get(p + ".resample_filter"), up > 1 ? (float)(up * up) : 1.f, L.fir);
+    if (c->weights.has(p + ".noise_const")) {
         L.has_noise = true;
-        L.noise_strength = H(c, p + ".noise_strength")[0];
-        if (int rc = upload(c, H(c, p + ".noise_const"), &L.noise_const)) return rc;
+        L.noise_strength = c->weights.get(p + ".noise_strength")[0];
+        if (int rc = upload(c, c->weights.get(p + ".noise_const"), &L.noise_const)) return rc;
     }
     if (L.modulated) {
         // affine: dense(w_dim + w0_dim, cin, bias_init=1), no activation (stylegan.py:270)
@@ -758,36 +680,34 @@ struct Walk {
     }
 };
 
-int check_ctx(const comodgan_ctx* c) { return c ? 0 : fail(ERR_INVALID, "null context"); }
+int check_ctx(const comodgan_ctx* c) { return c ? 0 : fail(MIGAN_ERR_INVALID, "null context"); }
 
 }  // namespace
 
 // =====================================================================================================================
 extern "C" {
 
-const char* comodgan_last_error(void) { return g_err.c_str(); }
+const char* comodgan_last_error(void) { return migan::g_last_error.c_str(); }
 
 int comodgan_create(int resolution, int device, comodgan_ctx** out) {
-    if (!out) return fail(ERR_INVALID, "out is null");
+    if (!out) return fail(MIGAN_ERR_INVALID, "out is null");
     int l2 = 0;
     while ((1 << l2) < resolution) ++l2;
     if (resolution < 8 || (1 << l2) != resolution)
-        return fail(ERR_INVALID, "resolution must be a power of two >= 8, got %d (ValueError in the reference)", resolution);
+        return fail(MIGAN_ERR_INVALID, "resolution must be a power of two >= 8, got %d (ValueError in the reference)", resolution);
     if (device >= 0) {
         const int e = dev_set(device);
-        if (e) return fail(ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
+        if (e) return fail(MIGAN_ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
     }
     comodgan_ctx* c = new comodgan_ctx();
     c->resolution = resolution;
     c->log2res = l2;
     c->device = device;
     build_specs(c);
-    c->host.resize(c->specs.size());
-    c->have.assign(c->specs.size(), false);
     if (const char* e = getenv("COMOD_COL_CAP_MB")) c->col_cap_floats = (size_t)std::max(1, atoi(e)) * (1 << 20) / 4;
     if (const char* e = getenv("COMOD_GEMM")) c->use_tc = (strcmp(e, "tc") == 0);
     if (c->use_tc && device >= 0) {
-        if (int e2 = tc_configure()) { delete c; return fail(ERR_CUDA, "wgmma kernel setup failed: %s", dev_err(e2)); }
+        if (int e2 = tc_configure()) { delete c; return fail(MIGAN_ERR_CUDA, "wgmma kernel setup failed: %s", dev_err(e2)); }
     }
     *out = c;
     return 0;
@@ -800,43 +720,31 @@ int comodgan_destroy(comodgan_ctx* c) {
     return 0;
 }
 
-int comodgan_num_weights(const comodgan_ctx* c) { return c ? (int)c->specs.size() : 0; }
+int comodgan_num_weights(const comodgan_ctx* c) { return c ? c->weights.size() : 0; }
 
 int comodgan_weight_info(const comodgan_ctx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
     if (int rc = check_ctx(c)) return rc;
-    if (index < 0 || index >= (int)c->specs.size()) return fail(ERR_INVALID, "weight index %d out of range", index);
-    const Spec& s = c->specs[index];
-    if (name) *name = s.name.c_str();
-    if (ndim) *ndim = s.ndim;
-    if (shape) for (int i = 0; i < 4; ++i) shape[i] = s.shape[i];
-    return 0;
+    return c->weights.info(index, name, ndim, shape);
 }
 
 int comodgan_set_weight(comodgan_ctx* c, const char* name, const float* host_data, int64_t numel) {
     if (int rc = check_ctx(c)) return rc;
-    if (!name || !host_data) return fail(ERR_INVALID, "null argument");
-    if (c->finalized) return fail(ERR_STATE, "weights already finalized");
-    auto it = c->index.find(name);
-    if (it == c->index.end()) return fail(ERR_INVALID, "unexpected key '%s' in state_dict", name);
-    const Spec& s = c->specs[it->second];
-    if (numel != s.numel()) return fail(ERR_INVALID, "size mismatch for %s: got %lld values, expected %lld", name, (long long)numel, (long long)s.numel());
-    c->host[it->second].assign(host_data, host_data + numel);
-    c->have[it->second] = true;
-    return 0;
+    if (!name || !host_data) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
+    return c->weights.set(name, host_data, numel);
 }
 
 int comodgan_finalize_weights(comodgan_ctx* c) {
     if (int rc = check_ctx(c)) return rc;
-    if (c->finalized) return fail(ERR_STATE, "weights already finalized");
-    if (c->device < 0) return fail(ERR_CUDA, "context was created without a CUDA device (description only)");
-    for (size_t i = 0; i < c->specs.size(); ++i)
-        if (!c->have[i]) return fail(ERR_INVALID, "missing key '%s' in state_dict", c->specs[i].name.c_str());
-    if (int e = dev_set(c->device)) return fail(ERR_CUDA, "cannot select device: %s", dev_err(e));
+    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
+    if (c->device < 0) return fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
+    if (const char* key = c->weights.first_missing()) return fail(MIGAN_ERR_INVALID, "missing key '%s' in the state_dict", key);
+    if (int e = dev_set(c->device)) return fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
     const int R = c->resolution, c4 = channels(4);
     int rc = 0;
     for (int i = 0; i < MAP_LAYERS && !rc; ++i)
         rc = pack_dense(c, c->mapping[i], "mapping.fc" + std::to_string(i), i == 0 ? Z_DIM : W_DIM, W_DIM, true, MAP_LR, nullptr, nullptr);
-    if (!rc) rc = upload(c, H(c, "mapping.w_avg"), &c->w_avg);
+    if (!rc) rc = upload(c, c->weights.get("mapping.w_avg"), &c->w_avg);
     // encoder
     const std::string eR = "encoder.b" + std::to_string(R);
     if (!rc) rc = pack_conv(c, c->fromrgb, eR + ".fromrgb", 4, channels(R), 1, 1, 1, R, CONV_PLAIN, 0);
@@ -868,11 +776,11 @@ int comodgan_finalize_weights(comodgan_ctx* c) {
         rc = pack_conv(c, b.conv0, p + ".conv0", channels(r / 2), channels(r), 3, 2, 1, r, CONV_SYNTH, 2 * bi - 1);
         if (!rc) rc = pack_conv(c, b.conv1, p + ".conv1", channels(r), channels(r), 3, 1, 1, r, CONV_SYNTH, 2 * bi);
         if (!rc) rc = pack_conv(c, b.torgb, p + ".torgb", channels(r), 3, 1, 1, 1, r, CONV_TORGB, 2 * bi + 1);
-        if (!rc) fir_taps(H(c, p + ".resample_filter"), 4.f, b.img_fir);
+        if (!rc) fir_taps(c->weights.get(p + ".resample_filter"), 4.f, b.img_fir);
     }
     if (rc) return rc;
-    if (int e = dev_sync()) return fail(ERR_CUDA, "weight upload failed: %s", dev_err(e));
-    for (auto& v : c->host) std::vector<float>().swap(v);
+    if (int e = dev_sync()) return fail(MIGAN_ERR_CUDA, "weight upload failed: %s", dev_err(e));
+    c->weights.release_host();
     c->finalized = true;
     return 0;
 }
@@ -903,14 +811,14 @@ int comodgan_forward(comodgan_ctx* c, const float* x, const float* z, float* y, 
                      int truncation_cutoff, int noise_mode, const float* noise, void* workspace, size_t workspace_bytes,
                      void* stream) {
     if (int rc = check_ctx(c)) return rc;
-    if (!c->finalized) return fail(ERR_STATE, "forward before comodgan_finalize_weights");
-    if (!x || !z || !y || n <= 0) return fail(ERR_INVALID, "bad x / z / y / n");
-    if (noise_mode < 0 || noise_mode > 2) return fail(ERR_INVALID, "noise_mode must be 0 (none), 1 (const) or 2 (random)");
-    if (noise_mode == COMODGAN_NOISE_RANDOM && !noise) return fail(ERR_INVALID, "noise_mode random needs the noise planes");
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(ERR_WORKSPACE, "workspace null or not 256-byte aligned");
+    if (!c->finalized) return fail(MIGAN_ERR_STATE, "forward before comodgan_finalize_weights");
+    if (!x || !z || !y || n <= 0) return fail(MIGAN_ERR_INVALID, "bad x / z / y / n");
+    if (noise_mode < 0 || noise_mode > 2) return fail(MIGAN_ERR_INVALID, "noise_mode must be 0 (none), 1 (const) or 2 (random)");
+    if (noise_mode == COMODGAN_NOISE_RANDOM && !noise) return fail(MIGAN_ERR_INVALID, "noise_mode random needs the noise planes");
+    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(MIGAN_ERR_WORKSPACE, "workspace null or not 256-byte aligned");
     const size_t need = comodgan_workspace_bytes(c, n);
-    if (workspace_bytes < need) return fail(ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", need, workspace_bytes);
-    if (int e = dev_set(c->device)) return fail(ERR_CUDA, "cannot select device: %s", dev_err(e));
+    if (workspace_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", need, workspace_bytes);
+    if (int e = dev_set(c->device)) return fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
     Runner R;
     R.dry = false;
     R.base = static_cast<char*>(workspace);
@@ -937,12 +845,12 @@ int b200_conv2d_resample(const float* x, const float* w, const float* f, float* 
                          int groups, int flip_weight, int flip_filter, void* workspace, size_t workspace_bytes,
                          size_t* workspace_needed, int* out_h, int* out_w, void* stream) {
     if (n <= 0 || cin <= 0 || cout <= 0 || h <= 0 || wd <= 0 || kh <= 0 || kw <= 0 || up < 1 || down < 1 || groups < 1)
-        return fail(ERR_INVALID, "conv2d_resample: bad shape arguments");
-    if (cin % groups || cout % groups) return fail(ERR_INVALID, "conv2d_resample: channels not divisible by groups");
+        return fail(MIGAN_ERR_INVALID, "conv2d_resample: bad shape arguments");
+    if (cin % groups || cout % groups) return fail(MIGAN_ERR_INVALID, "conv2d_resample: channels not divisible by groups");
     const bool no_filter = (fh <= 0 || fw <= 0);                       // f=None in the reference: 1x1 identity
     if (no_filter) { fh = fw = 1; f = nullptr; }
-    if (fh * fw > 64) return fail(ERR_INVALID, "conv2d_resample: filter larger than 64 taps");
-    if (y != nullptr && (!x || !w || (!no_filter && !f))) return fail(ERR_INVALID, "conv2d_resample: null tensor");
+    if (fh * fw > 64) return fail(MIGAN_ERR_INVALID, "conv2d_resample: filter larger than 64 taps");
+    if (y != nullptr && (!x || !w || (!no_filter && !f))) return fail(MIGAN_ERR_INVALID, "conv2d_resample: null tensor");
     // filter taps live in kernel parameters: fetch them from the device once (tiny, synchronous)
     float taps_raw[64] = {1.f};
     if (f && y) {
@@ -951,7 +859,7 @@ int b200_conv2d_resample(const float* x, const float* w, const float* f, float* 
 #else
         cudaError_t e = cudaMemcpyAsync(taps_raw, f, sizeof(float) * fh * fw, cudaMemcpyDeviceToHost, (cudaStream_t)stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
-        if (e != cudaSuccess) return fail(ERR_CUDA, "conv2d_resample: reading the filter failed: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "conv2d_resample: reading the filter failed: %s", cudaGetErrorString(e));
 #endif
     }
     auto make_taps = [&](bool identity, float gain, float out[64], int& ofh, int& ofw) {
@@ -1053,9 +961,9 @@ int b200_conv2d_resample(const float* x, const float* w, const float* f, float* 
         if (pass == 0) {
             if (workspace_needed) *workspace_needed = R.peak;
             if (y == nullptr) return 0;
-            if (H <= 0 || W <= 0) return fail(ERR_INVALID, "conv2d_resample: empty output");
-            if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(ERR_WORKSPACE, "workspace null or not 256-byte aligned");
-            if (workspace_bytes < R.peak) return fail(ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", R.peak, workspace_bytes);
+            if (H <= 0 || W <= 0) return fail(MIGAN_ERR_INVALID, "conv2d_resample: empty output");
+            if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(MIGAN_ERR_WORKSPACE, "workspace null or not 256-byte aligned");
+            if (workspace_bytes < R.peak) return fail(MIGAN_ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", R.peak, workspace_bytes);
             continue;
         }
         R.launch(NhwcToNchwK{cur, y, H, W, C, C, 0}, (int64_t)n * C * H * W);

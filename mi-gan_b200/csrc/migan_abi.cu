@@ -18,14 +18,17 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/migan_b200.h"
 #include "abi_error.h"
 #include "kernels.h"
 #include "sepconv_tc.h"
+#include "weight_registry.h"
 
 using migan::fail;
+using migan::WeightRegistry;
 
 namespace {
 
@@ -45,24 +48,15 @@ void pack_dw_tc(const float* w, const float* b, int cin, float* w9, float* bias)
     for (int c = 0; c < cin; ++c) bias[c] = b[c] * S;
 }
 
-// pointwise [cout,cin] -> fp16 hi / lo [cout][cin] of w * 2^k2 (round to nearest); returns the epilogue's
-// 1 / (kActSplitScale * 2^k2).  The power-of-two scale puts the largest weight in [8192, 16384): hi and lo both stay
-// well inside fp16's normal range, and the scale is undone exactly in the epilogue.
+// pointwise [cout,cin] -> fp16 hi / lo [cout][cin] of w * 2^k (split_pow2); returns the epilogue's 1 / (kActSplitScale * 2^k)
 float pack_pw_split(const float* w, int cout, int cin, __half* hi, __half* lo) {
-    float maxabs = 0.f;
-    for (size_t i = 0; i < (size_t)cin * cout; ++i)
-        if (std::isfinite(w[i])) maxabs = std::max(maxabs, std::fabs(w[i]));
-    int k2 = 0;
-    if (maxabs > 0.f) k2 = (int)std::floor(std::log2(16384.0 / (double)maxabs));
-    k2 = std::max(-14, std::min(24, k2));
-    const float wscale = std::ldexp(1.0f, k2);
-    for (size_t i = 0; i < (size_t)cin * cout; ++i) {
-        const float s = w[i] * wscale;
-        const __half h = __float2half_rn(s);
-        hi[i] = h;
-        lo[i] = __float2half_rn(s - __half2float(h));
-    }
-    return 1.0f / (wscale * 64.0f /* kActSplitScale */);
+    return 1.0f / (migan::split_pow2(w, (size_t)cin * cout, hi, lo) * 64.0f /* kActSplitScale */);
+}
+
+// [rows][cols] -> [cols][rows]
+void transpose(const float* src, int rows, int cols, float* dst) {
+    for (int i = 0; i < rows; ++i)
+        for (int j = 0; j < cols; ++j) dst[(size_t)j * rows + i] = src[(size_t)i * cols + j];
 }
 
 // * sqrt 2: the up-sampling taps, noise planes and fromrgb weights that the fused prologues use with the gain folded in
@@ -75,21 +69,8 @@ void pack_torgb(const float* w, const float* b, const float* fir, int cout, floa
     memcpy(w_out, w, sizeof(float) * 3 * cout);
     memcpy(b_out, b, sizeof(float) * 3);
     b_out[3] = 0.f;
-    if (fir)
-        for (int c = 0; c < 3; ++c)
-            for (int k = 0; k < 16; ++k) fir_out[k * 3 + c] = fir[c * 16 + k];
+    if (fir) transpose(fir, 3, 16, fir_out);
 }
-
-struct WeightSpec {
-    std::string name;
-    int ndim;
-    int64_t shape[4];
-    int64_t numel() const {
-        int64_t n = 1;
-        for (int i = 0; i < ndim; ++i) n *= shape[i];
-        return n;
-    }
-};
 
 // One SeparableConv2d (migan_inference.py:106-170), packed for the kernels.
 struct SepConv {
@@ -129,6 +110,15 @@ enum StepKind { K_STEM, K_DW, K_DWDOWN, K_GEMM_SIMT, K_SEPCONV_TC, K_UP2, K_TORG
 
 constexpr int PTR_X = 1, PTR_Y = 2;  // flags: operand is the caller's x / y
 
+// A tensor a step produces that migan_set_tap can copy out (debug)
+struct Tap {
+    std::string name;   // empty: none
+    const float* src = nullptr;
+    int C = 0, H = 0, W = 0;
+    bool planar = false;   // NCHW already (images): copied as it is, else NHWC -> NCHW
+    int flags = 0;         // PTR_Y: src is the caller's y
+};
+
 struct Step {
     StepKind kind;
     const SepConv* L = nullptr;
@@ -153,16 +143,7 @@ struct Step {
     // roofline bookkeeping: algorithmic bytes = own input(s) read once + output written once
     std::string label;
     double alg_bytes = 0, flops = 0;
-    // tap (debug): tensor produced by this step
-    std::string tap;
-    const float* tap_src = nullptr;
-    int tapC = 0, tapH = 0, tapW = 0;
-    bool tap_planar = false;
-    int tap_flags = 0;
-    // second tap (fused torgb: the image produced by the same launch)
-    std::string tap2;
-    const float* tap2_src = nullptr;
-    int tap2C = 0, tap2H = 0, tap2W = 0, tap2_flags = 0;
+    Tap tap[2];   // [1]: the image of a fused torgb, produced by the same launch
 };
 
 struct Plan {
@@ -198,10 +179,7 @@ struct SlotRing {
 
 struct migan_ctx {
     int resolution = 0, device = 0;
-    std::vector<WeightSpec> specs;
-    std::map<std::string, int> spec_index;
-    std::vector<std::vector<float>> host;  // host copies, by spec index
-    std::vector<bool> provided;
+    WeightRegistry weights;
     bool finalized = false;
 
     std::vector<int> enc_res;  // R .. 4
@@ -288,30 +266,19 @@ int SlotRing::end(migan_ctx* ctx, cudaStream_t st) {
     return MIGAN_OK;
 }
 
-void add_spec(migan_ctx* c, const std::string& name, std::initializer_list<int64_t> shape) {
-    WeightSpec s;
-    s.name = name;
-    s.ndim = (int)shape.size();
-    int i = 0;
-    for (int64_t d : shape) s.shape[i++] = d;
-    for (; i < 4; ++i) s.shape[i] = 1;
-    c->spec_index[name] = (int)c->specs.size();
-    c->specs.push_back(s);
-}
-
 // Key order = the reference state_dict (own params, own buffers, then children; SURVEY.md 8b).
-void add_sepconv_specs(migan_ctx* c, const SepConv& L) {
+void add_sepconv_specs(WeightRegistry& reg, const SepConv& L) {
     if (L.noise) {
-        add_spec(c, L.p + "noise_strength", {});
-        add_spec(c, L.p + "noise_const", {L.res_out, L.res_out});
+        reg.add(L.p + "noise_strength", {});
+        reg.add(L.p + "noise_const", {L.res_out, L.res_out});
     }
-    add_spec(c, L.p + "conv1.weight", {L.cin, 1, 3, 3});
-    add_spec(c, L.p + "conv1.bias", {L.cin});
-    add_spec(c, L.p + "conv2.weight", {L.cout, L.cin, 1, 1});
-    if (L.down) add_spec(c, L.p + "downsample.filter.weight", {L.cin, 1, 4, 4});
+    reg.add(L.p + "conv1.weight", {L.cin, 1, 3, 3});
+    reg.add(L.p + "conv1.bias", {L.cin});
+    reg.add(L.p + "conv2.weight", {L.cout, L.cin, 1, 1});
+    if (L.down) reg.add(L.p + "downsample.filter.weight", {L.cin, 1, 4, 4});
     if (L.up) {
-        add_spec(c, L.p + "upsample.filter_const", {1, 1, L.res_out, L.res_out});
-        add_spec(c, L.p + "upsample.filter.weight", {L.cout, 1, 4, 4});
+        reg.add(L.p + "upsample.filter_const", {1, 1, L.res_out, L.res_out});
+        reg.add(L.p + "upsample.filter.weight", {L.cout, 1, 4, 4});
     }
 }
 
@@ -324,19 +291,48 @@ SepConv make_sepconv(const std::string& p, int cin, int cout, int res_in, bool d
     return L;
 }
 
-const std::vector<float>& W(const migan_ctx* c, const std::string& name) {
-    return c->host[c->spec_index.at(name)];
-}
-
-// Bump allocator over a host staging image of the device weight arena.
-struct ArenaBuilder {
-    std::vector<unsigned char> bytes;
-    size_t alloc(size_t n) {
-        size_t off = align_up(bytes.size(), 256);
-        bytes.resize(off + n, 0);
-        return off;
+// Host image of one device allocation of packed tables, each at a 256-byte aligned offset.  table() returns a zeroed
+// host table to fill and records the pointer that upload() sets to the table's device address.
+class ArenaBuilder {
+  public:
+    template <class T>
+    std::remove_const_t<T>* table(T** dst, size_t count) {
+        using U = std::remove_const_t<T>;
+        bytes_ = align_up(bytes_, 256);
+        tables_.push_back({reinterpret_cast<void**>(const_cast<U**>(dst)), bytes_, std::vector<unsigned char>(sizeof(U) * count)});
+        bytes_ += sizeof(U) * count;
+        return reinterpret_cast<U*>(tables_.back().host.data());
     }
+    // Allocates *dev, copies the image there and points every recorded pointer into it.
+    cudaError_t upload(void** dev) const {
+        std::vector<unsigned char> image(bytes_);
+        for (const Table& t : tables_) memcpy(image.data() + t.off, t.host.data(), t.host.size());
+        cudaError_t e = cudaMalloc(dev, bytes_);
+        if (e != cudaSuccess) return e;
+        e = cudaMemcpy(*dev, image.data(), bytes_, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { cudaFree(*dev); *dev = nullptr; return e; }
+        for (const Table& t : tables_) *t.dst = static_cast<unsigned char*>(*dev) + t.off;
+        return cudaSuccess;
+    }
+
+  private:
+    struct Table {
+        void** dst;
+        size_t off;
+        std::vector<unsigned char> host;
+    };
+    std::list<Table> tables_;   // a std::list: the host tables of one packing call are filled together
+    size_t bytes_ = 0;
 };
+
+// The kernels implement zero insertion: filter_const must be that pattern (migan_inference.py:83-85).
+int check_zero_insertion(const std::vector<float>& fc, int r, const std::string& prefix) {
+    for (int y = 0; y < r; ++y)
+        for (int x = 0; x < r; ++x)
+            if (fc[(size_t)y * r + x] != (((y | x) & 1) ? 0.f : 1.f))
+                return fail(MIGAN_ERR_INVALID, "%supsample.filter_const is not the zero-insertion pattern at (%d,%d)", prefix.c_str(), y, x);
+    return MIGAN_OK;
+}
 
 }  // namespace
 
@@ -373,15 +369,15 @@ int migan_create(int resolution, int device, migan_ctx** out) {
     for (size_t i = 0; i < c->syn_res.size(); ++i) {
         const int r = c->syn_res[i];
         const std::string p = "synthesis.b" + std::to_string(r) + ".";
-        add_sepconv_specs(c.get(), c->syn1[i]);
-        add_sepconv_specs(c.get(), c->syn2[i]);
-        add_spec(c.get(), p + "torgb.weight", {3, channels(r), 1, 1});
-        add_spec(c.get(), p + "torgb.bias", {3});
+        add_sepconv_specs(c->weights, c->syn1[i]);
+        add_sepconv_specs(c->weights, c->syn2[i]);
+        c->weights.add(p + "torgb.weight", {3, channels(r), 1, 1});
+        c->weights.add(p + "torgb.bias", {3});
         ToRgb t;
         t.p = p; t.c = channels(r); t.res = r; t.has_up = (i > 0);
         if (t.has_up) {
-            add_spec(c.get(), p + "upsample.filter_const", {1, 1, r, r});
-            add_spec(c.get(), p + "upsample.filter.weight", {3, 1, 4, 4});
+            c->weights.add(p + "upsample.filter_const", {1, 1, r, r});
+            c->weights.add(p + "upsample.filter.weight", {3, 1, 4, 4});
         }
         c->torgb.push_back(t);
     }
@@ -391,16 +387,14 @@ int migan_create(int resolution, int device, migan_ctx** out) {
         const bool last = (i + 1 == c->enc_res.size());
         const int ci = channels(r), cj = last ? ci : channels(c->enc_res[i + 1]);
         if (i == 0) {
-            add_spec(c.get(), p + "fromrgb.weight", {ci, 4, 1, 1});
-            add_spec(c.get(), p + "fromrgb.bias", {ci});
+            c->weights.add(p + "fromrgb.weight", {ci, 4, 1, 1});
+            c->weights.add(p + "fromrgb.bias", {ci});
         }
         c->enc1.push_back(make_sepconv(p + "conv1.", ci, ci, r, false, false, false));
         c->enc2.push_back(make_sepconv(p + "conv2.", ci, cj, r, !last, false, false));
-        add_sepconv_specs(c.get(), c->enc1.back());
-        add_sepconv_specs(c.get(), c->enc2.back());
+        add_sepconv_specs(c->weights, c->enc1.back());
+        add_sepconv_specs(c->weights, c->enc2.back());
     }
-    c->host.resize(c->specs.size());
-    c->provided.assign(c->specs.size(), false);
 
     if (device >= 0) {
         int ndev = 0;
@@ -440,79 +434,39 @@ int migan_destroy(migan_ctx* ctx) {
     return MIGAN_OK;
 }
 
-int migan_num_weights(const migan_ctx* ctx) { return ctx ? (int)ctx->specs.size() : 0; }
+int migan_num_weights(const migan_ctx* ctx) { return ctx ? ctx->weights.size() : 0; }
 
 int migan_weight_info(const migan_ctx* ctx, int index, const char** name, int* ndim, int64_t shape[4]) {
-    if (!ctx || index < 0 || index >= (int)ctx->specs.size()) return fail(MIGAN_ERR_INVALID, "bad weight index %d", index);
-    const WeightSpec& s = ctx->specs[index];
-    if (name) *name = s.name.c_str();
-    if (ndim) *ndim = s.ndim;
-    if (shape)
-        for (int i = 0; i < 4; ++i) shape[i] = s.shape[i];
-    return MIGAN_OK;
+    if (!ctx) return fail(MIGAN_ERR_INVALID, "null ctx");
+    return ctx->weights.info(index, name, ndim, shape);
 }
 
+// A re-upload is accepted: the weights take effect at the next migan_finalize_weights.
 int migan_set_weight(migan_ctx* ctx, const char* name, const float* host_data, int64_t numel) {
     if (!ctx || !name || !host_data) return fail(MIGAN_ERR_INVALID, "null argument");
-    auto it = ctx->spec_index.find(name);
-    if (it == ctx->spec_index.end()) return fail(MIGAN_ERR_INVALID, "unexpected key '%s' for resolution %d", name, ctx->resolution);
-    const WeightSpec& s = ctx->specs[it->second];
-    if (s.numel() != numel)
-        return fail(MIGAN_ERR_INVALID, "size mismatch for '%s': expected %lld elements, got %lld", name, (long long)s.numel(), (long long)numel);
-    ctx->host[it->second].assign(host_data, host_data + numel);
-    ctx->provided[it->second] = true;
+    if (int rc = ctx->weights.set(name, host_data, numel)) return rc;
     ctx->finalized = false;
     return MIGAN_OK;
 }
 
-static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vector<std::pair<void**, size_t>>& fix) {
+static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab) {
+    const WeightRegistry& wr = ctx->weights;
     const int cin = L.cin, cout = L.cout;
-    {   // depthwise taps [cin,1,3,3] -> [9][cin]
-        const std::vector<float>& w = W(ctx, L.p + "conv1.weight");
-        size_t off = ab.alloc(sizeof(float) * 9 * cin);
-        float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        for (int c = 0; c < cin; ++c)
-            for (int t = 0; t < 9; ++t) d[t * cin + c] = w[c * 9 + t];
-        fix.push_back({reinterpret_cast<void**>(&L.w9), off});
-    }
-    {
-        const std::vector<float>& b = W(ctx, L.p + "conv1.bias");
-        size_t off = ab.alloc(sizeof(float) * cin);
-        memcpy(ab.bytes.data() + off, b.data(), sizeof(float) * cin);
-        fix.push_back({reinterpret_cast<void**>(&L.bias), off});
-    }
-    {   // wgmma prologue: activation gain and fp16-split scale folded into the depthwise taps
-        const std::vector<float>& w = W(ctx, L.p + "conv1.weight");
-        const std::vector<float>& b = W(ctx, L.p + "conv1.bias");
-        size_t off = ab.alloc(sizeof(float) * 9 * cin);
-        size_t offb = ab.alloc(sizeof(float) * cin);
-        pack_dw_tc(w.data(), b.data(), cin, reinterpret_cast<float*>(ab.bytes.data() + off),
-                   reinterpret_cast<float*>(ab.bytes.data() + offb));
-        fix.push_back({reinterpret_cast<void**>(&L.w9_tc), off});
-        fix.push_back({reinterpret_cast<void**>(&L.bias_tc), offb});
-    }
-    {   // pointwise [cout,cin,1,1] -> fp32 [cin][cout] and fp16 hi/lo [cout][cin]
-        const std::vector<float>& w = W(ctx, L.p + "conv2.weight");
-        size_t off = ab.alloc(sizeof(float) * cin * cout);
-        float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        for (int o = 0; o < cout; ++o)
-            for (int k = 0; k < cin; ++k) d[(size_t)k * cout + o] = w[(size_t)o * cin + k];
-        fix.push_back({reinterpret_cast<void**>(&L.pw_t), off});
-        size_t off_hi = ab.alloc(sizeof(__half) * cin * cout);
-        size_t off_lo = ab.alloc(sizeof(__half) * cin * cout);
-        L.tc_inv_scale = pack_pw_split(w.data(), cout, cin, reinterpret_cast<__half*>(ab.bytes.data() + off_hi),
-                                       reinterpret_cast<__half*>(ab.bytes.data() + off_lo));
-        fix.push_back({reinterpret_cast<void**>(&L.pw_hi), off_hi});
-        fix.push_back({reinterpret_cast<void**>(&L.pw_lo), off_lo});
-    }
+    const std::vector<float>& dw = wr.get(L.p + "conv1.weight");
+    const std::vector<float>& db = wr.get(L.p + "conv1.bias");
+    const std::vector<float>& pw = wr.get(L.p + "conv2.weight");
+    transpose(dw.data(), cin, 9, ab.table(&L.w9, 9 * cin));   // depthwise taps [cin,1,3,3] -> [9][cin]
+    memcpy(ab.table(&L.bias, cin), db.data(), sizeof(float) * cin);
+    float* w9_tc = ab.table(&L.w9_tc, 9 * cin);   // wgmma prologue: activation gain and fp16-split scale folded in
+    pack_dw_tc(dw.data(), db.data(), cin, w9_tc, ab.table(&L.bias_tc, cin));
+    // pointwise [cout,cin,1,1] -> fp32 [cin][cout] and fp16 hi/lo [cout][cin]
+    transpose(pw.data(), cout, cin, ab.table(&L.pw_t, (size_t)cin * cout));
+    __half* pw_hi = ab.table(&L.pw_hi, (size_t)cin * cout);
+    L.tc_inv_scale = pack_pw_split(pw.data(), cout, cin, pw_hi, ab.table(&L.pw_lo, (size_t)cin * cout));
     if (L.down || L.up) {
         const int cf = L.down ? cin : cout;
-        const std::vector<float>& f = W(ctx, L.p + (L.down ? "downsample.filter.weight" : "upsample.filter.weight"));
-        size_t off = ab.alloc(sizeof(float) * 16 * cf);
-        float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        for (int c = 0; c < cf; ++c)
-            for (int t = 0; t < 16; ++t) d[t * cf + c] = f[c * 16 + t];
-        fix.push_back({reinterpret_cast<void**>(&L.fir16), off});
+        const std::vector<float>& f = wr.get(L.p + (L.down ? "downsample.filter.weight" : "upsample.filter.weight"));
+        transpose(f.data(), cf, 16, ab.table(&L.fir16, 16 * cf));
         if (L.up) {   // the fused prologue keeps the 16 taps in registers: they must not depend on the channel
             L.up_uniform = true;
             for (int c = 1; c < cf && L.up_uniform; ++c)
@@ -521,29 +475,14 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
             scale_sqrt2(f.data(), 16, L.up_taps_s2);
         }
     }
-    if (L.up) {
-        // The kernels implement zero insertion; check filter_const is that pattern (migan_inference.py:83-85).
-        const std::vector<float>& fc = W(ctx, L.p + "upsample.filter_const");
-        const int r = L.res_out;
-        for (int y = 0; y < r; ++y)
-            for (int x = 0; x < r; ++x) {
-                const float want = ((y | x) & 1) ? 0.f : 1.f;
-                if (fc[(size_t)y * r + x] != want)
-                    return fail(MIGAN_ERR_INVALID, "%supsample.filter_const is not the zero-insertion pattern at (%d,%d)", L.p.c_str(), y, x);
-            }
-    }
+    if (L.up)
+        if (int rc = check_zero_insertion(wr.get(L.p + "upsample.filter_const"), L.res_out, L.p)) return rc;
     if (L.noise) {
-        const std::vector<float>& nc = W(ctx, L.p + "noise_const");
-        const float ns = W(ctx, L.p + "noise_strength")[0];
-        size_t off = ab.alloc(sizeof(float) * nc.size());
-        float* d = reinterpret_cast<float*>(ab.bytes.data() + off);
-        for (size_t i = 0; i < nc.size(); ++i) d[i] = nc[i] * ns;  // migan_inference.py:166
-        fix.push_back({reinterpret_cast<void**>(&L.noise_dev), off});
-        if (L.up) {
-            size_t off2 = ab.alloc(sizeof(float) * nc.size());
-            scale_sqrt2(reinterpret_cast<const float*>(ab.bytes.data() + off), nc.size(), reinterpret_cast<float*>(ab.bytes.data() + off2));
-            fix.push_back({reinterpret_cast<void**>(&L.noise_s2_dev), off2});
-        }
+        const std::vector<float>& nc = wr.get(L.p + "noise_const");
+        const float ns = wr.get(L.p + "noise_strength")[0];
+        float* noise = ab.table(&L.noise_dev, nc.size());
+        for (size_t i = 0; i < nc.size(); ++i) noise[i] = nc[i] * ns;  // migan_inference.py:166
+        if (L.up) scale_sqrt2(noise, nc.size(), ab.table(&L.noise_s2_dev, nc.size()));
     }
     return MIGAN_OK;
 }
@@ -551,52 +490,31 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab, std::vecto
 int migan_finalize_weights(migan_ctx* ctx) {
     if (!ctx) return fail(MIGAN_ERR_INVALID, "null ctx");
     if (ctx->device < 0) return fail(MIGAN_ERR_CUDA, "context was created without a CUDA device: this library has no CPU path");
-    for (size_t i = 0; i < ctx->specs.size(); ++i)
-        if (!ctx->provided[i]) return fail(MIGAN_ERR_STATE, "missing key '%s'", ctx->specs[i].name.c_str());
+    const WeightRegistry& wr = ctx->weights;
+    if (const char* key = wr.first_missing()) return fail(MIGAN_ERR_STATE, "missing key '%s' in the state_dict", key);
     ArenaBuilder ab;
-    std::vector<std::pair<void**, size_t>> fix;
     {
         const std::string p = "encoder.b" + std::to_string(ctx->resolution) + ".fromrgb.";
-        const std::vector<float>& w = W(ctx, p + "weight");
-        const std::vector<float>& b = W(ctx, p + "bias");
-        size_t ow = ab.alloc(sizeof(float) * w.size());
-        memcpy(ab.bytes.data() + ow, w.data(), sizeof(float) * w.size());
-        size_t ob = ab.alloc(sizeof(float) * b.size());
-        memcpy(ab.bytes.data() + ob, b.data(), sizeof(float) * b.size());
-        fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_w), ow});
-        fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_b), ob});
-        size_t ow2 = ab.alloc(sizeof(float) * w.size()), ob2 = ab.alloc(sizeof(float) * b.size());
-        scale_sqrt2(w.data(), w.size(), reinterpret_cast<float*>(ab.bytes.data() + ow2));
-        scale_sqrt2(b.data(), b.size(), reinterpret_cast<float*>(ab.bytes.data() + ob2));
-        fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_w_s2), ow2});
-        fix.push_back({reinterpret_cast<void**>(&ctx->fromrgb_b_s2), ob2});
+        const std::vector<float>& w = wr.get(p + "weight");
+        const std::vector<float>& b = wr.get(p + "bias");
+        memcpy(ab.table(&ctx->fromrgb_w, w.size()), w.data(), sizeof(float) * w.size());
+        memcpy(ab.table(&ctx->fromrgb_b, b.size()), b.data(), sizeof(float) * b.size());
+        scale_sqrt2(w.data(), w.size(), ab.table(&ctx->fromrgb_w_s2, w.size()));
+        scale_sqrt2(b.data(), b.size(), ab.table(&ctx->fromrgb_b_s2, b.size()));
     }
     for (auto* vec : {&ctx->enc1, &ctx->enc2, &ctx->syn1, &ctx->syn2})
-        for (SepConv& L : *vec) {
-            int rc = pack_sepconv(ctx, L, ab, fix);
-            if (rc) return rc;
-        }
+        for (SepConv& L : *vec)
+            if (int rc = pack_sepconv(ctx, L, ab)) return rc;
     for (ToRgb& t : ctx->torgb) {
-        const std::vector<float>& w = W(ctx, t.p + "torgb.weight");
-        const std::vector<float>& b = W(ctx, t.p + "torgb.bias");
-        size_t ow = ab.alloc(sizeof(float) * w.size());
-        size_t ob = ab.alloc(sizeof(float) * 4);
-        fix.push_back({reinterpret_cast<void**>(&t.w), ow});
-        fix.push_back({reinterpret_cast<void**>(&t.b), ob});
-        const float* f = nullptr;
-        size_t of = 0;
+        const std::vector<float>& w = wr.get(t.p + "torgb.weight");
+        float* tw = ab.table(&t.w, w.size());
+        float* tb = ab.table(&t.b, 4);
+        const float* fir = nullptr;
         if (t.has_up) {
-            const std::vector<float>& fc = W(ctx, t.p + "upsample.filter_const");
-            for (int y = 0; y < t.res; ++y)
-                for (int x = 0; x < t.res; ++x)
-                    if (fc[(size_t)y * t.res + x] != (((y | x) & 1) ? 0.f : 1.f))
-                        return fail(MIGAN_ERR_INVALID, "%supsample.filter_const is not the zero-insertion pattern", t.p.c_str());
-            f = W(ctx, t.p + "upsample.filter.weight").data();
-            of = ab.alloc(sizeof(float) * 48);
-            fix.push_back({reinterpret_cast<void**>(&t.fir), of});
+            if (int rc = check_zero_insertion(wr.get(t.p + "upsample.filter_const"), t.res, t.p)) return rc;
+            fir = wr.get(t.p + "upsample.filter.weight").data();
         }
-        pack_torgb(w.data(), b.data(), f, (int)(w.size() / 3), reinterpret_cast<float*>(ab.bytes.data() + ow),
-                   reinterpret_cast<float*>(ab.bytes.data() + ob), f ? reinterpret_cast<float*>(ab.bytes.data() + of) : nullptr);
+        pack_torgb(w.data(), wr.get(t.p + "torgb.bias").data(), fir, t.c, tw, tb, fir ? ab.table(&t.fir, 48) : nullptr);
     }
     CUDA_TRY(cudaSetDevice(ctx->device));
     if (ctx->arena) {
@@ -604,9 +522,7 @@ int migan_finalize_weights(migan_ctx* ctx) {
         CUDA_TRY(cudaFree(ctx->arena));
         ctx->arena = nullptr;
     }
-    CUDA_TRY(cudaMalloc(&ctx->arena, ab.bytes.size()));
-    CUDA_TRY(cudaMemcpy(ctx->arena, ab.bytes.data(), ab.bytes.size(), cudaMemcpyHostToDevice));
-    for (auto& f : fix) *f.first = static_cast<unsigned char*>(ctx->arena) + f.second;
+    CUDA_TRY(ab.upload(&ctx->arena));
     ctx->plans.clear();  // pointers changed
     ctx->plan = nullptr;
     ctx->tap_cache_path = -1;   // the FIR taps decide which stages are fused, so the tap list may change with the weights
@@ -712,12 +628,37 @@ StagingSlot staging_slot(const migan_ctx* c, int n, bool u8, unsigned char* area
     return {reinterpret_cast<float*>(part[0]), reinterpret_cast<float*>(part[1]), part[2], part[3], part[4], bytes};
 }
 
+// Where a call that stages its tensors behind the forward's workspace puts them.
+struct Staging {
+    size_t ws;         // the forward's workspace bytes: the staging slots follow them
+    int slot;
+    StagingSlot buf;
+};
+
+// What the graph, fp32-host and uint8 calls check and bind before their copies: the arguments, room for the workspace and
+// the staging slots (one, or two when the call takes its slot from the context's `ring`), the slot and the context's device.
+int bind_staging(migan_ctx* ctx, bool args_ok, int n, void* workspace, size_t workspace_bytes, bool u8, SlotRing migan_ctx::*ring,
+                 const char* what, Staging* out) {
+    if (!ctx || !args_ok || !workspace) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
+    const size_t ws = migan_workspace_bytes(ctx, n), need = ws + (ring ? 2 : 1) * staging_slot(ctx, n, u8).bytes;
+    if (workspace_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "workspace too small for %s: %zu < %zu bytes", what, workspace_bytes, need);
+    out->ws = ws;
+    out->slot = ring ? (ctx->*ring).next() : 0;
+    out->buf = staging_slot(ctx, n, u8, static_cast<unsigned char*>(workspace) + ws, out->slot);
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    return MIGAN_OK;
+}
+
 // What the tensor-core kernel's prologue rebuilds on chip instead of reading it from HBM (sepconv_tc.h SepconvSource).
 struct Fuse {
     bool stem = false;              // input = fromrgb(x): the stem tensor never exists (encoder.b{R}.conv1)
     const SepConv* up = nullptr;    // input = lrelu_agc(up2(up_t) + noise) + skip, `up` = the preceding up-sampling layer
     const float* up_t = nullptr;    // its raw low-resolution 1x1 output
     bool defer_up = false;          // this layer IS the up-sampling layer: emit only the raw 1x1 conv
+    const ToRgb* rgb = nullptr;     // torgb in the epilogue: image = torgb(out) + up2(rgb_lo), written to rgb_out
+    const float* rgb_lo = nullptr;  // the previous level's image (null at 4 x 4)
+    float* rgb_out = nullptr;       // null: the caller's y, and the feature map is not stored (last level)
 };
 
 struct PlanBuilder {
@@ -739,15 +680,11 @@ struct PlanBuilder {
             if (i != a && i != b) return i;
         return 0;
     }
-    void set_tap(Step& s, const std::string& name, const float* src, int C, int H, int W, bool planar = false, int flags = 0) {
-        s.tap = name; s.tap_src = src; s.tapC = C; s.tapH = H; s.tapW = W; s.tap_planar = planar; s.tap_flags = flags;
-    }
 
     // Emit one SeparableConv2d reading `in` (NHWC [n,h,w,cin] at res_in's extent); `skip` is added after the
     // final activation (decoder conv1, migan_inference.py:304-305).  Returns the output pointer.
     // in_idx: scratch index holding `in` (or -1 if it is a feat buffer); out_fixed: write there if non-null.
     int emit_sepconv(const SepConv& L, const float* in, int in_idx, float* out_fixed, const float* skip, int& out_idx, float*& out_ptr,
-                     const migan::SepconvTcRgb* rgb = nullptr, const std::string& rgb_tap = std::string(), int rgb_flags = 0,
                      const Fuse& fuse = Fuse()) {
         const int t1 = other(in_idx), t2 = other(in_idx, t1);
         const bool tc = (path != MIGAN_PATH_SIMT);
@@ -769,15 +706,15 @@ struct PlanBuilder {
                 }
             } else {
                 s.out = S[t1]; gemm_in = S[t1];
-                set_tap(s, L.p + "down", S[t1], L.cin, epw.h, epw.w);
+                s.tap[0] = {L.p + "down", S[t1], L.cin, epw.h, epw.w};
             }
             steps.push_back(s);
         } else if (!tc) {
             Step s; s.kind = K_DW; s.L = &L; s.in = in; s.out = S[t1]; s.n = n; s.H = ein.h; s.W = ein.w; s.C = L.cin;
-            set_tap(s, L.p + "dw_act", S[t1], L.cin, ein.h, ein.w);
+            s.tap[0] = {L.p + "dw_act", S[t1], L.cin, ein.h, ein.w};
             steps.push_back(s);
             gemm_in = S[t1];
-        } else if (L.cout >= 512 && !rgb && L.res_in >= 64) {
+        } else if (L.cout >= 512 && !fuse.rgb && L.res_in >= 64) {
             // Cout spans 8 N tiles: a fused prologue would re-run the depthwise stage per tile, so run it once as its
             // own kernel and hand the GEMM a pre-split operand.  Below 64 x 64 the repeated prologue is cheap and
             // saves a launch, so those levels keep the depthwise stage in the tensor-core kernel.
@@ -808,7 +745,7 @@ struct PlanBuilder {
                 d.source = presplit ? migan::SEPCONV_SRC_SPLIT : migan::SEPCONV_SRC_NHWC;
                 d.in_f32 = s.in; d.a_hi = ghi; d.a_lo = glo;
                 d.w9 = L.w9_tc; d.bias = L.bias_tc; d.w_hi = L.pw_hi; d.w_lo = L.pw_lo; d.inv_scale = L.tc_inv_scale;
-                d.noise = s.noise; d.out = pw_out; d.n = n; d.h = epw.h; d.w = epw.w; d.cin = L.cin; d.cout = L.cout; d.act = s.act; d.rgb = rgb;
+                d.noise = s.noise; d.out = pw_out; d.n = n; d.h = epw.h; d.w = epw.w; d.cin = L.cin; d.cout = L.cout; d.act = s.act;
                 d.noise_pitch = noise_pitch(epw.w);
                 if (fuse.stem) {
                     d.source = migan::SEPCONV_SRC_STEM; d.in_f32 = nullptr;
@@ -821,16 +758,20 @@ struct PlanBuilder {
                     memcpy(d.up_taps, fuse.up->up_taps_s2, sizeof(d.up_taps));
                     s.aux2 = fuse.up_t; s.fused_up = true;
                 }
-                const char* err = migan::sepconv_tc_plan_ex(&s.tc, d);
-                if (rgb) {
-                    s.io_flags |= rgb_flags;
-                    s.tap2 = rgb_tap; s.tap2_src = rgb->img_out; s.tap2C = 3; s.tap2H = epw.h; s.tap2W = epw.w; s.tap2_flags = rgb_flags;
+                migan::SepconvTcRgb rgb;
+                if (fuse.rgb) {
+                    rgb = {fuse.rgb->w, fuse.rgb->b, fuse.rgb->fir, fuse.rgb_lo, fuse.rgb_out, fuse.rgb_out ? 1 : 0};
+                    d.rgb = &rgb;
+                    const int flags = fuse.rgb_out ? 0 : PTR_Y;
+                    s.io_flags |= flags;
+                    s.tap[1] = {fuse.rgb->p + "img", fuse.rgb_out, 3, epw.h, epw.w, true, flags};
                 }
-                if (err) return fail(MIGAN_ERR_CUDA, "wgmma plan for %s failed: %s", L.p.c_str(), err);
+                if (const char* err = migan::sepconv_tc_plan_ex(&s.tc, d))
+                    return fail(MIGAN_ERR_CUDA, "wgmma plan for %s failed: %s", L.p.c_str(), err);
             } else {
                 s.kind = K_GEMM_SIMT; s.in = gemm_in;
             }
-            if (!(rgb && !rgb->store_out)) set_tap(s, L.p + (raw ? "pw" : "out"), pw_out, L.cout, epw.h, epw.w);
+            if (!(fuse.rgb && !fuse.rgb_out)) s.tap[0] = {L.p + (raw ? "pw" : "out"), pw_out, L.cout, epw.h, epw.w};
             steps.push_back(s);
         }
         out_ptr = pw_out; out_idx = pw_idx;
@@ -842,12 +783,12 @@ struct PlanBuilder {
             Step s; s.kind = K_UP2; s.L = &L; s.in = pw_out; s.out = up_out; s.aux = skip;
             s.noise = nz.plain; s.noise_pitch = nz.pitch;
             s.n = n; s.H = epw.h; s.W = epw.w; s.C = L.cout;
-            set_tap(s, L.p + (skip ? "out_skip" : "out"), up_out, L.cout, eout.h, eout.w);
+            s.tap[0] = {L.p + (skip ? "out_skip" : "out"), up_out, L.cout, eout.h, eout.w};
             steps.push_back(s);
             out_ptr = up_out; out_idx = up_idx;
         } else if (skip) {
             Step s; s.kind = K_ADD; s.out = pw_out; s.aux = skip; s.n = n; s.H = eout.h; s.W = eout.w; s.C = L.cout;
-            set_tap(s, L.p + "out_skip", pw_out, L.cout, eout.h, eout.w);
+            s.tap[0] = {L.p + "out_skip", pw_out, L.cout, eout.h, eout.w};
             steps.push_back(s);
         }
         return MIGAN_OK;
@@ -893,7 +834,7 @@ struct PlanBuilder {
         const bool fuse_stem = tcp && R >= 16 && channels(R) < 512;
         if (!fuse_stem) {
             Step s; s.kind = K_STEM; s.io_flags = PTR_X; s.out = S[0]; s.n = n; s.H = H; s.W = W; s.C = channels(R);
-            set_tap(s, "encoder.b" + std::to_string(R) + ".fromrgb", S[0], channels(R), H, W);
+            s.tap[0] = {"encoder.b" + std::to_string(R) + ".fromrgb", S[0], channels(R), H, W};
             steps.push_back(s);
         }
         const float* cur = S[0];
@@ -903,7 +844,7 @@ struct PlanBuilder {
             int oi; float* op;
             Fuse f1;
             f1.stem = (i == 0 && fuse_stem);
-            int rc = emit_sepconv(c->enc1[i], cur, cur_idx, feat[r], nullptr, oi, op, nullptr, std::string(), 0, f1);  // feat = conv1(x)
+            int rc = emit_sepconv(c->enc1[i], cur, cur_idx, feat[r], nullptr, oi, op, f1);  // feat = conv1(x)
             if (rc) return rc;
             rc = emit_sepconv(c->enc2[i], feat[r], -1, nullptr, nullptr, oi, op);      // x = conv2(feat)
             if (rc) return rc;
@@ -934,27 +875,22 @@ struct PlanBuilder {
                 fuse_rgb = migan::sepconv_tc_fuses_rgb(q);
             }
             Fuse f1; f1.defer_up = fuse_up;
-            int rc = emit_sepconv(L1, cur, cur_idx, nullptr, feat[r], oi, op, nullptr, std::string(), 0, f1);  // x = conv1(x) + enc_feat
+            int rc = emit_sepconv(L1, cur, cur_idx, nullptr, feat[r], oi, op, f1);  // x = conv1(x) + enc_feat
             if (rc) return rc;
             cur = op; cur_idx = oi;
             Fuse f2;
             const float* in2 = cur;
             if (fuse_up) { f2.up = &L1; f2.up_t = cur; in2 = feat[r]; }   // scratch bookkeeping still protects `cur` (= t)
-            if (fuse_rgb) {
-                migan::SepconvTcRgb rgb;
-                rgb.w = T.w; rgb.b = T.b; rgb.fir = T.fir; rgb.img_lo = img_lo; rgb.img_out = img_out; rgb.store_out = last ? 0 : 1;
-                rc = emit_sepconv(c->syn2[i], in2, cur_idx, nullptr, nullptr, oi, op, &rgb, T.p + "img", last ? PTR_Y : 0, f2);
-                if (rc) return rc;
-                cur = op; cur_idx = oi;
-            } else {
-                rc = emit_sepconv(c->syn2[i], in2, cur_idx, nullptr, nullptr, oi, op, nullptr, std::string(), 0, f2);
-                if (rc) return rc;
-                cur = op; cur_idx = oi;
+            if (fuse_rgb) { f2.rgb = &T; f2.rgb_lo = img_lo; f2.rgb_out = img_out; }
+            rc = emit_sepconv(L2, in2, cur_idx, nullptr, nullptr, oi, op, f2);
+            if (rc) return rc;
+            cur = op; cur_idx = oi;
+            if (!fuse_rgb) {
                 Step s; s.kind = K_TORGB; s.T = &T; s.in = cur; s.n = n; s.H = ext(r).h; s.W = ext(r).w; s.C = channels(r);
                 s.aux = img_lo;
                 if (last) { s.io_flags = PTR_Y; s.out = nullptr; }
                 else s.out = img_out;
-                set_tap(s, T.p + "img", s.out, 3, s.H, s.W, true, last ? PTR_Y : 0);
+                s.tap[0] = {T.p + "img", s.out, 3, s.H, s.W, true, last ? PTR_Y : 0};
                 steps.push_back(s);
             }
             img_cur = img_next;
@@ -991,10 +927,10 @@ struct PlanBuilder {
                     s.flops = px * (2.0 * s.L->cin * s.L->cout + ((s.in || s.fused_stem) ? 18.0 * s.L->cin : 0.0));
                     if (s.fused_stem) { s.alg_bytes = px * (4 + s.L->cout) * f; s.flops += px * s.L->cin * 8.0; }
                     if (s.fused_up) { s.alg_bytes += px * 0.25 * s.L->cin * f; s.flops += px * s.L->cin * 8.0; }   // + the low-res tensor
-                    if (!s.tap2.empty()) {   // fused torgb: + image in/out, - feature map if it is not stored
+                    if (!s.tap[1].name.empty()) {   // fused torgb: + image in/out, - feature map if it is not stored
                         s.alg_bytes += px * 3.75 * f;
                         s.flops += px * s.L->cout * 6;
-                        if (s.tap.empty()) s.alg_bytes -= px * s.L->cout * f;
+                        if (s.tap[0].name.empty()) s.alg_bytes -= px * s.L->cout * f;
                     }
                     break;
                 case K_UP2: s.alg_bytes = px * s.C * f * (1 + 4 + (s.aux ? 4 : 0)); s.flops = px * 4 * s.C * 8; break;
@@ -1078,17 +1014,13 @@ int run_step(migan_ctx* ctx, Step& s, const float* x, float* y, cudaStream_t st)
         return fail(MIGAN_ERR_CUDA, "kernel launch (step %s) failed: %s [wgmma pipeline timeout record 0x%x]", s.label.c_str(),
                     cudaGetErrorString(e), (unsigned)migan::sepconv_tc_timeout_record(ctx->device));
     ctx->last_launches++;
-    if (ctx->tap_dst && !s.tap.empty() && s.tap == ctx->tap_name) {
-        const float* src = (s.tap_flags & PTR_Y) ? y : s.tap_src;
-        if (s.tap_planar)
-            e = cudaMemcpyAsync(ctx->tap_dst, src, sizeof(float) * (size_t)s.n * s.tapC * s.tapH * s.tapW, cudaMemcpyDeviceToDevice, st);
+    for (const Tap& t : s.tap) {
+        if (!ctx->tap_dst || t.name.empty() || t.name != ctx->tap_name) continue;
+        const float* src = (t.flags & PTR_Y) ? y : t.src;
+        if (t.planar)
+            e = cudaMemcpyAsync(ctx->tap_dst, src, sizeof(float) * (size_t)s.n * t.C * t.H * t.W, cudaMemcpyDeviceToDevice, st);
         else
-            e = migan::launch_nhwc_to_nchw(src, ctx->tap_dst, s.n, s.tapH, s.tapW, s.tapC, st);
-        if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "tap copy failed: %s", cudaGetErrorString(e));
-    }
-    if (ctx->tap_dst && !s.tap2.empty() && s.tap2 == ctx->tap_name) {
-        const float* src = (s.tap2_flags & PTR_Y) ? y : s.tap2_src;
-        e = cudaMemcpyAsync(ctx->tap_dst, src, sizeof(float) * (size_t)s.n * s.tap2C * s.tap2H * s.tap2W, cudaMemcpyDeviceToDevice, st);
+            e = migan::launch_nhwc_to_nchw(src, ctx->tap_dst, s.n, t.H, t.W, t.C, st);
         if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "tap copy failed: %s", cudaGetErrorString(e));
     }
     return MIGAN_OK;
@@ -1155,18 +1087,12 @@ size_t migan_graph_staging_bytes(const migan_ctx* ctx, int n) {
 
 int migan_forward_graph(migan_ctx* ctx, const float* x, float* y, int n, void* workspace, size_t workspace_bytes,
                         int path, void* stream) {
-    if (!ctx || !x || !y || !workspace) return fail(MIGAN_ERR_INVALID, "null argument");
-    if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
-    const size_t ws = migan_workspace_bytes(ctx, n);
-    if (workspace_bytes < ws + migan_graph_staging_bytes(ctx, n))
-        return fail(MIGAN_ERR_WORKSPACE, "workspace too small for the graph staging buffers: %zu < %zu bytes", workspace_bytes,
-                    ws + migan_graph_staging_bytes(ctx, n));
-    const size_t px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
-    const StagingSlot stage = staging_slot(ctx, n, false, static_cast<unsigned char*>(workspace) + ws);
-    float* xg = stage.x;
-    float* yg = stage.y;
+    Staging sg;
+    if (int rc = bind_staging(ctx, x && y, n, workspace, workspace_bytes, false, nullptr, "the graph staging buffers", &sg)) return rc;
+    const size_t ws = sg.ws, px = (size_t)n * ctx->resolution * ctx->resolution * sizeof(float);
+    float* xg = sg.buf.x;
+    float* yg = sg.buf.y;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaSetDevice(ctx->device));
     if (!ctx->graph_exec || ctx->graph_n != n || ctx->graph_path != path || ctx->graph_ws != workspace || ctx->profiling || ctx->tap_dst) {
         if (ctx->graph_exec) { cudaGraphExecDestroy(ctx->graph_exec); ctx->graph_exec = nullptr; }
         if (ctx->profiling || ctx->tap_dst) {   // per-launch events / taps need the plain launch sequence
@@ -1232,17 +1158,13 @@ size_t migan_host_staging_bytes(const migan_ctx* ctx, int n) {
 // collects them with migan_host_wait).  Within a call the batch is split into micro-batches for the same reason.
 static int forward_host_enqueue(migan_ctx* ctx, const float* x_host, float* y_host, int n, void* workspace,
                                 size_t workspace_bytes, int path, void* stream, int* slot_out) {
-    if (!ctx || !x_host || !y_host || !workspace) return fail(MIGAN_ERR_INVALID, "null argument");
-    if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
-    const size_t ws = migan_workspace_bytes(ctx, n);
-    if (workspace_bytes < ws + migan_host_staging_bytes(ctx, n))
-        return fail(MIGAN_ERR_WORKSPACE, "workspace too small for host staging: %zu < %zu bytes", workspace_bytes,
-                    ws + migan_host_staging_bytes(ctx, n));
+    Staging sg;
+    if (int rc = bind_staging(ctx, x_host && y_host, n, workspace, workspace_bytes, false, &migan_ctx::host_ring, "host staging", &sg))
+        return rc;
     SlotRing& ring = ctx->host_ring;
-    const int slot = ring.next();
-    const StagingSlot stage = staging_slot(ctx, n, false, static_cast<unsigned char*>(workspace) + ws, slot);
+    const int slot = sg.slot;
+    const StagingSlot& stage = sg.buf;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaSetDevice(ctx->device));
     // Micro-batch pipeline: H2D of micro-batch k+1 and D2H of k-1 overlap the kernels of k (three streams).
     // The small-resolution layers cost a fixed time per forward, so the split is kept coarse.
     // Synchronous call (one batch, then wait): split it so the copies of one half overlap the kernels of the other
@@ -1266,7 +1188,7 @@ static int forward_host_enqueue(migan_ctx* ctx, const float* x_host, float* y_ho
     int launches = 0;
     for (int k = 0; k < M; ++k) {
         CUDA_TRY(cudaStreamWaitEvent(st, ev[2 * k], 0));
-        int rc = migan_forward(ctx, stage.x + k * xs, stage.y + k * ys, m, workspace, ws, path, stream);
+        int rc = migan_forward(ctx, stage.x + k * xs, stage.y + k * ys, m, workspace, sg.ws, path, stream);
         if (rc) return rc;
         launches += ctx->last_launches;
         CUDA_TRY(cudaEventRecord(ev[2 * k + 1], st));
@@ -1302,19 +1224,16 @@ size_t migan_u8_staging_bytes(const migan_ctx* ctx, int n) {
 // two-slot scheme as the fp32 host call: the copies of call c+1 / c-1 run under the kernels of call c.
 static int forward_u8_enqueue(migan_ctx* ctx, const uint8_t* img_host, const uint8_t* mask_host, uint8_t* out_host, int n,
                               void* workspace, size_t workspace_bytes, int path, void* stream, int* slot_out) {
-    if (!ctx || !img_host || !mask_host || !out_host || !workspace) return fail(MIGAN_ERR_INVALID, "null argument");
-    if (n <= 0) return fail(MIGAN_ERR_INVALID, "batch size must be positive, got %d", n);
-    const size_t ws = migan_workspace_bytes(ctx, n);
-    if (workspace_bytes < ws + migan_u8_staging_bytes(ctx, n))
-        return fail(MIGAN_ERR_WORKSPACE, "workspace too small for uint8 staging: %zu < %zu bytes", workspace_bytes,
-                    ws + migan_u8_staging_bytes(ctx, n));
+    Staging sg;
+    if (int rc = bind_staging(ctx, img_host && mask_host && out_host, n, workspace, workspace_bytes, true, &migan_ctx::u8_ring,
+                              "uint8 staging", &sg))
+        return rc;
     const int R = ctx->resolution;
     const size_t px = (size_t)n * R * R;
     SlotRing& ring = ctx->u8_ring;
-    const int slot = ring.next();
-    const StagingSlot stage = staging_slot(ctx, n, true, static_cast<unsigned char*>(workspace) + ws, slot);
+    const int slot = sg.slot;
+    const StagingSlot& stage = sg.buf;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaSetDevice(ctx->device));
     if (int rc = ring.begin(ctx, stage.x, st)) return rc;
     const SlotRing::Slot& ev = ring.slot[slot];
     CUDA_TRY(cudaMemcpyAsync(stage.img, img_host, 3 * px, cudaMemcpyHostToDevice, ctx->s_in));
@@ -1322,7 +1241,7 @@ static int forward_u8_enqueue(migan_ctx* ctx, const uint8_t* img_host, const uin
     CUDA_TRY(cudaEventRecord(ev.in, ctx->s_in));
     CUDA_TRY(cudaStreamWaitEvent(st, ev.in, 0));
     CUDA_TRY((cudaError_t)migan::launch_preprocess_u8(stage.img, stage.mask, stage.x, n, R, R, st));
-    if (int rc = migan_forward(ctx, stage.x, stage.y, n, workspace, ws, path, stream)) return rc;
+    if (int rc = migan_forward(ctx, stage.x, stage.y, n, workspace, sg.ws, path, stream)) return rc;
     CUDA_TRY((cudaError_t)migan::launch_postprocess_u8(stage.y, stage.img, stage.mask, stage.out, n, R, R, st));
     ctx->last_launches += 2;
     CUDA_TRY(cudaEventRecord(ev.compute_done, st));   // recorded again by ring.end() at the same point of st
@@ -1441,10 +1360,9 @@ int migan_tap_info(const migan_ctx* ctx, int path, int index, const char** name,
         int rc = pb.build();
         if (rc) return rc;
         cache.clear();
-        for (Step& s : pb.steps) {
-            if (!s.tap.empty()) cache.push_back({s.tap, {s.tapC, s.tapH, s.tapW}});
-            if (!s.tap2.empty()) cache.push_back({s.tap2, {s.tap2C, s.tap2H, s.tap2W}});
-        }
+        for (const Step& s : pb.steps)
+            for (const Tap& t : s.tap)
+                if (!t.name.empty()) cache.push_back({t.name, {t.C, t.H, t.W}});
         mctx->tap_cache_path = path;
     }
     if (index < 0 || index >= (int)cache.size()) return MIGAN_ERR_INVALID;
@@ -1513,35 +1431,33 @@ int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate
         (stem && (st_w.empty() || st_b.empty())) || (io->torgb && (rgb_w.empty() || rgb_b.empty())) ||
         (up && io->up_noise && up_noise.empty()) || (io->torgb && io->img_lo && rgb_fir.empty()))
         return fail(MIGAN_ERR_INVALID, "sepconv_tc: an operand the source needs is missing or unreadable");
-    // packed tables, one host buffer -> one device allocation
-    std::vector<unsigned char> host;
-    auto alloc = [&](size_t bytes) { const size_t off = host.size(); host.resize(off + align_up(bytes, 256)); return off; };
-    const size_t o_w9 = alloc(sizeof(float) * 9 * cin), o_b = alloc(sizeof(float) * cin);
-    const size_t o_hi = alloc(sizeof(__half) * cc), o_lo = alloc(sizeof(__half) * cc);
-    const size_t o_sw = alloc(sizeof(float) * st_w.size()), o_sb = alloc(sizeof(float) * st_b.size());
-    const size_t o_nz = alloc(sizeof(float) * up_noise.size());
-    const size_t o_rw = alloc(sizeof(float) * 3 * cout), o_rb = alloc(sizeof(float) * 4), o_rf = alloc(sizeof(float) * 48);
-    auto hf = [&](size_t off) { return reinterpret_cast<float*>(host.data() + off); };
-    if (dwsrc) pack_dw_tc(dw_w.data(), dw_b.data(), cin, hf(o_w9), hf(o_b));
-    d.inv_scale = pack_pw_split(pw_w.data(), cout, cin, reinterpret_cast<__half*>(host.data() + o_hi), reinterpret_cast<__half*>(host.data() + o_lo));
-    if (stem) { scale_sqrt2(st_w.data(), st_w.size(), hf(o_sw)); scale_sqrt2(st_b.data(), st_b.size(), hf(o_sb)); }
+    // packed as migan_finalize_weights packs them, into one device allocation
+    ArenaBuilder ab;
+    if (dwsrc) {
+        float* w9 = ab.table(&d.w9, 9 * (size_t)cin);
+        pack_dw_tc(dw_w.data(), dw_b.data(), cin, w9, ab.table(&d.bias, cin));
+    }
+    __half* w_hi = ab.table(&d.w_hi, cc);
+    d.inv_scale = pack_pw_split(pw_w.data(), cout, cin, w_hi, ab.table(&d.w_lo, cc));
+    if (stem) {
+        scale_sqrt2(st_w.data(), st_w.size(), ab.table(&d.stem_w, st_w.size()));
+        scale_sqrt2(st_b.data(), st_b.size(), ab.table(&d.stem_b, st_b.size()));
+    }
     if (up) scale_sqrt2(up_fir.data(), 16, d.up_taps);
-    if (!up_noise.empty()) scale_sqrt2(up_noise.data(), up_noise.size(), hf(o_nz));
-    if (io->torgb) pack_torgb(rgb_w.data(), rgb_b.data(), rgb_fir.empty() ? nullptr : rgb_fir.data(), cout, hf(o_rw), hf(o_rb), hf(o_rf));
-    unsigned char* dbuf = nullptr;
-    CUDA_TRY(cudaMalloc(&dbuf, host.size()));
-    std::unique_ptr<unsigned char, decltype(&cudaFree)> hold(dbuf, &cudaFree);
-    CUDA_TRY(cudaMemcpy(dbuf, host.data(), host.size(), cudaMemcpyHostToDevice));
-    auto df = [&](size_t off) { return reinterpret_cast<float*>(dbuf + off); };
+    if (!up_noise.empty()) scale_sqrt2(up_noise.data(), up_noise.size(), ab.table(&d.up_noise, up_noise.size()));
+    if (io->torgb) {
+        float* w = ab.table(&rgb.w, 3 * (size_t)cout);
+        float* b = ab.table(&rgb.b, 4);
+        pack_torgb(rgb_w.data(), rgb_b.data(), rgb_fir.empty() ? nullptr : rgb_fir.data(), cout, w, b, ab.table(&rgb.fir, 48));
+    }
+    void* dbuf = nullptr;
+    CUDA_TRY(ab.upload(&dbuf));
+    std::unique_ptr<void, decltype(&cudaFree)> hold(dbuf, &cudaFree);
     d.in_f32 = io->in;
     d.a_hi = static_cast<const __half*>(io->a_hi); d.a_lo = static_cast<const __half*>(io->a_lo);
-    if (dwsrc) { d.w9 = df(o_w9); d.bias = df(o_b); }
-    d.w_hi = reinterpret_cast<const __half*>(dbuf + o_hi); d.w_lo = reinterpret_cast<const __half*>(dbuf + o_lo);
     d.noise = io->noise; d.out = io->out;
-    if (up) { d.up_t = io->up_t; d.up_noise = up_noise.empty() ? nullptr : df(o_nz); }
-    if (stem) { d.stem_w = df(o_sw); d.stem_b = df(o_sb); }
+    if (up) d.up_t = io->up_t;
     if (io->torgb) {
-        rgb.w = df(o_rw); rgb.b = df(o_rb); rgb.fir = df(o_rf);
         rgb.img_lo = io->img_lo; rgb.img_out = io->img_out; rgb.store_out = io->store_out;
         if (!io->img_out) return fail(MIGAN_ERR_INVALID, "sepconv_tc: torgb needs img_out");
     }

@@ -201,15 +201,15 @@ def _conv2d_resample_general(x, w, f, up, down, padding, groups, flip_weight, fl
     px0, px1, py0, py1 = padding
     args = [n, cin, h, wd, cout, kh, kw, fh, fw, up, down, px0, px1, py0, py1, groups, int(bool(flip_weight)), int(bool(flip_filter))]
     need, oh, ow = ctypes.c_size_t(), ctypes.c_int(), ctypes.c_int()
-    _abi.check_comod(lib.b200_conv2d_resample(None, None, None, None, *args, None, 0, ctypes.byref(need), ctypes.byref(oh),
-                                              ctypes.byref(ow), None))
+    _abi.check(lib.b200_conv2d_resample(None, None, None, None, *args, None, 0, ctypes.byref(need), ctypes.byref(oh),
+                                        ctypes.byref(ow), None))
     y = torch.empty((n, cout, oh.value, ow.value), dtype=torch.float32, device=x.device)
     raw = torch.empty(need.value + 1024, dtype=torch.uint8, device=x.device)
     off = (-raw.data_ptr()) % 1024
     with _guard(x.device):
-        _abi.check_comod(lib.b200_conv2d_resample(x.data_ptr(), w.data_ptr(), f2d.data_ptr() if f2d is not None else None,
-                                                  y.data_ptr(), *args, raw.data_ptr() + off, need.value, None, None, None,
-                                                  _stream(x)))
+        _abi.check(lib.b200_conv2d_resample(x.data_ptr(), w.data_ptr(), f2d.data_ptr() if f2d is not None else None,
+                                            y.data_ptr(), *args, raw.data_ptr() + off, need.value, None, None, None,
+                                            _stream(x)))
     return y
 
 
