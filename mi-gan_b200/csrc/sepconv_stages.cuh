@@ -112,60 +112,64 @@ SC_DEV uint32_t a_off(int m, uint32_t j) { return (uint32_t)(m >> 3) * 1024u + (
 // ---------------------------------------------------------------------------------------------------------------
 // Depthwise 3x3 + bias + lrelu_agc on one 32-channel chunk -> its half of the A operand K block (fp16 hi/lo).
 // The taps / bias carry S = kSplit * sqrt(2):  S * clamp(lrelu(v) * sqrt2, +-256) == clamp(max(v', .2 v'), +-256 kSplit).
-// Worker = (column, 4-channel vector); it slides a 3x3 window down the TH rows: 3 LDS.128 per output row, all
-// offsets compile-time.  SeparableConv2d.conv1 + activation, migan_inference.py:155-157.
+// Worker = (2 adjacent columns, 4-channel vector, RH = 4 rows); it slides a 3 x 4 input window down its rows: 4 LDS.128
+// per input row for 2 output columns, (RH + 2) * 4 = 24 per 8 outputs (one column per worker took 30), all offsets
+// compile-time.  Every output is the 9-tap chain from the bias in the same order (tap column outer, tap row inner).
+// SeparableConv2d.conv1 + activation, migan_inference.py:155-157.
 //   sin   IN stage (float4 units)      w9/bias  [9][cin] / [cin] tap tables (shared memory or global)
 //   g     which 32-channel half of the 64-channel K block this chunk is (0/1);  cg0 = first channel of the chunk
 // ---------------------------------------------------------------------------------------------------------------
 template <int TN, int TH, int TW>
 SC_DEV void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_hi, uint8_t* __restrict__ a_lo,
                            const float* __restrict__ w9, const float* __restrict__ bias, int cin, int cg0, int g, int tg) {
-    constexpr int NCOLS = TN * TW;
+    constexpr int NPAIR = TN * TW / 2;                     // column pairs of the tile (8 at 16x8 / 8x8, 16 at 4x4)
+    constexpr int RH = 4;                                  // output rows per worker
+    constexpr int NSEG = TH / RH;                          // row segments per column pair (2, or 1 at 4x4)
     constexpr int ROW_F4 = (TW + 2) * 8;                   // float4 per halo'd input row (8 float4 / pixel)
+    static_assert(NPAIR * NSEG * 8 == 128, "one work item per prologue thread");
+    const int cvec = tg & 7, wk = tg >> 3;
+    // Swapping bits 0 and 1 of the worker index puts pairs 2 apart (columns 4 apart) in each half-warp: at 16x8 and 8x8
+    // tiles the two halves of a warp's STS.64 then land on distinct swizzle rows (bit 2 of m & 7 differs), 2 wavefronts.
+    const int u = (wk & ~3) | ((wk & 1) << 1) | ((wk >> 1) & 1);
+    const int pair = u % NPAIR, seg = u / NPAIR;
+    const int img_l = (2 * pair) / TW, x = (2 * pair) % TW, y0 = seg * RH;
+    const int cg = cg0 + cvec * 4;
+    F4 w[9];
 #pragma unroll
-    for (int rep = 0; rep < (NCOLS * 8 + 127) / 128; ++rep) {
-        const int item = tg + rep * 128;
-        const int cvec = item & 7, colidx = item >> 3;
-        const int col = (colidx & 3) * (NCOLS >> 2) + (colidx >> 2);   // spreads a warp over 4 distinct swizzle rows
-        const int img_l = col / TW, x = col % TW;
-        const int cg = cg0 + cvec * 4;
-        F4 w[9];
+    for (int t = 0; t < 9; ++t) w[t] = as_f4(*reinterpret_cast<const f4*>(w9 + t * cin + cg));
+    const F4 bv = as_f4(*reinterpret_cast<const f4*>(bias + cg));
+    const f4* base = sin + ((img_l * (TH + 2) + y0) * (TW + 2) + x) * 8 + cvec;
+    const uint32_t jchunk = (uint32_t)(g * 4 + (cvec >> 1));
+    const uint32_t sub = (uint32_t)(cvec & 1) * 8;
+    // One output row per step, both columns: two independent accumulation chains; the input rows rotate through r0..r2.
+    F4 r0[4], r1[4], r2[4];
 #pragma unroll
-        for (int t = 0; t < 9; ++t) w[t] = as_f4(*reinterpret_cast<const f4*>(w9 + t * cin + cg));
-        const F4 bv = as_f4(*reinterpret_cast<const f4*>(bias + cg));
-        const f4* base = sin + (img_l * (TH + 2) * (TW + 2) + x) * 8 + cvec;
-        const uint32_t jchunk = (uint32_t)(g * 4 + (cvec >> 1));
-        const uint32_t sub = (uint32_t)(cvec & 1) * 8;
-        // Two output rows per step: four independent accumulation chains, loads of both rows issued up front.
-        F4 r0[3], r1[3], r2[3], r3[3];
+    for (int d = 0; d < 4; ++d) { r0[d] = as_f4(base[d * 8]); r1[d] = as_f4(base[ROW_F4 + d * 8]); }
 #pragma unroll
-        for (int d = 0; d < 3; ++d) { r0[d] = as_f4(base[d * 8]); r1[d] = as_f4(base[ROW_F4 + d * 8]); }
+    for (int y = 0; y < RH; ++y) {
 #pragma unroll
-        for (int y = 0; y < TH; y += 2) {
+        for (int d = 0; d < 4; ++d) r2[d] = as_f4(base[(y + 2) * ROW_F4 + d * 8]);
+        F4 a = bv, b = bv;                                 // columns x, x + 1
 #pragma unroll
-            for (int d = 0; d < 3; ++d) { r2[d] = as_f4(base[(y + 2) * ROW_F4 + d * 8]); r3[d] = as_f4(base[(y + 3) * ROW_F4 + d * 8]); }
-            F4 a = bv, b = bv;
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                fma4p(a, w[d], r0[d]);     fma4p(b, w[d], r1[d]);
-                fma4p(a, w[3 + d], r1[d]); fma4p(b, w[3 + d], r2[d]);
-                fma4p(a, w[6 + d], r2[d]); fma4p(b, w[6 + d], r3[d]);
-            }
-            constexpr float kLim = kClamp * kSplit;
-            uint32_t hi0x, hi0y, lo0x, lo0y, hi1x, hi1y, lo1x, lo1y;
-            split_pack2(unpk(act_pair(a.lo, kLim)), hi0x, lo0x);
-            split_pack2(unpk(act_pair(b.lo, kLim)), hi1x, lo1x);
-            split_pack2(unpk(act_pair(a.hi, kLim)), hi0y, lo0y);
-            split_pack2(unpk(act_pair(b.hi, kLim)), hi1y, lo1y);
-            const int m0 = (img_l * TH + y) * TW + x, m1 = m0 + TW;      // rows of the M tile
-            const uint32_t off0 = a_off(m0, jchunk) + sub, off1 = a_off(m1, jchunk) + sub;
-            st_u2(a_hi + off0, hi0x, hi0y);
-            st_u2(a_lo + off0, lo0x, lo0y);
-            st_u2(a_hi + off1, hi1x, hi1y);
-            st_u2(a_lo + off1, lo1x, lo1y);
-#pragma unroll
-            for (int d = 0; d < 3; ++d) { r0[d] = r2[d]; r1[d] = r3[d]; }
+        for (int d = 0; d < 3; ++d) {
+            fma4p(a, w[d], r0[d]);     fma4p(b, w[d], r0[d + 1]);
+            fma4p(a, w[3 + d], r1[d]); fma4p(b, w[3 + d], r1[d + 1]);
+            fma4p(a, w[6 + d], r2[d]); fma4p(b, w[6 + d], r2[d + 1]);
         }
+        constexpr float kLim = kClamp * kSplit;
+        uint32_t hi0x, hi0y, lo0x, lo0y, hi1x, hi1y, lo1x, lo1y;
+        split_pack2(unpk(act_pair(a.lo, kLim)), hi0x, lo0x);
+        split_pack2(unpk(act_pair(b.lo, kLim)), hi1x, lo1x);
+        split_pack2(unpk(act_pair(a.hi, kLim)), hi0y, lo0y);
+        split_pack2(unpk(act_pair(b.hi, kLim)), hi1y, lo1y);
+        const int m0 = (img_l * TH + y0 + y) * TW + x, m1 = m0 + 1;      // rows of the M tile
+        const uint32_t off0 = a_off(m0, jchunk) + sub, off1 = a_off(m1, jchunk) + sub;
+        st_u2(a_hi + off0, hi0x, hi0y);
+        st_u2(a_lo + off0, lo0x, lo0y);
+        st_u2(a_hi + off1, hi1x, hi1y);
+        st_u2(a_lo + off1, lo1x, lo1y);
+#pragma unroll
+        for (int d = 0; d < 4; ++d) { r0[d] = r1[d]; r1[d] = r2[d]; }
     }
 }
 

@@ -382,20 +382,28 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
             ep_nz = reinterpret_cast<const float*>(smem_gen + p.off_ep + re.stage * p.ep_stage_stride);
             ep_img = ep_nz + p.ep_off_img / 4;
         }
+        // pixel of the thread's row r (0..3): image / row / column inside the tile and in the tensor
+        struct RowPx { int limg, ly, lx, pimg, poy, pox; bool valid; };
+        auto row_px = [&](int r) {
+            const int m = (r >> 1) * 64 + wq * 16 + (lane >> 2) + 8 * (r & 1);
+            RowPx q;
+            q.limg = m >> (p.l_tw + p.l_th); q.ly = (m >> p.l_tw) & (p.tile_h - 1); q.lx = m & (p.tile_w - 1);
+            q.pimg = tc.n0 + q.limg; q.poy = tc.y0 + q.ly; q.pox = tc.x0 + q.lx;
+            q.valid = q.pimg < p.n && q.poy < p.H && q.pox < p.W;   // partial tiles at the right / bottom edge
+            return q;
+        };
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
             const int h = r >> 1, i = r & 1;
-            const int m = h * 64 + wq * 16 + (lane >> 2) + 8 * i;
-            const int limg = m >> (p.l_tw + p.l_th), ly = (m >> p.l_tw) & (p.tile_h - 1), lx = m & (p.tile_w - 1);
-            const int pimg = tc.n0 + limg, poy = tc.y0 + ly, pox = tc.x0 + lx;
-            const bool valid = pimg < p.n && poy < p.H && pox < p.W;   // partial tiles at the right / bottom edge
+            const RowPx q = row_px(r);
+            const int ly = q.ly, lx = q.lx, pimg = q.pimg, poy = q.poy, pox = q.pox;
+            const bool valid = q.valid;
             // The NZ window is zero past the extents; rows of images past n read some noise but are never stored.
             float nz;
             if constexpr (kRing) nz = p.noise ? ep_nz[(ly << p.l_tw) + lx] : 0.f;
             else nz = (p.noise && valid) ? __ldg(p.noise + poy * p.noise_pitch + pox) : 0.f;
             const float nz_g = nz * kActGain;
             float* out_px = p.out + (((size_t)pimg * p.H + poy) * p.W + pox) * p.cout + chan0 + 2 * (lane & 3);
-            float s0 = 0.f, s1 = 0.f, s2 = 0.f;      // torgb partial sums over this thread's channels
 #pragma unroll
             for (int jj = 0; jj < NT / 8; ++jj) {
                 float o[2];
@@ -408,28 +416,45 @@ __device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t smem_base
                     } else {
                         o[c] = fmaf(v, p.inv_scale, nz);
                     }
-                }
-                if (p.torgb) {                       // 1x1 conv Cout -> 3 on the activated row (the CTA tile holds all of cout)
-                    const int ch = chan0 + 8 * jj + 2 * (lane & 3);
-                    s0 = fmaf(o[1], s_rgb[ch + 1], fmaf(o[0], s_rgb[ch], s0));
-                    s1 = fmaf(o[1], s_rgb[p.cout + ch + 1], fmaf(o[0], s_rgb[p.cout + ch], s1));
-                    s2 = fmaf(o[1], s_rgb[2 * p.cout + ch + 1], fmaf(o[0], s_rgb[2 * p.cout + ch], s2));
+                    acc[h][jj * 4 + i * 2 + c] = o[c];   // the activated row, for torgb below
                 }
                 if (p.store_out && valid) *reinterpret_cast<float2*>(out_px + 8 * jj) = make_float2(o[0], o[1]);
             }
-            if (p.torgb) {
-                // img = upsample(img_lo) + (torgb(x) + b)   (migan_inference.py:308-313); planar NCHW.  The quad holds the
-                // pixel's channels of this N tile: sum its partials; lane k of the quad owns colour k of the row and adds
-                // the N tiles up in registers.  After the group's last N tile it writes the pixel.
+        }
+        if (p.torgb) {
+            // 1x1 conv Cout -> 3 on the activated rows (the CTA tile holds all of cout).  One pass per colour, channel pairs
+            // outside and the four rows inside, so each weight pair is read from shared memory once per tile, not once per
+            // row; every row still adds the pairs in jj order.  (All three colours in one pass would hold 12 partial sums
+            // and spill under the 184-register ceiling.)  The quad holds the pixel's channels of this N tile: it sums its
+            // partials, and lane k keeps colour k (lane 3 a copy of colour 2).
+            const int k = lane & 3;
+            float sk[4];
 #pragma unroll
-                for (int x = 1; x < 4; x <<= 1) {
-                    s0 += __shfl_xor_sync(0xffffffffu, s0, x);
-                    s1 += __shfl_xor_sync(0xffffffffu, s1, x);
-                    s2 += __shfl_xor_sync(0xffffffffu, s2, x);
+            for (int c = 0; c < 3; ++c) {
+                float s[4] = {0.f, 0.f, 0.f, 0.f};     // colour c over this thread's channels, per pixel row
+#pragma unroll
+                for (int jj = 0; jj < NT / 8; ++jj) {
+                    const int ch = chan0 + 8 * jj + 2 * k;   // even, and cout is even: an 8-byte aligned pair
+                    const float2 w = *reinterpret_cast<const float2*>(s_rgb + c * p.cout + ch);
+#pragma unroll
+                    for (int r = 0; r < 4; ++r)
+                        s[r] = fmaf(acc[r >> 1][jj * 4 + (r & 1) * 2 + 1], w.y, fmaf(acc[r >> 1][jj * 4 + (r & 1) * 2], w.x, s[r]));
                 }
-                const int k = lane & 3;
-                const float sk = k == 0 ? s0 : (k == 1 ? s1 : s2);
-                rgb_acc[r] = first_n ? sk : rgb_acc[r] + sk;
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+#pragma unroll
+                    for (int x = 1; x < 4; x <<= 1) s[r] += __shfl_xor_sync(0xffffffffu, s[r], x);
+                    if (c == 0 || k >= c) sk[r] = s[r];
+                }
+            }
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const RowPx q = row_px(r);
+                const int limg = q.limg, pimg = q.pimg, poy = q.poy, pox = q.pox;
+                const bool valid = q.valid;
+                // img = upsample(img_lo) + (torgb(x) + b)   (migan_inference.py:308-313); planar NCHW.  Lane k adds colour k
+                // of the row up over the group's N tiles in registers; after the last N tile it writes the pixel.
+                rgb_acc[r] = first_n ? sk[r] : rgb_acc[r] + sk[r];
                 if (last_n && k < 3 && valid) {
                     float rv = rgb_acc[r] + s_rgb[kRgbBias + k];
                     if (p.img_lo) {
