@@ -1,0 +1,546 @@
+// C ABI + host runtime of the FID InceptionV3 feature extractor and of the feature statistics (include/inception_b200.h).
+//
+// The network is pytorch_fid's fid_inception_v3(): torchvision's Inception3 (1008 classes, no aux logits) whose
+// Mixed_5b..5d (InceptionA), 6b..6e (InceptionC) and 7b (InceptionE) average their branch_pool with
+// count_include_pad=False and whose Mixed_7c max-pools it (3 x 3, stride 1, padding 1); input resized to 299 x 299
+// (bilinear, align_corners=False) and mapped to [-1, 1]; output the 2048-d average pool.
+//
+// Lowering: activations NHWC fp32.  Every BasicConv2d (conv without bias, BatchNorm2d(eps=0.001) in eval mode, ReLU) is
+// one launch of the tensor-core implicit GEMM (inception.cu) with the BatchNorm folded into its weights and bias at
+// finalize, writing its channel slice of the block's concatenated output.  Resize, pools and the global average are
+// item kernels (inception_kernels.cuh).  The host walk below is the forward; it runs as a dry pass (workspace size,
+// launch plan) and as the launching pass, in the product library and in the emulation build alike.
+#include <algorithm>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/inception_b200.h"
+#include "inception_kernels.cuh"
+#include "weight_registry.h"
+
+namespace {
+using migan::fail;
+
+constexpr double kBnEps = 0.001;
+constexpr int kOS = INCEPTION_SIZE, kFeat = INCEPTION_FEATURES;
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+inline int round_up(int v, int a) { return (v + a - 1) / a * a; }
+
+// One BasicConv2d: its state_dict prefix, shape and, after finalize, the packed operand.
+struct ConvL {
+    std::string name;
+    int cin = 0, cinp = 0, cout = 0, kh = 1, kw = 1, stride = 1, ph = 0, pw = 0;
+    int KP = 0, NP = 0;
+    float* bhi = nullptr;   // [NP][KP] TF32 hi of the folded weight, K-major
+    float* blo = nullptr;   // [NP][KP] TF32 lo
+    float* bias = nullptr;  // [cout] folded bias
+};
+
+// ---- device memory and the convolution: the only things that differ between the product and the emulation build ----
+#ifdef MIGAN_EMULATE
+int dev_set(int) { return 0; }
+int dev_alloc(void** p, size_t bytes) { *p = aligned_alloc(256, align_up(std::max<size_t>(bytes, 1), 256)); return *p ? 0 : 1; }
+void dev_free(void* p) { free(p); }
+int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t) { memcpy(d, s, bytes); return 0; }
+int dev_sync() { return 0; }
+const char* dev_err(int) { return "emulation"; }
+// The tensor-core kernel's arithmetic: hi*hi into one sum, hi*lo + lo*hi into a second, added with the bias, ReLU.
+int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
+                int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
+                ck_stream_t) {
+    const int64_t P = (int64_t)n * OH * OW;
+#pragma omp parallel
+    {
+        std::vector<float> ah(KP), al(KP);
+#pragma omp for schedule(static)
+        for (int64_t p = 0; p < P; ++p) {
+            const int ox = (int)(p % OW), oy = (int)(p / OW % OH);
+            const int64_t img = p / ((int64_t)OW * OH);
+            for (int k = 0; k < KP; ++k) {
+                const int tap = k / cinp, ci = k % cinp;
+                float v = 0.f;
+                if (tap < kh * kw) {
+                    const int iy = oy * stride - ph + tap / kw, ix = ox * stride - pw + tap % kw;
+                    if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = x[((img * H + iy) * (int64_t)W + ix) * cinp + ci];
+                }
+                incep::tf32_split(v, ah[k], al[k]);
+            }
+            for (int o = 0; o < cout; ++o) {
+                const float* bh = bhi + (int64_t)o * KP;
+                const float* bl = blo + (int64_t)o * KP;
+                float acc = 0.f, cor = 0.f;
+                for (int k = 0; k < KP; ++k) {
+                    acc += ah[k] * bh[k];
+                    cor += ah[k] * bl[k];
+                    cor += al[k] * bh[k];
+                }
+                y[p * ct + c0 + o] = std::max(acc + cor + bias[o], 0.f);
+            }
+        }
+    }
+    return 0;
+}
+#else
+int dev_set(int d) { return (int)cudaSetDevice(d); }
+int dev_alloc(void** p, size_t bytes) { return (int)cudaMalloc(p, std::max<size_t>(bytes, 256)); }
+void dev_free(void* p) { cudaFree(p); }
+int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t st) { return (int)cudaMemcpyAsync(d, s, bytes, cudaMemcpyDefault, st); }
+int dev_sync() { return (int)cudaDeviceSynchronize(); }
+const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
+int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
+                int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
+                ck_stream_t s) {
+    migan::IncepConvArgs a{x, bhi, blo, bias, y, n, H, W, cinp, OH, OW, kh, kw, stride, ph, pw, cout, KP, round_up(cout, 64), ct, c0};
+    return (int)migan::launch_incep_conv(a, s);
+}
+#endif
+
+inline int pack_kp(int taps, int cinp) { return round_up(taps * cinp, 32); }
+
+// ---- workspace walker ------------------------------------------------------------------------------------------------
+struct Runner {
+    bool dry = true;
+    char* base = nullptr;
+    size_t cap = 0, off = 0, peak = 0;
+    ck_stream_t s = nullptr;
+    int rc = 0, launches = 0;
+    std::string* plan = nullptr;   // one line per launch when set
+
+    float* take(size_t floats) {
+        float* p = reinterpret_cast<float*>(base + off);
+        off += align_up(floats * sizeof(float), 256);
+        peak = std::max(peak, off);
+        if (!dry && off > cap && !rc) rc = fail(MIGAN_ERR_WORKSPACE, "workspace too small: need > %zu bytes, have %zu", off, cap);
+        return p;
+    }
+    void note(const char* fmt, ...) __attribute__((format(printf, 2, 3))) {
+        if (!plan) return;
+        char buf[256];
+        va_list ap;
+        va_start(ap, fmt);
+        vsnprintf(buf, sizeof(buf), fmt, ap);
+        va_end(ap);
+        *plan += buf;
+        *plan += "\n";
+    }
+    template <class F>
+    void launch(const F& f, int64_t items) {
+        if (dry || rc || items <= 0) return;
+        const int e = (int)comod::ck_launch(f, items, s);
+        if (e) rc = fail(MIGAN_ERR_CUDA, "kernel launch failed: %s", dev_err(e));
+        ++launches;
+    }
+};
+
+// Activation tensor [n][H][W][C] in the workspace.
+struct Act {
+    float* p;
+    int H, W, C;
+};
+
+}  // namespace
+
+struct inception_ctx {
+    int device = -1;
+    bool finalized = false;
+    migan::WeightRegistry weights;
+    std::vector<ConvL> convs;             // state_dict order
+    std::map<std::string, int> index;     // name -> convs[]
+    std::vector<void*> allocs;
+    int last_launches = 0;
+};
+
+namespace {
+
+// The network's 94 BasicConv2d in torchvision's registration order (= state_dict order).
+void build_specs(inception_ctx* c) {
+    auto add = [&](const std::string& name, int cin, int cout, int kh, int kw, int stride = 1, int ph = 0, int pw = 0) {
+        ConvL L;
+        L.name = name; L.cin = cin; L.cinp = round_up(cin, 4); L.cout = cout;
+        L.kh = kh; L.kw = kw; L.stride = stride; L.ph = ph; L.pw = pw;
+        L.KP = pack_kp(kh * kw, L.cinp);
+        L.NP = round_up(cout, 64);
+        c->index[name] = (int)c->convs.size();
+        c->convs.push_back(L);
+        c->weights.add(name + ".conv.weight", {cout, cin, kh, kw});
+        for (const char* leaf : {".bn.weight", ".bn.bias", ".bn.running_mean", ".bn.running_var"}) c->weights.add(name + leaf, {cout});
+    };
+    add("Conv2d_1a_3x3", 3, 32, 3, 3, 2);
+    add("Conv2d_2a_3x3", 32, 32, 3, 3);
+    add("Conv2d_2b_3x3", 32, 64, 3, 3, 1, 1, 1);
+    add("Conv2d_3b_1x1", 64, 80, 1, 1);
+    add("Conv2d_4a_3x3", 80, 192, 3, 3);
+    auto block_a = [&](const std::string& p, int cin, int pool) {
+        add(p + ".branch1x1", cin, 64, 1, 1);
+        add(p + ".branch5x5_1", cin, 48, 1, 1);
+        add(p + ".branch5x5_2", 48, 64, 5, 5, 1, 2, 2);
+        add(p + ".branch3x3dbl_1", cin, 64, 1, 1);
+        add(p + ".branch3x3dbl_2", 64, 96, 3, 3, 1, 1, 1);
+        add(p + ".branch3x3dbl_3", 96, 96, 3, 3, 1, 1, 1);
+        add(p + ".branch_pool", cin, pool, 1, 1);
+    };
+    block_a("Mixed_5b", 192, 32);
+    block_a("Mixed_5c", 256, 64);
+    block_a("Mixed_5d", 288, 64);
+    add("Mixed_6a.branch3x3", 288, 384, 3, 3, 2);
+    add("Mixed_6a.branch3x3dbl_1", 288, 64, 1, 1);
+    add("Mixed_6a.branch3x3dbl_2", 64, 96, 3, 3, 1, 1, 1);
+    add("Mixed_6a.branch3x3dbl_3", 96, 96, 3, 3, 2);
+    auto block_c = [&](const std::string& p, int c7) {
+        add(p + ".branch1x1", 768, 192, 1, 1);
+        add(p + ".branch7x7_1", 768, c7, 1, 1);
+        add(p + ".branch7x7_2", c7, c7, 1, 7, 1, 0, 3);
+        add(p + ".branch7x7_3", c7, 192, 7, 1, 1, 3, 0);
+        add(p + ".branch7x7dbl_1", 768, c7, 1, 1);
+        add(p + ".branch7x7dbl_2", c7, c7, 7, 1, 1, 3, 0);
+        add(p + ".branch7x7dbl_3", c7, c7, 1, 7, 1, 0, 3);
+        add(p + ".branch7x7dbl_4", c7, c7, 7, 1, 1, 3, 0);
+        add(p + ".branch7x7dbl_5", c7, 192, 1, 7, 1, 0, 3);
+        add(p + ".branch_pool", 768, 192, 1, 1);
+    };
+    block_c("Mixed_6b", 128);
+    block_c("Mixed_6c", 160);
+    block_c("Mixed_6d", 160);
+    block_c("Mixed_6e", 192);
+    add("Mixed_7a.branch3x3_1", 768, 192, 1, 1);
+    add("Mixed_7a.branch3x3_2", 192, 320, 3, 3, 2);
+    add("Mixed_7a.branch7x7x3_1", 768, 192, 1, 1);
+    add("Mixed_7a.branch7x7x3_2", 192, 192, 1, 7, 1, 0, 3);
+    add("Mixed_7a.branch7x7x3_3", 192, 192, 7, 1, 1, 3, 0);
+    add("Mixed_7a.branch7x7x3_4", 192, 192, 3, 3, 2);
+    auto block_e = [&](const std::string& p, int cin) {
+        add(p + ".branch1x1", cin, 320, 1, 1);
+        add(p + ".branch3x3_1", cin, 384, 1, 1);
+        add(p + ".branch3x3_2a", 384, 384, 1, 3, 1, 0, 1);
+        add(p + ".branch3x3_2b", 384, 384, 3, 1, 1, 1, 0);
+        add(p + ".branch3x3dbl_1", cin, 448, 1, 1);
+        add(p + ".branch3x3dbl_2", 448, 384, 3, 3, 1, 1, 1);
+        add(p + ".branch3x3dbl_3a", 384, 384, 1, 3, 1, 0, 1);
+        add(p + ".branch3x3dbl_3b", 384, 384, 3, 1, 1, 1, 0);
+        add(p + ".branch_pool", cin, 192, 1, 1);
+    };
+    block_e("Mixed_7b", 1280);
+    block_e("Mixed_7c", 2048);
+    c->weights.add("fc.weight", {1008, kFeat});
+    c->weights.add("fc.bias", {1008});
+}
+
+// Folds BatchNorm into the convolution in double, rounds once to fp32, and packs the TF32 operand on the device.
+int pack_conv(inception_ctx* c, ConvL& L) {
+    const migan::WeightRegistry& reg = c->weights;
+    const std::vector<float>& w = reg.get(L.name + ".conv.weight");
+    const std::vector<float>& g = reg.get(L.name + ".bn.weight");
+    const std::vector<float>& be = reg.get(L.name + ".bn.bias");
+    const std::vector<float>& mu = reg.get(L.name + ".bn.running_mean");
+    const std::vector<float>& var = reg.get(L.name + ".bn.running_var");
+    const size_t per = (size_t)L.cin * L.kh * L.kw;
+    std::vector<float> wf(w.size()), bf(L.cout);
+    for (int o = 0; o < L.cout; ++o) {
+        const double s = (double)g[o] / std::sqrt((double)var[o] + kBnEps);
+        for (size_t j = 0; j < per; ++j) wf[o * per + j] = (float)((double)w[o * per + j] * s);
+        bf[o] = (float)((double)be[o] - (double)mu[o] * s);
+    }
+    const size_t packed = (size_t)L.NP * L.KP;
+    void *hi = nullptr, *lo = nullptr, *bias = nullptr, *wd = nullptr;
+    int e = dev_alloc(&hi, packed * 4);
+    if (!e) { c->allocs.push_back(hi); e = dev_alloc(&lo, packed * 4); }
+    if (!e) { c->allocs.push_back(lo); e = dev_alloc(&bias, bf.size() * 4); }
+    if (!e) { c->allocs.push_back(bias); e = dev_alloc(&wd, wf.size() * 4); }
+    if (e) return fail(MIGAN_ERR_CUDA, "device allocation failed: %s", dev_err(e));
+    e = dev_copy(bias, bf.data(), bf.size() * 4, nullptr);
+    if (!e) e = dev_copy(wd, wf.data(), wf.size() * 4, nullptr);
+    if (!e) e = (int)comod::ck_launch(incep::PackTf32K{(const float*)wd, (float*)hi, (float*)lo, L.cin, L.cinp, L.cout, L.kh, L.kw, L.KP},
+                                      (int64_t)packed, nullptr);
+    if (!e) e = dev_sync();
+    dev_free(wd);
+    if (e) return fail(MIGAN_ERR_CUDA, "packing '%s' failed: %s", L.name.c_str(), dev_err(e));
+    L.bhi = (float*)hi; L.blo = (float*)lo; L.bias = (float*)bias;
+    return MIGAN_OK;
+}
+
+// ---- the forward walk ------------------------------------------------------------------------------------------------
+struct Walk {
+    const inception_ctx* c;
+    Runner& R;
+    int n;
+
+    Act alloc(int H, int W, int C) { return Act{R.take((size_t)n * H * W * C), H, W, C}; }
+
+    // BasicConv2d `name` on `in`, into channels [c0, c0 + cout) of `out` (allocated when out.p is null)
+    Act conv(const char* name, const Act& in, Act out = Act{nullptr, 0, 0, 0}, int c0 = 0) {
+        const ConvL& L = c->convs[c->index.at(name)];
+        const int OH = (in.H + 2 * L.ph - L.kh) / L.stride + 1, OW = (in.W + 2 * L.pw - L.kw) / L.stride + 1;
+        if (!out.p) out = alloc(OH, OW, L.cout);
+        if (in.C != L.cinp || out.H != OH || out.W != OW || c0 + L.cout > out.C) {
+            if (!R.rc) R.rc = fail(MIGAN_ERR_INVALID, "internal: %s: shapes do not chain", name);
+            return out;
+        }
+        R.note("conv %s in=%dx%dx%d out=%dx%dx%d k=%dx%d s=%d p=%d,%d ct=%d c0=%d", name, in.H, in.W, in.C, OH, OW, L.cout,
+               L.kh, L.kw, L.stride, L.ph, L.pw, out.C, c0);
+        if (!R.dry && !R.rc) {
+            const int e = conv_launch(in.p, L.bhi, L.blo, L.bias, out.p, n, in.H, in.W, L.cinp, OH, OW, L.kh, L.kw, L.stride,
+                                      L.ph, L.pw, L.cout, L.KP, out.C, c0, R.s);
+            if (e) R.rc = fail(MIGAN_ERR_CUDA, "convolution %s failed: %s", name, dev_err(e));
+            ++R.launches;
+        }
+        return out;
+    }
+
+    Act pool(int kind, const char* name, const Act& in, Act out = Act{nullptr, 0, 0, 0}, int c0 = 0) {
+        const int OH = kind == INCEPTION_POOL_MAX_S2 ? (in.H - 3) / 2 + 1 : in.H;
+        const int OW = kind == INCEPTION_POOL_MAX_S2 ? (in.W - 3) / 2 + 1 : in.W;
+        if (!out.p) out = alloc(OH, OW, in.C);
+        static const char* kinds[] = {"max_s2", "avg_s1", "max_s1"};
+        R.note("pool %s %s in=%dx%dx%d out=%dx%dx%d ct=%d c0=%d", kinds[kind], name, in.H, in.W, in.C, OH, OW, in.C, out.C, c0);
+        R.launch(incep::PoolK{in.p, out.p, kind, in.H, in.W, in.C, OH, OW, out.C, c0}, (int64_t)n * OH * OW * (in.C / 4));
+        return out;
+    }
+
+    Act block_a(const std::string& p, const Act& x, int pool_features) {
+        Act y = alloc(x.H, x.W, 224 + pool_features);
+        const size_t m = R.off;
+        conv((p + ".branch1x1").c_str(), x, y, 0);
+        conv((p + ".branch5x5_2").c_str(), conv((p + ".branch5x5_1").c_str(), x), y, 64);
+        Act t = conv((p + ".branch3x3dbl_2").c_str(), conv((p + ".branch3x3dbl_1").c_str(), x));
+        conv((p + ".branch3x3dbl_3").c_str(), t, y, 128);
+        conv((p + ".branch_pool").c_str(), pool(INCEPTION_POOL_AVG_S1, (p + ".branch_pool").c_str(), x), y, 224);
+        R.off = m;
+        return y;
+    }
+    Act block_b(const std::string& p, const Act& x) {
+        Act y = alloc((x.H - 3) / 2 + 1, (x.W - 3) / 2 + 1, 480 + x.C);
+        const size_t m = R.off;
+        conv((p + ".branch3x3").c_str(), x, y, 0);
+        Act t = conv((p + ".branch3x3dbl_2").c_str(), conv((p + ".branch3x3dbl_1").c_str(), x));
+        conv((p + ".branch3x3dbl_3").c_str(), t, y, 384);
+        pool(INCEPTION_POOL_MAX_S2, (p + ".branch_pool").c_str(), x, y, 480);
+        R.off = m;
+        return y;
+    }
+    Act block_c(const std::string& p, const Act& x) {
+        Act y = alloc(x.H, x.W, 768);
+        const size_t m = R.off;
+        conv((p + ".branch1x1").c_str(), x, y, 0);
+        Act t = conv((p + ".branch7x7_2").c_str(), conv((p + ".branch7x7_1").c_str(), x));
+        conv((p + ".branch7x7_3").c_str(), t, y, 192);
+        t = conv((p + ".branch7x7dbl_1").c_str(), x);
+        for (const char* s : {".branch7x7dbl_2", ".branch7x7dbl_3", ".branch7x7dbl_4"}) t = conv((p + s).c_str(), t);
+        conv((p + ".branch7x7dbl_5").c_str(), t, y, 384);
+        conv((p + ".branch_pool").c_str(), pool(INCEPTION_POOL_AVG_S1, (p + ".branch_pool").c_str(), x), y, 576);
+        R.off = m;
+        return y;
+    }
+    Act block_d(const std::string& p, const Act& x) {
+        Act y = alloc((x.H - 3) / 2 + 1, (x.W - 3) / 2 + 1, 512 + x.C);
+        const size_t m = R.off;
+        conv((p + ".branch3x3_2").c_str(), conv((p + ".branch3x3_1").c_str(), x), y, 0);
+        Act t = conv((p + ".branch7x7x3_1").c_str(), x);
+        for (const char* s : {".branch7x7x3_2", ".branch7x7x3_3"}) t = conv((p + s).c_str(), t);
+        conv((p + ".branch7x7x3_4").c_str(), t, y, 320);
+        pool(INCEPTION_POOL_MAX_S2, (p + ".branch_pool").c_str(), x, y, 512);
+        R.off = m;
+        return y;
+    }
+    Act block_e(const std::string& p, const Act& x, int pool_kind) {
+        Act y = alloc(x.H, x.W, 2048);
+        const size_t m = R.off;
+        conv((p + ".branch1x1").c_str(), x, y, 0);
+        Act t = conv((p + ".branch3x3_1").c_str(), x);
+        conv((p + ".branch3x3_2a").c_str(), t, y, 320);
+        conv((p + ".branch3x3_2b").c_str(), t, y, 704);
+        t = conv((p + ".branch3x3dbl_2").c_str(), conv((p + ".branch3x3dbl_1").c_str(), x));
+        conv((p + ".branch3x3dbl_3a").c_str(), t, y, 1088);
+        conv((p + ".branch3x3dbl_3b").c_str(), t, y, 1472);
+        conv((p + ".branch_pool").c_str(), pool(pool_kind, (p + ".branch_pool").c_str(), x), y, 1856);
+        R.off = m;
+        return y;
+    }
+
+    void run(const float* img, int H, int W, float* feats) {
+        Act x = alloc(kOS, kOS, 4);
+        R.note("resize in=%dx%dx3 out=%dx%dx4", H, W, kOS, kOS);
+        R.launch(incep::ResizeK{img, x.p, H, W, kOS}, (int64_t)n * kOS * kOS);
+        x = conv("Conv2d_1a_3x3", x);
+        x = conv("Conv2d_2a_3x3", x);
+        x = conv("Conv2d_2b_3x3", x);
+        x = pool(INCEPTION_POOL_MAX_S2, "maxpool1", x);
+        x = conv("Conv2d_3b_1x1", x);
+        x = conv("Conv2d_4a_3x3", x);
+        x = pool(INCEPTION_POOL_MAX_S2, "maxpool2", x);
+        x = block_a("Mixed_5b", x, 32);
+        x = block_a("Mixed_5c", x, 64);
+        x = block_a("Mixed_5d", x, 64);
+        x = block_b("Mixed_6a", x);
+        for (const char* b : {"Mixed_6b", "Mixed_6c", "Mixed_6d", "Mixed_6e"}) x = block_c(b, x);
+        x = block_d("Mixed_7a", x);
+        x = block_e("Mixed_7b", x, INCEPTION_POOL_AVG_S1);
+        x = block_e("Mixed_7c", x, INCEPTION_POOL_MAX_S1);
+        R.note("avgpool in=%dx%dx%d out=%d", x.H, x.W, x.C, kFeat);
+        R.launch(incep::GlobalAvgK{x.p, feats, x.H * x.W, x.C}, (int64_t)n * x.C);
+    }
+};
+
+int check_ctx(const inception_ctx* c) { return c ? 0 : fail(MIGAN_ERR_INVALID, "null context"); }
+
+int check_images(int n, int H, int W) {
+    if (n < 1 || H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "bad batch: n=%d H=%d W=%d (all >= 1)", n, H, W);
+    return 0;
+}
+
+}  // namespace
+
+// =====================================================================================================================
+extern "C" {
+
+int inception_create(int device, inception_ctx** out) {
+    if (!out) return fail(MIGAN_ERR_INVALID, "out is null");
+    if (device >= 0) {
+        if (const int e = dev_set(device)) return fail(MIGAN_ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
+    }
+    inception_ctx* c = new inception_ctx();
+    c->device = device;
+    build_specs(c);
+    *out = c;
+    return 0;
+}
+
+int inception_destroy(inception_ctx* c) {
+    if (!c) return 0;
+    for (void* p : c->allocs) dev_free(p);
+    delete c;
+    return 0;
+}
+
+int inception_num_weights(const inception_ctx* c) { return c ? c->weights.size() : 0; }
+
+int inception_weight_info(const inception_ctx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
+    if (int rc = check_ctx(c)) return rc;
+    return c->weights.info(index, name, ndim, shape);
+}
+
+int inception_set_weight(inception_ctx* c, const char* name, const float* host_data, int64_t numel) {
+    if (int rc = check_ctx(c)) return rc;
+    if (!name || !host_data) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
+    const size_t len = strlen(name), tail = strlen("num_batches_tracked");
+    if (len >= tail && strcmp(name + len - tail, "num_batches_tracked") == 0) return MIGAN_OK;
+    return c->weights.set(name, host_data, numel);
+}
+
+int inception_finalize_weights(inception_ctx* c) {
+    if (int rc = check_ctx(c)) return rc;
+    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
+    if (const char* key = c->weights.first_missing()) return fail(MIGAN_ERR_INVALID, "missing key '%s' in the state_dict", key);
+    if (c->device < 0) return fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
+    if (int e = dev_set(c->device)) return fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
+    for (ConvL& L : c->convs)
+        if (int rc = pack_conv(c, L)) return rc;
+    c->weights.release_host();
+    c->finalized = true;
+    return 0;
+}
+
+size_t inception_workspace_bytes(const inception_ctx* c, int n, int H, int W) {
+    if (!c || n < 1 || H < 1 || W < 1) return 0;
+    Runner R;
+    Walk w{c, R, n};
+    w.run(nullptr, H, W, nullptr);
+    return R.rc ? 0 : R.peak;
+}
+
+int inception_launch_plan(const inception_ctx* c, int n, int H, int W, char* buf, int cap) {
+    if (int rc = check_ctx(c)) return rc < 0 ? rc : -rc;
+    if (check_images(n, H, W)) return -MIGAN_ERR_INVALID;
+    std::string plan;
+    Runner R;
+    R.plan = &plan;
+    Walk w{c, R, n};
+    w.run(nullptr, H, W, nullptr);
+    if (buf && cap > 0) {
+        const size_t k = std::min(plan.size(), (size_t)cap - 1);
+        memcpy(buf, plan.data(), k);
+        buf[k] = 0;
+    }
+    return (int)plan.size();
+}
+
+int inception_features(inception_ctx* c, const float* x, int n, int H, int W, float* feats, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+    if (int rc = check_ctx(c)) return rc;
+    if (!c->finalized) return fail(MIGAN_ERR_STATE, "forward before inception_finalize_weights");
+    if (!x || !feats) return fail(MIGAN_ERR_INVALID, "null x / feats");
+    if (int rc = check_images(n, H, W)) return rc;
+    if (!workspace) return fail(MIGAN_ERR_INVALID, "null workspace");
+    Runner R;
+    R.dry = false;
+    R.base = static_cast<char*>(workspace);
+    R.cap = workspace_bytes;
+    R.s = static_cast<ck_stream_t>(stream);
+    Walk w{c, R, n};
+    w.run(x, H, W, feats);
+    c->last_launches = R.launches;
+    return R.rc;
+}
+
+int inception_last_launch_count(const inception_ctx* c) { return c ? c->last_launches : 0; }
+
+int inception_resize(const float* x, int n, int H, int W, float* y, void* stream) {
+    if (!x || !y) return fail(MIGAN_ERR_INVALID, "null x / y");
+    if (int rc = check_images(n, H, W)) return rc;
+    CUDA_TRY(comod::ck_launch(incep::ResizeK{x, y, H, W, kOS}, (int64_t)n * kOS * kOS, static_cast<ck_stream_t>(stream)));
+    return 0;
+}
+
+int inception_pool(int kind, const float* x, int n, int H, int W, int C, float* y, int ct, int c0, void* stream) {
+    if (!x || !y) return fail(MIGAN_ERR_INVALID, "null x / y");
+    if (kind < 0 || kind > 2) return fail(MIGAN_ERR_INVALID, "unknown pool kind %d", kind);
+    if (int rc = check_images(n, H, W)) return rc;
+    if (C < 4 || C % 4 || c0 % 4 || ct % 4 || c0 < 0 || c0 + C > ct)
+        return fail(MIGAN_ERR_INVALID, "channels C=%d into [%d, %d) of %d: multiples of 4 within the output", C, c0, c0 + C, ct);
+    if (kind == INCEPTION_POOL_MAX_S2 && (H < 3 || W < 3)) return fail(MIGAN_ERR_INVALID, "max pool 3x3/2 needs H, W >= 3");
+    const int OH = kind == INCEPTION_POOL_MAX_S2 ? (H - 3) / 2 + 1 : H, OW = kind == INCEPTION_POOL_MAX_S2 ? (W - 3) / 2 + 1 : W;
+    CUDA_TRY(comod::ck_launch(incep::PoolK{x, y, kind, H, W, C, OH, OW, ct, c0}, (int64_t)n * OH * OW * (C / 4),
+                              static_cast<ck_stream_t>(stream)));
+    return 0;
+}
+
+int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* w, const float* bias, int cout, int kh,
+                     int kw, int stride, int ph, int pw, float* y, int ct, int c0, void* workspace, size_t workspace_bytes,
+                     size_t* workspace_needed, void* stream) {
+    if (int rc = check_images(n, H, W)) return rc;
+    if (cin < 4 || cin % 4 || cout < 1 || kh < 1 || kw < 1 || stride < 1 || ph < 0 || pw < 0)
+        return fail(MIGAN_ERR_INVALID, "bad convolution: cin=%d (multiple of 4) cout=%d k=%dx%d stride=%d pad=%d,%d", cin, cout,
+                    kh, kw, stride, ph, pw);
+    const int OH = (H + 2 * ph - kh) / stride + 1, OW = (W + 2 * pw - kw) / stride + 1;
+    if (OH < 1 || OW < 1) return fail(MIGAN_ERR_INVALID, "empty convolution output");
+    if (c0 < 0 || c0 + cout > ct) return fail(MIGAN_ERR_INVALID, "channels [%d, %d) outside the %d-channel output", c0, c0 + cout, ct);
+    const int KP = pack_kp(kh * kw, cin), NP = round_up(cout, 64);
+    const size_t need = 2 * align_up((size_t)NP * KP * 4, 256);
+    if (workspace_needed) *workspace_needed = need;
+    if (!workspace) return 0;
+    if (!x || !w || !bias || !y) return fail(MIGAN_ERR_INVALID, "null x / w / bias / y");
+    if (workspace_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", need, workspace_bytes);
+    float* hi = static_cast<float*>(workspace);
+    float* lo = reinterpret_cast<float*>(static_cast<char*>(workspace) + need / 2);
+    const ck_stream_t s = static_cast<ck_stream_t>(stream);
+    CUDA_TRY(comod::ck_launch(incep::PackTf32K{w, hi, lo, cin, cin, cout, kh, kw, KP}, (int64_t)NP * KP, s));
+    CUDA_TRY(conv_launch(x, hi, lo, bias, y, n, H, W, cin, OH, OW, kh, kw, stride, ph, pw, cout, KP, ct, c0, s));
+    return 0;
+}
+
+int fid_stats_update(const float* x, int n, int dim, double* shift, double* sum, double* sumsq, int first, void* stream) {
+    if (!x || !shift || !sum || !sumsq) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (n < 1 || dim < 1 || dim > 65536) return fail(MIGAN_ERR_INVALID, "bad feature batch n=%d dim=%d", n, dim);
+    const ck_stream_t s = static_cast<ck_stream_t>(stream);
+    if (first) CUDA_TRY(comod::ck_launch(incep::StatsShiftK{x, shift, n, dim}, dim, s));
+    CUDA_TRY(comod::ck_launch(incep::StatsUpdateK{x, shift, sum, sumsq, n, dim}, (int64_t)dim * dim, s));
+    return 0;
+}
+
+}  // extern "C"

@@ -1,0 +1,174 @@
+// Item kernels of the FID InceptionV3 forward and of the feature statistics (inception_abi.cu), in the style of
+// comod_kernels.cuh: each functor produces output item i from global memory only and launches through ck_launch(), so
+// the same code runs as a host loop in the emulation build (-DMIGAN_EMULATE).  The convolutions are not here: they are
+// the tensor-core implicit GEMM of inception.cu.
+//
+// Layout: activations NHWC fp32 [n][H][W][C]; a functor that writes a channel slice takes the output's channel pitch
+// ct and offset c0 (the concatenation of an Inception block's branches costs nothing).
+#pragma once
+#include <string.h>
+
+#include "comod_kernels.cuh"
+
+namespace incep {
+
+using comod::f4;
+using comod::ld4;
+using comod::st4;
+
+// ---- TF32 split of the convolution operands ---------------------------------------------------------------------
+// hi = v with its low 13 mantissa bits cleared (a TF32 value, same exponent range as fp32), lo = v - hi (exact in
+// fp32) rounded to the nearest TF32 value, ties away (cvt.rna.tf32.f32): hi + lo = v to about 2^-21 relative, and each
+// product hi*hi, hi*lo, lo*hi of two TF32 values is exact in fp32.
+CK_HD uint32_t f2u(float v) {
+#ifdef __CUDA_ARCH__
+    return __float_as_uint(v);
+#else
+    uint32_t u; memcpy(&u, &v, 4); return u;
+#endif
+}
+CK_HD float u2f(uint32_t u) {
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(u);
+#else
+    float v; memcpy(&v, &u, 4); return v;
+#endif
+}
+CK_HD float tf32_trunc(float v) { return u2f(f2u(v) & 0xffffe000u); }
+CK_HD float tf32_rna(float v) { return u2f((f2u(v) + 0x1000u) & 0xffffe000u); }
+CK_HD void tf32_split(float v, float& hi, float& lo) {
+    hi = tf32_trunc(v);
+    lo = tf32_rna(v - hi);
+}
+
+// Packed weight operand of one convolution: K-major rows hi[o][k], lo[o][k] (NP x KP), k = (ky*kw + kx)*cinp + ci from
+// w[cout][cin][kh][kw]; zero for ci >= cin (the first layer's 3 channels padded to 4), o >= cout and k >= kh*kw*cinp.
+struct PackTf32K {     // items = NP*KP
+    const float* w; float* hi; float* lo;
+    int cin, cinp, cout, kh, kw, KP;
+    CK_HD void operator()(int64_t i) const {
+        const int k = (int)(i % KP), o = (int)(i / KP);
+        float v = 0.f;
+        const int tap = k / cinp, ci = k - tap * cinp;
+        if (o < cout && tap < kh * kw && ci < cin) v = w[(((int64_t)o * cin + ci) * kh + tap / kw) * kw + tap % kw];
+        float h, l;
+        tf32_split(v, h, l);
+        hi[i] = h;
+        lo[i] = l;
+    }
+};
+
+// ---- input stage: F.interpolate(x, (299, 299), mode="bilinear", align_corners=False), then 2x - 1 ---------------
+// NCHW [n][3][H][W] -> NHWC [n][299][299][4], channel 3 zero (the first convolution reads 4-channel pixels).  Source
+// index as ATen computes it in fp32: max(scale * (o + 0.5) - 0.5, 0), scale = in / out.
+struct ResizeK {       // items = n*OS*OS
+    const float* in; float* out; int H, W, OS;
+    CK_HD void operator()(int64_t i) const {
+        const int ox = (int)(i % OS); int64_t t = i / OS;
+        const int oy = (int)(t % OS); const int64_t n = t / OS;
+        const float sy = fmaxf((float)H / (float)OS * ((float)oy + 0.5f) - 0.5f, 0.f);
+        const float sx = fmaxf((float)W / (float)OS * ((float)ox + 0.5f) - 0.5f, 0.f);
+        const int y0 = (int)sy, x0 = (int)sx;
+        const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+        const float ly = fminf(fmaxf(sy - (float)y0, 0.f), 1.f), lx = fminf(fmaxf(sx - (float)x0, 0.f), 1.f);
+        const float hy = 1.f - ly, hx = 1.f - lx;
+        float v[3];
+        for (int c = 0; c < 3; ++c) {
+            const float* p = in + (n * 3 + c) * (int64_t)H * W;
+            const float a = hx * p[(int64_t)y0 * W + x0] + lx * p[(int64_t)y0 * W + x1];
+            const float b = hx * p[(int64_t)y1 * W + x0] + lx * p[(int64_t)y1 * W + x1];
+            v[c] = 2.f * (hy * a + ly * b) - 1.f;
+        }
+        st4(out + i * 4, f4{v[0], v[1], v[2], 0.f});
+    }
+};
+
+// ---- pools (3 x 3 windows) ------------------------------------------------------------------------------------------
+// kind 0: max, stride 2, no padding (max_pool2d(3, 2)); 1: average, stride 1, padding 1, count_include_pad=False (the
+// FID blocks' branch_pool); 2: max, stride 1, padding 1 (Mixed_7c's branch_pool; padding never wins a max).
+// out[n][oy][ox][c0 + c] of a ct-channel tensor; C a multiple of 4.
+struct PoolK {         // items = n*OH*OW*C/4
+    const float* in; float* out; int kind, H, W, C, OH, OW, ct, c0;
+    CK_HD void operator()(int64_t i) const {
+        const int cq = C >> 2;
+        const int c = (int)(i % cq) * 4; int64_t t = i / cq;
+        const int ox = (int)(t % OW); t /= OW;
+        const int oy = (int)(t % OH); const int64_t n = t / OH;
+        const int s = kind == 0 ? 2 : 1, p = kind == 0 ? 0 : 1;
+        const bool avg = kind == 1;
+        f4 acc = avg ? f4{0.f, 0.f, 0.f, 0.f} : f4{-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        int count = 0;
+        for (int ky = 0; ky < 3; ++ky) {
+            const int iy = oy * s - p + ky;
+            if (iy < 0 || iy >= H) continue;
+            for (int kx = 0; kx < 3; ++kx) {
+                const int ix = ox * s - p + kx;
+                if (ix < 0 || ix >= W) continue;
+                const f4 v = ld4(in + ((n * H + iy) * (int64_t)W + ix) * C + c);
+                if (avg) {
+                    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+                } else {
+                    acc.x = fmaxf(acc.x, v.x); acc.y = fmaxf(acc.y, v.y); acc.z = fmaxf(acc.z, v.z); acc.w = fmaxf(acc.w, v.w);
+                }
+                ++count;
+            }
+        }
+        if (avg) {
+            const float d = (float)count;
+            acc.x /= d; acc.y /= d; acc.z /= d; acc.w /= d;
+        }
+        st4(out + ((n * OH + oy) * (int64_t)OW + ox) * ct + c0 + c, acc);
+    }
+};
+
+// adaptive_avg_pool2d(x, 1): out[n][c] = mean over the H*W pixels, summed in pixel order.
+struct GlobalAvgK {    // items = n*C
+    const float* in; float* out; int HW, C;
+    CK_HD void operator()(int64_t i) const {
+        const int c = (int)(i % C); const int64_t n = i / C;
+        float s = 0.f;
+        for (int p = 0; p < HW; ++p) s += in[(n * HW + p) * C + c];
+        out[i] = s / (float)HW;
+    }
+};
+
+// ---- feature statistics (float64) -------------------------------------------------------------------------------
+struct StatsShiftK {   // items = dim: shift[d] = mean over the batch of x[:, d]
+    const float* x; double* shift; int n, dim;
+    CK_HD void operator()(int64_t d) const {
+        double s = 0.0;
+        for (int r = 0; r < n; ++r) s += (double)x[(int64_t)r * dim + d];
+        shift[d] = s / n;
+    }
+};
+// One entry of the rank-n update: sumsq[a][b] += sum_r (x[r][a] - shift[a]) (x[r][b] - shift[b]); the diagonal items
+// also add sum[a].  Entries (a, b) and (b, a) see the same products in the same order: the result is exactly symmetric.
+struct StatsUpdateK {  // items = dim*dim
+    const float* x; const double* shift; double* sum; double* sumsq; int n, dim;
+    CK_HD void operator()(int64_t i) const {
+        const int a = (int)(i / dim), b = (int)(i % dim);
+        const double sa = shift[a], sb = shift[b];
+        double acc = 0.0, s1 = 0.0;
+        for (int r = 0; r < n; ++r) {
+            const double va = (double)x[(int64_t)r * dim + a] - sa, vb = (double)x[(int64_t)r * dim + b] - sb;
+            acc += va * vb;
+            s1 += va;
+        }
+        sumsq[i] += acc;
+        if (a == b) sum[a] += s1;
+    }
+};
+
+}  // namespace incep
+
+#ifndef MIGAN_EMULATE
+namespace migan {
+// One convolution on the tensor-core kernel (inception.cu): y[p][c0 + o] = relu(sum_k A[p][k] * B[o][k] + bias[o]) for
+// o < cout, A gathered from x[n][H][W][cinp] (k = (ky*kw + kx)*cinp + ci, zero outside the image), B = bhi + blo.
+struct IncepConvArgs {
+    const float* x; const float* bhi; const float* blo; const float* bias; float* y;
+    int n, H, W, cinp, OH, OW, kh, kw, stride, ph, pw, cout, KP, NP, ct, c0;
+};
+cudaError_t launch_incep_conv(const IncepConvArgs& a, cudaStream_t s);
+}  // namespace migan
+#endif

@@ -19,7 +19,8 @@ import sys
 
 
 def install() -> None:
-    """Patch `lib.model_zoo.migan_inference.Generator` (the reference must be importable)."""
+    """Patch `lib.model_zoo.migan_inference.Generator` (the reference must be importable), the Co-Mod-GAN modules and,
+    when pytorch_fid is importable, its InceptionV3 and calculate_frechet_distance."""
     import migan_b200
 
     ref_mod = importlib.import_module("lib.model_zoo.migan_inference")
@@ -32,6 +33,19 @@ def install() -> None:
     for name in ("Generator", "Mapping", "Encoder", "Synthesis"):
         setattr(ref_cm, "Reference" + name, getattr(ref_cm, name))
         setattr(ref_cm, name, getattr(comodgan, name))
+    # FID (scripts/evaluate_fid_lpips.py imports InceptionV3 and calculate_frechet_distance from pytorch_fid)
+    try:
+        fid_inception = importlib.import_module("pytorch_fid.inception")
+        fid_score = importlib.import_module("pytorch_fid.fid_score")
+    except ImportError:
+        return
+    from migan_b200 import fid
+
+    fid_inception.ReferenceInceptionV3 = fid_inception.InceptionV3
+    fid_inception.InceptionV3 = fid.InceptionV3
+    fid_score.ReferenceInceptionV3 = fid_score.InceptionV3
+    fid_score.InceptionV3 = fid.InceptionV3
+    fid_score.calculate_frechet_distance = fid.calculate_frechet_distance
 
 
 def main(argv=None) -> None:
