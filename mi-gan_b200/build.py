@@ -18,7 +18,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libmigan_b200.so")
 STAMP = os.path.join(LIBDIR, "libmigan_b200.stamp")
 
-SOURCES = ["elementwise.cu", "gemm_simt.cu", "ops.cu", "sepconv_tc.cu", "abi_error.cu", "migan_abi.cu", "comodgan_abi.cu", "prepost.cu", "pipeline.cu", "demo_resize.cu", "fullres.cu", "holewin.cu", "masks.cu", "reparam.cu", "inception.cu", "inception_abi.cu"]
+SOURCES = ["elementwise.cu", "gemm_simt.cu", "ops.cu", "sepconv_tc.cu", "abi_error.cu", "migan_abi.cu", "comodgan_abi.cu", "prepost.cu", "pipeline.cu", "demo_resize.cu", "fullres.cu", "holewin.cu", "masks.cu", "reparam.cu", "inception.cu", "inception_abi.cu", "lpips_abi.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -37,7 +37,8 @@ def _source_hash() -> str:
     h = hashlib.sha256()
     files = sorted(os.listdir(CSRC)) + [os.path.join("..", "..", "include", "migan_b200.h"),
                                         os.path.join("..", "..", "include", "comodgan_b200.h"),
-                                        os.path.join("..", "..", "include", "inception_b200.h")]
+                                        os.path.join("..", "..", "include", "inception_b200.h"),
+                                        os.path.join("..", "..", "include", "lpips_b200.h")]
     for name in files:
         path = os.path.join(CSRC, name)
         if os.path.isfile(path):

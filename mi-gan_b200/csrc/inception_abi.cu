@@ -10,139 +10,25 @@
 // finalize, writing its channel slice of the block's concatenated output.  Resize, pools and the global average are
 // item kernels (inception_kernels.cuh).  The host walk below is the forward; it runs as a dry pass (workspace size,
 // launch plan) and as the launching pass, in the product library and in the emulation build alike.
-#include <algorithm>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
 #include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/inception_b200.h"
-#include "inception_kernels.cuh"
+#include "conv_runtime.h"
 #include "weight_registry.h"
 
 namespace {
 using migan::fail;
+using incep::Act;
+using incep::ConvL;
+using incep::Runner;
+using incep::dev_err;
+using incep::dev_set;
 
 constexpr double kBnEps = 0.001;
 constexpr int kOS = INCEPTION_SIZE, kFeat = INCEPTION_FEATURES;
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-inline int round_up(int v, int a) { return (v + a - 1) / a * a; }
-
-// One BasicConv2d: its state_dict prefix, shape and, after finalize, the packed operand.
-struct ConvL {
-    std::string name;
-    int cin = 0, cinp = 0, cout = 0, kh = 1, kw = 1, stride = 1, ph = 0, pw = 0;
-    int KP = 0, NP = 0;
-    float* bhi = nullptr;   // [NP][KP] TF32 hi of the folded weight, K-major
-    float* blo = nullptr;   // [NP][KP] TF32 lo
-    float* bias = nullptr;  // [cout] folded bias
-};
-
-// ---- device memory and the convolution: the only things that differ between the product and the emulation build ----
-#ifdef MIGAN_EMULATE
-int dev_set(int) { return 0; }
-int dev_alloc(void** p, size_t bytes) { *p = aligned_alloc(256, align_up(std::max<size_t>(bytes, 1), 256)); return *p ? 0 : 1; }
-void dev_free(void* p) { free(p); }
-int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t) { memcpy(d, s, bytes); return 0; }
-int dev_sync() { return 0; }
-const char* dev_err(int) { return "emulation"; }
-// The tensor-core kernel's arithmetic: hi*hi into one sum, hi*lo + lo*hi into a second, added with the bias, ReLU.
-int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
-                int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
-                ck_stream_t) {
-    const int64_t P = (int64_t)n * OH * OW;
-#pragma omp parallel
-    {
-        std::vector<float> ah(KP), al(KP);
-#pragma omp for schedule(static)
-        for (int64_t p = 0; p < P; ++p) {
-            const int ox = (int)(p % OW), oy = (int)(p / OW % OH);
-            const int64_t img = p / ((int64_t)OW * OH);
-            for (int k = 0; k < KP; ++k) {
-                const int tap = k / cinp, ci = k % cinp;
-                float v = 0.f;
-                if (tap < kh * kw) {
-                    const int iy = oy * stride - ph + tap / kw, ix = ox * stride - pw + tap % kw;
-                    if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = x[((img * H + iy) * (int64_t)W + ix) * cinp + ci];
-                }
-                incep::tf32_split(v, ah[k], al[k]);
-            }
-            for (int o = 0; o < cout; ++o) {
-                const float* bh = bhi + (int64_t)o * KP;
-                const float* bl = blo + (int64_t)o * KP;
-                float acc = 0.f, cor = 0.f;
-                for (int k = 0; k < KP; ++k) {
-                    acc += ah[k] * bh[k];
-                    cor += ah[k] * bl[k];
-                    cor += al[k] * bh[k];
-                }
-                y[p * ct + c0 + o] = std::max(acc + cor + bias[o], 0.f);
-            }
-        }
-    }
-    return 0;
-}
-#else
-int dev_set(int d) { return (int)cudaSetDevice(d); }
-int dev_alloc(void** p, size_t bytes) { return (int)cudaMalloc(p, std::max<size_t>(bytes, 256)); }
-void dev_free(void* p) { cudaFree(p); }
-int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t st) { return (int)cudaMemcpyAsync(d, s, bytes, cudaMemcpyDefault, st); }
-int dev_sync() { return (int)cudaDeviceSynchronize(); }
-const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
-int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
-                int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
-                ck_stream_t s) {
-    migan::IncepConvArgs a{x, bhi, blo, bias, y, n, H, W, cinp, OH, OW, kh, kw, stride, ph, pw, cout, KP, round_up(cout, 64), ct, c0};
-    return (int)migan::launch_incep_conv(a, s);
-}
-#endif
-
-inline int pack_kp(int taps, int cinp) { return round_up(taps * cinp, 32); }
-
-// ---- workspace walker ------------------------------------------------------------------------------------------------
-struct Runner {
-    bool dry = true;
-    char* base = nullptr;
-    size_t cap = 0, off = 0, peak = 0;
-    ck_stream_t s = nullptr;
-    int rc = 0, launches = 0;
-    std::string* plan = nullptr;   // one line per launch when set
-
-    float* take(size_t floats) {
-        float* p = reinterpret_cast<float*>(base + off);
-        off += align_up(floats * sizeof(float), 256);
-        peak = std::max(peak, off);
-        if (!dry && off > cap && !rc) rc = fail(MIGAN_ERR_WORKSPACE, "workspace too small: need > %zu bytes, have %zu", off, cap);
-        return p;
-    }
-    void note(const char* fmt, ...) __attribute__((format(printf, 2, 3))) {
-        if (!plan) return;
-        char buf[256];
-        va_list ap;
-        va_start(ap, fmt);
-        vsnprintf(buf, sizeof(buf), fmt, ap);
-        va_end(ap);
-        *plan += buf;
-        *plan += "\n";
-    }
-    template <class F>
-    void launch(const F& f, int64_t items) {
-        if (dry || rc || items <= 0) return;
-        const int e = (int)comod::ck_launch(f, items, s);
-        if (e) rc = fail(MIGAN_ERR_CUDA, "kernel launch failed: %s", dev_err(e));
-        ++launches;
-    }
-};
-
-// Activation tensor [n][H][W][C] in the workspace.
-struct Act {
-    float* p;
-    int H, W, C;
-};
 
 }  // namespace
 
@@ -161,13 +47,8 @@ namespace {
 // The network's 94 BasicConv2d in torchvision's registration order (= state_dict order).
 void build_specs(inception_ctx* c) {
     auto add = [&](const std::string& name, int cin, int cout, int kh, int kw, int stride = 1, int ph = 0, int pw = 0) {
-        ConvL L;
-        L.name = name; L.cin = cin; L.cinp = round_up(cin, 4); L.cout = cout;
-        L.kh = kh; L.kw = kw; L.stride = stride; L.ph = ph; L.pw = pw;
-        L.KP = pack_kp(kh * kw, L.cinp);
-        L.NP = round_up(cout, 64);
         c->index[name] = (int)c->convs.size();
-        c->convs.push_back(L);
+        c->convs.push_back(incep::conv_layer(name, cin, cout, kh, kw, stride, ph, pw));
         c->weights.add(name + ".conv.weight", {cout, cin, kh, kw});
         for (const char* leaf : {".bn.weight", ".bn.bias", ".bn.running_mean", ".bn.running_var"}) c->weights.add(name + leaf, {cout});
     };
@@ -246,22 +127,7 @@ int pack_conv(inception_ctx* c, ConvL& L) {
         for (size_t j = 0; j < per; ++j) wf[o * per + j] = (float)((double)w[o * per + j] * s);
         bf[o] = (float)((double)be[o] - (double)mu[o] * s);
     }
-    const size_t packed = (size_t)L.NP * L.KP;
-    void *hi = nullptr, *lo = nullptr, *bias = nullptr, *wd = nullptr;
-    int e = dev_alloc(&hi, packed * 4);
-    if (!e) { c->allocs.push_back(hi); e = dev_alloc(&lo, packed * 4); }
-    if (!e) { c->allocs.push_back(lo); e = dev_alloc(&bias, bf.size() * 4); }
-    if (!e) { c->allocs.push_back(bias); e = dev_alloc(&wd, wf.size() * 4); }
-    if (e) return fail(MIGAN_ERR_CUDA, "device allocation failed: %s", dev_err(e));
-    e = dev_copy(bias, bf.data(), bf.size() * 4, nullptr);
-    if (!e) e = dev_copy(wd, wf.data(), wf.size() * 4, nullptr);
-    if (!e) e = (int)comod::ck_launch(incep::PackTf32K{(const float*)wd, (float*)hi, (float*)lo, L.cin, L.cinp, L.cout, L.kh, L.kw, L.KP},
-                                      (int64_t)packed, nullptr);
-    if (!e) e = dev_sync();
-    dev_free(wd);
-    if (e) return fail(MIGAN_ERR_CUDA, "packing '%s' failed: %s", L.name.c_str(), dev_err(e));
-    L.bhi = (float*)hi; L.blo = (float*)lo; L.bias = (float*)bias;
-    return MIGAN_OK;
+    return incep::upload_conv(L, wf.data(), bf.data(), c->allocs);
 }
 
 // ---- the forward walk ------------------------------------------------------------------------------------------------
@@ -275,30 +141,14 @@ struct Walk {
     // BasicConv2d `name` on `in`, into channels [c0, c0 + cout) of `out` (allocated when out.p is null)
     Act conv(const char* name, const Act& in, Act out = Act{nullptr, 0, 0, 0}, int c0 = 0) {
         const ConvL& L = c->convs[c->index.at(name)];
-        const int OH = (in.H + 2 * L.ph - L.kh) / L.stride + 1, OW = (in.W + 2 * L.pw - L.kw) / L.stride + 1;
-        if (!out.p) out = alloc(OH, OW, L.cout);
-        if (in.C != L.cinp || out.H != OH || out.W != OW || c0 + L.cout > out.C) {
-            if (!R.rc) R.rc = fail(MIGAN_ERR_INVALID, "internal: %s: shapes do not chain", name);
-            return out;
-        }
-        R.note("conv %s in=%dx%dx%d out=%dx%dx%d k=%dx%d s=%d p=%d,%d ct=%d c0=%d", name, in.H, in.W, in.C, OH, OW, L.cout,
-               L.kh, L.kw, L.stride, L.ph, L.pw, out.C, c0);
-        if (!R.dry && !R.rc) {
-            const int e = conv_launch(in.p, L.bhi, L.blo, L.bias, out.p, n, in.H, in.W, L.cinp, OH, OW, L.kh, L.kw, L.stride,
-                                      L.ph, L.pw, L.cout, L.KP, out.C, c0, R.s);
-            if (e) R.rc = fail(MIGAN_ERR_CUDA, "convolution %s failed: %s", name, dev_err(e));
-            ++R.launches;
-        }
+        if (!out.p) out = alloc((in.H + 2 * L.ph - L.kh) / L.stride + 1, (in.W + 2 * L.pw - L.kw) / L.stride + 1, L.cout);
+        incep::conv_step(R, L, n, in, out, c0);
         return out;
     }
 
     Act pool(int kind, const char* name, const Act& in, Act out = Act{nullptr, 0, 0, 0}, int c0 = 0) {
-        const int OH = kind == INCEPTION_POOL_MAX_S2 ? (in.H - 3) / 2 + 1 : in.H;
-        const int OW = kind == INCEPTION_POOL_MAX_S2 ? (in.W - 3) / 2 + 1 : in.W;
-        if (!out.p) out = alloc(OH, OW, in.C);
-        static const char* kinds[] = {"max_s2", "avg_s1", "max_s1"};
-        R.note("pool %s %s in=%dx%dx%d out=%dx%dx%d ct=%d c0=%d", kinds[kind], name, in.H, in.W, in.C, OH, OW, in.C, out.C, c0);
-        R.launch(incep::PoolK{in.p, out.p, kind, in.H, in.W, in.C, OH, OW, out.C, c0}, (int64_t)n * OH * OW * (in.C / 4));
+        if (!out.p) out = alloc(incep::pool_out(kind, in.H), incep::pool_out(kind, in.W), in.C);
+        incep::pool_step(R, kind, name, n, in, out, c0);
         return out;
     }
 
@@ -412,7 +262,7 @@ int inception_create(int device, inception_ctx** out) {
 
 int inception_destroy(inception_ctx* c) {
     if (!c) return 0;
-    for (void* p : c->allocs) dev_free(p);
+    for (void* p : c->allocs) incep::dev_free(p);
     delete c;
     return 0;
 }
@@ -520,8 +370,8 @@ int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* 
     const int OH = (H + 2 * ph - kh) / stride + 1, OW = (W + 2 * pw - kw) / stride + 1;
     if (OH < 1 || OW < 1) return fail(MIGAN_ERR_INVALID, "empty convolution output");
     if (c0 < 0 || c0 + cout > ct) return fail(MIGAN_ERR_INVALID, "channels [%d, %d) outside the %d-channel output", c0, c0 + cout, ct);
-    const int KP = pack_kp(kh * kw, cin), NP = round_up(cout, 64);
-    const size_t need = 2 * align_up((size_t)NP * KP * 4, 256);
+    const int KP = incep::pack_kp(kh * kw, cin), NP = incep::round_up(cout, 64);
+    const size_t need = 2 * incep::align_up((size_t)NP * KP * 4, 256);
     if (workspace_needed) *workspace_needed = need;
     if (!workspace) return 0;
     if (!x || !w || !bias || !y) return fail(MIGAN_ERR_INVALID, "null x / w / bias / y");
@@ -530,7 +380,7 @@ int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* 
     float* lo = reinterpret_cast<float*>(static_cast<char*>(workspace) + need / 2);
     const ck_stream_t s = static_cast<ck_stream_t>(stream);
     CUDA_TRY(comod::ck_launch(incep::PackTf32K{w, hi, lo, cin, cin, cout, kh, kw, KP}, (int64_t)NP * KP, s));
-    CUDA_TRY(conv_launch(x, hi, lo, bias, y, n, H, W, cin, OH, OW, kh, kw, stride, ph, pw, cout, KP, ct, c0, s));
+    CUDA_TRY(incep::conv_launch(x, hi, lo, bias, y, n, H, W, cin, OH, OW, kh, kw, stride, ph, pw, cout, KP, ct, c0, s));
     return 0;
 }
 

@@ -19,8 +19,9 @@ import sys
 
 
 def install() -> None:
-    """Patch `lib.model_zoo.migan_inference.Generator` (the reference must be importable), the Co-Mod-GAN modules and,
-    when pytorch_fid is importable, its InceptionV3 and calculate_frechet_distance."""
+    """Patch `lib.model_zoo.migan_inference.Generator` (the reference must be importable), the Co-Mod-GAN modules,
+    when pytorch_fid is importable its InceptionV3 and calculate_frechet_distance, and when lpips is importable its
+    LPIPS."""
     import migan_b200
 
     ref_mod = importlib.import_module("lib.model_zoo.migan_inference")
@@ -33,7 +34,12 @@ def install() -> None:
     for name in ("Generator", "Mapping", "Encoder", "Synthesis"):
         setattr(ref_cm, "Reference" + name, getattr(ref_cm, name))
         setattr(ref_cm, name, getattr(comodgan, name))
-    # FID (scripts/evaluate_fid_lpips.py imports InceptionV3 and calculate_frechet_distance from pytorch_fid)
+    _install_fid()
+    _install_lpips()
+
+
+def _install_fid() -> None:
+    """FID: scripts/evaluate_fid_lpips.py imports InceptionV3 and calculate_frechet_distance from pytorch_fid."""
     try:
         fid_inception = importlib.import_module("pytorch_fid.inception")
         fid_score = importlib.import_module("pytorch_fid.fid_score")
@@ -46,6 +52,18 @@ def install() -> None:
     fid_score.ReferenceInceptionV3 = fid_score.InceptionV3
     fid_score.InceptionV3 = fid.InceptionV3
     fid_score.calculate_frechet_distance = fid.calculate_frechet_distance
+
+
+def _install_lpips() -> None:
+    """LPIPS: scripts/evaluate_fid_lpips.py does `import lpips` and calls `lpips.LPIPS(net="alex")`."""
+    try:
+        ref_lpips = importlib.import_module("lpips")
+    except ImportError:
+        return
+    from migan_b200 import lpips
+
+    ref_lpips.ReferenceLPIPS = ref_lpips.LPIPS
+    ref_lpips.LPIPS = lpips.LPIPS
 
 
 def main(argv=None) -> None:
