@@ -12,6 +12,8 @@ Public surface (mirrors the reference's for this path):
     fid.InceptionV3 / fid.FeatureStatistics / fid.calculate_frechet_distance
                                      pytorch_fid's FID features, statistics and distance (InceptionV3 on tensor cores)
     lpips.LPIPS                      drop-in for lpips.LPIPS(net="alex"): the script's LPIPS distance (AlexNet on tensor cores)
+    metrics.compute_ssim / metrics.SSIM / metrics.compute_psnr
+                                     the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double
     generate_masks                   python -m migan_b200.generate_masks: the reference script's CLI and files
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
@@ -19,12 +21,12 @@ Public surface (mirrors the reference's for this path):
 
 The directory is named `mi-gan_b200`; import it as `migan_b200` (repo-root shim `migan_b200.py`).
 """
-from . import arch, build, demo, evaluate, export, fid, fullres, holewin, lpips, masks, ops, parallel, pipeline, synthetic  # noqa: F401
+from . import arch, build, demo, evaluate, export, fid, fullres, holewin, lpips, masks, metrics, ops, parallel, pipeline, synthetic  # noqa: F401
 from .fullres import FullResPipeline  # noqa: F401
 from .holewin import HoleWindowPipeline  # noqa: F401
 from .evaluate import EvalPipeline  # noqa: F401
 from .masks import RandomMaskStream  # noqa: F401
 from .generator import Generator  # noqa: F401
 
-__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "lpips", "masks", "ops", "parallel", "pipeline", "synthetic"]
+__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "lpips", "masks", "metrics", "ops", "parallel", "pipeline", "synthetic"]
 __version__ = "0.1.0"
