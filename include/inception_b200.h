@@ -10,6 +10,8 @@
  *                                      and shapes (472 entries besides num_batches_tracked, fc.* accepted and unused)
  *   inception_features                 model(x)[0].view(n, 2048): the 2048-d pool3 features of x[n,3,H,W] in [0, 1]
  *   fid_stats_update                   the float64 running sums behind np.mean / np.cov(rowvar=False) of the features
+ *   fid_stats_mean_cov                 the mean and covariance from those sums, on the device
+ *   fid_frechet_distance               the Fréchet distance of two (mu, sigma) on the device (float64 eigensolver)
  */
 #ifndef INCEPTION_B200_H_
 #define INCEPTION_B200_H_
@@ -70,6 +72,29 @@ int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* 
  * first != 0), sum[dim] += sum_i (x_i - shift), sumsq[dim][dim] += sum_i (x_i - shift)(x_i - shift)^T.  Then
  * mean = shift + sum / N and cov = (sumsq - sum sum^T / N) / (N - 1). */
 int fid_stats_update(const float* x, int n, int dim, double* shift, double* sum, double* sumsq, int first, void* stream);
+/* mu[dim] = shift + sum / count and sigma[dim][dim] = (sumsq - sum sum^T / count) / (count - 1) from the sums above
+ * (float64, device), each operation rounded on its own: bitwise what FeatureStatistics.mean_cov() computes on the host.
+ * count >= 2.  Asynchronous on `stream`. */
+int fid_stats_mean_cov(const double* shift, const double* sum, const double* sumsq, int64_t count, int dim, double* mu,
+                       double* sigma, void* stream);
+
+/* ---- Fréchet distance ----------------------------------------------------------------------------------------------
+ * FID = ||mu1 - mu2||^2 + tr S1 + tr S2 - 2 tr sqrt(S1 S2) in float64 for covariances S1, S2 [dim][dim] (device,
+ * symmetric positive semi-definite; each is symmetrised once as (S + S^T) / 2).  tr sqrt(S1 S2) is the sum of
+ * sqrt(max(lambda, 0)) over the eigenvalues of D^1/2 V^T S2 V D^1/2, S1 = V D V^T (negative d clamped to 0): two
+ * block-Jacobi eigensolves on the device, no non-symmetric product.  No atomics and fixed-order sums: the same inputs
+ * give the same bytes on every run.
+ *
+ * out_host[4] (HOST) = {||mu1 - mu2||^2, tr S1, tr S2, tr sqrt(S1 S2)}; FID = out[0] + out[1] + out[2] - 2 out[3].
+ * sweeps_host (HOST, may be NULL) receives the Jacobi sweeps of the two eigensolves (int[2]).
+ * SYNCHRONOUS on `stream`: the solver reads a convergence value back once per sweep, and the call returns with the
+ * result on the host.  Refused with MIGAN_ERR_INVALID: dim outside 1..FID_FRECHET_MAX_DIM, null pointers, non-finite
+ * input, no convergence within 40 sweeps; with MIGAN_ERR_WORKSPACE: a workspace that is short or not 256-byte aligned. */
+#define FID_FRECHET_MAX_DIM 4096
+/* Device bytes fid_frechet_distance needs (about 4 N^2 doubles, N = dim rounded up to 64); 0 on bad arguments. */
+size_t fid_frechet_workspace_bytes(int dim);
+int fid_frechet_distance(const double* mu1, const double* sigma1, const double* mu2, const double* sigma2, int dim,
+                         double out_host[4], int* sweeps_host, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,6 +11,8 @@ Public surface (mirrors the reference's for this path):
     evaluate.EvalPipeline            evaluate_fid_lpips.py's batch around the generator: resizes, composite, normalisations
     fid.InceptionV3 / fid.FeatureStatistics / fid.calculate_frechet_distance
                                      pytorch_fid's FID features, statistics and distance (InceptionV3 on tensor cores)
+    fid.frechet_distance / FeatureStatistics.frechet_distance
+                                     the Frechet distance on the GPU (fp64 block-Jacobi eigensolver, deterministic)
     lpips.LPIPS                      drop-in for lpips.LPIPS(net="alex"): the script's LPIPS distance (AlexNet on tensor cores)
     metrics.compute_ssim / metrics.SSIM / metrics.compute_psnr
                                      the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double

@@ -1,0 +1,291 @@
+// C ABI of the Fréchet distance (include/inception_b200.h): fid_stats_mean_cov, fid_frechet_workspace_bytes and
+// fid_frechet_distance.  Argument checks, workspace layout, the eigensolver's sweep loop and the launches; the
+// arithmetic is frechet_kernels.cuh's.  The kernels here run its phases with a block's threads at once, and the
+// emulation build (MIGAN_EMULATE) runs the same phases with the threads of a block in turn.
+//
+// Workspace (N = dim rounded up to a multiple of 64, each region 256-byte aligned): A, V, B, W (N x N doubles each),
+// the pair factors (N / 64 of 64 x 64), sqrt(d) (N), the column partials of the norm (2N), 8 scalars.
+#include <math.h>
+#include <string.h>
+
+#include <vector>
+
+#include "../../include/inception_b200.h"
+#include "abi_error.h"
+#include "frechet_kernels.cuh"
+
+namespace {
+using frechet::kG;
+using frechet::kLd;
+using frechet::kThreads;
+using frechet::kTileDoubles;
+using migan::fail;
+
+constexpr int kMaxSweeps = 40;
+static_assert(frechet::kMaxDim == FID_FRECHET_MAX_DIM, "one cap");
+constexpr size_t kPairSmem = (2 * kTileDoubles + 4 * frechet::kB) * sizeof(double);
+constexpr size_t kUpdateSmem = 3 * kTileDoubles * sizeof(double);
+constexpr size_t kGemmSmem = 2 * kTileDoubles * sizeof(double);
+
+#ifdef MIGAN_EMULATE
+int pair_launch(const frechet::PairArgs& a, int blocks, ck_stream_t) {
+#pragma omp parallel for schedule(dynamic)
+    for (int k = 0; k < blocks; ++k) {
+        std::vector<double> S(kTileDoubles), J(kTileDoubles), cs(4 * frechet::kB);
+        for (int t = 0; t < kThreads; ++t) a.load(k, t, S.data(), J.data());
+        for (int sweep = 0; sweep < frechet::kMaxInner; ++sweep) {
+            int rotated = 0;
+            for (int step = 0; step < kG - 1; ++step) {
+                int go = 0;
+                for (int t = 0; t < frechet::kB; ++t) go |= a.rot(step, t, S.data(), cs.data());
+                if (!go) continue;
+                for (int t = 0; t < kThreads; ++t) a.apply(step, t, S.data(), J.data(), cs.data());
+                rotated = 1;
+            }
+            if (!rotated) break;
+        }
+        for (int t = 0; t < kThreads; ++t) a.store(k, t, S.data(), J.data());
+    }
+    return 0;
+}
+
+int update_launch(const frechet::UpdateArgs& a, ck_stream_t) {
+    const int64_t blocks = a.blocks();
+#pragma omp parallel for schedule(dynamic)
+    for (int64_t b = 0; b < blocks; ++b) {
+        std::vector<double> X(kTileDoubles), P(kTileDoubles), R(kTileDoubles);
+        std::vector<frechet::Acc> c(kThreads);
+        for (int t = 0; t < kThreads; ++t) a.load(b, t, X.data(), P.data(), R.data());
+        for (int t = 0; t < kThreads; ++t) a.right(t, c[t], X.data(), P.data());
+        for (int t = 0; t < kThreads; ++t) a.after_right(b, t, c[t], X.data());
+        if (b >= a.tilesA) continue;
+        for (int t = 0; t < kThreads; ++t) a.left(b, t, c[t], X.data(), R.data());
+    }
+    return 0;
+}
+
+int gemm_launch(const frechet::GemmArgs& a, ck_stream_t) {
+    const int64_t blocks = (int64_t)(a.N / kG) * (a.N / kG);
+#pragma omp parallel for schedule(dynamic)
+    for (int64_t b = 0; b < blocks; ++b) {
+        std::vector<double> Xs(kTileDoubles), Ys(kTileDoubles);
+        std::vector<frechet::Acc> c(kThreads);
+        for (int t = 0; t < kThreads; ++t) frechet::acc_zero(c[t]);
+        for (int k0 = 0; k0 < a.N; k0 += kG) {
+            for (int t = 0; t < kThreads; ++t) a.stage(b, t, k0, Xs.data(), Ys.data());
+            for (int t = 0; t < kThreads; ++t) a.product(t, c[t], Xs.data(), Ys.data());
+        }
+        for (int t = 0; t < kThreads; ++t) a.store(b, t, c[t]);
+    }
+    return 0;
+}
+
+int to_host(void* dst, const void* src, size_t bytes, ck_stream_t) {
+    memcpy(dst, src, bytes);
+    return 0;
+}
+#else
+__global__ void __launch_bounds__(kThreads) frechet_pair_kernel(const __grid_constant__ frechet::PairArgs a) {
+    extern __shared__ __align__(16) double smem[];
+    double* S = smem;
+    double* J = S + kTileDoubles;
+    double* cs = J + kTileDoubles;
+    const int k = blockIdx.x, t = threadIdx.x;
+    a.load(k, t, S, J);
+    __syncthreads();
+    for (int sweep = 0; sweep < frechet::kMaxInner; ++sweep) {
+        int rotated = 0;
+        for (int step = 0; step < kG - 1; ++step) {
+            const int go = t < frechet::kB ? a.rot(step, t, S, cs) : 0;
+            if (!__syncthreads_or(go)) continue;   // the same answer in every thread: the branch is uniform
+            a.apply(step, t, S, J, cs);
+            rotated = 1;
+            __syncthreads();
+        }
+        if (!rotated) break;
+    }
+    a.store(k, t, S, J);
+}
+
+__global__ void __launch_bounds__(kThreads) frechet_update_kernel(const __grid_constant__ frechet::UpdateArgs a) {
+    extern __shared__ __align__(16) double smem[];
+    double* X = smem;
+    double* P = X + kTileDoubles;
+    double* R = P + kTileDoubles;
+    const int64_t b = blockIdx.x;
+    const int t = threadIdx.x;
+    a.load(b, t, X, P, R);
+    __syncthreads();
+    frechet::Acc c;
+    a.right(t, c, X, P);
+    __syncthreads();
+    a.after_right(b, t, c, X);
+    if (b >= a.tilesA) return;
+    __syncthreads();
+    a.left(b, t, c, X, R);
+}
+
+__global__ void __launch_bounds__(kThreads) frechet_gemm_kernel(const __grid_constant__ frechet::GemmArgs a) {
+    extern __shared__ __align__(16) double smem[];
+    double* Xs = smem;
+    double* Ys = Xs + kTileDoubles;
+    const int64_t b = blockIdx.x;
+    const int t = threadIdx.x;
+    frechet::Acc c;
+    frechet::acc_zero(c);
+    for (int k0 = 0; k0 < a.N; k0 += kG) {
+        a.stage(b, t, k0, Xs, Ys);
+        __syncthreads();
+        a.product(t, c, Xs, Ys);
+        __syncthreads();
+    }
+    a.store(b, t, c);
+}
+
+template <class K>
+int set_smem(K kernel, size_t bytes) {
+    return (int)cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
+int pair_launch(const frechet::PairArgs& a, int blocks, ck_stream_t s) {
+    if (int e = set_smem(frechet_pair_kernel, kPairSmem)) return e;
+    frechet_pair_kernel<<<blocks, kThreads, kPairSmem, s>>>(a);
+    return (int)cudaGetLastError();
+}
+
+int update_launch(const frechet::UpdateArgs& a, ck_stream_t s) {
+    if (int e = set_smem(frechet_update_kernel, kUpdateSmem)) return e;
+    frechet_update_kernel<<<(unsigned)a.blocks(), kThreads, kUpdateSmem, s>>>(a);
+    return (int)cudaGetLastError();
+}
+
+int gemm_launch(const frechet::GemmArgs& a, ck_stream_t s) {
+    if (int e = set_smem(frechet_gemm_kernel, kGemmSmem)) return e;
+    frechet_gemm_kernel<<<(unsigned)((a.N / kG) * (a.N / kG)), kThreads, kGemmSmem, s>>>(a);
+    return (int)cudaGetLastError();
+}
+
+int to_host(void* dst, const void* src, size_t bytes, ck_stream_t s) {
+    if (cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s)) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+}
+#endif
+
+int padded(int dim) { return (dim + kG - 1) / kG * kG; }
+size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+
+struct Layout {
+    size_t A, V, B, W, J, sd, part, scal, total;
+};
+
+Layout layout(int dim) {
+    const size_t N = (size_t)padded(dim), mat = align256(N * N * sizeof(double));
+    Layout L;
+    L.A = 0;
+    L.V = L.A + mat;
+    L.B = L.V + mat;
+    L.W = L.B + mat;
+    L.J = L.W + mat;
+    L.sd = L.J + align256(N / kG * kG * kG * sizeof(double));
+    L.part = L.sd + align256(N * sizeof(double));
+    L.scal = L.part + align256(2 * N * sizeof(double));
+    L.total = L.scal + align256(8 * sizeof(double));
+    return L;
+}
+
+int check_dim(const char* who, int dim) {
+    if (dim < 1 || dim > frechet::kMaxDim)
+        return fail(MIGAN_ERR_INVALID, "%s: dim %d outside 1..%d", who, dim, frechet::kMaxDim);
+    return 0;
+}
+
+// Block-Jacobi sweeps on A (and V when given) until off(A) <= dim 2^-53 ||A||_F; the sweeps taken in *sweeps.
+int solve(double* A, double* V, double* J, double* part, double* scal, int dim, int N, int* sweeps, ck_stream_t s) {
+    const int nb = N / frechet::kB, groups = nb / 2;
+    const double tol = (double)dim * frechet::kEps;
+    for (int sweep = 0;; ++sweep) {
+        CUDA_TRY(comod::ck_launch(frechet::ColNormK{A, part, N}, N, s));
+        CUDA_TRY(comod::ck_launch(frechet::NormSumK{part, scal, N}, 1, s));
+        double norm[2];
+        CUDA_TRY(to_host(norm, scal, sizeof(norm), s));
+        if (!isfinite(norm[1])) return fail(MIGAN_ERR_INVALID, "frechet: the covariances are not finite");
+        if (norm[0] <= tol * tol * norm[1]) {
+            *sweeps = sweep;
+            return 0;
+        }
+        if (sweep == kMaxSweeps)
+            return fail(MIGAN_ERR_INVALID, "frechet: the eigensolver did not converge in %d sweeps (off/norm %.3g)",
+                        kMaxSweeps, sqrt(norm[0] / norm[1]));
+        for (int r = 0; r < nb - 1; ++r) {
+            CUDA_TRY(pair_launch(frechet::PairArgs{A, J, N, nb, r}, groups, s));
+            CUDA_TRY(update_launch(frechet::UpdateArgs{A, V, J, N, nb, r, groups * (groups + 1) / 2}, s));
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" {
+
+int fid_stats_mean_cov(const double* shift, const double* sum, const double* sumsq, int64_t count, int dim, double* mu,
+                       double* sigma, void* stream) {
+    if (!shift || !sum || !sumsq || !mu || !sigma) return fail(MIGAN_ERR_INVALID, "fid_stats_mean_cov: null argument");
+    if (dim < 1 || dim > 65536) return fail(MIGAN_ERR_INVALID, "fid_stats_mean_cov: dim %d outside 1..65536", dim);
+    if (count < 2) return fail(MIGAN_ERR_INVALID, "fid_stats_mean_cov: needs at least 2 rows, has %lld", (long long)count);
+    CUDA_TRY(comod::ck_launch(frechet::MeanCovK{shift, sum, sumsq, mu, sigma, dim, (double)count}, (int64_t)dim * dim,
+                              static_cast<ck_stream_t>(stream)));
+    return 0;
+}
+
+size_t fid_frechet_workspace_bytes(int dim) {
+    if (dim < 1 || dim > frechet::kMaxDim) return 0;
+    return layout(dim).total;
+}
+
+int fid_frechet_distance(const double* mu1, const double* sigma1, const double* mu2, const double* sigma2, int dim,
+                         double out[4], int* sweeps, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!mu1 || !sigma1 || !mu2 || !sigma2 || !out)
+        return fail(MIGAN_ERR_INVALID, "fid_frechet_distance: null mu1 / sigma1 / mu2 / sigma2 / out");
+    if (int rc = check_dim("fid_frechet_distance", dim)) return rc;
+    const Layout L = layout(dim);
+    if (!workspace) return fail(MIGAN_ERR_INVALID, "fid_frechet_distance: null workspace");
+    if (reinterpret_cast<uintptr_t>(workspace) % 256)
+        return fail(MIGAN_ERR_WORKSPACE, "fid_frechet_distance: workspace not 256-byte aligned");
+    if (workspace_bytes < L.total)
+        return fail(MIGAN_ERR_WORKSPACE, "fid_frechet_distance: workspace of %zu bytes, %zu needed", workspace_bytes,
+                    L.total);
+    char* ws = static_cast<char*>(workspace);
+    double* A = reinterpret_cast<double*>(ws + L.A);
+    double* V = reinterpret_cast<double*>(ws + L.V);
+    double* B = reinterpret_cast<double*>(ws + L.B);
+    double* W = reinterpret_cast<double*>(ws + L.W);
+    double* J = reinterpret_cast<double*>(ws + L.J);
+    double* sd = reinterpret_cast<double*>(ws + L.sd);
+    double* part = reinterpret_cast<double*>(ws + L.part);
+    double* scal = reinterpret_cast<double*>(ws + L.scal);
+    const int N = padded(dim);
+    const int64_t NN = (int64_t)N * N;
+    const ck_stream_t s = static_cast<ck_stream_t>(stream);
+    int sw[2] = {0, 0};
+
+    // S1 = V D V^T
+    CUDA_TRY(comod::ck_launch(frechet::LoadK{sigma1, A, V, dim, N}, NN, s));
+    CUDA_TRY(comod::ck_launch(frechet::LoadK{sigma2, B, nullptr, dim, N}, NN, s));
+    if (int rc = solve(A, V, J, part, scal, dim, N, &sw[0], s)) return rc;
+    // M = D^1/2 (V^T S2 V) D^1/2, then its eigenvalues
+    CUDA_TRY(comod::ck_launch(frechet::CutoffK{A, scal + 4, dim, N}, 1, s));
+    CUDA_TRY(comod::ck_launch(frechet::SqrtDiagK{A, scal + 4, sd, N}, N, s));
+    CUDA_TRY(gemm_launch(frechet::GemmArgs{B, V, W, N}, s));   // W = S2^T V = S2 V
+    CUDA_TRY(gemm_launch(frechet::GemmArgs{V, W, B, N}, s));   // B = V^T S2 V
+    CUDA_TRY(comod::ck_launch(frechet::ScaleK{B, sd, A, N}, NN, s));
+    if (int rc = solve(A, nullptr, J, part, scal, dim, N, &sw[1], s)) return rc;
+    CUDA_TRY(comod::ck_launch(frechet::ResultK{mu1, sigma1, mu2, sigma2, A, scal, dim, N}, 1, s));
+    CUDA_TRY(to_host(out, scal, 4 * sizeof(double), s));
+    if (sweeps) {
+        sweeps[0] = sw[0];
+        sweeps[1] = sw[1];
+    }
+    return 0;
+}
+
+}  // extern "C"

@@ -5,7 +5,9 @@
     for real in batches:
         stats.add(model(real)[0].squeeze(-1).squeeze(-1))
     mu, sigma = stats.mean_cov()                            # np.mean / np.cov(rowvar=False), float64
-    fid = calculate_frechet_distance(mu, sigma, mu2, sigma2)
+    fid = calculate_frechet_distance(mu, sigma, mu2, sigma2)   # pytorch_fid's scipy route, on the host
+    fid = stats.frechet_distance(stats_fake)                # or all on the device (float64 eigensolver)
+    fid = frechet_distance(mu, sigma, mu2, sigma2)          # the same from numpy arrays or CUDA tensors
 
 The network runs in the C-ABI library (`include/inception_b200.h`): 94 convolutions on the tensor-core implicit GEMM
 with TF32 hi / lo operands in three passes (fp32-faithful), BatchNorm folded at load time.  There is no CPU path.
@@ -14,7 +16,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, List, Tuple, Union
+from typing import Dict, List, NamedTuple, Tuple, Union
 
 import numpy as np
 import torch
@@ -51,6 +53,14 @@ SYMBOLS = [
     ("fid_stats_update", ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
 ]
+# csrc/frechet.cu: the device mean / covariance and the Fréchet distance
+FRECHET_SYMBOLS = [
+    ("fid_stats_mean_cov", ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int64, ctypes.c_int] + [ctypes.c_void_p] * 3),
+    ("fid_frechet_workspace_bytes", ctypes.c_size_t, [ctypes.c_int]),
+    ("fid_frechet_distance", ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.POINTER(ctypes.c_double),
+                                            ctypes.POINTER(ctypes.c_int), ctypes.c_void_p, ctypes.c_size_t,
+                                            ctypes.c_void_p]),
+]
 
 _bound = set()
 
@@ -61,6 +71,18 @@ def lib(handle=None):
     if id(h) not in _bound:
         _abi.bind(h, SYMBOLS)
         _bound.add(id(h))
+    return h
+
+
+_frechet_bound = set()
+
+
+def frechet_lib(handle=None):
+    """The product library (or `handle`, another build of csrc/frechet.cu) with the Fréchet symbols bound."""
+    h = lib(handle)
+    if id(h) not in _frechet_bound:
+        _abi.bind(h, FRECHET_SYMBOLS)
+        _frechet_bound.add(id(h))
     return h
 
 
@@ -257,6 +279,30 @@ class FeatureStatistics:
         sigma = (s2 - np.outer(s1, s1) / n) / (n - 1)
         return mu, sigma
 
+    def mean_cov_device(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """mean_cov() computed on the device, as float64 CUDA tensors: the same bits, and no host copy of a matrix."""
+        if self.count < 2:
+            raise ValueError("FeatureStatistics needs at least 2 feature rows, has %d" % self.count)
+        mu = torch.empty(self.dim, dtype=torch.float64, device=self.device)
+        sigma = torch.empty((self.dim, self.dim), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            _abi.check(frechet_lib().fid_stats_mean_cov(self.shift.data_ptr(), self.sum.data_ptr(), self.sumsq.data_ptr(),
+                                                self.count, self.dim, mu.data_ptr(), sigma.data_ptr(),
+                                                torch.cuda.current_stream(self.device).cuda_stream))
+        return mu, sigma
+
+    def frechet_distance(self, other: "FeatureStatistics") -> float:
+        """The FID between these statistics and `other`'s, computed on the device from both objects' sums."""
+        if not isinstance(other, FeatureStatistics):
+            raise TypeError("frechet_distance takes another FeatureStatistics")
+        if other.dim != self.dim:
+            raise ValueError("training and test covariances have different dimensions")
+        if other.device != self.device:
+            raise ValueError("both statistics must be on one device, got %s and %s" % (self.device, other.device))
+        mu1, sigma1 = self.mean_cov_device()
+        mu2, sigma2 = other.mean_cov_device()
+        return _frechet(mu1, sigma1, mu2, sigma2).fid
+
 
 def calculate_frechet_distance(mu1, sigma1, mu2, sigma2, eps: float = 1e-6) -> float:
     """||mu1 - mu2||^2 + tr(sigma1) + tr(sigma2) - 2 tr(sqrt(sigma1 sigma2)), with scipy's sqrtm on the host.  A singular
@@ -277,3 +323,92 @@ def calculate_frechet_distance(mu1, sigma1, mu2, sigma2, eps: float = 1e-6) -> f
             raise ValueError("Imaginary component {}".format(np.max(np.abs(covmean.imag))))
         covmean = covmean.real
     return float(diff.dot(diff) + np.trace(sigma1) + np.trace(sigma2) - 2 * np.trace(covmean))
+
+
+class FrechetTerms(NamedTuple):
+    """The Fréchet distance and its terms: fid = mean_term + trace1 + trace2 - 2 * trace_sqrt.  `sweeps`: the Jacobi
+    sweeps of the two eigensolves (sigma1's, then the one behind tr sqrt(sigma1 sigma2))."""
+    fid: float
+    mean_term: float
+    trace1: float
+    trace2: float
+    trace_sqrt: float
+    sweeps: Tuple[int, int]
+
+
+MAX_DIM = 4096
+_workspace: Dict[tuple, torch.Tensor] = {}
+
+
+def _check_covariance(name, x, xp) -> None:
+    """Finite, and symmetric to 1e-9 of the largest entry (xp: numpy or torch)."""
+    if not bool(xp.isfinite(x).all()):
+        raise ValueError("%s has non-finite values" % name)
+    if name.startswith("sigma") and float(xp.abs(x - x.T).max()) > 1e-9 * float(xp.abs(x).max()):
+        raise ValueError("%s is not symmetric to 1e-9 of its largest entry, so it is not a covariance" % name)
+
+
+def frechet_distance(mu1, sigma1, mu2, sigma2) -> float:
+    """||mu1 - mu2||^2 + tr(sigma1) + tr(sigma2) - 2 tr(sqrt(sigma1 sigma2)) in float64 on the GPU.
+
+    Takes float64 numpy arrays (for example np.load of a pytorch_fid .npz with `mu` and `sigma`) or CUDA tensors; host
+    arrays are uploaded once.  sigma1 and sigma2 must be covariances: finite and symmetric to 1e-9 of their largest
+    entry.  tr sqrt comes from two float64 block-Jacobi eigensolves (no matrix square root of the non-symmetric
+    product): the square roots of eigenvalues that rounding left slightly negative count as 0."""
+    return frechet_terms(mu1, sigma1, mu2, sigma2).fid
+
+
+def frechet_terms(mu1, sigma1, mu2, sigma2) -> FrechetTerms:
+    """frechet_distance() with its terms and the eigensolver's sweeps."""
+    names = ("mu1", "sigma1", "mu2", "sigma2")
+    args = [x.detach() if isinstance(x, torch.Tensor) and x.is_cuda else np.asarray(x, dtype=np.float64)
+            for x in (mu1, sigma1, mu2, sigma2)]
+    shapes = [tuple(x.shape) for x in args]
+    if len(shapes[0]) != 1 or len(shapes[2]) != 1 or len(shapes[1]) != 2 or len(shapes[3]) != 2:
+        raise ValueError("expected mu of shape [d] and sigma of shape [d, d]")
+    if shapes[0] != shapes[2]:
+        raise ValueError("training and test mean vectors have different lengths")
+    if shapes[1] != shapes[3]:
+        raise ValueError("training and test covariances have different dimensions")
+    if shapes[1] != (shapes[0][0], shapes[0][0]):
+        raise ValueError("sigma of shape %s does not match mu of length %d" % (shapes[1], shapes[0][0]))
+    if not 1 <= shapes[0][0] <= MAX_DIM:
+        raise ValueError("feature dimension %d outside 1..%d" % (shapes[0][0], MAX_DIM))
+    for name, x in zip(names, args):
+        if isinstance(x, np.ndarray):
+            _check_covariance(name, x, np)
+    cuda = [x for x in args if isinstance(x, torch.Tensor)]
+    device = cuda[0].device if cuda else torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+        t = []
+        for name, x in zip(names, args):
+            if isinstance(x, torch.Tensor):
+                x = x.to(device=device, dtype=torch.float64).contiguous()
+                _check_covariance(name, x, torch)
+            else:
+                x = torch.from_numpy(np.ascontiguousarray(x)).to(device)
+            t.append(x)
+        return _frechet(*t)
+
+
+def _frechet(mu1, sigma1, mu2, sigma2, handle=None) -> FrechetTerms:
+    """The library call on float64 contiguous CUDA tensors of one device."""
+    L = frechet_lib(handle)
+    d = int(mu1.shape[0])
+    if d < 1 or d > MAX_DIM:
+        raise ValueError("feature dimension %d outside 1..%d" % (d, MAX_DIM))
+    device = mu1.device
+    key = (device, d)
+    ws = _workspace.get(key)
+    if ws is None:
+        _workspace.clear()
+        ws = torch.empty(int(L.fid_frechet_workspace_bytes(d)), dtype=torch.uint8, device=device)
+        _workspace[key] = ws
+    out = (ctypes.c_double * 4)()
+    sweeps = (ctypes.c_int * 2)()
+    with torch.cuda.device(device):
+        _abi.check(L.fid_frechet_distance(mu1.data_ptr(), sigma1.data_ptr(), mu2.data_ptr(), sigma2.data_ptr(), d, out,
+                                          sweeps, ws.data_ptr(), ws.numel(),
+                                          torch.cuda.current_stream(device).cuda_stream), L)
+    fid = out[0] + out[1] + out[2] - 2 * out[3]
+    return FrechetTerms(float(fid), out[0], out[1], out[2], out[3], (sweeps[0], sweeps[1]))
