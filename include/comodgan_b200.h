@@ -58,6 +58,28 @@ int comodgan_forward(comodgan_ctx* ctx, const float* x, const float* z, float* y
                      float truncation_psi, int truncation_cutoff, int noise_mode, const float* noise,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* Seeded noise: reproducible per-request draws for RANDOM mode, generated on the device.  Request i (seed s_i) has
+ * streams p = 0 (z, 512 values) and p = 1 + j (noise plane j, r_j * r_j values, row-major).  Stream p is numpy's
+ * Philox4x64-10 with key [s_i, p] and a zero counter, i.e. the words of
+ *     np.random.Philox(key=np.array([s_i, p], np.uint64)).random_raw(m);
+ * values 2t and 2t+1 come from words a = w[2t], b = w[2t+1] by Box-Muller in double: u1 = ((a >> 11) + 1) 2^-53,
+ * u2 = (b >> 11) 2^-53, rho = sqrt(-2 ln u1), (rho cos 2 pi u2, rho sin 2 pi u2), each rounded once to float.
+ * A request's values do not depend on n or on its position in the call.
+ *
+ * comodgan_seeded_noise: z[n,512] (NULL: not drawn) and the planes in comodgan_forward's RANDOM layout (NULL: not drawn)
+ * for n host seeds.  One launch per 64 requests; the seeds travel in the kernel parameters (no copy, no synchronisation).
+ * Device pointers 16-byte aligned.  Asynchronous on `stream`; the context needs a device but not its weights. */
+int comodgan_seeded_noise(const comodgan_ctx* ctx, const uint64_t* seeds_host, int n,
+                          float* z_or_null, float* planes_or_null, void* stream);
+/* Workspace of comodgan_forward_seeded: the planes, z, then comodgan_workspace_bytes(ctx, n). */
+size_t comodgan_workspace_bytes_seeded(const comodgan_ctx* ctx, int n);
+/* Draws the planes (and z when z_or_null is NULL) into the workspace, then runs comodgan_forward in RANDOM mode on them:
+ * y equals comodgan_forward(..., COMODGAN_NOISE_RANDOM, planes) on the same planes, byte for byte.  Asynchronous. */
+int comodgan_forward_seeded(comodgan_ctx* ctx, const float* x, const uint64_t* seeds_host, const float* z_or_null,
+                            float* y, int n, float truncation_psi, int truncation_cutoff,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
+/* Kernel launches of the last comodgan_forward / comodgan_forward_seeded (the latter's noise launches included). */
 int comodgan_last_launch_count(const comodgan_ctx* ctx);
 
 /* Debug/test tap (see migan_set_tap): copy the named intermediate, as NCHW fp32, into dst during the next forwards.

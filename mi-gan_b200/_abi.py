@@ -182,6 +182,10 @@ COMOD_SYMBOLS = [
     ("comodgan_noise_plane_res", c_int, [c_void_p, c_int]),
     ("comodgan_forward", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_int, c_void_p,
                                  c_void_p, c_size_t, c_void_p]),
+    ("comodgan_seeded_noise", c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    ("comodgan_workspace_bytes_seeded", c_size_t, [c_void_p, c_int]),
+    ("comodgan_forward_seeded", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int,
+                                        c_void_p, c_size_t, c_void_p]),
     ("comodgan_last_launch_count", c_int, [c_void_p]),
     ("comodgan_set_tap", c_int, [c_void_p, c_char_p, c_void_p]),
     ("b200_conv2d_resample", c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 18 +

@@ -3,21 +3,27 @@
 from __future__ import annotations
 
 import ctypes
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
 
+from . import comodgan
 from .generator import Generator
 
 
-def load_generator(pipeline: torch.nn.Module, model_or_state_dict, resolution: int, device) -> Generator:
+def load_generator(pipeline: torch.nn.Module, model_or_state_dict, resolution: int, device, accept_comodgan: bool = False):
     """The generator of `pipeline`, on the CUDA `device` in eval mode.  `model_or_state_dict`: a `migan_b200.Generator` of
-    that resolution, a state_dict, or a file `torch.load` reads one from."""
+    that resolution, a state_dict, or a file `torch.load` reads one from.  With `accept_comodgan`, also a
+    `migan_b200.comodgan.Generator` of that resolution (Co-Mod-GAN checkpoints come in through `comodgan.load`)."""
     device = torch.device(device)
     if device.type != "cuda":
         raise RuntimeError("migan_b200.%s runs on a CUDA device (there is no CPU path); got %s" % (type(pipeline).__name__, device))
-    if isinstance(model_or_state_dict, Generator):
+    if accept_comodgan and isinstance(model_or_state_dict, comodgan.Generator):
+        if model_or_state_dict.img_resolution != resolution:
+            raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_or_state_dict.img_resolution, resolution))
+        model = model_or_state_dict
+    elif isinstance(model_or_state_dict, Generator):
         if model_or_state_dict.resolution != resolution:
             raise RuntimeError("generator resolution %d != pipeline resolution %d" % (model_or_state_dict.resolution, resolution))
         model = model_or_state_dict
@@ -26,6 +32,49 @@ def load_generator(pipeline: torch.nn.Module, model_or_state_dict, resolution: i
         sd = model_or_state_dict if isinstance(model_or_state_dict, dict) else torch.load(model_or_state_dict, map_location="cpu")
         model.load_state_dict(sd)
     return model.to(device).eval()
+
+
+class NoiseSeeds:
+    """The noise seeds of a pipeline that accepts a Co-Mod-GAN generator, and its generator chunking.
+
+    The k-th image the pipeline processes without explicit seeds, counted across calls, gets the seed
+    noise_seed * 2**32 + k (k = `noise_index`, readable and settable).  A Co-Mod-GAN pass runs its generator in chunks of
+    at most `generator_batch` images.  MI-GAN generators draw no noise: they take no seeds and run the pass whole."""
+
+    def __init__(self, model, noise_seed: int, generator_batch: int):
+        if not 0 <= int(noise_seed) < 1 << 32:
+            raise ValueError("noise_seed must lie in [0, 2**32), got %d" % noise_seed)
+        if int(generator_batch) < 1:
+            raise ValueError("generator_batch must be >= 1, got %d" % generator_batch)
+        self.comodgan = isinstance(model, comodgan.Generator)
+        self.noise_seed, self.generator_batch, self.noise_index = int(noise_seed), int(generator_batch), 0
+
+    def take(self, name: str, n: int, seeds) -> Optional[np.ndarray]:
+        """The uint64 seeds of the next n images (None for MI-GAN); `seeds` overrides the counter, which then stays."""
+        if not self.comodgan:
+            if seeds is not None:
+                raise ValueError("%s.forward_batch: seeds= needs a Co-Mod-GAN generator; MI-GAN draws no noise" % name)
+            return None
+        if seeds is not None:
+            out = comodgan.seed_array(seeds)
+            if len(out) != n:
+                raise ValueError("%s.forward_batch: %d seeds for %d images" % (name, len(out), n))
+            return out
+        k0, self.noise_index = self.noise_index, self.noise_index + n
+        return np.array([(self.noise_seed << 32) + k for k in range(k0, k0 + n)], dtype=np.uint64)
+
+    def run(self, model, x: torch.Tensor, seeds: Optional[np.ndarray]) -> Tuple[torch.Tensor, int]:
+        """(y, launches): the generator over x [n, 4, R, R], in chunks for Co-Mod-GAN, and its kernel launches."""
+        if seeds is None:
+            y = model(x)
+            return y, model.last_launch_count()
+        n, gb = x.shape[0], self.generator_batch
+        y = torch.empty((n, 3, x.shape[2], x.shape[3]), dtype=torch.float32, device=x.device)
+        launches = 0
+        for c in range(0, n, gb):
+            model(x[c:c + gb], seeds=seeds[c:c + gb], _out=y[c:c + gb])
+            launches += model.last_launch_count()
+        return y, launches
 
 
 def _to(t: torch.Tensor, device, non_blocking: bool) -> torch.Tensor:
@@ -47,9 +96,9 @@ class _Call:
 class _Queued(torch.nn.Module):
     """A pipeline whose calls may only be enqueued (`forward_batch(..., wait=False)`) and waited for later."""
 
-    def __init__(self, model_or_state_dict, resolution: int, device):
+    def __init__(self, model_or_state_dict, resolution: int, device, accept_comodgan: bool = False):
         super().__init__()
-        self.model = load_generator(self, model_or_state_dict, resolution, device)
+        self.model = load_generator(self, model_or_state_dict, resolution, device, accept_comodgan)
         self.res = int(resolution)
         self._pending: List[_Call] = []                     # calls of forward_batch(..., wait=False) not yet waited for
 
@@ -79,8 +128,8 @@ class _PhotoPipeline(_Queued):
     """What the photo pipelines share: HWC uint8 photos as numpy arrays or CPU / CUDA tensors, their checks, one generator
     workspace and the copy of the results back to the host."""
 
-    def __init__(self, model_or_state_dict, resolution: int, device):
-        super().__init__(model_or_state_dict, resolution, device)
+    def __init__(self, model_or_state_dict, resolution: int, device, accept_comodgan: bool = False):
+        super().__init__(model_or_state_dict, resolution, device, accept_comodgan)
         self._ws = None                                      # the generator workspace, grown to the largest chunk seen
 
     @classmethod

@@ -17,6 +17,7 @@ import ctypes
 import math
 from typing import Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -165,14 +166,15 @@ class _Engine:
         _abi.check(self.lib.comodgan_finalize_weights(self.handle))
         self.weights_version = version
 
-    def workspace(self, n: int) -> torch.Tensor:
-        ws = self.workspaces.get(n)
+    def workspace(self, n: int, seeded: bool = False) -> torch.Tensor:
+        ws = self.workspaces.get((n, seeded))
         if ws is None:
-            nbytes = self.lib.comodgan_workspace_bytes(self.handle, n)
+            size = self.lib.comodgan_workspace_bytes_seeded if seeded else self.lib.comodgan_workspace_bytes
+            nbytes = size(self.handle, n)
             raw = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
             off = (-raw.data_ptr()) % 1024
             ws = raw[off:off + nbytes]
-            self.workspaces = {n: ws}
+            self.workspaces = {(n, seeded): ws}
         return ws
 
 
@@ -212,7 +214,7 @@ class Generator(nn.Module):
             eng.upload(self.img_resolution, self.state_dict(keep_vars=True), version)
         return eng
 
-    def _validate(self, x, z):
+    def _validate(self, x, z, draw_z: bool = True):
         r = self.img_resolution
         if not isinstance(x, torch.Tensor) or x.dim() != 4 or tuple(x.shape[1:]) != (4, r, r):
             raise RuntimeError("expected x of shape [N, 4, %d, %d] (mask-0.5, img*mask)" % (r, r))
@@ -226,6 +228,8 @@ class Generator(nn.Module):
         if next(self.parameters()).device != x.device:
             raise RuntimeError("input is on %s but the module parameters are on %s" % (x.device, next(self.parameters()).device))
         if z is None:
+            if not draw_z:
+                return x.contiguous(), None
             z = torch.randn([x.shape[0], 512]).to(x.device)          # comodgan.py:444-445
         if tuple(z.shape) != (x.shape[0], self.z_dim):
             raise RuntimeError("expected z of shape [%d, %d], got %s" % (x.shape[0], self.z_dim, tuple(z.shape)))
@@ -233,41 +237,78 @@ class Generator(nn.Module):
 
     @torch.no_grad()
     def forward(self, x, z=None, c=None, truncation_psi=1, truncation_cutoff=None, noise_mode="random",
-                return_intermediate_outs=False, *, noise: Optional[torch.Tensor] = None, _tap=None):
+                return_intermediate_outs=False, *, noise: Optional[torch.Tensor] = None, seeds=None, _tap=None,
+                _out: Optional[torch.Tensor] = None):
         """x: 4-channel mask+rgb input.  `noise` (optional, noise_mode='random'): the N(0,1) planes to use instead of
-        fresh torch.randn draws, concatenated in forward order (see `noise_plane_shapes`)."""
+        fresh torch.randn draws, concatenated in forward order (see `noise_plane_shapes`).  `seeds` (optional,
+        noise_mode='random'): one 64-bit seed per image, a sequence or an int64 / uint64 tensor; the planes, and z when it
+        is None, are then drawn on the device from the seeded streams of `seeded_noise`, so image i's draws depend on
+        seeds[i] alone."""
         if c is not None:
             raise NotImplementedError("conditional mapping (c_dim > 0) is not part of the Co-Mod-GAN demo configuration")
         if return_intermediate_outs:
             raise NotImplementedError("return_intermediate_outs is a training-loss hook (lib/experiments/loss.py); not built")
         if noise_mode not in NOISE_MODES:
             raise AssertionError("noise_mode must be one of %s" % sorted(NOISE_MODES))      # stylegan.py:282
-        x, z = self._validate(x, z)
+        if seeds is not None:
+            if noise_mode != "random":
+                raise ValueError("seeds draw the random noise planes: they need noise_mode='random', got %r" % noise_mode)
+            if noise is not None:
+                raise ValueError("pass seeds or noise, not both")
+            seeds = seed_array(seeds)
+        x, z = self._validate(x, z) if seeds is None else self._validate(x, z, draw_z=False)
         n, r = x.shape[0], self.img_resolution
+        if seeds is not None and len(seeds) != n:
+            raise ValueError("%d seeds for %d images" % (len(seeds), n))
         with _guard(x.device):
             eng = self._engine(x.device)
             planes = None
-            if noise_mode == "random":
+            if noise_mode == "random" and seeds is None:
                 total = n * sum(v * v for v in eng.noise_res)
                 planes = torch.randn(total, device=x.device) if noise is None else noise.to(x.device, torch.float32).contiguous().reshape(-1)
                 if planes.numel() != total:
                     raise RuntimeError("noise must hold %d values" % total)
-            y = torch.empty((n, 3, r, r), dtype=torch.float32, device=x.device)
-            ws = eng.workspace(n)
+            y = torch.empty((n, 3, r, r), dtype=torch.float32, device=x.device) if _out is None else _out
+            ws = eng.workspace(n, seeded=seeds is not None)
             stream = _stream(x.device)
             tap_buf = None
             if _tap is not None:
                 tap_buf = torch.zeros((n,) + tuple(_tap[1]), dtype=torch.float32, device=x.device)
                 _abi.check(eng.lib.comodgan_set_tap(eng.handle, _tap[0].encode(), tap_buf.data_ptr()))
+            psi, cutoff = float(truncation_psi), -1 if truncation_cutoff is None else int(truncation_cutoff)
             try:
-                _abi.check(eng.lib.comodgan_forward(
-                    eng.handle, x.data_ptr(), z.data_ptr(), y.data_ptr(), n, float(truncation_psi),
-                    -1 if truncation_cutoff is None else int(truncation_cutoff), NOISE_MODES[noise_mode],
-                    planes.data_ptr() if planes is not None else None, ws.data_ptr(), ws.numel(), stream))
+                if seeds is not None:
+                    _abi.check(eng.lib.comodgan_forward_seeded(
+                        eng.handle, x.data_ptr(), seeds.ctypes.data, z.data_ptr() if z is not None else None, y.data_ptr(),
+                        n, psi, cutoff, ws.data_ptr(), ws.numel(), stream))
+                else:
+                    _abi.check(eng.lib.comodgan_forward(
+                        eng.handle, x.data_ptr(), z.data_ptr(), y.data_ptr(), n, psi, cutoff, NOISE_MODES[noise_mode],
+                        planes.data_ptr() if planes is not None else None, ws.data_ptr(), ws.numel(), stream))
             finally:
                 if _tap is not None:
                     eng.lib.comodgan_set_tap(eng.handle, None, None)
         return (y, tap_buf) if _tap is not None else y
+
+    @torch.no_grad()
+    def seeded_noise(self, seeds) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(z [n, 512], planes) that `forward(..., seeds=seeds)` draws, as CUDA tensors on the module's device.  planes is
+        flat, in `forward(noise=...)`'s layout.  Request i's stream p (0: z, 1 + j: noise plane j) is numpy's
+        Philox4x64-10 with key [seeds[i], p], turned into normals by float64 Box-Muller (include/comodgan_b200.h)."""
+        seeds = seed_array(seeds)
+        n = len(seeds)
+        if n == 0:
+            raise ValueError("no seeds")
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("migan_b200.comodgan.Generator runs on a CUDA device; the module is on %s" % dev)
+        with _guard(dev):
+            eng = self._engine(dev)
+            z = torch.empty((n, self.z_dim), dtype=torch.float32, device=dev)
+            planes = torch.empty(n * sum(v * v for v in eng.noise_res), dtype=torch.float32, device=dev)
+            _abi.check(eng.lib.comodgan_seeded_noise(eng.handle, seeds.ctypes.data, n, z.data_ptr(), planes.data_ptr(),
+                                                     _stream(dev)))
+        return z, planes
 
     def noise_plane_shapes(self, n: int):
         """[(n, r, r)] of the planes `forward(..., noise_mode='random', noise=...)` consumes, in order."""
@@ -277,3 +318,34 @@ class Generator(nn.Module):
     def last_launch_count(self) -> int:
         eng = next(iter(self._engines.values()))
         return int(eng.lib.comodgan_last_launch_count(eng.handle))
+
+
+def seed_array(seeds) -> np.ndarray:
+    """`seeds` (a sequence of ints in [0, 2**64) or an int64 / uint64 tensor, whose bits are taken as they are) as a
+    contiguous uint64 numpy array."""
+    if isinstance(seeds, torch.Tensor):
+        if seeds.dtype not in (torch.int64, torch.uint64) or seeds.dim() != 1:
+            raise ValueError("seeds must be a 1-D int64 or uint64 tensor, got %s %s" % (seeds.dtype, tuple(seeds.shape)))
+        return np.ascontiguousarray(seeds.detach().cpu().view(torch.int64).numpy().view(np.uint64))
+    seeds = [int(s) for s in seeds]
+    if any(s < 0 or s >= 1 << 64 for s in seeds):
+        raise ValueError("seeds must lie in [0, 2**64)")
+    return np.array(seeds, dtype=np.uint64)
+
+
+def load(model_or_state_dict_or_path, resolution: int) -> Generator:
+    """The Co-Mod-GAN generator of scripts/demo.py (:95-106) in eval mode: `Generator(Mapping(num_ws), Encoder(R),
+    Synthesis(R))` with num_ws = 14 at 256 and 16 at 512, loaded from a state_dict or a file `torch.load` reads one from.
+    A `Generator` of that resolution is returned as it is, in eval mode."""
+    resolution = int(resolution)
+    if isinstance(model_or_state_dict_or_path, Generator):
+        if model_or_state_dict_or_path.img_resolution != resolution:
+            raise ValueError("generator resolution %d != %d" % (model_or_state_dict_or_path.img_resolution, resolution))
+        return model_or_state_dict_or_path.eval()
+    synthesis = Synthesis(resolution=resolution)
+    g = Generator(Mapping(num_ws=synthesis.num_ws), Encoder(resolution=resolution), synthesis)
+    sd = model_or_state_dict_or_path
+    if not isinstance(sd, dict):
+        sd = torch.load(sd, map_location="cpu")
+    g.load_state_dict(sd)
+    return g.eval()

@@ -366,4 +366,94 @@ struct ConcatK {       // items = n*(Da+Db): out[n] = [a[n] | b[n]]             
     }
 };
 
+// ---- seeded noise: per-request N(0,1) streams (include/comodgan_b200.h, comodgan_seeded_noise) -----------------------
+// Stream p of request k is numpy's Philox4x64-10 with key [seed_k, p] and a zero counter: block b (words 4b .. 4b+3 of
+// `np.random.Philox(key=...).random_raw`) is the cipher of counter [b + 1, 0, 0, 0] -- numpy increments before the first
+// block.  Words a = w[2t], b = w[2t+1] give values 2t, 2t+1 by Box-Muller in double, each rounded once to float.
+constexpr int kNoiseMaxRequests = 64;     // requests per launch
+constexpr int kNoiseMaxStreams = 32;      // z and the noise planes of one request (1 + 2 * (log2(R) - 2) <= 32)
+
+CK_HD uint64_t mulhi64(uint64_t a, uint64_t b) {
+#ifdef __CUDA_ARCH__
+    return __umul64hi(a, b);
+#else
+    return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+
+// The four 64-bit words of block `blk` of the stream with key (k0, k1).
+CK_HD void philox4x64_10(uint64_t blk, uint64_t k0, uint64_t k1, uint64_t w[4]) {
+    uint64_t c0 = blk + 1, c1 = 0, c2 = 0, c3 = 0;
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
+        const uint64_t lo0 = 0xD2E7470EE14C6C93ull * c0, hi0 = mulhi64(0xD2E7470EE14C6C93ull, c0);
+        const uint64_t lo1 = 0xCA5A826395121157ull * c2, hi1 = mulhi64(0xCA5A826395121157ull, c2);
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+    }
+    w[0] = c0; w[1] = c1; w[2] = c2; w[3] = c3;
+}
+
+// cos t and sin t for 0 <= t < 2 pi, within about one double ulp.  The device's cos / sin carry a Payne-Hanek path for
+// huge arguments that costs a 40-byte stack frame; t < 2 pi needs only a Cody-Waite reduction by pi/2 and fdlibm's
+// kernels on [-pi/4, pi/4].  Every multiply-add is an explicit fma, so the device and the emulation build round alike.
+CK_HD void cos_sin_2pi(double t, double* c, double* s) {
+    const double kd = rint(t * 0.63661977236758134308);                     // quadrant, 0 .. 4
+    const double r = fma(-kd, 6.07710050650619224932e-11, fma(-kd, 1.57079632673412561417e+00, t));
+    const double z = r * r;
+    const double ps = fma(z, fma(z, fma(z, fma(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08),
+                                        2.75573137070700676789e-06), -1.98412698298579493134e-04), 8.33333333332248946124e-03);
+    const double sr = fma(r * z, fma(z, ps, -1.66666666666666324348e-01), r);
+    const double pc = fma(z, fma(z, fma(z, fma(z, fma(z, -1.13596475577881948265e-11, 2.08757232129817482790e-09),
+                                                -2.75573143513906633035e-07), 2.48015872894767294178e-05),
+                                 -1.38888888888741095749e-03), 4.16666666666666019037e-02);
+    const double cr = 1.0 - fma(0.5, z, -(z * z) * pc);
+    switch ((int)kd & 3) {
+        case 0: *c = cr; *s = sr; break;
+        case 1: *c = -sr; *s = cr; break;
+        case 2: *c = -cr; *s = -sr; break;
+        default: *c = sr; *s = -cr; break;
+    }
+}
+
+// (rho cos 2 pi u2, rho sin 2 pi u2), u1 = ((a >> 11) + 1) 2^-53 in (0, 1], u2 = (b >> 11) 2^-53, rho = sqrt(-2 ln u1).
+CK_HD void box_muller(uint64_t a, uint64_t b, float* v0, float* v1) {
+    const double u1 = (double)((a >> 11) + 1) * 0x1.0p-53, u2 = (double)(b >> 11) * 0x1.0p-53;
+    const double rho = sqrt(-2.0 * log(u1));
+    double c, s;
+    cos_sin_2pi(6.283185307179586 * u2, &c, &s);
+    *v0 = (float)(rho * c);
+    *v1 = (float)(rho * s);
+}
+
+// One launch over up to kNoiseMaxRequests requests.  Every request has the same streams: stream q holds blk0[q + 1] -
+// blk0[q] Philox blocks (4 values each) and writes them to out[q] + k * stride[q], k the request's index in the launch.
+struct SeededNoiseBatch {
+    int64_t start[kNoiseMaxRequests + 1];     // item prefix: start[k] = k * blk0[ns]
+    uint64_t seed[kNoiseMaxRequests];
+    int64_t blk0[kNoiseMaxStreams + 1];       // first block of each stream within a request; blk0[ns] = blocks per request
+    float* out[kNoiseMaxStreams];
+    int64_t stride[kNoiseMaxStreams];         // floats between consecutive requests of stream q
+    uint64_t id[kNoiseMaxStreams];            // p: 0 = z, 1 + j = noise plane j
+    int n, ns;
+};
+static_assert(sizeof(SeededNoiseBatch) <= 4000, "the noise descriptor must fit the classic 4 KB kernel parameter space");
+
+struct SeededNoiseK {  // items = n * blk0[ns]: one Philox block -> four values, one 16-byte store
+    const SeededNoiseBatch& b;
+    CK_HD void operator()(int64_t i) const {
+        const int64_t per = b.blk0[b.ns];
+        const int k = (int)(i / per);
+        const int64_t j = i - (int64_t)k * per;
+        const int q = find_request(b.blk0, b.ns, j);
+        const int64_t blk = j - b.blk0[q];
+        uint64_t w[4];
+        philox4x64_10((uint64_t)blk, b.seed[k], b.id[q], w);
+        f4 v;
+        box_muller(w[0], w[1], &v.x, &v.y);
+        box_muller(w[2], w[3], &v.z, &v.w);
+        st4(b.out[q] + k * b.stride[q] + 4 * blk, v);
+    }
+};
+
 }  // namespace comod

@@ -830,6 +830,81 @@ int comodgan_forward(comodgan_ctx* c, const float* x, const float* z, float* y, 
     return rc;
 }
 
+// Launches of comodgan_seeded_noise for n requests (one per kNoiseMaxRequests); -1 and the error set on a bad argument.
+static int seeded_noise(const comodgan_ctx* c, const uint64_t* seeds, int n, float* z, float* planes, void* stream) {
+    if (int rc = check_ctx(c)) return -rc;
+    if (!seeds || n <= 0) return -fail(MIGAN_ERR_INVALID, "seeded noise: null seeds or n <= 0");
+    if (!z && !planes) return -fail(MIGAN_ERR_INVALID, "seeded noise: neither z nor planes given");
+    if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(planes)) & 15)
+        return -fail(MIGAN_ERR_INVALID, "seeded noise: z and planes must be 16-byte aligned");
+    if (c->device < 0) return -fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
+    if (int e = dev_set(c->device)) return -fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
+    const int np = comodgan_num_noise_planes(c);
+    int launches = 0;
+    for (int k0 = 0; k0 < n; k0 += kNoiseMaxRequests) {
+        SeededNoiseBatch b;
+        b.n = std::min(kNoiseMaxRequests, n - k0);
+        b.ns = 0;
+        int64_t blocks = 0, plane_off = 0;   // plane_off: floats of the planes before plane j, per request
+        auto add = [&](float* out, int64_t stride, uint64_t id, int64_t values) {
+            b.out[b.ns] = out; b.stride[b.ns] = stride; b.id[b.ns] = id; b.blk0[b.ns] = blocks;
+            blocks += values / 4;
+            ++b.ns;
+        };
+        if (z) add(z + (int64_t)k0 * Z_DIM, Z_DIM, 0, Z_DIM);
+        for (int j = 0; j < np; ++j) {
+            const int64_t r2 = (int64_t)comodgan_noise_plane_res(c, j) * comodgan_noise_plane_res(c, j);
+            if (planes) add(planes + plane_off * n + k0 * r2, r2, 1 + (uint64_t)j, r2);
+            plane_off += r2;
+        }
+        b.blk0[b.ns] = blocks;
+        for (int k = 0; k < b.n; ++k) { b.seed[k] = seeds[k0 + k]; b.start[k] = k * blocks; }
+        b.start[b.n] = b.n * blocks;
+        if (const int e = (int)batch_launch<SeededNoiseK>(b, static_cast<ck_stream_t>(stream)))
+            return -fail(MIGAN_ERR_CUDA, "seeded noise launch failed: %s", dev_err(e));
+        ++launches;
+    }
+    return launches;
+}
+
+int comodgan_seeded_noise(const comodgan_ctx* c, const uint64_t* seeds_host, int n, float* z, float* planes, void* stream) {
+    const int launches = seeded_noise(c, seeds_host, n, z, planes, stream);
+    return launches < 0 ? -launches : 0;
+}
+
+// Everything comodgan_forward_seeded places in its workspace: the planes, z, then the forward's own workspace.
+static size_t seeded_planes_bytes(const comodgan_ctx* c, int n) {
+    size_t per = 0;
+    for (int j = 0; j < comodgan_num_noise_planes(c); ++j) per += (size_t)comodgan_noise_plane_res(c, j) * comodgan_noise_plane_res(c, j);
+    return align_up(per * n * sizeof(float), 256);
+}
+
+size_t comodgan_workspace_bytes_seeded(const comodgan_ctx* c, int n) {
+    const size_t fwd = comodgan_workspace_bytes(c, n);
+    if (!fwd) return 0;
+    return seeded_planes_bytes(c, n) + align_up((size_t)n * Z_DIM * sizeof(float), 256) + fwd;
+}
+
+int comodgan_forward_seeded(comodgan_ctx* c, const float* x, const uint64_t* seeds_host, const float* z, float* y, int n,
+                            float truncation_psi, int truncation_cutoff, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = check_ctx(c)) return rc;
+    if (!c->finalized) return fail(MIGAN_ERR_STATE, "forward before comodgan_finalize_weights");
+    if (!x || !y || !seeds_host || n <= 0) return fail(MIGAN_ERR_INVALID, "bad x / seeds / y / n");
+    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(MIGAN_ERR_WORKSPACE, "workspace null or not 256-byte aligned");
+    const size_t need = comodgan_workspace_bytes_seeded(c, n);
+    if (workspace_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "workspace too small: need %zu bytes, have %zu", need, workspace_bytes);
+    char* ws = static_cast<char*>(workspace);
+    float* planes = reinterpret_cast<float*>(ws);
+    const size_t zoff = seeded_planes_bytes(c, n), foff = zoff + align_up((size_t)n * Z_DIM * sizeof(float), 256);
+    float* zs = z ? nullptr : reinterpret_cast<float*>(ws + zoff);
+    const int launches = seeded_noise(c, seeds_host, n, zs, planes, stream);
+    if (launches < 0) return -launches;
+    const int rc = comodgan_forward(c, x, z ? z : zs, y, n, truncation_psi, truncation_cutoff, COMODGAN_NOISE_RANDOM, planes,
+                                    ws + foff, workspace_bytes - foff, stream);
+    if (!rc) c->last_launches += launches;
+    return rc;
+}
+
 int comodgan_last_launch_count(const comodgan_ctx* c) { return c ? c->last_launches : 0; }
 
 int comodgan_set_tap(comodgan_ctx* c, const char* name, float* dst) {

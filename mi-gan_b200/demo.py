@@ -16,8 +16,10 @@ include/migan_b200.h, one launch per stage for every request):
     -> height pass + composite
 
 OpenCV's cubic resize is reproduced as its scalar path computes it (`cv2.setUseOptimized(False)`); OpenCV's default
-optimised path differs from it by at most 1 in a small fraction of values.  The generator's output does not depend on the
-batch size, so request i of a batch gets the bytes of a call with request i alone.  There is no CPU path.
+optimised path differs from it by at most 1 in a small fraction of values.  MI-GAN's output does not depend on the
+batch size, so request i of a batch gets the bytes of a call with request i alone.  Co-Mod-GAN's does (one style RMS over
+the batch, stylegan.py:146): its requests get the same bytes for the same `generator_batch` chunking.  There is no CPU
+path.
 """
 from __future__ import annotations
 
@@ -26,9 +28,11 @@ from typing import List, Sequence, Tuple, Union
 import torch
 
 from . import _abi
-from ._request_path import _PhotoPipeline, _to
+from ._request_path import NoiseSeeds, _PhotoPipeline, _to
 
 MASK_MAX = 512          # read_mask's first resize (demo.py:28)
+# Co-Mod-GAN images per generator forward: its workspace is 9.8 GiB at 16 images of 512^2 (5.7 GiB at 256^2)
+GENERATOR_BATCH = 16
 
 
 def resized_size(w: int, h: int, max_size: int) -> Tuple[int, int]:
@@ -40,21 +44,35 @@ def resized_size(w: int, h: int, max_size: int) -> Tuple[int, int]:
 
 
 class DemoPipeline(_PhotoPipeline):
-    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from."""
+    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from; or a
+    `migan_b200.comodgan.Generator` of the same resolution (see `comodgan.load`).  Co-Mod-GAN draws its noise planes and
+    z from seeded streams on the device: the k-th image processed gets seed `noise_seed * 2**32 + k` (`noise_index` = k)
+    unless `forward_batch(..., seeds=...)` names them, and the generator runs in chunks of at most `generator_batch`."""
 
-    def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda"):
-        super().__init__(model_or_state_dict, resolution, device)
+    def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda", *,
+                 noise_seed: int = 0, generator_batch: int = GENERATOR_BATCH):
+        super().__init__(model_or_state_dict, resolution, device, accept_comodgan=True)
         self.device_ = torch.device(device)
+        self.noise = NoiseSeeds(self.model, noise_seed, generator_batch)
         self.last_sizes: List[Tuple[int, int]] = []       # (w', h') of every result of the last completed call(s)
-        self.last_launches = 0                             # kernel launches (generator excluded) of the last pass
+        self.last_launches = 0                             # kernel launches of the last pass (MI-GAN: generator excluded)
+
+    @property
+    def noise_index(self) -> int:
+        """How many images have drawn their Co-Mod-GAN noise from the pipeline's counter; settable."""
+        return self.noise.noise_index
+
+    @noise_index.setter
+    def noise_index(self, k: int) -> None:
+        self.noise.noise_index = int(k)
 
     def _set_record(self, record: list) -> None:
         self.last_sizes = record
 
     # -- one pass ---------------------------------------------------------------------------------------------------
-    def _pass(self, imgs, masks, inverts, outs) -> None:
+    def _pass(self, imgs, masks, inverts, outs, seeds) -> None:
         """Enqueue one pass over <= 32 requests: imgs [H,W,3] / masks [Hm,Wm,C] uint8 CUDA contiguous, outs [h',w',3]
-        uint8 CUDA contiguous, all on one device."""
+        uint8 CUDA contiguous, all on one device; seeds: the pass's Co-Mod-GAN seeds (None for MI-GAN)."""
         lib = _abi.load()
         n = len(imgs)
         dev = imgs[0].device
@@ -73,12 +91,12 @@ class DemoPipeline(_PhotoPipeline):
             scratch = torch.empty(need, dtype=torch.uint8, device=dev)
             x = torch.empty((n, 4, self.res, self.res), dtype=torch.float32, device=dev)
             _abi.check(lib.b200_demo_preprocess(reqs, n, self.res, x.data_ptr(), scratch.data_ptr(), need, stream))
-            y = self.model(x)
+            y, gen_launches = self.noise.run(self.model, x, seeds)
             if y.dtype != torch.float32 or tuple(y.shape) != (n, 3, self.res, self.res) or not y.is_contiguous():
                 raise RuntimeError("generator output must be contiguous float32 (%d,3,%d,%d)" % (n, self.res, self.res))
             _abi.check(lib.b200_demo_postprocess(y.data_ptr(), reqs, n, self.res, scratch.data_ptr(), need, stream))
         down = any((int(r.out_w), int(r.out_h)) != (int(r.W), int(r.H)) for r in reqs)
-        self.last_launches = 2 + (2 if down else 0) + 2
+        self.last_launches = 2 + (2 if down else 0) + 2 + (gen_launches if seeds is not None else 0)
 
     # -- public calls -----------------------------------------------------------------------------------------------
     def _check_mask_size(self, i, img, mask) -> None:
@@ -98,15 +116,18 @@ class DemoPipeline(_PhotoPipeline):
 
     @torch.no_grad()
     def forward_batch(self, imgs: Sequence, masks: Sequence, invert: Union[bool, Sequence[bool]] = False,
-                      wait: bool = True) -> list:
+                      wait: bool = True, seeds=None) -> list:
         """Many requests of any sizes, one pass per 32.  imgs[i]: uint8 [H,W,3]; masks[i]: uint8 [Hm,Wm] or [Hm,Wm,C];
         numpy arrays or CPU / CUDA tensors; `invert` one flag or one per request.  Returns the composed images, uint8
         [h',w',3]: numpy for numpy photos, a tensor on the photo's device otherwise.  `last_sizes` holds every (w', h').
 
         wait=False only enqueues the work on the current stream and returns the output tensors, which hold the results
         (and `last_sizes` is set) after `wait()`.  CPU photos must then be pinned tensors (`pin_memory()`), since they are
-        copied asynchronously; pageable CPU masks are staged through pinned memory."""
+        copied asynchronously; pageable CPU masks are staged through pinned memory.
+
+        seeds (Co-Mod-GAN only, else ValueError): one 64-bit seed per request instead of the pipeline's counter."""
         kinds, checked, inverts = self._requests(imgs, masks, invert, wait)
+        seeds = self.noise.take("DemoPipeline", len(checked), seeds)
         if not checked:
             return []
         dev = self._device()
@@ -117,5 +138,5 @@ class DemoPipeline(_PhotoPipeline):
         outs_d = [torch.empty((h, w, 3), dtype=torch.uint8, device=dev) for w, h in sizes]
         for c in range(0, len(checked), _abi.PIPE_MAX_BATCH):
             s = slice(c, c + _abi.PIPE_MAX_BATCH)
-            self._pass(imgs_d[s], masks_d[s], inverts[s], outs_d[s])
+            self._pass(imgs_d[s], masks_d[s], inverts[s], outs_d[s], None if seeds is None else seeds[s])
         return self._complete(kinds, outs_d, sizes, (imgs_d, masks_d, outs_d), torch.cuda.current_stream(dev), wait)

@@ -25,26 +25,41 @@ import numpy as np
 import torch
 
 from . import _abi
-from ._request_path import _to, load_generator
+from .demo import GENERATOR_BATCH
+from ._request_path import NoiseSeeds, _to, load_generator
 from .masks import RandomMaskStream
 
 
 class EvalPipeline(torch.nn.Module):
-    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from.  `seed`: the
-    script's np.random.seed, for the generated masks."""
+    """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from; or a
+    `migan_b200.comodgan.Generator` of the same resolution (see `comodgan.load`).  `seed`: the script's np.random.seed,
+    for the generated masks.  Co-Mod-GAN draws its noise planes and z from seeded streams on the device: the k-th image
+    processed gets seed `noise_seed * 2**32 + k` (`noise_index` = k) unless `forward_batch(..., seeds=...)` names them,
+    and the generator runs in chunks of at most `generator_batch`."""
 
-    def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0):
+    def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0, *,
+                 noise_seed: int = 0, generator_batch: int = GENERATOR_BATCH):
         super().__init__()
-        self.model = load_generator(self, model_or_state_dict, resolution, device)
+        self.model = load_generator(self, model_or_state_dict, resolution, device, accept_comodgan=True)
         self.res = int(resolution)
         self.device_ = torch.device(device)
         self.masks = RandomMaskStream(self.res, seed=seed, device=self.device_)
+        self.noise = NoiseSeeds(self.model, noise_seed, generator_batch)
         self.last_launches = []                 # kernel launches of each pass of the last call, generator included
+
+    @property
+    def noise_index(self) -> int:
+        """How many images have drawn their Co-Mod-GAN noise from the pipeline's counter; settable."""
+        return self.noise.noise_index
+
+    @noise_index.setter
+    def noise_index(self, k: int) -> None:
+        self.noise.noise_index = int(k)
 
     @staticmethod
     def pass_launches(resized: bool, generator: int) -> int:
         """Launches of one pass: tables, [two resize passes when a photo is not R x R], R x R + x, the generator's, the
-        composite."""
+        composite.  `generator` is the sum over the pass's generator chunks (Co-Mod-GAN: noise launches included)."""
         return 2 + (2 if resized else 0) + generator + 1
 
     def _check(self, i, img, mask):
@@ -59,12 +74,14 @@ class EvalPipeline(torch.nn.Module):
         return img, mask
 
     @torch.no_grad()
-    def forward_batch(self, imgs: Sequence, masks: Optional[Sequence] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(real, composed), CUDA float32 [n, 3, R, R] each.  masks=None takes the next n generated masks."""
+    def forward_batch(self, imgs: Sequence, masks: Optional[Sequence] = None, seeds=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(real, composed), CUDA float32 [n, 3, R, R] each.  masks=None takes the next n generated masks.  seeds
+        (Co-Mod-GAN only, else ValueError): one 64-bit noise seed per image instead of the pipeline's counter."""
         imgs = list(imgs)
         n, R, dev = len(imgs), self.res, self.device_
         if masks is not None and len(masks) != n:
             raise ValueError("EvalPipeline.forward_batch: %d images and %d masks" % (n, len(masks)))
+        seeds = self.noise.take("EvalPipeline", n, seeds)
         checked = [self._check(i, img, None if masks is None else masks[i]) for i, img in enumerate(imgs)]
         real = torch.empty((n, 3, R, R), dtype=torch.float32, device=dev)
         composed = torch.empty((n, 3, R, R), dtype=torch.float32, device=dev)
@@ -96,10 +113,10 @@ class EvalPipeline(torch.nn.Module):
                 x = torch.empty((k, 4, R, R), dtype=torch.float32, device=dev)
                 _abi.check(lib.b200_eval_preprocess(reqs, k, R, x.data_ptr(), real[c].data_ptr(), scratch.data_ptr(), need,
                                                     stream))
-                y = self.model(x)
+                y, gen_launches = self.noise.run(self.model, x, None if seeds is None else seeds[c:c + k])
                 _abi.check(lib.b200_eval_composite(x.data_ptr(), y.data_ptr(), k, R, real[c].data_ptr(),
                                                    composed[c].data_ptr(), stream))
                 keep.append((scratch, x, y))
-                self.last_launches.append(self.pass_launches(resized, self.model.last_launch_count()))
+                self.last_launches.append(self.pass_launches(resized, gen_launches))
             torch.cuda.current_stream(dev).synchronize()   # the inputs and the pass buffers are freed on return
         return real, composed
