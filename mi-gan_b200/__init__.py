@@ -17,6 +17,7 @@ Public surface (mirrors the reference's for this path):
     metrics.compute_ssim / metrics.SSIM / metrics.compute_psnr
                                      the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double
     generate_masks                   python -m migan_b200.generate_masks: the reference script's CLI and files
+    evaluate_fid_lpips               python -m migan_b200.evaluate_fid_lpips: the evaluation script's CLI, sharded over GPUs
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
     build.build()                    compile the C-ABI library (nvcc, sm_90a)

@@ -1,0 +1,427 @@
+"""scripts/evaluate_fid_lpips.py on the GPU: the same command line and the same two result lines, on one GPU or all the
+GPUs of a box, with results that do not depend on how many.
+
+    python -m migan_b200.evaluate_fid_lpips --model-name migan-512 --model-path M.pt --real-dir DIR [--mask-dir MASKS]
+    torchrun --nproc_per_node=8 -m migan_b200.evaluate_fid_lpips --model-name migan-512 ...
+
+Differences from the reference script:
+
+* the images are the top-level files of `--real-dir` with a suffix in {.jpg, .jpeg, .JPG, .JPEG, .png, .PNG}, **sorted
+  by name** (the script takes `Path.iterdir()`'s order, which is not reproducible).  For a flat directory with lowercase
+  suffixes this is the order `generate_masks` uses, so generated masks pair with images as in the files it writes;
+* `--batch-size` defaults to 32 (one `EvalPipeline` pass) instead of 8.  It sets the chunk, the unit of work; results
+  depend on it at rounding level (the feature sums are grouped by chunk), not on the number of GPUs;
+* Co-Mod-GAN draws its noise from seeded streams: image k gets seed `noise_seed * 2**32 + k` (`--noise-seed`, default 0);
+* `--real-stats PATH` scores against stored real-image statistics (pytorch_fid's `.npz` with `mu` and `sigma`) and skips
+  Inception on the real images; `--save-real-stats PATH` writes them;
+* `--inception-weights` and `--lpips-weights` take state_dict files; without them the cached weight files are read, as
+  `fid.InceptionV3()` and `lpips.LPIPS()` do.  Nothing is downloaded;
+* FID is computed on the GPU (`FeatureStatistics.frechet_distance`), not with scipy's `sqrtm`.  Only CUDA devices run.
+
+Sharding: the sorted list is cut into chunks of `--batch-size` consecutive images and chunk j runs on rank j % W.  A chunk
+is always one `EvalPipeline.forward_batch` call, one LPIPS call and one Inception call on (real, composed), so its
+outputs are the same bytes on any rank at any W.  Per round of W chunks every rank sends its chunk's features and LPIPS
+values to rank 0 in one fixed-size gather (a rank without a chunk sends padding), and rank 0 adds them to the feature
+statistics in chunk order, one `FeatureStatistics.add` per chunk, so the sums see the same rows in the same groups at
+every W.  Generated masks come from one sequential stream: every rank advances its own stream through all chunks and
+keeps the masks of its own.
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import time
+from collections import deque
+from concurrent.futures import ThreadPoolExecutor
+from pathlib import Path
+from typing import List, NamedTuple, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+import torch.distributed as dist
+
+from . import _abi, comodgan, fid, lpips
+from ._request_path import load_generator
+from .evaluate import EvalPipeline
+
+MODELS = {"migan-256": ("migan", 256), "migan-512": ("migan", 512),
+          "comodgan-256": ("comodgan", 256), "comodgan-512": ("comodgan", 512)}
+IMG_EXTENSIONS = {".jpg", ".jpeg", ".JPG", ".JPEG", ".png", ".PNG"}
+BATCH_SIZE = _abi.PIPE_MAX_BATCH
+PREFETCH = 2                    # chunks decoded ahead of the one the GPU works on
+MASK_SKIP = 256                 # generated masks skipped per RandomMaskStream.next call
+
+
+def resolution(model_name: str) -> int:
+    if model_name not in MODELS:
+        raise Exception("Unsupported model name.")
+    return MODELS[model_name][1]
+
+
+# -- dataset --------------------------------------------------------------------------------------------------------
+
+def list_images(real_dir) -> List[Path]:
+    """The top-level image files of `real_dir` (InferenceDataset's suffixes), sorted by name."""
+    return sorted((p for p in Path(real_dir).iterdir() if p.suffix in IMG_EXTENSIONS and p.is_file()),
+                  key=lambda p: p.name)
+
+
+def list_masks(images: Sequence[Path], mask_dir) -> List[Path]:
+    """`<mask_dir>/<stem>.png` of every image; FileNotFoundError names the first that is missing."""
+    masks = [Path(mask_dir) / ("%s.png" % p.stem) for p in images]
+    for m, p in zip(masks, images):
+        if not m.is_file():
+            raise FileNotFoundError("no mask %s for image %s" % (m, p.name))
+    return masks
+
+
+def decode_photo(path) -> np.ndarray:
+    from PIL import Image
+    with Image.open(path) as im:
+        return np.array(im.convert("RGB"))
+
+
+def decode_mask(path) -> np.ndarray:
+    from PIL import Image
+    with Image.open(path) as im:
+        return np.array(im.convert("L"))
+
+
+# -- chunks ---------------------------------------------------------------------------------------------------------
+
+def chunk_bounds(n: int, batch_size: int) -> List[Tuple[int, int]]:
+    """[start, end) of each chunk: `batch_size` consecutive images, the last one possibly short."""
+    if n < 0 or batch_size < 1:
+        raise ValueError("bad chunking (%d images, batch size %d)" % (n, batch_size))
+    return [(a, min(a + batch_size, n)) for a in range(0, n, batch_size)]
+
+
+def num_rounds(n_chunks: int, world_size: int) -> int:
+    """Rounds every rank joins: round r holds chunks r*W ... r*W + W - 1."""
+    return -(-n_chunks // world_size)
+
+
+def round_chunk(r: int, rank: int, n_chunks: int, world_size: int) -> Optional[int]:
+    """The chunk rank `rank` runs in round r (chunk j runs on rank j % W), or None when it has none left."""
+    j = r * world_size + rank
+    return j if j < n_chunks else None
+
+
+# -- per-rank work --------------------------------------------------------------------------------------------------
+
+class ChunkResult(NamedTuple):
+    """What a chunk sends to rank 0: float32 features [c, 2048] (`real` None when the real statistics are loaded from a
+    file) and LPIPS values [c]."""
+    index: int
+    start: int
+    real: Optional[torch.Tensor]
+    fake: torch.Tensor
+    lpips: torch.Tensor
+
+
+class EvalSetup:
+    """What every rank of one evaluation shares: the file lists, the chunking and the networks, on `device`."""
+
+    def __init__(self, model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
+                 num_workers: int = 2, noise_seed: int = 0, real_features: bool = True, inception_weights=None,
+                 lpips_weights=None):
+        self.res = resolution(model_name)
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("evaluate_fid_lpips runs on a CUDA device (there is no CPU path); got %s" % self.device)
+        if batch_size < 1:
+            raise ValueError("--batch-size must be >= 1, got %d" % batch_size)
+        self.images = list_images(real_dir)
+        if len(self.images) < 2:
+            raise ValueError("%s holds %d images; FID needs at least 2" % (real_dir, len(self.images)))
+        self.masks = None if mask_dir is None else list_masks(self.images, mask_dir)
+        self.chunks = chunk_bounds(len(self.images), int(batch_size))
+        self.num_workers = max(1, int(num_workers))
+        self.noise_seed = int(noise_seed)
+        self.real_features = bool(real_features)
+        if MODELS[model_name][0] == "comodgan":
+            self.model = comodgan.load(model, self.res).to(self.device)
+        else:
+            self.model = load_generator(self, model, self.res, self.device)
+        self.inception = fid.InceptionV3(weights=inception_weights)
+        self.lpips = lpips.LPIPS(net="alex", weights=lpips_weights).to(self.device)
+
+    @property
+    def feature_width(self) -> int:
+        """Floats per image in a round's gather buffer: the features, then the LPIPS value."""
+        return (2 if self.real_features else 1) * fid.FEATURES + 1
+
+
+class RankWorker:
+    """Rank `rank` of `world_size`: its own `EvalPipeline` (and mask stream) and its host decode pool.  `run_round(r)`
+    runs this rank's chunk of round r; call it for r = 0, 1, ... in order.  Usable as a context manager (`close()` stops
+    the decode threads)."""
+
+    def __init__(self, setup: EvalSetup, rank: int, world_size: int):
+        if world_size < 1 or not 0 <= rank < world_size:
+            raise ValueError("bad rank %d of %d" % (rank, world_size))
+        self.setup, self.rank, self.world_size = setup, rank, world_size
+        self.pipe = EvalPipeline(setup.model, setup.res, device=setup.device, seed=0, noise_seed=setup.noise_seed)
+        self.rounds = num_rounds(len(setup.chunks), world_size)
+        self.own = [j for j in range(rank, len(setup.chunks), world_size)]
+        self._pool = ThreadPoolExecutor(max_workers=setup.num_workers)
+        self._pending = deque()          # (chunk, [futures]) decoding ahead, in chunk order
+        self._next = 0                   # index into self.own of the next chunk to submit for decoding
+        self._mask_pos = 0               # images whose generated masks this rank's stream has passed
+        self.decode_wait_s = 0.0         # host time spent waiting for decoded chunks
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def close(self) -> None:
+        for _, futs in self._pending:
+            for f in futs:
+                f.cancel()
+        self._pending.clear()
+        self._pool.shutdown(wait=True)
+
+    def _submit(self) -> None:
+        while len(self._pending) < PREFETCH and self._next < len(self.own):
+            j = self.own[self._next]
+            self._next += 1
+            a, b = self.setup.chunks[j]
+            futs = [self._pool.submit(decode_photo, p) for p in self.setup.images[a:b]]
+            if self.setup.masks is not None:
+                futs += [self._pool.submit(decode_mask, p) for p in self.setup.masks[a:b]]
+            self._pending.append((j, futs))
+
+    def _decoded(self, j: int):
+        self._submit()
+        got, futs = self._pending.popleft()
+        assert got == j, "chunks must be run in round order"
+        t = time.perf_counter()
+        arrays = [f.result() for f in futs]
+        self.decode_wait_s += time.perf_counter() - t
+        self._submit()                   # keep PREFETCH chunks decoding while the GPU works
+        a, b = self.setup.chunks[j]
+        c = b - a
+        return arrays[:c], (arrays[c:] if self.setup.masks is not None else None)
+
+    def _skip_masks(self, upto: int) -> None:
+        """Advance the generated-mask stream to image `upto`: the masks of other ranks' chunks are drawn and dropped."""
+        while self._mask_pos < upto:
+            k = min(MASK_SKIP, upto - self._mask_pos)
+            self.pipe.masks.next(k)
+            self._mask_pos += k
+
+    @torch.no_grad()
+    def run_chunk(self, j: int) -> ChunkResult:
+        setup = self.setup
+        a, b = setup.chunks[j]
+        photos, masks = self._decoded(j)
+        if masks is None:
+            self._skip_masks(a)
+            self._mask_pos = b
+        self.pipe.noise_index = a
+        real, composed = self.pipe.forward_batch(photos, masks)
+        values = setup.lpips(real, composed, normalize=True).view(-1)
+        c = b - a
+        if setup.real_features:
+            feats = setup.inception(torch.cat([real, composed]))[0].view(2 * c, fid.FEATURES)
+            return ChunkResult(j, a, feats[:c], feats[c:], values)
+        return ChunkResult(j, a, None, setup.inception(composed)[0].view(c, fid.FEATURES), values)
+
+    def run_round(self, r: int) -> Optional[ChunkResult]:
+        j = round_chunk(r, self.rank, len(self.setup.chunks), self.world_size)
+        return None if j is None else self.run_chunk(j)
+
+
+# -- transport and merge --------------------------------------------------------------------------------------------
+
+def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[int, int]], width: int, device,
+                 group=None) -> List[ChunkResult]:
+    """One round's chunk results on rank 0, in chunk order ([] on the other ranks).  Every rank of `group` calls it
+    once per round, with its chunk's result or None: it sends one [batch, width] float32 buffer (features, then the
+    LPIPS value; zero rows pad a short or absent chunk) in one gather.  `width` is 2 * 2048 + 1, or 2048 + 1 without
+    real features."""
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    batch = chunks[0][1] - chunks[0][0]
+    F = fid.FEATURES
+    fake_at, lpips_at = width - 1 - F, width - 1          # real features, when sent, occupy [0, F)
+    buf = torch.zeros((batch, width), dtype=torch.float32, device=device)
+    if result is not None:
+        c = result.fake.shape[0]
+        if fake_at:
+            buf[:c, :F] = result.real
+        buf[:c, fake_at:lpips_at] = result.fake
+        buf[:c, lpips_at] = result.lpips
+    bufs = [torch.empty_like(buf) for _ in range(world)] if rank == 0 else None
+    dist.gather(buf, bufs, dst=0, group=group)
+    if rank != 0:
+        return []
+    out = []
+    for k, got in enumerate(bufs):
+        j = round_chunk(r, k, len(chunks), world)
+        if j is not None:
+            a, b = chunks[j]
+            c = b - a
+            out.append(ChunkResult(j, a, got[:c, :F] if fake_at else None, got[:c, fake_at:lpips_at], got[:c, lpips_at]))
+    return out
+
+
+class EvalResult(NamedTuple):
+    fid: float
+    lpips: float                      # np.mean of lpips_values, the script's reduction
+    lpips_values: np.ndarray          # float64 [count], dataset (sorted) order
+    count: int
+    decode_wait_s: float = 0.0        # rank 0's host time waiting for decoded chunks
+    seconds: float = 0.0              # rank 0's wall time of the chunk loop and the distance
+
+
+class Merge:
+    """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`."""
+
+    def __init__(self, n: int, device, real_features: bool = True):
+        self.n, self.device = n, torch.device(device)
+        self.real = fid.FeatureStatistics(device=self.device) if real_features else None
+        self.fake = fid.FeatureStatistics(device=self.device)
+        self.values = torch.empty(n, dtype=torch.float32, device=self.device)
+        self.next_chunk = 0
+        self.count = 0
+
+    def add(self, chunk: ChunkResult) -> None:
+        if chunk.index != self.next_chunk:
+            raise RuntimeError("chunk %d merged before chunk %d" % (chunk.index, self.next_chunk))
+        c = chunk.fake.shape[0]
+        if self.real is not None:
+            self.real.add(chunk.real)
+        self.fake.add(chunk.fake)
+        self.values[chunk.start:chunk.start + c] = chunk.lpips.to(self.device)
+        self.next_chunk += 1
+        self.count += c
+
+    def real_statistics(self) -> Tuple[np.ndarray, np.ndarray]:
+        """(mu, sigma) of the real features as float64 numpy arrays, from `mean_cov_device()`."""
+        mu, sigma = self.real.mean_cov_device()
+        return mu.cpu().numpy(), sigma.cpu().numpy()
+
+    def result(self, real_stats=None) -> EvalResult:
+        """The FID against the merged real statistics, or against `real_stats` = (mu, sigma) when given."""
+        if self.count != self.n:
+            raise RuntimeError("merged %d of %d images" % (self.count, self.n))
+        if real_stats is None:
+            value = self.real.frechet_distance(self.fake)
+        else:
+            value = fid.frechet_distance(real_stats[0], real_stats[1], *self.fake.mean_cov_device())
+        values = self.values.cpu().numpy().astype(np.float64)
+        return EvalResult(float(value), float(np.mean(values)), values, self.n)
+
+
+def load_real_stats(path) -> Tuple[np.ndarray, np.ndarray]:
+    with np.load(path) as f:
+        return np.asarray(f["mu"], dtype=np.float64), np.asarray(f["sigma"], dtype=np.float64)
+
+
+def save_real_stats(path, mu: np.ndarray, sigma: np.ndarray) -> None:
+    """pytorch_fid's layout: an .npz with `mu` and `sigma`, written to `path` as given."""
+    with open(path, "wb") as f:
+        np.savez(f, mu=mu, sigma=sigma)
+
+
+# -- entry points ---------------------------------------------------------------------------------------------------
+
+def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
+             num_workers: int = 2, noise_seed: int = 0, real_stats=None, save_real_stats_to=None,
+             inception_weights=None, lpips_weights=None) -> Optional[EvalResult]:
+    """FID and LPIPS of `model` over `real_dir`, as the command prints them.  `model`: a state_dict, a path to one, or a
+    generator object (MI-GAN `Generator`, or `comodgan.Generator` for the comodgan names).  `real_stats`: a path to an
+    .npz with `mu` and `sigma` (or such a pair); `save_real_stats_to`: where to write the real statistics.
+    `inception_weights` / `lpips_weights`: state_dicts or paths instead of the cached weight files.
+
+    In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
+    rank 0 returns the result; the other ranks return None."""
+    if real_stats is not None and save_real_stats_to is not None:
+        raise ValueError("--real-stats and --save-real-stats exclude each other: with stored statistics the real images "
+                         "are not scored")
+    distributed = dist.is_available() and dist.is_initialized()
+    world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
+    if real_stats is not None and not isinstance(real_stats, tuple):
+        real_stats = load_real_stats(real_stats)
+    setup = EvalSetup(model_name, model, real_dir, mask_dir, device=device, batch_size=batch_size,
+                      num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
+                      inception_weights=inception_weights, lpips_weights=lpips_weights)
+    merge = Merge(len(setup.images), setup.device, setup.real_features) if rank == 0 else None
+    t0 = time.perf_counter()
+    with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
+        for r in range(worker.rounds):
+            got = worker.run_round(r)
+            if distributed:
+                got = gather_round(got, r, setup.chunks, setup.feature_width, setup.device)
+            else:
+                got = [got]
+            for chunk in got:
+                merge.add(chunk)
+        if merge is None:
+            return None
+        if save_real_stats_to is not None:
+            save_real_stats(save_real_stats_to, *merge.real_statistics())
+        res = merge.result(real_stats)
+        torch.cuda.synchronize(setup.device)
+    return res._replace(decode_wait_s=worker.decode_wait_s, seconds=time.perf_counter() - t0)
+
+
+def get_args(argv=None):
+    parser = argparse.ArgumentParser(prog="python -m migan_b200.evaluate_fid_lpips")
+    parser.add_argument("--model-name", type=str, help="One of [migan-256, migan-512, comodgan-256, comodgan-512]")
+    parser.add_argument("--model-path", type=Path, help="Saved model path.", required=True)
+    parser.add_argument("--real-dir", type=Path, help="Real dataset directory path.", required=True)
+    parser.add_argument("--mask-dir", type=Path, help="Pre-generated mask directory path.", required=False)
+    parser.add_argument("--device", type=str, help="Device to use (CUDA only).", required=False, default="cuda")
+    parser.add_argument("--batch-size", type=int, help="Images per chunk (the unit of work).", required=False,
+                        default=BATCH_SIZE)
+    parser.add_argument("--num-workers", type=int, help="Host decode threads.", required=False, default=2)
+    parser.add_argument("--noise-seed", type=int, default=0, help="Co-Mod-GAN: image k gets noise seed "
+                        "noise_seed * 2**32 + k.")
+    parser.add_argument("--save-real-stats", type=Path, default=None, help="Write the real images' mu and sigma (.npz).")
+    parser.add_argument("--real-stats", type=Path, default=None, help="Score against stored real mu and sigma (.npz).")
+    parser.add_argument("--inception-weights", type=Path, default=None, help="FID Inception state_dict file.")
+    parser.add_argument("--lpips-weights", type=Path, default=None, help="LPIPS (alex) state_dict file.")
+    return parser.parse_args(argv)
+
+
+def device_for(requested: str, world_size: int, local_rank: int) -> torch.device:
+    """The CUDA device of this process: `requested` alone, `cuda:LOCAL_RANK` under torchrun."""
+    dev = torch.device(requested)
+    if dev.type != "cuda":
+        raise RuntimeError("evaluate_fid_lpips runs on CUDA devices only (there is no CPU path); got --device %s"
+                           % requested)
+    if world_size > 1:
+        if dev.index is not None:
+            raise ValueError("--device %s: with several processes each one uses cuda:LOCAL_RANK; pass --device cuda"
+                             % requested)
+        return torch.device("cuda", local_rank)
+    return dev
+
+
+def main(argv=None) -> None:
+    args = get_args(argv)
+    resolution(args.model_name)
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    device = device_for(args.device, world, local_rank)
+    if world > 1:
+        torch.cuda.set_device(device)
+        dist.init_process_group("nccl", device_id=device)
+    try:
+        res = evaluate(args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device,
+                       batch_size=args.batch_size, num_workers=args.num_workers, noise_seed=args.noise_seed,
+                       real_stats=args.real_stats, save_real_stats_to=args.save_real_stats,
+                       inception_weights=args.inception_weights, lpips_weights=args.lpips_weights)
+    finally:
+        if world > 1:
+            dist.destroy_process_group()
+    if res is not None:
+        print("FID:", res.fid)
+        print("LPIPS: ", res.lpips)
+
+
+if __name__ == "__main__":
+    main()
