@@ -18,12 +18,19 @@ Public surface (mirrors the reference's for this path):
                                      the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double
     generate_masks                   python -m migan_b200.generate_masks: the reference script's CLI and files
     evaluate_fid_lpips               python -m migan_b200.evaluate_fid_lpips: the evaluation script's CLI, sharded over GPUs
+    demo (python -m)                 python -m migan_b200.demo: scripts/demo.py's CLI and files, sharded over GPUs
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
     build.build()                    compile the C-ABI library (nvcc, sm_90a)
 
 The directory is named `mi-gan_b200`; import it as `migan_b200` (repo-root shim `migan_b200.py`).
 """
+import warnings as _warnings
+
+# `python -m migan_b200.demo` runs demo.py as __main__ after this package has imported it as `migan_b200.demo`.  Its
+# __main__ block only calls demo_command.main, so runpy's warning about the module's second copy does not apply.
+_warnings.filterwarnings("ignore", message=r"'migan_b200\.demo' found in sys\.modules", category=RuntimeWarning)
+
 from . import arch, build, demo, evaluate, export, fid, fullres, holewin, lpips, masks, metrics, ops, parallel, pipeline, synthetic  # noqa: F401
 from .fullres import FullResPipeline  # noqa: F401
 from .holewin import HoleWindowPipeline  # noqa: F401

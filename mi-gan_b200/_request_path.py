@@ -116,12 +116,13 @@ class _Queued(torch.nn.Module):
         if record:
             self._set_record(record)
 
-    def wait(self) -> None:
+    def wait(self, calls: Optional[int] = None) -> None:
         """Block until every call enqueued with `forward_batch(..., wait=False)` has finished: its results are written and
         the per-request record of those calls (`last_boxes`, `last_sizes`, `last_extents` or `last_windows`) is set, in
-        submission order."""
-        calls, self._pending = self._pending, []
-        self._finish(calls)
+        submission order.  `calls`: wait only for the oldest that many calls; the later ones stay queued."""
+        k = len(self._pending) if calls is None else max(0, min(int(calls), len(self._pending)))
+        done, self._pending = self._pending[:k], self._pending[k:]
+        self._finish(done)
 
 
 class _PhotoPipeline(_Queued):

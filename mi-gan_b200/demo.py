@@ -140,3 +140,9 @@ class DemoPipeline(_PhotoPipeline):
             s = slice(c, c + _abi.PIPE_MAX_BATCH)
             self._pass(imgs_d[s], masks_d[s], inverts[s], outs_d[s], None if seeds is None else seeds[s])
         return self._complete(kinds, outs_d, sizes, (imgs_d, masks_d, outs_d), torch.cuda.current_stream(dev), wait)
+
+
+if __name__ == "__main__":
+    # python -m migan_b200.demo: scripts/demo.py's command line (migan_b200/demo_command.py)
+    from .demo_command import main
+    main()
