@@ -12,6 +12,7 @@
  *   fid_stats_update                   the float64 running sums behind np.mean / np.cov(rowvar=False) of the features
  *   fid_stats_mean_cov                 the mean and covariance from those sums, on the device
  *   fid_frechet_distance               the Fréchet distance of two (mu, sigma) on the device (float64 eigensolver)
+ *   ids_scores                         P-IDS and U-IDS of paired real / fake features (float64 finite-Newton SVM)
  */
 #ifndef INCEPTION_B200_H_
 #define INCEPTION_B200_H_
@@ -95,6 +96,32 @@ int fid_stats_mean_cov(const double* shift, const double* sum, const double* sum
 size_t fid_frechet_workspace_bytes(int dim);
 int fid_frechet_distance(const double* mu1, const double* sigma1, const double* mu2, const double* sigma2, int dim,
                          double out_host[4], int* sweeps_host, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- Inception discriminative scores (P-IDS, U-IDS) ------------------------------------------------------------------
+ * The linear SVM of sklearn.svm.LinearSVC(dual=False) on paired rows real[n][dim] (label +1) and fake[n][dim] (label
+ * -1): the minimiser b* = (w, intercept) of f(b) = 1/2 |b|^2 + C sum_i max(0, 1 - y_i b.[x_i, 1])^2 with C = 1 (the
+ * intercept regularised as a weight on a constant feature, as liblinear does), found to float64 rounding by the finite
+ * Newton method on the device (Gram on fp64 DMMA tiles, blocked Cholesky, exact line search).  With o_i = b*.[x_i, 1]:
+ *   U-IDS = (#{real: o <= 0} + #{fake: o > 0}) / 2n      P-IDS = #{i: o_fake,i > o_real,i} / n.
+ * The features are read as stored (dtype IDS_FLOAT32 or IDS_FLOAT64, device, row-major) and promoted exactly to float64.
+ * No atomics and fixed-order sums: the same inputs give the same bytes on every run and on any stream.
+ *
+ * coef (device, float64 [dim]) = w.  out_host[5] (HOST) = {P-IDS, U-IDS, intercept, f(b*), |grad f(b*)| / |grad f(0)|}.
+ * iterations_host[2] (HOST) = {Newton iterations, the rule that ended the solve: IDS_STOP_ACTIVE_SET (the active set at
+ * the Newton point equals the one it was solved on, so it is the minimiser) or IDS_STOP_GRADIENT (relative gradient
+ * <= 1e-12)}.  SYNCHRONOUS on `stream`: the host reads a small status back once per Newton iteration.  Refused with
+ * MIGAN_ERR_INVALID: null pointers, n < 1, dim outside 1..IDS_MAX_DIM, n x 2 x (dim + 1) >= 2^31, an unknown dtype,
+ * non-finite features, a workspace that is short or not 256-byte aligned, no convergence in 100 iterations (the
+ * message gives the last active-set change). */
+#define IDS_MAX_DIM 4096
+#define IDS_FLOAT32 0
+#define IDS_FLOAT64 1
+#define IDS_STOP_ACTIVE_SET 1
+#define IDS_STOP_GRADIENT 2
+/* Device bytes ids_scores needs; 0 on bad arguments. */
+size_t ids_workspace_bytes(int64_t n, int dim);
+int ids_scores(const void* real, const void* fake, int64_t n, int dim, int dtype, double* coef, double out_host[5],
+               int iterations_host[2], void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -16,14 +16,18 @@ Differences from the reference script:
   Inception on the real images; `--save-real-stats PATH` writes them;
 * `--inception-weights` and `--lpips-weights` take state_dict files; without them the cached weight files are read, as
   `fid.InceptionV3()` and `lpips.LPIPS()` do.  Nothing is downloaded;
-* FID is computed on the GPU (`FeatureStatistics.frechet_distance`), not with scipy's `sqrtm`.  Only CUDA devices run.
+* FID is computed on the GPU (`FeatureStatistics.frechet_distance`), not with scipy's `sqrtm`.  Only CUDA devices run;
+* `--ids` also prints Co-Mod-GAN's paired and unpaired Inception discriminative scores (`P-IDS:`, `U-IDS:`) after the two
+  lines, from the real and composed features of every image (`ids.inception_discriminative_scores`).  Rank 0 keeps
+  those features on the device (16 KiB per image), so `--ids` does not combine with `--real-stats`.
 
 Sharding: the sorted list is cut into chunks of `--batch-size` consecutive images and chunk j runs on rank j % W.  A chunk
 is always one `EvalPipeline.forward_batch` call, one LPIPS call and one Inception call on (real, composed), so its
 outputs are the same bytes on any rank at any W.  Per round of W chunks every rank sends its chunk's features and LPIPS
 values to rank 0 in one fixed-size gather (a rank without a chunk sends padding), and rank 0 adds them to the feature
 statistics in chunk order, one `FeatureStatistics.add` per chunk, so the sums see the same rows in the same groups at
-every W.  Generated masks come from one sequential stream: every rank advances its own stream through all chunks and
+every W; with `--ids` it also keeps them in dataset order, so the scores are the same bits at every W.  Generated
+masks come from one sequential stream: every rank advances its own stream through all chunks and
 keeps the masks of its own.
 """
 from __future__ import annotations
@@ -40,7 +44,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import _abi, comodgan, fid, lpips
+from . import _abi, comodgan, fid, ids, lpips
 from ._request_path import load_generator
 from .evaluate import EvalPipeline
 
@@ -274,15 +278,23 @@ class EvalResult(NamedTuple):
     count: int
     decode_wait_s: float = 0.0        # rank 0's host time waiting for decoded chunks
     seconds: float = 0.0              # rank 0's wall time of the chunk loop and the distance
+    p_ids: Optional[float] = None     # with ids=True: the paired and unpaired Inception discriminative scores
+    u_ids: Optional[float] = None
 
 
 class Merge:
-    """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`."""
+    """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`.  With `keep_features` it also
+    keeps every real and composed feature row in dataset order on the device, for the discriminative scores."""
 
-    def __init__(self, n: int, device, real_features: bool = True):
+    def __init__(self, n: int, device, real_features: bool = True, keep_features: bool = False):
         self.n, self.device = n, torch.device(device)
         self.real = fid.FeatureStatistics(device=self.device) if real_features else None
         self.fake = fid.FeatureStatistics(device=self.device)
+        if keep_features and not real_features:
+            raise ValueError("the discriminative scores need the real features")
+        self.kept = None
+        if keep_features:
+            self.kept = [torch.empty((n, fid.FEATURES), dtype=torch.float32, device=self.device) for _ in range(2)]
         self.values = torch.empty(n, dtype=torch.float32, device=self.device)
         self.next_chunk = 0
         self.count = 0
@@ -295,6 +307,9 @@ class Merge:
             self.real.add(chunk.real)
         self.fake.add(chunk.fake)
         self.values[chunk.start:chunk.start + c] = chunk.lpips.to(self.device)
+        if self.kept is not None:
+            self.kept[0][chunk.start:chunk.start + c] = chunk.real
+            self.kept[1][chunk.start:chunk.start + c] = chunk.fake
         self.next_chunk += 1
         self.count += c
 
@@ -312,7 +327,11 @@ class Merge:
         else:
             value = fid.frechet_distance(real_stats[0], real_stats[1], *self.fake.mean_cov_device())
         values = self.values.cpu().numpy().astype(np.float64)
-        return EvalResult(float(value), float(np.mean(values)), values, self.n)
+        res = EvalResult(float(value), float(np.mean(values)), values, self.n)
+        if self.kept is not None:
+            scores = ids.inception_discriminative_scores(*self.kept)
+            res = res._replace(p_ids=scores.p_ids, u_ids=scores.u_ids)
+        return res
 
 
 def load_real_stats(path) -> Tuple[np.ndarray, np.ndarray]:
@@ -330,17 +349,21 @@ def save_real_stats(path, mu: np.ndarray, sigma: np.ndarray) -> None:
 
 def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
              num_workers: int = 2, noise_seed: int = 0, real_stats=None, save_real_stats_to=None,
-             inception_weights=None, lpips_weights=None) -> Optional[EvalResult]:
+             inception_weights=None, lpips_weights=None, ids: bool = False) -> Optional[EvalResult]:
     """FID and LPIPS of `model` over `real_dir`, as the command prints them.  `model`: a state_dict, a path to one, or a
     generator object (MI-GAN `Generator`, or `comodgan.Generator` for the comodgan names).  `real_stats`: a path to an
     .npz with `mu` and `sigma` (or such a pair); `save_real_stats_to`: where to write the real statistics.
-    `inception_weights` / `lpips_weights`: state_dicts or paths instead of the cached weight files.
+    `inception_weights` / `lpips_weights`: state_dicts or paths instead of the cached weight files.  `ids`: also the
+    paired and unpaired Inception discriminative scores (`p_ids`, `u_ids`); it needs the real features, so it excludes
+    `real_stats`.
 
     In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
     rank 0 returns the result; the other ranks return None."""
     if real_stats is not None and save_real_stats_to is not None:
         raise ValueError("--real-stats and --save-real-stats exclude each other: with stored statistics the real images "
                          "are not scored")
+    if ids and real_stats is not None:
+        raise ValueError("--ids needs the real images' features, which stored statistics (--real-stats) do not carry")
     distributed = dist.is_available() and dist.is_initialized()
     world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
     if real_stats is not None and not isinstance(real_stats, tuple):
@@ -348,7 +371,7 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
     setup = EvalSetup(model_name, model, real_dir, mask_dir, device=device, batch_size=batch_size,
                       num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
                       inception_weights=inception_weights, lpips_weights=lpips_weights)
-    merge = Merge(len(setup.images), setup.device, setup.real_features) if rank == 0 else None
+    merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids) if rank == 0 else None
     t0 = time.perf_counter()
     with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
         for r in range(worker.rounds):
@@ -384,6 +407,8 @@ def get_args(argv=None):
     parser.add_argument("--real-stats", type=Path, default=None, help="Score against stored real mu and sigma (.npz).")
     parser.add_argument("--inception-weights", type=Path, default=None, help="FID Inception state_dict file.")
     parser.add_argument("--lpips-weights", type=Path, default=None, help="LPIPS (alex) state_dict file.")
+    parser.add_argument("--ids", action="store_true", help="Also print P-IDS and U-IDS (Co-Mod-GAN's Inception "
+                        "discriminative scores).")
     return parser.parse_args(argv)
 
 
@@ -414,13 +439,16 @@ def main(argv=None) -> None:
         res = evaluate(args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device,
                        batch_size=args.batch_size, num_workers=args.num_workers, noise_seed=args.noise_seed,
                        real_stats=args.real_stats, save_real_stats_to=args.save_real_stats,
-                       inception_weights=args.inception_weights, lpips_weights=args.lpips_weights)
+                       inception_weights=args.inception_weights, lpips_weights=args.lpips_weights, ids=args.ids)
     finally:
         if world > 1:
             dist.destroy_process_group()
     if res is not None:
         print("FID:", res.fid)
         print("LPIPS: ", res.lpips)
+        if args.ids:
+            print("P-IDS:", res.p_ids)
+            print("U-IDS:", res.u_ids)
 
 
 if __name__ == "__main__":
