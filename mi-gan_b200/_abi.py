@@ -6,6 +6,8 @@ import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
 
+import torch
+
 from . import build as _build
 
 OK, ERR_INVALID, ERR_CUDA, ERR_STATE, ERR_WORKSPACE = 0, 1, 2, 3, 4
@@ -206,6 +208,33 @@ def bind(lib, symbols):
         fn.argtypes = argtypes
     return lib
 
+
+_bound = set()
+
+
+def library(symbols, handle=None):
+    """`handle` (the product library when None) with `symbols` bound; each list is bound once per handle.  A handle can
+    be another build of the same sources, such as an emulation build."""
+    h = handle if handle is not None else load()
+    if (id(h), id(symbols)) not in _bound:
+        bind(h, symbols)
+        _bound.add((id(h), id(symbols)))
+    return h
+
+
+class Workspace:
+    """One device buffer, kept while the key of the calls that use it stays the same: a new key frees it and allocates
+    nbytes() bytes."""
+
+    def __init__(self):
+        self.key, self.buf = None, None
+
+    def get(self, key, nbytes, device) -> torch.Tensor:
+        if self.buf is None or key != self.key:
+            self.buf = None
+            self.buf = torch.empty(int(nbytes()), dtype=torch.uint8, device=device)
+            self.key = key
+        return self.buf
 
 
 class MiganError(RuntimeError):

@@ -6,6 +6,9 @@
 //   convolution       conv_launch: the kernel's launch, or in the emulation build the same arithmetic as a host loop
 //   weights           ConvL (one convolution's shape and packed operand), upload_conv (TF32 hi / lo packing)
 //   forward walk      Runner (workspace bump allocator, launch counting, launch plan), Act, conv_step, pool_step
+//   context           NetCtx and the life cycle behind both networks' C calls: create, destroy, the weight registry
+//                     calls, finalize (call order, then the network's packing), workspace_bytes, launch_plan, forward.
+//                     Each network keeps its spec list, its packing, its input checks and its walk.
 #pragma once
 #include <algorithm>
 #include <cstdarg>
@@ -18,6 +21,7 @@
 #include "../../include/inception_b200.h"
 #include "abi_error.h"
 #include "inception_kernels.cuh"
+#include "weight_registry.h"
 
 namespace incep {
 
@@ -194,6 +198,122 @@ inline void pool_step(Runner& R, int kind, const char* name, int n, const Act& i
     static const char* kinds[] = {"max_s2", "avg_s1", "max_s1"};
     R.note("pool %s %s in=%dx%dx%d out=%dx%dx%d ct=%d c0=%d", kinds[kind], name, in.H, in.W, in.C, OH, OW, in.C, out.C, c0);
     R.launch(PoolK{in.p, out.p, kind, in.H, in.W, in.C, OH, OW, out.C, c0}, (int64_t)n * OH * OW * (in.C / 4));
+}
+
+// ---- network context -------------------------------------------------------------------------------------------------
+// What a network's context holds besides its own constants: device -1 describes the network (weight spec, workspace
+// size, launch plan) and cannot be finalized.
+struct NetCtx {
+    int device = -1;
+    bool finalized = false;
+    migan::WeightRegistry weights;
+    std::vector<ConvL> convs;
+    std::vector<void*> allocs;   // device memory freed with the context
+    int last_launches = 0;
+};
+
+inline int check_ctx(const NetCtx* c) { return c ? 0 : migan::fail(MIGAN_ERR_INVALID, "null context"); }
+
+// The templates over a network's context type are static, so that the library exports the networks' C calls and no
+// instantiation of them.
+template <class Ctx>
+static int create(int device, Ctx** out, void (*build_specs)(Ctx*)) {
+    if (!out) return migan::fail(MIGAN_ERR_INVALID, "out is null");
+    if (device >= 0) {
+        if (const int e = dev_set(device)) return migan::fail(MIGAN_ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
+    }
+    Ctx* c = new Ctx();
+    c->device = device;
+    build_specs(c);
+    *out = c;
+    return 0;
+}
+
+template <class Ctx>
+static int destroy(Ctx* c) {
+    if (!c) return 0;
+    for (void* p : c->allocs) dev_free(p);
+    delete c;
+    return 0;
+}
+
+inline int num_weights(const NetCtx* c) { return c ? c->weights.size() : 0; }
+
+inline int weight_info(const NetCtx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
+    if (int rc = check_ctx(c)) return rc;
+    return c->weights.info(index, name, ndim, shape);
+}
+
+// Keeps a host copy of one state_dict entry until finalize.  A key ending in `dropped` (when given) is accepted and
+// not kept.
+inline int set_weight(NetCtx* c, const char* name, const float* data, int64_t numel, const char* dropped = nullptr) {
+    if (int rc = check_ctx(c)) return rc;
+    if (!name || !data) return migan::fail(MIGAN_ERR_INVALID, "null argument");
+    if (c->finalized) return migan::fail(MIGAN_ERR_STATE, "weights already finalized");
+    if (dropped) {
+        const size_t len = strlen(name), tail = strlen(dropped);
+        if (len >= tail && strcmp(name + len - tail, dropped) == 0) return MIGAN_OK;
+    }
+    return c->weights.set(name, data, numel);
+}
+
+// Checks the call order and the registry, then `pack` uploads the network's weights on the context's device; the host
+// copies go once it succeeds.
+template <class Ctx>
+static int finalize(Ctx* c, int (*pack)(Ctx*)) {
+    if (int rc = check_ctx(c)) return rc;
+    if (c->finalized) return migan::fail(MIGAN_ERR_STATE, "weights already finalized");
+    if (const char* key = c->weights.first_missing()) return migan::fail(MIGAN_ERR_INVALID, "missing key '%s' in the state_dict", key);
+    if (c->device < 0) return migan::fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
+    if (int e = dev_set(c->device)) return migan::fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
+    if (int rc = pack(c)) return rc;
+    c->weights.release_host();
+    c->finalized = true;
+    return 0;
+}
+
+// `walk(R)` runs the network's forward walk on Runner R: dry here, so it only sizes the workspace (0 when the walk fails).
+template <class WalkFn>
+size_t workspace_bytes(const WalkFn& walk) {
+    Runner R;
+    walk(R);
+    return R.rc ? 0 : R.peak;
+}
+
+// The walk's launch plan into buf, truncated to cap - 1 characters and terminated; returns the plan's full length.
+template <class WalkFn>
+int launch_plan(const WalkFn& walk, char* buf, int cap) {
+    std::string plan;
+    Runner R;
+    R.plan = &plan;
+    walk(R);
+    if (buf && cap > 0) {
+        const size_t k = std::min(plan.size(), (size_t)cap - 1);
+        memcpy(buf, plan.data(), k);
+        buf[k] = 0;
+    }
+    return (int)plan.size();
+}
+
+// The checks that open a forward, before the network's own.
+inline int check_forward(const NetCtx* c, const char* finalize_call) {
+    if (int rc = check_ctx(c)) return rc;
+    if (!c->finalized) return migan::fail(MIGAN_ERR_STATE, "forward before %s", finalize_call);
+    return 0;
+}
+
+// The launching pass of the walk on `stream` within workspace[0, bytes).
+template <class WalkFn>
+int forward(NetCtx* c, void* workspace, size_t bytes, void* stream, const WalkFn& walk) {
+    if (!workspace) return migan::fail(MIGAN_ERR_INVALID, "null workspace");
+    Runner R;
+    R.dry = false;
+    R.base = static_cast<char*>(workspace);
+    R.cap = bytes;
+    R.s = static_cast<ck_stream_t>(stream);
+    walk(R);
+    c->last_launches = R.launches;
+    return R.rc;
 }
 
 }  // namespace incep

@@ -24,22 +24,15 @@ using migan::fail;
 using incep::Act;
 using incep::ConvL;
 using incep::Runner;
-using incep::dev_err;
-using incep::dev_set;
 
 constexpr double kBnEps = 0.001;
 constexpr int kOS = INCEPTION_SIZE, kFeat = INCEPTION_FEATURES;
 
 }  // namespace
 
-struct inception_ctx {
-    int device = -1;
-    bool finalized = false;
-    migan::WeightRegistry weights;
-    std::vector<ConvL> convs;             // state_dict order
+// convs in state_dict order
+struct inception_ctx : incep::NetCtx {
     std::map<std::string, int> index;     // name -> convs[]
-    std::vector<void*> allocs;
-    int last_launches = 0;
 };
 
 namespace {
@@ -236,10 +229,14 @@ struct Walk {
     }
 };
 
-int check_ctx(const inception_ctx* c) { return c ? 0 : fail(MIGAN_ERR_INVALID, "null context"); }
-
 int check_images(int n, int H, int W) {
     if (n < 1 || H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "bad batch: n=%d H=%d W=%d (all >= 1)", n, H, W);
+    return 0;
+}
+
+int pack_weights(inception_ctx* c) {
+    for (ConvL& L : c->convs)
+        if (int rc = pack_conv(c, L)) return rc;
     return 0;
 }
 
@@ -248,94 +245,38 @@ int check_images(int n, int H, int W) {
 // =====================================================================================================================
 extern "C" {
 
-int inception_create(int device, inception_ctx** out) {
-    if (!out) return fail(MIGAN_ERR_INVALID, "out is null");
-    if (device >= 0) {
-        if (const int e = dev_set(device)) return fail(MIGAN_ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
-    }
-    inception_ctx* c = new inception_ctx();
-    c->device = device;
-    build_specs(c);
-    *out = c;
-    return 0;
-}
-
-int inception_destroy(inception_ctx* c) {
-    if (!c) return 0;
-    for (void* p : c->allocs) incep::dev_free(p);
-    delete c;
-    return 0;
-}
-
-int inception_num_weights(const inception_ctx* c) { return c ? c->weights.size() : 0; }
+int inception_create(int device, inception_ctx** out) { return incep::create(device, out, build_specs); }
+int inception_destroy(inception_ctx* c) { return incep::destroy(c); }
+int inception_num_weights(const inception_ctx* c) { return incep::num_weights(c); }
 
 int inception_weight_info(const inception_ctx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
-    if (int rc = check_ctx(c)) return rc;
-    return c->weights.info(index, name, ndim, shape);
+    return incep::weight_info(c, index, name, ndim, shape);
 }
 
+// pytorch_fid's state_dict holds the BatchNorm counters `*.num_batches_tracked`, which the network does not use.
 int inception_set_weight(inception_ctx* c, const char* name, const float* host_data, int64_t numel) {
-    if (int rc = check_ctx(c)) return rc;
-    if (!name || !host_data) return fail(MIGAN_ERR_INVALID, "null argument");
-    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
-    const size_t len = strlen(name), tail = strlen("num_batches_tracked");
-    if (len >= tail && strcmp(name + len - tail, "num_batches_tracked") == 0) return MIGAN_OK;
-    return c->weights.set(name, host_data, numel);
+    return incep::set_weight(c, name, host_data, numel, "num_batches_tracked");
 }
 
-int inception_finalize_weights(inception_ctx* c) {
-    if (int rc = check_ctx(c)) return rc;
-    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
-    if (const char* key = c->weights.first_missing()) return fail(MIGAN_ERR_INVALID, "missing key '%s' in the state_dict", key);
-    if (c->device < 0) return fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
-    if (int e = dev_set(c->device)) return fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
-    for (ConvL& L : c->convs)
-        if (int rc = pack_conv(c, L)) return rc;
-    c->weights.release_host();
-    c->finalized = true;
-    return 0;
-}
+int inception_finalize_weights(inception_ctx* c) { return incep::finalize(c, pack_weights); }
 
 size_t inception_workspace_bytes(const inception_ctx* c, int n, int H, int W) {
     if (!c || n < 1 || H < 1 || W < 1) return 0;
-    Runner R;
-    Walk w{c, R, n};
-    w.run(nullptr, H, W, nullptr);
-    return R.rc ? 0 : R.peak;
+    return incep::workspace_bytes([&](Runner& R) { Walk{c, R, n}.run(nullptr, H, W, nullptr); });
 }
 
 int inception_launch_plan(const inception_ctx* c, int n, int H, int W, char* buf, int cap) {
-    if (int rc = check_ctx(c)) return rc < 0 ? rc : -rc;
-    if (check_images(n, H, W)) return -MIGAN_ERR_INVALID;
-    std::string plan;
-    Runner R;
-    R.plan = &plan;
-    Walk w{c, R, n};
-    w.run(nullptr, H, W, nullptr);
-    if (buf && cap > 0) {
-        const size_t k = std::min(plan.size(), (size_t)cap - 1);
-        memcpy(buf, plan.data(), k);
-        buf[k] = 0;
-    }
-    return (int)plan.size();
+    if (int rc = incep::check_ctx(c)) return -rc;
+    if (int rc = check_images(n, H, W)) return -rc;
+    return incep::launch_plan([&](Runner& R) { Walk{c, R, n}.run(nullptr, H, W, nullptr); }, buf, cap);
 }
 
 int inception_features(inception_ctx* c, const float* x, int n, int H, int W, float* feats, void* workspace,
                        size_t workspace_bytes, void* stream) {
-    if (int rc = check_ctx(c)) return rc;
-    if (!c->finalized) return fail(MIGAN_ERR_STATE, "forward before inception_finalize_weights");
+    if (int rc = incep::check_forward(c, "inception_finalize_weights")) return rc;
     if (!x || !feats) return fail(MIGAN_ERR_INVALID, "null x / feats");
     if (int rc = check_images(n, H, W)) return rc;
-    if (!workspace) return fail(MIGAN_ERR_INVALID, "null workspace");
-    Runner R;
-    R.dry = false;
-    R.base = static_cast<char*>(workspace);
-    R.cap = workspace_bytes;
-    R.s = static_cast<ck_stream_t>(stream);
-    Walk w{c, R, n};
-    w.run(x, H, W, feats);
-    c->last_launches = R.launches;
-    return R.rc;
+    return incep::forward(c, workspace, workspace_bytes, stream, [&](Runner& R) { Walk{c, R, n}.run(x, H, W, feats); });
 }
 
 int inception_last_launch_count(const inception_ctx* c) { return c ? c->last_launches : 0; }

@@ -23,7 +23,6 @@ using incep::Act;
 using incep::ConvL;
 using incep::Runner;
 using incep::dev_err;
-using incep::dev_set;
 using migan::fail;
 
 constexpr int kLayers = LPIPS_LAYERS;
@@ -71,15 +70,10 @@ int reduce_launch(const lpips::ReduceArgs& a, ck_stream_t s) {
 
 }  // namespace
 
-struct lpips_ctx {
-    int device = -1;
-    bool finalized = false;
-    migan::WeightRegistry weights;
-    std::vector<ConvL> convs;             // features.0, .3, .6, .8, .10
+// convs: features.0, .3, .6, .8, .10
+struct lpips_ctx : incep::NetCtx {
     float shift[3] = {0.f, 0.f, 0.f}, scale[3] = {1.f, 1.f, 1.f};
     float* lin = nullptr;                 // the five lin{k} weights, concatenated (device)
-    std::vector<void*> allocs;
-    int last_launches = 0;
 };
 
 namespace {
@@ -166,8 +160,6 @@ struct Walk {
     }
 };
 
-int check_ctx(const lpips_ctx* c) { return c ? 0 : fail(MIGAN_ERR_INVALID, "null context"); }
-
 int check_pairs(int n, int H, int W) {
     if (n < 1 || H < LPIPS_MIN_SIZE || W < LPIPS_MIN_SIZE)
         return fail(MIGAN_ERR_INVALID, "bad batch: n=%d H=%d W=%d (n >= 1; H, W >= %d, the smallest size AlexNet's second max "
@@ -175,50 +167,8 @@ int check_pairs(int n, int H, int W) {
     return 0;
 }
 
-}  // namespace
-
-// =====================================================================================================================
-extern "C" {
-
-int lpips_create(int device, lpips_ctx** out) {
-    if (!out) return fail(MIGAN_ERR_INVALID, "out is null");
-    if (device >= 0) {
-        if (const int e = dev_set(device)) return fail(MIGAN_ERR_CUDA, "cannot select device %d: %s", device, dev_err(e));
-    }
-    lpips_ctx* c = new lpips_ctx();
-    c->device = device;
-    build_specs(c);
-    *out = c;
-    return 0;
-}
-
-int lpips_destroy(lpips_ctx* c) {
-    if (!c) return 0;
-    for (void* p : c->allocs) incep::dev_free(p);
-    delete c;
-    return 0;
-}
-
-int lpips_num_weights(const lpips_ctx* c) { return c ? c->weights.size() : 0; }
-
-int lpips_weight_info(const lpips_ctx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
-    if (int rc = check_ctx(c)) return rc;
-    return c->weights.info(index, name, ndim, shape);
-}
-
-int lpips_set_weight(lpips_ctx* c, const char* name, const float* host_data, int64_t numel) {
-    if (int rc = check_ctx(c)) return rc;
-    if (!name || !host_data) return fail(MIGAN_ERR_INVALID, "null argument");
-    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
-    return c->weights.set(name, host_data, numel);
-}
-
-int lpips_finalize_weights(lpips_ctx* c) {
-    if (int rc = check_ctx(c)) return rc;
-    if (c->finalized) return fail(MIGAN_ERR_STATE, "weights already finalized");
-    if (const char* key = c->weights.first_missing()) return fail(MIGAN_ERR_INVALID, "missing key '%s' in the state_dict", key);
-    if (c->device < 0) return fail(MIGAN_ERR_CUDA, "context was created without a CUDA device (description only)");
-    if (int e = dev_set(c->device)) return fail(MIGAN_ERR_CUDA, "cannot select device: %s", dev_err(e));
+// The ScalingLayer constants on the host, the convolutions' TF32 operands and the lin{k} weights on the device.
+int pack_weights(lpips_ctx* c) {
     const migan::WeightRegistry& reg = c->weights;
     for (int i = 0; i < 3; ++i) {
         c->shift[i] = reg.get("scaling_layer.shift")[i];
@@ -237,51 +187,46 @@ int lpips_finalize_weights(lpips_ctx* c) {
     if (!e) e = incep::dev_sync();
     if (e) return fail(MIGAN_ERR_CUDA, "uploading the linear layers failed: %s", dev_err(e));
     c->lin = (float*)d;
-    c->weights.release_host();
-    c->finalized = true;
     return 0;
 }
 
+}  // namespace
+
+// =====================================================================================================================
+extern "C" {
+
+int lpips_create(int device, lpips_ctx** out) { return incep::create(device, out, build_specs); }
+int lpips_destroy(lpips_ctx* c) { return incep::destroy(c); }
+int lpips_num_weights(const lpips_ctx* c) { return incep::num_weights(c); }
+
+int lpips_weight_info(const lpips_ctx* c, int index, const char** name, int* ndim, int64_t shape[4]) {
+    return incep::weight_info(c, index, name, ndim, shape);
+}
+
+int lpips_set_weight(lpips_ctx* c, const char* name, const float* host_data, int64_t numel) {
+    return incep::set_weight(c, name, host_data, numel);
+}
+
+int lpips_finalize_weights(lpips_ctx* c) { return incep::finalize(c, pack_weights); }
+
 size_t lpips_workspace_bytes(const lpips_ctx* c, int n, int H, int W) {
     if (!c || n < 1 || H < LPIPS_MIN_SIZE || W < LPIPS_MIN_SIZE) return 0;
-    Runner R;
-    Walk w{c, R, n};
-    w.run(nullptr, nullptr, H, W, 0, nullptr, nullptr);
-    return R.rc ? 0 : R.peak;
+    return incep::workspace_bytes([&](Runner& R) { Walk{c, R, n}.run(nullptr, nullptr, H, W, 0, nullptr, nullptr); });
 }
 
 int lpips_launch_plan(const lpips_ctx* c, int n, int H, int W, char* buf, int cap) {
-    if (int rc = check_ctx(c)) return -rc;
-    if (check_pairs(n, H, W)) return -MIGAN_ERR_INVALID;
-    std::string plan;
-    Runner R;
-    R.plan = &plan;
-    Walk w{c, R, n};
-    w.run(nullptr, nullptr, H, W, 0, nullptr, nullptr);
-    if (buf && cap > 0) {
-        const size_t k = std::min(plan.size(), (size_t)cap - 1);
-        memcpy(buf, plan.data(), k);
-        buf[k] = 0;
-    }
-    return (int)plan.size();
+    if (int rc = incep::check_ctx(c)) return -rc;
+    if (int rc = check_pairs(n, H, W)) return -rc;
+    return incep::launch_plan([&](Runner& R) { Walk{c, R, n}.run(nullptr, nullptr, H, W, 0, nullptr, nullptr); }, buf, cap);
 }
 
 int lpips_forward(lpips_ctx* c, const float* in0, const float* in1, int n, int H, int W, int normalize, float* out,
                   float* per_layer, void* workspace, size_t workspace_bytes, void* stream) {
-    if (int rc = check_ctx(c)) return rc;
-    if (!c->finalized) return fail(MIGAN_ERR_STATE, "forward before lpips_finalize_weights");
+    if (int rc = incep::check_forward(c, "lpips_finalize_weights")) return rc;
     if (!in0 || !in1 || !out) return fail(MIGAN_ERR_INVALID, "null in0 / in1 / out");
     if (int rc = check_pairs(n, H, W)) return rc;
-    if (!workspace) return fail(MIGAN_ERR_INVALID, "null workspace");
-    Runner R;
-    R.dry = false;
-    R.base = static_cast<char*>(workspace);
-    R.cap = workspace_bytes;
-    R.s = static_cast<ck_stream_t>(stream);
-    Walk w{c, R, n};
-    w.run(in0, in1, H, W, normalize, out, per_layer);
-    c->last_launches = R.launches;
-    return R.rc;
+    return incep::forward(c, workspace, workspace_bytes, stream,
+                          [&](Runner& R) { Walk{c, R, n}.run(in0, in1, H, W, normalize, out, per_layer); });
 }
 
 int lpips_last_launch_count(const lpips_ctx* c) { return c ? c->last_launches : 0; }

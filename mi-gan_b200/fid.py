@@ -22,7 +22,7 @@ import numpy as np
 import torch
 from scipy import linalg
 
-from . import _abi
+from . import _abi, _convnet
 
 FEATURES = 2048
 WEIGHTS_FILE = "pt_inception-2015-12-05-6726825d.pth"
@@ -62,44 +62,20 @@ FRECHET_SYMBOLS = [
                                             ctypes.c_void_p]),
 ]
 
-_bound = set()
-
 
 def lib(handle=None):
     """The product library with this module's symbols bound (`handle`: another build of the same sources)."""
-    h = handle if handle is not None else _abi.load()
-    if id(h) not in _bound:
-        _abi.bind(h, SYMBOLS)
-        _bound.add(id(h))
-    return h
-
-
-_frechet_bound = set()
+    return _abi.library(SYMBOLS, handle)
 
 
 def frechet_lib(handle=None):
     """The product library (or `handle`, another build of csrc/frechet.cu) with the Fréchet symbols bound."""
-    h = lib(handle)
-    if id(h) not in _frechet_bound:
-        _abi.bind(h, FRECHET_SYMBOLS)
-        _frechet_bound.add(id(h))
-    return h
+    return _abi.library(FRECHET_SYMBOLS, lib(handle))
 
 
 def weight_spec(handle=None) -> List[Tuple[str, Tuple[int, ...]]]:
     """(key, shape) of every state_dict entry the library takes, in state_dict order (num_batches_tracked aside)."""
-    L = lib(handle)
-    h = ctypes.c_void_p()
-    _abi.check(L.inception_create(-1, ctypes.byref(h)), L)
-    try:
-        out = []
-        name, nd, shape = ctypes.c_char_p(), ctypes.c_int(), (ctypes.c_int64 * 4)()
-        for i in range(L.inception_num_weights(h)):
-            _abi.check(L.inception_weight_info(h, i, ctypes.byref(name), ctypes.byref(nd), shape), L)
-            out.append((name.value.decode(), tuple(int(v) for v in shape[:nd.value])))
-        return out
-    finally:
-        L.inception_destroy(h)
+    return _convnet.weight_spec(lib(handle), "inception")
 
 
 def default_weights_path() -> str:
@@ -120,7 +96,7 @@ def _load_weights(weights) -> Dict[str, torch.Tensor]:
     return dict(weights)
 
 
-class InceptionV3(torch.nn.Module):
+class InceptionV3(_convnet.Network):
     """pytorch_fid.inception.InceptionV3 at the configuration evaluate_fid_lpips.py uses: block 3 (2048-d pool3),
     resize to 299 x 299, inputs in [0, 1] normalised to [-1, 1], the FID Inception blocks.  forward(x) returns
     [features [n, 2048, 1, 1]] as CUDA float32."""
@@ -140,17 +116,9 @@ class InceptionV3(torch.nn.Module):
                     "use_fid_inception=True) is built; got %s=%r" % (k, v))
         self.output_blocks = [3]
         self.last_needed_block = 3
-        self._state = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in _load_weights(weights).items()
-                       if not k.endswith("num_batches_tracked")}
-        _Engine(None, self._state)   # checks the keys on the host now: missing, unknown or mis-shaped fail by name
-        self._engines = {}
-
-    def _engine(self, device):
-        eng = self._engines.get(device)
-        if eng is None:
-            eng = _Engine(device, self._state)
-            self._engines[device] = eng
-        return eng
+        state = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in _load_weights(weights).items()
+                 if not k.endswith("num_batches_tracked")}
+        self._set_state(lib(), "inception", state)
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
@@ -170,10 +138,6 @@ class InceptionV3(torch.nn.Module):
                                                       ws.numel(), torch.cuda.current_stream(x.device).cuda_stream))
         return [feats.view(n, FEATURES, 1, 1)]
 
-    def last_launch_count(self) -> int:
-        eng = next(iter(self._engines.values()))
-        return int(eng.lib.inception_last_launch_count(eng.handle))
-
     def launch_plan(self, n: int, H: int, W: int) -> List[str]:
         """The forward's launches for n images of H x W, one line each."""
         return launch_plan(n, H, W)
@@ -181,62 +145,7 @@ class InceptionV3(torch.nn.Module):
 
 def launch_plan(n: int, H: int, W: int, handle=None) -> List[str]:
     """The forward's launches for n images of H x W, one line each ("<kind> <name> key=value ...")."""
-    L = lib(handle)
-    h = ctypes.c_void_p()
-    _abi.check(L.inception_create(-1, ctypes.byref(h)), L)
-    try:
-        size = L.inception_launch_plan(h, n, H, W, None, 0)
-        if size < 0:
-            _abi.check(-size, L)
-        buf = ctypes.create_string_buffer(size + 1)
-        L.inception_launch_plan(h, n, H, W, buf, size + 1)
-        return buf.value.decode().splitlines()
-    finally:
-        L.inception_destroy(h)
-
-
-class _Engine:
-    """One library context: device None = description only (weights parsed, nothing uploaded)."""
-
-    def __init__(self, device, state: Dict[str, torch.Tensor], handle=None):
-        self.lib = lib(handle)
-        self.handle = ctypes.c_void_p()
-        index = -1 if device is None else (device.index if device.index is not None else torch.cuda.current_device())
-        _abi.check(self.lib.inception_create(index, ctypes.byref(self.handle)), self.lib)
-        self.workspaces: Dict[tuple, torch.Tensor] = {}
-        self.device = device
-        for k, t in state.items():
-            t = t.detach().to("cpu", torch.float32).contiguous()
-            _abi.check(self.lib.inception_set_weight(self.handle, k.encode(), t.data_ptr(), t.numel()), self.lib)
-        if device is not None:
-            _abi.check(self.lib.inception_finalize_weights(self.handle), self.lib)
-        else:
-            missing = self._first_missing(state)
-            if missing:
-                raise _abi.MiganError(_abi.ERR_INVALID, "missing key '%s' in the state_dict" % missing)
-
-    def _first_missing(self, state):
-        name, nd, shape = ctypes.c_char_p(), ctypes.c_int(), (ctypes.c_int64 * 4)()
-        for i in range(self.lib.inception_num_weights(self.handle)):
-            self.lib.inception_weight_info(self.handle, i, ctypes.byref(name), ctypes.byref(nd), shape)
-            if name.value.decode() not in state:
-                return name.value.decode()
-        return None
-
-    def workspace(self, n, H, W) -> torch.Tensor:
-        ws = self.workspaces.get((n, H, W))
-        if ws is None:
-            nbytes = int(self.lib.inception_workspace_bytes(self.handle, n, H, W))
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self.workspaces = {(n, H, W): ws}
-        return ws
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.inception_destroy(self.handle)
-        except Exception:
-            pass
+    return _convnet.launch_plan(lib(handle), "inception", n, H, W)
 
 
 class FeatureStatistics:
@@ -337,7 +246,7 @@ class FrechetTerms(NamedTuple):
 
 
 MAX_DIM = 4096
-_workspace: Dict[tuple, torch.Tensor] = {}
+_workspace = _abi.Workspace()
 
 
 def _check_covariance(name, x, xp) -> None:
@@ -398,12 +307,7 @@ def _frechet(mu1, sigma1, mu2, sigma2, handle=None) -> FrechetTerms:
     if d < 1 or d > MAX_DIM:
         raise ValueError("feature dimension %d outside 1..%d" % (d, MAX_DIM))
     device = mu1.device
-    key = (device, d)
-    ws = _workspace.get(key)
-    if ws is None:
-        _workspace.clear()
-        ws = torch.empty(int(L.fid_frechet_workspace_bytes(d)), dtype=torch.uint8, device=device)
-        _workspace[key] = ws
+    ws = _workspace.get((device, d), lambda: L.fid_frechet_workspace_bytes(d), device)
     out = (ctypes.c_double * 4)()
     sweeps = (ctypes.c_int * 2)()
     with torch.cuda.device(device):

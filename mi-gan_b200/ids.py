@@ -17,7 +17,7 @@ scores agree with sklearn's up to the rows sklearn leaves within its tolerance o
 from __future__ import annotations
 
 import ctypes
-from typing import Dict, NamedTuple
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -35,16 +35,10 @@ SYMBOLS = [
                                   ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
 ]
 
-_bound = set()
-
 
 def ids_lib(handle=None):
     """The product library (or `handle`, another build of csrc/ids.cu) with the IDS symbols bound."""
-    h = fid.lib(handle)
-    if id(h) not in _bound:
-        _abi.bind(h, SYMBOLS)
-        _bound.add(id(h))
-    return h
+    return _abi.library(SYMBOLS, fid.lib(handle))
 
 
 class IDSResult(NamedTuple):
@@ -60,7 +54,7 @@ class IDSResult(NamedTuple):
     stop_rule: str = "active set"
 
 
-_workspace: Dict[tuple, torch.Tensor] = {}
+_workspace = _abi.Workspace()
 
 
 def _prepare(name, x):
@@ -116,12 +110,7 @@ def _scores(real, fake, handle=None) -> IDSResult:
     L = ids_lib(handle)
     n, d = (int(v) for v in real.shape)
     device = real.device
-    key = (device, n, d)
-    ws = _workspace.get(key)
-    if ws is None:
-        _workspace.clear()
-        ws = torch.empty(int(L.ids_workspace_bytes(n, d)), dtype=torch.uint8, device=device)
-        _workspace[key] = ws
+    ws = _workspace.get((device, n, d), lambda: L.ids_workspace_bytes(n, d), device)
     coef = torch.empty(d, dtype=torch.float64, device=device)
     out = (ctypes.c_double * 5)()
     its = (ctypes.c_int * 2)()

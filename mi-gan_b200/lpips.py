@@ -17,7 +17,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from . import _abi
+from . import _abi, _convnet
 
 LAYERS = 5
 MIN_SIZE = 31
@@ -49,48 +49,20 @@ SYMBOLS = [
      [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
 ]
 
-_bound = set()
-
 
 def lib(handle=None):
     """The product library with this module's symbols bound (`handle`: another build of the same sources)."""
-    h = handle if handle is not None else _abi.load()
-    if id(h) not in _bound:
-        _abi.bind(h, SYMBOLS)
-        _bound.add(id(h))
-    return h
+    return _abi.library(SYMBOLS, handle)
 
 
 def weight_spec(handle=None) -> List[Tuple[str, Tuple[int, ...]]]:
     """(key, shape) of every state_dict entry the library takes, in state_dict order (the `lins.*` aliases aside)."""
-    L = lib(handle)
-    h = ctypes.c_void_p()
-    _abi.check(L.lpips_create(-1, ctypes.byref(h)), L)
-    try:
-        out = []
-        name, nd, shape = ctypes.c_char_p(), ctypes.c_int(), (ctypes.c_int64 * 4)()
-        for i in range(L.lpips_num_weights(h)):
-            _abi.check(L.lpips_weight_info(h, i, ctypes.byref(name), ctypes.byref(nd), shape), L)
-            out.append((name.value.decode(), tuple(int(v) for v in shape[:nd.value])))
-        return out
-    finally:
-        L.lpips_destroy(h)
+    return _convnet.weight_spec(lib(handle), "lpips")
 
 
 def launch_plan(n: int, H: int, W: int, handle=None) -> List[str]:
     """The forward's launches for n pairs of H x W, one line each ("<kind> <name> key=value ...")."""
-    L = lib(handle)
-    h = ctypes.c_void_p()
-    _abi.check(L.lpips_create(-1, ctypes.byref(h)), L)
-    try:
-        size = L.lpips_launch_plan(h, n, H, W, None, 0)
-        if size < 0:
-            _abi.check(-size, L)
-        buf = ctypes.create_string_buffer(size + 1)
-        L.lpips_launch_plan(h, n, H, W, buf, size + 1)
-        return buf.value.decode().splitlines()
-    finally:
-        L.lpips_destroy(h)
+    return _convnet.launch_plan(lib(handle), "lpips", n, H, W)
 
 
 def default_alexnet_path() -> str:
@@ -157,7 +129,7 @@ def _canonical(state: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     return out
 
 
-class LPIPS(torch.nn.Module):
+class LPIPS(_convnet.Network):
     """lpips.LPIPS at the configuration evaluate_fid_lpips.py uses: net="alex", version "0.1", linear layers, not
     spatial, eval mode.  forward(in0, in1) returns CUDA float32 [n, 1, 1, 1]."""
 
@@ -174,17 +146,8 @@ class LPIPS(torch.nn.Module):
         if not pretrained and weights is None:
             raise NotImplementedError("pretrained=False (randomly initialised linear layers) is not built; pass weights=")
         self.pnet_type, self.version, self.spatial, self.L = "alex", "0.1", False, LAYERS
-        state = _default_weights(model_path) if weights is None else _load(weights)
-        self._state = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in _canonical(state).items()}
-        _Engine(None, self._state)   # checks the keys on the host now: missing, unknown or mis-shaped fail by name
-        self._engines = {}
-
-    def _engine(self, device):
-        eng = self._engines.get(device)
-        if eng is None:
-            eng = _Engine(device, self._state)
-            self._engines[device] = eng
-        return eng
+        state = _canonical(_default_weights(model_path) if weights is None else _load(weights))
+        self._set_state(lib(), "lpips", {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in state.items()})
 
     @torch.no_grad()
     def forward(self, in0: torch.Tensor, in1: torch.Tensor, retPerLayer=False, normalize=False):
@@ -220,54 +183,7 @@ class LPIPS(torch.nn.Module):
             return val, [per[k].view(n, 1, 1, 1) for k in range(LAYERS)]
         return val
 
-    def last_launch_count(self) -> int:
-        eng = next(iter(self._engines.values()))
-        return int(eng.lib.lpips_last_launch_count(eng.handle))
-
     def launch_plan(self, n: int, H: int, W: int) -> List[str]:
         """The forward's launches for n pairs of H x W, one line each."""
         return launch_plan(n, H, W)
 
-
-class _Engine:
-    """One library context: device None = description only (weights parsed, nothing uploaded)."""
-
-    def __init__(self, device, state: Dict[str, torch.Tensor], handle=None):
-        self.lib = lib(handle)
-        self.handle = ctypes.c_void_p()
-        index = -1 if device is None else (device.index if device.index is not None else torch.cuda.current_device())
-        _abi.check(self.lib.lpips_create(index, ctypes.byref(self.handle)), self.lib)
-        self.workspaces: Dict[tuple, torch.Tensor] = {}
-        self.device = device
-        for k, t in state.items():
-            t = t.detach().to("cpu", torch.float32).contiguous()
-            _abi.check(self.lib.lpips_set_weight(self.handle, k.encode(), t.data_ptr(), t.numel()), self.lib)
-        if device is not None:
-            _abi.check(self.lib.lpips_finalize_weights(self.handle), self.lib)
-        else:
-            missing = self._first_missing(state)
-            if missing:
-                raise _abi.MiganError(_abi.ERR_INVALID, "missing key '%s' in the state_dict" % missing)
-
-    def _first_missing(self, state):
-        name, nd, shape = ctypes.c_char_p(), ctypes.c_int(), (ctypes.c_int64 * 4)()
-        for i in range(self.lib.lpips_num_weights(self.handle)):
-            self.lib.lpips_weight_info(self.handle, i, ctypes.byref(name), ctypes.byref(nd), shape)
-            if name.value.decode() not in state:
-                return name.value.decode()
-        return None
-
-    def workspace(self, n, H, W) -> torch.Tensor:
-        ws = self.workspaces.get((n, H, W))
-        if ws is None:
-            nbytes = int(self.lib.lpips_workspace_bytes(self.handle, n, H, W))
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self.workspaces = {(n, H, W): ws}
-        return ws
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.lpips_destroy(self.handle)
-        except Exception:
-            pass

@@ -30,16 +30,10 @@ SYMBOLS = [
      [ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
 ]
 
-_bound = set()
-
 
 def lib(handle=None):
     """The product library with this module's symbols bound (`handle`: another build of the same sources)."""
-    h = handle if handle is not None else _abi.load()
-    if id(h) not in _bound:
-        _abi.bind(h, SYMBOLS)
-        _bound.add(id(h))
-    return h
+    return _abi.library(SYMBOLS, handle)
 
 
 def gaussian_taps(window_size: int) -> torch.Tensor:
