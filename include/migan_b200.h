@@ -445,6 +445,55 @@ typedef struct migan_sepconv_tc_plan {
  * i-th entry of its candidate list (MIGAN_ERR_INVALID if that layout does not fit).  `plan` receives the record. */
 int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate, migan_sepconv_tc_plan* plan, void* stream);
 
+/* Test hook: one launch of a CUDA-core stage kernel of the forward (elementwise.cu) on caller-provided operands, packed by
+ * the same functions the weight loader uses.  Device pointers, reference layouts.  The package never calls it. */
+enum { MIGAN_STAGE_STEM = 0, MIGAN_STAGE_DW = 1, MIGAN_STAGE_DOWN = 2, MIGAN_STAGE_UP2 = 3, MIGAN_STAGE_TORGB = 4,
+       MIGAN_STAGE_NOISE_TILE = 5, MIGAN_STAGE_ADD = 6 };
+/* The down-sampling kernel forms: fp32 output (CUDA-core path), or the tensor-core GEMM's pre-split fp16 operand from the
+ * register-streaming or the TMA-staged kernel.  MIGAN_DOWN_AUTO: the form a forward picks for the layer. */
+enum { MIGAN_DOWN_AUTO = -1, MIGAN_DOWN_F32 = 0, MIGAN_DOWN_SPLIT = 1, MIGAN_DOWN_TMA = 2 };
+
+typedef struct migan_stage_io {
+    int kind;                   /* MIGAN_STAGE_* */
+    int n, h, w, c;             /* the kernel's input extent and channels (UP2: the low-resolution side; NOISE_TILE: the
+                                   tiled plane, n and c unused; ADD: n * h * w * c elements) */
+    int tc;                     /* DOWN with MIGAN_DOWN_AUTO: 1 the tensor-core path, 0 the CUDA-core path */
+    int level;                  /* DOWN with MIGAN_DOWN_AUTO: the layer's nominal output side (R x R forward: h / 2) */
+    int r;                      /* NOISE_TILE: side of the source plane */
+    int noise_pitch;            /* UP2 / NOISE_TILE: floats between noise rows (>= 2w / w) */
+    const float* in;            /* STEM: NCHW [n,4,h,w]; DW / DOWN / UP2 / TORGB: NHWC [n,h,w,c]; NOISE_TILE: [r][r];
+                                   ADD: the addend */
+    const float* dw_w;          /* DW / DOWN: depthwise [c,1,3,3] */
+    const float* dw_b;          /* DW / DOWN: [c] */
+    const float* fir;           /* DOWN / UP2: [c,1,4,4]; TORGB: [3,1,4,4] image up-sampling taps (read if img_lo) */
+    const float* fromrgb_w;     /* STEM: [c,4] */
+    const float* fromrgb_b;     /* STEM: [c] */
+    const float* rgb_w;         /* TORGB: [3,c] */
+    const float* rgb_b;         /* TORGB: [3] */
+    const float* img_lo;        /* TORGB: [n,3,h/2,w/2] or NULL */
+    const float* noise;         /* UP2: [2h][noise_pitch] or NULL */
+    const float* skip;          /* UP2: NHWC [n,2h,2w,c] or NULL */
+    float* out;                 /* STEM / DW: NHWC [n,h,w,c]; DOWN fp32: [n,h/2,w/2,c]; UP2: [n,2h,2w,c]; TORGB: NCHW
+                                   [n,3,h,w]; NOISE_TILE: [h][noise_pitch]; ADD: the tensor added to in place */
+    void* out_hi;               /* DW / DOWN split forms: fp16 hi / lo of the activation * 64 (DOWN: * 64 * 2^-fir_shift) */
+    void* out_lo;
+} migan_stage_io;
+
+typedef struct migan_stage_plan {
+    int kind;
+    int down_form;              /* DOWN: the MIGAN_DOWN_* form that ran; -1 otherwise */
+    int rs;                     /* rows per thread of the DW / DOWN kernels, 0 otherwise */
+    int cg;                     /* DOWN split: the C template; TORGB: G lanes per pixel; 0 otherwise */
+    int grid;                   /* blocks of the (first) launch */
+    int groups;                 /* launches (image groups of < 2^31 work items) */
+    int fir_shift;              /* DOWN tensor-core forms: m of the 2^-m folded into the taps (the GEMM undoes it) */
+} migan_stage_plan;
+
+/* Plans (and, when the kind's weights are given -- or, for NOISE_TILE / ADD, `in` -- runs to completion on `stream`) one
+ * stage launch.  variant: the DOWN form, MIGAN_DOWN_AUTO for a forward's choice; ignored by the other kinds.  A form the
+ * launcher refuses for the shape returns MIGAN_ERR_INVALID and launches nothing.  Plan-only calls touch no device. */
+int migan_debug_stage(const migan_stage_io* io, int variant, migan_stage_plan* plan, void* stream);
+
 /* upfirdn2d(x[n,c,h,w], f[fh,fw]) -> y[n,c,oh,ow], oh = (h*upy + pady0 + pady1 - fh + downy) / downy
  * (upfirdn2d.cpp:32-33).  f == NULL means the 1x1 identity filter.  Device pointers. */
 int b200_upfirdn2d(const float* x, const float* f, float* y, int n, int c, int h, int w, int fh, int fw,

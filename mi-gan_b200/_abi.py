@@ -89,6 +89,27 @@ class SepconvTcPlan(ctypes.Structure):
         return {name: getattr(self, name) for name in self.RING_FIELDS}
 
 
+STAGE_STEM, STAGE_DW, STAGE_DOWN, STAGE_UP2, STAGE_TORGB, STAGE_NOISE_TILE, STAGE_ADD = range(7)
+DOWN_AUTO, DOWN_F32, DOWN_SPLIT, DOWN_TMA = -1, 0, 1, 2
+
+
+class StageIO(ctypes.Structure):
+    """migan_stage_io: the operands of one stage-kernel launch (test hook)."""
+    _fields_ = [("kind", c_int), ("n", c_int), ("h", c_int), ("w", c_int), ("c", c_int), ("tc", c_int), ("level", c_int),
+                ("r", c_int), ("noise_pitch", c_int), ("in_", c_void_p), ("dw_w", c_void_p), ("dw_b", c_void_p),
+                ("fir", c_void_p), ("fromrgb_w", c_void_p), ("fromrgb_b", c_void_p), ("rgb_w", c_void_p),
+                ("rgb_b", c_void_p), ("img_lo", c_void_p), ("noise", c_void_p), ("skip", c_void_p), ("out", c_void_p),
+                ("out_hi", c_void_p), ("out_lo", c_void_p)]
+
+
+class StagePlan(ctypes.Structure):
+    """migan_stage_plan: what one stage launch ran."""
+    _fields_ = [(name, c_int) for name in ("kind", "down_form", "rs", "cg", "grid", "groups", "fir_shift")]
+
+    def as_dict(self):
+        return {name: getattr(self, name) for name, _ in self._fields_}
+
+
 # Every symbol include/migan_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("migan_last_error", c_char_p, []),
@@ -165,6 +186,7 @@ SYMBOLS = [
     ("migan_tap_info", c_int, [c_void_p, c_int, c_int, POINTER(c_char_p), POINTER(c_int)]),
     ("migan_debug_tc_timeout", c_int, [c_int]),
     ("migan_debug_sepconv_tc", c_int, [POINTER(SepconvTcIO), c_int, c_int, POINTER(SepconvTcPlan), c_void_p]),
+    ("migan_debug_stage", c_int, [POINTER(StageIO), c_int, POINTER(StagePlan), c_void_p]),
     ("b200_upfirdn2d", c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 14 + [c_int, c_float, c_void_p]),
     ("b200_conv1x1_nhwc", c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     ("b200_bias_act", c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_float, c_float, c_float, c_void_p]),

@@ -16,7 +16,8 @@ constexpr float kActClamp = 256.0f;
 
 // Power-of-two scales applied before the fp16 hi/lo split of the pointwise-conv
 // operands (undone exactly in the epilogue).  Activations are clamped to +-256 before
-// every 1x1 conv, so 2^6 keeps them < 65504; weights are unit-L2-norm rows (|w| <= 1)
+// every 1x1 conv, so 2^6 keeps them <= 16384 (a down-sampling layer's FIR of them is
+// kept <= 32768 by a per-layer 2^-m in its taps, migan_abi.cu pack_down_fir); weights are unit-L2-norm rows (|w| <= 1)
 // in released checkpoints, the scale is chosen per layer on the host from max|w|.
 constexpr float kActSplitScale = 64.0f;
 

@@ -67,12 +67,17 @@ stem_fromrgb_kernel(const float* __restrict__ x, const float* __restrict__ w, co
     }
 }
 
-// Launch helper: split the batch so that one launch indexes < 2^31 work items.
+// Launch helper: split the batch so that one launch indexes < 2^31 work items (one 256-thread block per 256 items).
 template <typename F>
-static cudaError_t for_image_groups(int n, size_t items_per_image, F&& launch) {
+static cudaError_t for_image_groups(int n, size_t items_per_image, StageLaunch* sl, F&& launch) {
     const int max_imgs = (int)std::max<size_t>(1, ((size_t)1 << 31) / std::max<size_t>(items_per_image, 1));
     for (int i0 = 0; i0 < n; i0 += max_imgs) {
-        launch(i0, std::min(max_imgs, n - i0));
+        const int cnt = std::min(max_imgs, n - i0);
+        if (sl) {
+            if (sl->groups++ == 0) sl->grid = blocks_for((int64_t)(items_per_image * cnt), 256);
+            if (sl->dry) continue;
+        }
+        launch(i0, cnt);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
@@ -82,10 +87,10 @@ static cudaError_t for_image_groups(int n, size_t items_per_image, F&& launch) {
 static inline int host_log2(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
 
 cudaError_t launch_stem(const float* x, const float* w, const float* b, float* out,
-                        int n, int H, int W, int C0, cudaStream_t s) {
+                        int n, int H, int W, int C0, cudaStream_t s, StageLaunch* sl) {
     if ((H * W) % 4 != 0) return cudaErrorInvalidValue;
     const size_t per_img = (size_t)H * W / 4 * (C0 / 4);
-    return for_image_groups(n, per_img, [&](int i0, int cnt) {
+    return for_image_groups(n, per_img, sl, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         launch_pdl(stem_fromrgb_kernel, dim3((items + 255) / 256), dim3(256), 0, s, x + (size_t)i0 * 4 * H * W, w, b, out + (size_t)i0 * H * W * C0,
                    items, FastDiv((uint32_t)(H * W)), host_log2(C0 / 4));
@@ -193,10 +198,11 @@ dw3x3_act_kernel(const float* __restrict__ in, const float* __restrict__ w9, con
 }
 
 cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, float* out, __half* out_hi, __half* out_lo,
-                         int n, int H, int W, int C, cudaStream_t s) {
+                         int n, int H, int W, int C, cudaStream_t s, StageLaunch* sl) {
     const int rs = (H >= 8) ? 8 : 4, strips = (H + rs - 1) / rs, pairs = (W + 1) / 2;
     const size_t per_img = (size_t)strips * pairs * (C / 2);
-    return for_image_groups(n, per_img, [&](int i0, int cnt) {
+    if (sl) sl->rs = rs;
+    return for_image_groups(n, per_img, sl, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t off = (size_t)i0 * H * W * C;
         auto kern = (rs == 8) ? dw3x3_act_kernel<8> : dw3x3_act_kernel<4>;
@@ -227,8 +233,7 @@ cudaError_t launch_dw3x3(const float* in, const float* w9, const float* bias, fl
 template <int RS>
 __global__ void __launch_bounds__(256, RS == 8 ? 1 : 2)
 dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, const float* __restrict__ bias,
-                  const float* __restrict__ fir16, float* __restrict__ out_f32,
-                  __half* __restrict__ out_hi, __half* __restrict__ out_lo, uint32_t items, int H2, int W2, int lcp,
+                  const float* __restrict__ fir16, float* __restrict__ out_f32, uint32_t items, int H2, int W2, int lcp,
                   FastDiv pairs, FastDiv strips) {
     const uint32_t idx = blockIdx.x * 256u + threadIdx.x;
     const int W = 2 * W2, H = 2 * H2, C = 2 << lcp;
@@ -328,15 +333,7 @@ dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, co
                 for (int e = 0; e < 2; ++e) {
                     if (((q - 3) >> 1) >= rows_out || (e == 1 && !col1_ok)) continue;   // outside the output
                     const size_t o = ((img * H2 + orow) * W2 + ox0 + e) * (size_t)C + c;
-                    const float2 ov = unpk2(accA[e]);
-                    if (out_f32) *reinterpret_cast<float2*>(out_f32 + o) = ov;
-                    if (out_hi) {
-                        __half h0, l0, h1, l1;
-                        split_f16(ov.x, kActSplitScale, h0, l0);
-                        split_f16(ov.y, kActSplitScale, h1, l1);
-                        *reinterpret_cast<__half2*>(out_hi + o) = __halves2half2(h0, h1);
-                        *reinterpret_cast<__half2*>(out_lo + o) = __halves2half2(l0, l1);
-                    }
+                    *reinterpret_cast<float2*>(out_f32 + o) = unpk2(accA[e]);
                 }
             }
             if (q & 1) { accA[0] = accB[0]; accA[1] = accB[1]; accB[0] = 0ull; accB[1] = 0ull; }
@@ -348,18 +345,17 @@ dw3x3_down_kernel(const float* __restrict__ in, const float* __restrict__ w9, co
 
 cudaError_t configure_elementwise() { return cudaSuccess; }
 
-cudaError_t launch_dw3x3_down(const float* in, const float* w9, const float* bias, const float* fir16,
-                              float* out_f32, __half* out_hi, __half* out_lo,
-                              int n, int H, int W, int C, cudaStream_t s) {
+cudaError_t launch_dw3x3_down(const float* in, const float* w9, const float* bias, const float* fir16, float* out_f32,
+                              int n, int H, int W, int C, cudaStream_t s, StageLaunch* sl) {
     const int H2 = H / 2, W2 = W / 2;
     const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs, pairs = (W2 + 1) / 2;
     const size_t per_img = (size_t)strips * pairs * (C / 2);
-    return for_image_groups(n, per_img, [&](int i0, int cnt) {
+    if (sl) sl->rs = rs;
+    return for_image_groups(n, per_img, sl, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t oi = (size_t)i0 * H * W * C, oo = (size_t)i0 * H2 * W2 * C;
         auto kern = (rs == 8) ? dw3x3_down_kernel<8> : dw3x3_down_kernel<4>;
-        kern<<<(items + 255) / 256, 256, 16 * C * sizeof(float), s>>>(in + oi, w9, bias, fir16, out_f32 ? out_f32 + oo : nullptr,
-                                                out_hi ? out_hi + oo : nullptr, out_lo ? out_lo + oo : nullptr,
+        kern<<<(items + 255) / 256, 256, 16 * C * sizeof(float), s>>>(in + oi, w9, bias, fir16, out_f32 + oo,
                                                 items, H2, W2, host_log2(C / 2), FastDiv((uint32_t)pairs), FastDiv((uint32_t)strips));
     });
 }
@@ -497,26 +493,23 @@ static void launch_down_split_inst(const float* in, const float* w9s, const floa
                H2, W2, FastDiv((uint32_t)((W2 + 1) / 2)), FastDiv((uint32_t)strips));
 }
 
-// w9s / biass: depthwise taps and bias * kActSplitScale * sqrt(2).  C in {64, 128, 256, 512}.
+// w9s / biass: depthwise taps and bias * kActSplitScale * sqrt(2).  A forward runs this kernel below 16 x 16 output
+// levels, all of which have 512 channels (channels(r) = 512 for r <= 64), so C = 512 is the one instance.
 cudaError_t launch_dw3x3_down_split(const float* in, const float* w9s, const float* biass, const float* fir16,
-                                    __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s) {
+                                    __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s, StageLaunch* sl) {
     const int H2 = H / 2, W2 = W / 2;
-    if (W2 < 2 || H2 < 1 || (C != 64 && C != 128 && C != 256 && C != 512)) return cudaErrorInvalidValue;
+    if (W2 < 2 || H2 < 1 || C != 512) return cudaErrorInvalidValue;
     const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs;
     const size_t per_img = (size_t)strips * ((W2 + 1) / 2) * (C / 2);
-    return for_image_groups(n, per_img, [&](int i0, int cnt) {
+    if (sl) { sl->rs = rs; sl->cg = C; }
+    return for_image_groups(n, per_img, sl, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const float* ip = in + (size_t)i0 * H * W * C;
         __half* hp = out_hi + (size_t)i0 * H2 * W2 * C;
         __half* lp = out_lo + (size_t)i0 * H2 * W2 * C;
 #define MIGAN_DOWN_CASE(RS_, C_) launch_down_split_inst<RS_, C_>(ip, w9s, biass, fir16, hp, lp, items, W2, H2, strips, s)
-        if (rs == 8) {
-            if (C == 64) MIGAN_DOWN_CASE(8, 64); else if (C == 128) MIGAN_DOWN_CASE(8, 128);
-            else if (C == 256) MIGAN_DOWN_CASE(8, 256); else MIGAN_DOWN_CASE(8, 512);
-        } else {
-            if (C == 64) MIGAN_DOWN_CASE(4, 64); else if (C == 128) MIGAN_DOWN_CASE(4, 128);
-            else if (C == 256) MIGAN_DOWN_CASE(4, 256); else MIGAN_DOWN_CASE(4, 512);
-        }
+        if (rs == 8) MIGAN_DOWN_CASE(8, 512);
+        else MIGAN_DOWN_CASE(4, 512);
 #undef MIGAN_DOWN_CASE
     });
 }
@@ -673,20 +666,23 @@ dw3x3_down_tma_kernel(const __grid_constant__ DownTensorMap desc, const float* _
 }
 
 cudaError_t launch_dw3x3_down_tma(const DownTensorMap& desc, const float* w9s, const float* biass, const float* fir16,
-                                  __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s) {
+                                  __half* out_hi, __half* out_lo, int n, int H, int W, int C, cudaStream_t s, StageLaunch* sl) {
     const int H2 = H / 2, W2 = W / 2;
-    if (W2 < 16 || W2 % 2 != 0 || H2 < 1 || C % 64 != 0) return cudaErrorInvalidValue;
-    const int rs = (H2 >= 8) ? 8 : 4, strips = (H2 + rs - 1) / rs, slabs = C / 64, xtiles = (W2 + 15) / 16;
+    // a forward runs this kernel from 16 x 16 output levels up, so 8-row strips (RS = 8) are the one instance
+    if (W2 < 16 || W2 % 2 != 0 || H2 < 8 || C % 64 != 0) return cudaErrorInvalidValue;
+    constexpr int rs = 8;
+    const int strips = (H2 + rs - 1) / rs, slabs = C / 64, xtiles = (W2 + 15) / 16;
     if (slabs & (slabs - 1)) return cudaErrorInvalidValue;
     const size_t blocks = (size_t)n * strips * xtiles * slabs;
     if (blocks == 0 || blocks > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    if (sl) { sl->rs = rs; sl->groups = 1; sl->grid = (unsigned)blocks; if (sl->dry) return cudaSuccess; }
     const size_t smem = (size_t)kDownRing * kDownRowBytes + 16 * 64 * sizeof(float);
-    static bool attr_set[2] = {false, false};
-    auto kern = (rs == 8) ? dw3x3_down_tma_kernel<8> : dw3x3_down_tma_kernel<4>;
-    if (!attr_set[rs == 8]) {
+    static bool attr_set = false;
+    auto kern = dw3x3_down_tma_kernel<rs>;
+    if (!attr_set) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        attr_set[rs == 8] = true;
+        attr_set = true;
     }
     return launch_pdl(kern, dim3((unsigned)blocks), dim3(288), smem, s, desc, w9s, biass, fir16, out_hi, out_lo, C, H2, W2, xtiles,
                       strips, host_log2(slabs));
@@ -753,9 +749,9 @@ up2_noise_act_skip_kernel(const float* __restrict__ t, const float* __restrict__
 }
 
 cudaError_t launch_up2(const float* t, const float* fir16, const float* noise, int noise_pitch, const float* skip,
-                       float* out, int n, int h, int w, int C, cudaStream_t s) {
+                       float* out, int n, int h, int w, int C, cudaStream_t s, StageLaunch* sl) {
     const size_t per_img = (size_t)h * w * (C / 4);
-    return for_image_groups(n, per_img, [&](int i0, int cnt) {
+    return for_image_groups(n, per_img, sl, [&](int i0, int cnt) {
         const uint32_t items = (uint32_t)(per_img * cnt);
         const size_t oi = (size_t)i0 * h * w * C, oo = (size_t)i0 * 4 * h * w * C;
         launch_pdl(up2_noise_act_skip_kernel, dim3((items + 255) / 256), dim3(256), 16 * C * sizeof(float), s,
@@ -828,8 +824,14 @@ torgb_img_kernel(const float* __restrict__ x, const float* __restrict__ w, const
 }
 
 cudaError_t launch_torgb(const float* x, const float* w, const float* b, const float* img_lo,
-                         const float* fir16x3, float* img_out, int n, int h, int wd, int C, cudaStream_t s) {
+                         const float* fir16x3, float* img_out, int n, int h, int wd, int C, cudaStream_t s, StageLaunch* sl) {
     const int64_t npix = (int64_t)n * h * wd;
+    if (sl) {
+        sl->cg = (C / 4 >= 32) ? 32 : 16;
+        sl->groups = 1;
+        sl->grid = blocks_for(npix * sl->cg, 256);
+        if (sl->dry) return cudaSuccess;
+    }
     if (C / 4 >= 32) {
         const int64_t threads = npix * 32;
         launch_pdl(torgb_img_kernel<32>, dim3(blocks_for(threads, 256)), dim3(256), 0, s, x, w, b, img_lo, fir16x3, img_out, npix, h, wd, C);
@@ -857,11 +859,12 @@ noise_tile_kernel(const __grid_constant__ NoiseTileBatch b) {
     }
 }
 
-cudaError_t launch_noise_tile(const NoiseTileBatch& b, cudaStream_t s) {
+cudaError_t launch_noise_tile(const NoiseTileBatch& b, cudaStream_t s, StageLaunch* sl) {
     if (b.count < 1 || b.count > kMaxNoiseTiles) return cudaErrorInvalidValue;
     int64_t most = 0;
     for (int i = 0; i < b.count; ++i) most = std::max<int64_t>(most, (int64_t)b.t[i].H * b.t[i].pitch);
     const unsigned bx = (unsigned)std::min<int64_t>(blocks_for(most, 256), 512);
+    if (sl) { sl->groups = 1; sl->grid = bx * (unsigned)b.count; if (sl->dry) return cudaSuccess; }
     return launch_pdl(noise_tile_kernel, dim3(bx, (unsigned)b.count), dim3(256), 0, s, b);
 }
 
@@ -878,7 +881,8 @@ add_inplace_kernel(float* __restrict__ x, const float* __restrict__ y, int64_t n
     reinterpret_cast<float4*>(x)[i] = a;
 }
 
-cudaError_t launch_add(float* x, const float* y, int64_t numel, cudaStream_t s) {
+cudaError_t launch_add(float* x, const float* y, int64_t numel, cudaStream_t s, StageLaunch* sl) {
+    if (sl) { sl->groups = 1; sl->grid = blocks_for(numel / 4, 256); if (sl->dry) return cudaSuccess; }
     launch_pdl(add_inplace_kernel, dim3(blocks_for(numel / 4, 256)), dim3(256), 0, s, x, y, numel / 4);
     return cudaGetLastError();
 }

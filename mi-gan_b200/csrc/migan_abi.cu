@@ -72,6 +72,25 @@ void pack_torgb(const float* w, const float* b, const float* fir, int cout, floa
     if (fir) transpose(fir, 3, 16, fir_out);
 }
 
+// Down-sampling taps [cin,1,4,4] -> fir16 [16][cin] (fp32 kernel) and fir16_tc = fir16 * 2^-m (tensor-core feed); returns m.
+// The tensor-core feed applies the taps to activations clamped at +-256 * kActSplitScale = +-16384 and rounds the result to
+// the fp16 hi of the GEMM operand, so |hi| <= 16384 * max_c sum_t |f[c][t]| * 2^-m must stay below fp16's 65504: m is the
+// least that brings it to <= 32768, and the layer's GEMM undoes 2^-m exactly (tc_inv_scale).  Filters with sum |f| <= 2,
+// the constructor's [1,3,3,1] among them, get m = 0 and fir16_tc == fir16.
+int pack_down_fir(const float* f, int cin, float* fir16, float* fir16_tc) {
+    transpose(f, cin, 16, fir16);
+    double most = 0.0;
+    for (int c = 0; c < cin; ++c) {
+        double sum = 0.0;
+        for (int t = 0; t < 16; ++t) sum += std::fabs((double)f[c * 16 + t]);
+        most = std::max(most, sum);
+    }
+    int m = 0;
+    while (m < 64 && std::ldexp(most, -m) > 2.0) ++m;
+    for (int i = 0; i < 16 * cin; ++i) fir16_tc[i] = std::ldexp(fir16[i], -m);
+    return m;
+}
+
 // One SeparableConv2d (migan_inference.py:106-170), packed for the kernels.
 struct SepConv {
     std::string p;  // state_dict prefix, e.g. "encoder.b256.conv2."
@@ -88,8 +107,10 @@ struct SepConv {
     float* pw_t = nullptr;    // [cin][cout] fp32 (CUDA-core GEMM)
     __half* pw_hi = nullptr;  // [cout][cin] fp16 hi part of w * 2^k   (wgmma, K-major)
     __half* pw_lo = nullptr;  // [cout][cin] fp16 lo part
-    float tc_inv_scale = 1.f; // 1 / (kActSplitScale * 2^k)
+    float tc_inv_scale = 1.f; // 1 / (kActSplitScale * 2^k * 2^-down_shift)
     float* fir16 = nullptr;   // [16][cin] (down) or [16][cout] (up), tap-major
+    float* fir16_tc = nullptr;   // down: fir16 * 2^-down_shift, the taps of the tensor-core feed's down-sampling kernels
+    int down_shift = 0;
     float* noise_dev = nullptr;  // [res_out^2] = noise_const * noise_strength (the plane of an R x R forward)
     // fused up-sampling prologue of the NEXT layer (sepconv_tc SEPCONV_SRC_UP): needs channel-uniform FIR taps
     bool up_uniform = false;
@@ -138,7 +159,7 @@ struct Step {
     bool want_f32 = false;
     migan::SepconvTcArgs tc;  // resolved wgmma launch (tensor maps, tiling)
     migan::DownTensorMap down_map;   // K_DWDOWN on the TMA-staged kernel: tensor map of the input
-    bool down_tma = false;
+    int down_form = MIGAN_DOWN_F32;  // K_DWDOWN: which kernel (down_form())
     migan::NoiseTileBatch noise_tiles;   // K_NOISE: the tiled noise planes of a fully convolutional forward
     // roofline bookkeeping: algorithmic bytes = own input(s) read once + output written once
     std::string label;
@@ -449,16 +470,33 @@ int migan_set_weight(migan_ctx* ctx, const char* name, const float* host_data, i
     return MIGAN_OK;
 }
 
+// The depthwise tables of a layer: fp32 [9][cin] + bias (CUDA-core kernels) and the pack_dw_tc copies (tensor-core feed).
+static void pack_depthwise(SepConv& L, const float* dw, const float* db, ArenaBuilder& ab) {
+    const int cin = L.cin;
+    transpose(dw, cin, 9, ab.table(&L.w9, 9 * cin));   // depthwise taps [cin,1,3,3] -> [9][cin]
+    memcpy(ab.table(&L.bias, cin), db, sizeof(float) * cin);
+    float* w9_tc = ab.table(&L.w9_tc, 9 * cin);         // wgmma prologue: activation gain and fp16-split scale folded in
+    pack_dw_tc(dw, db, cin, w9_tc, ab.table(&L.bias_tc, cin));
+}
+
+// The FIR tables of a down ([cin,1,4,4]) or up ([cout,1,4,4]) layer.
+static void pack_fir(SepConv& L, const float* f, ArenaBuilder& ab) {
+    const int cf = L.down ? L.cin : L.cout;
+    if (L.down) {
+        float* fir16 = ab.table(&L.fir16, 16 * cf);
+        L.down_shift = pack_down_fir(f, cf, fir16, ab.table(&L.fir16_tc, 16 * cf));
+    } else {
+        transpose(f, cf, 16, ab.table(&L.fir16, 16 * cf));
+    }
+}
+
 static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab) {
     const WeightRegistry& wr = ctx->weights;
     const int cin = L.cin, cout = L.cout;
     const std::vector<float>& dw = wr.get(L.p + "conv1.weight");
     const std::vector<float>& db = wr.get(L.p + "conv1.bias");
     const std::vector<float>& pw = wr.get(L.p + "conv2.weight");
-    transpose(dw.data(), cin, 9, ab.table(&L.w9, 9 * cin));   // depthwise taps [cin,1,3,3] -> [9][cin]
-    memcpy(ab.table(&L.bias, cin), db.data(), sizeof(float) * cin);
-    float* w9_tc = ab.table(&L.w9_tc, 9 * cin);   // wgmma prologue: activation gain and fp16-split scale folded in
-    pack_dw_tc(dw.data(), db.data(), cin, w9_tc, ab.table(&L.bias_tc, cin));
+    pack_depthwise(L, dw.data(), db.data(), ab);
     // pointwise [cout,cin,1,1] -> fp32 [cin][cout] and fp16 hi/lo [cout][cin]
     transpose(pw.data(), cout, cin, ab.table(&L.pw_t, (size_t)cin * cout));
     __half* pw_hi = ab.table(&L.pw_hi, (size_t)cin * cout);
@@ -466,7 +504,8 @@ static int pack_sepconv(migan_ctx* ctx, SepConv& L, ArenaBuilder& ab) {
     if (L.down || L.up) {
         const int cf = L.down ? cin : cout;
         const std::vector<float>& f = wr.get(L.p + (L.down ? "downsample.filter.weight" : "upsample.filter.weight"));
-        transpose(f.data(), cf, 16, ab.table(&L.fir16, 16 * cf));
+        pack_fir(L, f.data(), ab);
+        L.tc_inv_scale = std::ldexp(L.tc_inv_scale, L.down_shift);   // the down operand arrives * 2^-down_shift
         if (L.up) {   // the fused prologue keeps the 16 taps in registers: they must not depend on the channel
             L.up_uniform = true;
             for (int c = 1; c < cf && L.up_uniform; ++c)
@@ -661,6 +700,22 @@ struct Fuse {
     float* rgb_out = nullptr;       // null: the caller's y, and the feature map is not stored (last level)
 };
 
+// The down-sampling kernel of a layer whose 1x1 conv runs at level res_pw: on the tensor-core path the fp16 hi/lo GEMM
+// operand, with its input rows staged through shared memory by TMA from 16 x 16 levels up and streamed through registers
+// below; fp32 on the CUDA-core path.
+int down_form(bool tc, int res_pw) { return !tc ? MIGAN_DOWN_F32 : res_pw >= 16 ? MIGAN_DOWN_TMA : MIGAN_DOWN_SPLIT; }
+
+// One down-sampling launch of layer L in `form` on the input extent H x W (`map`: the TMA form's tensor map of `in`).
+cudaError_t run_down(const SepConv& L, int form, const migan::DownTensorMap& map, const float* in, float* out, __half* hi, __half* lo,
+                     int n, int H, int W, cudaStream_t st, migan::StageLaunch* sl = nullptr) {
+    switch (form) {
+        case MIGAN_DOWN_TMA: return migan::launch_dw3x3_down_tma(map, L.w9_tc, L.bias_tc, L.fir16_tc, hi, lo, n, H, W, L.cin, st, sl);
+        case MIGAN_DOWN_SPLIT: return migan::launch_dw3x3_down_split(in, L.w9_tc, L.bias_tc, L.fir16_tc, hi, lo, n, H, W, L.cin, st, sl);
+        case MIGAN_DOWN_F32: return migan::launch_dw3x3_down(in, L.w9, L.bias, L.fir16, out, n, H, W, L.cin, st, sl);
+    }
+    return cudaErrorInvalidValue;
+}
+
 struct PlanBuilder {
     migan_ctx* c;
     int n, path;
@@ -695,15 +750,14 @@ struct PlanBuilder {
         bool presplit = L.down;
         if (L.down) {
             Step s; s.kind = K_DWDOWN; s.L = &L; s.in = in; s.n = n; s.H = ein.h; s.W = ein.w; s.C = L.cin;
+            s.down_form = down_form(tc, L.res_pw);
             if (tc) {
                 s.hi = reinterpret_cast<__half*>(S[t1]);
                 s.lo = s.hi + (size_t)n * epw.h * epw.w * L.cin;
                 ghi = s.hi; glo = s.lo;
-                if (L.res_pw >= 16) {   // rows staged through shared memory by TMA (elementwise.cu)
+                if (s.down_form == MIGAN_DOWN_TMA)
                     if (const char* err = migan::make_down_tensor_map(&s.down_map, in, n, ein.h, ein.w, L.cin))
                         return fail(MIGAN_ERR_CUDA, "tensor map for %sdownsample failed: %s", L.p.c_str(), err);
-                    s.down_tma = true;
-                }
             } else {
                 s.out = S[t1]; gemm_in = S[t1];
                 s.tap[0] = {L.p + "down", S[t1], L.cin, epw.h, epw.w};
@@ -983,12 +1037,7 @@ int run_step(migan_ctx* ctx, Step& s, const float* x, float* y, cudaStream_t st)
             e = migan::launch_dw3x3(in, s.L->w9, s.L->bias, s.out, s.hi, s.lo, s.n, s.H, s.W, s.C, st);
             break;
         case K_DWDOWN:
-            if (s.down_tma)
-                e = migan::launch_dw3x3_down_tma(s.down_map, s.L->w9_tc, s.L->bias_tc, s.L->fir16, s.hi, s.lo, s.n, s.H, s.W, s.C, st);
-            else if (s.hi && !s.out && s.W >= 8)   // tensor-core feed: specialised kernel on the pre-scaled tap table
-                e = migan::launch_dw3x3_down_split(in, s.L->w9_tc, s.L->bias_tc, s.L->fir16, s.hi, s.lo, s.n, s.H, s.W, s.C, st);
-            else
-                e = migan::launch_dw3x3_down(in, s.L->w9, s.L->bias, s.L->fir16, s.out, s.hi, s.lo, s.n, s.H, s.W, s.C, st);
+            e = run_down(*s.L, s.down_form, s.down_map, in, s.out, s.hi, s.lo, s.n, s.H, s.W, st);
             break;
         case K_GEMM_SIMT:
             e = migan::launch_pw_gemm_simt(in, s.L->pw_t, out, (int64_t)s.n * s.H * s.W, s.L->cin, s.L->cout,
@@ -1469,6 +1518,120 @@ int migan_debug_sepconv_tc(const migan_sepconv_tc_io* io, int sms, int candidate
     const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess)
         return fail(MIGAN_ERR_CUDA, "sepconv_tc launch failed: %s (timeout record %d)", cudaGetErrorString(e), migan::sepconv_tc_timeout_record(dev));
+    return MIGAN_OK;
+}
+
+int migan_debug_stage(const migan_stage_io* io, int variant, migan_stage_plan* plan, void* stream) {
+    if (!io) return fail(MIGAN_ERR_INVALID, "stage: null io");
+    const int kind = io->kind, n = io->n, h = io->h, w = io->w, C = io->c;
+    if (kind < MIGAN_STAGE_STEM || kind > MIGAN_STAGE_ADD) return fail(MIGAN_ERR_INVALID, "stage: bad kind %d", kind);
+    if (kind == MIGAN_STAGE_NOISE_TILE ? (h < 1 || w < 1 || io->r < 1 || io->noise_pitch < w)
+                                       : (n < 1 || h < 1 || w < 1 || C < 4 || C % 4 != 0))
+        return fail(MIGAN_ERR_INVALID, "stage: bad shape");
+    if (kind == MIGAN_STAGE_DOWN && (variant < MIGAN_DOWN_AUTO || variant > MIGAN_DOWN_TMA))
+        return fail(MIGAN_ERR_INVALID, "stage: bad down-sampling form %d", variant);
+    const float* weights[] = {io->fromrgb_w, io->dw_w, io->dw_w, io->fir, io->rgb_w, io->in, io->in};
+    const bool run = weights[kind] != nullptr;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    migan::StageLaunch sl;
+    sl.dry = !run;
+    int form = -1;
+    if (kind == MIGAN_STAGE_DOWN)
+        form = variant != MIGAN_DOWN_AUTO ? variant : down_form(io->tc != 0, io->level > 0 ? io->level : std::min(h, w) / 2);
+    // the caller's weights, fetched after the work already queued on `stream`, and packed as migan_finalize_weights packs them
+    SepConv L;
+    L.cin = L.cout = C;
+    L.down = kind == MIGAN_STAGE_DOWN;
+    L.up = kind == MIGAN_STAGE_UP2;
+    ToRgb T;
+    float *stem_w = nullptr, *stem_b = nullptr;
+    void* dbuf = nullptr;
+    if (run && kind != MIGAN_STAGE_NOISE_TILE && kind != MIGAN_STAGE_ADD) {
+        auto fetch = [&](const float* src, size_t count) {
+            std::vector<float> v(count);
+            if (!src || cudaMemcpyAsync(v.data(), src, count * sizeof(float), cudaMemcpyDeviceToHost, st) != cudaSuccess) v.clear();
+            return v;
+        };
+        const bool dw = kind == MIGAN_STAGE_DW || L.down, rgb = kind == MIGAN_STAGE_TORGB;
+        CUDA_TRY(cudaStreamSynchronize(st));
+        const std::vector<float> dw_w = dw ? fetch(io->dw_w, 9 * (size_t)C) : std::vector<float>();
+        const std::vector<float> dw_b = dw ? fetch(io->dw_b, C) : std::vector<float>();
+        const std::vector<float> fir = (L.down || L.up) ? fetch(io->fir, 16 * (size_t)C) : rgb && io->img_lo ? fetch(io->fir, 48) : std::vector<float>();
+        const std::vector<float> st_w = kind == MIGAN_STAGE_STEM ? fetch(io->fromrgb_w, 4 * (size_t)C) : std::vector<float>();
+        const std::vector<float> st_b = kind == MIGAN_STAGE_STEM ? fetch(io->fromrgb_b, C) : std::vector<float>();
+        const std::vector<float> rgb_w = rgb ? fetch(io->rgb_w, 3 * (size_t)C) : std::vector<float>();
+        const std::vector<float> rgb_b = rgb ? fetch(io->rgb_b, 3) : std::vector<float>();
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if ((dw && (dw_w.empty() || dw_b.empty())) || ((L.down || L.up || (rgb && io->img_lo)) && fir.empty()) ||
+            (kind == MIGAN_STAGE_STEM && (st_w.empty() || st_b.empty())) || (rgb && (rgb_w.empty() || rgb_b.empty())))
+            return fail(MIGAN_ERR_INVALID, "stage: an operand the kind needs is missing or unreadable");
+        ArenaBuilder ab;
+        if (dw) pack_depthwise(L, dw_w.data(), dw_b.data(), ab);
+        if (L.down || L.up) pack_fir(L, fir.data(), ab);
+        if (kind == MIGAN_STAGE_STEM) {   // the stem kernel reads fromrgb as uploaded
+            memcpy(ab.table(&stem_w, st_w.size()), st_w.data(), sizeof(float) * st_w.size());
+            memcpy(ab.table(&stem_b, st_b.size()), st_b.data(), sizeof(float) * st_b.size());
+        }
+        if (rgb) {
+            float* tw = ab.table(&T.w, rgb_w.size());
+            float* tb = ab.table(&T.b, 4);
+            pack_torgb(rgb_w.data(), rgb_b.data(), io->img_lo ? fir.data() : nullptr, C, tw, tb, io->img_lo ? ab.table(&T.fir, 48) : nullptr);
+        }
+        CUDA_TRY(ab.upload(&dbuf));
+    }
+    std::unique_ptr<void, decltype(&cudaFree)> hold(dbuf, &cudaFree);
+    if (run) {
+        const bool split = kind == MIGAN_STAGE_DOWN && form != MIGAN_DOWN_F32;
+        const bool needs_out = !(split || (kind == MIGAN_STAGE_DW && io->out_hi));
+        if ((needs_out && !io->out) || ((split || (kind == MIGAN_STAGE_DW && io->out_hi)) && (!io->out_hi || !io->out_lo)))
+            return fail(MIGAN_ERR_INVALID, "stage: an output the launch writes is missing");
+    }
+    __half* hi = static_cast<__half*>(io->out_hi);
+    __half* lo = static_cast<__half*>(io->out_lo);
+    cudaError_t e = cudaSuccess;
+    switch (kind) {
+        case MIGAN_STAGE_STEM:
+            e = migan::launch_stem(io->in, stem_w, stem_b, io->out, n, h, w, C, st, &sl);
+            break;
+        case MIGAN_STAGE_DW:
+            e = migan::launch_dw3x3(io->in, L.w9, L.bias, io->out, hi, lo, n, h, w, C, st, &sl);
+            break;
+        case MIGAN_STAGE_DOWN: {
+            migan::DownTensorMap map{};
+            migan::StageLaunch probe;
+            probe.dry = true;
+            if (run_down(L, form, map, io->in, io->out, hi, lo, n, h, w, st, &probe) != cudaSuccess)
+                return fail(MIGAN_ERR_INVALID, "stage: the launcher refuses this shape");
+            if (run && form == MIGAN_DOWN_TMA)   // as PlanBuilder makes it
+                if (const char* err = migan::make_down_tensor_map(&map, io->in, n, h, w, C))
+                    return fail(MIGAN_ERR_INVALID, "stage: tensor map for the down-sampling input failed: %s", err);
+            e = run_down(L, form, map, io->in, io->out, hi, lo, n, h, w, st, &sl);
+            break;
+        }
+        case MIGAN_STAGE_UP2:
+            e = migan::launch_up2(io->in, L.fir16, io->noise, io->noise_pitch, io->skip, io->out, n, h, w, C, st, &sl);
+            break;
+        case MIGAN_STAGE_TORGB:
+            e = migan::launch_torgb(io->in, T.w, T.b, io->img_lo, T.fir, io->out, n, h, w, C, st, &sl);
+            break;
+        case MIGAN_STAGE_NOISE_TILE: {
+            migan::NoiseTileBatch b{};
+            b.count = 1;
+            b.t[0] = {io->in, io->out, io->r, h, w, io->noise_pitch};
+            e = migan::launch_noise_tile(b, st, &sl);
+            break;
+        }
+        case MIGAN_STAGE_ADD:
+            e = migan::launch_add(io->out, io->in, (int64_t)n * h * w * C, st, &sl);
+            break;
+    }
+    if (e == cudaErrorInvalidValue && sl.groups == 0) return fail(MIGAN_ERR_INVALID, "stage: the launcher refuses this shape");
+    if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "stage launch failed: %s", cudaGetErrorString(e));
+    if (plan) *plan = {kind, form, sl.rs, sl.cg, (int)sl.grid, sl.groups, L.down_shift};
+    if (run) {
+        e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "stage launch failed: %s", cudaGetErrorString(e));
+    }
     return MIGAN_OK;
 }
 
