@@ -9,6 +9,7 @@ Public surface (mirrors the reference's for this path):
     holewin.HoleWindowPipeline       the same, but only on windows around the holes; the rest of the photo is untouched
     masks.RandomMaskStream           scripts/generate_masks.py's RandomMask(s) on the GPU: same bytes, same numpy stream
     evaluate.EvalPipeline            evaluate_fid_lpips.py's batch around the generator: resizes, composite, normalisations
+    evaluate.ResultsPipeline         the same batch around another method's result images in place of the generator
     fid.InceptionV3 / fid.FeatureStatistics / fid.calculate_frechet_distance
                                      pytorch_fid's FID features, statistics and distance (InceptionV3 on tensor cores)
     fid.frechet_distance / FeatureStatistics.frechet_distance
@@ -20,6 +21,8 @@ Public surface (mirrors the reference's for this path):
                                      the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double
     generate_masks                   python -m migan_b200.generate_masks: the reference script's CLI and files
     evaluate_fid_lpips               python -m migan_b200.evaluate_fid_lpips: the evaluation script's CLI, sharded over GPUs
+    score_results                    python -m migan_b200.score_results: the evaluation protocol over a directory of any
+                                     method's result images, sharded over GPUs
     demo (python -m)                 python -m migan_b200.demo: scripts/demo.py's CLI and files, sharded over GPUs
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
@@ -36,9 +39,9 @@ _warnings.filterwarnings("ignore", message=r"'migan_b200\.demo' found in sys\.mo
 from . import arch, build, demo, evaluate, export, fid, fullres, holewin, ids, lpips, masks, metrics, ops, parallel, pipeline, synthetic  # noqa: F401
 from .fullres import FullResPipeline  # noqa: F401
 from .holewin import HoleWindowPipeline  # noqa: F401
-from .evaluate import EvalPipeline  # noqa: F401
+from .evaluate import EvalPipeline, ResultsPipeline  # noqa: F401
 from .masks import RandomMaskStream  # noqa: F401
 from .generator import Generator  # noqa: F401
 
-__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "ids", "lpips", "masks", "metrics", "ops", "parallel", "pipeline", "synthetic"]
+__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "ResultsPipeline", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "ids", "lpips", "masks", "metrics", "ops", "parallel", "pipeline", "synthetic"]
 __version__ = "0.1.0"

@@ -22,7 +22,8 @@ Differences from the reference script:
   those features on the device (16 KiB per image), so `--ids` does not combine with `--real-stats`.
 
 Sharding: the sorted list is cut into chunks of `--batch-size` consecutive images and chunk j runs on rank j % W.  A chunk
-is always one `EvalPipeline.forward_batch` call, one LPIPS call and one Inception call on (real, composed), so its
+is always one `EvalPipeline.forward_batch` call (`ResultsPipeline.forward_batch` when `python -m
+migan_b200.score_results` scores result files instead), one LPIPS call and one Inception call on (real, composed), so its
 outputs are the same bytes on any rank at any W.  Per round of W chunks every rank sends its chunk's features and LPIPS
 values to rank 0 in one fixed-size gather (a rank without a chunk sends padding), and rank 0 adds them to the feature
 statistics in chunk order, one `FeatureStatistics.add` per chunk, so the sums see the same rows in the same groups at
@@ -46,7 +47,7 @@ import torch.distributed as dist
 
 from . import _abi, comodgan, fid, ids, lpips
 from ._request_path import load_generator
-from .evaluate import EvalPipeline
+from .evaluate import EvalPipeline, ResultsPipeline
 
 MODELS = {"migan-256": ("migan", 256), "migan-512": ("migan", 512),
           "comodgan-256": ("comodgan", 256), "comodgan-512": ("comodgan", 512)}
@@ -70,9 +71,14 @@ def list_images(real_dir) -> List[Path]:
                   key=lambda p: p.name)
 
 
+def stem_pngs(images: Sequence[Path], directory) -> List[Path]:
+    """`<directory>/<stem>.png` of every image (a.b.jpg -> a.b.png), whether it exists or not."""
+    return [Path(directory) / ("%s.png" % p.stem) for p in images]
+
+
 def list_masks(images: Sequence[Path], mask_dir) -> List[Path]:
     """`<mask_dir>/<stem>.png` of every image; FileNotFoundError names the first that is missing."""
-    masks = [Path(mask_dir) / ("%s.png" % p.stem) for p in images]
+    masks = stem_pngs(images, mask_dir)
     for m, p in zip(masks, images):
         if not m.is_file():
             raise FileNotFoundError("no mask %s for image %s" % (m, p.name))
@@ -124,12 +130,23 @@ class ChunkResult(NamedTuple):
 
 
 class EvalSetup:
-    """What every rank of one evaluation shares: the file lists, the chunking and the networks, on `device`."""
+    """What every rank of one evaluation shares: the file lists, the chunking and the networks, on `device`.
 
-    def __init__(self, model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
-                 num_workers: int = 2, noise_seed: int = 0, real_features: bool = True, inception_weights=None,
-                 lpips_weights=None):
-        self.res = resolution(model_name)
+    The composite's fill-in comes from one of two sources.  A generator: `model_name` and `model`.  Or a method's result
+    files: `results`, the result file of each image of `list_images(real_dir)` in that order, with `model_name` and
+    `model` None and `res` the resolution R (`score_results` plans and checks these lists)."""
+
+    def __init__(self, model_name: Optional[str], model, real_dir, mask_dir=None, *, device="cuda",
+                 batch_size: int = BATCH_SIZE, num_workers: int = 2, noise_seed: int = 0, real_features: bool = True,
+                 inception_weights=None, lpips_weights=None, results: Optional[Sequence] = None,
+                 res: Optional[int] = None):
+        if results is None:
+            self.res = resolution(model_name)
+        elif model_name is not None or model is not None or res is None:
+            raise ValueError("EvalSetup: result files take the place of the generator: pass model_name=None, "
+                             "model=None and res=R")
+        else:
+            self.res = int(res)
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("evaluate_fid_lpips runs on a CUDA device (there is no CPU path); got %s" % self.device)
@@ -138,12 +155,17 @@ class EvalSetup:
         self.images = list_images(real_dir)
         if len(self.images) < 2:
             raise ValueError("%s holds %d images; FID needs at least 2" % (real_dir, len(self.images)))
+        self.results = None if results is None else [Path(r) for r in results]
+        if self.results is not None and len(self.results) != len(self.images):
+            raise ValueError("EvalSetup: %d result files for %d images" % (len(self.results), len(self.images)))
         self.masks = None if mask_dir is None else list_masks(self.images, mask_dir)
         self.chunks = chunk_bounds(len(self.images), int(batch_size))
         self.num_workers = max(1, int(num_workers))
         self.noise_seed = int(noise_seed)
         self.real_features = bool(real_features)
-        if MODELS[model_name][0] == "comodgan":
+        if self.results is not None:
+            self.model = None
+        elif MODELS[model_name][0] == "comodgan":
             self.model = comodgan.load(model, self.res).to(self.device)
         else:
             self.model = load_generator(self, model, self.res, self.device)
@@ -157,7 +179,8 @@ class EvalSetup:
 
 
 class RankWorker:
-    """Rank `rank` of `world_size`: its own `EvalPipeline` (and mask stream) and its host decode pool.  `run_round(r)`
+    """Rank `rank` of `world_size`: its own `EvalPipeline`, or `ResultsPipeline` for result files (and the pipeline's
+    mask stream), and its host decode pool.  `run_round(r)`
     runs this rank's chunk of round r; call it for r = 0, 1, ... in order.  Usable as a context manager (`close()` stops
     the decode threads)."""
 
@@ -165,7 +188,10 @@ class RankWorker:
         if world_size < 1 or not 0 <= rank < world_size:
             raise ValueError("bad rank %d of %d" % (rank, world_size))
         self.setup, self.rank, self.world_size = setup, rank, world_size
-        self.pipe = EvalPipeline(setup.model, setup.res, device=setup.device, seed=0, noise_seed=setup.noise_seed)
+        if setup.results is None:
+            self.pipe = EvalPipeline(setup.model, setup.res, device=setup.device, seed=0, noise_seed=setup.noise_seed)
+        else:
+            self.pipe = ResultsPipeline(setup.res, device=setup.device, seed=0)
         self.rounds = num_rounds(len(setup.chunks), world_size)
         self.own = [j for j in range(rank, len(setup.chunks), world_size)]
         self._pool = ThreadPoolExecutor(max_workers=setup.num_workers)
@@ -193,6 +219,8 @@ class RankWorker:
             self._next += 1
             a, b = self.setup.chunks[j]
             futs = [self._pool.submit(decode_photo, p) for p in self.setup.images[a:b]]
+            if self.setup.results is not None:
+                futs += [self._pool.submit(decode_photo, p) for p in self.setup.results[a:b]]
             if self.setup.masks is not None:
                 futs += [self._pool.submit(decode_mask, p) for p in self.setup.masks[a:b]]
             self._pending.append((j, futs))
@@ -207,7 +235,10 @@ class RankWorker:
         self._submit()                   # keep PREFETCH chunks decoding while the GPU works
         a, b = self.setup.chunks[j]
         c = b - a
-        return arrays[:c], (arrays[c:] if self.setup.masks is not None else None)
+        photos = arrays[:c]
+        results = None if self.setup.results is None else arrays[c:2 * c]
+        masks = None if self.setup.masks is None else arrays[-c:]
+        return photos, results, masks
 
     def _skip_masks(self, upto: int) -> None:
         """Advance the generated-mask stream to image `upto`: the masks of other ranks' chunks are drawn and dropped."""
@@ -220,12 +251,15 @@ class RankWorker:
     def run_chunk(self, j: int) -> ChunkResult:
         setup = self.setup
         a, b = setup.chunks[j]
-        photos, masks = self._decoded(j)
+        photos, results, masks = self._decoded(j)
         if masks is None:
             self._skip_masks(a)
             self._mask_pos = b
-        self.pipe.noise_index = a
-        real, composed = self.pipe.forward_batch(photos, masks)
+        if results is None:
+            self.pipe.noise_index = a
+            real, composed = self.pipe.forward_batch(photos, masks)
+        else:
+            real, composed = self.pipe.forward_batch(photos, results, masks)
         values = setup.lpips(real, composed, normalize=True).view(-1)
         c = b - a
         if setup.real_features:
@@ -359,18 +393,29 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
 
     In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
     rank 0 returns the result; the other ranks return None."""
-    if real_stats is not None and save_real_stats_to is not None:
-        raise ValueError("--real-stats and --save-real-stats exclude each other: with stored statistics the real images "
-                         "are not scored")
-    if ids and real_stats is not None:
-        raise ValueError("--ids needs the real images' features, which stored statistics (--real-stats) do not carry")
-    distributed = dist.is_available() and dist.is_initialized()
-    world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
+    check_stats_args(real_stats, save_real_stats_to, ids)
     if real_stats is not None and not isinstance(real_stats, tuple):
         real_stats = load_real_stats(real_stats)
     setup = EvalSetup(model_name, model, real_dir, mask_dir, device=device, batch_size=batch_size,
                       num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
                       inception_weights=inception_weights, lpips_weights=lpips_weights)
+    return run_setup(setup, real_stats, save_real_stats_to, ids)
+
+
+def check_stats_args(real_stats, save_real_stats_to, ids: bool) -> None:
+    """The refusals of --real-stats, --save-real-stats and --ids, before any work."""
+    if real_stats is not None and save_real_stats_to is not None:
+        raise ValueError("--real-stats and --save-real-stats exclude each other: with stored statistics the real images "
+                         "are not scored")
+    if ids and real_stats is not None:
+        raise ValueError("--ids needs the real images' features, which stored statistics (--real-stats) do not carry")
+
+
+def run_setup(setup: EvalSetup, real_stats=None, save_real_stats_to=None, ids: bool = False) -> Optional[EvalResult]:
+    """Every round of `setup`'s chunks on this rank, merged on rank 0 in chunk order (see `evaluate`); `real_stats`: a
+    loaded (mu, sigma) pair or None."""
+    distributed = dist.is_available() and dist.is_initialized()
+    world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
     merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids) if rank == 0 else None
     t0 = time.perf_counter()
     with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
@@ -412,12 +457,11 @@ def get_args(argv=None):
     return parser.parse_args(argv)
 
 
-def device_for(requested: str, world_size: int, local_rank: int) -> torch.device:
+def device_for(requested: str, world_size: int, local_rank: int, command: str = "evaluate_fid_lpips") -> torch.device:
     """The CUDA device of this process: `requested` alone, `cuda:LOCAL_RANK` under torchrun."""
     dev = torch.device(requested)
     if dev.type != "cuda":
-        raise RuntimeError("evaluate_fid_lpips runs on CUDA devices only (there is no CPU path); got --device %s"
-                           % requested)
+        raise RuntimeError("%s runs on CUDA devices only (there is no CPU path); got --device %s" % (command, requested))
     if world_size > 1:
         if dev.index is not None:
             raise ValueError("--device %s: with several processes each one uses cuda:LOCAL_RANK; pass --device cuda"
@@ -426,29 +470,41 @@ def device_for(requested: str, world_size: int, local_rank: int) -> torch.device
     return dev
 
 
-def main(argv=None) -> None:
-    args = get_args(argv)
-    resolution(args.model_name)
+def run_command(requested_device: str, call, command: str = "evaluate_fid_lpips") -> Optional[EvalResult]:
+    """`call(device)` in this process: alone, or under torchrun (WORLD_SIZE > 1) as one rank of an NCCL process group
+    that lives for the call."""
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
-    device = device_for(args.device, world, local_rank)
+    device = device_for(requested_device, world, local_rank, command)
     if world > 1:
         torch.cuda.set_device(device)
         dist.init_process_group("nccl", device_id=device)
     try:
-        res = evaluate(args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device,
-                       batch_size=args.batch_size, num_workers=args.num_workers, noise_seed=args.noise_seed,
-                       real_stats=args.real_stats, save_real_stats_to=args.save_real_stats,
-                       inception_weights=args.inception_weights, lpips_weights=args.lpips_weights, ids=args.ids)
+        return call(device)
     finally:
         if world > 1:
             dist.destroy_process_group()
+
+
+def print_result(res: Optional[EvalResult], ids: bool) -> None:
+    """The script's two result lines on rank 0, and the discriminative scores' two with `ids`."""
     if res is not None:
         print("FID:", res.fid)
         print("LPIPS: ", res.lpips)
-        if args.ids:
+        if ids:
             print("P-IDS:", res.p_ids)
             print("U-IDS:", res.u_ids)
+
+
+def main(argv=None) -> None:
+    args = get_args(argv)
+    resolution(args.model_name)
+    res = run_command(args.device, lambda device: evaluate(
+        args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device, batch_size=args.batch_size,
+        num_workers=args.num_workers, noise_seed=args.noise_seed, real_stats=args.real_stats,
+        save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
+        lpips_weights=args.lpips_weights, ids=args.ids))
+    print_result(res, args.ids)
 
 
 if __name__ == "__main__":
