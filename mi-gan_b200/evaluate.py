@@ -5,6 +5,7 @@
     real, composed = pipe.forward_batch(imgs)              # generated masks: RandomMask after np.random.seed(seed)
     real, composed = pipe.forward_batch(imgs, masks)       # masks read from --mask-dir
     real, composed = ResultsPipeline(512).forward_batch(imgs, results, masks)   # results in place of the generator
+    real, composed, hole = pipe.forward_batch(imgs, masks, hole_fraction=True)   # and each R x R mask's hole share
 
 `imgs[i]` is `np.array(Image.open(p).convert("RGB"))` of any size (uint8 [H, W, 3]); `masks[i]` is
 `np.array(Image.open(mask_path).convert("L"))` (uint8 [Hm, Wm]).  `real` and `composed` are CUDA float32 [n, 3, R, R]:
@@ -88,11 +89,14 @@ class _EvalBatch(torch.nn.Module):
         keep.append(scratch)
         return resized
 
-    def _passes(self, imgs: Sequence, masks: Optional[Sequence], fill_in, fills: Optional[Sequence] = None):
+    def _passes(self, imgs: Sequence, masks: Optional[Sequence], fill_in, fills: Optional[Sequence] = None,
+                hole_fraction: bool = False):
         """(real, composed) of the photos `imgs`: per pass of up to PIPE_MAX_BATCH photos, the photos' preprocess, then
         `fill_in(c, k, x, fills_d, masks_d, stream, keep) -> (y, launches)` gives the fill-in y [k, 3, R, R] of photos
         c .. c+k (v * 2 / 255 - 1), then the composite.  `fills`: per-photo uint8 [H, W, 3] inputs of the fill-in,
-        checked as the photos are and handed to `fill_in` on the device as `fills_d` (None without them)."""
+        checked as the photos are and handed to `fill_in` on the device as `fills_d` (None without them).
+        `hole_fraction`: also return CUDA float32 [n], 1 - mean of each R x R mask the composite used (x channel 0 is
+        mask - 0.5), computed on the current stream."""
         imgs = list(imgs)
         n, R, dev = len(imgs), self.res, self.device_
         name = type(self).__name__
@@ -104,8 +108,10 @@ class _EvalBatch(torch.nn.Module):
         fills = None if fills is None else [self._check(i, f, None, "result")[0] for i, f in enumerate(fills)]
         real = torch.empty((n, 3, R, R), dtype=torch.float32, device=dev)
         composed = torch.empty((n, 3, R, R), dtype=torch.float32, device=dev)
+        holes = torch.empty(n, dtype=torch.float32, device=dev) if hole_fraction else None
+        out = (real, composed) if holes is None else (real, composed, holes)
         if n == 0:
-            return real, composed
+            return out
         with torch.cuda.device(dev):
             imgs_d = [_to(img, dev, False) for img, _ in checked]
             fills_d = None if fills is None else [_to(f, dev, False) for f in fills]
@@ -126,10 +132,12 @@ class _EvalBatch(torch.nn.Module):
                                            stream, keep)
                 _abi.check(lib.b200_eval_composite(x.data_ptr(), y.data_ptr(), k, R, real[c].data_ptr(),
                                                    composed[c].data_ptr(), stream))
+                if holes is not None:
+                    holes[c:c + k] = 1 - (x[:, 0] + 0.5).mean((1, 2))
                 keep.append((x, y))
                 self.last_launches.append(self.pass_launches(resized, fill_launches))
             torch.cuda.current_stream(dev).synchronize()   # the inputs and the pass buffers are freed on return
-        return real, composed
+        return out
 
 
 class EvalPipeline(_EvalBatch):
@@ -156,15 +164,17 @@ class EvalPipeline(_EvalBatch):
         self.noise.noise_index = int(k)
 
     @torch.no_grad()
-    def forward_batch(self, imgs: Sequence, masks: Optional[Sequence] = None, seeds=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    def forward_batch(self, imgs: Sequence, masks: Optional[Sequence] = None, seeds=None, *,
+                      hole_fraction: bool = False) -> Tuple[torch.Tensor, ...]:
         """(real, composed), CUDA float32 [n, 3, R, R] each.  masks=None takes the next n generated masks.  seeds
-        (Co-Mod-GAN only, else ValueError): one 64-bit noise seed per image instead of the pipeline's counter."""
+        (Co-Mod-GAN only, else ValueError): one 64-bit noise seed per image instead of the pipeline's counter.
+        hole_fraction=True adds a third tensor, CUDA float32 [n]: the share of hole pixels in each R x R mask."""
         imgs = list(imgs)
         seeds = self.noise.take("EvalPipeline", len(imgs), seeds)
 
         def generate(c, k, x, fills_d, masks_d, stream, keep):
             return self.noise.run(self.model, x, None if seeds is None else seeds[c:c + k])
-        return self._passes(imgs, masks, generate)
+        return self._passes(imgs, masks, generate, hole_fraction=hole_fraction)
 
 
 class ResultsPipeline(_EvalBatch):
@@ -179,9 +189,10 @@ class ResultsPipeline(_EvalBatch):
     generated masks."""
 
     @torch.no_grad()
-    def forward_batch(self, imgs: Sequence, results: Sequence, masks: Optional[Sequence] = None
-                      ) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(real, composed), CUDA float32 [n, 3, R, R] each.  masks=None takes the next n generated masks."""
+    def forward_batch(self, imgs: Sequence, results: Sequence, masks: Optional[Sequence] = None, *,
+                      hole_fraction: bool = False) -> Tuple[torch.Tensor, ...]:
+        """(real, composed), CUDA float32 [n, 3, R, R] each.  masks=None takes the next n generated masks.
+        hole_fraction=True adds a third tensor, CUDA float32 [n]: the share of hole pixels in each R x R mask."""
         R = self.res
 
         def resize(c, k, x, fills_d, masks_d, stream, keep):
@@ -192,4 +203,4 @@ class ResultsPipeline(_EvalBatch):
             resized = self._preprocess(_abi.load(), fills_d, masks_d, x_unused, y, stream, keep)
             keep.append(x_unused)
             return y, self.preprocess_launches(resized)
-        return self._passes(imgs, masks, resize, results)
+        return self._passes(imgs, masks, resize, results, hole_fraction)

@@ -19,7 +19,15 @@ Differences from the reference script:
 * FID is computed on the GPU (`FeatureStatistics.frechet_distance`), not with scipy's `sqrtm`.  Only CUDA devices run;
 * `--ids` also prints Co-Mod-GAN's paired and unpaired Inception discriminative scores (`P-IDS:`, `U-IDS:`) after the two
   lines, from the real and composed features of every image (`ids.inception_discriminative_scores`).  Rank 0 keeps
-  those features on the device (16 KiB per image), so `--ids` does not combine with `--real-stats`.
+  those features on the device (16 KiB per image), so `--ids` does not combine with `--real-stats`;
+* `--ssim` and `--psnr` also print `SSIM:` and `PSNR:` after the two lines: the means of the per-image
+  `metrics.compute_ssim(real, composed, window_size=11, size_average=False)` and `metrics.compute_psnr(composed, real,
+  for_dataset=None)` (rgb_range 1, nothing shaved; an image whose composite equals the photo has PSNR inf, and so does
+  the mean), the reference's `eva_ssim` / `eva_psnr` on the tensors LPIPS sees;
+* `--per-image PATH` writes one CSV row per image in the sorted order: `name` (the photo's path relative to
+  `--real-dir`), `hole_fraction` (the share of hole pixels in its R x R mask), `lpips`, then `ssim` and `psnr` when
+  asked for, every number as `repr(float)` of the float64 value.  The file is written under a temporary name and moved
+  into place.
 
 Sharding: the sorted list is cut into chunks of `--batch-size` consecutive images and chunk j runs on rank j % W.  A chunk
 is always one `EvalPipeline.forward_batch` call (`ResultsPipeline.forward_batch` when `python -m
@@ -27,25 +35,28 @@ migan_b200.score_results` scores result files instead), one LPIPS call and one I
 outputs are the same bytes on any rank at any W.  Per round of W chunks every rank sends its chunk's features and LPIPS
 values to rank 0 in one fixed-size gather (a rank without a chunk sends padding), and rank 0 adds them to the feature
 statistics in chunk order, one `FeatureStatistics.add` per chunk, so the sums see the same rows in the same groups at
-every W; with `--ids` it also keeps them in dataset order, so the scores are the same bits at every W.  Generated
+every W; with `--ids` it also keeps them in dataset order, so the scores are the same bits at every W.  The optional
+per-image values (hole fraction, SSIM, PSNR) travel as extra columns of the same gather and are kept at their global
+index as the LPIPS values are, so their means and the CSV are the same bytes at every W.  Generated
 masks come from one sequential stream: every rank advances its own stream through all chunks and
 keeps the masks of its own.
 """
 from __future__ import annotations
 
 import argparse
+import csv
 import os
 import time
 from collections import deque
 from concurrent.futures import ThreadPoolExecutor
 from pathlib import Path
-from typing import List, NamedTuple, Optional, Sequence, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import _abi, comodgan, fid, ids, lpips
+from . import _abi, comodgan, fid, ids, lpips, metrics
 from ._request_path import load_generator
 from .evaluate import EvalPipeline, ResultsPipeline
 
@@ -55,6 +66,8 @@ IMG_EXTENSIONS = {".jpg", ".jpeg", ".JPG", ".JPEG", ".png", ".PNG"}
 BATCH_SIZE = _abi.PIPE_MAX_BATCH
 PREFETCH = 2                    # chunks decoded ahead of the one the GPU works on
 MASK_SKIP = 256                 # generated masks skipped per RandomMaskStream.next call
+EXTRA_VALUES = ("hole_fraction", "ssim", "psnr")    # optional per-image values, in their gather-column order
+PER_IMAGE_COLUMNS = ("name", "hole_fraction", "lpips", "ssim", "psnr")   # the per-image table's column order
 
 
 def resolution(model_name: str) -> int:
@@ -121,12 +134,14 @@ def round_chunk(r: int, rank: int, n_chunks: int, world_size: int) -> Optional[i
 
 class ChunkResult(NamedTuple):
     """What a chunk sends to rank 0: float32 features [c, 2048] (`real` None when the real statistics are loaded from a
-    file) and LPIPS values [c]."""
+    file), LPIPS values [c] and, when the setup asks for any, the extra per-image values [c, len(extra_values)] in
+    `EvalSetup.extra_values` order."""
     index: int
     start: int
     real: Optional[torch.Tensor]
     fake: torch.Tensor
     lpips: torch.Tensor
+    extra: Optional[torch.Tensor] = None
 
 
 class EvalSetup:
@@ -134,12 +149,15 @@ class EvalSetup:
 
     The composite's fill-in comes from one of two sources.  A generator: `model_name` and `model`.  Or a method's result
     files: `results`, the result file of each image of `list_images(real_dir)` in that order, with `model_name` and
-    `model` None and `res` the resolution R (`score_results` plans and checks these lists)."""
+    `model` None and `res` the resolution R (`score_results` plans and checks these lists).
+
+    `ssim` / `psnr`: every chunk also computes each image's SSIM / PSNR; `per_image`: each image's hole fraction too, and
+    rank 0's result keeps the per-image table (`EvalResult.per_image`)."""
 
     def __init__(self, model_name: Optional[str], model, real_dir, mask_dir=None, *, device="cuda",
                  batch_size: int = BATCH_SIZE, num_workers: int = 2, noise_seed: int = 0, real_features: bool = True,
                  inception_weights=None, lpips_weights=None, results: Optional[Sequence] = None,
-                 res: Optional[int] = None):
+                 res: Optional[int] = None, ssim: bool = False, psnr: bool = False, per_image: bool = False):
         if results is None:
             self.res = resolution(model_name)
         elif model_name is not None or model is not None or res is None:
@@ -152,6 +170,7 @@ class EvalSetup:
             raise RuntimeError("evaluate_fid_lpips runs on a CUDA device (there is no CPU path); got %s" % self.device)
         if batch_size < 1:
             raise ValueError("--batch-size must be >= 1, got %d" % batch_size)
+        self.real_dir = Path(real_dir)
         self.images = list_images(real_dir)
         if len(self.images) < 2:
             raise ValueError("%s holds %d images; FID needs at least 2" % (real_dir, len(self.images)))
@@ -163,6 +182,8 @@ class EvalSetup:
         self.num_workers = max(1, int(num_workers))
         self.noise_seed = int(noise_seed)
         self.real_features = bool(real_features)
+        self.per_image = bool(per_image)
+        self.extra_values = tuple(v for v, on in zip(EXTRA_VALUES, (per_image, ssim, psnr)) if on)
         if self.results is not None:
             self.model = None
         elif MODELS[model_name][0] == "comodgan":
@@ -174,8 +195,13 @@ class EvalSetup:
 
     @property
     def feature_width(self) -> int:
-        """Floats per image in a round's gather buffer: the features, then the LPIPS value."""
-        return (2 if self.real_features else 1) * fid.FEATURES + 1
+        """Floats per image in a round's gather buffer: the features, the LPIPS value, then the extra values."""
+        return (2 if self.real_features else 1) * fid.FEATURES + 1 + len(self.extra_values)
+
+    @property
+    def names(self) -> List[str]:
+        """Each image's path relative to `real_dir`, with POSIX separators, in the sorted order."""
+        return [p.relative_to(self.real_dir).as_posix() for p in self.images]
 
 
 class RankWorker:
@@ -255,17 +281,25 @@ class RankWorker:
         if masks is None:
             self._skip_masks(a)
             self._mask_pos = b
+        holes = "hole_fraction" in setup.extra_values
         if results is None:
             self.pipe.noise_index = a
-            real, composed = self.pipe.forward_batch(photos, masks)
+            got = self.pipe.forward_batch(photos, masks, hole_fraction=holes)
         else:
-            real, composed = self.pipe.forward_batch(photos, results, masks)
+            got = self.pipe.forward_batch(photos, results, masks, hole_fraction=holes)
+        real, composed = got[0], got[1]
         values = setup.lpips(real, composed, normalize=True).view(-1)
+        extra = [got[2]] if holes else []
+        if "ssim" in setup.extra_values:
+            extra.append(metrics.compute_ssim(real, composed, window_size=11, size_average=False))
+        if "psnr" in setup.extra_values:
+            extra.append(metrics.compute_psnr(composed, real, for_dataset=None))
+        extra = torch.stack(extra, 1) if extra else None
         c = b - a
         if setup.real_features:
             feats = setup.inception(torch.cat([real, composed]))[0].view(2 * c, fid.FEATURES)
-            return ChunkResult(j, a, feats[:c], feats[c:], values)
-        return ChunkResult(j, a, None, setup.inception(composed)[0].view(c, fid.FEATURES), values)
+            return ChunkResult(j, a, feats[:c], feats[c:], values, extra)
+        return ChunkResult(j, a, None, setup.inception(composed)[0].view(c, fid.FEATURES), values, extra)
 
     def run_round(self, r: int) -> Optional[ChunkResult]:
         j = round_chunk(r, self.rank, len(self.setup.chunks), self.world_size)
@@ -275,15 +309,16 @@ class RankWorker:
 # -- transport and merge --------------------------------------------------------------------------------------------
 
 def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[int, int]], width: int, device,
-                 group=None) -> List[ChunkResult]:
+                 group=None, extra: int = 0) -> List[ChunkResult]:
     """One round's chunk results on rank 0, in chunk order ([] on the other ranks).  Every rank of `group` calls it
-    once per round, with its chunk's result or None: it sends one [batch, width] float32 buffer (features, then the
-    LPIPS value; zero rows pad a short or absent chunk) in one gather.  `width` is 2 * 2048 + 1, or 2048 + 1 without
-    real features."""
+    once per round, with its chunk's result or None: it sends one [batch, width] float32 buffer (features, the LPIPS
+    value, then `extra` per-image values; zero rows pad a short or absent chunk) in one gather.  `width` is
+    2 * 2048 + 1 + extra, or 2048 + 1 + extra without real features."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     batch = chunks[0][1] - chunks[0][0]
     F = fid.FEATURES
-    fake_at, lpips_at = width - 1 - F, width - 1          # real features, when sent, occupy [0, F)
+    lpips_at = width - 1 - extra
+    fake_at = lpips_at - F                                # real features, when sent, occupy [0, F)
     buf = torch.zeros((batch, width), dtype=torch.float32, device=device)
     if result is not None:
         c = result.fake.shape[0]
@@ -291,6 +326,8 @@ def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[i
             buf[:c, :F] = result.real
         buf[:c, fake_at:lpips_at] = result.fake
         buf[:c, lpips_at] = result.lpips
+        if extra:
+            buf[:c, lpips_at + 1:] = result.extra
     bufs = [torch.empty_like(buf) for _ in range(world)] if rank == 0 else None
     dist.gather(buf, bufs, dst=0, group=group)
     if rank != 0:
@@ -301,11 +338,12 @@ def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[i
         if j is not None:
             a, b = chunks[j]
             c = b - a
-            out.append(ChunkResult(j, a, got[:c, :F] if fake_at else None, got[:c, fake_at:lpips_at], got[:c, lpips_at]))
+            out.append(ChunkResult(j, a, got[:c, :F] if fake_at else None, got[:c, fake_at:lpips_at], got[:c, lpips_at],
+                                   got[:c, lpips_at + 1:] if extra else None))
     return out
 
 
-class EvalResult(NamedTuple):
+class _EvalFields(NamedTuple):
     fid: float
     lpips: float                      # np.mean of lpips_values, the script's reduction
     lpips_values: np.ndarray          # float64 [count], dataset (sorted) order
@@ -316,11 +354,31 @@ class EvalResult(NamedTuple):
     u_ids: Optional[float] = None
 
 
+class EvalResult(_EvalFields):
+    """The evaluation's result: a tuple of the eight fields above.  The attributes below are kept outside the tuple, so
+    its length, unpacking and equality stay those of the fields; each is None unless asked for.
+
+    * `ssim` / `psnr`: `np.mean` of the per-image SSIM / PSNR values (inf when an image's PSNR is inf);
+    * `per_image`: {column: values} in `PER_IMAGE_COLUMNS` order: "name" (list of str), then float64 [count] arrays
+      "hole_fraction", "lpips" and, when computed, "ssim" and "psnr", all in dataset (sorted) order."""
+    ssim: Optional[float] = None
+    psnr: Optional[float] = None
+    per_image: Optional[Dict[str, Union[List[str], np.ndarray]]] = None
+
+    def _replace(self, **fields) -> "EvalResult":
+        out = super()._replace(**fields)
+        out.__dict__.update(self.__dict__)
+        return out
+
+
 class Merge:
     """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`.  With `keep_features` it also
-    keeps every real and composed feature row in dataset order on the device, for the discriminative scores."""
+    keeps every real and composed feature row in dataset order on the device, for the discriminative scores.
+    `extra_values`: the names of the chunks' extra per-image values (`EvalSetup.extra_values`), kept at their global
+    index as the LPIPS values are; `names`: each image's name, for the per-image table of the result."""
 
-    def __init__(self, n: int, device, real_features: bool = True, keep_features: bool = False):
+    def __init__(self, n: int, device, real_features: bool = True, keep_features: bool = False,
+                 extra_values: Sequence[str] = (), names: Optional[Sequence[str]] = None):
         self.n, self.device = n, torch.device(device)
         self.real = fid.FeatureStatistics(device=self.device) if real_features else None
         self.fake = fid.FeatureStatistics(device=self.device)
@@ -330,6 +388,15 @@ class Merge:
         if keep_features:
             self.kept = [torch.empty((n, fid.FEATURES), dtype=torch.float32, device=self.device) for _ in range(2)]
         self.values = torch.empty(n, dtype=torch.float32, device=self.device)
+        self.extra_values = tuple(extra_values)
+        if any(v not in EXTRA_VALUES for v in self.extra_values):
+            raise ValueError("extra per-image values are among %s; got %s" % (EXTRA_VALUES, self.extra_values))
+        self.extra = None
+        if self.extra_values:
+            self.extra = torch.empty((n, len(self.extra_values)), dtype=torch.float32, device=self.device)
+        if names is not None and len(names) != n:
+            raise ValueError("%d names for %d images" % (len(names), n))
+        self.names = None if names is None else list(names)
         self.next_chunk = 0
         self.count = 0
 
@@ -341,6 +408,8 @@ class Merge:
             self.real.add(chunk.real)
         self.fake.add(chunk.fake)
         self.values[chunk.start:chunk.start + c] = chunk.lpips.to(self.device)
+        if self.extra is not None:
+            self.extra[chunk.start:chunk.start + c] = chunk.extra.to(self.device)
         if self.kept is not None:
             self.kept[0][chunk.start:chunk.start + c] = chunk.real
             self.kept[1][chunk.start:chunk.start + c] = chunk.fake
@@ -365,7 +434,37 @@ class Merge:
         if self.kept is not None:
             scores = ids.inception_discriminative_scores(*self.kept)
             res = res._replace(p_ids=scores.p_ids, u_ids=scores.u_ids)
+        columns = {"lpips": values}
+        if self.extra is not None:
+            extra = self.extra.cpu().numpy().astype(np.float64)
+            columns.update((v, extra[:, k]) for k, v in enumerate(self.extra_values))
+        if "ssim" in columns:
+            res.ssim = float(np.mean(columns["ssim"]))
+        if "psnr" in columns:
+            res.psnr = float(np.mean(columns["psnr"]))
+        if self.names is not None:
+            columns["name"] = self.names
+            res.per_image = {k: columns[k] for k in PER_IMAGE_COLUMNS if k in columns}
         return res
+
+
+def write_per_image(path, per_image) -> None:
+    """`per_image` (`EvalResult.per_image`) as a CSV file at `path`: a header of its columns, then one row per image,
+    each number as `repr(float)` (so inf is written `inf`).  It is written to a temporary name in the same directory
+    and moved into place with `os.replace`, so `path` never holds a partial table."""
+    path = Path(path)
+    columns = list(per_image)
+    tmp = path.with_name(".%s.%d.tmp" % (path.name, os.getpid()))
+    try:
+        with open(tmp, "w", newline="", encoding="utf-8") as f:
+            w = csv.writer(f, lineterminator="\n")
+            w.writerow(columns)
+            for i, name in enumerate(per_image["name"]):
+                w.writerow([name] + [repr(float(per_image[k][i])) for k in columns[1:]])
+        os.replace(tmp, path)
+    except BaseException:
+        tmp.unlink(missing_ok=True)
+        raise
 
 
 def load_real_stats(path) -> Tuple[np.ndarray, np.ndarray]:
@@ -383,13 +482,15 @@ def save_real_stats(path, mu: np.ndarray, sigma: np.ndarray) -> None:
 
 def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
              num_workers: int = 2, noise_seed: int = 0, real_stats=None, save_real_stats_to=None,
-             inception_weights=None, lpips_weights=None, ids: bool = False) -> Optional[EvalResult]:
+             inception_weights=None, lpips_weights=None, ids: bool = False, ssim: bool = False, psnr: bool = False,
+             per_image: bool = False) -> Optional[EvalResult]:
     """FID and LPIPS of `model` over `real_dir`, as the command prints them.  `model`: a state_dict, a path to one, or a
     generator object (MI-GAN `Generator`, or `comodgan.Generator` for the comodgan names).  `real_stats`: a path to an
     .npz with `mu` and `sigma` (or such a pair); `save_real_stats_to`: where to write the real statistics.
     `inception_weights` / `lpips_weights`: state_dicts or paths instead of the cached weight files.  `ids`: also the
     paired and unpaired Inception discriminative scores (`p_ids`, `u_ids`); it needs the real features, so it excludes
-    `real_stats`.
+    `real_stats`.  `ssim` / `psnr`: also the mean SSIM / PSNR (`EvalResult.ssim` / `.psnr`); `per_image`: also the
+    per-image table (`EvalResult.per_image`).
 
     In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
     rank 0 returns the result; the other ranks return None."""
@@ -398,7 +499,8 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
         real_stats = load_real_stats(real_stats)
     setup = EvalSetup(model_name, model, real_dir, mask_dir, device=device, batch_size=batch_size,
                       num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
-                      inception_weights=inception_weights, lpips_weights=lpips_weights)
+                      inception_weights=inception_weights, lpips_weights=lpips_weights, ssim=ssim, psnr=psnr,
+                      per_image=per_image)
     return run_setup(setup, real_stats, save_real_stats_to, ids)
 
 
@@ -413,16 +515,21 @@ def check_stats_args(real_stats, save_real_stats_to, ids: bool) -> None:
 
 def run_setup(setup: EvalSetup, real_stats=None, save_real_stats_to=None, ids: bool = False) -> Optional[EvalResult]:
     """Every round of `setup`'s chunks on this rank, merged on rank 0 in chunk order (see `evaluate`); `real_stats`: a
-    loaded (mu, sigma) pair or None."""
+    loaded (mu, sigma) pair or None.  The setup's `ssim`, `psnr` and `per_image` choices fill the result's attributes of
+    those names."""
     distributed = dist.is_available() and dist.is_initialized()
     world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
-    merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids) if rank == 0 else None
+    merge = None
+    if rank == 0:
+        merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids,
+                      extra_values=setup.extra_values, names=setup.names if setup.per_image else None)
     t0 = time.perf_counter()
     with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
         for r in range(worker.rounds):
             got = worker.run_round(r)
             if distributed:
-                got = gather_round(got, r, setup.chunks, setup.feature_width, setup.device)
+                got = gather_round(got, r, setup.chunks, setup.feature_width, setup.device,
+                                   extra=len(setup.extra_values))
             else:
                 got = [got]
             for chunk in got:
@@ -454,7 +561,22 @@ def get_args(argv=None):
     parser.add_argument("--lpips-weights", type=Path, default=None, help="LPIPS (alex) state_dict file.")
     parser.add_argument("--ids", action="store_true", help="Also print P-IDS and U-IDS (Co-Mod-GAN's Inception "
                         "discriminative scores).")
+    add_per_image_args(parser)
     return parser.parse_args(argv)
+
+
+def add_per_image_args(parser: argparse.ArgumentParser) -> None:
+    """--ssim, --psnr and --per-image, shared with score_results."""
+    parser.add_argument("--ssim", action="store_true", help="Also print the mean SSIM (window 11).")
+    parser.add_argument("--psnr", action="store_true", help="Also print the mean PSNR (rgb_range 1, nothing shaved).")
+    parser.add_argument("--per-image", type=Path, default=None, metavar="PATH",
+                        help="Write one CSV row per image: name, hole_fraction, lpips[, ssim][, psnr].")
+
+
+def check_per_image_path(path) -> None:
+    """Refuse a --per-image file whose directory does not exist, before any work."""
+    if path is not None and not Path(path).parent.is_dir():
+        raise ValueError("--per-image %s: the directory %s does not exist" % (path, Path(path).parent))
 
 
 def device_for(requested: str, world_size: int, local_rank: int, command: str = "evaluate_fid_lpips") -> torch.device:
@@ -486,25 +608,39 @@ def run_command(requested_device: str, call, command: str = "evaluate_fid_lpips"
             dist.destroy_process_group()
 
 
-def print_result(res: Optional[EvalResult], ids: bool) -> None:
-    """The script's two result lines on rank 0, and the discriminative scores' two with `ids`."""
+def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr: bool = False) -> None:
+    """The script's two result lines on rank 0, then the mean SSIM and PSNR with `ssim` / `psnr`, then the
+    discriminative scores' two with `ids`."""
     if res is not None:
         print("FID:", res.fid)
         print("LPIPS: ", res.lpips)
+        if ssim:
+            print("SSIM:", res.ssim)
+        if psnr:
+            print("PSNR:", res.psnr)
         if ids:
             print("P-IDS:", res.p_ids)
             print("U-IDS:", res.u_ids)
 
 
+def finish_command(res: Optional[EvalResult], args) -> None:
+    """Rank 0's output: the result lines, and the --per-image file."""
+    print_result(res, args.ids, args.ssim, args.psnr)
+    if res is not None and args.per_image is not None:
+        write_per_image(args.per_image, res.per_image)
+
+
 def main(argv=None) -> None:
     args = get_args(argv)
     resolution(args.model_name)
+    check_per_image_path(args.per_image)
     res = run_command(args.device, lambda device: evaluate(
         args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device, batch_size=args.batch_size,
         num_workers=args.num_workers, noise_seed=args.noise_seed, real_stats=args.real_stats,
         save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
-        lpips_weights=args.lpips_weights, ids=args.ids))
-    print_result(res, args.ids)
+        lpips_weights=args.lpips_weights, ids=args.ids, ssim=args.ssim, psnr=args.psnr,
+        per_image=args.per_image is not None))
+    finish_command(res, args)
 
 
 if __name__ == "__main__":

@@ -13,8 +13,8 @@ runs, as in the script; a result the method already composited under the same ma
 from `--mask-dir` (`<stem>.png`, 255 = known) or, without it, from the generated stream with seed 0, as in
 `evaluate_fid_lpips`.
 
-It prints `evaluate_fid_lpips`'s lines (`FID:`, `LPIPS: `, and with `--ids` `P-IDS:` and `U-IDS:`), with its chunking,
-sharding, ordered merge and statistics files: `--save-real-stats` writes the same statistics the evaluation command
+It prints `evaluate_fid_lpips`'s lines (`FID:`, `LPIPS: `, with `--ssim` `SSIM:`, with `--psnr` `PSNR:`, and with `--ids`
+`P-IDS:` and `U-IDS:`), writes its `--per-image` CSV, and has its chunking, sharding, ordered merge and statistics files: `--save-real-stats` writes the same statistics the evaluation command
 writes for the same real directory, R and batch size, and `--real-stats` reads either's.
 
 Before any GPU work one planning pass reads the header (size and mode; no pixels) of every photo, result and mask and
@@ -66,9 +66,10 @@ def check_files(images: Sequence[Path], results: Sequence[Path], masks: Optional
 
 def score(real_dir, results_dir, mask_dir=None, *, resolution: int, device="cuda", batch_size: int = E.BATCH_SIZE,
           num_workers: int = 2, real_stats=None, save_real_stats_to=None, inception_weights=None, lpips_weights=None,
-          ids: bool = False) -> Optional[E.EvalResult]:
+          ids: bool = False, ssim: bool = False, psnr: bool = False, per_image: bool = False) -> Optional[E.EvalResult]:
     """FID and LPIPS of the result files in `results_dir` against the photos of `real_dir`, as the command prints them
-    (`evaluate_fid_lpips.evaluate`'s `EvalResult`).  `resolution`: R, 256 or 512.  The other arguments are `evaluate`'s.
+    (`evaluate_fid_lpips.evaluate`'s `EvalResult`).  `resolution`: R, 256 or 512.  The other arguments are `evaluate`'s,
+    `ssim`, `psnr` and `per_image` among them.
 
     The argument checks and the planning pass (`PlanError`) come before any device is touched.  In an initialised
     process group rank 0 returns the result; the other ranks return None."""
@@ -84,7 +85,8 @@ def score(real_dir, results_dir, mask_dir=None, *, resolution: int, device="cuda
         real_stats = E.load_real_stats(real_stats)
     setup = E.EvalSetup(None, None, real_dir, mask_dir, device=device, batch_size=batch_size, num_workers=num_workers,
                         real_features=real_stats is None, inception_weights=inception_weights,
-                        lpips_weights=lpips_weights, results=results, res=resolution)
+                        lpips_weights=lpips_weights, results=results, res=resolution, ssim=ssim, psnr=psnr,
+                        per_image=per_image)
     return E.run_setup(setup, real_stats, save_real_stats_to, ids)
 
 
@@ -105,18 +107,21 @@ def get_args(argv=None):
     parser.add_argument("--lpips-weights", type=Path, default=None, help="LPIPS (alex) state_dict file.")
     parser.add_argument("--ids", action="store_true", help="Also print P-IDS and U-IDS (Co-Mod-GAN's Inception "
                         "discriminative scores).")
+    E.add_per_image_args(parser)
     return parser.parse_args(argv)
 
 
 def main(argv=None) -> None:
     args = get_args(argv)
     E.check_stats_args(args.real_stats, args.save_real_stats, args.ids)
+    E.check_per_image_path(args.per_image)
     res = E.run_command(args.device, lambda device: score(
         args.real_dir, args.results_dir, args.mask_dir, resolution=args.resolution, device=device,
         batch_size=args.batch_size, num_workers=args.num_workers, real_stats=args.real_stats,
         save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
-        lpips_weights=args.lpips_weights, ids=args.ids), "score_results")
-    E.print_result(res, args.ids)
+        lpips_weights=args.lpips_weights, ids=args.ids, ssim=args.ssim, psnr=args.psnr,
+        per_image=args.per_image is not None), "score_results")
+    E.finish_command(res, args)
 
 
 if __name__ == "__main__":
