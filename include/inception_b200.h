@@ -10,6 +10,7 @@
  *                                      and shapes (472 entries besides num_batches_tracked, fc.* accepted and unused)
  *   inception_features                 model(x)[0].view(n, 2048): the 2048-d pool3 features of x[n,3,H,W] in [0, 1]
  *   fid_stats_update                   the float64 running sums behind np.mean / np.cov(rowvar=False) of the features
+ *   fid_stats_update_binned            the same sums for up to 32 bins of rows at once (statistics per hole size)
  *   fid_stats_mean_cov                 the mean and covariance from those sums, on the device
  *   fid_frechet_distance               the Fréchet distance of two (mu, sigma) on the device (float64 eigensolver)
  *   ids_scores                         P-IDS and U-IDS of paired real / fake features (float64 finite-Newton SVM)
@@ -73,6 +74,14 @@ int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* 
  * first != 0), sum[dim] += sum_i (x_i - shift), sumsq[dim][dim] += sum_i (x_i - shift)(x_i - shift)^T.  Then
  * mean = shift + sum / N and cov = (sumsq - sum sum^T / N) / (N - 1). */
 int fid_stats_update(const float* x, int n, int dim, double* shift, double* sum, double* sumsq, int first, void* stream);
+/* fid_stats_update for nbins (1..FID_STATS_MAX_BINS) sets of sums at once, all on the device: row r of x[n][dim] goes to
+ * bin[r] (int32 [n]; -1, or any value outside [0, nbins): no bin), and bin b holds shift[b][dim], sum[b][dim],
+ * sumsq[b][dim][dim] and count[b] (int64).  Bitwise, every bin ends as if fid_stats_update had run on its rows x[bin == b]
+ * in row order, with first = (count[b] == 0), for every call that gives it a row; nothing of a bin changes otherwise.
+ * No host synchronisation: the bin counts stay on the device. */
+#define FID_STATS_MAX_BINS 32
+int fid_stats_update_binned(const float* x, const int* bin, int n, int dim, int nbins, double* shift, double* sum,
+                            double* sumsq, int64_t* count, void* stream);
 /* mu[dim] = shift + sum / count and sigma[dim][dim] = (sumsq - sum sum^T / count) / (count - 1) from the sums above
  * (float64, device), each operation rounded on its own: bitwise what FeatureStatistics.mean_cov() computes on the host.
  * count >= 2.  Asynchronous on `stream`. */

@@ -316,10 +316,10 @@ typedef struct {
 int b200_window_preprocess(const migan_window_request* reqs_host, int n, void* stream);
 int b200_window_postprocess(const migan_window_request* reqs_host, int n, void* stream);
 
-/* Free-form masks of the evaluation protocol: RandomMask(s) of scripts/generate_masks.py (hole_range [0, 1]), byte for
- * byte and at the same position of numpy's legacy global stream.  One RandomMask result is the first *attempt* whose hole
- * count lies in (0, s^2); an attempt's draws never depend on earlier results, so the stream is a fixed sequence of
- * attempts:
+/* Free-form masks of the evaluation protocol: RandomMask(s, hole_range) of scripts/generate_masks.py, byte for byte and
+ * at the same position of numpy's legacy global stream.  One RandomMask result is the first *attempt* whose hole
+ * count lies in (0, s^2) (hole_range [0, 1]; [h_min, h_max] of migan_mask_hole_bounds for another range); an attempt's
+ * draws never depend on earlier results, so the stream is a fixed sequence of attempts:
  *   migan_np_seed            HOST: np.random.seed(seed) for an integer seed (MT19937 init_genrand, no cached gaussian).
  *   migan_mask_plan          HOST: the draws of the next n_attempts attempts of RandomMask(s), from *state (advanced):
  *                            one migan_mask_record each (records_host), and, when states_host is not NULL, the state
@@ -329,7 +329,15 @@ int b200_window_postprocess(const migan_window_request* reqs_host, int n, void* 
  *                            wide-line polygons and ellipse stamps, exact) and writes its hole count to holes[k].
  *   b200_mask_compact        DEVICE: copies the first min(n, accepted) accepted attempts (0 < holes < s^2), in attempt
  *                            order, to out [n][s][s].
- * s: MIGAN_MASK_MIN_SIZE..MIGAN_MASK_MAX_SIZE; n_attempts: 1..MIGAN_MASK_MAX_ATTEMPTS per call. */
+ * s: MIGAN_MASK_MIN_SIZE..MIGAN_MASK_MAX_SIZE; n_attempts: 1..MIGAN_MASK_MAX_ATTEMPTS per call.
+ * Another hole_range [lo, hi] (0 <= lo < hi <= 1, lo + hi >= 0.2: below that RandomMask draws numpy's refused
+ * randint(0)):
+ *   migan_mask_plan_range    HOST: migan_mask_plan with RandomMask's int(10 * coef), int(5 * coef) and int(20 * coef)
+ *                            tries, coef = min(lo + hi, 1.0) in float64.  [0, 1] gives migan_mask_plan's records.
+ *   migan_mask_hole_bounds   HOST: the hole counts RandomMask(s, [lo, hi]) keeps, [*h_min, *h_max] (empty when
+ *                            *h_min > *h_max): hole_ratio = 1 - fl((s^2 - holes) / s^2) in float64, rejected when
+ *                            hole_ratio <= lo or hole_ratio >= hi.  [0, 1] gives [1, s^2 - 1].
+ *   b200_mask_compact_range  DEVICE: b200_mask_compact keeping the attempts with h_min <= holes <= h_max. */
 #define MIGAN_MASK_MIN_SIZE 2
 #define MIGAN_MASK_MAX_SIZE 4096
 #define MIGAN_MASK_MAX_ATTEMPTS 65535
@@ -354,6 +362,11 @@ int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_re
                     migan_np_random* states_host);
 int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream);
 int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream);
+int migan_mask_plan_range(migan_np_random* state, int s, double lo, double hi, int n_attempts,
+                          migan_mask_record* records_host, migan_np_random* states_host);
+int migan_mask_hole_bounds(int s, double lo, double hi, int* h_min, int* h_max);
+int b200_mask_compact_range(const uint8_t* attempts, const int* holes, int n_attempts, int s, int h_min, int h_max, int n,
+                            uint8_t* out, void* stream);
 
 /* Training snapshot -> inference filter, scripts/export_inference_model.py:18-27 (`get_source_w`): out[cout][fan] =
  * v * rsqrt(sum_fan v^2 + 1e-8) with v = (w_0 + ... + w_{k-1}) / sqrt(k) for a re-parameterised layer (k tensors) or v = w_0

@@ -172,6 +172,10 @@ SYMBOLS = [
     ("migan_mask_plan", c_int, [POINTER(NpRandom), c_int, c_int, c_void_p, c_void_p]),
     ("b200_mask_raster", c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("b200_mask_compact", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    ("migan_mask_plan_range", c_int, [POINTER(NpRandom), c_int, ctypes.c_double, ctypes.c_double, c_int, c_void_p,
+                                      c_void_p]),
+    ("migan_mask_hole_bounds", c_int, [c_int, ctypes.c_double, ctypes.c_double, POINTER(c_int), POINTER(c_int)]),
+    ("b200_mask_compact_range", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("b200_reparam_filter", c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     ("b200_stream_memops_available", c_int, []),
     ("b200_stream_wait_value32", c_int, [c_void_p, c_void_p, ctypes.c_uint32]),

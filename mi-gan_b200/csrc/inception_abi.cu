@@ -334,4 +334,16 @@ int fid_stats_update(const float* x, int n, int dim, double* shift, double* sum,
     return 0;
 }
 
+int fid_stats_update_binned(const float* x, const int* bin, int n, int dim, int nbins, double* shift, double* sum,
+                            double* sumsq, int64_t* count, void* stream) {
+    if (!x || !bin || !shift || !sum || !sumsq || !count) return fail(MIGAN_ERR_INVALID, "null argument");
+    if (n < 1 || dim < 1 || dim > 65536) return fail(MIGAN_ERR_INVALID, "bad feature batch n=%d dim=%d", n, dim);
+    if (nbins < 1 || nbins > FID_STATS_MAX_BINS) return fail(MIGAN_ERR_INVALID, "%d bins (1 to %d)", nbins, FID_STATS_MAX_BINS);
+    const ck_stream_t s = static_cast<ck_stream_t>(stream);
+    CUDA_TRY(comod::ck_launch(incep::StatsShiftBinnedK{x, bin, count, shift, n, dim}, (int64_t)nbins * dim, s));
+    CUDA_TRY(comod::ck_launch(incep::StatsUpdateBinnedK{x, bin, shift, sum, sumsq, count, n, dim},
+                              (int64_t)nbins * dim * dim, s));
+    return 0;
+}
+
 }  // extern "C"

@@ -159,6 +159,47 @@ struct StatsUpdateK {  // items = dim*dim
     }
 };
 
+
+// The same two sums for each bin b of [nbins] over the rows r with bin[r] == b, in row order (a row whose bin is outside
+// [0, nbins) is in none): the very operations StatsShiftK / StatsUpdateK perform on x[bin == b], and nothing for a bin
+// with no row.  A bin's shift is set by the first call that gives it rows (count[b] == 0 before the call).
+struct StatsShiftBinnedK {   // items = nbins*dim
+    const float* x; const int* bin; const int64_t* count; double* shift; int n, dim;
+    CK_HD void operator()(int64_t i) const {
+        const int b = (int)(i / dim), d = (int)(i % dim);
+        if (count[b] != 0) return;
+        double s = 0.0;
+        int c = 0;
+        for (int r = 0; r < n; ++r) {
+            if (bin[r] != b) continue;
+            s += (double)x[(int64_t)r * dim + d];
+            ++c;
+        }
+        if (c) shift[(int64_t)b * dim + d] = s / c;
+    }
+};
+struct StatsUpdateBinnedK {  // items = nbins*dim*dim; item (b, 0, 0) also adds the bin's rows to count[b]
+    const float* x; const int* bin; const double* shift; double* sum; double* sumsq; int64_t* count; int n, dim;
+    CK_HD void operator()(int64_t i) const {
+        const int64_t dd = (int64_t)dim * dim, e = i % dd;
+        const int bn = (int)(i / dd), a = (int)(e / dim), b = (int)(e % dim);
+        const double sa = shift[(int64_t)bn * dim + a], sb = shift[(int64_t)bn * dim + b];
+        double acc = 0.0, s1 = 0.0;
+        int c = 0;
+        for (int r = 0; r < n; ++r) {
+            if (bin[r] != bn) continue;
+            const double va = (double)x[(int64_t)r * dim + a] - sa, vb = (double)x[(int64_t)r * dim + b] - sb;
+            acc += va * vb;
+            s1 += va;
+            ++c;
+        }
+        if (!c) return;
+        sumsq[i] += acc;
+        if (a == b) sum[(int64_t)bn * dim + a] += s1;
+        if (e == 0) count[bn] += c;
+    }
+};
+
 }  // namespace incep
 
 #ifndef MIGAN_EMULATE

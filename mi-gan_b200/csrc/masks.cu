@@ -1,10 +1,11 @@
 // Free-form masks of the evaluation protocol: RandomMask(s) of scripts/generate_masks.py (which the evaluation script's
-// InferenceDataset also calls), identical bytes at the same position of numpy's legacy global stream.
+// InferenceDataset also calls) and RandomMask(s, hole_range), identical bytes at the same position of numpy's legacy
+// global stream.
 //
 //   migan_np_seed -> migan_mask_plan (host: numpy's RandomState draws, one fixed-size record per attempt)
 //   --H2D--> mask_raster_kernel (an attempt's row band per CTA: rectangles, brush quads and discs painted as bit rows in
 //   shared memory, 16-byte stores of 255 / 0, one hole-count atomic per CTA) -> mask_compact_kernel (the first n
-//   attempts with 0 < holes < s^2, in attempt order)
+//   attempts with h_min <= holes <= h_max, in attempt order; (0, s^2) for hole_range [0, 1])
 //
 // The brush is Pillow's (12.x) ImageDraw: a polyline of width w is the union of its two-point wide lines; each is a quad
 // filled by Pillow's polygon scanline rule, which is not translation-invariant, so the quad rows are computed at absolute
@@ -54,7 +55,8 @@ MK_CONST uint8_t kDiscHalf[18][24] = {
     {23, 23, 23, 23, 23, 22, 22, 22, 22, 21, 21, 20, 20, 19, 18, 17, 17, 16, 14, 13, 12, 10, 8, 4},
 };
 
-CK_HD bool mask_accepted(int holes, int s) { return holes > 0 && holes < s * s; }
+// An attempt is kept when its hole count lies in [h_min, h_max] (migan_mask_hole_bounds; (0, s^2) for hole_range [0, 1]).
+CK_HD bool mask_accepted(int holes, int h_min, int h_max) { return holes >= h_min && holes <= h_max; }
 
 // Pillow's ROUND_UP / ROUND_DOWN of a float: f + 0.5f / f - 0.5f in float for f >= 0, |f| +- 0.5 in double below.
 PP_D int mk_round_up(float f) { return f >= 0.f ? (int)floorf(PP_ADD(f, 0.5f)) : -(int)floor(fabs((double)f) + 0.5); }
@@ -237,9 +239,10 @@ inline int mask_raster_launch(const migan_mask_record* recs, int n_att, int s, u
     return 0;
 }
 
-inline int mask_compact_launch(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out, ck_stream_t) {
+inline int mask_compact_launch(const uint8_t* attempts, const int* holes, int n_att, int s, int h_min, int h_max, int n,
+                               uint8_t* out, ck_stream_t) {
     for (int a = 0, j = 0; a < n_att && j < n; ++a)
-        if (mask_accepted(holes[a], s)) memcpy(out + (int64_t)(j++) * s * s, attempts + (int64_t)a * s * s, (size_t)s * s);
+        if (mask_accepted(holes[a], h_min, h_max)) memcpy(out + (int64_t)(j++) * s * s, attempts + (int64_t)a * s * s, (size_t)s * s);
     return 0;
 }
 #else
@@ -265,7 +268,7 @@ __global__ void __launch_bounds__(MK_THREADS) mask_raster_kernel(const migan_mas
 constexpr int MK_COPY_BYTES = MK_THREADS * 16 * 4;
 __global__ void __launch_bounds__(MK_THREADS) mask_compact_kernel(const uint8_t* __restrict__ attempts,
                                                                   const int* __restrict__ holes, int n_att, int s,
-                                                                  uint8_t* __restrict__ out) {
+                                                                  int h_min, int h_max, uint8_t* __restrict__ out) {
     __shared__ int src;
     const int j = blockIdx.y;
     if (threadIdx.x < 32) {
@@ -273,7 +276,7 @@ __global__ void __launch_bounds__(MK_THREADS) mask_compact_kernel(const uint8_t*
         int seen = 0, found = -1;
         for (int base = 0; base < n_att && found < 0; base += 32) {
             const int a = base + lane;
-            const unsigned m = __ballot_sync(0xFFFFFFFFu, a < n_att && mask_accepted(holes[a], s));
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, a < n_att && mask_accepted(holes[a], h_min, h_max));
             const int c = __popc(m);
             if (seen + c > j) {
                 unsigned mm = m;
@@ -305,11 +308,11 @@ inline cudaError_t mask_raster_launch(const migan_mask_record* recs, int n_att, 
     return cudaGetLastError();
 }
 
-inline cudaError_t mask_compact_launch(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out,
-                                       ck_stream_t st) {
+inline cudaError_t mask_compact_launch(const uint8_t* attempts, const int* holes, int n_att, int s, int h_min, int h_max,
+                                       int n, uint8_t* out, ck_stream_t st) {
     const int64_t plane = (int64_t)s * s;
     mask_compact_kernel<<<dim3((unsigned)((plane + MK_COPY_BYTES - 1) / MK_COPY_BYTES), n), MK_THREADS, 0, st>>>(
-        attempts, holes, n_att, s, out);
+        attempts, holes, n_att, s, h_min, h_max, out);
     return cudaGetLastError();
 }
 #endif
@@ -412,10 +415,11 @@ void wide_line_quad(int x0, int y0, int x1, int y1, int width, int16_t* q) {
     for (int i = 0; i < 8; ++i) q[i] = (int16_t)v[i];
 }
 
-// One attempt of RandomMask(s): its draws in the reference's order (scripts/generate_masks.py RandomMask / RandomBrush).
-void plan_attempt(migan_np_random& st, int s, migan_mask_record& r) {
+// One attempt of RandomMask(s, hole_range): its draws in the reference's order (scripts/generate_masks.py RandomMask /
+// RandomBrush).  tries = {int(10 * coef), int(5 * coef), int(20 * coef)}; {10, 5, 20} for hole_range [0, 1].
+void plan_attempt(migan_np_random& st, int s, const int (&tries)[3], migan_mask_record& r) {
     r.n_rects = r.n_segments = r.n_discs = 0;
-    const int tries[2] = {10, 5}, sizes[2] = {s / 2, s};
+    const int sizes[2] = {s / 2, s};
     for (int f = 0; f < 2; ++f) {
         const int64_t n = randint(st, 0, tries[f]);
         for (int64_t t = 0; t < n; ++t) {
@@ -428,7 +432,7 @@ void plan_attempt(migan_np_random& st, int s, migan_mask_record& r) {
     }
     const double mean = 2 * M_PI / 5, spread = 2 * M_PI / 15;
     const double radius = sqrt((double)(s * s + s * s)) / 8, scale = floor(radius / 2);
-    const int64_t ntry = randint(st, 0, 20);
+    const int64_t ntry = randint(st, 0, tries[2]);
     for (int64_t t = 0; t < ntry; ++t) {
         const int nv = (int)randint(st, 4, 18);
         const double lo = mean - uniform(st, 0, spread);
@@ -477,11 +481,55 @@ int check_mask_size(const char* who, int s, int n_att) {
     return MIGAN_OK;
 }
 
-int mask_plan(migan_np_random* st, int s, int n_att, migan_mask_record* recs, migan_np_random* states) {
+// RandomMask's coef = min(lo + hi, 1.0) and its tries int(10 * coef), int(5 * coef), int(20 * coef), as Python evaluates
+// them in float64.  Refuses a range outside 0 <= lo < hi <= 1 and one with int(5 * coef) == 0 (lo + hi < 0.2), where
+// numpy's randint(0) raises.
+int hole_range_tries(const char* who, double lo, double hi, int (&tries)[3]) {
+    if (!(std::isfinite(lo) && std::isfinite(hi) && 0.0 <= lo && lo < hi && hi <= 1.0))
+        return fail(MIGAN_ERR_INVALID, "%s: hole_range [%.17g, %.17g] (0 <= lo < hi <= 1)", who, lo, hi);
+    const double sum = lo + hi, coef = sum < 1.0 ? sum : 1.0;
+    tries[0] = (int)(10.0 * coef);
+    tries[1] = (int)(5.0 * coef);
+    tries[2] = (int)(20.0 * coef);
+    if (tries[1] == 0)
+        return fail(MIGAN_ERR_INVALID, "%s: hole_range [%.17g, %.17g] draws randint(int(5 * %.17g)) = randint(0), which numpy "
+                    "refuses (lo + hi >= 0.2)", who, lo, hi, coef);
+    return MIGAN_OK;
+}
+
+// The hole counts RandomMask(s, [lo, hi]) keeps: hole_ratio = 1 - np.mean(mask) = 1 - fl(k / s^2) with k = s^2 - holes
+// known pixels, rejected when hole_ratio <= lo or hole_ratio >= hi.  hole_ratio never decreases with the hole count, so
+// the kept counts are one interval [*h_min, *h_max] (empty when *h_min > *h_max), found by bisection.
+static double hole_ratio(int holes, int s) {
+    const double n = (double)s * s;
+    return 1.0 - (n - holes) / n;
+}
+
+int hole_bounds(int s, double lo, double hi, int* h_min, int* h_max) {
+    int tries[3];
+    if (int rc = hole_range_tries("mask_hole_bounds", lo, hi, tries)) return rc;
+    const int n = s * s;
+    int a = 0, b = n + 1;                                    // above lo: never at 0 holes; b = n + 1 stands for none
+    while (b - a > 1) {
+        const int m = a + (b - a) / 2;
+        (hole_ratio(m, s) > lo ? b : a) = m;
+    }
+    *h_min = b;
+    a = -1, b = n;                                           // below hi: never at n holes; a = -1 stands for none
+    while (b - a > 1) {
+        const int m = a + (b - a) / 2;
+        (hole_ratio(m, s) < hi ? a : b) = m;
+    }
+    *h_max = a;
+    return MIGAN_OK;
+}
+
+int mask_plan(migan_np_random* st, int s, const int (&tries)[3], int n_att, migan_mask_record* recs,
+              migan_np_random* states) {
     if (int rc = check_mask_size("mask_plan", s, n_att)) return rc;
     if (st->pos < 0 || st->pos > MT_N) return fail(MIGAN_ERR_INVALID, "mask_plan: state position %d (0 to %d)", st->pos, MT_N);
     for (int k = 0; k < n_att; ++k) {
-        plan_attempt(*st, s, recs[k]);
+        plan_attempt(*st, s, tries, recs[k]);
         if (states) states[k] = *st;
     }
     return MIGAN_OK;
@@ -491,9 +539,10 @@ int launch_mask_raster(const migan_mask_record* recs, int n_att, int s, uint8_t*
     return (int)comod::mask_raster_launch(recs, n_att, s, attempts, holes, st);
 }
 
-int launch_mask_compact(const uint8_t* attempts, const int* holes, int n_att, int s, int n, uint8_t* out, ck_stream_t st) {
+int launch_mask_compact(const uint8_t* attempts, const int* holes, int n_att, int s, int h_min, int h_max, int n,
+                        uint8_t* out, ck_stream_t st) {
     if (n < 1) return 0;
-    return (int)comod::mask_compact_launch(attempts, holes, n_att, s, n, out, st);
+    return (int)comod::mask_compact_launch(attempts, holes, n_att, s, h_min, h_max, n, out, st);
 }
 
 }  // namespace migan
@@ -511,7 +560,22 @@ int migan_np_seed(migan_np_random* state, uint32_t seed) {
 
 int migan_mask_plan(migan_np_random* state, int s, int n_attempts, migan_mask_record* records, migan_np_random* states) {
     if (!state || !records) return fail(MIGAN_ERR_INVALID, "mask_plan: null argument");
-    return migan::mask_plan(state, s, n_attempts, records, states);
+    return migan::mask_plan(state, s, {10, 5, 20}, n_attempts, records, states);
+}
+
+int migan_mask_plan_range(migan_np_random* state, int s, double lo, double hi, int n_attempts, migan_mask_record* records,
+                          migan_np_random* states) {
+    if (!state || !records) return fail(MIGAN_ERR_INVALID, "mask_plan_range: null argument");
+    int tries[3];
+    if (int rc = migan::hole_range_tries("mask_plan_range", lo, hi, tries)) return rc;
+    return migan::mask_plan(state, s, tries, n_attempts, records, states);
+}
+
+int migan_mask_hole_bounds(int s, double lo, double hi, int* h_min, int* h_max) {
+    if (!h_min || !h_max) return fail(MIGAN_ERR_INVALID, "mask_hole_bounds: null argument");
+    if (s < MIGAN_MASK_MIN_SIZE || s > MIGAN_MASK_MAX_SIZE)
+        return fail(MIGAN_ERR_INVALID, "mask_hole_bounds: mask size %d (%d to %d)", s, MIGAN_MASK_MIN_SIZE, MIGAN_MASK_MAX_SIZE);
+    return migan::hole_bounds(s, lo, hi, h_min, h_max);
 }
 
 int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, uint8_t* attempts, int* holes, void* stream) {
@@ -522,12 +586,17 @@ int b200_mask_raster(const migan_mask_record* records, int n_attempts, int s, ui
     return MIGAN_OK;
 }
 
-int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream) {
+int b200_mask_compact_range(const uint8_t* attempts, const int* holes, int n_attempts, int s, int h_min, int h_max, int n,
+                            uint8_t* out, void* stream) {
     if (int rc = migan::check_mask_size("mask_compact", s, n_attempts)) return rc;
     if (n < 0 || n > 65535) return fail(MIGAN_ERR_INVALID, "mask_compact: %d masks (0 to 65535 per call)", n);
     if (!attempts || !holes || (n && !out)) return fail(MIGAN_ERR_INVALID, "mask_compact: null argument");
-    CUDA_TRY(migan::launch_mask_compact(attempts, holes, n_attempts, s, n, out, static_cast<ck_stream_t>(stream)));
+    CUDA_TRY(migan::launch_mask_compact(attempts, holes, n_attempts, s, h_min, h_max, n, out, static_cast<ck_stream_t>(stream)));
     return MIGAN_OK;
+}
+
+int b200_mask_compact(const uint8_t* attempts, const int* holes, int n_attempts, int s, int n, uint8_t* out, void* stream) {
+    return b200_mask_compact_range(attempts, holes, n_attempts, s, 1, s * s - 1, n, out, stream);
 }
 
 }  // extern "C"

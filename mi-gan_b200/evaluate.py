@@ -38,14 +38,15 @@ class _EvalBatch(torch.nn.Module):
     """The evaluation batch without its fill-in: the input checks, the mask stream and the per-pass loop that every
     source of the composite's fill-in (a generator, or a method's result images) shares."""
 
-    def __init__(self, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0):
+    def __init__(self, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0,
+                 hole_range: Tuple[float, float] = (0.0, 1.0)):
         super().__init__()
         self.res = int(resolution)
         self.device_ = torch.device(device)
         if self.device_.type != "cuda":
             raise RuntimeError("migan_b200.%s runs on a CUDA device (there is no CPU path); got %s"
                                % (type(self).__name__, self.device_))
-        self.masks = RandomMaskStream(self.res, seed=seed, device=self.device_)
+        self.masks = RandomMaskStream(self.res, seed=seed, device=self.device_, hole_range=hole_range)
         self.last_launches = []                 # kernel launches of each pass of the last call, fill-in included
 
     @staticmethod
@@ -143,14 +144,15 @@ class _EvalBatch(torch.nn.Module):
 class EvalPipeline(_EvalBatch):
     """`model_or_state_dict`: a `migan_b200.Generator`, a state_dict, or a file `torch.load` reads one from; or a
     `migan_b200.comodgan.Generator` of the same resolution (see `comodgan.load`).  `seed`: the script's np.random.seed,
-    for the generated masks.  Co-Mod-GAN draws its noise planes and z from seeded streams on the device: the k-th image
-    processed gets seed `noise_seed * 2**32 + k` (`noise_index` = k) unless `forward_batch(..., seeds=...)` names them,
-    and the generator runs in chunks of at most `generator_batch`."""
+    and `hole_range` RandomMask's, for the generated masks.  Co-Mod-GAN draws its noise planes and z from seeded streams
+    on the device: the k-th image processed gets seed `noise_seed * 2**32 + k` (`noise_index` = k) unless
+    `forward_batch(..., seeds=...)` names them, and the generator runs in chunks of at most `generator_batch`."""
 
     def __init__(self, model_or_state_dict, resolution: int, device: Union[str, torch.device] = "cuda", seed: int = 0, *,
-                 noise_seed: int = 0, generator_batch: int = GENERATOR_BATCH):
+                 noise_seed: int = 0, generator_batch: int = GENERATOR_BATCH,
+                 hole_range: Tuple[float, float] = (0.0, 1.0)):
         model = load_generator(self, model_or_state_dict, resolution, device, accept_comodgan=True)
-        super().__init__(resolution, device, seed)
+        super().__init__(resolution, device, seed, hole_range)
         self.model = model
         self.noise = NoiseSeeds(self.model, noise_seed, generator_batch)
 
@@ -185,8 +187,8 @@ class ResultsPipeline(_EvalBatch):
     photo's own stage -- PIL BICUBIC to R x R when it is not that size, v * 2 / 255 - 1 -- and takes the place of
     `output_imgs` in :244-249: composed = masks * imgs + (1 - masks) * result, then (v * 0.5 + 0.5).clamp(0, 1) of both.
     The composite always runs, as in the script; a result that the method already composited under the same mask comes
-    out unchanged.  `ResultsPipeline(resolution, device="cuda", seed=0)`; `seed`: the script's np.random.seed, for the
-    generated masks."""
+    out unchanged.  `ResultsPipeline(resolution, device="cuda", seed=0, hole_range=(0.0, 1.0))`; `seed`: the script's
+    np.random.seed, and `hole_range` RandomMask's, for the generated masks."""
 
     @torch.no_grad()
     def forward_batch(self, imgs: Sequence, results: Sequence, masks: Optional[Sequence] = None, *,

@@ -27,7 +27,13 @@ Differences from the reference script:
 * `--per-image PATH` writes one CSV row per image in the sorted order: `name` (the photo's path relative to
   `--real-dir`), `hole_fraction` (the share of hole pixels in its R x R mask), `lpips`, then `ssim` and `psnr` when
   asked for, every number as `repr(float)` of the float64 value.  The file is written under a temporary name and moved
-  into place.
+  into place;
+* `--hole-bins EDGES` (comma-separated, strictly increasing, from 0 to 1, 2 to 33 edges) also prints one `HOLE` line per
+  bin of hole fraction h, image i in bin j when e_j <= h_i < e_{j+1} (the last bin also takes h = 1): its image count,
+  the FID of its composed images against the real statistics of *all* images (or `--real-stats`), and the means of its
+  per-image LPIPS, SSIM and PSNR values, and with `--ids` its P-IDS and U-IDS; `nan` where a bin has too few images;
+* `--hole-range LO HI` draws the generated masks from RandomMask(R, [LO, HI]) (`RandomMaskStream(R, 0, hole_range)`)
+  instead of [0, 1]; it does not combine with `--mask-dir`.
 
 Sharding: the sorted list is cut into chunks of `--batch-size` consecutive images and chunk j runs on rank j % W.  A chunk
 is always one `EvalPipeline.forward_batch` call (`ResultsPipeline.forward_batch` when `python -m
@@ -39,12 +45,15 @@ every W; with `--ids` it also keeps them in dataset order, so the scores are the
 per-image values (hole fraction, SSIM, PSNR) travel as extra columns of the same gather and are kept at their global
 index as the LPIPS values are, so their means and the CSV are the same bytes at every W.  Generated
 masks come from one sequential stream: every rank advances its own stream through all chunks and
-keeps the masks of its own.
+keeps the masks of its own.  With `--hole-bins` the hole fraction travels in the gather too, rank 0 computes each
+chunk's bins on the device and adds its composed features to one `BinnedFeatureStatistics` in chunk order, so the bins
+see the same rows in the same groups at every W.
 """
 from __future__ import annotations
 
 import argparse
 import csv
+import math
 import os
 import time
 from collections import deque
@@ -59,6 +68,7 @@ import torch.distributed as dist
 from . import _abi, comodgan, fid, ids, lpips, metrics
 from ._request_path import load_generator
 from .evaluate import EvalPipeline, ResultsPipeline
+from .masks import check_hole_range
 
 MODELS = {"migan-256": ("migan", 256), "migan-512": ("migan", 512),
           "comodgan-256": ("comodgan", 256), "comodgan-512": ("comodgan", 512)}
@@ -68,6 +78,7 @@ PREFETCH = 2                    # chunks decoded ahead of the one the GPU works 
 MASK_SKIP = 256                 # generated masks skipped per RandomMaskStream.next call
 EXTRA_VALUES = ("hole_fraction", "ssim", "psnr")    # optional per-image values, in their gather-column order
 PER_IMAGE_COLUMNS = ("name", "hole_fraction", "lpips", "ssim", "psnr")   # the per-image table's column order
+FULL_RANGE = (0.0, 1.0)         # RandomMask's default hole_range
 
 
 def resolution(model_name: str) -> int:
@@ -152,12 +163,16 @@ class EvalSetup:
     `model` None and `res` the resolution R (`score_results` plans and checks these lists).
 
     `ssim` / `psnr`: every chunk also computes each image's SSIM / PSNR; `per_image`: each image's hole fraction too, and
-    rank 0's result keeps the per-image table (`EvalResult.per_image`)."""
+    rank 0's result keeps the per-image table (`EvalResult.per_image`).  `hole_bins`: the edges of the hole-fraction
+    bins rank 0 scores (`EvalResult.by_hole`; the hole fraction is then computed too); `hole_range`: RandomMask's
+    hole_range for the generated masks."""
 
     def __init__(self, model_name: Optional[str], model, real_dir, mask_dir=None, *, device="cuda",
                  batch_size: int = BATCH_SIZE, num_workers: int = 2, noise_seed: int = 0, real_features: bool = True,
                  inception_weights=None, lpips_weights=None, results: Optional[Sequence] = None,
-                 res: Optional[int] = None, ssim: bool = False, psnr: bool = False, per_image: bool = False):
+                 res: Optional[int] = None, ssim: bool = False, psnr: bool = False, per_image: bool = False,
+                 hole_bins: Optional[Sequence[float]] = None, hole_range: Sequence[float] = FULL_RANGE):
+        self.hole_bins, self.hole_range = check_hole_args(hole_bins, hole_range, mask_dir)
         if results is None:
             self.res = resolution(model_name)
         elif model_name is not None or model is not None or res is None:
@@ -183,7 +198,8 @@ class EvalSetup:
         self.noise_seed = int(noise_seed)
         self.real_features = bool(real_features)
         self.per_image = bool(per_image)
-        self.extra_values = tuple(v for v, on in zip(EXTRA_VALUES, (per_image, ssim, psnr)) if on)
+        holes = per_image or self.hole_bins is not None
+        self.extra_values = tuple(v for v, on in zip(EXTRA_VALUES, (holes, ssim, psnr)) if on)
         if self.results is not None:
             self.model = None
         elif MODELS[model_name][0] == "comodgan":
@@ -215,9 +231,10 @@ class RankWorker:
             raise ValueError("bad rank %d of %d" % (rank, world_size))
         self.setup, self.rank, self.world_size = setup, rank, world_size
         if setup.results is None:
-            self.pipe = EvalPipeline(setup.model, setup.res, device=setup.device, seed=0, noise_seed=setup.noise_seed)
+            self.pipe = EvalPipeline(setup.model, setup.res, device=setup.device, seed=0, noise_seed=setup.noise_seed,
+                                     hole_range=setup.hole_range)
         else:
-            self.pipe = ResultsPipeline(setup.res, device=setup.device, seed=0)
+            self.pipe = ResultsPipeline(setup.res, device=setup.device, seed=0, hole_range=setup.hole_range)
         self.rounds = num_rounds(len(setup.chunks), world_size)
         self.own = [j for j in range(rank, len(setup.chunks), world_size)]
         self._pool = ThreadPoolExecutor(max_workers=setup.num_workers)
@@ -354,16 +371,34 @@ class _EvalFields(NamedTuple):
     u_ids: Optional[float] = None
 
 
+class HoleBin(NamedTuple):
+    """The scores of the images whose hole fraction h lies in [lo, hi) ([lo, hi] for the last bin).  `fid`: the bin's
+    composed images against the real statistics of all images; `lpips`, `ssim`, `psnr`: np.mean of the bin's per-image
+    values.  nan where the bin has too few images (2 for FID and the discriminative scores, 1 for the means); None
+    where the value was not asked for."""
+    lo: float
+    hi: float
+    count: int
+    fid: float
+    lpips: float
+    ssim: Optional[float] = None
+    psnr: Optional[float] = None
+    p_ids: Optional[float] = None
+    u_ids: Optional[float] = None
+
+
 class EvalResult(_EvalFields):
     """The evaluation's result: a tuple of the eight fields above.  The attributes below are kept outside the tuple, so
     its length, unpacking and equality stay those of the fields; each is None unless asked for.
 
     * `ssim` / `psnr`: `np.mean` of the per-image SSIM / PSNR values (inf when an image's PSNR is inf);
     * `per_image`: {column: values} in `PER_IMAGE_COLUMNS` order: "name" (list of str), then float64 [count] arrays
-      "hole_fraction", "lpips" and, when computed, "ssim" and "psnr", all in dataset (sorted) order."""
+      "hole_fraction", "lpips" and, when computed, "ssim" and "psnr", all in dataset (sorted) order;
+    * `by_hole`: with hole bins, one `HoleBin` per bin in edge order."""
     ssim: Optional[float] = None
     psnr: Optional[float] = None
     per_image: Optional[Dict[str, Union[List[str], np.ndarray]]] = None
+    by_hole: Optional[Tuple[HoleBin, ...]] = None
 
     def _replace(self, **fields) -> "EvalResult":
         out = super()._replace(**fields)
@@ -375,10 +410,13 @@ class Merge:
     """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`.  With `keep_features` it also
     keeps every real and composed feature row in dataset order on the device, for the discriminative scores.
     `extra_values`: the names of the chunks' extra per-image values (`EvalSetup.extra_values`), kept at their global
-    index as the LPIPS values are; `names`: each image's name, for the per-image table of the result."""
+    index as the LPIPS values are; `names`: each image's name, for the per-image table of the result; `hole_bins`: the
+    edges of the hole-fraction bins (the extra values then hold "hole_fraction"): each chunk's composed features also
+    go to one `BinnedFeatureStatistics` by their bins, computed on the device."""
 
     def __init__(self, n: int, device, real_features: bool = True, keep_features: bool = False,
-                 extra_values: Sequence[str] = (), names: Optional[Sequence[str]] = None):
+                 extra_values: Sequence[str] = (), names: Optional[Sequence[str]] = None,
+                 hole_bins: Optional[Sequence[float]] = None):
         self.n, self.device = n, torch.device(device)
         self.real = fid.FeatureStatistics(device=self.device) if real_features else None
         self.fake = fid.FeatureStatistics(device=self.device)
@@ -397,6 +435,13 @@ class Merge:
         if names is not None and len(names) != n:
             raise ValueError("%d names for %d images" % (len(names), n))
         self.names = None if names is None else list(names)
+        self.hole_bins = self.binned = None
+        if hole_bins is not None:
+            if "hole_fraction" not in self.extra_values:
+                raise ValueError("hole bins need the hole fraction among the extra per-image values")
+            self.hole_bins = tuple(float(e) for e in hole_bins)
+            self.inner_edges = torch.tensor(self.hole_bins[1:-1], dtype=torch.float64, device=self.device)
+            self.binned = fid.BinnedFeatureStatistics(len(self.hole_bins) - 1, device=self.device)
         self.next_chunk = 0
         self.count = 0
 
@@ -407,6 +452,9 @@ class Merge:
         if self.real is not None:
             self.real.add(chunk.real)
         self.fake.add(chunk.fake)
+        if self.binned is not None:
+            hole = chunk.extra[:, self.extra_values.index("hole_fraction")].to(self.device)
+            self.binned.add(chunk.fake, hole_bin_index(hole, self.inner_edges))
         self.values[chunk.start:chunk.start + c] = chunk.lpips.to(self.device)
         if self.extra is not None:
             self.extra[chunk.start:chunk.start + c] = chunk.extra.to(self.device)
@@ -445,7 +493,72 @@ class Merge:
         if self.names is not None:
             columns["name"] = self.names
             res.per_image = {k: columns[k] for k in PER_IMAGE_COLUMNS if k in columns}
+        if self.binned is not None:
+            res.by_hole = self.hole_results(columns, real_stats)
         return res
+
+    def hole_results(self, columns, real_stats=None) -> Tuple[HoleBin, ...]:
+        """One `HoleBin` per bin: the bins of the merged hole fractions, the binned composed statistics against the
+        real ones of all images (or `real_stats`), and the per-image columns' means over each bin."""
+        bins = hole_bin_index(torch.from_numpy(columns["hole_fraction"]), self.inner_edges.cpu()).numpy()
+        counts = self.binned.counts()
+        want = np.bincount(bins, minlength=len(counts))
+        if not np.array_equal(counts, want):
+            raise RuntimeError("binned feature counts %s differ from the hole fractions' %s" % (counts, want))
+        real = real_stats if real_stats is not None else self.real.mean_cov_device()
+        out = []
+        for b, (lo, hi) in enumerate(zip(self.hole_bins[:-1], self.hole_bins[1:])):
+            idx = np.flatnonzero(bins == b)
+            n = len(idx)
+            fid_b = fid.frechet_distance(*real, *self.binned.mean_cov_device(b, n)) if n >= 2 else math.nan
+            means = {k: float(np.mean(columns[k][idx])) if n else math.nan for k in ("lpips", "ssim", "psnr")
+                     if k in columns}
+            p_ids = u_ids = None
+            if self.kept is not None:
+                p_ids = u_ids = math.nan
+                if n >= 2:
+                    at = torch.from_numpy(idx).to(self.device)
+                    scores = ids.inception_discriminative_scores(self.kept[0][at], self.kept[1][at])
+                    p_ids, u_ids = scores.p_ids, scores.u_ids
+            out.append(HoleBin(lo, hi, n, float(fid_b), means["lpips"], means.get("ssim"), means.get("psnr"), p_ids,
+                               u_ids))
+        return tuple(out)
+
+
+def hole_bin_index(hole: torch.Tensor, inner_edges: torch.Tensor) -> torch.Tensor:
+    """int32 bin of each hole fraction (float32, compared as float64) among the bins of edges 0, *inner_edges, 1: bin j
+    when e_j <= h < e_{j+1}, and the last bin also takes h = 1.  On the tensors' device."""
+    return torch.searchsorted(inner_edges, hole.to(torch.float64).contiguous(), right=True).to(torch.int32)
+
+
+def parse_hole_bins(text: str) -> Tuple[float, ...]:
+    """--hole-bins EDGES: comma-separated edges, checked as `check_hole_bins` does."""
+    try:
+        edges = [float(v) for v in text.split(",")]
+    except ValueError:
+        raise ValueError("--hole-bins %r: a comma-separated list of numbers, e.g. 0,0.2,0.4,1" % text) from None
+    return check_hole_bins(edges)
+
+
+def check_hole_bins(edges: Sequence[float]) -> Tuple[float, ...]:
+    """2 to 33 finite, strictly increasing edges from 0 to 1 (1 to 32 bins)."""
+    edges = tuple(float(e) for e in edges)
+    if not 2 <= len(edges) <= fid.MAX_BINS + 1:
+        raise ValueError("--hole-bins: %d edges (2 to %d: 1 to %d bins)" % (len(edges), fid.MAX_BINS + 1, fid.MAX_BINS))
+    if edges[0] != 0.0 or edges[-1] != 1.0 or not all(math.isfinite(e) for e in edges):
+        raise ValueError("--hole-bins %s: the edges run from 0 to 1" % ",".join(map(repr, edges)))
+    if any(b <= a for a, b in zip(edges, edges[1:])):
+        raise ValueError("--hole-bins %s: the edges must increase strictly" % ",".join(map(repr, edges)))
+    return edges
+
+
+def check_hole_args(hole_bins, hole_range, mask_dir) -> Tuple[Optional[Tuple[float, ...]], Tuple[float, float]]:
+    """The refusals of --hole-bins and --hole-range, before any work: (edges or None, (lo, hi))."""
+    edges = None if hole_bins is None else check_hole_bins(hole_bins)
+    lo_hi = check_hole_range(hole_range, "--hole-range")
+    if lo_hi != FULL_RANGE and mask_dir is not None:
+        raise ValueError("--hole-range draws the generated masks; it does not combine with --mask-dir")
+    return edges, lo_hi
 
 
 def write_per_image(path, per_image) -> None:
@@ -483,24 +596,27 @@ def save_real_stats(path, mu: np.ndarray, sigma: np.ndarray) -> None:
 def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", batch_size: int = BATCH_SIZE,
              num_workers: int = 2, noise_seed: int = 0, real_stats=None, save_real_stats_to=None,
              inception_weights=None, lpips_weights=None, ids: bool = False, ssim: bool = False, psnr: bool = False,
-             per_image: bool = False) -> Optional[EvalResult]:
+             per_image: bool = False, hole_bins: Optional[Sequence[float]] = None,
+             hole_range: Sequence[float] = FULL_RANGE) -> Optional[EvalResult]:
     """FID and LPIPS of `model` over `real_dir`, as the command prints them.  `model`: a state_dict, a path to one, or a
     generator object (MI-GAN `Generator`, or `comodgan.Generator` for the comodgan names).  `real_stats`: a path to an
     .npz with `mu` and `sigma` (or such a pair); `save_real_stats_to`: where to write the real statistics.
     `inception_weights` / `lpips_weights`: state_dicts or paths instead of the cached weight files.  `ids`: also the
     paired and unpaired Inception discriminative scores (`p_ids`, `u_ids`); it needs the real features, so it excludes
     `real_stats`.  `ssim` / `psnr`: also the mean SSIM / PSNR (`EvalResult.ssim` / `.psnr`); `per_image`: also the
-    per-image table (`EvalResult.per_image`).
+    per-image table (`EvalResult.per_image`).  `hole_bins`: the edges of hole-fraction bins, scored one by one
+    (`EvalResult.by_hole`); `hole_range`: RandomMask's hole_range for the generated masks (not with `mask_dir`).
 
     In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
     rank 0 returns the result; the other ranks return None."""
     check_stats_args(real_stats, save_real_stats_to, ids)
+    check_hole_args(hole_bins, hole_range, mask_dir)
     if real_stats is not None and not isinstance(real_stats, tuple):
         real_stats = load_real_stats(real_stats)
     setup = EvalSetup(model_name, model, real_dir, mask_dir, device=device, batch_size=batch_size,
                       num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
                       inception_weights=inception_weights, lpips_weights=lpips_weights, ssim=ssim, psnr=psnr,
-                      per_image=per_image)
+                      per_image=per_image, hole_bins=hole_bins, hole_range=hole_range)
     return run_setup(setup, real_stats, save_real_stats_to, ids)
 
 
@@ -522,7 +638,8 @@ def run_setup(setup: EvalSetup, real_stats=None, save_real_stats_to=None, ids: b
     merge = None
     if rank == 0:
         merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids,
-                      extra_values=setup.extra_values, names=setup.names if setup.per_image else None)
+                      extra_values=setup.extra_values, names=setup.names if setup.per_image else None,
+                      hole_bins=setup.hole_bins)
     t0 = time.perf_counter()
     with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
         for r in range(worker.rounds):
@@ -566,11 +683,23 @@ def get_args(argv=None):
 
 
 def add_per_image_args(parser: argparse.ArgumentParser) -> None:
-    """--ssim, --psnr and --per-image, shared with score_results."""
+    """--ssim, --psnr, --per-image, --hole-bins and --hole-range, shared with score_results."""
     parser.add_argument("--ssim", action="store_true", help="Also print the mean SSIM (window 11).")
     parser.add_argument("--psnr", action="store_true", help="Also print the mean PSNR (rgb_range 1, nothing shaved).")
     parser.add_argument("--per-image", type=Path, default=None, metavar="PATH",
                         help="Write one CSV row per image: name, hole_fraction, lpips[, ssim][, psnr].")
+    parser.add_argument("--hole-bins", type=str, default=None, metavar="EDGES",
+                        help="Also print the scores per bin of hole fraction, e.g. 0,0.1,0.2,0.3,0.4,0.5,0.6,1.")
+    parser.add_argument("--hole-range", type=float, nargs=2, default=None, metavar=("LO", "HI"),
+                        help="Draw the generated masks from RandomMask(R, [LO, HI]) (not with --mask-dir).")
+
+
+def check_hole_flags(args) -> Tuple[Optional[Tuple[float, ...]], Tuple[float, float]]:
+    """--hole-bins and --hole-range of a parsed command line, checked before any work: (edges or None, (lo, hi))."""
+    if args.hole_range is not None and args.mask_dir is not None:
+        raise ValueError("--hole-range draws the generated masks; it does not combine with --mask-dir")
+    edges = None if args.hole_bins is None else parse_hole_bins(args.hole_bins)
+    return check_hole_args(edges, FULL_RANGE if args.hole_range is None else args.hole_range, args.mask_dir)
 
 
 def check_per_image_path(path) -> None:
@@ -608,9 +737,20 @@ def run_command(requested_device: str, call, command: str = "evaluate_fid_lpips"
             dist.destroy_process_group()
 
 
+def hole_line(b: HoleBin, last: bool) -> str:
+    """`HOLE [lo, hi): images n FID f LPIPS l[ SSIM s][ PSNR p][ P-IDS a U-IDS u]`, every number repr(float); the last
+    bin is closed, `[lo, 1.0]`."""
+    line = "HOLE [%r, %r%s: images %d FID %r LPIPS %r" % (float(b.lo), float(b.hi), "]" if last else ")", b.count,
+                                                          float(b.fid), float(b.lpips))
+    for name, v in (("SSIM", b.ssim), ("PSNR", b.psnr), ("P-IDS", b.p_ids), ("U-IDS", b.u_ids)):
+        if v is not None:
+            line += " %s %r" % (name, float(v))
+    return line
+
+
 def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr: bool = False) -> None:
     """The script's two result lines on rank 0, then the mean SSIM and PSNR with `ssim` / `psnr`, then the
-    discriminative scores' two with `ids`."""
+    discriminative scores' two with `ids`, then one `hole_line` per bin with hole bins."""
     if res is not None:
         print("FID:", res.fid)
         print("LPIPS: ", res.lpips)
@@ -621,6 +761,9 @@ def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr:
         if ids:
             print("P-IDS:", res.p_ids)
             print("U-IDS:", res.u_ids)
+        if res.by_hole is not None:
+            for k, b in enumerate(res.by_hole):
+                print(hole_line(b, k == len(res.by_hole) - 1))
 
 
 def finish_command(res: Optional[EvalResult], args) -> None:
@@ -634,12 +777,13 @@ def main(argv=None) -> None:
     args = get_args(argv)
     resolution(args.model_name)
     check_per_image_path(args.per_image)
+    hole_bins, hole_range = check_hole_flags(args)
     res = run_command(args.device, lambda device: evaluate(
         args.model_name, args.model_path, args.real_dir, args.mask_dir, device=device, batch_size=args.batch_size,
         num_workers=args.num_workers, noise_seed=args.noise_seed, real_stats=args.real_stats,
         save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
         lpips_weights=args.lpips_weights, ids=args.ids, ssim=args.ssim, psnr=args.psnr,
-        per_image=args.per_image is not None))
+        per_image=args.per_image is not None, hole_bins=hole_bins, hole_range=hole_range))
     finish_command(res, args)
 
 

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, List, NamedTuple, Tuple, Union
+from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -52,7 +52,10 @@ SYMBOLS = [
                            ctypes.POINTER(ctypes.c_size_t), ctypes.c_void_p]),
     ("fid_stats_update", ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
+    ("fid_stats_update_binned", ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 3 +
+     [ctypes.c_void_p] * 5),
 ]
+MAX_BINS = 32                                  # include/inception_b200.h FID_STATS_MAX_BINS; 32 MiB per bin at d = 2048
 # csrc/frechet.cu: the device mean / covariance and the Fréchet distance
 FRECHET_SYMBOLS = [
     ("fid_stats_mean_cov", ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int64, ctypes.c_int] + [ctypes.c_void_p] * 3),
@@ -211,6 +214,62 @@ class FeatureStatistics:
         mu1, sigma1 = self.mean_cov_device()
         mu2, sigma2 = other.mean_cov_device()
         return _frechet(mu1, sigma1, mu2, sigma2).fid
+
+
+class BinnedFeatureStatistics:
+    """`nbins` FeatureStatistics at once: `add(feats, bins)` gives row i to bin bins[i] (-1: to none), on the device and
+    with no host synchronisation.  Bin b holds, bit for bit, what a FeatureStatistics holds after add(feats[bins == b])
+    for every call in turn (calls with no row in b skipped)."""
+
+    def __init__(self, nbins: int, dim: int = FEATURES, device: Union[str, torch.device] = "cuda"):
+        self.nbins, self.dim = int(nbins), int(dim)
+        if not 1 <= self.nbins <= MAX_BINS:
+            raise ValueError("BinnedFeatureStatistics: %d bins (1 to %d)" % (self.nbins, MAX_BINS))
+        self.device = torch.device(device)
+        self.shift = torch.zeros((self.nbins, self.dim), dtype=torch.float64, device=self.device)
+        self.sum = torch.zeros((self.nbins, self.dim), dtype=torch.float64, device=self.device)
+        self.sumsq = torch.zeros((self.nbins, self.dim, self.dim), dtype=torch.float64, device=self.device)
+        self.count = torch.zeros(self.nbins, dtype=torch.int64, device=self.device)
+
+    @torch.no_grad()
+    def add(self, feats: torch.Tensor, bins: torch.Tensor) -> None:
+        """feats: [n, dim] (or [n, dim, 1, 1]) CUDA tensor; bins: [n] CUDA integer tensor, -1 for a row in no bin."""
+        f = feats.reshape(feats.shape[0], -1)
+        if f.shape[1] != self.dim:
+            raise ValueError("expected features of dimension %d, got %d" % (self.dim, f.shape[1]))
+        if not f.is_cuda or not bins.is_cuda:
+            raise RuntimeError("BinnedFeatureStatistics.add takes CUDA features and bins")
+        if tuple(bins.shape) != (f.shape[0],) or bins.dtype not in (torch.int32, torch.int64):
+            raise ValueError("bins must be an integer tensor of shape [%d], got %s %s" % (f.shape[0], bins.dtype,
+                                                                                        tuple(bins.shape)))
+        if f.shape[0] == 0:
+            return
+        f = f.to(device=self.device, dtype=torch.float32).contiguous()
+        b = bins.to(device=self.device, dtype=torch.int32).contiguous()
+        with torch.cuda.device(self.device):
+            _abi.check(lib().fid_stats_update_binned(f.data_ptr(), b.data_ptr(), f.shape[0], self.dim, self.nbins,
+                                                     self.shift.data_ptr(), self.sum.data_ptr(), self.sumsq.data_ptr(),
+                                                     self.count.data_ptr(),
+                                                     torch.cuda.current_stream(self.device).cuda_stream))
+
+    def counts(self) -> np.ndarray:
+        """The rows each bin has received: int64 [nbins] (one device-to-host copy)."""
+        return self.count.cpu().numpy()
+
+    def mean_cov_device(self, b: int, count: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Bin b's FeatureStatistics.mean_cov_device(): float64 CUDA tensors.  `count` (the bin's entry of counts())
+        saves the copy of the counts."""
+        n = int(self.counts()[b]) if count is None else int(count)
+        if n < 2:
+            raise ValueError("BinnedFeatureStatistics: bin %d needs at least 2 feature rows, has %d" % (b, n))
+        mu = torch.empty(self.dim, dtype=torch.float64, device=self.device)
+        sigma = torch.empty((self.dim, self.dim), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            _abi.check(frechet_lib().fid_stats_mean_cov(self.shift[b].data_ptr(), self.sum[b].data_ptr(),
+                                                        self.sumsq[b].data_ptr(), n, self.dim, mu.data_ptr(),
+                                                        sigma.data_ptr(),
+                                                        torch.cuda.current_stream(self.device).cuda_stream))
+        return mu, sigma
 
 
 def calculate_frechet_distance(mu1, sigma1, mu2, sigma2, eps: float = 1e-6) -> float:

@@ -1,11 +1,12 @@
 """Rate of the evaluation protocol's free-form masks: `RandomMaskStream` on cuda:0 at s = 256 and 512, seed 0.
 
-Reported per size: GPU masks/s of `next(256)` (p50 [min, max] over `--repeats` calls, each ending in the stream's own
+Reported per size and hole range (`--hole-range LO HI`, repeatable; [0, 1] always runs first): GPU masks/s of `next(256)` (p50 [min, max] over `--repeats` calls, each ending in the stream's own
 synchronisation), the library's host planner time per attempt (the part of a call that runs on one host core), and the
-share of the stream's attempts accepted.  The card's name and power limit are read in the same run.  The masks
+share of the stream's attempts accepted with its inverse, the attempts per accepted mask.  The ranges run in turn,
+--repeats rounds of one call each, so each range's p50 and range come from calls alternating with the others'.  The card's name and power limit are read in the same run.  The masks
 themselves are checked against the reference's in tests/test_masks_gpu.py.
 
-    python tools/mask_throughput.py [--repeats 10] [--out tools/out/mask_throughput.json]
+    python tools/mask_throughput.py [--repeats 10] [--hole-range 0.1 0.2 --hole-range 0.5 0.6] [--out FILE]
 """
 import argparse
 import ctypes
@@ -41,36 +42,44 @@ def planner_us_per_attempt(s: int, attempts: int = 256) -> float:
     return (time.perf_counter() - t) / attempts * 1e6
 
 
-def gpu_rate(s: int, repeats: int):
-    stream = RandomMaskStream(s, seed=0)
+def gpu_rates(s: int, repeats: int, ranges):
+    """masks/s of next(BATCH) per hole range, the ranges alternating call by call; and each stream."""
+    streams = [RandomMaskStream(s, seed=0, hole_range=r) for r in ranges]
     out = torch.empty((BATCH, s, s), dtype=torch.uint8, device="cuda")
-    stream.next(BATCH, out=out)                     # warm-up at the timed shape
-    rates = []
+    for stream in streams:
+        stream.next(BATCH, out=out)                 # warm-up at the timed shape
+    rates = [[] for _ in ranges]
     for _ in range(repeats):
-        torch.cuda.synchronize()
-        t = time.perf_counter()
-        stream.next(BATCH, out=out)
-        torch.cuda.synchronize()
-        rates.append(BATCH / (time.perf_counter() - t))
-    return rates, stream.attempts, stream._accepted
+        for k, stream in enumerate(streams):
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            stream.next(BATCH, out=out)
+            torch.cuda.synchronize()
+            rates[k].append(BATCH / (time.perf_counter() - t))
+    return rates, streams
 
 
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=10)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--hole-range", type=float, nargs=2, action="append", default=[], metavar=("LO", "HI"))
     args = ap.parse_args()
     assert torch.cuda.is_available(), "mask_throughput measures on a GPU"
+    ranges = [(0.0, 1.0)] + [tuple(r) for r in args.hole_range]
     res = {"card": card(), "batch": BATCH, "sizes": {}}
     for s in (256, 512):
-        rates, att, acc = gpu_rate(s, args.repeats)
-        row = {"gpu_masks_per_s_p50": statistics.median(rates), "gpu_masks_per_s_min": min(rates),
-               "gpu_masks_per_s_max": max(rates),
-               "planner_us_per_attempt": planner_us_per_attempt(s), "accepted_share": acc / att}
-        res["sizes"][str(s)] = row
-        print("s=%d: GPU %.0f masks/s [%.0f, %.0f]; planner %.1f us/attempt; %.4f of attempts accepted"
-              % (s, row["gpu_masks_per_s_p50"], row["gpu_masks_per_s_min"], row["gpu_masks_per_s_max"],
-                 row["planner_us_per_attempt"], row["accepted_share"]))
+        rates, streams = gpu_rates(s, args.repeats, ranges)
+        for r, rate, stream in zip(ranges, rates, streams):
+            row = {"gpu_masks_per_s_p50": statistics.median(rate), "gpu_masks_per_s_min": min(rate),
+                   "gpu_masks_per_s_max": max(rate), "accepted_share": stream._accepted / stream.attempts,
+                   "attempts_per_mask": stream.attempts / stream._accepted}
+            if r == (0.0, 1.0):
+                row["planner_us_per_attempt"] = planner_us_per_attempt(s)
+            res["sizes"]["%d %s" % (s, list(r))] = row
+            print("s=%d hole_range %s: GPU %.0f masks/s [%.0f, %.0f]; %.2f attempts per mask"
+                  % (s, list(r), row["gpu_masks_per_s_p50"], row["gpu_masks_per_s_min"], row["gpu_masks_per_s_max"],
+                     row["attempts_per_mask"]))
     print("card:", res["card"])
     print(json.dumps(res))
     if args.out:
