@@ -14,6 +14,7 @@
  *   fid_stats_mean_cov                 the mean and covariance from those sums, on the device
  *   fid_frechet_distance               the Fréchet distance of two (mu, sigma) on the device (float64 eigensolver)
  *   ids_scores                         P-IDS and U-IDS of paired real / fake features (float64 finite-Newton SVM)
+ *   kid_subset_terms                   the per-subset kernel sums of the kernel Inception distance (float64 DMMA)
  */
 #ifndef INCEPTION_B200_H_
 #define INCEPTION_B200_H_
@@ -131,6 +132,30 @@ int fid_frechet_distance(const double* mu1, const double* sigma1, const double* 
 size_t ids_workspace_bytes(int64_t n, int dim);
 int ids_scores(const void* real, const void* fake, int64_t n, int dim, int dtype, double* coef, double out_host[5],
                int iterations_host[2], void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- Kernel Inception distance (KID) ---------------------------------------------------------------------------------
+ * The kernel sums behind the unbiased MMD^2 estimate of Binkowski et al. 2018 under the cubic polynomial kernel
+ * k(u, v) = t t t, t = (u.v) / dim + 1, in float64, on num_subsets = S subsets of m rows.  Subset s takes the fake rows
+ * fake_idx_host[s][0..m) of fake[n_fake][dim] (X) and the real rows real_idx_host[s][0..m) of real[n_real][dim] (Y):
+ *   terms[s][0] = Sxx = sum_{i != j} k(x_i, x_j)   terms[s][1] = Syy = sum_{i != j} k(y_i, y_j)
+ *   terms[s][2] = Sxy = sum_{i, j} k(x_i, y_j)
+ * and its estimate is ((Sxx + Syy) / (m - 1) - 2 Sxy / m) / m; the caller draws the subsets and finishes the mean.
+ * The features are read as stored (dtype IDS_FLOAT32 or IDS_FLOAT64, device, row-major) and promoted exactly to float64;
+ * the Gram products run on 64 x 64 fp64 DMMA tiles, the rows gathered through the index tables.  No atomics and sums in
+ * an order fixed by the shapes: the same inputs give the same bytes on every run and on any stream.
+ *
+ * real_idx_host, fake_idx_host: HOST int32 [S][m], checked on the host (each entry in range, the m entries of a subset
+ * distinct) and copied into the workspace on `stream`; they may be freed when the call returns.  terms: device float64
+ * [S][3].  ASYNCHRONOUS on `stream`: nothing is read back.  Refused with MIGAN_ERR_INVALID: null pointers, S < 1,
+ * m < 2, m above n_real or n_fake, n_real or n_fake >= 2^31, dim outside 1..KID_MAX_DIM, an unknown dtype, an index out
+ * of range or repeated within a subset, S x m or the tile grid reaching 2^31; with MIGAN_ERR_WORKSPACE: a workspace that
+ * is short or not 256-byte aligned.  Non-finite features are not checked here: they make the sums non-finite. */
+#define KID_MAX_DIM 4096
+/* Device bytes kid_subset_terms needs (the index tables and S x 3 x ceil(m / 64)^2 tile partials); 0 on bad arguments. */
+size_t kid_workspace_bytes(int num_subsets, int m);
+int kid_subset_terms(const void* real, int64_t n_real, const void* fake, int64_t n_fake, int dim, int dtype,
+                     const int32_t* real_idx_host, const int32_t* fake_idx_host, int num_subsets, int m, double* terms,
+                     void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
