@@ -12,28 +12,7 @@
 //
 // Layout: activations NHWC fp32 [n][H][W][C]; GEMM operands row-major; all indices 64-bit.
 #pragma once
-#include <math.h>
-#include <stdint.h>
-
-#ifdef MIGAN_EMULATE
-#define CK_HD inline
-typedef void* ck_stream_t;
-#else
-#include <cuda_runtime.h>
-#define CK_HD __host__ __device__ __forceinline__
-typedef cudaStream_t ck_stream_t;
-#endif
-
-#ifdef MIGAN_EMULATE
-typedef _Float16 ck_half;                       // IEEE binary16, round-to-nearest-even conversions (GCC, x86-64)
-CK_HD ck_half ck_f2h(float v) { return (ck_half)v; }
-CK_HD float ck_h2f(ck_half h) { return (float)h; }
-#else
-#include <cuda_fp16.h>
-typedef __half ck_half;
-CK_HD ck_half ck_f2h(float v) { return __float2half_rn(v); }
-CK_HD float ck_h2f(ck_half h) { return __half2float(h); }
-#endif
+#include "portable.cuh"
 
 namespace comod {
 
@@ -41,27 +20,6 @@ struct alignas(16) f4 { float x, y, z, w; };
 struct alignas(8) h4 { ck_half x, y, z, w; };
 CK_HD f4 ld4(const float* p) { return *reinterpret_cast<const f4*>(p); }
 CK_HD void st4(float* p, const f4& v) { *reinterpret_cast<f4*>(p) = v; }
-
-#ifdef MIGAN_EMULATE
-template <class F>
-inline int ck_launch(const F& f, int64_t items, ck_stream_t) {
-#pragma omp parallel for schedule(static)
-    for (int64_t i = 0; i < items; ++i) f(i);
-    return 0;
-}
-#else
-template <class F>
-__global__ void __launch_bounds__(256) ck_items_kernel(const F f, const int64_t items) {
-    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i < items) f(i);
-}
-template <class F>
-inline cudaError_t ck_launch(const F& f, int64_t items, ck_stream_t s) {
-    if (items <= 0) return cudaSuccess;
-    ck_items_kernel<F><<<(unsigned)((items + 255) / 256), 256, 0, s>>>(f, items);
-    return cudaGetLastError();
-}
-#endif
 
 // ---- batches of requests in one launch ---------------------------------------------------------------------------
 // A batch descriptor holds n requests r[] and the launch's item prefix start[]: item i belongs to the request k with

@@ -45,17 +45,9 @@ constexpr float MAP_LR = 0.01f;                                          // styl
 constexpr float SQRT2 = 1.41421356237309515f;
 
 inline int channels(int res) { return std::min(32768 / res, 512); }   // comodgan.py:140-141 (ch_base 32768, ch_max 512)
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-inline int round_up(int v, int a) { return (v + a - 1) / a * a; }
 
-// ---- device memory / GEMM: the only things that differ between the product and the emulation build ---------------
+// ---- GEMMs: the kernels, or in the emulation build the same arithmetic as host loops -------------------------------
 #ifdef MIGAN_EMULATE
-int dev_set(int) { return 0; }
-int dev_alloc(void** p, size_t bytes) { *p = aligned_alloc(256, align_up(std::max<size_t>(bytes, 1), 256)); return *p ? 0 : 1; }
-void dev_free(void* p) { free(p); }
-int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t) { memcpy(d, s, bytes); return 0; }
-int dev_sync() { return 0; }
-const char* dev_err(int) { return "emulation"; }
 int gemm_f32(const float* A, const float* Bt, float* out, int64_t P, int K, int N, ck_stream_t) {
 #pragma omp parallel for schedule(static)
     for (int64_t p = 0; p < P; ++p) {
@@ -89,12 +81,6 @@ const char* gemm_tc(const ck_half* a_hi, const ck_half* a_lo, const ck_half* b_h
 }
 int tc_configure() { return 0; }
 #else
-int dev_set(int d) { return (int)cudaSetDevice(d); }
-int dev_alloc(void** p, size_t bytes) { return (int)cudaMalloc(p, std::max<size_t>(bytes, 256)); }
-void dev_free(void* p) { cudaFree(p); }
-int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t st) { return (int)cudaMemcpyAsync(d, s, bytes, cudaMemcpyDefault, st); }
-int dev_sync() { return (int)cudaDeviceSynchronize(); }
-const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
 int gemm_f32(const float* A, const float* Bt, float* out, int64_t P, int K, int N, ck_stream_t s) {
     return (int)migan::launch_pw_gemm_simt(A, Bt, out, P, K, N, nullptr, 1, 1, 1, 0, s);
 }
@@ -929,13 +915,8 @@ int b200_conv2d_resample(const float* x, const float* w, const float* f, float* 
     // filter taps live in kernel parameters: fetch them from the device once (tiny, synchronous)
     float taps_raw[64] = {1.f};
     if (f && y) {
-#ifdef MIGAN_EMULATE
-        memcpy(taps_raw, f, sizeof(float) * fh * fw);
-#else
-        cudaError_t e = cudaMemcpyAsync(taps_raw, f, sizeof(float) * fh * fw, cudaMemcpyDeviceToHost, (cudaStream_t)stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
-        if (e != cudaSuccess) return fail(MIGAN_ERR_CUDA, "conv2d_resample: reading the filter failed: %s", cudaGetErrorString(e));
-#endif
+        if (int e = to_host(taps_raw, f, sizeof(float) * fh * fw, static_cast<ck_stream_t>(stream)))
+            return fail(MIGAN_ERR_CUDA, "conv2d_resample: reading the filter failed: %s", dev_err(e));
     }
     auto make_taps = [&](bool identity, float gain, float out[64], int& ofh, int& ofw) {
         if (identity || no_filter) { ofh = ofw = 1; out[0] = gain; return; }

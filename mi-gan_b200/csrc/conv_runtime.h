@@ -2,7 +2,6 @@
 // InceptionV3 (inception_abi.cu) and the LPIPS AlexNet (lpips_abi.cu).  Header-only, so each runtime compiles alone,
 // in the product library and in the emulation build (-DMIGAN_EMULATE) alike.
 //
-//   device memory     dev_set / dev_alloc / dev_free / dev_copy / dev_sync / dev_err
 //   convolution       conv_launch: the kernel's launch, or in the emulation build the same arithmetic as a host loop
 //   weights           ConvL (one convolution's shape and packed operand), upload_conv (TF32 hi / lo packing)
 //   forward walk      Runner (workspace bump allocator, launch counting, launch plan), Act, conv_step, pool_step
@@ -25,9 +24,6 @@
 
 namespace incep {
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-inline int round_up(int v, int a) { return (v + a - 1) / a * a; }
-
 // One convolution: its state_dict prefix, shape and, after finalize, the packed operand.
 struct ConvL {
     std::string name;
@@ -38,14 +34,8 @@ struct ConvL {
     float* bias = nullptr;  // [cout]
 };
 
-// ---- device memory and the convolution: the only things that differ between the product and the emulation build ----
+// ---- the convolution: the kernel's launch, or in the emulation build the same arithmetic as a host loop ------------
 #ifdef MIGAN_EMULATE
-inline int dev_set(int) { return 0; }
-inline int dev_alloc(void** p, size_t bytes) { *p = aligned_alloc(256, align_up(std::max<size_t>(bytes, 1), 256)); return *p ? 0 : 1; }
-inline void dev_free(void* p) { free(p); }
-inline int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t) { memcpy(d, s, bytes); return 0; }
-inline int dev_sync() { return 0; }
-inline const char* dev_err(int) { return "emulation"; }
 // The tensor-core kernel's arithmetic: hi*hi into one sum, hi*lo + lo*hi into a second, added with the bias, ReLU.
 inline int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
                        int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
@@ -83,12 +73,6 @@ inline int conv_launch(const float* x, const float* bhi, const float* blo, const
     return 0;
 }
 #else
-inline int dev_set(int d) { return (int)cudaSetDevice(d); }
-inline int dev_alloc(void** p, size_t bytes) { return (int)cudaMalloc(p, std::max<size_t>(bytes, 256)); }
-inline void dev_free(void* p) { cudaFree(p); }
-inline int dev_copy(void* d, const void* s, size_t bytes, ck_stream_t st) { return (int)cudaMemcpyAsync(d, s, bytes, cudaMemcpyDefault, st); }
-inline int dev_sync() { return (int)cudaDeviceSynchronize(); }
-inline const char* dev_err(int e) { return cudaGetErrorString((cudaError_t)e); }
 inline int conv_launch(const float* x, const float* bhi, const float* blo, const float* bias, float* y, int n, int H, int W,
                        int cinp, int OH, int OW, int kh, int kw, int stride, int ph, int pw, int cout, int KP, int ct, int c0,
                        ck_stream_t s) {

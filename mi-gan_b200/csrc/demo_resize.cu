@@ -27,27 +27,10 @@
 //   height pass (both only when a photo is larger than R) -> R x R resize + mask + x  |  y -> uint8 + OpenCV width pass
 //   -> OpenCV height pass + composite.
 // Item kernels (comod_kernels.cuh style): the emulation build (tests/emul/build_emul.py) runs the very same functors on
-// the CPU.  Every product and sum is rounded on its own (no FMA contraction), in double where the libraries use double.
+// the CPU.  Every product and sum is rounded on its own (the *_rn functions of portable.cuh, no FMA contraction), in
+// double where the libraries use double.
 #include "prepost.cuh"
 #include "abi_error.h"
-
-#ifdef MIGAN_EMULATE
-#define DM_DMUL(a, b) ((a) * (b))
-#define DM_DADD(a, b) ((a) + (b))
-#define DM_DDIV(a, b) ((a) / (b))
-#define DM_FMUL(a, b) ((a) * (b))
-#define DM_FADD(a, b) ((a) + (b))
-#define DM_FDIV(a, b) ((a) / (b))
-#define DM_D inline
-#else
-#define DM_DMUL(a, b) __dmul_rn((a), (b))
-#define DM_DADD(a, b) __dadd_rn((a), (b))
-#define DM_DDIV(a, b) __ddiv_rn((a), (b))
-#define DM_FMUL(a, b) __fmul_rn((a), (b))
-#define DM_FADD(a, b) __fadd_rn((a), (b))
-#define DM_FDIV(a, b) __fdiv_rn((a), (b))
-#define DM_D __device__ __forceinline__
-#endif
 
 namespace comod {
 
@@ -62,35 +45,35 @@ CK_HD int pil_ksize(int in_size, int out_size) {
     return (int)ceil(2.0 * (scale < 1.0 ? 1.0 : scale)) * 2 + 1;
 }
 
-DM_D double pil_bicubic(double x) {     // bicubic_filter, a = -0.5
+CK_D double pil_bicubic(double x) {     // bicubic_filter, a = -0.5
     if (x < 0.0) x = -x;
-    if (x < 1.0) return DM_DADD(DM_DMUL(DM_DMUL(DM_DADD(DM_DMUL(1.5, x), -2.5), x), x), 1.0);   // ((a+2)x - (a+3))x x + 1
-    if (x < 2.0) return DM_DMUL(DM_DADD(DM_DMUL(DM_DADD(DM_DMUL(DM_DADD(x, -5.0), x), 8.0), x), -4.0), -0.5);  // (((x-5)x+8)x-4)a
+    if (x < 1.0) return dadd_rn(dmul_rn(dmul_rn(dadd_rn(dmul_rn(1.5, x), -2.5), x), x), 1.0);   // ((a+2)x - (a+3))x x + 1
+    if (x < 2.0) return dmul_rn(dadd_rn(dmul_rn(dadd_rn(dmul_rn(dadd_rn(x, -5.0), x), 8.0), x), -4.0), -0.5);  // (((x-5)x+8)x-4)a
     return 0.0;
 }
 
 // Entry x of Pillow's bicubic table in_size -> out_size (precompute_coeffs + normalize_coeffs_8bpc): the first source
 // index and `ksize` fixed-point taps, zero past the window.  The weights are recomputed for the division by their sum
 // instead of being held in a local array (a 4K photo has 31 taps).
-DM_D void pil_entry(int in_size, int out_size, int ksize, int x, int* xmin, int* k) {
-    const double scale = DM_DDIV((double)in_size, (double)out_size);
+CK_D void pil_entry(int in_size, int out_size, int ksize, int x, int* xmin, int* k) {
+    const double scale = ddiv_rn((double)in_size, (double)out_size);
     const double fs = scale < 1.0 ? 1.0 : scale;
-    const double support = DM_DMUL(2.0, fs);
-    const double ss = DM_DDIV(1.0, fs);
-    const double center = DM_DMUL(DM_DADD((double)x, 0.5), scale);
-    int lo = (int)DM_DADD(DM_DADD(center, -support), 0.5);
+    const double support = dmul_rn(2.0, fs);
+    const double ss = ddiv_rn(1.0, fs);
+    const double center = dmul_rn(dadd_rn((double)x, 0.5), scale);
+    int lo = (int)dadd_rn(dadd_rn(center, -support), 0.5);
     if (lo < 0) lo = 0;
-    int hi = (int)DM_DADD(DM_DADD(center, support), 0.5);
+    int hi = (int)dadd_rn(dadd_rn(center, support), 0.5);
     if (hi > in_size) hi = in_size;
     int n = hi - lo;
     n = n < 0 ? 0 : (n > ksize ? ksize : n);
     double ww = 0.0;
-    for (int i = 0; i < n; ++i) ww = DM_DADD(ww, pil_bicubic(DM_DMUL(DM_DADD(DM_DADD((double)(i + lo), -center), 0.5), ss)));
+    for (int i = 0; i < n; ++i) ww = dadd_rn(ww, pil_bicubic(dmul_rn(dadd_rn(dadd_rn((double)(i + lo), -center), 0.5), ss)));
     for (int i = 0; i < n; ++i) {
-        double w = pil_bicubic(DM_DMUL(DM_DADD(DM_DADD((double)(i + lo), -center), 0.5), ss));
-        if (ww != 0.0) w = DM_DDIV(w, ww);
-        const double q = DM_DMUL(w, (double)(1 << PIL_BITS));
-        k[i] = w < 0.0 ? (int)DM_DADD(q, -0.5) : (int)DM_DADD(q, 0.5);
+        double w = pil_bicubic(dmul_rn(dadd_rn(dadd_rn((double)(i + lo), -center), 0.5), ss));
+        if (ww != 0.0) w = ddiv_rn(w, ww);
+        const double q = dmul_rn(w, (double)(1 << PIL_BITS));
+        k[i] = w < 0.0 ? (int)dadd_rn(q, -0.5) : (int)dadd_rn(q, 0.5);
     }
     for (int i = n; i < ksize; ++i) k[i] = 0;
     *xmin = lo;
@@ -98,31 +81,31 @@ DM_D void pil_entry(int in_size, int out_size, int ksize, int x, int* xmin, int*
 
 // Source index of output x of Pillow's NEAREST resize in_size -> out_size (ImagingScaleAffine): the coordinate starts at
 // s / 2 and adds s = in / out per output, in double; the same accumulation is replayed here for every output.
-DM_D int pil_nearest(int in_size, int out_size, int x) {
+CK_D int pil_nearest(int in_size, int out_size, int x) {
     if (in_size == out_size) return x;
-    const double s = DM_DDIV((double)in_size, (double)out_size);
-    double xo = DM_DADD(0.0, DM_DMUL(s, 0.5));
-    for (int i = 0; i < x; ++i) xo = DM_DADD(xo, s);
+    const double s = ddiv_rn((double)in_size, (double)out_size);
+    double xo = dadd_rn(0.0, dmul_rn(s, 0.5));
+    for (int i = 0; i < x; ++i) xo = dadd_rn(xo, s);
     const int v = xo < 0.0 ? -1 : (int)xo;
     return v < 0 ? 0 : (v >= in_size ? in_size - 1 : v);
 }
 
 // Entry d of OpenCV's INTER_CUBIC table in_size -> out_size (resizeGeneric, interpolateCubic, fixed point): the first tap's
 // neighbour sx (taps at sx-1 .. sx+2, clamped to the image by the caller) and the four coefficients in units of 1/2048.
-DM_D void cv_entry(int in_size, int out_size, int d, int* sx, int* c) {
-    const double scale = DM_DDIV(1.0, DM_DDIV((double)out_size, (double)in_size));     // 1. / inv_scale
-    const float f = (float)DM_DADD(DM_DMUL(DM_DADD((double)d, 0.5), scale), -0.5);
+CK_D void cv_entry(int in_size, int out_size, int d, int* sx, int* c) {
+    const double scale = ddiv_rn(1.0, ddiv_rn((double)out_size, (double)in_size));     // 1. / inv_scale
+    const float f = (float)dadd_rn(dmul_rn(dadd_rn((double)d, 0.5), scale), -0.5);
     const int s = (int)floorf(f);
-    const float x = DM_FADD(f, -(float)s);
-    const float x1 = DM_FADD(x, 1.f), y = DM_FADD(1.f, -x);
+    const float x = fadd_rn(f, -(float)s);
+    const float x1 = fadd_rn(x, 1.f), y = fadd_rn(1.f, -x);
     const float A = -0.75f;
-    const float c0 = DM_FADD(DM_FMUL(DM_FADD(DM_FMUL(DM_FADD(DM_FMUL(A, x1), 3.75f), x1), -6.f), x1), 3.f);   // ((A(x+1) - 5A)(x+1) + 8A)(x+1) - 4A
-    const float c1 = DM_FADD(DM_FMUL(DM_FMUL(DM_FADD(DM_FMUL(1.25f, x), -2.25f), x), x), 1.f);              // ((A+2)x - (A+3))x x + 1
-    const float c2 = DM_FADD(DM_FMUL(DM_FMUL(DM_FADD(DM_FMUL(1.25f, y), -2.25f), y), y), 1.f);
-    const float c3 = DM_FADD(DM_FADD(DM_FADD(1.f, -c0), -c1), -c2);
+    const float c0 = fadd_rn(fmul_rn(fadd_rn(fmul_rn(fadd_rn(fmul_rn(A, x1), 3.75f), x1), -6.f), x1), 3.f);   // ((A(x+1) - 5A)(x+1) + 8A)(x+1) - 4A
+    const float c1 = fadd_rn(fmul_rn(fmul_rn(fadd_rn(fmul_rn(1.25f, x), -2.25f), x), x), 1.f);              // ((A+2)x - (A+3))x x + 1
+    const float c2 = fadd_rn(fmul_rn(fmul_rn(fadd_rn(fmul_rn(1.25f, y), -2.25f), y), y), 1.f);
+    const float c3 = fadd_rn(fadd_rn(fadd_rn(1.f, -c0), -c1), -c2);
     *sx = s;
-    c[0] = (int)rintf(DM_FMUL(c0, 2048.f)); c[1] = (int)rintf(DM_FMUL(c1, 2048.f));
-    c[2] = (int)rintf(DM_FMUL(c2, 2048.f)); c[3] = (int)rintf(DM_FMUL(c3, 2048.f));
+    c[0] = (int)rintf(fmul_rn(c0, 2048.f)); c[1] = (int)rintf(fmul_rn(c1, 2048.f));
+    c[2] = (int)rintf(fmul_rn(c2, 2048.f)); c[3] = (int)rintf(fmul_rn(c3, 2048.f));
 }
 
 CK_HD int dm_clamp(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
@@ -184,7 +167,7 @@ CK_HD int64_t demo_items(int stage, const DemoReq& r, int R) {
 // Every table entry of every request.  items per request = demo_items(DS_TABLES)
 struct DemoTablesK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int R = b.res;
@@ -216,7 +199,7 @@ struct DemoTablesK {
 // Width pass of the down-scale, W -> w1 on every photo row.  items per request = H * w1 (0 when the photo fits)
 struct DemoDownWK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -238,7 +221,7 @@ struct DemoDownWK {
 // Height pass of the down-scale, H -> h1, into img_resized.  items per request = h1 * w1 (0 when the photo fits)
 struct DemoDownHK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -260,7 +243,7 @@ struct DemoDownHK {
 // mask_resized -> R x R (NEAREST), then PreU8K's arithmetic (prepost.cu) into x[k].  items per request = R * R
 struct DemoSquareK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -296,14 +279,14 @@ struct DemoSquareK {
 // composed.  m = x channel 0 + 0.5.  items = n * R * R
 struct EvalCompositeK {
     const float* x; const float* y; float* real; float* composed; int64_t plane;
-    PP_D static float unit(float v) { return fminf(fmaxf(PP_ADD(PP_MUL(v, 0.5f), 0.5f), 0.f), 1.f); }
-    PP_D void operator()(int64_t i) const {
+    CK_D static float unit(float v) { return fminf(fmaxf(fadd_rn(fmul_rn(v, 0.5f), 0.5f), 0.f), 1.f); }
+    CK_D void operator()(int64_t i) const {
         const int64_t k = i / plane, p = i - k * plane;
-        const float m = PP_ADD(x[k * 4 * plane + p], 0.5f);
+        const float m = fadd_rn(x[k * 4 * plane + p], 0.5f);
         for (int c = 0; c < 3; ++c) {
             const int64_t o = (k * 3 + c) * plane + p;
             const float v = real[o];
-            composed[o] = unit(PP_ADD(PP_MUL(m, v), PP_MUL(PP_ADD(1.f, -m), y[o])));
+            composed[o] = unit(fadd_rn(fmul_rn(m, v), fmul_rn(fadd_rn(1.f, -m), y[o])));
             real[o] = unit(v);
         }
     }
@@ -313,7 +296,7 @@ struct EvalCompositeK {
 // items per request = R * w1
 struct DemoPostWK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -337,7 +320,7 @@ struct DemoPostWK {
 // mask is 255, the resized result elsewhere.  items per request = h1 * w1
 struct DemoOutK {
     const DemoBatch& b;
-    DM_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const DemoReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -355,15 +338,15 @@ struct DemoOutK {
         float bk[4];
         const int* src[4];
         for (int tp = 0; tp < 4; ++tp) {
-            bk[tp] = DM_FMUL((float)cy[tp], 1.f / (2048.f * 2048.f));
+            bk[tp] = fmul_rn((float)cy[tp], 1.f / (2048.f * 2048.f));
             src[tp] = r.ptmp + ((int64_t)dm_clamp(s - 1 + tp, 0, R - 1) * r.w1 + x) * 3;
         }
         const int body = (3 * r.w1 / CV_LANES) * CV_LANES;     // the row's values in OpenCV's vector body
         for (int c = 0; c < 3; ++c) {
             if (3 * x + c < body) {
-                float acc = DM_FADD(DM_FMUL((float)src[3][c], bk[3]), DM_FMUL((float)src[2][c], bk[2]));
-                acc = DM_FADD(acc, DM_FMUL((float)src[1][c], bk[1]));
-                acc = DM_FADD(acc, DM_FMUL((float)src[0][c], bk[0]));
+                float acc = fadd_rn(fmul_rn((float)src[3][c], bk[3]), fmul_rn((float)src[2][c], bk[2]));
+                acc = fadd_rn(acc, fmul_rn((float)src[1][c], bk[1]));
+                acc = fadd_rn(acc, fmul_rn((float)src[0][c], bk[0]));
                 o[c] = (uint8_t)fminf(fmaxf(rintf(acc), 0.f), 255.f);
             } else {                                            // the scalar tail: fixed point, 2 x 11 fraction bits
                 const int acc = src[0][c] * cy[0] + src[1][c] * cy[1] + src[2][c] * cy[2] + src[3][c] * cy[3];
@@ -380,8 +363,6 @@ namespace migan {
 int demo_resized_size(int w, int h, int max_size, int* ow, int* oh);
 
 namespace {
-
-inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // The descriptors of a pass, with every request's regions carved out of `scratch` (nullptr: sizes only); returns the bytes.
 // eval: the evaluation batch's layout -- the photo goes straight to R x R (one PIL resize, w1 = h1 = R, when it is not

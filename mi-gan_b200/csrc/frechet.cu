@@ -79,11 +79,6 @@ int gemm_launch(const frechet::GemmArgs& a, ck_stream_t) {
     }
     return 0;
 }
-
-int to_host(void* dst, const void* src, size_t bytes, ck_stream_t) {
-    memcpy(dst, src, bytes);
-    return 0;
-}
 #else
 __global__ void __launch_bounds__(kThreads) frechet_pair_kernel(const __grid_constant__ frechet::PairArgs a) {
     extern __shared__ __align__(16) double smem[];
@@ -142,11 +137,6 @@ __global__ void __launch_bounds__(kThreads) frechet_gemm_kernel(const __grid_con
     a.store(b, t, c);
 }
 
-template <class K>
-int set_smem(K kernel, size_t bytes) {
-    return (int)cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
-
 int pair_launch(const frechet::PairArgs& a, int blocks, ck_stream_t s) {
     if (int e = set_smem(frechet_pair_kernel, kPairSmem)) return e;
     frechet_pair_kernel<<<blocks, kThreads, kPairSmem, s>>>(a);
@@ -164,15 +154,9 @@ int gemm_launch(const frechet::GemmArgs& a, ck_stream_t s) {
     frechet_gemm_kernel<<<(unsigned)((a.N / kG) * (a.N / kG)), kThreads, kGemmSmem, s>>>(a);
     return (int)cudaGetLastError();
 }
-
-int to_host(void* dst, const void* src, size_t bytes, ck_stream_t s) {
-    if (cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s)) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-}
 #endif
 
 int padded(int dim) { return (dim + kG - 1) / kG * kG; }
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
 struct Layout {
     size_t A, V, B, W, J, sd, part, scal, total;

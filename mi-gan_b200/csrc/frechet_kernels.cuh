@@ -25,10 +25,7 @@
 
 namespace frechet {
 
-using metrics::dadd;
 using metrics::ddiv;
-using metrics::dmul;
-using metrics::dsub;
 
 constexpr int kB = 32;              // block size of the eigensolver
 constexpr int kG = 2 * kB;          // one pair of blocks: the subproblem and the tile size
@@ -65,8 +62,8 @@ struct MeanCovK {
     const double* shift; const double* sum; const double* sumsq; double* mu; double* sigma; int dim; double n;
     CK_HD void operator()(int64_t i) const {
         const int a = (int)(i / dim), b = (int)(i % dim);
-        sigma[i] = ddiv(dsub(sumsq[i], ddiv(dmul(sum[a], sum[b]), n)), dsub(n, 1.0));
-        if (a == 0) mu[b] = dadd(shift[b], ddiv(sum[b], n));
+        sigma[i] = ddiv(dsub_rn(sumsq[i], ddiv(dmul_rn(sum[a], sum[b]), n)), dsub_rn(n, 1.0));
+        if (a == 0) mu[b] = dadd_rn(shift[b], ddiv(sum[b], n));
     }
 };
 
@@ -76,7 +73,7 @@ struct LoadK {
     CK_HD void operator()(int64_t i) const {
         const int r = (int)(i / N), c = (int)(i % N);
         double v = 0.0;
-        if (r < n && c < n) v = dmul(0.5, dadd(S[(int64_t)r * n + c], S[(int64_t)c * n + r]));
+        if (r < n && c < n) v = dmul_rn(0.5, dadd_rn(S[(int64_t)r * n + c], S[(int64_t)c * n + r]));
         A[i] = v;
         if (V) V[i] = r == c ? 1.0 : 0.0;
     }
@@ -91,7 +88,7 @@ struct LoadK {
 CK_HD double rank_cutoff(const double* A, int dim, int N) {
     double m = 0.0;
     for (int i = 0; i < N; ++i) m = fmax(m, dabs(A[(int64_t)i * N + i]));
-    return dmul(dmul((double)dim, 2.0 * kEps), m);
+    return dmul_rn(dmul_rn((double)dim, 2.0 * kEps), m);
 }
 // cut[0] = rank_cutoff(A).  items = 1.
 struct CutoffK {
@@ -113,7 +110,7 @@ struct ScaleK {
     const double* W; const double* sd; double* M; int N;
     CK_HD void operator()(int64_t e) const {
         const int i = (int)(e / N), j = (int)(e % N);
-        M[e] = dmul(dmul(0.5, dadd(W[e], W[(int64_t)j * N + i])), dmul(sd[i], sd[j]));
+        M[e] = dmul_rn(dmul_rn(0.5, dadd_rn(W[e], W[(int64_t)j * N + i])), dmul_rn(sd[i], sd[j]));
     }
 };
 
@@ -126,7 +123,7 @@ struct ColNormK {
             if (i != j) off = fma(A[(int64_t)i * N + j], A[(int64_t)i * N + j], off);
         const double d = A[j * N + j];
         part[2 * j] = off;
-        part[2 * j + 1] = dmul(d, d);
+        part[2 * j + 1] = dmul_rn(d, d);
     }
 };
 // out[0] = off(A)^2, out[1] = ||A||_F^2, columns in order.  items = 1.
@@ -135,11 +132,11 @@ struct NormSumK {
     CK_HD void operator()(int64_t) const {
         double off = 0.0, diag = 0.0;
         for (int j = 0; j < N; ++j) {
-            off = dadd(off, part[2 * j]);
-            diag = dadd(diag, part[2 * j + 1]);
+            off = dadd_rn(off, part[2 * j]);
+            diag = dadd_rn(diag, part[2 * j + 1]);
         }
         out[0] = off;
-        out[1] = dadd(off, diag);
+        out[1] = dadd_rn(off, diag);
     }
 };
 
@@ -149,14 +146,14 @@ struct ResultK {
     CK_HD void operator()(int64_t) const {
         double dm = 0.0, t1 = 0.0, t2 = 0.0, ts = 0.0;
         for (int i = 0; i < n; ++i) {
-            const double d = dsub(mu1[i], mu2[i]);
+            const double d = dsub_rn(mu1[i], mu2[i]);
             dm = fma(d, d, dm);
-            t1 = dadd(t1, s1[(int64_t)i * n + i]);
-            t2 = dadd(t2, s2[(int64_t)i * n + i]);
+            t1 = dadd_rn(t1, s1[(int64_t)i * n + i]);
+            t2 = dadd_rn(t2, s2[(int64_t)i * n + i]);
         }
         for (int i = 0; i < N; ++i) {
             const double l = A[(int64_t)i * N + i];
-            if (l > 0.0) ts = dadd(ts, dsqrt(l));
+            if (l > 0.0) ts = dadd_rn(ts, dsqrt(l));
         }
         out[0] = dm;
         out[1] = t1;
@@ -237,17 +234,17 @@ struct PairArgs {
         circle(kG, step, t, &i, &j);
         const double aii = S[i * kLd + i], ajj = S[j * kLd + j], aij = S[i * kLd + j];
         double c = 1.0, s = 0.0, tn = 0.0, cm1 = 0.0;
-        const int go = dabs(aij) > dmul(dmul(kEps, dsqrt(dabs(aii))), dsqrt(dabs(ajj)));
+        const int go = dabs(aij) > dmul_rn(dmul_rn(kEps, dsqrt(dabs(aii))), dsqrt(dabs(ajj)));
         if (go) {
             // Golub & Van Loan's sym.schur2: tau = (a_jj - a_ii) / (2 a_ij), t = sign(tau) / (|tau| + sqrt(1 + tau^2))
-            const double tau = ddiv(dsub(ajj, aii), dmul(2.0, aij));
+            const double tau = ddiv(dsub_rn(ajj, aii), dmul_rn(2.0, aij));
             const double at = dabs(tau);
-            tn = at > 1e150 ? ddiv(0.5, at) : ddiv(1.0, dadd(at, dsqrt(fma(at, at, 1.0))));
+            tn = at > 1e150 ? ddiv(0.5, at) : ddiv(1.0, dadd_rn(at, dsqrt(fma(at, at, 1.0))));
             if (tau < 0.0) tn = -tn;
             const double r = dsqrt(fma(tn, tn, 1.0));
             c = ddiv(1.0, r);
-            s = dmul(tn, c);
-            cm1 = -ddiv(dmul(tn, tn), dmul(r, dadd(1.0, r)));   // c - 1 without the cancellation
+            s = dmul_rn(tn, c);
+            cm1 = -ddiv(dmul_rn(tn, tn), dmul_rn(r, dadd_rn(1.0, r)));   // c - 1 without the cancellation
         }
         cs[4 * t] = c;
         cs[4 * t + 1] = s;
@@ -276,11 +273,11 @@ struct PairArgs {
             const double cq = cs[4 * Q], sq = cs[4 * Q + 1];
             const double bik = S[i * kLd + k], bil = S[i * kLd + l], bjk = S[j * kLd + k], bjl = S[j * kLd + l];
             // rows: i' = c i - s j, j' = s i + c j
-            const double tik = fma(cp, bik, -dmul(sp, bjk)), til = fma(cp, bil, -dmul(sp, bjl));
-            const double tjk = fma(sp, bik, dmul(cp, bjk)), tjl = fma(sp, bil, dmul(cp, bjl));
+            const double tik = fma(cp, bik, -dmul_rn(sp, bjk)), til = fma(cp, bil, -dmul_rn(sp, bjl));
+            const double tjk = fma(sp, bik, dmul_rn(cp, bjk)), tjl = fma(sp, bil, dmul_rn(cp, bjl));
             // columns: k' = c k - s l, l' = s k + c l
-            const double nik = fma(cq, tik, -dmul(sq, til)), nil = fma(sq, tik, dmul(cq, til));
-            const double njk = fma(cq, tjk, -dmul(sq, tjl)), njl = fma(sq, tjk, dmul(cq, tjl));
+            const double nik = fma(cq, tik, -dmul_rn(sq, til)), nil = fma(sq, tik, dmul_rn(cq, til));
+            const double njk = fma(cq, tjk, -dmul_rn(sq, tjl)), njl = fma(sq, tjk, dmul_rn(cq, tjl));
             S[i * kLd + k] = S[k * kLd + i] = nik;
             S[i * kLd + l] = S[l * kLd + i] = nil;
             S[j * kLd + k] = S[k * kLd + j] = njk;
@@ -292,9 +289,9 @@ struct PairArgs {
             circle(kG, step, P, &i, &j);
             const double s = cs[4 * P + 1], cm1 = cs[4 * P + 3];
             const double ki = Jl[r * kLd + i], kj = Jl[r * kLd + j];
-            const double ji = dadd(r == i ? 1.0 : 0.0, ki), jj = dadd(r == j ? 1.0 : 0.0, kj);
-            Jl[r * kLd + i] = dadd(ki, fma(cm1, ji, -dmul(s, jj)));
-            Jl[r * kLd + j] = dadd(kj, fma(s, ji, dmul(cm1, jj)));
+            const double ji = dadd_rn(r == i ? 1.0 : 0.0, ki), jj = dadd_rn(r == j ? 1.0 : 0.0, kj);
+            Jl[r * kLd + i] = dadd_rn(ki, fma(cm1, ji, -dmul_rn(s, jj)));
+            Jl[r * kLd + j] = dadd_rn(kj, fma(s, ji, dmul_rn(cm1, jj)));
         }
     }
 

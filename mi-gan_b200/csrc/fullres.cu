@@ -52,7 +52,7 @@ CK_HD int64_t fullres_post_items(const FullResReq& r) { return (int64_t)r.H * r.
 // when Wp % 4 == 0 (always at R >= 16: Wp is a multiple of R / 4), scalar stores otherwise.
 struct FullResPreK {
     const FullResBatch& b;
-    PP_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const FullResReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -95,7 +95,7 @@ struct FullResPreK {
 // outside the window is written.
 struct FullResPostK {
     const FullResBatch& b;
-    PP_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const FullResReq& r = b.r[k];
         const int64_t j = i - b.start[k];

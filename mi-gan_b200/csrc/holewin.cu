@@ -53,7 +53,7 @@ CK_HD CellsBlock cells_block(const CellsBatch& b, int64_t blk) {
 }
 
 // Thread tid of nthr: the 16-byte chunks of the block's rows; flags[c] = 1 when cell cx0 + c holds a hole pixel.
-PP_D void cells_block_scan(const CellsBatch& b, const CellsBlock& g, int tid, int nthr, uint8_t* flags) {
+CK_D void cells_block_scan(const CellsBatch& b, const CellsBlock& g, int tid, int nthr, uint8_t* flags) {
     const CellsReq& r = b.r[g.k];
     const int C = r.C, ch = mask_channel(C);
     const int64_t span = (int64_t)(g.px1 - g.px0) * C;            // bytes of the block's part of a row
@@ -97,7 +97,7 @@ PP_D void cells_block_scan(const CellsBatch& b, const CellsBlock& g, int tid, in
     }
 }
 
-PP_D void cells_block_store(const CellsBatch& b, const CellsBlock& g, int tid, int nthr, const uint8_t* flags,
+CK_D void cells_block_store(const CellsBatch& b, const CellsBlock& g, int tid, int nthr, const uint8_t* flags,
                             uint8_t* cells) {
     const CellsReq& r = b.r[g.k];
     uint8_t* out = cells + b.cell_start[g.k] + (int64_t)g.cy * r.gw + g.cx0;

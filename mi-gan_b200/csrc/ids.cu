@@ -108,11 +108,6 @@ int line_launch(const ids::LineArgs& a, ck_stream_t) {
     a.scal[ids::kStep] = ls.t;
     return 0;
 }
-
-int to_host(void* dst, const void* src, size_t bytes, ck_stream_t) {
-    memcpy(dst, src, bytes);
-    return 0;
-}
 #else
 __global__ void __launch_bounds__(kThreads) ids_gram_kernel(const __grid_constant__ ids::GramArgs a) {
     extern __shared__ __align__(16) double smem[];
@@ -211,11 +206,6 @@ __global__ void __launch_bounds__(kThreads) ids_line_kernel(const __grid_constan
     if (t == 0) a.scal[ids::kStep] = ls.t;
 }
 
-template <class K>
-int set_smem(K kernel, size_t bytes) {
-    return (int)cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
-
 int gram_launch(const ids::GramArgs& a, ck_stream_t s) {
     if (int e = set_smem(ids_gram_kernel, kTileSmem)) return e;
     ids_gram_kernel<<<(unsigned)a.tiles(), kThreads, kTileSmem, s>>>(a);
@@ -250,15 +240,9 @@ int line_launch(const ids::LineArgs& a, ck_stream_t s) {
     ids_line_kernel<<<1, kThreads, kLineSmem, s>>>(a);
     return (int)cudaGetLastError();
 }
-
-int to_host(void* dst, const void* src, size_t bytes, ck_stream_t s) {
-    if (cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s)) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-}
 #endif
 
 int padded(int dim) { return (dim + 1 + kG - 1) / kG * kG; }
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
 struct Layout {
     size_t beta, bbar, g, r, o, ob, idx, part, off, lanes, ps, pt, G, scal, total;

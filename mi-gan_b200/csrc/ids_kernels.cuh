@@ -28,10 +28,7 @@ using frechet::kG;
 using frechet::kLd;
 using frechet::kThreads;
 using frechet::kTileDoubles;
-using metrics::dadd;
 using metrics::ddiv;
-using metrics::dmul;
-using metrics::dsub;
 
 constexpr int kMaxDim = 4096;
 constexpr int kChunk = 256;          // rows per chunk of the row reductions and of the gradient's column sums
@@ -60,7 +57,7 @@ struct Data {
 };
 
 CK_HD int64_t chunks_of(int64_t rows) { return (rows + kChunk - 1) / kChunk; }
-CK_HD bool active(double y, double o) { return dmul(y, o) < 1.0; }
+CK_HD bool active(double y, double o) { return dmul_rn(y, o) < 1.0; }
 
 // b = k (k + 1) / 2 + l, l <= k: the lower tile (k, l).
 CK_HD void lower_tile(int64_t b, int* k, int* l) {
@@ -86,7 +83,7 @@ struct NonFiniteK {
         for (int64_t i = c * kChunk; i < end; ++i)
             for (int k = 0; k < X.d; ++k) {
                 const double v = X.x(i, k);
-                if (!(v - v == 0.0)) bad = dadd(bad, 1.0);
+                if (!(v - v == 0.0)) bad = dadd_rn(bad, 1.0);
             }
         part[c] = bad;
     }
@@ -97,7 +94,7 @@ struct SumK {
     const double* part; double* out; int64_t len;
     CK_HD void operator()(int64_t) const {
         double s = 0.0;
-        for (int64_t c = 0; c < len; ++c) s = dadd(s, part[c]);
+        for (int64_t c = 0; c < len; ++c) s = dadd_rn(s, part[c]);
         out[0] = s;
     }
 };
@@ -109,7 +106,7 @@ struct ActiveCountK {
         double k = 0.0;
         const int64_t end = X.rows() < (c + 1) * kChunk ? X.rows() : (c + 1) * kChunk;
         for (int64_t i = c * kChunk; i < end; ++i)
-            if (active(X.y(i), o[i])) k = dadd(k, 1.0);
+            if (active(X.y(i), o[i])) k = dadd_rn(k, 1.0);
         part[c] = k;
     }
 };
@@ -151,7 +148,7 @@ struct GradPartK {
         for (int64_t k = h * kChunk; k < end; ++k) {
             const int64_t i = idx[k];
             const double x = X.xt(i, c), y = X.y(i);
-            s = fma(x, dsub(y, o[i]), s);
+            s = fma(x, dsub_rn(y, o[i]), s);
             t = fma(x, y, t);
         }
         ps[h * Dp + c] = s;
@@ -166,11 +163,11 @@ struct GradK {
         double s = 0.0, t = 0.0;
         if (c < D)
             for (int64_t h = 0; h < chunks; ++h) {
-                s = dadd(s, ps[h * Dp + c]);
-                t = dadd(t, pt[h * Dp + c]);
+                s = dadd_rn(s, ps[h * Dp + c]);
+                t = dadd_rn(t, pt[h * Dp + c]);
             }
-        g[c] = c < D ? dsub(beta[c], dmul(kTwoC, s)) : 0.0;
-        r[c] = c < D ? dmul(kTwoC, t) : 0.0;
+        g[c] = c < D ? dsub_rn(beta[c], dmul_rn(kTwoC, s)) : 0.0;
+        r[c] = c < D ? dmul_rn(kTwoC, t) : 0.0;
     }
 };
 
@@ -201,8 +198,8 @@ struct MarginK {
     const double* part; const double* beta; double* o; int d;
     CK_HD void operator()(int64_t i) const {
         double s = 0.0;
-        for (int l = 0; l < kLanes; ++l) s = dadd(s, part[i * kLanes + l]);
-        o[i] = dadd(s, beta[d]);
+        for (int l = 0; l < kLanes; ++l) s = dadd_rn(s, part[i * kLanes + l]);
+        o[i] = dadd_rn(s, beta[d]);
     }
 };
 
@@ -213,7 +210,7 @@ struct MismatchK {
         double k = 0.0;
         const int64_t end = X.rows() < (c + 1) * kChunk ? X.rows() : (c + 1) * kChunk;
         for (int64_t i = c * kChunk; i < end; ++i)
-            if (active(X.y(i), o[i]) != active(X.y(i), ob[i])) k = dadd(k, 1.0);
+            if (active(X.y(i), o[i]) != active(X.y(i), ob[i])) k = dadd_rn(k, 1.0);
         part[c] = k;
     }
 };
@@ -222,7 +219,7 @@ struct MismatchK {
 struct StepK {
     double* beta; const double* bbar; const double* scal;
     CK_HD void operator()(int64_t c) const {
-        beta[c] = scal[kMismatch] == 0.0 ? bbar[c] : fma(scal[kStep], dsub(bbar[c], beta[c]), beta[c]);
+        beta[c] = scal[kMismatch] == 0.0 ? bbar[c] : fma(scal[kStep], dsub_rn(bbar[c], beta[c]), beta[c]);
     }
 };
 
@@ -234,10 +231,10 @@ struct ScorePartK {
         double h = 0.0, wrong = 0.0, pairs = 0.0;
         const int64_t end = X.rows() < (c + 1) * kChunk ? X.rows() : (c + 1) * kChunk;
         for (int64_t i = c * kChunk; i < end; ++i) {
-            const double y = X.y(i), m = dsub(1.0, dmul(y, o[i]));
+            const double y = X.y(i), m = dsub_rn(1.0, dmul_rn(y, o[i]));
             if (m > 0.0) h = fma(m, m, h);
-            if (i < X.n ? o[i] <= 0.0 : o[i] > 0.0) wrong = dadd(wrong, 1.0);
-            if (i < X.n && o[i + X.n] > o[i]) pairs = dadd(pairs, 1.0);
+            if (i < X.n ? o[i] <= 0.0 : o[i] > 0.0) wrong = dadd_rn(wrong, 1.0);
+            if (i < X.n && o[i + X.n] > o[i]) pairs = dadd_rn(pairs, 1.0);
         }
         part[3 * c] = h;
         part[3 * c + 1] = wrong;
@@ -252,16 +249,16 @@ struct ScoreK {
     CK_HD void operator()(int64_t) const {
         double h = 0.0, wrong = 0.0, pairs = 0.0, bb = 0.0;
         for (int64_t c = 0; c < chunks; ++c) {
-            h = dadd(h, part[3 * c]);
-            wrong = dadd(wrong, part[3 * c + 1]);
-            pairs = dadd(pairs, part[3 * c + 2]);
+            h = dadd_rn(h, part[3 * c]);
+            wrong = dadd_rn(wrong, part[3 * c + 1]);
+            pairs = dadd_rn(pairs, part[3 * c + 2]);
         }
         for (int c = 0; c <= d; ++c) bb = fma(beta[c], beta[c], bb);
         for (int c = 0; c < d; ++c) coef[c] = beta[c];
         scal[kPairs] = pairs;
         scal[kWrong] = wrong;
         scal[kHinge] = h;
-        scal[kObjective] = dadd(dmul(0.5, bb), h);   // C = 1
+        scal[kObjective] = dadd_rn(dmul_rn(0.5, bb), h);   // C = 1
     }
 };
 
@@ -304,7 +301,7 @@ struct GramArgs {
             for (int h = 0; h < 2; ++h) {
                 const int col = bj * kG + acc_col(t, nt, h);
                 if (col > row) continue;
-                G[(int64_t)row * Dp + col] = dadd(row == col ? 1.0 : 0.0, dmul(kTwoC, c.v[nt][h]));
+                G[(int64_t)row * Dp + col] = dadd_rn(row == col ? 1.0 : 0.0, dmul_rn(kTwoC, c.v[nt][h]));
             }
     }
 };
@@ -448,7 +445,7 @@ struct LineArgs {
     CK_HD void dir_part(int t, double* part) const {
         double bd = 0.0, dd = 0.0;
         for (int c = t; c < Dp; c += kThreads) {
-            const double dc = dsub(bbar[c], beta[c]);
+            const double dc = dsub_rn(bbar[c], beta[c]);
             bd = fma(beta[c], dc, bd);
             dd = fma(dc, dc, dd);
         }
@@ -461,12 +458,12 @@ struct LineArgs {
         double ae = 0.0, ee = 0.0, moved = 0.0;
         for (int64_t i = t; i < X.rows(); i += kThreads) {
             const double y = X.y(i);
-            const double a = dsub(1.0, dmul(y, o[i])), e = dmul(y, dsub(ob[i], o[i]));
-            if (dsub(a, dmul(mid, e)) > 0.0) {
+            const double a = dsub_rn(1.0, dmul_rn(y, o[i])), e = dmul_rn(y, dsub_rn(ob[i], o[i]));
+            if (dsub_rn(a, dmul_rn(mid, e)) > 0.0) {
                 ae = fma(a, e, ae);
                 ee = fma(e, e, ee);
             }
-            if ((dsub(a, dmul(lo, e)) > 0.0) != (dsub(a, dmul(hi, e)) > 0.0)) moved = dadd(moved, 1.0);
+            if ((dsub_rn(a, dmul_rn(lo, e)) > 0.0) != (dsub_rn(a, dmul_rn(hi, e)) > 0.0)) moved = dadd_rn(moved, 1.0);
         }
         part[3 * t] = ae;
         part[3 * t + 1] = ee;
@@ -477,9 +474,9 @@ struct LineArgs {
 CK_HD void sum_parts(const double* part, double s[3]) {
     s[0] = s[1] = s[2] = 0.0;
     for (int t = 0; t < kThreads; ++t) {
-        s[0] = dadd(s[0], part[3 * t]);
-        s[1] = dadd(s[1], part[3 * t + 1]);
-        s[2] = dadd(s[2], part[3 * t + 2]);
+        s[0] = dadd_rn(s[0], part[3 * t]);
+        s[1] = dadd_rn(s[1], part[3 * t + 1]);
+        s[2] = dadd_rn(s[2], part[3 * t + 2]);
     }
 }
 
@@ -499,15 +496,15 @@ struct LineSearch {
         bisect = 0;
         steps = 0;
     }
-    CK_HD double mid() const { return bisect ? dmul(0.5, dadd(lo, hi)) : hi; }
+    CK_HD double mid() const { return bisect ? dmul_rn(0.5, dadd_rn(lo, hi)) : hi; }
     CK_HD double eval_lo() const { return bisect ? lo : hi; }
     // Takes the sums at (eval_lo(), hi, mid()); returns 1 when t is final.
     CK_HD int next(const double s[3]) {
-        const double P = dsub(bd, dmul(kTwoC, s[0])), Q = dadd(dd, dmul(kTwoC, s[1]));
+        const double P = dsub_rn(bd, dmul_rn(kTwoC, s[0])), Q = dadd_rn(dd, dmul_rn(kTwoC, s[1]));
         if (!bisect) {
             if (fma(hi, Q, P) < 0.0 && steps < kMaxBracket) {
                 lo = hi;
-                hi = dmul(2.0, hi);
+                hi = dmul_rn(2.0, hi);
                 ++steps;
                 return 0;
             }

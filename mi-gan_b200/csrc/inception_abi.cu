@@ -311,8 +311,8 @@ int inception_conv2d(const float* x, int n, int H, int W, int cin, const float* 
     const int OH = (H + 2 * ph - kh) / stride + 1, OW = (W + 2 * pw - kw) / stride + 1;
     if (OH < 1 || OW < 1) return fail(MIGAN_ERR_INVALID, "empty convolution output");
     if (c0 < 0 || c0 + cout > ct) return fail(MIGAN_ERR_INVALID, "channels [%d, %d) outside the %d-channel output", c0, c0 + cout, ct);
-    const int KP = incep::pack_kp(kh * kw, cin), NP = incep::round_up(cout, 64);
-    const size_t need = 2 * incep::align_up((size_t)NP * KP * 4, 256);
+    const int KP = incep::pack_kp(kh * kw, cin), NP = round_up(cout, 64);
+    const size_t need = 2 * align_up((size_t)NP * KP * 4, 256);
     if (workspace_needed) *workspace_needed = need;
     if (!workspace) return 0;
     if (!x || !w || !bias || !y) return fail(MIGAN_ERR_INVALID, "null x / w / bias / y");

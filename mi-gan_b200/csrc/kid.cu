@@ -42,11 +42,6 @@ int tile_launch(const kid::TileArgs& a, ck_stream_t) {
     }
     return 0;
 }
-
-int to_device(void* dst, const void* src, size_t bytes, ck_stream_t) {
-    memcpy(dst, src, bytes);
-    return 0;
-}
 #else
 __global__ void __launch_bounds__(kThreads) kid_tile_kernel(const __grid_constant__ kid::TileArgs a) {
     extern __shared__ __align__(16) double smem[];
@@ -71,20 +66,11 @@ __global__ void __launch_bounds__(kThreads) kid_tile_kernel(const __grid_constan
 }
 
 int tile_launch(const kid::TileArgs& a, ck_stream_t s) {
-    if (cudaError_t e = cudaFuncSetAttribute(kid_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)kTileSmem))
-        return (int)e;
+    if (int e = set_smem(kid_tile_kernel, kTileSmem)) return e;
     kid_tile_kernel<<<(unsigned)a.blocks(), kThreads, kTileSmem, s>>>(a);
     return (int)cudaGetLastError();
 }
-
-// A pageable source is staged before the call returns, so the caller may free its tables at once.
-int to_device(void* dst, const void* src, size_t bytes, ck_stream_t s) {
-    return (int)cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s);
-}
 #endif
-
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
 struct Layout {
     size_t fake_idx, real_idx, partials, total;

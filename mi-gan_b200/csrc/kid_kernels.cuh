@@ -30,9 +30,7 @@ using frechet::kG;
 using frechet::kLd;
 using frechet::kThreads;
 using frechet::kTileDoubles;
-using metrics::dadd;
 using metrics::ddiv;
-using metrics::dmul;
 
 constexpr int kMaxDim = 4096;
 constexpr int kLanes = kThreads / 32;             // the reduction's second level: one lane per warp's worth of threads
@@ -119,8 +117,8 @@ struct TileArgs {
             for (int h = 0; h < 2; ++h) {
                 const int j = T.bj * kG + acc_col(t, nt, h);
                 if (i >= m || j >= m || (T.kind != kXY && i == j)) continue;
-                const double u = dadd(ddiv(c.v[nt][h], d), 1.0);
-                sum = dadd(sum, dmul(dmul(u, u), u));
+                const double u = dadd_rn(ddiv(c.v[nt][h], d), 1.0);
+                sum = dadd_rn(sum, dmul_rn(dmul_rn(u, u), u));
             }
         red[t] = sum;
     }
@@ -128,7 +126,7 @@ struct TileArgs {
     CK_HD void combine(int t, double* red) const {
         if (t >= kLanes) return;
         double sum = 0.0;
-        for (int k = 0; k < 32; ++k) sum = dadd(sum, red[32 * t + k]);
+        for (int k = 0; k < 32; ++k) sum = dadd_rn(sum, red[32 * t + k]);
         red[kThreads + t] = sum;
     }
     // partials[s][kind][slot] = the lanes in order, twice for an off-diagonal tile of X X^T or Y Y^T.
@@ -136,8 +134,8 @@ struct TileArgs {
         if (t != 0) return;
         const Tile T = tile(b);
         double sum = 0.0;
-        for (int w = 0; w < kLanes; ++w) sum = dadd(sum, red[kThreads + w]);
-        if (T.kind != kXY && T.bi != T.bj) sum = dmul(2.0, sum);
+        for (int w = 0; w < kLanes; ++w) sum = dadd_rn(sum, red[kThreads + w]);
+        if (T.kind != kXY && T.bi != T.bj) sum = dmul_rn(2.0, sum);
         partials[((int64_t)T.s * kKinds + T.kind) * nb() * nb() + T.slot] = sum;
     }
 };
@@ -149,7 +147,7 @@ struct TermsK {
         const int64_t count = e % kKinds == kXY ? (int64_t)nb * nb : lower_tiles(nb);
         const double* p = partials + e * nb * nb;
         double sum = 0.0;
-        for (int64_t k = 0; k < count; ++k) sum = dadd(sum, p[k]);
+        for (int64_t k = 0; k < count; ++k) sum = dadd_rn(sum, p[k]);
         terms[e] = sum;
     }
 };

@@ -22,7 +22,6 @@ namespace {
 using incep::Act;
 using incep::ConvL;
 using incep::Runner;
-using incep::dev_err;
 using migan::fail;
 
 constexpr int kLayers = LPIPS_LAYERS;
@@ -182,9 +181,9 @@ int pack_weights(lpips_ctx* c) {
         lin.insert(lin.end(), w.begin(), w.end());
     }
     void* d = nullptr;
-    int e = incep::dev_alloc(&d, lin.size() * 4);
-    if (!e) { c->allocs.push_back(d); e = incep::dev_copy(d, lin.data(), lin.size() * 4, nullptr); }
-    if (!e) e = incep::dev_sync();
+    int e = dev_alloc(&d, lin.size() * 4);
+    if (!e) { c->allocs.push_back(d); e = dev_copy(d, lin.data(), lin.size() * 4, nullptr); }
+    if (!e) e = dev_sync();
     if (e) return fail(MIGAN_ERR_CUDA, "uploading the linear layers failed: %s", dev_err(e));
     c->lin = (float*)d;
     return 0;

@@ -9,8 +9,8 @@
 //
 // The brush is Pillow's (12.x) ImageDraw: a polyline of width w is the union of its two-point wide lines; each is a quad
 // filled by Pillow's polygon scanline rule, which is not translation-invariant, so the quad rows are computed at absolute
-// coordinates with Pillow's float32 operations each rounded on its own (PP_MUL / PP_ADD / PP_DIV of prepost.cuh), and the
-// vertex discs are one fixed stamp per radius (kDiscHalf).  The brush is painted at the un-flipped coordinates and each
+// coordinates with Pillow's float32 operations each rounded on its own (fmul_rn / fadd_rn / fdiv_rn of portable.cuh), and
+// the vertex discs are one fixed stamp per radius (kDiscHalf).  The brush is painted at the un-flipped coordinates and each
 // span mirrored into the output, so the flips cost nothing.  oracle/masks_oracle.py states the same rules in numpy.
 // The emulation build (tests/emul/build_emul.py) runs the same block functions with the threads of a block in turn.
 #include "prepost.cuh"
@@ -59,14 +59,14 @@ MK_CONST uint8_t kDiscHalf[18][24] = {
 CK_HD bool mask_accepted(int holes, int h_min, int h_max) { return holes >= h_min && holes <= h_max; }
 
 // Pillow's ROUND_UP / ROUND_DOWN of a float: f + 0.5f / f - 0.5f in float for f >= 0, |f| +- 0.5 in double below.
-PP_D int mk_round_up(float f) { return f >= 0.f ? (int)floorf(PP_ADD(f, 0.5f)) : -(int)floor(fabs((double)f) + 0.5); }
-PP_D int mk_round_down(float f) { return f >= 0.f ? (int)ceilf(PP_ADD(f, -0.5f)) : -(int)ceil(fabs((double)f) - 0.5); }
+CK_D int mk_round_up(float f) { return f >= 0.f ? (int)floorf(fadd_rn(f, 0.5f)) : -(int)floor(fabs((double)f) + 0.5); }
+CK_D int mk_round_down(float f) { return f >= 0.f ? (int)ceilf(fadd_rn(f, -0.5f)) : -(int)ceil(fabs((double)f) - 0.5); }
 
 struct MkEdge { int x0, y0, ymin, ymax; float dx; };
-PP_D float mk_edge_x(const MkEdge& e, int y) { return PP_ADD(PP_MUL((float)(y - e.y0), e.dx), (float)e.x0); }
+CK_D float mk_edge_x(const MkEdge& e, int y) { return fadd_rn(fmul_rn((float)(y - e.y0), e.dx), (float)e.x0); }
 
 // xx[i] = v for a run-time i, with every index constant after unrolling (the list stays in registers).
-PP_D void mk_set(float (&xx)[8], int i, float v) {
+CK_D void mk_set(float (&xx)[8], int i, float v) {
 #pragma unroll
     for (int q = 0; q < 8; ++q)
         if (q == i) xx[q] = v;
@@ -76,7 +76,7 @@ PP_D void mk_set(float (&xx)[8], int i, float v) {
 // inclusive span before clipping (horizontal edges first, then the scanline pairs).  Pillow's edge table holds the
 // non-horizontal edges in order; `rank` is an edge's index there.
 template <class F>
-PP_D void mk_quad_row(const int16_t* q, int s, int y, F&& span) {
+CK_D void mk_quad_row(const int16_t* q, int s, int y, F&& span) {
     MkEdge e[4];
     bool flat[4];
     int ymin = s - 1, ymax = 0;
@@ -88,7 +88,7 @@ PP_D void mk_quad_row(const int16_t* q, int s, int y, F&& span) {
         ymax = hi > ymax ? hi : ymax;
         flat[i] = ya == yb;                                  // drawn as a line, left out of the edge table
         if (flat[i] && y == ya) span(xa < xb ? xa : xb, xa < xb ? xb : xa);
-        e[i] = MkEdge{xa, ya, lo, hi, flat[i] ? 0.f : PP_DIV((float)(xb - xa), (float)(yb - ya))};
+        e[i] = MkEdge{xa, ya, lo, hi, flat[i] ? 0.f : fdiv_rn((float)(xb - xa), (float)(yb - ya))};
     }
     ymin = ymin < 0 ? 0 : ymin;
     ymax = ymax > s ? s : ymax;
@@ -114,8 +114,8 @@ PP_D void mk_quad_row(const int16_t* q, int s, int y, F&& span) {
                     const int off = y == ymax ? -1 : 1;
                     const float a = mk_edge_x(e[i], y + off), b = mk_edge_x(o, y + off);
                     float v;
-                    if (y == e[i].ymax) v = e[i].dx > 0.f ? PP_ADD(fmaxf(a, b), 1.f) : PP_ADD(fminf(a, b), -1.f);
-                    else v = e[i].dx > 0.f ? fminf(a, b) : PP_ADD(fmaxf(a, b), 1.f);
+                    if (y == e[i].ymax) v = e[i].dx > 0.f ? fadd_rn(fmaxf(a, b), 1.f) : fadd_rn(fminf(a, b), -1.f);
+                    else v = e[i].dx > 0.f ? fminf(a, b) : fadd_rn(fmaxf(a, b), 1.f);
                     mk_set(xx, rank, v);                     // Pillow overwrites the entry at the edge's table index
                     done = true;
                 }
@@ -136,7 +136,7 @@ PP_D void mk_quad_row(const int16_t* q, int s, int y, F&& span) {
         if (i < j) span(mk_round_up(xx[i - 1]), mk_round_down(xx[i]));
 }
 
-PP_D void mk_or(uint32_t* w, uint32_t m) {
+CK_D void mk_or(uint32_t* w, uint32_t m) {
 #ifdef MIGAN_EMULATE
     *w |= m;
 #else
@@ -145,7 +145,7 @@ PP_D void mk_or(uint32_t* w, uint32_t m) {
 }
 
 // Sets columns [a, b] (clipped to the canvas; mirrored when flip) of one bit row.
-PP_D void mk_fill(uint32_t* row, int s, int a, int b, bool flip) {
+CK_D void mk_fill(uint32_t* row, int s, int a, int b, bool flip) {
     a = a < 0 ? 0 : a;
     b = b > s - 1 ? s - 1 : b;
     if (a > b) return;
@@ -158,7 +158,7 @@ PP_D void mk_fill(uint32_t* row, int s, int a, int b, bool flip) {
 
 // Thread tid of nthr: every (primitive, row) item of output rows [y0, y0 + rows) of attempt `r`; bits [rows][w32] = 1
 // where a hole is.  Rectangles are at output coordinates; the brush is evaluated on the un-flipped row and mirrored.
-PP_D void mask_band_paint(const migan_mask_record& r, int s, int y0, int rows, int w32, int tid, int nthr, uint32_t* bits) {
+CK_D void mask_band_paint(const migan_mask_record& r, int s, int y0, int rows, int w32, int tid, int nthr, uint32_t* bits) {
     const int nr = r.n_rects, nq = r.n_segments, items = (nr + nq + r.n_discs) * rows;
     const bool flip_cols = (r.flips & 2) != 0;
     for (int i = tid; i < items; i += nthr) {
@@ -187,7 +187,7 @@ PP_D void mask_band_paint(const migan_mask_record& r, int s, int y0, int rows, i
 
 // Thread tid of nthr: the band's bytes (255 known, 0 hole) in 16-column chunks, one 16-byte store each when s % 16 == 0;
 // returns the thread's hole count.
-PP_D int mask_band_store(int s, int y0, int rows, int w32, int tid, int nthr, const uint32_t* bits, uint8_t* out) {
+CK_D int mask_band_store(int s, int y0, int rows, int w32, int tid, int nthr, const uint32_t* bits, uint8_t* out) {
     const int nck = (s + 15) >> 4;
     int holes = 0;
     for (int i = tid; i < rows * nck; i += nthr) {

@@ -21,7 +21,7 @@ using migan::fail;
 #ifdef MIGAN_EMULATE
 double host_tree(double* s) {
     for (int stride = kThreads / 2; stride > 0; stride >>= 1)
-        for (int t = 0; t < stride; ++t) s[t] = metrics::dadd(s[t], s[t + stride]);
+        for (int t = 0; t < stride; ++t) s[t] = dadd_rn(s[t], s[t + stride]);
     return s[0];
 }
 
@@ -55,7 +55,7 @@ int reduce_launch(const metrics::ReduceArgs& a, ck_stream_t) {
         double s[metrics::kWarp];
         for (int l = 0; l < metrics::kWarp; ++l) s[l] = a.lane_sum(i, l);
         for (int off = metrics::kWarp / 2; off > 0; off >>= 1)
-            for (int l = 0; l < off; ++l) s[l] = metrics::dadd(s[l], s[l + off]);
+            for (int l = 0; l < off; ++l) s[l] = dadd_rn(s[l], s[l + off]);
         a.finish_image(i, s[0]);
     }
     a.finish_mean();
@@ -67,7 +67,7 @@ __device__ __forceinline__ void block_tree(double* s, double v, double* out) {
     s[t] = v;
     __syncthreads();
     for (int stride = kThreads / 2; stride > 0; stride >>= 1) {
-        if (t < stride) s[t] = metrics::dadd(s[t], s[t + stride]);
+        if (t < stride) s[t] = dadd_rn(s[t], s[t + stride]);
         __syncthreads();
     }
     if (t == 0) *out = s[0];
@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(kThreads) metrics_reduce_kernel(const __grid_c
     const int lane = threadIdx.x % metrics::kWarp, warp = threadIdx.x / metrics::kWarp;
     for (int64_t i = warp; i < a.n; i += kThreads / metrics::kWarp) {
         double s = a.lane_sum(i, lane);
-        for (int off = metrics::kWarp / 2; off > 0; off >>= 1) s = metrics::dadd(s, __shfl_down_sync(0xffffffffu, s, off));
+        for (int off = metrics::kWarp / 2; off > 0; off >>= 1) s = dadd_rn(s, __shfl_down_sync(0xffffffffu, s, off));
         if (lane == 0) a.finish_image(i, s);
     }
     __syncthreads();   // the per-image sums in global memory are visible to thread 0
@@ -109,8 +109,7 @@ __global__ void __launch_bounds__(kThreads) metrics_reduce_kernel(const __grid_c
 
 int ssim_launch(const metrics::SsimArgs& a, int64_t blocks, ck_stream_t s) {
     const int smem = (int)a.smem_bytes();
-    cudaError_t e = cudaFuncSetAttribute(metrics_ssim_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
+    if (int e = set_smem(metrics_ssim_tile_kernel, smem)) return e;
     metrics_ssim_tile_kernel<<<(unsigned)blocks, kThreads, smem, s>>>(a);
     return (int)cudaGetLastError();
 }

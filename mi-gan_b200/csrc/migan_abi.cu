@@ -33,7 +33,6 @@ using migan::WeightRegistry;
 namespace {
 
 inline int channels(int res) { return std::min(32768 / res, 512); }  // migan_inference.py:222-223
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ---- operand packing of the tensor-core SeparableConv2d kernel (sepconv_tc.h), shared by the weight loader and the
 // single-launch test hook (migan_debug_sepconv_tc) so that a test runs on exactly the tables a forward uses ----

@@ -20,26 +20,14 @@
 // start[]: item i belongs to the request k with start[k] <= i < start[k + 1].  The single-request entry points are the
 // batch of one.  The device-planned form (pipe_plan_kernel) writes the descriptors to the scratch instead, and the same
 // functors read them from shared memory, so a pass needs no host round trip.  Item kernels (comod_kernels.cuh style): the emulation build runs the very same functors on the CPU
-// against the oracle; the hole flags use a shared-memory kernel on the GPU and the per-request HoleFlagsK there.
+// against the oracle; the hole flags use a shared-memory kernel on the GPU and the per-request HoleFlagsK there.  The
+// arithmetic is rounded operation by operation with the *_rn functions of portable.cuh, so both builds agree bit for bit.
 #include "comod_kernels.cuh"
 #include "abi_error.h"
 
 #ifdef MIGAN_EMULATE
-#include <cmath>
-#define PL_MUL(a, b) ((a) * (b))
-#define PL_ADD(a, b) ((a) + (b))
-#define PL_DIV(a, b) ((a) / (b))
-#define PL_FMA(a, b, c) fmaf((a), (b), (c))
-#define PL_RINT(a) rintf(a)
-#define PL_D inline
 #define PL_GLOBAL(p) (p)
 #else
-#define PL_MUL(a, b) __fmul_rn((a), (b))
-#define PL_ADD(a, b) __fadd_rn((a), (b))
-#define PL_DIV(a, b) __fdiv_rn((a), (b))
-#define PL_FMA(a, b, c) __fmaf_rn((a), (b), (c))
-#define PL_RINT(a) rintf(a)
-#define PL_D __device__ __forceinline__
 // The request pointers are global memory.  A planned launch reads them from shared memory, where the compiler cannot see
 // that and would emit generic loads and stores; this says so.
 template <class T>
@@ -50,16 +38,16 @@ __device__ __forceinline__ T* pl_global(T* p) { __builtin_assume(__isGlobal(p));
 namespace comod {
 
 // torch's mode='nearest' source index (ATen/native/UpSample.h nearest_neighbor_compute_source_index)
-PL_D int nearest_src(int dst, int in_size, int out_size) {
+CK_D int nearest_src(int dst, int in_size, int out_size) {
     if (in_size == out_size) return dst;
-    const float scale = PL_DIV((float)in_size, (float)out_size);
-    const int s = (int)floorf(PL_MUL((float)dst, scale));
+    const float scale = fdiv_rn((float)in_size, (float)out_size);
+    const int s = (int)floorf(fmul_rn((float)dst, scale));
     return s < in_size - 1 ? s : in_size - 1;
 }
 
 struct NearestU8K {    // items = oh*ow: one uint8 plane [H][W] -> [oh][ow]
     const uint8_t* in; uint8_t* out; int H, W, oh, ow;
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int y = (int)(i / ow), x = (int)(i - (int64_t)y * ow);
         out[i] = in[(int64_t)nearest_src(y, H, oh) * W + nearest_src(x, W, ow)];
     }
@@ -68,7 +56,7 @@ struct NearestU8K {    // items = oh*ow: one uint8 plane [H][W] -> [oh][ow]
 #ifdef MIGAN_EMULATE   // the GPU build runs hole_flags_batch_kernel (shared memory, warp votes) instead
 struct HoleFlagsK {    // items = W + H: flags[x] = column x contains a value < 255, flags[W + y] likewise for row y  (:144-149)
     const uint8_t* mask; uint8_t* flags; int H, W;
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         uint8_t f = 0;
         if (i < W) { for (int y = 0; y < H && !f; ++y) f = mask[(int64_t)y * W + i] < 255; }
         else { const uint8_t* r = mask + (i - W) * (int64_t)W; for (int x = 0; x < W && !f; ++x) f = r[x] < 255; }
@@ -80,7 +68,6 @@ struct HoleFlagsK {    // items = W + H: flags[x] = column x contains a value < 
 // One axis of the anti-aliased bilinear filter: for output index i the first source index, the tap count and the taps.
 struct AaTable { int* xmin; int* xsize; float* w; int maxk; };
 
-CK_HD size_t pl_align256(size_t b) { return (b + 255) & ~(size_t)255; }
 CK_HD int pl_min(int a, int b) { return a < b ? a : b; }
 CK_HD int pl_max(int a, int b) { return a > b ? a : b; }
 
@@ -115,38 +102,38 @@ CK_HD AaTable aa_table(int* base, int out_size, int maxk) {
     t.maxk = maxk;
     t.xmin = base;
     t.xsize = base + out_size;
-    t.w = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(base) + pl_align256((size_t)out_size * 2 * sizeof(int)));
+    t.w = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(base) + align256((size_t)out_size * 2 * sizeof(int)));
     return t;
 }
 
-PL_D void aa_weights(const AaTable& t, int in_size, int out_size, int64_t i) {    // entry i of the table in_size -> out_size
+CK_D void aa_weights(const AaTable& t, int in_size, int out_size, int64_t i) {    // entry i of the table in_size -> out_size
     float* w = t.w + i * t.maxk;
     if (in_size == out_size) {                          // the reference skips this pass: identity table
         t.xmin[i] = (int)i; t.xsize[i] = 1; w[0] = 1.f;
         for (int j = 1; j < t.maxk; ++j) w[j] = 0.f;
         return;
     }
-    const float scale = PL_DIV((float)in_size, (float)out_size);           // area_pixel_compute_scale<float>
+    const float scale = fdiv_rn((float)in_size, (float)out_size);           // area_pixel_compute_scale<float>
     const bool down = scale >= 1.0f;
     const float support = down ? scale : 1.f;                              // (interp_size * 0.5) * scale, interp_size = 2
     const float invscale = down ? (float)(1.0 / (double)scale) : 1.f;
     const float center = (float)((double)scale * ((double)i + 0.5));
-    int lo = (int)((double)PL_ADD(center, -support) + 0.5);
+    int lo = (int)((double)fadd_rn(center, -support) + 0.5);
     if (lo < 0) lo = 0;
-    int hi = (int)((double)PL_ADD(center, support) + 0.5);
+    int hi = (int)((double)fadd_rn(center, support) + 0.5);
     if (hi > in_size) hi = in_size;
     int n = hi - lo;
     n = n < 0 ? 0 : (n > t.maxk ? t.maxk : n);
     float total = 0.f;
     for (int j = 0; j < n; ++j) {
-        float a = (float)(((double)PL_ADD((float)(j + lo), -center) + 0.5) * (double)invscale);
+        float a = (float)(((double)fadd_rn((float)(j + lo), -center) + 0.5) * (double)invscale);
         a = fabsf(a);
-        const float v = a < 1.0f ? PL_ADD(1.f, -a) : 0.f;                  // aa_filter (triangle)
+        const float v = a < 1.0f ? fadd_rn(1.f, -a) : 0.f;                  // aa_filter (triangle)
         w[j] = v;
-        total = PL_ADD(total, v);
+        total = fadd_rn(total, v);
     }
     if (total != 0.f)
-        for (int j = 0; j < n; ++j) w[j] = PL_DIV(w[j], total);
+        for (int j = 0; j < n; ++j) w[j] = fdiv_rn(w[j], total);
     for (int j = n; j < t.maxk; ++j) w[j] = 0.f;
     t.xmin[i] = lo; t.xsize[i] = n;
 }
@@ -202,7 +189,7 @@ CK_HD int64_t stage_items(int stage, const PipeReq& r, int res) {
 template <int POST>
 struct AaWeightsBatchK {
     const PipeBatch& b;
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -217,12 +204,12 @@ struct AaWeightsBatchK {
 template <int SRC>
 struct ResizeWidthBatchK {
     const PipeBatch& b;
-    PL_D float load(const void* src, int64_t o) const {
+    CK_D float load(const void* src, int64_t o) const {
         if (SRC == 0) return (float)static_cast<const uint8_t*>(src)[o];
-        float g = PL_MUL(PL_ADD(PL_MUL(static_cast<const float*>(src)[o], 0.5f), 0.5f), 255.f);   // ((y * 0.5 + 0.5) * 255)
+        float g = fmul_rn(fadd_rn(fmul_rn(static_cast<const float*>(src)[o], 0.5f), 0.5f), 255.f);   // ((y * 0.5 + 0.5) * 255)
         return fminf(fmaxf(g, 0.f), 255.f);                                                       // .clamp(0, 255)
     }
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -235,8 +222,8 @@ struct ResizeWidthBatchK {
         const int y = (int)(q % rows); const int c = (int)(q / rows);
         const int64_t base = c * plane_stride + (int64_t)y * row_stride + t.xmin[x];
         const float* w = t.w + (int64_t)x * t.maxk;
-        float acc = PL_MUL(load(src, base), w[0]);
-        for (int jj = 1; jj < t.xsize[x]; ++jj) acc = PL_FMA(load(src, base + jj), w[jj], acc);
+        float acc = fmul_rn(load(src, base), w[0]);
+        for (int jj = 1; jj < t.xsize[x]; ++jj) acc = fma_rn(load(src, base + jj), w[jj], acc);
         PL_GLOBAL(r.tmp)[j] = acc;
     }
 };
@@ -245,7 +232,7 @@ struct ResizeWidthBatchK {
 // mask, normalise, x[k] = cat([mask - 0.5, image * mask]).  items per request = res * res
 struct PreprocessBatchK {
     const PipeBatch& b;
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -254,16 +241,16 @@ struct PreprocessBatchK {
         const int64_t plane = (int64_t)res * res;
         float* x = PL_GLOBAL(b.x) + (int64_t)k * 4 * plane;
         const AaTable t = aa_table(PL_GLOBAL(r.th), res, r.kh);
-        const float m = PL_DIV((float)PL_GLOBAL(r.mask)[(int64_t)nearest_src(oy, hc, res) * r.W + nearest_src(ox, r.wc, res)], 255.f);
-        x[j] = PL_ADD(m, -0.5f);
+        const float m = fdiv_rn((float)PL_GLOBAL(r.mask)[(int64_t)nearest_src(oy, hc, res) * r.W + nearest_src(ox, r.wc, res)], 255.f);
+        x[j] = fadd_rn(m, -0.5f);
         const float* w = t.w + (int64_t)oy * t.maxk;
         for (int c = 0; c < 3; ++c) {
             const float* p = PL_GLOBAL(r.tmp) + ((int64_t)c * hc + t.xmin[oy]) * res + ox;
-            float acc = PL_MUL(p[0], w[0]);
-            for (int jj = 1; jj < t.xsize[oy]; ++jj) acc = PL_FMA(p[(int64_t)jj * res], w[jj], acc);
-            const float v = (float)(uint8_t)PL_RINT(acc);                                        // round(), .to(uint8)
-            const float n = PL_ADD(PL_DIV(PL_MUL(v, 2.f), 255.f), -1.f);                         // image * 2 / 255 - 1
-            x[(c + 1) * plane + j] = PL_MUL(n, m);
+            float acc = fmul_rn(p[0], w[0]);
+            for (int jj = 1; jj < t.xsize[oy]; ++jj) acc = fma_rn(p[(int64_t)jj * res], w[jj], acc);
+            const float v = (float)(uint8_t)rintf(acc);                                        // round(), .to(uint8)
+            const float n = fadd_rn(fdiv_rn(fmul_rn(v, 2.f), 255.f), -1.f);                         // image * 2 / 255 - 1
+            x[(c + 1) * plane + j] = fmul_rn(n, m);
         }
     }
 };
@@ -274,7 +261,7 @@ struct PreprocessBatchK {
 // reference, which slices the crop before post-processing.  items per request = hc * wc
 struct FeatherResizeBatchK {
     const PipeBatch& b;
-    PL_D void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int k = find_request(b.start, b.n, i);
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
@@ -301,18 +288,18 @@ struct FeatherResizeBatchK {
                 acc += (double)b.k[(dy + 2) * 5 + (dx + 2)] * (double)mx;
             }
         }
-        const float wgt = PL_DIV((float)acc, 255.f);
-        const float inv = PL_ADD(1.f, -wgt);
+        const float wgt = fdiv_rn((float)acc, 255.f);
+        const float inv = fadd_rn(1.f, -wgt);
         const AaTable t = aa_table(PL_GLOBAL(r.th), hc, r.kh);
         const float* wt = t.w + (int64_t)h * t.maxk;
         const int y0 = t.xmin[h], taps = t.xsize[h];
         const int64_t img_plane = (int64_t)r.H * W;
         for (int c = 0; c < 3; ++c) {
             const float* p = PL_GLOBAL(r.tmp) + ((int64_t)c * b.res + y0) * wc + w;                      // tmp [3][res][wc]
-            float g = PL_MUL(p[0], wt[0]);
-            for (int jj = 1; jj < taps; ++jj) g = PL_FMA(p[(int64_t)jj * wc], wt[jj], g);
+            float g = fmul_rn(p[0], wt[0]);
+            for (int jj = 1; jj < taps; ++jj) g = fma_rn(p[(int64_t)jj * wc], wt[jj], g);
             uint8_t* px = PL_GLOBAL(r.image) + c * img_plane + (int64_t)h * W + w;
-            const float v = PL_ADD(PL_MUL((float)*px, wgt), PL_MUL(g, inv));
+            const float v = fadd_rn(fmul_rn((float)*px, wgt), fmul_rn(g, inv));
             *px = (uint8_t)fminf(fmaxf(v, 0.f), 255.f);
         }
     }
@@ -549,7 +536,6 @@ namespace migan {
 namespace {
 
 using comod::aa_maxk;
-inline size_t align256(size_t b) { return comod::pl_align256(b); }
 inline size_t table_bytes(int in_size, int out_size) {
     return align256((size_t)out_size * 2 * sizeof(int)) + align256((size_t)out_size * aa_maxk(in_size, out_size) * sizeof(float));
 }

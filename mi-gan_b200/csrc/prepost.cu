@@ -16,12 +16,7 @@ namespace comod {
 
 struct PreU8K {        // items = n*H*W
     const uint8_t* img; const uint8_t* mask; float* x; int64_t HW;
-#ifdef MIGAN_EMULATE
-    inline
-#else
-    __device__ __forceinline__
-#endif
-    void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int64_t n = i / HW, p = i - n * HW;
         const float m = mask[i] == 255 ? 1.f : 0.f;                        // mask // 255            (demo.py:60)
         float* xo = x + n * 4 * HW + p;
@@ -32,12 +27,7 @@ struct PreU8K {        // items = n*H*W
 
 struct PostU8K {       // items = n*H*W
     const float* y; const uint8_t* img; const uint8_t* mask; uint8_t* out; int64_t HW;
-#ifdef MIGAN_EMULATE
-    inline
-#else
-    __device__ __forceinline__
-#endif
-    void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int64_t n = i / HW, p = i - n * HW;
         const bool known = mask[i] == 255;
         for (int c = 0; c < 3; ++c)                                         // img*mask + result*(1-mask)  (demo.py:140)
@@ -53,12 +43,7 @@ struct PostU8K {       // items = n*H*W
 // known pixel v into v - 1 after the uint8 truncation (torch's convolution returns exactly 255 there).
 struct FeatherK {      // items = n*H*W
     const float* y; const uint8_t* img; const uint8_t* mask; uint8_t* out; int H, W; float k[25];
-#ifdef MIGAN_EMULATE
-    inline
-#else
-    __device__ __forceinline__
-#endif
-    void operator()(int64_t i) const {
+    CK_D void operator()(int64_t i) const {
         const int64_t HW = (int64_t)H * W;
         const int64_t n = i / HW, p = i - n * HW;
         const int h = (int)(p / W), w = (int)(p - (int64_t)h * W);
@@ -84,13 +69,13 @@ struct FeatherK {      // items = n*H*W
                 acc += (double)k[(dy + 2) * 5 + (dx + 2)] * (double)mx;
             }
         }
-        const float wgt = PP_DIV((float)acc, 255.f);                        // mask / 255                         (:240)
-        const float inv = PP_ADD(1.f, -wgt);
+        const float wgt = fdiv_rn((float)acc, 255.f);                        // mask / 255                         (:240)
+        const float inv = fadd_rn(1.f, -wgt);
         for (int c = 0; c < 3; ++c) {
             const int64_t o = (n * 3 + c) * HW + p;
-            float g = PP_MUL(PP_ADD(PP_MUL(y[o], 0.5f), 0.5f), 255.f);       // ((y * 0.5 + 0.5) * 255)             (:234)
+            float g = fmul_rn(fadd_rn(fmul_rn(y[o], 0.5f), 0.5f), 255.f);       // ((y * 0.5 + 0.5) * 255)             (:234)
             g = fminf(fmaxf(g, 0.f), 255.f);
-            const float v = PP_ADD(PP_MUL((float)img[o], wgt), PP_MUL(g, inv));   // image * mask + out * (1 - mask)   (:241)
+            const float v = fadd_rn(fmul_rn((float)img[o], wgt), fmul_rn(g, inv));   // image * mask + out * (1 - mask)   (:241)
             out[o] = (uint8_t)fminf(fmaxf(v, 0.f), 255.f);                   // .clamp(0, 255).to(uint8)             (:242)
         }
     }

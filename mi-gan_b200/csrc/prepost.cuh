@@ -1,22 +1,10 @@
 // Per-pixel arithmetic of the uint8 request paths (scripts/demo.py:56-66 and :135-142), shared by every kernel that
 // builds the generator's input from a photo or composes its output: PreU8K / PostU8K (prepost.cu), the demo request
 // path (demo_resize.cu) and the full-resolution path (fullres.cu).  One definition, so those kernels agree bit for bit
-// by construction.  Every product of the reference is rounded separately (no FMA contraction) to stay bit-exact with
-// torch; the emulation build (-DMIGAN_EMULATE, -ffp-contract=off) runs the same expressions on the CPU.
+// by construction.  Every product of the reference is rounded separately (the *_rn functions of portable.cuh, no FMA
+// contraction) to stay bit-exact with torch, in the product and the emulation build alike.
 #pragma once
 #include "comod_kernels.cuh"
-
-#ifdef MIGAN_EMULATE
-#define PP_MUL(a, b) ((a) * (b))
-#define PP_ADD(a, b) ((a) + (b))
-#define PP_DIV(a, b) ((a) / (b))
-#define PP_D inline
-#else
-#define PP_MUL(a, b) __fmul_rn((a), (b))
-#define PP_ADD(a, b) __fadd_rn((a), (b))
-#define PP_DIV(a, b) __fdiv_rn((a), (b))
-#define PP_D __device__ __forceinline__
-#endif
 
 namespace comod {
 
@@ -30,14 +18,14 @@ CK_HD bool mask_known(const uint8_t* mask, int64_t W, int C, int invert, int y, 
 }
 
 // x channel 0 from the mask value m = mask // 255 (0 or 1): mask - 0.5                          (demo.py:60, :65)
-PP_D float pre_mask_value(float m) { return PP_ADD(m, -0.5f); }
+CK_D float pre_mask_value(float m) { return fadd_rn(m, -0.5f); }
 // x channel 1 + c from the photo's uint8 value v: (v * 2 / 255 - 1) * mask                      (:61, :65)
-PP_D float pre_img_value(uint8_t v, float m) { return PP_MUL(PP_ADD(PP_DIV(PP_MUL((float)v, 2.f), 255.f), -1.f), m); }
+CK_D float pre_img_value(uint8_t v, float m) { return fmul_rn(fadd_rn(fdiv_rn(fmul_rn((float)v, 2.f), 255.f), -1.f), m); }
 // The generator's output value -> uint8: (y * 0.5 + 0.5).clamp(0, 1) * 255, truncated by .to(uint8)   (:135-136)
-PP_D uint8_t post_u8(float y) {
-    float t = PP_ADD(PP_MUL(y, 0.5f), 0.5f);
+CK_D uint8_t post_u8(float y) {
+    float t = fadd_rn(fmul_rn(y, 0.5f), 0.5f);
     t = fminf(fmaxf(t, 0.f), 1.f);
-    return (uint8_t)PP_MUL(t, 255.f);
+    return (uint8_t)fmul_rn(t, 255.f);
 }
 
 }  // namespace comod

@@ -6,24 +6,10 @@
 // The fp32 operations are the reference's, in its order (sequential adds, true division by (float)sqrt(k), 1 / sqrt(s));
 // the sum of squares is accumulated in fp64 and rounded once, where torch's CPU reduction uses a vectorised fp32 tree --
 // so the result agrees with the reference to a few ulp, not bit for bit (tests: relative error < 1e-6).
-// Item kernel (comod_kernels.cuh style): the emulation build runs the same functor on the CPU.
+// Item kernel (comod_kernels.cuh style), each fp32 operation rounded on its own (portable.cuh): the emulation build runs
+// the same functor on the CPU.
 #include "comod_kernels.cuh"
 #include "abi_error.h"
-
-#ifdef MIGAN_EMULATE
-#include <cmath>
-#define RP_ADD(a, b) ((a) + (b))
-#define RP_MUL(a, b) ((a) * (b))
-#define RP_DIV(a, b) ((a) / (b))
-#define RP_SQRT(a) sqrtf(a)
-#define RP_D inline
-#else
-#define RP_ADD(a, b) __fadd_rn((a), (b))
-#define RP_MUL(a, b) __fmul_rn((a), (b))
-#define RP_DIV(a, b) __fdiv_rn((a), (b))
-#define RP_SQRT(a) __fsqrt_rn(a)
-#define RP_D __device__ __forceinline__
-#endif
 
 namespace comod {
 
@@ -31,17 +17,17 @@ constexpr int kMaxReparam = 16;
 
 struct ReparamFilterK {   // items = cout
     const float* w[kMaxReparam]; int k; int64_t fan; float div; float* out;
-    RP_D float merged(int64_t idx) const {
+    CK_D float merged(int64_t idx) const {
         float v = w[0][idx];
-        for (int j = 1; j < k; ++j) v = RP_ADD(v, w[j][idx]);
-        return k > 1 ? RP_DIV(v, div) : v;
+        for (int j = 1; j < k; ++j) v = fadd_rn(v, w[j][idx]);
+        return k > 1 ? fdiv_rn(v, div) : v;
     }
-    RP_D void operator()(int64_t o) const {
+    CK_D void operator()(int64_t o) const {
         double acc = 0.0;
-        for (int64_t i = 0; i < fan; ++i) { const float v = merged(o * fan + i); acc += (double)RP_MUL(v, v); }
-        const float s = RP_ADD((float)acc, 1e-8f);
-        const float r = RP_DIV(1.f, RP_SQRT(s));
-        for (int64_t i = 0; i < fan; ++i) out[o * fan + i] = RP_MUL(merged(o * fan + i), r);
+        for (int64_t i = 0; i < fan; ++i) { const float v = merged(o * fan + i); acc += (double)fmul_rn(v, v); }
+        const float s = fadd_rn((float)acc, 1e-8f);
+        const float r = fdiv_rn(1.f, fsqrt_rn(s));
+        for (int64_t i = 0; i < fan; ++i) out[o * fan + i] = fmul_rn(merged(o * fan + i), r);
     }
 };
 

@@ -20,17 +20,7 @@
 // A operand (one K block of 64 channels, M = 128 pixel rows): fp16 hi and lo planes, wgmma K-major SWIZZLE_128B:
 //   byte(m, k) = (m >> 3) * 1024 + (m & 7) * 128 + (((k >> 3) ^ (m & 7)) << 4) + (k & 7) * 2
 #pragma once
-#include <stdint.h>
-
-#ifdef MIGAN_EMULATE
-#include <math.h>
-#include <string.h>
-#define SC_DEV static inline
-#else
-#include <cuda_fp16.h>
-#include <cuda_runtime.h>
-#define SC_DEV __device__ __forceinline__
-#endif
+#include "portable.cuh"
 
 namespace migan {
 namespace stages {
@@ -49,65 +39,65 @@ constexpr int kAuxLeft = 4;                    // the windows start at column x0
 struct P2 { float x, y; };
 typedef P2 f2;
 struct alignas(16) f4 { float x, y, z, w; };
-SC_DEV P2 pk(float lo, float hi) { P2 r; r.x = lo; r.y = hi; return r; }
-SC_DEV P2 ffma2(P2 a, P2 b, P2 c) { return pk(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-SC_DEV P2 fmul2(P2 a, P2 b) { return pk(a.x * b.x, a.y * b.y); }
-SC_DEV P2 fadd2(P2 a, P2 b) { return pk(a.x + b.x, a.y + b.y); }
-SC_DEV uint32_t f2_to_h2(float lo, float hi) {
+CK_D P2 pk(float lo, float hi) { P2 r; r.x = lo; r.y = hi; return r; }
+CK_D P2 ffma2(P2 a, P2 b, P2 c) { return pk(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+CK_D P2 fmul2(P2 a, P2 b) { return pk(a.x * b.x, a.y * b.y); }
+CK_D P2 fadd2(P2 a, P2 b) { return pk(a.x + b.x, a.y + b.y); }
+CK_D uint32_t f2_to_h2(float lo, float hi) {
     _Float16 a = (_Float16)lo, b = (_Float16)hi;
     uint16_t ua, ub; memcpy(&ua, &a, 2); memcpy(&ub, &b, 2);
     return (uint32_t)ua | ((uint32_t)ub << 16);
 }
-SC_DEV uint32_t fbits(float v) { uint32_t u; memcpy(&u, &v, 4); return u; }
-SC_DEV float bitsf(uint32_t u) { float v; memcpy(&v, &u, 4); return v; }
-SC_DEV float ldg1(const float* p) { return *p; }
-SC_DEV void st_u2(uint8_t* p, uint32_t a, uint32_t b) { memcpy(p, &a, 4); memcpy(p + 4, &b, 4); }
-SC_DEV float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
+CK_D uint32_t fbits(float v) { uint32_t u; memcpy(&u, &v, 4); return u; }
+CK_D float bitsf(uint32_t u) { float v; memcpy(&v, &u, 4); return v; }
+CK_D float ldg1(const float* p) { return *p; }
+CK_D void st_u2(uint8_t* p, uint32_t a, uint32_t b) { memcpy(p, &a, 4); memcpy(p + 4, &b, 4); }
+CK_D float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 #else
 typedef float2 P2;
 typedef float2 f2;
 typedef float4 f4;
-SC_DEV P2 pk(float lo, float hi) { return make_float2(lo, hi); }
-SC_DEV P2 ffma2(P2 a, P2 b, P2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
-SC_DEV P2 fmul2(P2 a, P2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-SC_DEV P2 fadd2(P2 a, P2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-SC_DEV uint32_t f2_to_h2(float lo, float hi) { __half2 h = __floats2half2_rn(lo, hi); return *reinterpret_cast<uint32_t*>(&h); }
-SC_DEV uint32_t fbits(float v) { return __float_as_uint(v); }
-SC_DEV float bitsf(uint32_t u) { return __uint_as_float(u); }
-SC_DEV float ldg1(const float* p) { return __ldg(p); }
-SC_DEV void st_u2(uint8_t* p, uint32_t a, uint32_t b) { *reinterpret_cast<uint2*>(p) = make_uint2(a, b); }
-SC_DEV float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
+CK_D P2 pk(float lo, float hi) { return make_float2(lo, hi); }
+CK_D P2 ffma2(P2 a, P2 b, P2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+CK_D P2 fmul2(P2 a, P2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+CK_D P2 fadd2(P2 a, P2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+CK_D uint32_t f2_to_h2(float lo, float hi) { __half2 h = __floats2half2_rn(lo, hi); return *reinterpret_cast<uint32_t*>(&h); }
+CK_D uint32_t fbits(float v) { return __float_as_uint(v); }
+CK_D float bitsf(uint32_t u) { return __uint_as_float(u); }
+CK_D float ldg1(const float* p) { return __ldg(p); }
+CK_D void st_u2(uint8_t* p, uint32_t a, uint32_t b) { *reinterpret_cast<uint2*>(p) = make_uint2(a, b); }
+CK_D float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 #endif
-SC_DEV P2 unpk(P2 v) { return v; }
-SC_DEV P2 fsub2(P2 a, P2 b) { return ffma2(b, pk(-1.0f, -1.0f), a); }     // a - b, exact
-SC_DEV P2 p2zero() { return pk(0.0f, 0.0f); }
+CK_D P2 unpk(P2 v) { return v; }
+CK_D P2 fsub2(P2 a, P2 b) { return ffma2(b, pk(-1.0f, -1.0f), a); }     // a - b, exact
+CK_D P2 p2zero() { return pk(0.0f, 0.0f); }
 typedef P2 u64;   // historical name of the packed pair in this file
 
-SC_DEV int imin(int a, int b) { return a < b ? a : b; }
-SC_DEV int imax(int a, int b) { return a > b ? a : b; }
-SC_DEV int iclamp(int v, int lo, int hi) { return imin(imax(v, lo), hi); }
+CK_D int imin(int a, int b) { return a < b ? a : b; }
+CK_D int imax(int a, int b) { return a > b ? a : b; }
+CK_D int iclamp(int v, int lo, int hi) { return imin(imax(v, lo), hi); }
 
 struct F4 { u64 lo, hi; };   // four floats as two packed pairs (the registers of a float4)
-SC_DEV F4 as_f4(const f4 v) { F4 r; r.lo = pk(v.x, v.y); r.hi = pk(v.z, v.w); return r; }
-SC_DEV f4 to_f4(const F4 v) { f4 r; r.x = v.lo.x; r.y = v.lo.y; r.z = v.hi.x; r.w = v.hi.y; return r; }
-SC_DEV void fma4p(F4& acc, const F4 w, const F4 v) { acc.lo = ffma2(w.lo, v.lo, acc.lo); acc.hi = ffma2(w.hi, v.hi, acc.hi); }
-SC_DEV void fma4s(F4& acc, const u64 w2, const F4 v) { acc.lo = ffma2(w2, v.lo, acc.lo); acc.hi = ffma2(w2, v.hi, acc.hi); }
+CK_D F4 as_f4(const f4 v) { F4 r; r.lo = pk(v.x, v.y); r.hi = pk(v.z, v.w); return r; }
+CK_D f4 to_f4(const F4 v) { f4 r; r.x = v.lo.x; r.y = v.lo.y; r.z = v.hi.x; r.w = v.hi.y; return r; }
+CK_D void fma4p(F4& acc, const F4 w, const F4 v) { acc.lo = ffma2(w.lo, v.lo, acc.lo); acc.hi = ffma2(w.hi, v.hi, acc.hi); }
+CK_D void fma4s(F4& acc, const u64 w2, const F4 v) { acc.lo = ffma2(w2, v.lo, acc.lo); acc.hi = ffma2(w2, v.hi, acc.hi); }
 
 // clamp(max(v, 0.2 v), +-lim) on a pair: lrelu_agc with the gain already folded into v (v = gain * pre-activation)
-SC_DEV P2 act_pair(P2 v, float lim) {
+CK_D P2 act_pair(P2 v, float lim) {
     const P2 b = fmul2(v, pk(kAlpha, kAlpha));
     return pk(fminf(fmax3(v.x, b.x, -lim), lim), fminf(fmax3(v.y, b.y, -lim), lim));
 }
 // fp32 pair s (|s| <= 16384) -> fp16x2 hi and lo with hi + lo ~= s to 22 bits.  hi = s with the low 13 mantissa bits
 // cleared (exactly representable in fp16), lo = fp16(s - hi).
-SC_DEV void split_pack2(const P2 s, uint32_t& hi, uint32_t& lo) {
+CK_D void split_pack2(const P2 s, uint32_t& hi, uint32_t& lo) {
     const float hx = bitsf(fbits(s.x) & 0xFFFFE000u), hy = bitsf(fbits(s.y) & 0xFFFFE000u);
     const P2 d = fsub2(s, pk(hx, hy));
     hi = f2_to_h2(hx, hy);
     lo = f2_to_h2(d.x, d.y);
 }
 // byte offset of (row m, 16-byte chunk j of the 128-byte K row) in a SWIZZLE_128B K-major operand plane
-SC_DEV uint32_t a_off(int m, uint32_t j) { return (uint32_t)(m >> 3) * 1024u + (uint32_t)(m & 7) * 128u + ((j ^ (uint32_t)(m & 7)) << 4); }
+CK_D uint32_t a_off(int m, uint32_t j) { return (uint32_t)(m >> 3) * 1024u + (uint32_t)(m & 7) * 128u + ((j ^ (uint32_t)(m & 7)) << 4); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Depthwise 3x3 + bias + lrelu_agc on one 32-channel chunk -> its half of the A operand K block (fp16 hi/lo).
@@ -120,7 +110,7 @@ SC_DEV uint32_t a_off(int m, uint32_t j) { return (uint32_t)(m >> 3) * 1024u + (
 //   g     which 32-channel half of the 64-channel K block this chunk is (0/1);  cg0 = first channel of the chunk
 // ---------------------------------------------------------------------------------------------------------------
 template <int TN, int TH, int TW>
-SC_DEV void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_hi, uint8_t* __restrict__ a_lo,
+CK_D void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_hi, uint8_t* __restrict__ a_lo,
                            const float* __restrict__ w9, const float* __restrict__ bias, int cin, int cg0, int g, int tg) {
     constexpr int NPAIR = TN * TW / 2;                     // column pairs of the tile (8 at 16x8 / 8x8, 16 at 4x4)
     constexpr int RH = 4;                                  // output rows per worker
@@ -191,7 +181,7 @@ SC_DEV void prologue_chunk(const f4* __restrict__ sin, uint8_t* __restrict__ a_h
 // ---------------------------------------------------------------------------------------------------------------
 struct UpTaps { float f[16]; };
 
-SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
+CK_D void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
                         int y0, int x0, int H, int W, int has_noise, int tg) {
     const int cvec = tg & 7;
 #pragma unroll 1
@@ -233,7 +223,7 @@ SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const fl
 }
 
 // The same on a square R x R image.
-SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
+CK_D void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const float* __restrict__ nz, const UpTaps& taps,
                         int y0, int x0, int R, int has_noise, int tg) {
     prestage_up(in, ta, nz, taps, y0, x0, R, R, has_noise, tg);
 }
@@ -246,7 +236,7 @@ SC_DEV void prestage_up(f4* __restrict__ in, const f4* __restrict__ ta, const fl
 // Worker item = (pixel of the 10 x 18 window, channel vector): 1440 items per chunk.
 // ---------------------------------------------------------------------------------------------------------------
 template <bool kBorder>
-SC_DEV void prestage_stem_t(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
+CK_D void prestage_stem_t(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
                             const float* __restrict__ bs, int cg0, int y0, int x0, int H, int W, int tg) {
     const int cvec = tg & 7;
     const int ch = cg0 + cvec * 4;
@@ -281,13 +271,13 @@ SC_DEV void prestage_stem_t(f4* __restrict__ in, const float* __restrict__ xa, c
 }
 // Tiles that touch (or reach past) the image border zero the pixels outside the image; interior tiles (most of them)
 // skip the test.
-SC_DEV void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
+CK_D void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
                           const float* __restrict__ bs, int cg0, int y0, int x0, int H, int W, int tg) {
     if (y0 == 0 || x0 == 0 || y0 + 8 >= H || x0 + 16 >= W) prestage_stem_t<true>(in, xa, ws, bs, cg0, y0, x0, H, W, tg);
     else prestage_stem_t<false>(in, xa, ws, bs, cg0, y0, x0, H, W, tg);
 }
 // The same on a square R x R image.
-SC_DEV void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
+CK_D void prestage_stem(f4* __restrict__ in, const float* __restrict__ xa, const float* __restrict__ ws,
                           const float* __restrict__ bs, int cg0, int y0, int x0, int R, int tg) {
     prestage_stem(in, xa, ws, bs, cg0, y0, x0, R, R, tg);
 }

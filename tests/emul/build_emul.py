@@ -3,9 +3,10 @@
 The sources compile as plain C++ with ``-DMIGAN_EMULATE``: every launch becomes a host loop over the very same kernel
 functors (``comod_kernels.cuh``), block functions run with the threads of a block in turn, and the GEMMs are reference
 loops.  The index math, the resampler and mask arithmetic, the batching, the host planners and the C ABI's argument
-checks are then checked against the oracles on a machine without a GPU.  ``-ffp-contract=off`` keeps every product and
-sum rounded on its own, as the device code's explicit ``__fmul_rn`` / ``__fadd_rn`` do.  The package never loads these
-libraries, and the product library contains no host loop (it is compiled without the macro).
+checks are then checked against the oracles on a machine without a GPU.  ``csrc/portable.cuh`` holds what differs
+between the two builds; ``-ffp-contract=off`` keeps every product and sum of its ``*_rn`` functions rounded on its own,
+as their ``__f*_rn`` / ``__d*_rn`` intrinsics do on the device.  The package never loads these libraries, and the
+product library contains no host loop (it is compiled without the macro).
 
 - ``build()``: the Co-Mod-GAN host runtime and every request path with their ``extern "C"`` entry points and the error
   unit behind ``migan_last_error`` (``tests/test_*_emul.py``).
