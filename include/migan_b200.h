@@ -199,6 +199,31 @@ int b200_pipeline_preprocess_planned(const migan_pipe_request* reqs_host, int n,
 int b200_pipeline_postprocess_planned(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
                                       const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
 
+/* The crop pipeline on decoded photos and raw masks.  The entry points above take image [3][H][W] (MIGAN_LAYOUT_CHW);
+ * the *_layout forms take the layout of every image of the call: MIGAN_LAYOUT_CHW, or MIGAN_LAYOUT_HWC for image
+ * [H][W][3] (a decoder's photo), with the same results bit for bit on the transposed image.  The planned descriptors
+ * carry the layout, so a pass planned by b200_pipeline_plan_batch_layout runs b200_pipeline_preprocess_planned and
+ * b200_pipeline_postprocess_planned as they are.
+ *   b200_pipeline_mask_planes  one launch for 1..MIGAN_PIPE_MAX_BATCH raw masks (masks_host: HOST array): mask u8
+ *                              [hm][wm][channels] as decoded -> out u8 [H][W] (DEVICE), 255 = known, 0 = hole, by
+ *                              create_onnx_pipeline.py's read_mask (:27-45: alpha of LA / RGBA, R of RGB, L; 255 - v if
+ *                              invert; v < 255 -> 0) and the NEAREST resize to H x W (:255), the plane the stages above read */
+#define MIGAN_LAYOUT_CHW 0
+#define MIGAN_LAYOUT_HWC 1
+typedef struct {
+    const uint8_t* mask;   /* DEVICE u8 [hm][wm][channels], channels 1..4 */
+    uint8_t* out;          /* DEVICE u8 [H][W] */
+    int hm, wm, channels, invert;
+    int H, W;
+} migan_raw_mask;
+int b200_pipeline_mask_planes(const migan_raw_mask* masks_host, int n, void* stream);
+int b200_pipeline_preprocess_batch_layout(const migan_pipe_request* reqs_host, int n, int resolution, int layout, float* x_n4rr,
+                                          void* scratch, size_t scratch_bytes, void* stream);
+int b200_pipeline_postprocess_batch_layout(const float* y_n3rr, const migan_pipe_request* reqs_host, int n, int resolution,
+                                           int layout, const float* k25_host, void* scratch, size_t scratch_bytes, void* stream);
+int b200_pipeline_plan_batch_layout(const migan_pipe_request* reqs_host, int n, int resolution, int padding, int layout,
+                                    const uint8_t* flags, int* boxes_dev, void* scratch, size_t scratch_bytes, void* stream);
+
 /* The reference demo's request path at any photo size (scripts/demo.py:26-66, :120-143), for a batch of
  * 1..MIGAN_PIPE_MAX_BATCH requests, one launch per stage:
  *   photo  -> PIL BICUBIC down-scale to at most R (only when W > R or H > R): img_resized, out_w x out_h

@@ -4,6 +4,7 @@ Public surface (mirrors the reference's for this path):
     Generator(resolution)            drop-in for lib.model_zoo.migan_inference.Generator
     ops.upfirdn2d / ops.bias_act ... drop-ins for torch_utils.ops.{upfirdn2d,bias_act,conv2d_resample}
     pipeline.MIGAN_Pipeline          drop-in for scripts/create_onnx_pipeline.py:MIGAN_Pipeline (any-size image + mask -> in-place result)
+    pipeline.CropPipeline            the same crop pipeline on decoded photos [H,W,3] and raw masks of any size
     demo.DemoPipeline                scripts/demo.py's request path at any photo size (PIL / OpenCV resizes on the GPU)
     fullres.FullResPipeline          photos of any size inpainted at their own resolution (reflect padding on the GPU)
     holewin.HoleWindowPipeline       the same, but only on windows around the holes; the rest of the photo is untouched
@@ -25,6 +26,7 @@ Public surface (mirrors the reference's for this path):
     score_results                    python -m migan_b200.score_results: the evaluation protocol over a directory of any
                                      method's result images, sharded over GPUs
     demo (python -m)                 python -m migan_b200.demo: scripts/demo.py's CLI and files, sharded over GPUs
+    crop_results                     python -m migan_b200.crop_results: create_onnx_pipeline.py's sample loop, sharded over GPUs
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)
     parallel.ShardedGenerator        batch sharding over the GPUs of one box + one all-gather of the outputs
     build.build()                    compile the C-ABI library (nvcc, sm_90a)

@@ -21,6 +21,15 @@ class PipeRequest(ctypes.Structure):
     _fields_ = [("image", c_void_p), ("mask", c_void_p), ("H", c_int), ("W", c_int), ("box", c_int * 4)]
 
 
+LAYOUT_CHW, LAYOUT_HWC = 0, 1
+
+
+class RawMask(ctypes.Structure):
+    """migan_raw_mask: one raw mask of b200_pipeline_mask_planes."""
+    _fields_ = [("mask", c_void_p), ("out", c_void_p), ("hm", c_int), ("wm", c_int), ("channels", c_int),
+                ("invert", c_int), ("H", c_int), ("W", c_int)]
+
+
 class DemoRequest(ctypes.Structure):
     """migan_demo_request: one request of the demo request path (b200_demo_*)."""
     _fields_ = [("img", c_void_p), ("H", c_int), ("W", c_int), ("mask", c_void_p), ("Hm", c_int), ("Wm", c_int),
@@ -152,6 +161,10 @@ SYMBOLS = [
     ("b200_pipeline_plan_batch", c_int, [POINTER(PipeRequest), c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_preprocess_planned", c_int, [POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("b200_pipeline_postprocess_planned", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_mask_planes", c_int, [POINTER(RawMask), c_int, c_void_p]),
+    ("b200_pipeline_preprocess_batch_layout", c_int, [POINTER(PipeRequest), c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_postprocess_batch_layout", c_int, [c_void_p, POINTER(PipeRequest), c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("b200_pipeline_plan_batch_layout", c_int, [POINTER(PipeRequest), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("migan_demo_resized_size", c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]),
     ("b200_demo_scratch_bytes", c_size_t, [POINTER(DemoRequest), c_int, c_int]),
     ("b200_demo_preprocess", c_int, [POINTER(DemoRequest), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),

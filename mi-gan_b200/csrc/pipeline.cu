@@ -23,6 +23,7 @@
 // against the oracle; the hole flags use a shared-memory kernel on the GPU and the per-request HoleFlagsK there.  The
 // arithmetic is rounded operation by operation with the *_rn functions of portable.cuh, so both builds agree bit for bit.
 #include "comod_kernels.cuh"
+#include "prepost.cuh"
 #include "abi_error.h"
 
 #ifdef MIGAN_EMULATE
@@ -50,6 +51,28 @@ struct NearestU8K {    // items = oh*ow: one uint8 plane [H][W] -> [oh][ow]
     CK_D void operator()(int64_t i) const {
         const int y = (int)(i / ow), x = (int)(i - (int64_t)y * ow);
         out[i] = in[(int64_t)nearest_src(y, H, oh) * W + nearest_src(x, W, ow)];
+    }
+};
+
+// A raw decoded mask -> the [H][W] plane the crop pipeline reads (255 = known, 0 = hole): create_onnx_pipeline.py's
+// read_mask (:27-45; channel, 255 - v when inverting, v < 255 -> 0) and the NEAREST resize to the image size (:255) in
+// one launch.  The per-pixel map commutes with NEAREST, so the plane is resize(read_mask(m)) whichever runs first.
+// items per request = H * W
+struct MaskBatch {
+    int64_t start[MIGAN_PIPE_MAX_BATCH + 1];
+    migan_raw_mask r[MIGAN_PIPE_MAX_BATCH];
+    int n;
+};
+static_assert(sizeof(MaskBatch) <= 4000, "the mask batch must fit the classic 4 KB kernel parameter space");
+struct MaskPlaneBatchK {
+    const MaskBatch& b;
+    CK_D void operator()(int64_t i) const {
+        const int k = find_request(b.start, b.n, i);
+        const migan_raw_mask& r = b.r[k];
+        const int64_t j = i - b.start[k];
+        const int y = (int)(j / r.W), x = (int)(j - (int64_t)y * r.W);
+        const bool known = mask_known(r.mask, r.wm, r.channels, r.invert, nearest_src(y, r.hm, r.H), nearest_src(x, r.wm, r.W));
+        r.out[j] = known ? 255 : 0;
     }
 };
 
@@ -138,11 +161,14 @@ CK_D void aa_weights(const AaTable& t, int in_size, int out_size, int64_t i) {  
     t.xmin[i] = lo; t.xsize[i] = n;
 }
 
-// One request of a batched launch.  image / mask point at the crop origin (row stride W, plane stride H*W); tw / th are
-// the width / height tables (aa_table layout) and tmp the width pass's output, all in the caller's scratch.
+// One request of a batched launch.  image / mask point at the crop origin; the mask has row stride W, and image pixel
+// (c, y, x) lies at c * cs + (y * W + x) * ps: (ps, cs) = (1, H*W) for a [3][H][W] image, (3, 1) for [H][W][3]
+// (image_strides).  tw / th are the width / height tables (aa_table layout) and tmp the width pass's output, all in the
+// caller's scratch.
 struct PipeReq {
     uint8_t* image; const uint8_t* mask; float* tmp; int* tw; int* th;
-    int H, W, hc, wc, kw, kh;
+    int64_t cs;
+    int H, W, hc, wc, kw, kh, ps;
 };
 struct PipeBatch {
     int64_t start[MIGAN_PIPE_MAX_BATCH + 1];   // item prefix of the launch
@@ -153,15 +179,21 @@ struct PipeBatch {
 };
 static_assert(sizeof(PipeBatch) <= 4000, "the batch descriptor must fit the classic 4 KB kernel parameter space");
 
-// Request `image` / `mask` ([3][H][W] / [H][W]) cropped to box for one phase: the crop-origin pointers, the crop size and
-// the tap counts of the two axis tables.  tw / th / tmp are wherever the caller carved them.
-CK_HD PipeReq crop_request(uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, bool post,
-                           int* tw, int* th, float* tmp) {
+// Pixel and channel strides of an H x W image in either layout (MIGAN_LAYOUT_CHW / _HWC).
+CK_HD void image_strides(int layout, int H, int W, int& ps, int64_t& cs) {
+    if (layout == MIGAN_LAYOUT_HWC) { ps = 3; cs = 1; }
+    else { ps = 1; cs = (int64_t)H * W; }
+}
+
+// Request `image` / `mask` (strides ps / cs, [H][W]) cropped to box for one phase: the crop-origin pointers, the crop
+// size and the tap counts of the two axis tables.  tw / th / tmp are wherever the caller carved them.
+CK_HD PipeReq crop_request(uint8_t* image, const uint8_t* mask, int H, int W, int ps, int64_t cs, const int* box, int res,
+                           bool post, int* tw, int* th, float* tmp) {
     PipeReq r;
     const int x0 = box[0], y0 = box[2];
-    r.H = H; r.W = W;
+    r.H = H; r.W = W; r.ps = ps; r.cs = cs;
     r.wc = box[1] - x0; r.hc = box[3] - y0;
-    r.image = image + (int64_t)y0 * W + x0;
+    r.image = image + ((int64_t)y0 * W + x0) * ps;
     r.mask = mask + (int64_t)y0 * W + x0;
     r.kw = post ? aa_maxk(res, r.wc) : aa_maxk(r.wc, res);
     r.kh = post ? aa_maxk(res, r.hc) : aa_maxk(r.hc, res);
@@ -199,8 +231,8 @@ struct AaWeightsBatchK {
     }
 };
 
-// Width pass.  SRC = 0: uint8 planes of the image crop -> tmp [3][hc][res]; SRC = 1: generator output y mapped to [0, 255]
-// on load (:239) -> tmp [3][res][wc].  items per request = 3 * rows * ow
+// Width pass.  SRC = 0: uint8 image crop (either layout) -> tmp [3][hc][res]; SRC = 1: generator output y mapped to
+// [0, 255] on load (:239) -> tmp [3][res][wc].  items per request = 3 * rows * ow
 template <int SRC>
 struct ResizeWidthBatchK {
     const PipeBatch& b;
@@ -214,16 +246,17 @@ struct ResizeWidthBatchK {
         const PipeReq& r = b.r[k];
         const int64_t j = i - b.start[k];
         const int ow = SRC ? r.wc : b.res, rows = SRC ? b.res : r.hc;
-        const int64_t plane_stride = SRC ? (int64_t)b.res * b.res : (int64_t)r.H * r.W;
-        const int row_stride = SRC ? b.res : r.W;
+        const int64_t plane_stride = SRC ? (int64_t)b.res * b.res : r.cs;
+        const int64_t ps = SRC ? 1 : r.ps;
+        const int64_t row_stride = SRC ? (int64_t)b.res : (int64_t)r.W * r.ps;
         const void* src = SRC ? static_cast<const void*>(PL_GLOBAL(b.y) + (int64_t)k * 3 * b.res * b.res) : static_cast<const void*>(PL_GLOBAL(r.image));
         const AaTable t = aa_table(PL_GLOBAL(r.tw), ow, r.kw);
         const int x = (int)(j % ow); const int64_t q = j / ow;
         const int y = (int)(q % rows); const int c = (int)(q / rows);
-        const int64_t base = c * plane_stride + (int64_t)y * row_stride + t.xmin[x];
+        const int64_t base = c * plane_stride + (int64_t)y * row_stride + t.xmin[x] * ps;
         const float* w = t.w + (int64_t)x * t.maxk;
         float acc = fmul_rn(load(src, base), w[0]);
-        for (int jj = 1; jj < t.xsize[x]; ++jj) acc = fma_rn(load(src, base + jj), w[jj], acc);
+        for (int jj = 1; jj < t.xsize[x]; ++jj) acc = fma_rn(load(src, base + jj * ps), w[jj], acc);
         PL_GLOBAL(r.tmp)[j] = acc;
     }
 };
@@ -293,12 +326,12 @@ struct FeatherResizeBatchK {
         const AaTable t = aa_table(PL_GLOBAL(r.th), hc, r.kh);
         const float* wt = t.w + (int64_t)h * t.maxk;
         const int y0 = t.xmin[h], taps = t.xsize[h];
-        const int64_t img_plane = (int64_t)r.H * W;
+        uint8_t* const pix = PL_GLOBAL(r.image) + ((int64_t)h * W + w) * r.ps;
         for (int c = 0; c < 3; ++c) {
             const float* p = PL_GLOBAL(r.tmp) + ((int64_t)c * b.res + y0) * wc + w;                      // tmp [3][res][wc]
             float g = fmul_rn(p[0], wt[0]);
             for (int jj = 1; jj < taps; ++jj) g = fma_rn(p[(int64_t)jj * wc], wt[jj], g);
-            uint8_t* px = PL_GLOBAL(r.image) + c * img_plane + (int64_t)h * W + w;
+            uint8_t* px = pix + c * r.cs;
             const float v = fadd_rn(fmul_rn((float)*px, wgt), fmul_rn(g, inv));
             *px = (uint8_t)fminf(fmaxf(v, 0.f), 255.f);
         }
@@ -315,7 +348,8 @@ struct FeatherResizeBatchK {
 struct PlanReq { uint8_t* image; const uint8_t* mask; int64_t foff; int H, W; int* tw[2]; int* th[2]; float* tmp[2]; };
 // What the planning step writes at the start of the scratch.
 struct PipePlan { PipeBatch b[2]; int64_t start[ST_COUNT][MIGAN_PIPE_MAX_BATCH + 1]; };
-struct PlanArgs { PlanReq q[MIGAN_PIPE_MAX_BATCH]; PipePlan* plan; int* boxes; const uint8_t* flags; int n, res, padding; };
+// layout: MIGAN_LAYOUT_CHW or _HWC, for every image of the batch.
+struct PlanArgs { PlanReq q[MIGAN_PIPE_MAX_BATCH]; PipePlan* plan; int* boxes; const uint8_t* flags; int n, res, padding, layout; };
 static_assert(sizeof(PlanArgs) <= 4000, "the planning arguments must fit the classic 4 KB kernel parameter space");
 // One launch of a planned batch: its phase's descriptor and item prefix in device memory, and what is known only when the
 // launch is enqueued (the model input x, the model output y, the feather taps).
@@ -327,8 +361,10 @@ CK_HD void plan_request(const PlanArgs& a, int k, int x_min, int x_max, int y_mi
     int box[4];
     crop_box_from_extent(x_min, x_max, y_min, y_max, q.H, q.W, a.res, a.padding, box);
     for (int i = 0; i < 4; ++i) a.boxes[4 * k + i] = box[i];
+    int ps; int64_t cs;
+    image_strides(a.layout, q.H, q.W, ps, cs);
     for (int p = 0; p < 2; ++p)
-        a.plan->b[p].r[k] = crop_request(q.image, q.mask, q.H, q.W, box, a.res, p == 1, q.tw[p], q.th[p], q.tmp[p]);
+        a.plan->b[p].r[k] = crop_request(q.image, q.mask, q.H, q.W, ps, cs, box, a.res, p == 1, q.tw[p], q.th[p], q.tmp[p]);
 }
 
 // Item prefix of one stage, once every request is planned; the sizes of both descriptors.
@@ -442,8 +478,9 @@ __device__ __forceinline__ void warp_flags_extent(const uint8_t* p, int len, int
 }
 
 // One CTA, one warp per request: the request's column and row extents from its flags, then lane 0 plans the request.
-// Once every request is planned, threads 0..5 write the six item prefixes.
-__global__ void __launch_bounds__(32 * MIGAN_PIPE_MAX_BATCH) pipe_plan_kernel(const __grid_constant__ PlanArgs a) {
+// Once every request is planned, threads 0..5 write the six item prefixes.  The launch is one CTA, so it asks for one
+// resident CTA and not the two per SM that would cap it at 32 registers (and spill the image strides to the stack).
+__global__ void __launch_bounds__(32 * MIGAN_PIPE_MAX_BATCH, 1) pipe_plan_kernel(const __grid_constant__ PlanArgs a) {
     const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (k < a.n) {
         const PlanReq& q = a.q[k];
@@ -548,13 +585,15 @@ inline size_t post_bytes(int hc, int wc, int res) {   // res -> crop: tmp [3][re
 }
 
 // Descriptors of the whole batch for one phase, carved out of `scratch` request after request.
-comod::PipeBatch plan_batch(const migan_pipe_request* q, int n, int res, bool post, void* scratch) {
+comod::PipeBatch plan_batch(const migan_pipe_request* q, int n, int res, int layout, bool post, void* scratch) {
     comod::PipeBatch b = {};
     b.n = n; b.res = res;
     unsigned char* p = static_cast<unsigned char*>(scratch);
     for (int k = 0; k < n; ++k) {
         comod::PipeReq& r = b.r[k];
-        r = comod::crop_request(q[k].image, q[k].mask, q[k].H, q[k].W, q[k].box, res, post, nullptr, nullptr, nullptr);
+        int ps; int64_t cs;
+        comod::image_strides(layout, q[k].H, q[k].W, ps, cs);
+        r = comod::crop_request(q[k].image, q[k].mask, q[k].H, q[k].W, ps, cs, q[k].box, res, post, nullptr, nullptr, nullptr);
         const int ow = post ? r.wc : res, oh = post ? r.hc : res;
         r.tw = reinterpret_cast<int*>(p);
         p += align256((size_t)ow * 2 * sizeof(int)) + align256((size_t)ow * r.kw * sizeof(float));
@@ -611,14 +650,14 @@ struct PlannedLayout {
     int64_t items[comod::ST_COUNT];
     size_t bytes;
 };
-void planned_layout(const migan_pipe_request* q, int n, int res, void* scratch, PlannedLayout& L) {
+void planned_layout(const migan_pipe_request* q, int n, int res, int layout, void* scratch, PlannedLayout& L) {
     const uintptr_t base = reinterpret_cast<uintptr_t>(scratch);
     const size_t data = align256(sizeof(comod::PipePlan));
     size_t off[2] = {data, data};
     int64_t foff = 0;
     L.a = {};
     L.a.plan = reinterpret_cast<comod::PipePlan*>(base);
-    L.a.n = n; L.a.res = res;
+    L.a.n = n; L.a.res = res; L.a.layout = layout;
     for (int st = 0; st < comod::ST_COUNT; ++st) L.items[st] = 0;
     for (int k = 0; k < n; ++k) {
         comod::PlanReq& r = L.a.q[k];
@@ -632,7 +671,7 @@ void planned_layout(const migan_pipe_request* q, int n, int res, void* scratch, 
             r.tmp[p] = reinterpret_cast<float*>(base + off[p]); off[p] += b[3 * p + 2];
         }
         const int whole[4] = {0, r.W, 0, r.H};
-        const comod::PipeReq w = comod::crop_request(r.image, r.mask, r.H, r.W, whole, res, false, nullptr, nullptr, nullptr);
+        const comod::PipeReq w = comod::crop_request(r.image, r.mask, r.H, r.W, 1, 0, whole, res, false, nullptr, nullptr, nullptr);
         for (int st = 0; st < comod::ST_COUNT; ++st) L.items[st] += comod::stage_items(st, w, res);
     }
     L.bytes = off[0] > off[1] ? off[0] : off[1];
@@ -660,6 +699,11 @@ size_t pipeline_batch_scratch_bytes(const migan_pipe_request* q, int n, int res)
     return pre > post ? pre : post;
 }
 
+int check_layout(const char* who, int layout) {
+    if (layout != MIGAN_LAYOUT_CHW && layout != MIGAN_LAYOUT_HWC) return fail(MIGAN_ERR_INVALID, "%s: bad image layout %d", who, layout);
+    return MIGAN_OK;
+}
+
 int check_pipe_batch(const char* who, const migan_pipe_request* q, int n, int res, bool boxes) {
     if (int rc = check_batch_size(who, q, n)) return rc;
     if (res < 1) return fail(MIGAN_ERR_INVALID, "%s: bad resolution %d", who, res);
@@ -678,6 +722,29 @@ int check_pipe_batch(const char* who, const migan_pipe_request* q, int n, int re
 int launch_resize_nearest_u8(const uint8_t* in, int H, int W, uint8_t* out, int oh, int ow, ck_stream_t s) {
     comod::NearestU8K k{in, out, H, W, oh, ow};
     return (int)comod::ck_launch(k, (int64_t)oh * ow, s);
+}
+
+int check_raw_masks(const char* who, const migan_raw_mask* m, int n) {
+    if (int rc = check_batch_size(who, m, n)) return rc;
+    for (int k = 0; k < n; ++k) {
+        const migan_raw_mask& r = m[k];
+        if (!r.mask || !r.out) return fail(MIGAN_ERR_INVALID, "%s: request %d: null mask or output", who, k);
+        if (r.hm < 1 || r.wm < 1 || r.H < 1 || r.W < 1)
+            return fail(MIGAN_ERR_INVALID, "%s: request %d: bad size %d x %d -> %d x %d", who, k, r.hm, r.wm, r.H, r.W);
+        if (int rc = check_mask_channels(who, k, r.channels)) return rc;
+    }
+    return MIGAN_OK;
+}
+
+int launch_mask_planes(const migan_raw_mask* m, int n, ck_stream_t s) {
+    comod::MaskBatch b = {};
+    b.n = n;
+    for (int k = 0; k < n; ++k) {
+        b.r[k] = m[k];
+        b.r[k].invert = m[k].invert != 0;
+        b.start[k + 1] = b.start[k] + (int64_t)m[k].H * m[k].W;
+    }
+    return (int)comod::batch_launch<comod::MaskPlaneBatchK>(b, s);
 }
 
 int launch_hole_flags_batch(const migan_pipe_request* q, int n, uint8_t* flags, ck_stream_t s) {
@@ -719,8 +786,9 @@ void crop_box_from_flags(const uint8_t* flags, int H, int W, int res, int paddin
 }
 
 // Three launches for the whole batch: both tables of every request, the width pass, the height pass fused into x.
-int launch_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res, float* x, void* scratch, ck_stream_t s) {
-    comod::PipeBatch b = plan_batch(q, n, res, false, scratch);
+int launch_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res, int layout, float* x, void* scratch,
+                                     ck_stream_t s) {
+    comod::PipeBatch b = plan_batch(q, n, res, layout, false, scratch);
     b.x = x;
     int e;
     comod::set_items(b, comod::ST_AA_PRE, comod::stage_items);
@@ -732,9 +800,9 @@ int launch_pipeline_preprocess_batch(const migan_pipe_request* q, int n, int res
 }
 
 // Three launches for the whole batch: both tables of every request, the width pass, the height pass fused into the blend.
-int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* q, int n, int res, const float* k25_host,
-                                      void* scratch, ck_stream_t s) {
-    comod::PipeBatch b = plan_batch(q, n, res, true, scratch);
+int launch_pipeline_postprocess_batch(const float* y, const migan_pipe_request* q, int n, int res, int layout,
+                                      const float* k25_host, void* scratch, ck_stream_t s) {
+    comod::PipeBatch b = plan_batch(q, n, res, layout, true, scratch);
     b.y = y;
     for (int i = 0; i < 25; ++i) b.k[i] = k25_host[i];
     int e;
@@ -755,15 +823,16 @@ int check_pipe_planned(const char* who, const migan_pipe_request* q, int n, int 
 
 size_t pipeline_batch_scratch_bound(const migan_pipe_request* q, int n, int res) {
     PlannedLayout L;
-    planned_layout(q, n, res, nullptr, L);
+    planned_layout(q, n, res, MIGAN_LAYOUT_CHW, nullptr, L);
     return L.bytes;
 }
 
-// One launch: every request's crop window from the flags, both phases' descriptors and the six item prefixes.
-int launch_pipeline_plan_batch(const migan_pipe_request* q, int n, int res, int padding, const uint8_t* flags, int* boxes,
-                               void* scratch, ck_stream_t s) {
+// One launch: every request's crop window from the flags, both phases' descriptors and the six item prefixes.  The
+// descriptors carry the image layout, so the planned pre- and post-processing take none.
+int launch_pipeline_plan_batch(const migan_pipe_request* q, int n, int res, int padding, int layout, const uint8_t* flags,
+                               int* boxes, void* scratch, ck_stream_t s) {
     PlannedLayout L;
-    planned_layout(q, n, res, scratch, L);
+    planned_layout(q, n, res, layout, scratch, L);
     L.a.flags = flags; L.a.boxes = boxes; L.a.padding = padding;
     return (int)comod::pipe_plan(L.a, s);
 }
@@ -771,7 +840,7 @@ int launch_pipeline_plan_batch(const migan_pipe_request* q, int n, int res, int 
 // The launches of launch_pipeline_preprocess_batch on the planned descriptors.
 int launch_pipeline_preprocess_planned(const migan_pipe_request* q, int n, int res, float* x, void* scratch, ck_stream_t s) {
     PlannedLayout L;
-    planned_layout(q, n, res, scratch, L);
+    planned_layout(q, n, res, MIGAN_LAYOUT_CHW, scratch, L);      // the layout is in the planned descriptors
     comod::PlannedLaunch a = {};
     a.desc = &L.a.plan->b[0]; a.x = x;
     int e;
@@ -787,7 +856,7 @@ int launch_pipeline_preprocess_planned(const migan_pipe_request* q, int n, int r
 int launch_pipeline_postprocess_planned(const float* y, const migan_pipe_request* q, int n, int res, const float* k25_host,
                                         void* scratch, ck_stream_t s) {
     PlannedLayout L;
-    planned_layout(q, n, res, scratch, L);
+    planned_layout(q, n, res, MIGAN_LAYOUT_CHW, scratch, L);      // the layout is in the planned descriptors
     comod::PlannedLaunch a = {};
     a.desc = &L.a.plan->b[1]; a.y = y;
     for (int i = 0; i < 25; ++i) a.k[i] = k25_host[i];
@@ -803,13 +872,13 @@ int launch_pipeline_postprocess_planned(const float* y, const migan_pipe_request
 int launch_pipeline_preprocess(const uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res, float* x,
                                void* scratch, ck_stream_t s) {
     const migan_pipe_request q = one_request(image, mask, H, W, box);
-    return launch_pipeline_preprocess_batch(&q, 1, res, x, scratch, s);
+    return launch_pipeline_preprocess_batch(&q, 1, res, MIGAN_LAYOUT_CHW, x, scratch, s);
 }
 
 int launch_pipeline_postprocess(const float* y, uint8_t* image, const uint8_t* mask, int H, int W, const int* box, int res,
                                 const float* k25_host, void* scratch, ck_stream_t s) {
     const migan_pipe_request q = one_request(image, mask, H, W, box);
-    return launch_pipeline_postprocess_batch(y, &q, 1, res, k25_host, scratch, s);
+    return launch_pipeline_postprocess_batch(y, &q, 1, res, MIGAN_LAYOUT_CHW, k25_host, scratch, s);
 }
 
 }  // namespace migan
@@ -893,7 +962,7 @@ int b200_pipeline_preprocess_batch(const migan_pipe_request* reqs, int n, int re
     if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_batch: null argument");
     const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY(migan::launch_pipeline_preprocess_batch(reqs, n, res, x, scratch, static_cast<ck_stream_t>(stream)));
+    CUDA_TRY(migan::launch_pipeline_preprocess_batch(reqs, n, res, MIGAN_LAYOUT_CHW, x, scratch, static_cast<ck_stream_t>(stream)));
     return MIGAN_OK;
 }
 
@@ -903,7 +972,7 @@ int b200_pipeline_postprocess_batch(const float* y, const migan_pipe_request* re
     if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_batch: null argument");
     const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY(migan::launch_pipeline_postprocess_batch(y, reqs, n, res, k25, scratch, static_cast<ck_stream_t>(stream)));
+    CUDA_TRY(migan::launch_pipeline_postprocess_batch(y, reqs, n, res, MIGAN_LAYOUT_CHW, k25, scratch, static_cast<ck_stream_t>(stream)));
     return MIGAN_OK;
 }
 
@@ -919,7 +988,7 @@ int b200_pipeline_plan_batch(const migan_pipe_request* reqs, int n, int res, int
     if (!flags || !boxes || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch: null argument");
     const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_plan_batch: scratch of %zu bytes, need %zu", scratch_bytes, need);
-    CUDA_TRY(migan::launch_pipeline_plan_batch(reqs, n, res, padding, flags, boxes, scratch, static_cast<ck_stream_t>(stream)));
+    CUDA_TRY(migan::launch_pipeline_plan_batch(reqs, n, res, padding, MIGAN_LAYOUT_CHW, flags, boxes, scratch, static_cast<ck_stream_t>(stream)));
     return MIGAN_OK;
 }
 
@@ -940,6 +1009,47 @@ int b200_pipeline_postprocess_planned(const float* y, const migan_pipe_request* 
     const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
     if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_planned: scratch of %zu bytes, need %zu", scratch_bytes, need);
     CUDA_TRY(migan::launch_pipeline_postprocess_planned(y, reqs, n, res, k25, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+// ---- images in either layout, raw masks ----
+int b200_pipeline_mask_planes(const migan_raw_mask* masks, int n, void* stream) {
+    if (int rc = migan::check_raw_masks("pipeline_mask_planes", masks, n)) return rc;
+    CUDA_TRY(migan::launch_mask_planes(masks, n, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_preprocess_batch_layout(const migan_pipe_request* reqs, int n, int res, int layout, float* x, void* scratch,
+                                          size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_layout("pipeline_preprocess_batch_layout", layout)) return rc;
+    if (int rc = migan::check_pipe_batch("pipeline_preprocess_batch_layout", reqs, n, res, true)) return rc;
+    if (!x || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_preprocess_batch_layout: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_preprocess_batch_layout: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_preprocess_batch(reqs, n, res, layout, x, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_postprocess_batch_layout(const float* y, const migan_pipe_request* reqs, int n, int res, int layout,
+                                           const float* k25, void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_layout("pipeline_postprocess_batch_layout", layout)) return rc;
+    if (int rc = migan::check_pipe_batch("pipeline_postprocess_batch_layout", reqs, n, res, true)) return rc;
+    if (!y || !k25 || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_postprocess_batch_layout: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bytes(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_postprocess_batch_layout: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_postprocess_batch(y, reqs, n, res, layout, k25, scratch, static_cast<ck_stream_t>(stream)));
+    return MIGAN_OK;
+}
+
+int b200_pipeline_plan_batch_layout(const migan_pipe_request* reqs, int n, int res, int padding, int layout, const uint8_t* flags,
+                                    int* boxes, void* scratch, size_t scratch_bytes, void* stream) {
+    if (int rc = migan::check_layout("pipeline_plan_batch_layout", layout)) return rc;
+    if (int rc = migan::check_pipe_planned("pipeline_plan_batch_layout", reqs, n, res)) return rc;
+    if (padding < 0) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch_layout: padding %d", padding);
+    if (!flags || !boxes || !scratch) return fail(MIGAN_ERR_INVALID, "pipeline_plan_batch_layout: null argument");
+    const size_t need = migan::pipeline_batch_scratch_bound(reqs, n, res);
+    if (scratch_bytes < need) return fail(MIGAN_ERR_WORKSPACE, "pipeline_plan_batch_layout: scratch of %zu bytes, need %zu", scratch_bytes, need);
+    CUDA_TRY(migan::launch_pipeline_plan_batch(reqs, n, res, padding, layout, flags, boxes, scratch, static_cast<ck_stream_t>(stream)));
     return MIGAN_OK;
 }
 

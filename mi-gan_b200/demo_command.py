@@ -123,10 +123,11 @@ def _header(path):
         return im.size, im.mode, len(im.getbands())
 
 
-def _size_check(pipeline: str, res: int):
+def _size_check(pipeline, res: int):
     """The pipeline's own `_check_mask_size` on header sizes: it reads only `res`, its name and the two shapes, so it
-    runs on a stand-in and zero-byte arrays of those shapes instead of a pipeline on the GPU."""
-    cls = PIPELINES[pipeline]
+    runs on a stand-in and zero-byte arrays of those shapes instead of a pipeline on the GPU.  `pipeline`: a name of
+    PIPELINES or a pipeline class."""
+    cls = PIPELINES[pipeline] if isinstance(pipeline, str) else pipeline
     stand_in = types.SimpleNamespace(res=res, _name=cls._name)
 
     def check(photo_size, mask_size, mask_bands) -> None:
@@ -224,6 +225,8 @@ class DemoSetup:
     """What every rank of one run shares: the planned items, the chunking and the generator on `device`.  The plan and
     its checks (`PlanError`) come before the generator is loaded, so a bad data set costs no GPU work."""
 
+    prog = "migan_b200.demo"            # the name progress lines start with
+
     def __init__(self, model_name: str, model, images_dir, masks_dir, output_dir, *, invert_mask: bool = False,
                  device="cuda", batch_size: int = BATCH_SIZE, num_workers: int = 2, noise_seed: int = 0,
                  pipeline: str = "demo", margin: Optional[int] = None):
@@ -269,6 +272,12 @@ class DemoSetup:
             return None
         a, b = self.chunks[j]
         return np.array([(self.noise_seed << 32) + it.index for it in self.items[a:b]], dtype=np.uint64)
+
+    def forward(self, pipe, j: int, photos, masks) -> list:
+        """Enqueue chunk j's `forward_batch(..., wait=False)` on `pipe`; returns its output tensors."""
+        if self.pipeline == "demo":
+            return pipe.forward_batch(photos, masks, self.invert_mask, wait=False, seeds=self.seeds(j))
+        return pipe.forward_batch(photos, masks, self.invert_mask, wait=False)
 
 
 class RunStats(NamedTuple):
@@ -325,8 +334,8 @@ def run_rank(setup: DemoSetup, rank: int = 0, world_size: int = 1, progress: boo
             done_images += b - a
             if progress and rank == 0:
                 el = time.perf_counter() - t0
-                print("migan_b200.demo: chunk %d of %d done (images %d-%d); rank 0: %d images in %.1f s"
-                      % (j + 1, len(setup.chunks), a, b - 1, done_images, el), file=sys.stderr, flush=True)
+                print("%s: chunk %d of %d done (images %d-%d); rank 0: %d images in %.1f s"
+                      % (setup.prog, j + 1, len(setup.chunks), a, b - 1, done_images, el), file=sys.stderr, flush=True)
 
         with torch.cuda.device(dev):
             for j in own:
@@ -335,10 +344,7 @@ def run_rank(setup: DemoSetup, rank: int = 0, world_size: int = 1, progress: boo
                 assert got == j
                 photos = timed("decode", lambda: [f.result() for f in photo_futs])
                 masks = timed("decode", lambda: [f.result() for f in mask_futs])
-                if setup.pipeline == "demo":
-                    outs = pipe.forward_batch(photos, masks, setup.invert_mask, wait=False, seeds=setup.seeds(j))
-                else:
-                    outs = pipe.forward_batch(photos, masks, setup.invert_mask, wait=False)
+                outs = setup.forward(pipe, j, photos, masks)
                 del photos, masks                # the pipeline keeps them until the chunk is waited for
                 on_gpu.append((j, outs))
                 if len(on_gpu) > 1:
