@@ -15,6 +15,7 @@
  *   fid_frechet_distance               the Fréchet distance of two (mu, sigma) on the device (float64 eigensolver)
  *   ids_scores                         P-IDS and U-IDS of paired real / fake features (float64 finite-Newton SVM)
  *   kid_subset_terms                   the per-subset kernel sums of the kernel Inception distance (float64 DMMA)
+ *   prdc_counts                        the counts behind precision, recall, density and coverage (float64 DMMA)
  */
 #ifndef INCEPTION_B200_H_
 #define INCEPTION_B200_H_
@@ -156,6 +157,44 @@ size_t kid_workspace_bytes(int num_subsets, int m);
 int kid_subset_terms(const void* real, int64_t n_real, const void* fake, int64_t n_fake, int dim, int dtype,
                      const int32_t* real_idx_host, const int32_t* fake_idx_host, int num_subsets, int m, double* terms,
                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- Precision, recall, density and coverage -------------------------------------------------------------------------
+ * The k-nearest-neighbour manifold metrics of Kynkaanniemi et al. 2019 and Naeem et al. 2020 between real[n_real][dim]
+ * (Y) and fake[n_fake][dim] (X), on squared Euclidean distances in float64.  r_i is the (k + 1)-th smallest of
+ * {|Y_i - Y_j|^2 : j = 1..n_real}, row i itself included (so duplicate rows count as neighbours), s_j the same within X,
+ * and every comparison is `<=`:
+ *   out_counts[0] = #{j : exists i, |X_j - Y_i|^2 <= r_i}        precision = out_counts[0] / n_fake
+ *   out_counts[1] = #{i : exists j, |Y_i - X_j|^2 <= s_j}        recall    = out_counts[1] / n_real
+ *   out_counts[2] = sum_j #{i : |X_j - Y_i|^2 <= r_i}            density   = out_counts[2] / (k n_fake)
+ *   out_counts[3] = #{i : min_j |Y_i - X_j|^2 <= r_i}            coverage  = out_counts[3] / n_real
+ * The features are read as stored (dtype IDS_FLOAT32 or IDS_FLOAT64, device, row-major) and promoted exactly to float64.
+ * |a - b|^2 = max(0, |a|^2 + |b|^2 - 2 a.b) with every term from 64 x 64 fp64 DMMA tiles in one column order, so
+ * identical rows are at distance exactly 0.  No N x N or N x M matrix is formed: three passes keep per-row lists of the
+ * k + 1 smallest values, per-row counters and per-row flags.  The same inputs give the same bytes on every run, on any
+ * stream and for any order of the rows.
+ *
+ * out_counts: device int64 [4].  ASYNCHRONOUS on `stream`: nothing is read back.  Refused with MIGAN_ERR_INVALID: null
+ * pointers, k outside 1..PRDC_MAX_K, k + 1 above n_real or n_fake, n_real or n_fake >= 2^31, dim outside
+ * 1..PRDC_MAX_DIM, an unknown dtype; with MIGAN_ERR_WORKSPACE: a workspace that is short or not 256-byte aligned.
+ * Non-finite features are not checked here.
+ *
+ * prdc_real_radii computes the real side alone (|Y_i|^2 and r_i) into the start of the workspace, and
+ * prdc_counts_with_real_radii then scores a fake set against them without recomputing them: the same counts as
+ * prdc_counts, for any number of fake sets against one real set, as long as the workspace is not used for anything
+ * else in between and is sized for the largest n_fake.  prdc_counts is the two calls in turn. */
+#define PRDC_MAX_DIM 4096
+#define PRDC_MAX_K 32
+/* Device bytes prdc_counts needs; 0 on bad arguments.  With T(n) = ceil(n / 64), S(n) = min(8, T(n)),
+ * L = max(n_real, n_fake) and each region rounded up to 256 bytes: 8 n_real twice (norms, radii), 8 n_fake twice,
+ * 2048 (k + 1) T(L) S(L) (the neighbour lists), 256 S(n_real) T(n_fake) (the per-row counters), 4 n_real twice (the
+ * flags) and 16 (T(n_real) + T(n_fake)) (the partial totals). */
+size_t prdc_workspace_bytes(int64_t n_real, int64_t n_fake, int dim, int k);
+int prdc_counts(const void* real, int64_t n_real, const void* fake, int64_t n_fake, int dim, int dtype, int k,
+                int64_t* out_counts, void* workspace, size_t workspace_bytes, void* stream);
+int prdc_real_radii(const void* real, int64_t n_real, int dim, int dtype, int k, void* workspace,
+                    size_t workspace_bytes, void* stream);
+int prdc_counts_with_real_radii(const void* real, int64_t n_real, const void* fake, int64_t n_fake, int dim, int dtype,
+                                int k, int64_t* out_counts, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -18,6 +18,8 @@ Public surface (mirrors the reference's for this path):
     ids.inception_discriminative_scores
                                      Co-Mod-GAN's P-IDS and U-IDS (LinearSVC(dual=False) solved on the GPU, fp64 Newton)
     kid.kernel_inception_distance    the kernel Inception distance (StyleGAN2-ADA's KID, fp64 tensor-core kernel sums)
+    prdc.precision_recall_density_coverage
+                                      k-NN precision, recall, density and coverage (fp64 tensor-core distances)
     lpips.LPIPS                      drop-in for lpips.LPIPS(net="alex"): the script's LPIPS distance (AlexNet on tensor cores)
     metrics.compute_ssim / metrics.SSIM / metrics.compute_psnr
                                      the reference's SSIM (pytorch-ssim) and PSNR evaluators' arithmetic, in double
@@ -39,12 +41,12 @@ import warnings as _warnings
 # __main__ block only calls demo_command.main, so runpy's warning about the module's second copy does not apply.
 _warnings.filterwarnings("ignore", message=r"'migan_b200\.demo' found in sys\.modules", category=RuntimeWarning)
 
-from . import arch, build, demo, evaluate, export, fid, fullres, holewin, ids, kid, lpips, masks, metrics, ops, parallel, pipeline, synthetic  # noqa: F401
+from . import arch, build, demo, evaluate, export, fid, fullres, holewin, ids, kid, lpips, masks, metrics, ops, parallel, pipeline, prdc, synthetic  # noqa: F401
 from .fullres import FullResPipeline  # noqa: F401
 from .holewin import HoleWindowPipeline  # noqa: F401
 from .evaluate import EvalPipeline, ResultsPipeline  # noqa: F401
 from .masks import RandomMaskStream  # noqa: F401
 from .generator import Generator  # noqa: F401
 
-__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "ResultsPipeline", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "ids", "kid", "lpips", "masks", "metrics", "ops", "parallel", "pipeline", "synthetic"]
+__all__ = ["EvalPipeline", "FullResPipeline", "Generator", "HoleWindowPipeline", "RandomMaskStream", "ResultsPipeline", "arch", "build", "demo", "evaluate", "export", "fid", "fullres", "holewin", "ids", "kid", "lpips", "masks", "metrics", "ops", "parallel", "pipeline", "prdc", "synthetic"]
 __version__ = "0.1.0"

@@ -18,7 +18,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libmigan_b200.so")
 STAMP = os.path.join(LIBDIR, "libmigan_b200.stamp")
 
-SOURCES = ["elementwise.cu", "gemm_simt.cu", "ops.cu", "sepconv_tc.cu", "abi_error.cu", "migan_abi.cu", "comodgan_abi.cu", "prepost.cu", "pipeline.cu", "demo_resize.cu", "fullres.cu", "holewin.cu", "masks.cu", "reparam.cu", "inception.cu", "inception_abi.cu", "lpips_abi.cu", "metrics.cu", "frechet.cu", "ids.cu", "kid.cu"]
+SOURCES = ["elementwise.cu", "gemm_simt.cu", "ops.cu", "sepconv_tc.cu", "abi_error.cu", "migan_abi.cu", "comodgan_abi.cu", "prepost.cu", "pipeline.cu", "demo_resize.cu", "fullres.cu", "holewin.cu", "masks.cu", "reparam.cu", "inception.cu", "inception_abi.cu", "lpips_abi.cu", "metrics.cu", "frechet.cu", "ids.cu", "kid.cu", "prdc.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -23,6 +23,10 @@ Differences from the reference script:
 * `--kid` also prints the kernel Inception distance (`KID:`) after all the lines above, from the same kept features:
   `kid.kernel_inception_distance(real, composed)` with 100 subsets of min(n, 1000) images and seed 0, StyleGAN2-ADA's
   unbiased estimator on pytorch_fid's features.  Like `--ids` it does not combine with `--real-stats`;
+* `--prdc` also prints `Precision:`, `Recall:`, `Density:` and `Coverage:` after all the lines above (after `KID:`),
+  from the same kept features: `prdc.precision_recall_density_coverage(real, composed)` with k = 3, the k-nearest-
+  neighbour manifold metrics of StyleGAN2-ADA's `pr50k3` and of Naeem et al. on pytorch_fid's features.  Like `--ids`
+  it does not combine with `--real-stats`;
 * `--ssim` and `--psnr` also print `SSIM:` and `PSNR:` after the two lines: the means of the per-image
   `metrics.compute_ssim(real, composed, window_size=11, size_average=False)` and `metrics.compute_psnr(composed, real,
   for_dataset=None)` (rgb_range 1, nothing shaved; an image whose composite equals the photo has PSNR inf, and so does
@@ -34,8 +38,10 @@ Differences from the reference script:
 * `--hole-bins EDGES` (comma-separated, strictly increasing, from 0 to 1, 2 to 33 edges) also prints one `HOLE` line per
   bin of hole fraction h, image i in bin j when e_j <= h_i < e_{j+1} (the last bin also takes h = 1): its image count,
   the FID of its composed images against the real statistics of *all* images (or `--real-stats`), and the means of its
-  per-image LPIPS, SSIM and PSNR values, with `--ids` its P-IDS and U-IDS, and with `--kid` the KID of its composed
-  images against the real images of all images (a fresh RandomState(0) per bin); `nan` where a bin has too few images;
+  per-image LPIPS, SSIM and PSNR values, with `--ids` its P-IDS and U-IDS, with `--kid` the KID of its composed
+  images against the real images of all images (a fresh RandomState(0) per bin), and with `--prdc` the precision,
+  recall, density and coverage of its composed images against the real images of all images (the real radii computed
+  once); `nan` where a bin has too few images;
 * `--hole-range LO HI` draws the generated masks from RandomMask(R, [LO, HI]) (`RandomMaskStream(R, 0, hole_range)`)
   instead of [0, 1]; it does not combine with `--mask-dir`.
 
@@ -45,7 +51,7 @@ migan_b200.score_results` scores result files instead), one LPIPS call and one I
 outputs are the same bytes on any rank at any W.  Per round of W chunks every rank sends its chunk's features and LPIPS
 values to rank 0 in one fixed-size gather (a rank without a chunk sends padding), and rank 0 adds them to the feature
 statistics in chunk order, one `FeatureStatistics.add` per chunk, so the sums see the same rows in the same groups at
-every W; with `--ids` or `--kid` it also keeps them in dataset order, so the scores are the same bits at every W.  The optional
+every W; with `--ids`, `--kid` or `--prdc` it also keeps them in dataset order, so the scores are the same bits at every W.  The optional
 per-image values (hole fraction, SSIM, PSNR) travel as extra columns of the same gather and are kept at their global
 index as the LPIPS values are, so their means and the CSV are the same bytes at every W.  Generated
 masks come from one sequential stream: every rank advances its own stream through all chunks and
@@ -71,6 +77,7 @@ import torch.distributed as dist
 
 from . import _abi, comodgan, fid, ids, lpips, metrics
 from . import kid as kid_metric
+from . import prdc as prdc_metric
 from ._request_path import load_generator
 from .evaluate import EvalPipeline, ResultsPipeline
 from .masks import check_hole_range
@@ -84,6 +91,7 @@ MASK_SKIP = 256                 # generated masks skipped per RandomMaskStream.n
 EXTRA_VALUES = ("hole_fraction", "ssim", "psnr")    # optional per-image values, in their gather-column order
 PER_IMAGE_COLUMNS = ("name", "hole_fraction", "lpips", "ssim", "psnr")   # the per-image table's column order
 FULL_RANGE = (0.0, 1.0)         # RandomMask's default hole_range
+PRDC_K = 3                      # the neighbourhood size of --prdc: StyleGAN2-ADA's pr50k3
 
 
 def resolution(model_name: str) -> int:
@@ -379,9 +387,10 @@ class _EvalFields(NamedTuple):
 class HoleBin(NamedTuple):
     """The scores of the images whose hole fraction h lies in [lo, hi) ([lo, hi] for the last bin).  `fid`: the bin's
     composed images against the real statistics of all images; `lpips`, `ssim`, `psnr`: np.mean of the bin's per-image
-    values; `kid`: the KID of the bin's composed features against the real features of all images.  nan where the bin
-    has too few images (2 for FID, the discriminative scores and KID, 1 for the means); None where the value was not
-    asked for."""
+    values; `kid`: the KID of the bin's composed features against the real features of all images; `precision`,
+    `recall`, `density`, `coverage`: those of the bin's composed features against the real features of all images
+    (k = 3).  nan where the bin has too few images (2 for FID, the discriminative scores and KID, k + 1 = 4 for the
+    four manifold metrics, 1 for the means); None where the value was not asked for."""
     lo: float
     hi: float
     count: int
@@ -392,6 +401,10 @@ class HoleBin(NamedTuple):
     p_ids: Optional[float] = None
     u_ids: Optional[float] = None
     kid: Optional[float] = None
+    precision: Optional[float] = None
+    recall: Optional[float] = None
+    density: Optional[float] = None
+    coverage: Optional[float] = None
 
 
 class EvalResult(_EvalFields):
@@ -402,12 +415,15 @@ class EvalResult(_EvalFields):
     * `per_image`: {column: values} in `PER_IMAGE_COLUMNS` order: "name" (list of str), then float64 [count] arrays
       "hole_fraction", "lpips" and, when computed, "ssim" and "psnr", all in dataset (sorted) order;
     * `by_hole`: with hole bins, one `HoleBin` per bin in edge order;
-    * `kid`: the kernel Inception distance of the composed features against the real ones (`kid_metric.KIDResult.kid`)."""
+    * `kid`: the kernel Inception distance of the composed features against the real ones (`kid_metric.KIDResult.kid`);
+    * `prdc`: precision, recall, density and coverage of the composed features against the real ones, k = 3
+      (`prdc_metric.PRDCResult`)."""
     ssim: Optional[float] = None
     psnr: Optional[float] = None
     per_image: Optional[Dict[str, Union[List[str], np.ndarray]]] = None
     by_hole: Optional[Tuple[HoleBin, ...]] = None
     kid: Optional[float] = None
+    prdc: Optional[prdc_metric.PRDCResult] = None
 
     def _replace(self, **fields) -> "EvalResult":
         out = super()._replace(**fields)
@@ -418,7 +434,8 @@ class EvalResult(_EvalFields):
 class Merge:
     """Rank 0's ordered merge: `add` the chunk results in chunk order, then `result()`.  With `keep_features` it also
     keeps every real and composed feature row in dataset order on the device, for the discriminative scores; with `kid`
-    it keeps them too, for the kernel Inception distance.
+    it keeps them too, for the kernel Inception distance, and with `prdc` for precision, recall, density and coverage
+    (the real radii computed once for the overall value and every bin).
     `extra_values`: the names of the chunks' extra per-image values (`EvalSetup.extra_values`), kept at their global
     index as the LPIPS values are; `names`: each image's name, for the per-image table of the result; `hole_bins`: the
     edges of the hole-fraction bins (the extra values then hold "hole_fraction"): each chunk's composed features also
@@ -426,15 +443,15 @@ class Merge:
 
     def __init__(self, n: int, device, real_features: bool = True, keep_features: bool = False,
                  extra_values: Sequence[str] = (), names: Optional[Sequence[str]] = None,
-                 hole_bins: Optional[Sequence[float]] = None, kid: bool = False):
+                 hole_bins: Optional[Sequence[float]] = None, kid: bool = False, prdc: bool = False):
         self.n, self.device = n, torch.device(device)
         self.real = fid.FeatureStatistics(device=self.device) if real_features else None
         self.fake = fid.FeatureStatistics(device=self.device)
-        if (keep_features or kid) and not real_features:
-            raise ValueError("the discriminative scores and KID need the real features")
-        self.ids, self.kid = bool(keep_features), bool(kid)
+        if (keep_features or kid or prdc) and not real_features:
+            raise ValueError("the discriminative scores, KID and the manifold metrics need the real features")
+        self.ids, self.kid, self.prdc = bool(keep_features), bool(kid), bool(prdc)
         self.kept = None
-        if keep_features or kid:
+        if keep_features or kid or prdc:
             self.kept = [torch.empty((n, fid.FEATURES), dtype=torch.float32, device=self.device) for _ in range(2)]
         self.values = torch.empty(n, dtype=torch.float32, device=self.device)
         self.extra_values = tuple(extra_values)
@@ -495,6 +512,10 @@ class Merge:
             res = res._replace(p_ids=scores.p_ids, u_ids=scores.u_ids)
         if self.kid:
             res.kid = kid_metric.kernel_inception_distance(*self.kept).kid
+        radii = None
+        if self.prdc:
+            radii = prdc_metric.RealRadii(self.kept[0], PRDC_K, max_fake=self.n)
+            res.prdc = prdc_metric.precision_recall_density_coverage(radii, self.kept[1])
         columns = {"lpips": values}
         if self.extra is not None:
             extra = self.extra.cpu().numpy().astype(np.float64)
@@ -507,12 +528,13 @@ class Merge:
             columns["name"] = self.names
             res.per_image = {k: columns[k] for k in PER_IMAGE_COLUMNS if k in columns}
         if self.binned is not None:
-            res.by_hole = self.hole_results(columns, real_stats)
+            res.by_hole = self.hole_results(columns, real_stats, radii)
         return res
 
-    def hole_results(self, columns, real_stats=None) -> Tuple[HoleBin, ...]:
+    def hole_results(self, columns, real_stats=None, radii=None) -> Tuple[HoleBin, ...]:
         """One `HoleBin` per bin: the bins of the merged hole fractions, the binned composed statistics against the
-        real ones of all images (or `real_stats`), and the per-image columns' means over each bin."""
+        real ones of all images (or `real_stats`), and the per-image columns' means over each bin; with `radii`
+        (`prdc_metric.RealRadii` of all real features) each bin's composed features against them."""
         bins = hole_bin_index(torch.from_numpy(columns["hole_fraction"]), self.inner_edges.cpu()).numpy()
         counts = self.binned.counts()
         want = np.bincount(bins, minlength=len(counts))
@@ -537,8 +559,13 @@ class Merge:
                 kid = math.nan
                 if at is not None:
                     kid = kid_metric.kernel_inception_distance(self.kept[0], self.kept[1][at]).kid
+            manifold = (None,) * 4
+            if self.prdc:
+                manifold = (math.nan,) * 4
+                if n > PRDC_K:
+                    manifold = tuple(prdc_metric.precision_recall_density_coverage(radii, self.kept[1][at])[:4])
             out.append(HoleBin(lo, hi, n, float(fid_b), means["lpips"], means.get("ssim"), means.get("psnr"), p_ids,
-                               u_ids, kid))
+                               u_ids, kid, *manifold))
         return tuple(out)
 
 
@@ -614,7 +641,7 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
              num_workers: int = 2, noise_seed: int = 0, real_stats=None, save_real_stats_to=None,
              inception_weights=None, lpips_weights=None, ids: bool = False, ssim: bool = False, psnr: bool = False,
              per_image: bool = False, hole_bins: Optional[Sequence[float]] = None,
-             hole_range: Sequence[float] = FULL_RANGE, kid: bool = False) -> Optional[EvalResult]:
+             hole_range: Sequence[float] = FULL_RANGE, kid: bool = False, prdc: bool = False) -> Optional[EvalResult]:
     """FID and LPIPS of `model` over `real_dir`, as the command prints them.  `model`: a state_dict, a path to one, or a
     generator object (MI-GAN `Generator`, or `comodgan.Generator` for the comodgan names).  `real_stats`: a path to an
     .npz with `mu` and `sigma` (or such a pair); `save_real_stats_to`: where to write the real statistics.
@@ -624,10 +651,11 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
     per-image table (`EvalResult.per_image`).  `hole_bins`: the edges of hole-fraction bins, scored one by one
     (`EvalResult.by_hole`); `hole_range`: RandomMask's hole_range for the generated masks (not with `mask_dir`).
     `kid`: also the kernel Inception distance (`EvalResult.kid`, and per bin); like `ids` it excludes `real_stats`.
+    `prdc`: also precision, recall, density and coverage (`EvalResult.prdc`, and per bin); it excludes `real_stats` too.
 
     In an initialised process group (one process per GPU, `device` this rank's), the chunks are sharded round-robin and
     rank 0 returns the result; the other ranks return None."""
-    check_stats_args(real_stats, save_real_stats_to, ids, kid)
+    check_stats_args(real_stats, save_real_stats_to, ids, kid, prdc)
     check_hole_args(hole_bins, hole_range, mask_dir)
     if real_stats is not None and not isinstance(real_stats, tuple):
         real_stats = load_real_stats(real_stats)
@@ -635,11 +663,11 @@ def evaluate(model_name: str, model, real_dir, mask_dir=None, *, device="cuda", 
                       num_workers=num_workers, noise_seed=noise_seed, real_features=real_stats is None,
                       inception_weights=inception_weights, lpips_weights=lpips_weights, ssim=ssim, psnr=psnr,
                       per_image=per_image, hole_bins=hole_bins, hole_range=hole_range)
-    return run_setup(setup, real_stats, save_real_stats_to, ids, kid)
+    return run_setup(setup, real_stats, save_real_stats_to, ids, kid, prdc)
 
 
-def check_stats_args(real_stats, save_real_stats_to, ids: bool, kid: bool = False) -> None:
-    """The refusals of --real-stats, --save-real-stats, --ids and --kid, before any work."""
+def check_stats_args(real_stats, save_real_stats_to, ids: bool, kid: bool = False, prdc: bool = False) -> None:
+    """The refusals of --real-stats, --save-real-stats, --ids, --kid and --prdc, before any work."""
     if real_stats is not None and save_real_stats_to is not None:
         raise ValueError("--real-stats and --save-real-stats exclude each other: with stored statistics the real images "
                          "are not scored")
@@ -647,20 +675,22 @@ def check_stats_args(real_stats, save_real_stats_to, ids: bool, kid: bool = Fals
         raise ValueError("--ids needs the real images' features, which stored statistics (--real-stats) do not carry")
     if kid and real_stats is not None:
         raise ValueError("--kid needs the real images' features, which stored statistics (--real-stats) do not carry")
+    if prdc and real_stats is not None:
+        raise ValueError("--prdc needs the real images' features, which stored statistics (--real-stats) do not carry")
 
 
 def run_setup(setup: EvalSetup, real_stats=None, save_real_stats_to=None, ids: bool = False,
-              kid: bool = False) -> Optional[EvalResult]:
+              kid: bool = False, prdc: bool = False) -> Optional[EvalResult]:
     """Every round of `setup`'s chunks on this rank, merged on rank 0 in chunk order (see `evaluate`); `real_stats`: a
     loaded (mu, sigma) pair or None.  The setup's `ssim`, `psnr` and `per_image` choices fill the result's attributes of
-    those names; `kid` fills `EvalResult.kid` (and each bin's)."""
+    those names; `kid` fills `EvalResult.kid` (and each bin's), `prdc` fills `EvalResult.prdc` (and each bin's four)."""
     distributed = dist.is_available() and dist.is_initialized()
     world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
     merge = None
     if rank == 0:
         merge = Merge(len(setup.images), setup.device, setup.real_features, keep_features=ids,
                       extra_values=setup.extra_values, names=setup.names if setup.per_image else None,
-                      hole_bins=setup.hole_bins, kid=kid)
+                      hole_bins=setup.hole_bins, kid=kid, prdc=prdc)
     t0 = time.perf_counter()
     with torch.cuda.device(setup.device), RankWorker(setup, rank, world) as worker:
         for r in range(worker.rounds):
@@ -700,6 +730,7 @@ def get_args(argv=None):
     parser.add_argument("--ids", action="store_true", help="Also print P-IDS and U-IDS (Co-Mod-GAN's Inception "
                         "discriminative scores).")
     add_kid_arg(parser)
+    add_prdc_arg(parser)
     add_per_image_args(parser)
     return parser.parse_args(argv)
 
@@ -708,6 +739,12 @@ def add_kid_arg(parser: argparse.ArgumentParser) -> None:
     """--kid, shared with score_results."""
     parser.add_argument("--kid", action="store_true", help="Also print the kernel Inception distance (KID: 100 subsets "
                         "of min(n, 1000) images, seed 0).")
+
+
+def add_prdc_arg(parser: argparse.ArgumentParser) -> None:
+    """--prdc, shared with score_results."""
+    parser.add_argument("--prdc", action="store_true", help="Also print precision, recall, density and coverage "
+                        "(k-nearest-neighbour manifold metrics, k = 3).")
 
 
 def add_per_image_args(parser: argparse.ArgumentParser) -> None:
@@ -766,21 +803,23 @@ def run_command(requested_device: str, call, command: str = "evaluate_fid_lpips"
 
 
 def hole_line(b: HoleBin, last: bool) -> str:
-    """`HOLE [lo, hi): images n FID f LPIPS l[ SSIM s][ PSNR p][ P-IDS a U-IDS u][ KID k]`, every number repr(float);
-    the last bin is closed, `[lo, 1.0]`."""
+    """`HOLE [lo, hi): images n FID f LPIPS l[ SSIM s][ PSNR p][ P-IDS a U-IDS u][ KID k][ Precision p Recall r
+    Density d Coverage c]`, every number repr(float); the last bin is closed, `[lo, 1.0]`."""
     line = "HOLE [%r, %r%s: images %d FID %r LPIPS %r" % (float(b.lo), float(b.hi), "]" if last else ")", b.count,
                                                           float(b.fid), float(b.lpips))
-    for name, v in (("SSIM", b.ssim), ("PSNR", b.psnr), ("P-IDS", b.p_ids), ("U-IDS", b.u_ids), ("KID", b.kid)):
+    for name, v in (("SSIM", b.ssim), ("PSNR", b.psnr), ("P-IDS", b.p_ids), ("U-IDS", b.u_ids), ("KID", b.kid),
+                    ("Precision", b.precision), ("Recall", b.recall), ("Density", b.density),
+                    ("Coverage", b.coverage)):
         if v is not None:
             line += " %s %r" % (name, float(v))
     return line
 
 
 def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr: bool = False,
-                 kid: bool = False) -> None:
+                 kid: bool = False, prdc: bool = False) -> None:
     """The script's two result lines on rank 0, then the mean SSIM and PSNR with `ssim` / `psnr`, then the
-    discriminative scores' two with `ids`, then `KID: <repr>` with `kid`, then one `hole_line` per bin with hole
-    bins."""
+    discriminative scores' two with `ids`, then `KID: <repr>` with `kid`, then `Precision: <repr>`, `Recall: <repr>`,
+    `Density: <repr>` and `Coverage: <repr>` with `prdc`, then one `hole_line` per bin with hole bins."""
     if res is not None:
         print("FID:", res.fid)
         print("LPIPS: ", res.lpips)
@@ -793,6 +832,9 @@ def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr:
             print("U-IDS:", res.u_ids)
         if kid:
             print("KID: %r" % float(res.kid))
+        if prdc:
+            for name in ("precision", "recall", "density", "coverage"):
+                print("%s: %r" % (name.capitalize(), float(getattr(res.prdc, name))))
         if res.by_hole is not None:
             for k, b in enumerate(res.by_hole):
                 print(hole_line(b, k == len(res.by_hole) - 1))
@@ -800,7 +842,7 @@ def print_result(res: Optional[EvalResult], ids: bool, ssim: bool = False, psnr:
 
 def finish_command(res: Optional[EvalResult], args) -> None:
     """Rank 0's output: the result lines, and the --per-image file."""
-    print_result(res, args.ids, args.ssim, args.psnr, args.kid)
+    print_result(res, args.ids, args.ssim, args.psnr, args.kid, args.prdc)
     if res is not None and args.per_image is not None:
         write_per_image(args.per_image, res.per_image)
 
@@ -815,7 +857,8 @@ def main(argv=None) -> None:
         num_workers=args.num_workers, noise_seed=args.noise_seed, real_stats=args.real_stats,
         save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
         lpips_weights=args.lpips_weights, ids=args.ids, ssim=args.ssim, psnr=args.psnr,
-        per_image=args.per_image is not None, hole_bins=hole_bins, hole_range=hole_range, kid=args.kid))
+        per_image=args.per_image is not None, hole_bins=hole_bins, hole_range=hole_range, kid=args.kid,
+        prdc=args.prdc))
     finish_command(res, args)
 
 

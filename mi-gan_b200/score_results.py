@@ -14,7 +14,7 @@ from `--mask-dir` (`<stem>.png`, 255 = known) or, without it, from the generated
 `evaluate_fid_lpips`.
 
 It prints `evaluate_fid_lpips`'s lines (`FID:`, `LPIPS: `, with `--ssim` `SSIM:`, with `--psnr` `PSNR:`, and with `--ids`
-`P-IDS:` and `U-IDS:`, with `--kid` `KID:`, then with `--hole-bins` one `HOLE` line per bin), writes its `--per-image` CSV, and has its chunking, sharding, ordered merge and statistics files: `--save-real-stats` writes the same statistics the evaluation command
+`P-IDS:` and `U-IDS:`, with `--kid` `KID:`, with `--prdc` `Precision:`, `Recall:`, `Density:` and `Coverage:`, then with `--hole-bins` one `HOLE` line per bin), writes its `--per-image` CSV, and has its chunking, sharding, ordered merge and statistics files: `--save-real-stats` writes the same statistics the evaluation command
 writes for the same real directory, R and batch size, and `--real-stats` reads either's.
 
 Before any GPU work one planning pass reads the header (size and mode; no pixels) of every photo, result and mask and
@@ -68,14 +68,14 @@ def score(real_dir, results_dir, mask_dir=None, *, resolution: int, device="cuda
           num_workers: int = 2, real_stats=None, save_real_stats_to=None, inception_weights=None, lpips_weights=None,
           ids: bool = False, ssim: bool = False, psnr: bool = False, per_image: bool = False,
           hole_bins: Optional[Sequence[float]] = None,
-          hole_range: Sequence[float] = E.FULL_RANGE, kid: bool = False) -> Optional[E.EvalResult]:
+          hole_range: Sequence[float] = E.FULL_RANGE, kid: bool = False, prdc: bool = False) -> Optional[E.EvalResult]:
     """FID and LPIPS of the result files in `results_dir` against the photos of `real_dir`, as the command prints them
     (`evaluate_fid_lpips.evaluate`'s `EvalResult`).  `resolution`: R, 256 or 512.  The other arguments are `evaluate`'s,
-    `ssim`, `psnr`, `per_image`, `hole_bins`, `hole_range` and `kid` among them.
+    `ssim`, `psnr`, `per_image`, `hole_bins`, `hole_range`, `kid` and `prdc` among them.
 
     The argument checks and the planning pass (`PlanError`) come before any device is touched.  In an initialised
     process group rank 0 returns the result; the other ranks return None."""
-    E.check_stats_args(real_stats, save_real_stats_to, ids, kid)
+    E.check_stats_args(real_stats, save_real_stats_to, ids, kid, prdc)
     E.check_hole_args(hole_bins, hole_range, mask_dir)
     if resolution not in RESOLUTIONS:
         raise ValueError("--resolution must be one of %s, got %r" % (", ".join(map(str, RESOLUTIONS)), resolution))
@@ -90,7 +90,7 @@ def score(real_dir, results_dir, mask_dir=None, *, resolution: int, device="cuda
                         real_features=real_stats is None, inception_weights=inception_weights,
                         lpips_weights=lpips_weights, results=results, res=resolution, ssim=ssim, psnr=psnr,
                         per_image=per_image, hole_bins=hole_bins, hole_range=hole_range)
-    return E.run_setup(setup, real_stats, save_real_stats_to, ids, kid)
+    return E.run_setup(setup, real_stats, save_real_stats_to, ids, kid, prdc)
 
 
 def get_args(argv=None):
@@ -111,13 +111,14 @@ def get_args(argv=None):
     parser.add_argument("--ids", action="store_true", help="Also print P-IDS and U-IDS (Co-Mod-GAN's Inception "
                         "discriminative scores).")
     E.add_kid_arg(parser)
+    E.add_prdc_arg(parser)
     E.add_per_image_args(parser)
     return parser.parse_args(argv)
 
 
 def main(argv=None) -> None:
     args = get_args(argv)
-    E.check_stats_args(args.real_stats, args.save_real_stats, args.ids, args.kid)
+    E.check_stats_args(args.real_stats, args.save_real_stats, args.ids, args.kid, args.prdc)
     E.check_per_image_path(args.per_image)
     hole_bins, hole_range = E.check_hole_flags(args)
     res = E.run_command(args.device, lambda device: score(
@@ -125,7 +126,8 @@ def main(argv=None) -> None:
         batch_size=args.batch_size, num_workers=args.num_workers, real_stats=args.real_stats,
         save_real_stats_to=args.save_real_stats, inception_weights=args.inception_weights,
         lpips_weights=args.lpips_weights, ids=args.ids, ssim=args.ssim, psnr=args.psnr,
-        per_image=args.per_image is not None, hole_bins=hole_bins, hole_range=hole_range, kid=args.kid),
+        per_image=args.per_image is not None, hole_bins=hole_bins, hole_range=hole_range, kid=args.kid,
+        prdc=args.prdc),
         "score_results")
     E.finish_command(res, args)
 
