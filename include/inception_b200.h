@@ -9,6 +9,7 @@
  *   inception_set_weight / _finalize   load_state_dict of pt_inception-2015-12-05: torchvision Inception3 key names
  *                                      and shapes (472 entries besides num_batches_tracked, fc.* accepted and unused)
  *   inception_features                 model(x)[0].view(n, 2048): the 2048-d pool3 features of x[n,3,H,W] in [0, 1]
+ *   inception_features_u8              the same features of decoded uint8 photos of mixed sizes, in one call
  *   fid_stats_update                   the float64 running sums behind np.mean / np.cov(rowvar=False) of the features
  *   fid_stats_update_binned            the same sums for up to 32 bins of rows at once (statistics per hole size)
  *   fid_stats_mean_cov                 the mean and covariance from those sums, on the device
@@ -52,6 +53,19 @@ int inception_features(inception_ctx* ctx, const float* x, int n, int H, int W, 
                        size_t workspace_bytes, void* stream);
 int inception_last_launch_count(const inception_ctx* ctx);
 
+/* ---- decoded photos of any sizes -------------------------------------------------------------------------------------
+ * feats[n][2048] of n photos packed in `photos` (device, uint8 HWC RGB), photo i at byte offset off[i] with size
+ * h[i] x w[i]; off / h / w are HOST arrays, read during the call.  Equals inception_features on each photo's ToTensor
+ * (v / 255 as fp32, [3][h][w]), bit for bit: the input stage evaluates the resize's expression on v / 255 rounded once,
+ * and the walk after it is the same.  The input stage is one launch per INCEPTION_U8_TABLE photos (their table travels
+ * in the kernel parameter); offsets are 64-bit, so the packed buffer may exceed 2^31 bytes.  The workspace depends on n
+ * only.  Refused with MIGAN_ERR_INVALID: null pointers, n < 1, a photo of h or w < 1 or a negative offset.
+ * Asynchronous on `stream`. */
+#define INCEPTION_U8_TABLE 64
+size_t inception_workspace_bytes_u8(const inception_ctx* ctx, int n);
+int inception_features_u8(inception_ctx* ctx, const uint8_t* photos, const int64_t* off, const int* h, const int* w,
+                          int n, float* feats, void* workspace, size_t workspace_bytes, void* stream);
+
 /* The forward's launches for n images of H x W, one per line ("<kind> <name> key=value ..."), written to buf (NUL
  * terminated, truncated to cap bytes); returns the full length.  Works on a description-only context. */
 int inception_launch_plan(const inception_ctx* ctx, int n, int H, int W, char* buf, int cap);
@@ -59,6 +73,9 @@ int inception_launch_plan(const inception_ctx* ctx, int n, int H, int W, char* b
 /* ---- kernels on their own (device pointers, NHWC fp32 unless stated) ----------------------------------------------- */
 /* y[n][299][299][4] = 2 * bilinear(x[n][3][H][W] -> 299 x 299, align_corners=False, no antialias) - 1; channel 3 = 0. */
 int inception_resize(const float* x, int n, int H, int W, float* y, void* stream);
+/* The input stage of inception_features_u8 on its own: y[n][299][299][4] from n packed uint8 photos (off / h / w HOST
+ * arrays, as there) = inception_resize of each photo's ToTensor, bit for bit. */
+int inception_input_u8(const uint8_t* photos, const int64_t* off, const int* h, const int* w, int n, float* y, void* stream);
 #define INCEPTION_POOL_MAX_S2 0     /* max 3x3, stride 2, no padding */
 #define INCEPTION_POOL_AVG_S1 1     /* average 3x3, stride 1, padding 1, count_include_pad=False */
 #define INCEPTION_POOL_MAX_S1 2     /* max 3x3, stride 1, padding 1 */

@@ -27,6 +27,8 @@ Public surface (mirrors the reference's for this path):
     evaluate_fid_lpips               python -m migan_b200.evaluate_fid_lpips: the evaluation script's CLI, sharded over GPUs
     score_results                    python -m migan_b200.score_results: the evaluation protocol over a directory of any
                                      method's result images, sharded over GPUs
+    fid_score                        python -m migan_b200.fid_score: pytorch_fid's CLI over two image folders of any photo
+                                     sizes (uint8 upload, fid.InceptionV3.features_u8), sharded over GPUs
     demo (python -m)                 python -m migan_b200.demo: scripts/demo.py's CLI and files, sharded over GPUs
     crop_results                     python -m migan_b200.crop_results: create_onnx_pipeline.py's sample loop, sharded over GPUs
     export.copy_weights              drop-in for scripts/export_inference_model.py:copy_weights (filters computed on the GPU)

@@ -147,6 +147,14 @@ struct Runner {
         if (e) rc = migan::fail(MIGAN_ERR_CUDA, "kernel launch failed: %s", dev_err(e));
         ++launches;
     }
+    // One launch of F over a batch descriptor passed by value (comod::batch_launch).
+    template <class F, class Batch>
+    void launch_batch(const Batch& b) {
+        if (dry || rc || b.start[b.n] <= 0) return;
+        const int e = (int)comod::batch_launch<F>(b, s);
+        if (e) rc = migan::fail(MIGAN_ERR_CUDA, "kernel launch failed: %s", dev_err(e));
+        ++launches;
+    }
 };
 
 // Activation tensor [n][H][W][C] in the workspace.

@@ -209,6 +209,22 @@ struct Walk {
         Act x = alloc(kOS, kOS, 4);
         R.note("resize in=%dx%dx3 out=%dx%dx4", H, W, kOS, kOS);
         R.launch(incep::ResizeK{img, x.p, H, W, kOS}, (int64_t)n * kOS * kOS);
+        body(x, feats);
+    }
+
+    // The same walk from packed uint8 photos (off / h / w: host arrays of n): one input launch per table of photos.
+    void run_u8(const uint8_t* photos, const int64_t* off, const int* h, const int* w, float* feats) {
+        Act x = alloc(kOS, kOS, 4);
+        for (int k = 0; k < n; k += INCEPTION_U8_TABLE) {
+            const int m = std::min(INCEPTION_U8_TABLE, n - k);
+            R.note("resize_u8 photos=%d..%d out=%dx%dx4", k, k + m - 1, kOS, kOS);
+            if (!R.dry) R.launch_batch<incep::ResizeU8K>(incep::u8_table(photos, off, h, w, k, m, x.p, kOS));
+        }
+        body(x, feats);
+    }
+
+    // Everything after the input stage: x is the [n][299][299][4] input.
+    void body(Act x, float* feats) {
         x = conv("Conv2d_1a_3x3", x);
         x = conv("Conv2d_2a_3x3", x);
         x = conv("Conv2d_2b_3x3", x);
@@ -231,6 +247,16 @@ struct Walk {
 
 int check_images(int n, int H, int W) {
     if (n < 1 || H < 1 || W < 1) return fail(MIGAN_ERR_INVALID, "bad batch: n=%d H=%d W=%d (all >= 1)", n, H, W);
+    return 0;
+}
+
+int check_photos(const uint8_t* photos, const int64_t* off, const int* h, const int* w, int n) {
+    if (!photos || !off || !h || !w) return fail(MIGAN_ERR_INVALID, "null photos / off / h / w");
+    if (n < 1) return fail(MIGAN_ERR_INVALID, "bad batch: n=%d (>= 1)", n);
+    for (int i = 0; i < n; ++i)
+        if (h[i] < 1 || w[i] < 1 || off[i] < 0)
+            return fail(MIGAN_ERR_INVALID, "photo %d: %dx%d at byte offset %lld (sizes >= 1, offset >= 0)", i, h[i], w[i],
+                        (long long)off[i]);
     return 0;
 }
 
@@ -279,12 +305,35 @@ int inception_features(inception_ctx* c, const float* x, int n, int H, int W, fl
     return incep::forward(c, workspace, workspace_bytes, stream, [&](Runner& R) { Walk{c, R, n}.run(x, H, W, feats); });
 }
 
+size_t inception_workspace_bytes_u8(const inception_ctx* c, int n) {
+    if (!c || n < 1) return 0;
+    return incep::workspace_bytes([&](Runner& R) { Walk{c, R, n}.run_u8(nullptr, nullptr, nullptr, nullptr, nullptr); });
+}
+
+int inception_features_u8(inception_ctx* c, const uint8_t* photos, const int64_t* off, const int* h, const int* w, int n,
+                          float* feats, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = incep::check_forward(c, "inception_finalize_weights")) return rc;
+    if (!feats) return fail(MIGAN_ERR_INVALID, "null feats");
+    if (int rc = check_photos(photos, off, h, w, n)) return rc;
+    return incep::forward(c, workspace, workspace_bytes, stream,
+                          [&](Runner& R) { Walk{c, R, n}.run_u8(photos, off, h, w, feats); });
+}
+
 int inception_last_launch_count(const inception_ctx* c) { return c ? c->last_launches : 0; }
 
 int inception_resize(const float* x, int n, int H, int W, float* y, void* stream) {
     if (!x || !y) return fail(MIGAN_ERR_INVALID, "null x / y");
     if (int rc = check_images(n, H, W)) return rc;
     CUDA_TRY(comod::ck_launch(incep::ResizeK{x, y, H, W, kOS}, (int64_t)n * kOS * kOS, static_cast<ck_stream_t>(stream)));
+    return 0;
+}
+
+int inception_input_u8(const uint8_t* photos, const int64_t* off, const int* h, const int* w, int n, float* y, void* stream) {
+    if (!y) return fail(MIGAN_ERR_INVALID, "null y");
+    if (int rc = check_photos(photos, off, h, w, n)) return rc;
+    for (int k = 0; k < n; k += INCEPTION_U8_TABLE)
+        CUDA_TRY(comod::batch_launch<incep::ResizeU8K>(incep::u8_table(photos, off, h, w, k, std::min(INCEPTION_U8_TABLE, n - k),
+                                                                        y, kOS), static_cast<ck_stream_t>(stream)));
     return 0;
 }
 

@@ -8,6 +8,7 @@
 #pragma once
 #include <string.h>
 
+#include "../../include/inception_b200.h"
 #include "comod_kernels.cuh"
 
 namespace incep {
@@ -59,29 +60,91 @@ struct PackTf32K {     // items = NP*KP
 };
 
 // ---- input stage: F.interpolate(x, (299, 299), mode="bilinear", align_corners=False), then 2x - 1 ---------------
-// NCHW [n][3][H][W] -> NHWC [n][299][299][4], channel 3 zero (the first convolution reads 4-channel pixels).  Source
-// index as ATen computes it in fp32: max(scale * (o + 0.5) - 0.5, 0), scale = in / out.
+// One output pixel (oy, ox) of an H x W image whose channel c at (y, x) is px(c, y, x), as NHWC {v0, v1, v2, 0}: channel
+// 3 is zero (the first convolution reads 4-channel pixels).  Source index as ATen computes it in fp32:
+// max(scale * (o + 0.5) - 0.5, 0), scale = in / out.  Both input layouts below evaluate this one expression, so an image
+// gives the same bits through either when their loaders return the same floats.
+//
+// Every rounding is explicit (portable.cuh): these are the operations nvcc emits for the plain expression, FMAs where
+// it contracts, and the ones ATen's CPU kernel performs, so the emulation build gives torch's CPU result bit for bit.
+template <class Px>
+CK_HD f4 bilinear_pixel(const Px& px, int H, int W, int OS, int oy, int ox) {
+    const float sy = fmaxf(fma_rn(fdiv_rn((float)H, (float)OS), fadd_rn((float)oy, 0.5f), -0.5f), 0.f);
+    const float sx = fmaxf(fma_rn(fdiv_rn((float)W, (float)OS), fadd_rn((float)ox, 0.5f), -0.5f), 0.f);
+    const int y0 = (int)sy, x0 = (int)sx;
+    const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+    const float ly = fminf(fmaxf(fsub_rn(sy, (float)y0), 0.f), 1.f), lx = fminf(fmaxf(fsub_rn(sx, (float)x0), 0.f), 1.f);
+    const float hy = fsub_rn(1.f, ly), hx = fsub_rn(1.f, lx);
+    float v[3];
+    for (int c = 0; c < 3; ++c) {
+        const float a = fma_rn(hx, px(c, y0, x0), fmul_rn(lx, px(c, y0, x1)));
+        const float b = fma_rn(hx, px(c, y1, x0), fmul_rn(lx, px(c, y1, x1)));
+        v[c] = fma_rn(fma_rn(hy, a, fmul_rn(ly, b)), 2.f, -1.f);
+    }
+    return f4{v[0], v[1], v[2], 0.f};
+}
+
+// fp32 NCHW [n][3][H][W] -> NHWC [n][299][299][4].
 struct ResizeK {       // items = n*OS*OS
     const float* in; float* out; int H, W, OS;
+    struct Px {
+        const float* p; int64_t plane; int W;
+        CK_HD float operator()(int c, int y, int x) const { return p[c * plane + (int64_t)y * W + x]; }
+    };
     CK_HD void operator()(int64_t i) const {
         const int ox = (int)(i % OS); int64_t t = i / OS;
         const int oy = (int)(t % OS); const int64_t n = t / OS;
-        const float sy = fmaxf((float)H / (float)OS * ((float)oy + 0.5f) - 0.5f, 0.f);
-        const float sx = fmaxf((float)W / (float)OS * ((float)ox + 0.5f) - 0.5f, 0.f);
-        const int y0 = (int)sy, x0 = (int)sx;
-        const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
-        const float ly = fminf(fmaxf(sy - (float)y0, 0.f), 1.f), lx = fminf(fmaxf(sx - (float)x0, 0.f), 1.f);
-        const float hy = 1.f - ly, hx = 1.f - lx;
-        float v[3];
-        for (int c = 0; c < 3; ++c) {
-            const float* p = in + (n * 3 + c) * (int64_t)H * W;
-            const float a = hx * p[(int64_t)y0 * W + x0] + lx * p[(int64_t)y0 * W + x1];
-            const float b = hx * p[(int64_t)y1 * W + x0] + lx * p[(int64_t)y1 * W + x1];
-            v[c] = 2.f * (hy * a + ly * b) - 1.f;
-        }
-        st4(out + i * 4, f4{v[0], v[1], v[2], 0.f});
+        const int64_t plane = (int64_t)H * W;
+        st4(out + i * 4, bilinear_pixel(Px{in + n * 3 * plane, plane, W}, H, W, OS, oy, ox));
     }
 };
+
+// Decoded photos of any sizes, uint8 HWC RGB, packed one after the other in one buffer -> NHWC [n][299][299][4].  The
+// loader is torchvision's ToTensor, v / 255 rounded once, so each photo's pixels equal ResizeK's on ToTensor(photo).
+// Up to INCEPTION_U8_TABLE photos per launch; the table travels by value in the kernel parameter (batch_launch) with
+// each photo's byte offset, its size and the launch's output item prefix: photo k owns items [start[k], start[k + 1]).
+struct ResizeU8Batch {
+    int64_t start[INCEPTION_U8_TABLE + 1];
+    int64_t off[INCEPTION_U8_TABLE];
+    int h[INCEPTION_U8_TABLE], w[INCEPTION_U8_TABLE];
+    const uint8_t* photos; float* out;   // out: the first photo's output
+    int n, OS;
+};
+static_assert(sizeof(ResizeU8Batch) <= 4000, "the photo table must fit the classic 4 KB kernel parameter space");
+
+struct ResizeU8K {     // items = n*OS*OS
+    const ResizeU8Batch& b;
+    struct Px {
+        const uint8_t* p; int W;
+        CK_HD float operator()(int c, int y, int x) const {
+            return fdiv_rn((float)p[((int64_t)y * W + x) * 3 + c], 255.f);
+        }
+    };
+    CK_HD void operator()(int64_t i) const {
+        const int k = comod::find_request(b.start, b.n, i);
+        const int64_t j = i - b.start[k];
+        const int ox = (int)(j % b.OS), oy = (int)(j / b.OS);
+        st4(b.out + i * 4, bilinear_pixel(Px{b.photos + b.off[k], b.w[k]}, b.h[k], b.w[k], b.OS, oy, ox));
+    }
+};
+
+// The table of photos [first, first + n) of a batch (n <= INCEPTION_U8_TABLE), writing y at the first one's output.
+inline ResizeU8Batch u8_table(const uint8_t* photos, const int64_t* off, const int* h, const int* w, int first, int n,
+                              float* y, int OS) {
+    ResizeU8Batch b;
+    b.photos = photos;
+    b.out = y + (int64_t)first * OS * OS * 4;
+    b.n = n;
+    b.OS = OS;
+    b.start[0] = 0;
+    for (int k = 0; k < n; ++k) {
+        b.off[k] = off[first + k];
+        b.h[k] = h[first + k];
+        b.w[k] = w[first + k];
+        b.start[k + 1] = b.start[k] + (int64_t)OS * OS;
+    }
+    return b;
+}
 
 // ---- pools (3 x 3 windows) ------------------------------------------------------------------------------------------
 // kind 0: max, stride 2, no padding (max_pool2d(3, 2)); 1: average, stride 1, padding 1, count_include_pad=False (the

@@ -339,15 +339,17 @@ class RankWorker:
 # -- transport and merge --------------------------------------------------------------------------------------------
 
 def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[int, int]], width: int, device,
-                 group=None, extra: int = 0) -> List[ChunkResult]:
+                 group=None, extra: int = 0, lpips: bool = True) -> List[ChunkResult]:
     """One round's chunk results on rank 0, in chunk order ([] on the other ranks).  Every rank of `group` calls it
     once per round, with its chunk's result or None: it sends one [batch, width] float32 buffer (features, the LPIPS
     value, then `extra` per-image values; zero rows pad a short or absent chunk) in one gather.  `width` is
-    2 * 2048 + 1 + extra, or 2048 + 1 + extra without real features."""
+    2 * 2048 + 1 + extra, or 2048 + 1 + extra without real features.  With `lpips` False the chunks carry features
+    alone (`lpips` None) and there is no LPIPS column: `width` is then 2048 (+ extra), as `fid_score` sends."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     batch = chunks[0][1] - chunks[0][0]
     F = fid.FEATURES
-    lpips_at = width - 1 - extra
+    nl = 1 if lpips else 0
+    lpips_at = width - nl - extra                         # the LPIPS column, when sent; the extra values follow it
     fake_at = lpips_at - F                                # real features, when sent, occupy [0, F)
     buf = torch.zeros((batch, width), dtype=torch.float32, device=device)
     if result is not None:
@@ -355,9 +357,10 @@ def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[i
         if fake_at:
             buf[:c, :F] = result.real
         buf[:c, fake_at:lpips_at] = result.fake
-        buf[:c, lpips_at] = result.lpips
+        if lpips:
+            buf[:c, lpips_at] = result.lpips
         if extra:
-            buf[:c, lpips_at + 1:] = result.extra
+            buf[:c, lpips_at + nl:] = result.extra
     bufs = [torch.empty_like(buf) for _ in range(world)] if rank == 0 else None
     dist.gather(buf, bufs, dst=0, group=group)
     if rank != 0:
@@ -368,8 +371,8 @@ def gather_round(result: Optional[ChunkResult], r: int, chunks: Sequence[Tuple[i
         if j is not None:
             a, b = chunks[j]
             c = b - a
-            out.append(ChunkResult(j, a, got[:c, :F] if fake_at else None, got[:c, fake_at:lpips_at], got[:c, lpips_at],
-                                   got[:c, lpips_at + 1:] if extra else None))
+            out.append(ChunkResult(j, a, got[:c, :F] if fake_at else None, got[:c, fake_at:lpips_at],
+                                   got[:c, lpips_at] if lpips else None, got[:c, lpips_at + nl:] if extra else None))
     return out
 
 

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, List, NamedTuple, Optional, Tuple, Union
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -41,6 +41,10 @@ SYMBOLS = [
     ("inception_features", ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     ("inception_last_launch_count", ctypes.c_int, [ctypes.c_void_p]),
+    ("inception_workspace_bytes_u8", ctypes.c_size_t, [ctypes.c_void_p, ctypes.c_int]),
+    ("inception_features_u8", ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int] + [ctypes.c_void_p] * 2 +
+     [ctypes.c_size_t, ctypes.c_void_p]),
+    ("inception_input_u8", ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] + [ctypes.c_void_p] * 2),
     ("inception_launch_plan", ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                              ctypes.c_char_p, ctypes.c_int]),
     ("inception_resize", ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
@@ -122,6 +126,7 @@ class InceptionV3(_convnet.Network):
         state = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in _load_weights(weights).items()
                  if not k.endswith("num_batches_tracked")}
         self._set_state(lib(), "inception", state)
+        self._staged: Dict[torch.device, Tuple[torch.Tensor, torch.cuda.Event]] = {}   # features_u8's pinned buffers
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
@@ -140,6 +145,62 @@ class InceptionV3(_convnet.Network):
                 _abi.check(eng.lib.inception_features(eng.handle, x.data_ptr(), n, H, W, feats.data_ptr(), ws.data_ptr(),
                                                       ws.numel(), torch.cuda.current_stream(x.device).cuda_stream))
         return [feats.view(n, FEATURES, 1, 1)]
+
+    @torch.no_grad()
+    def features_u8(self, photos: Sequence[np.ndarray], device=None) -> torch.Tensor:
+        """Features [n, 2048] (CUDA float32, on `device` or the current CUDA device) of decoded photos: host uint8
+        [H, W, 3] arrays of any sizes, such as `np.array(Image.open(p).convert("RGB"))`.  Row i equals
+        `self(ToTensor(photos[i])[None])[0]` bit for bit, for any batch and any mix of sizes in it.
+
+        The photos are packed into a pinned staging buffer and reach the device in one copy on the current stream; the
+        buffer is kept for the next call (it grows to the largest call's bytes) and is refilled only once that copy is
+        done."""
+        arrays = [np.ascontiguousarray(p) for p in photos]
+        for i, a in enumerate(arrays):
+            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
+                raise ValueError("features_u8: photo %d is %s %s; expected uint8 [H, W, 3] with H, W >= 1"
+                                 % (i, a.dtype, a.shape))
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("migan_b200.fid.InceptionV3 runs on H100 (sm_90a) only; got device %s. There is no CPU "
+                               "path." % device)
+        n = len(arrays)
+        feats = torch.empty((n, FEATURES), dtype=torch.float32, device=device)
+        if n == 0:
+            return feats
+        sizes = np.array([a.nbytes for a in arrays], dtype=np.int64)
+        off = np.zeros(n, dtype=np.int64)
+        np.cumsum(sizes[:-1], out=off[1:])
+        h = np.array([a.shape[0] for a in arrays], dtype=np.int32)
+        w = np.array([a.shape[1] for a in arrays], dtype=np.int32)
+        total = int(sizes.sum())
+        with torch.cuda.device(device):
+            eng = self._engine(device)
+            stream = torch.cuda.current_stream(device)
+            host, copied = self._staging(device, total)
+            flat = host.numpy()
+            for a, o in zip(arrays, off):
+                flat[o:o + a.nbytes] = a.reshape(-1)
+            photos_d = torch.empty(total, dtype=torch.uint8, device=device)
+            photos_d.copy_(host[:total], non_blocking=True)
+            copied.record(stream)
+            ws = eng._workspace.get(("u8", n), lambda: eng.lib.inception_workspace_bytes_u8(eng.handle, n), device)
+            _abi.check(eng.lib.inception_features_u8(eng.handle, photos_d.data_ptr(), off.ctypes.data, h.ctypes.data,
+                                                     w.ctypes.data, n, feats.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                     stream.cuda_stream))
+        return feats
+
+    def _staging(self, device, nbytes: int) -> Tuple[torch.Tensor, torch.cuda.Event]:
+        """The pinned staging buffer of `device`, at least nbytes long, once the copy that last read it is done, and the
+        event to record after the copy that reads it next."""
+        buf, done = self._staged.get(device, (None, None))
+        if done is not None:
+            done.synchronize()
+        if buf is None or buf.numel() < nbytes:
+            buf = None
+            buf = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+        self._staged[device] = (buf, torch.cuda.Event())
+        return self._staged[device]
 
     def launch_plan(self, n: int, H: int, W: int) -> List[str]:
         """The forward's launches for n images of H x W, one line each."""
