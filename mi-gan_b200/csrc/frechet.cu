@@ -1,14 +1,12 @@
 // C ABI of the Fréchet distance (include/inception_b200.h): fid_stats_mean_cov, fid_frechet_workspace_bytes and
 // fid_frechet_distance.  Argument checks, workspace layout, the eigensolver's sweep loop and the launches; the
-// arithmetic is frechet_kernels.cuh's.  The kernels here run its phases with a block's threads at once, and the
-// emulation build (MIGAN_EMULATE) runs the same phases with the threads of a block in turn.
+// arithmetic is frechet_kernels.cuh's.  Each block kernel is one body over portable.cuh's block layer: the kernel runs
+// it with a block's threads at once, and the emulation build (MIGAN_EMULATE) runs the same body on the host.
 //
 // Workspace (N = dim rounded up to a multiple of 64, each region 256-byte aligned): A, V, B, W (N x N doubles each),
 // the pair factors (N / 64 of 64 x 64), sqrt(d) (N), the column partials of the norm (2N), 8 scalars.
 #include <math.h>
 #include <string.h>
-
-#include <vector>
 
 #include "../../include/inception_b200.h"
 #include "abi_error.h"
@@ -27,114 +25,83 @@ constexpr size_t kPairSmem = (2 * kTileDoubles + 4 * frechet::kB) * sizeof(doubl
 constexpr size_t kUpdateSmem = 3 * kTileDoubles * sizeof(double);
 constexpr size_t kGemmSmem = 2 * kTileDoubles * sizeof(double);
 
+// Block k of the pair kernel: the subproblem of block pair k, rotated until an inner step rotates nothing.
+template <class B>
+CK_D void pair_block(const B& blk, const frechet::PairArgs& a, int k, double* smem) {
+    double* S = smem;
+    double* J = S + kTileDoubles;
+    double* cs = J + kTileDoubles;
+    blk.each([&](int t) { a.load(k, t, S, J); });
+    blk.sync();
+    for (int sweep = 0; sweep < frechet::kMaxInner; ++sweep) {
+        int rotated = 0;
+        for (int step = 0; step < kG - 1; ++step) {
+            if (!blk.any([&](int t) { return t < frechet::kB ? a.rot(step, t, S, cs) : 0; })) continue;
+            blk.each([&](int t) { a.apply(step, t, S, J, cs); });
+            rotated = 1;
+            blk.sync();
+        }
+        if (!rotated) break;
+    }
+    blk.each([&](int t) { a.store(k, t, S, J); });
+}
+
+template <class B>
+CK_D void update_block(const B& blk, const frechet::UpdateArgs& a, int64_t b, double* smem) {
+    double* X = smem;
+    double* P = X + kTileDoubles;
+    double* R = P + kTileDoubles;
+    blk.each([&](int t) { a.load(b, t, X, P, R); });
+    blk.sync();
+    frechet::Accs<B> c;
+    blk.each([&](int t) { a.right(t, c[t], X, P); });
+    blk.sync();
+    blk.each([&](int t) { a.after_right(b, t, c[t], X); });
+    if (b >= a.tilesA) return;
+    blk.sync();
+    blk.each([&](int t) { a.left(b, t, c[t], X, R); });
+}
+
+template <class B>
+CK_D void gemm_block(const B& blk, const frechet::GemmArgs& a, int64_t b, double* smem) {
+    double* Xs = smem;
+    double* Ys = Xs + kTileDoubles;
+    frechet::Accs<B> c;
+    frechet::panel_product(blk, c, a.N, Xs, Ys, a, b);
+    blk.each([&](int t) { a.store(b, t, c[t]); });
+}
+
+int64_t gemm_blocks(const frechet::GemmArgs& a) { return (int64_t)(a.N / kG) * (a.N / kG); }
+
 #ifdef MIGAN_EMULATE
 int pair_launch(const frechet::PairArgs& a, int blocks, ck_stream_t) {
-#pragma omp parallel for schedule(dynamic)
-    for (int k = 0; k < blocks; ++k) {
-        std::vector<double> S(kTileDoubles), J(kTileDoubles), cs(4 * frechet::kB);
-        for (int t = 0; t < kThreads; ++t) a.load(k, t, S.data(), J.data());
-        for (int sweep = 0; sweep < frechet::kMaxInner; ++sweep) {
-            int rotated = 0;
-            for (int step = 0; step < kG - 1; ++step) {
-                int go = 0;
-                for (int t = 0; t < frechet::kB; ++t) go |= a.rot(step, t, S.data(), cs.data());
-                if (!go) continue;
-                for (int t = 0; t < kThreads; ++t) a.apply(step, t, S.data(), J.data(), cs.data());
-                rotated = 1;
-            }
-            if (!rotated) break;
-        }
-        for (int t = 0; t < kThreads; ++t) a.store(k, t, S.data(), J.data());
-    }
-    return 0;
+    return ck_blocks<kThreads>(blocks, kPairSmem,
+                               [&](auto& blk, int64_t k, void* smem) { pair_block(blk, a, (int)k, (double*)smem); });
 }
 
 int update_launch(const frechet::UpdateArgs& a, ck_stream_t) {
-    const int64_t blocks = a.blocks();
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> X(kTileDoubles), P(kTileDoubles), R(kTileDoubles);
-        std::vector<frechet::Acc> c(kThreads);
-        for (int t = 0; t < kThreads; ++t) a.load(b, t, X.data(), P.data(), R.data());
-        for (int t = 0; t < kThreads; ++t) a.right(t, c[t], X.data(), P.data());
-        for (int t = 0; t < kThreads; ++t) a.after_right(b, t, c[t], X.data());
-        if (b >= a.tilesA) continue;
-        for (int t = 0; t < kThreads; ++t) a.left(b, t, c[t], X.data(), R.data());
-    }
-    return 0;
+    return ck_blocks<kThreads>(a.blocks(), kUpdateSmem,
+                               [&](auto& blk, int64_t b, void* smem) { update_block(blk, a, b, (double*)smem); });
 }
 
 int gemm_launch(const frechet::GemmArgs& a, ck_stream_t) {
-    const int64_t blocks = (int64_t)(a.N / kG) * (a.N / kG);
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> Xs(kTileDoubles), Ys(kTileDoubles);
-        std::vector<frechet::Acc> c(kThreads);
-        for (int t = 0; t < kThreads; ++t) frechet::acc_zero(c[t]);
-        for (int k0 = 0; k0 < a.N; k0 += kG) {
-            for (int t = 0; t < kThreads; ++t) a.stage(b, t, k0, Xs.data(), Ys.data());
-            for (int t = 0; t < kThreads; ++t) a.product(t, c[t], Xs.data(), Ys.data());
-        }
-        for (int t = 0; t < kThreads; ++t) a.store(b, t, c[t]);
-    }
-    return 0;
+    return ck_blocks<kThreads>(gemm_blocks(a), kGemmSmem,
+                               [&](auto& blk, int64_t b, void* smem) { gemm_block(blk, a, b, (double*)smem); });
 }
 #else
 __global__ void __launch_bounds__(kThreads) frechet_pair_kernel(const __grid_constant__ frechet::PairArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* S = smem;
-    double* J = S + kTileDoubles;
-    double* cs = J + kTileDoubles;
-    const int k = blockIdx.x, t = threadIdx.x;
-    a.load(k, t, S, J);
-    __syncthreads();
-    for (int sweep = 0; sweep < frechet::kMaxInner; ++sweep) {
-        int rotated = 0;
-        for (int step = 0; step < kG - 1; ++step) {
-            const int go = t < frechet::kB ? a.rot(step, t, S, cs) : 0;
-            if (!__syncthreads_or(go)) continue;   // the same answer in every thread: the branch is uniform
-            a.apply(step, t, S, J, cs);
-            rotated = 1;
-            __syncthreads();
-        }
-        if (!rotated) break;
-    }
-    a.store(k, t, S, J);
+    pair_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) frechet_update_kernel(const __grid_constant__ frechet::UpdateArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* X = smem;
-    double* P = X + kTileDoubles;
-    double* R = P + kTileDoubles;
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    a.load(b, t, X, P, R);
-    __syncthreads();
-    frechet::Acc c;
-    a.right(t, c, X, P);
-    __syncthreads();
-    a.after_right(b, t, c, X);
-    if (b >= a.tilesA) return;
-    __syncthreads();
-    a.left(b, t, c, X, R);
+    update_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) frechet_gemm_kernel(const __grid_constant__ frechet::GemmArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* Xs = smem;
-    double* Ys = Xs + kTileDoubles;
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    frechet::Acc c;
-    frechet::acc_zero(c);
-    for (int k0 = 0; k0 < a.N; k0 += kG) {
-        a.stage(b, t, k0, Xs, Ys);
-        __syncthreads();
-        a.product(t, c, Xs, Ys);
-        __syncthreads();
-    }
-    a.store(b, t, c);
+    gemm_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 int pair_launch(const frechet::PairArgs& a, int blocks, ck_stream_t s) {
@@ -151,7 +118,7 @@ int update_launch(const frechet::UpdateArgs& a, ck_stream_t s) {
 
 int gemm_launch(const frechet::GemmArgs& a, ck_stream_t s) {
     if (int e = set_smem(frechet_gemm_kernel, kGemmSmem)) return e;
-    frechet_gemm_kernel<<<(unsigned)((a.N / kG) * (a.N / kG)), kThreads, kGemmSmem, s>>>(a);
+    frechet_gemm_kernel<<<(unsigned)gemm_blocks(a), kThreads, kGemmSmem, s>>>(a);
     return (int)cudaGetLastError();
 }
 #endif

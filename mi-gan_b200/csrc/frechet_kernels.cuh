@@ -1,6 +1,6 @@
-// Arithmetic of the Fréchet distance (frechet.cu), written once for the device kernels and for the emulation build's
-// host loops, the way metrics_kernels.cuh is: the kernels run a phase with the threads of a block at once and
-// __syncthreads() between phases; under MIGAN_EMULATE the same phase functions run with the threads of a block in turn.
+// Arithmetic of the Fréchet distance (frechet.cu), written once for the device kernels and for the emulation build, the
+// way metrics_kernels.cuh is: a block kernel's body (portable.cuh's block layer) calls these phase functions for each
+// thread between its barriers, and the same body runs in both builds.
 // Everything is float64, there are no atomics, and every sum has a fixed order, so a call returns the same bytes on
 // every run.
 //
@@ -37,6 +37,16 @@ constexpr double kEps = 1.1102230246251565e-16;   // 2^-53
 constexpr int kTileDoubles = kG * kLd;
 
 CK_HD double dsqrt(double x) { return sqrt(x); }
+
+// One side's feature rows, fp32 or fp64 as stored, promoted exactly to fp64.
+struct Rows {
+    const void* p; int d, fp64;
+
+    CK_HD double x(int64_t row, int c) const {
+        const int64_t e = row * d + c;
+        return fp64 ? static_cast<const double*>(p)[e] : (double)static_cast<const float*>(p)[e];
+    }
+};
 CK_HD double dabs(double x) { return fabs(x); }
 
 // Round r (0 <= r < m - 1) of the circle pairing of m (even) players: pair k of m / 2, returned with a < b.
@@ -208,6 +218,23 @@ inline void tile_mma(Acc& c, int t, const double* X, int xr, int xc, const doubl
         }
 }
 #endif
+
+// A block's accumulators: one Acc per thread.
+template <class B>
+using Accs = typename B::template Local<Acc>;
+
+// c = the product of the panels over the K extent, kG columns at a time: a.stage(tile..., t, k0, Xs, Ys) writes thread
+// t's share of the panels Xs[k][x], Ys[k][x] of columns k0 .. k0 + kG, and the tile product adds them in k order.
+template <class B, class Args, class... Tile>
+CK_D void panel_product(const B& blk, Accs<B>& c, int K, double* Xs, double* Ys, const Args& a, Tile... tile) {
+    blk.each([&](int t) { acc_zero(c[t]); });
+    for (int k0 = 0; k0 < K; k0 += kG) {
+        blk.each([&](int t) { a.stage(tile..., t, k0, Xs, Ys); });
+        blk.sync();
+        blk.each([&](int t) { tile_mma(c[t], t, Xs, 1, kLd, Ys); });
+        blk.sync();
+    }
+}
 
 // ---- pair kernel ----------------------------------------------------------------------------------------------------
 // Block pair k of round `round`.  Shared memory: S and K = J - I (kG x kLd each), then kB rotations (c, s, t, c - 1).
@@ -402,7 +429,6 @@ struct GemmArgs {
             Ys[kk * kLd + x] = Y[(int64_t)(k0 + kk) * N + bj * kG + x];
         }
     }
-    CK_HD void product(int t, Acc& c, const double* Xs, const double* Ys) const { tile_mma(c, t, Xs, 1, kLd, Ys); }
     CK_HD void store(int64_t b, int t, const Acc& c) const {
         const int tn = N / kG, bi = (int)(b / tn), bj = (int)(b % tn);
         const int64_t r = (int64_t)bi * kG + acc_row(t);

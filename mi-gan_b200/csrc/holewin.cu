@@ -10,7 +10,8 @@
 // load when the chunk lies inside the row's bytes, byte loads at the ends), and a hole marks the cell's byte in shared
 // memory; the block then writes one byte per cell, so every cell byte is written exactly once and needs no clearing.
 // The hole test is prepost.cuh's (mask_channel + known_value), the same as the pre- and post-processing's.
-// The emulation build (tests/emul/build_emul.py) runs the same block functions with the threads of a block in turn.
+// The kernel is one body over portable.cuh's block layer, which the emulation build (tests/emul/build_emul.py) runs on
+// the host.
 #include "prepost.cuh"
 #include "abi_error.h"
 
@@ -104,27 +105,27 @@ CK_D void cells_block_store(const CellsBatch& b, const CellsBlock& g, int tid, i
     for (int t = tid; t < g.ncx; t += nthr) out[t] = flags[t];
 }
 
+template <class B>
+CK_D void hole_cells_block(const B& blk, const CellsBatch& b, int64_t blk_idx, uint8_t* flags, uint8_t* cells) {
+    const CellsBlock g = cells_block(b, blk_idx);
+    blk.each([&](int tid) {
+        for (int t = tid; t < g.ncx; t += HC_THREADS) flags[t] = 0;
+    });
+    blk.sync();
+    blk.each([&](int tid) { cells_block_scan(b, g, tid, HC_THREADS, flags); });
+    blk.sync();
+    blk.each([&](int tid) { cells_block_store(b, g, tid, HC_THREADS, flags, cells); });
+}
+
 #ifdef MIGAN_EMULATE
 inline int cells_launch(const CellsBatch& b, uint8_t* cells, ck_stream_t) {
-#pragma omp parallel for schedule(static)
-    for (int64_t blk = 0; blk < b.block_start[b.n]; ++blk) {
-        uint8_t flags[HC_MAX_S];
-        const CellsBlock g = cells_block(b, blk);
-        for (int t = 0; t < g.ncx; ++t) flags[t] = 0;
-        for (int tid = 0; tid < HC_THREADS; ++tid) cells_block_scan(b, g, tid, HC_THREADS, flags);
-        for (int tid = 0; tid < HC_THREADS; ++tid) cells_block_store(b, g, tid, HC_THREADS, flags, cells);
-    }
-    return 0;
+    return ck_blocks<HC_THREADS>(b.block_start[b.n], HC_MAX_S,
+                                 [&](auto& blk, int64_t k, void* flags) { hole_cells_block(blk, b, k, (uint8_t*)flags, cells); });
 }
 #else
 __global__ void __launch_bounds__(HC_THREADS) hole_cells_kernel(const __grid_constant__ CellsBatch b, uint8_t* cells) {
     __shared__ uint8_t flags[HC_MAX_S];
-    const CellsBlock g = cells_block(b, blockIdx.x);
-    for (int t = threadIdx.x; t < g.ncx; t += HC_THREADS) flags[t] = 0;
-    __syncthreads();
-    cells_block_scan(b, g, threadIdx.x, HC_THREADS, flags);
-    __syncthreads();
-    cells_block_store(b, g, threadIdx.x, HC_THREADS, flags, cells);
+    hole_cells_block(DeviceBlock(), b, blockIdx.x, flags, cells);
 }
 inline cudaError_t cells_launch(const CellsBatch& b, uint8_t* cells, ck_stream_t s) {
     hole_cells_kernel<<<(unsigned)b.block_start[b.n], HC_THREADS, 0, s>>>(b, cells);

@@ -1,15 +1,13 @@
 // C ABI of the Inception discriminative scores (include/inception_b200.h): ids_workspace_bytes and ids_scores.
-// Argument checks, workspace layout, the finite Newton loop and the launches; the arithmetic is ids_kernels.cuh's.  The
-// kernels here run its phases with a block's threads at once, and the emulation build (MIGAN_EMULATE) runs the same
-// phases with the threads of a block in turn.
+// Argument checks, workspace layout, the finite Newton loop and the launches; the arithmetic is ids_kernels.cuh's.  Each
+// block kernel is one body over portable.cuh's block layer, run with a block's threads at once on the device and on the
+// host in the emulation build (MIGAN_EMULATE).
 //
 // Workspace (M = 2n rows, Dp = dim + 1 rounded up to 64, H = chunks of 256 rows; each region 256-byte aligned):
 // b, b~, g, r (Dp each), o, ob (M), the active list (M ints), the chunk partials (3H) and offsets (H ints), the margin
 // lane partials (32 M), the gradient's column partials (2 H Dp), G (Dp x Dp), 16 status scalars.
 #include <math.h>
 #include <string.h>
-
-#include <vector>
 
 #include "../../include/inception_b200.h"
 #include "abi_error.h"
@@ -26,184 +24,157 @@ constexpr int kMaxIter = 100;
 constexpr double kGradTol = 1e-12;
 static_assert(ids::kMaxDim == IDS_MAX_DIM, "one cap");
 constexpr size_t kTileSmem = 2 * kTileDoubles * sizeof(double);
+constexpr size_t kDiagSmem = kTileDoubles * sizeof(double);
 constexpr size_t kLineSmem = 3 * kThreads * sizeof(double);
 
-#ifdef MIGAN_EMULATE
-int gram_launch(const ids::GramArgs& a, ck_stream_t) {
-    const int64_t blocks = a.tiles();
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> Xs(kTileDoubles), Ys(kTileDoubles);
-        std::vector<ids::Acc> c(kThreads);
-        for (int t = 0; t < kThreads; ++t) frechet::acc_zero(c[t]);
-        for (int k0 = 0, count = a.count(); k0 < count; k0 += kG) {
-            for (int t = 0; t < kThreads; ++t) a.stage(b, t, k0, Xs.data(), Ys.data());
-            for (int t = 0; t < kThreads; ++t) a.product(t, c[t], Xs.data(), Ys.data());
-        }
-        for (int t = 0; t < kThreads; ++t) a.store(b, t, c[t]);
-    }
-    return 0;
+template <class B>
+CK_D void gram_block(const B& blk, const ids::GramArgs& a, int64_t b, double* smem) {
+    double* Xs = smem;
+    double* Ys = Xs + kTileDoubles;
+    ids::Accs<B> c;
+    frechet::panel_product(blk, c, a.count(), Xs, Ys, a, b);
+    blk.each([&](int t) { a.store(b, t, c[t]); });
 }
 
-int diag_launch(const ids::CholArgs& a, ck_stream_t) {
-    std::vector<double> S(kTileDoubles);
-    for (int t = 0; t < kThreads; ++t) a.diag_load(t, S.data());
+template <class B>
+CK_D void diag_block(const B& blk, const ids::CholArgs& a, double* S) {
+    blk.each([&](int t) { a.diag_load(t, S); });
+    blk.sync();
     for (int j = 0; j < kG; ++j) {
-        for (int t = 0; t < kThreads; ++t) a.diag_scale(j, t, S.data());
-        for (int t = 0; t < kThreads; ++t) a.diag_update(j, t, S.data());
+        blk.each([&](int t) { a.diag_scale(j, t, S); });
+        blk.sync();
+        blk.each([&](int t) { a.diag_update(j, t, S); });
+        blk.sync();
     }
-    for (int t = 0; t < kThreads; ++t) a.diag_store(t, S.data());
-    return 0;
+    blk.each([&](int t) { a.diag_store(t, S); });
 }
 
-int panel_launch(const ids::CholArgs& a, int blocks, ck_stream_t) {
-#pragma omp parallel for schedule(dynamic)
-    for (int b = 0; b < blocks; ++b) {
-        std::vector<double> L(kTileDoubles), B(kTileDoubles);
-        for (int t = 0; t < kThreads; ++t) a.panel_load(b, t, L.data(), B.data());
-        for (int t = 0; t < kThreads; ++t) a.panel_solve(t, L.data(), B.data());
-        for (int t = 0; t < kThreads; ++t) a.panel_store(b, t, B.data());
+template <class B>
+CK_D void panel_block(const B& blk, const ids::CholArgs& a, int b, double* smem) {
+    double* L = smem;
+    double* P = L + kTileDoubles;
+    blk.each([&](int t) { a.panel_load(b, t, L, P); });
+    blk.sync();
+    blk.each([&](int t) { a.panel_solve(t, L, P); });
+    blk.sync();
+    blk.each([&](int t) { a.panel_store(b, t, P); });
+}
+
+template <class B>
+CK_D void trail_block(const B& blk, const ids::CholArgs& a, int64_t b, double* smem) {
+    double* Xs = smem;
+    double* Ys = Xs + kTileDoubles;
+    blk.each([&](int t) { a.trail_stage(b, t, Xs, Ys); });
+    blk.sync();
+    ids::Accs<B> c;
+    blk.each([&](int t) {
+        a.trail_product(b, t, c[t], Xs, Ys);
+        a.trail_store(b, t, c[t]);
+    });
+}
+
+template <class B>
+CK_D void solve_block(const B& blk, const ids::SolveArgs& a, double* smem) {
+    double* z = smem;
+    double* w = z + a.Dp;
+    blk.each([&](int t) { a.load(t, z); });
+    blk.sync();
+    for (int j = 0; j < a.Dp; ++j) {
+        blk.each([&](int t) { a.forward(j, t, z, w); });
+        blk.sync();
     }
-    return 0;
-}
-
-int trail_launch(const ids::CholArgs& a, int64_t blocks, ck_stream_t) {
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> Xs(kTileDoubles), Ys(kTileDoubles);
-        std::vector<ids::Acc> c(kThreads);
-        for (int t = 0; t < kThreads; ++t) a.trail_stage(b, t, Xs.data(), Ys.data());
-        for (int t = 0; t < kThreads; ++t) a.trail_product(b, t, c[t], Xs.data(), Ys.data());
-        for (int t = 0; t < kThreads; ++t) a.trail_store(b, t, c[t]);
+    for (int j = a.Dp - 1; j >= 0; --j) {
+        blk.each([&](int t) { a.backward(j, t, w); });
+        blk.sync();
     }
-    return 0;
 }
 
-int solve_launch(const ids::SolveArgs& a, ck_stream_t) {
-    std::vector<double> z(a.Dp), w(a.Dp);
-    for (int t = 0; t < kThreads; ++t) a.load(t, z.data());
-    for (int j = 0; j < a.Dp; ++j)
-        for (int t = 0; t < kThreads; ++t) a.forward(j, t, z.data(), w.data());
-    for (int j = a.Dp - 1; j >= 0; --j)
-        for (int t = 0; t < kThreads; ++t) a.backward(j, t, w.data());
-    return 0;
-}
-
-int line_launch(const ids::LineArgs& a, ck_stream_t) {
+template <class B>
+CK_D void line_block(const B& blk, const ids::LineArgs& a, double* part) {
     if (a.scal[ids::kMismatch] == 0.0) {
-        a.scal[ids::kStep] = 1.0;
-        return 0;
+        blk.each([&](int t) {
+            if (t == 0) a.scal[ids::kStep] = 1.0;
+        });
+        return;
     }
-    std::vector<double> part(3 * kThreads);
     double s[3];
-    for (int t = 0; t < kThreads; ++t) a.dir_part(t, part.data());
-    ids::sum_parts(part.data(), s);
+    blk.each([&](int t) { a.dir_part(t, part); });
+    blk.sync();
+    ids::sum_parts(part, s);
+    blk.sync();
     ids::LineSearch ls;
     ls.start(s);
     for (;;) {
-        for (int t = 0; t < kThreads; ++t) a.row_part(t, ls.eval_lo(), ls.hi, ls.mid(), part.data());
-        ids::sum_parts(part.data(), s);
-        if (ls.next(s)) break;
+        blk.each([&](int t) { a.row_part(t, ls.eval_lo(), ls.hi, ls.mid(), part); });
+        blk.sync();
+        ids::sum_parts(part, s);
+        blk.sync();
+        if (ls.next(s)) break;   // every thread takes the same decision from the same sums
     }
-    a.scal[ids::kStep] = ls.t;
-    return 0;
+    blk.each([&](int t) {
+        if (t == 0) a.scal[ids::kStep] = ls.t;
+    });
+}
+
+size_t solve_smem(const ids::SolveArgs& a) { return 2 * (size_t)a.Dp * sizeof(double); }
+
+#ifdef MIGAN_EMULATE
+int gram_launch(const ids::GramArgs& a, ck_stream_t) {
+    return ck_blocks<kThreads>(a.tiles(), kTileSmem,
+                               [&](auto& blk, int64_t b, void* smem) { gram_block(blk, a, b, (double*)smem); });
+}
+
+int diag_launch(const ids::CholArgs& a, ck_stream_t) {
+    return ck_blocks<kThreads>(1, kDiagSmem, [&](auto& blk, int64_t, void* smem) { diag_block(blk, a, (double*)smem); });
+}
+
+int panel_launch(const ids::CholArgs& a, int blocks, ck_stream_t) {
+    return ck_blocks<kThreads>(blocks, kTileSmem,
+                               [&](auto& blk, int64_t b, void* smem) { panel_block(blk, a, (int)b, (double*)smem); });
+}
+
+int trail_launch(const ids::CholArgs& a, int64_t blocks, ck_stream_t) {
+    return ck_blocks<kThreads>(blocks, kTileSmem,
+                               [&](auto& blk, int64_t b, void* smem) { trail_block(blk, a, b, (double*)smem); });
+}
+
+int solve_launch(const ids::SolveArgs& a, ck_stream_t) {
+    return ck_blocks<kThreads>(1, solve_smem(a),
+                               [&](auto& blk, int64_t, void* smem) { solve_block(blk, a, (double*)smem); });
+}
+
+int line_launch(const ids::LineArgs& a, ck_stream_t) {
+    return ck_blocks<kThreads>(1, kLineSmem, [&](auto& blk, int64_t, void* smem) { line_block(blk, a, (double*)smem); });
 }
 #else
 __global__ void __launch_bounds__(kThreads) ids_gram_kernel(const __grid_constant__ ids::GramArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* Xs = smem;
-    double* Ys = Xs + kTileDoubles;
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    ids::Acc c;
-    frechet::acc_zero(c);
-    for (int k0 = 0, count = a.count(); k0 < count; k0 += kG) {
-        a.stage(b, t, k0, Xs, Ys);
-        __syncthreads();
-        a.product(t, c, Xs, Ys);
-        __syncthreads();
-    }
-    a.store(b, t, c);
+    gram_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) ids_diag_kernel(const __grid_constant__ ids::CholArgs a) {
     extern __shared__ __align__(16) double smem[];
-    const int t = threadIdx.x;
-    a.diag_load(t, smem);
-    __syncthreads();
-    for (int j = 0; j < kG; ++j) {
-        a.diag_scale(j, t, smem);
-        __syncthreads();
-        a.diag_update(j, t, smem);
-        __syncthreads();
-    }
-    a.diag_store(t, smem);
+    diag_block(DeviceBlock(), a, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) ids_panel_kernel(const __grid_constant__ ids::CholArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* L = smem;
-    double* B = L + kTileDoubles;
-    const int b = blockIdx.x, t = threadIdx.x;
-    a.panel_load(b, t, L, B);
-    __syncthreads();
-    a.panel_solve(t, L, B);
-    __syncthreads();
-    a.panel_store(b, t, B);
+    panel_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) ids_trail_kernel(const __grid_constant__ ids::CholArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* Xs = smem;
-    double* Ys = Xs + kTileDoubles;
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    a.trail_stage(b, t, Xs, Ys);
-    __syncthreads();
-    ids::Acc c;
-    a.trail_product(b, t, c, Xs, Ys);
-    a.trail_store(b, t, c);
+    trail_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) ids_solve_kernel(const __grid_constant__ ids::SolveArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* z = smem;
-    double* w = z + a.Dp;
-    const int t = threadIdx.x;
-    a.load(t, z);
-    __syncthreads();
-    for (int j = 0; j < a.Dp; ++j) {
-        a.forward(j, t, z, w);
-        __syncthreads();
-    }
-    for (int j = a.Dp - 1; j >= 0; --j) {
-        a.backward(j, t, w);
-        __syncthreads();
-    }
+    solve_block(DeviceBlock(), a, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) ids_line_kernel(const __grid_constant__ ids::LineArgs a) {
     extern __shared__ __align__(16) double smem[];
-    const int t = threadIdx.x;
-    if (a.scal[ids::kMismatch] == 0.0) {
-        if (t == 0) a.scal[ids::kStep] = 1.0;
-        return;
-    }
-    double s[3];
-    a.dir_part(t, smem);
-    __syncthreads();
-    ids::sum_parts(smem, s);
-    __syncthreads();
-    ids::LineSearch ls;
-    ls.start(s);
-    for (;;) {
-        a.row_part(t, ls.eval_lo(), ls.hi, ls.mid(), smem);
-        __syncthreads();
-        ids::sum_parts(smem, s);
-        __syncthreads();
-        if (ls.next(s)) break;   // every thread takes the same decision from the same sums
-    }
-    if (t == 0) a.scal[ids::kStep] = ls.t;
+    line_block(DeviceBlock(), a, smem);
 }
 
 int gram_launch(const ids::GramArgs& a, ck_stream_t s) {
@@ -213,7 +184,7 @@ int gram_launch(const ids::GramArgs& a, ck_stream_t s) {
 }
 
 int diag_launch(const ids::CholArgs& a, ck_stream_t s) {
-    ids_diag_kernel<<<1, kThreads, kTileDoubles * sizeof(double), s>>>(a);
+    ids_diag_kernel<<<1, kThreads, kDiagSmem, s>>>(a);
     return (int)cudaGetLastError();
 }
 
@@ -230,7 +201,7 @@ int trail_launch(const ids::CholArgs& a, int64_t blocks, ck_stream_t s) {
 }
 
 int solve_launch(const ids::SolveArgs& a, ck_stream_t s) {
-    const size_t bytes = 2 * (size_t)a.Dp * sizeof(double);
+    const size_t bytes = solve_smem(a);
     if (int e = set_smem(ids_solve_kernel, bytes)) return e;
     ids_solve_kernel<<<1, kThreads, bytes, s>>>(a);
     return (int)cudaGetLastError();

@@ -22,6 +22,7 @@
 namespace ids {
 
 using frechet::Acc;
+using frechet::Accs;
 using frechet::acc_col;
 using frechet::acc_row;
 using frechet::kG;
@@ -289,9 +290,6 @@ struct GramArgs {
             Xs[kk * kLd + x] = u;
             Ys[kk * kLd + x] = v;
         }
-    }
-    CK_HD void product(int t, Acc& c, const double* Xs, const double* Ys) const {
-        frechet::tile_mma(c, t, Xs, 1, kLd, Ys);
     }
     CK_HD void store(int64_t b, int t, const Acc& c) const {
         int bi, bj;

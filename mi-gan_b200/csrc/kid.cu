@@ -1,7 +1,7 @@
 // C ABI of the kernel Inception distance (include/inception_b200.h): kid_workspace_bytes and kid_subset_terms.
 // Argument and index-table checks, workspace layout and the launches; the arithmetic is kid_kernels.cuh's.  The tile
-// kernel runs its phases with a block's threads at once, and the emulation build (MIGAN_EMULATE) runs the same phases
-// with the threads of a block in turn.
+// kernel is one body over portable.cuh's block layer, run with a block's threads at once on the device and on the host
+// in the emulation build (MIGAN_EMULATE).
 //
 // Workspace (nb = m rounded up to 64, over 64; each region 256-byte aligned): the fake and the real index tables
 // (S m ints each), the tile partials (S x 3 x nb^2 doubles).
@@ -24,45 +24,29 @@ static_assert(kid::kMaxDim == KID_MAX_DIM, "one cap");
 static_assert(IDS_FLOAT32 == 0 && IDS_FLOAT64 == 1, "the dtype codes of ids_scores");
 constexpr size_t kTileSmem = (2 * kTileDoubles + kRedDoubles) * sizeof(double);
 
+template <class B>
+CK_D void tile_block(const B& blk, const kid::TileArgs& a, int64_t b, double* smem) {
+    double* Xs = smem;
+    double* Ys = Xs + kTileDoubles;
+    double* red = Ys + kTileDoubles;
+    kid::Accs<B> c;
+    frechet::panel_product(blk, c, a.fake.d, Xs, Ys, a, b);
+    blk.each([&](int t) { a.reduce(b, t, c[t], red); });
+    blk.sync();
+    blk.each([&](int t) { a.combine(t, red); });
+    blk.sync();
+    blk.each([&](int t) { a.store(b, t, red); });
+}
+
 #ifdef MIGAN_EMULATE
 int tile_launch(const kid::TileArgs& a, ck_stream_t) {
-    const int64_t blocks = a.blocks();
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> Xs(kTileDoubles), Ys(kTileDoubles), red(kRedDoubles);
-        std::vector<kid::Acc> c(kThreads);
-        for (int t = 0; t < kThreads; ++t) frechet::acc_zero(c[t]);
-        for (int k0 = 0; k0 < a.fake.d; k0 += kG) {
-            for (int t = 0; t < kThreads; ++t) a.stage(b, t, k0, Xs.data(), Ys.data());
-            for (int t = 0; t < kThreads; ++t) a.product(t, c[t], Xs.data(), Ys.data());
-        }
-        for (int t = 0; t < kThreads; ++t) a.reduce(b, t, c[t], red.data());
-        for (int t = 0; t < kThreads; ++t) a.combine(t, red.data());
-        for (int t = 0; t < kThreads; ++t) a.store(b, t, red.data());
-    }
-    return 0;
+    return ck_blocks<kThreads>(a.blocks(), kTileSmem,
+                               [&](auto& blk, int64_t b, void* smem) { tile_block(blk, a, b, (double*)smem); });
 }
 #else
 __global__ void __launch_bounds__(kThreads) kid_tile_kernel(const __grid_constant__ kid::TileArgs a) {
     extern __shared__ __align__(16) double smem[];
-    double* Xs = smem;
-    double* Ys = Xs + kTileDoubles;
-    double* red = Ys + kTileDoubles;
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    kid::Acc c;
-    frechet::acc_zero(c);
-    for (int k0 = 0; k0 < a.fake.d; k0 += kG) {
-        a.stage(b, t, k0, Xs, Ys);
-        __syncthreads();
-        a.product(t, c, Xs, Ys);
-        __syncthreads();
-    }
-    a.reduce(b, t, c, red);
-    __syncthreads();
-    a.combine(t, red);
-    __syncthreads();
-    a.store(b, t, red);
+    tile_block(DeviceBlock(), a, blockIdx.x, smem);
 }
 
 int tile_launch(const kid::TileArgs& a, ck_stream_t s) {

@@ -24,28 +24,20 @@
 namespace kid {
 
 using frechet::Acc;
+using frechet::Accs;
 using frechet::acc_col;
 using frechet::acc_row;
 using frechet::kG;
 using frechet::kLd;
 using frechet::kThreads;
 using frechet::kTileDoubles;
+using frechet::Rows;
 using metrics::ddiv;
 
 constexpr int kMaxDim = 4096;
 constexpr int kLanes = kThreads / 32;             // the reduction's second level: one lane per warp's worth of threads
 constexpr int kRedDoubles = kThreads + kLanes;    // shared memory of the tile reduction
 enum Kind { kXX = 0, kYY = 1, kXY = 2, kKinds = 3 };
-
-// One side's feature rows, fp32 or fp64 as stored, promoted exactly to fp64.
-struct Rows {
-    const void* p; int d, fp64;
-
-    CK_HD double x(int64_t row, int c) const {
-        const int64_t e = row * d + c;
-        return fp64 ? static_cast<const double*>(p)[e] : (double)static_cast<const float*>(p)[e];
-    }
-};
 
 CK_HD int tiles_of(int m) { return (m + kG - 1) / kG; }
 CK_HD int64_t lower_tiles(int nb) { return (int64_t)nb * (nb + 1) / 2; }
@@ -103,9 +95,6 @@ struct TileArgs {
             Xs[k * kLd + x] = ra < m && c < A.d ? A.x(ia[ra], c) : 0.0;
             Ys[k * kLd + x] = rb < m && c < B.d ? B.x(ib[rb], c) : 0.0;
         }
-    }
-    CK_HD void product(int t, Acc& c, const double* Xs, const double* Ys) const {
-        frechet::tile_mma(c, t, Xs, 1, kLd, Ys);
     }
     // red[t] = thread t's kernel values in accumulator order, past m and the diagonal of X X^T, Y Y^T left out.
     CK_HD void reduce(int64_t b, int t, const Acc& c, double* red) const {

@@ -28,38 +28,31 @@ constexpr int kLayers = LPIPS_LAYERS;
 constexpr int kChannels[kLayers] = {64, 192, 384, 256, 256};
 
 // ---- the final reduction: one block per pair, fixed summation order (lpips::ReduceArgs) ----------------------------
+template <class B>
+CK_D void reduce_block(const B& blk, const lpips::ReduceArgs& a, int64_t i, double* s) {
+    float val = 0.f;   // thread 0's
+    for (int k = 0; k < kLayers; ++k) {
+        blk.each([&](int t) { s[t] = a.partial(i, k, t); });
+        block_tree<lpips::kReduceThreads>(blk, s);
+        blk.each([&](int t) {
+            if (t == 0) val += a.layer_term(i, k, s[0]);
+        });
+        blk.sync();
+    }
+    blk.each([&](int t) {
+        if (t == 0) a.out[i] = val;
+    });
+}
+
 #ifdef MIGAN_EMULATE
 int reduce_launch(const lpips::ReduceArgs& a, ck_stream_t) {
-    for (int64_t i = 0; i < a.n; ++i) {
-        float val = 0.f;
-        for (int k = 0; k < kLayers; ++k) {
-            double s[lpips::kReduceThreads];
-            for (int t = 0; t < lpips::kReduceThreads; ++t) s[t] = a.partial(i, k, t);
-            for (int stride = lpips::kReduceThreads / 2; stride > 0; stride >>= 1)
-                for (int t = 0; t < stride; ++t) s[t] += s[t + stride];
-            val += a.layer_term(i, k, s[0]);
-        }
-        a.out[i] = val;
-    }
-    return 0;
+    return ck_blocks<lpips::kReduceThreads>(a.n, lpips::kReduceThreads * sizeof(double),
+                                            [&](auto& blk, int64_t i, void* s) { reduce_block(blk, a, i, (double*)s); });
 }
 #else
 __global__ void __launch_bounds__(lpips::kReduceThreads) lpips_reduce_kernel(const lpips::ReduceArgs a) {
     __shared__ double s[lpips::kReduceThreads];
-    const int64_t i = blockIdx.x;
-    const int t = threadIdx.x;
-    float val = 0.f;
-    for (int k = 0; k < kLayers; ++k) {
-        s[t] = a.partial(i, k, t);
-        __syncthreads();
-        for (int stride = lpips::kReduceThreads / 2; stride > 0; stride >>= 1) {
-            if (t < stride) s[t] += s[t + stride];
-            __syncthreads();
-        }
-        if (t == 0) val += a.layer_term(i, k, s[0]);
-        __syncthreads();
-    }
-    if (t == 0) a.out[i] = val;
+    reduce_block(DeviceBlock(), a, blockIdx.x, s);
 }
 int reduce_launch(const lpips::ReduceArgs& a, ck_stream_t s) {
     lpips_reduce_kernel<<<a.n, lpips::kReduceThreads, 0, s>>>(a);

@@ -63,8 +63,8 @@ struct DistanceK {     // items = n*HW
     }
 };
 
-// The final reduction, one block of kReduceThreads per pair (lpips_abi.cu: a CUDA block with a shared-memory tree, or
-// the same arithmetic as a host loop in the emulation build).  For each layer k, thread t sums pixels t, t + 256, ... of
+// The final reduction, one block of kReduceThreads per pair (lpips_abi.cu: one body over portable.cuh's block layer,
+// with its shared-memory tree).  For each layer k, thread t sums pixels t, t + 256, ... of
 // pair i in double (partial()), the block adds the 256 partial sums in a fixed tree (stride 128, 64, ..., 1), and the
 // spatial mean rounded to fp32 is the layer term; the total adds the five terms in order, as lpips does
 // (val = 0; val += res[k]).  px: layer k's per-pixel values [n][hw[k]] at px + off[k].

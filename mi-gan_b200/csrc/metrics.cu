@@ -1,13 +1,12 @@
 // C ABI of the SSIM and PSNR evaluators (include/metrics_b200.h): argument checks, workspace layout and the two launches
-// of each call.  The arithmetic is metrics_kernels.cuh's; the kernels here run its phases with a block's threads at
-// once, and the emulation build (MIGAN_EMULATE) runs the same phases with the threads of a block in turn.
+// of each call.  The arithmetic is metrics_kernels.cuh's; the tile kernels are bodies over portable.cuh's block layer,
+// run with a block's threads at once on the device and on the host in the emulation build (MIGAN_EMULATE).
 //
 // Workspace: the partials of the first launch, [n][parts] doubles (SSIM: parts = C * tiles; PSNR: parts = row chunks),
 // then the n per-image sums.  No atomics: each block writes its own slot.
 #include <math.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "../../include/metrics_b200.h"
 #include "abi_error.h"
@@ -17,39 +16,54 @@ namespace {
 using metrics::kThreads;
 using migan::fail;
 
-// The fixed tree over a block's kThreads partial sums (stride 128, 64, ..., 1).
-#ifdef MIGAN_EMULATE
-double host_tree(double* s) {
-    for (int stride = kThreads / 2; stride > 0; stride >>= 1)
-        for (int t = 0; t < stride; ++t) s[t] = dadd_rn(s[t], s[t + stride]);
-    return s[0];
+// *out = the sum of the block's partials red[0 .. kThreads) in portable.cuh's fixed tree.
+template <class B>
+CK_D void tree_to(const B& blk, double* red, double* out) {
+    block_tree<kThreads>(blk, red);
+    blk.each([&](int t) {
+        if (t == 0) *out = red[0];
+    });
 }
 
+template <class B>
+CK_D void ssim_block(const B& blk, const metrics::SsimArgs& a, int64_t b, double* g, double* red, void* smem) {
+    double* hs = static_cast<double*>(smem);
+    float* sx = reinterpret_cast<float*>(hs + (int64_t)5 * a.in_h() * metrics::kTileW);
+    float* sy = sx + a.in_h() * a.in_w();
+    blk.each([&](int t) {
+        if (t < a.ws) g[t] = a.taps[t];
+        a.stage(b, t, sx, sy);
+    });
+    blk.sync();
+    blk.each([&](int t) { a.hpass(t, g, sx, sy, hs); });
+    blk.sync();
+    blk.each([&](int t) { red[t] = a.vpass(b, t, g, hs); });
+    tree_to(blk, red, a.partial + b);
+}
+
+template <class B>
+CK_D void psnr_block(const B& blk, const metrics::PsnrArgs& a, int64_t b, double* red) {
+    blk.each([&](int t) { red[t] = a.thread_sum(b, t); });
+    tree_to(blk, red, a.partial + b);
+}
+
+#ifdef MIGAN_EMULATE
 int ssim_launch(const metrics::SsimArgs& a, int64_t blocks, ck_stream_t) {
-#pragma omp parallel for schedule(dynamic)
-    for (int64_t b = 0; b < blocks; ++b) {
-        std::vector<double> hs((size_t)5 * a.in_h() * metrics::kTileW);
-        std::vector<float> sx((size_t)a.in_h() * a.in_w()), sy(sx.size());
-        double g[metrics::kMaxWindow], s[kThreads];
-        for (int k = 0; k < a.ws; ++k) g[k] = a.taps[k];
-        for (int t = 0; t < kThreads; ++t) a.stage(b, t, sx.data(), sy.data());
-        for (int t = 0; t < kThreads; ++t) a.hpass(t, g, sx.data(), sy.data(), hs.data());
-        for (int t = 0; t < kThreads; ++t) s[t] = a.vpass(b, t, g, hs.data());
-        a.partial[b] = host_tree(s);
-    }
-    return 0;
+    const size_t statics = (metrics::kMaxWindow + kThreads) * sizeof(double);
+    return ck_blocks<kThreads>(blocks, statics + a.smem_bytes(), [&](auto& blk, int64_t b, void* smem) {
+        double* g = static_cast<double*>(smem);
+        double* red = g + metrics::kMaxWindow;
+        ssim_block(blk, a, b, g, red, red + kThreads);
+    });
 }
 
 int psnr_launch(const metrics::PsnrArgs& a, int64_t blocks, ck_stream_t) {
-#pragma omp parallel for schedule(static)
-    for (int64_t b = 0; b < blocks; ++b) {
-        double s[kThreads];
-        for (int t = 0; t < kThreads; ++t) s[t] = a.thread_sum(b, t);
-        a.partial[b] = host_tree(s);
-    }
-    return 0;
+    return ck_blocks<kThreads>(blocks, kThreads * sizeof(double),
+                               [&](auto& blk, int64_t b, void* smem) { psnr_block(blk, a, b, (double*)smem); });
 }
 
+// The per-image reduction is a warp's shuffle tree on the device, which the block layer has no counterpart for; the
+// emulation build adds the lanes in the same tree.
 int reduce_launch(const metrics::ReduceArgs& a, ck_stream_t) {
     for (int64_t i = 0; i < a.n; ++i) {
         double s[metrics::kWarp];
@@ -62,38 +76,16 @@ int reduce_launch(const metrics::ReduceArgs& a, ck_stream_t) {
     return 0;
 }
 #else
-__device__ __forceinline__ void block_tree(double* s, double v, double* out) {
-    const int t = threadIdx.x;
-    s[t] = v;
-    __syncthreads();
-    for (int stride = kThreads / 2; stride > 0; stride >>= 1) {
-        if (t < stride) s[t] = dadd_rn(s[t], s[t + stride]);
-        __syncthreads();
-    }
-    if (t == 0) *out = s[0];
-}
-
 __global__ void __launch_bounds__(kThreads) metrics_ssim_tile_kernel(const __grid_constant__ metrics::SsimArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ double g[metrics::kMaxWindow];
     __shared__ double red[kThreads];
-    const int64_t b = blockIdx.x;
-    const int t = threadIdx.x;
-    double* hs = reinterpret_cast<double*>(smem);
-    float* sx = reinterpret_cast<float*>(hs + (int64_t)5 * a.in_h() * metrics::kTileW);
-    float* sy = sx + a.in_h() * a.in_w();
-    if (t < a.ws) g[t] = a.taps[t];
-    a.stage(b, t, sx, sy);
-    __syncthreads();
-    a.hpass(t, g, sx, sy, hs);
-    __syncthreads();
-    block_tree(red, a.vpass(b, t, g, hs), a.partial + b);
+    ssim_block(DeviceBlock(), a, blockIdx.x, g, red, smem);
 }
 
 __global__ void __launch_bounds__(kThreads) metrics_psnr_kernel(const __grid_constant__ metrics::PsnrArgs a) {
     __shared__ double red[kThreads];
-    const int64_t b = blockIdx.x;
-    block_tree(red, a.thread_sum(b, threadIdx.x), a.partial + b);
+    psnr_block(DeviceBlock(), a, blockIdx.x, red);
 }
 
 __global__ void __launch_bounds__(kThreads) metrics_reduce_kernel(const __grid_constant__ metrics::ReduceArgs a) {

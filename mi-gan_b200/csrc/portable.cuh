@@ -3,8 +3,8 @@
 // The product library is compiled by nvcc for sm_90a.  The emulation build (tests/emul/build_emul.py) compiles the same
 // sources as plain C++ with -DMIGAN_EMULATE -ffp-contract=off and runs the kernels' functors and block functions as
 // host loops, so their arithmetic and index math are checked on a machine without a GPU.  This header decides, per
-// build, the function qualifiers, the half type, the item launch, the rounding of arithmetic and device memory; the
-// host loops that stand in for a block kernel or a GEMM stay next to the kernel they emulate.
+// build, the function qualifiers, the half type, the item launch, the block layer, the rounding of arithmetic and device
+// memory; the host loops that stand in for a GEMM stay next to the kernel they emulate.
 //
 // Rounding: an operation written with one of the *_rn functions below is rounded on its own.  On the device that is
 // the matching __f*_rn / __d*_rn intrinsic, which nvcc never contracts into an FMA; in the emulation build it is the
@@ -18,6 +18,7 @@
 #include <algorithm>
 
 #ifdef MIGAN_EMULATE
+#include <vector>
 #define CK_HD inline
 #define CK_D inline
 typedef void* ck_stream_t;
@@ -119,3 +120,64 @@ int set_smem(K kernel, size_t bytes) {
     return (int)cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 #endif
+
+// ---- block kernels ----------------------------------------------------------------------------------------------------
+// A block kernel is one body over a block blk, run by both builds: blk.each(f) runs f(t) for every thread t of the
+// block (on the device, f(threadIdx.x) in all threads at once; in the emulation build, t = 0, 1, ... in turn),
+// blk.sync() is the barrier between two phases, and blk.any(f) is a barrier that returns whether f(t) is nonzero in
+// some thread.  A value that every thread of a block holds equal is a plain local of the body; a value that differs per
+// thread is a Local<T>, indexed by the thread.  Code between two barriers must not race.  ck_blocks runs a body over a
+// grid of blocks on the host, each with an arena in place of the block's shared memory.
+#ifdef MIGAN_EMULATE
+template <int N>
+struct HostBlock {
+    template <class T>
+    struct Local {
+        T v[N];
+        T& operator[](int t) { return v[t]; }
+    };
+    template <class F> void each(F f) const { for (int t = 0; t < N; ++t) f(t); }
+    void sync() const {}
+    template <class F> bool any(F f) const {
+        int r = 0;
+        for (int t = 0; t < N; ++t) r |= f(t);
+        return r != 0;
+    }
+};
+// body(blk, b, smem) for every block b in [0, blocks); smem is smem_bytes, 16-byte aligned, the block's own.
+template <int N, class F>
+int ck_blocks(int64_t blocks, size_t smem_bytes, const F& body) {
+#pragma omp parallel
+    {
+        std::vector<double> arena(smem_bytes / sizeof(double) + 1);
+        const HostBlock<N> blk;
+#pragma omp for schedule(dynamic)
+        for (int64_t b = 0; b < blocks; ++b) body(blk, b, static_cast<void*>(arena.data()));
+    }
+    return 0;
+}
+#else
+struct DeviceBlock {
+    template <class T>
+    struct Local {
+        T v;
+        CK_D T& operator[](int) { return v; }
+    };
+    template <class F> CK_D void each(F f) const { f((int)threadIdx.x); }
+    CK_D void sync() const { __syncthreads(); }
+    template <class F> CK_D bool any(F f) const { return __syncthreads_or(f((int)threadIdx.x)) != 0; }
+};
+#endif
+
+// s[0] = s[0] + ... + s[N - 1] in a fixed tree (stride N / 2, N / 4, ..., 1), visible to every thread on return.  s
+// holds one partial per thread, written before the call.
+template <int N, class B>
+CK_D void block_tree(const B& blk, double* s) {
+    blk.sync();
+    for (int stride = N / 2; stride > 0; stride >>= 1) {
+        blk.each([&](int t) {
+            if (t < stride) s[t] = dadd_rn(s[t], s[t + stride]);
+        });
+        blk.sync();
+    }
+}

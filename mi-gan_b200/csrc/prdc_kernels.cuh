@@ -38,21 +38,12 @@ using frechet::kG;
 using frechet::kLd;
 using frechet::kThreads;
 using frechet::kTileDoubles;
+using frechet::Rows;
 
 constexpr int kMaxDim = 4096;
 constexpr int kMaxK = 32;        // the neighbourhood size: lists of at most 33 values per thread
 constexpr int kSplits = 8;       // column splits of a pass: a block walks at most ceil(tiles / 8) column tiles
 enum Mode { kNorms = 0, kRadii = 1, kCross = 2 };
-
-// One side's feature rows, fp32 or fp64 as stored, promoted exactly to fp64.
-struct Rows {
-    const void* p; int d, fp64;
-
-    CK_HD double x(int64_t row, int c) const {
-        const int64_t e = row * d + c;
-        return fp64 ? static_cast<const double*>(p)[e] : (double)static_cast<const float*>(p)[e];
-    }
-};
 
 CK_HD int tiles_of(int64_t n) { return (int)((n + kG - 1) / kG); }
 CK_HD int splits_of(int col_tiles) { return col_tiles < kSplits ? col_tiles : kSplits; }
